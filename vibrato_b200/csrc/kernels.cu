@@ -19,18 +19,6 @@
 #define VBT_K3_MIN_BLOCKS 16
 #endif
 
-// A batch whose byte offsets k_count_chars refused is not touched by any later kernel: the sizes derived from
-// the offsets (slots, workspace bounds) cannot be trusted.
-#ifndef VBT_GUARD_OFFSETS
-#define VBT_GUARD_OFFSETS 1
-#endif
-#if VBT_GUARD_OFFSETS
-#define VBT_STAND_DOWN_IF_REJECTED(b) \
-    if (*(b).flags & kFlagsStandDown) return
-#else
-#define VBT_STAND_DOWN_IF_REJECTED(b) (void)0
-#endif
-
 namespace vbt {
 
 namespace {
@@ -38,6 +26,10 @@ namespace {
 constexpr uint32_t kMask = 0x7FFFFFFFu;
 constexpr uint32_t kFlag = 0x80000000u;
 constexpr unsigned kFull = 0xFFFFFFFFu;
+
+// A batch whose byte offsets k_count_chars refused is not touched by any later kernel: the sizes derived from
+// the offsets (slots, workspace bounds) cannot be trusted.
+__device__ __forceinline__ bool stand_down(uint32_t batch_flags) { return batch_flags & kFlagsStandDown; }
 
 // CharInfo bit fields (dictionary/character.rs:10-24,72-94)
 __device__ __forceinline__ uint32_t ci_cate(uint32_t ci) { return ci & 0x3FFFFu; }
@@ -218,7 +210,7 @@ __device__ __forceinline__ void decode_one(const DictView& d, const Batch& b, ui
 }
 
 __global__ void __launch_bounds__(256) k_decode(DictView d, Batch b) {
-    VBT_STAND_DOWN_IF_REJECTED(b);
+    if (stand_down(*b.flags)) return;
     const uint32_t w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const uint32_t lane = threadIdx.x & 31;
 #pragma unroll 1
@@ -352,13 +344,12 @@ __device__ __forceinline__ uint32_t gen_unknown(const DictView& d, uint32_t sw, 
 }
 
 __global__ void __launch_bounds__(256) k_candidates(DictView d, Batch b) {
-    constexpr bool COUNT = false;  // M/T/P/W are produced by k_candidate_stats in counted runs
     const uint32_t slot = blockIdx.x * blockDim.x + threadIdx.x;
     const uint32_t lane = threadIdx.x & 31;
-    // A rejected batch (see VBT_STAND_DOWN_IF_REJECTED) leaves every thread out of range.  The flag word is read
-    // next to the slot total instead of in front of it: with 256-thread blocks that live for one trie walk, a
-    // dependent extra round trip at the top costs 8 % of this kernel (profiles/r01e_k3_variants_ab.md).
-    const uint32_t batch_flags = VBT_GUARD_OFFSETS ? *b.flags : 0u;
+    // A rejected batch (see stand_down) leaves every thread out of range.  The flag word is read next to the slot
+    // total instead of in front of it: with 256-thread blocks that live for one trie walk, a dependent extra round
+    // trip at the top costs 8 % of this kernel (profiles/r01e_k3_variants_ab.md).
+    const uint32_t batch_flags = *b.flags;
     const uint32_t total_slots = b.slot_off[b.n_sent];
     if (slot == 0 && total_slots > b.launch_slots) atomicOr(b.flags, kFlagSlotsOverflow);
     const bool in_range = slot < total_slots && !(batch_flags & kFlagBadOffsets);
@@ -388,13 +379,12 @@ __global__ void __launch_bounds__(256) k_candidates(DictView d, Batch b) {
     if (active) {
         uint32_t cu = 0;
         if (d.usr_table)
-            cu = walk_lexicon<false, COUNT>(d.usr_nodes, d.usr_num_nodes, d.usr_post, b.code_usr, b.groupable, sw,
+            cu = walk_lexicon<false, false>(d.usr_nodes, d.usr_num_nodes, d.usr_post, b.code_usr, b.groupable, sw,
                                             nullptr, nullptr, st, &hb, kSegUser);
-        uint32_t cs = walk_lexicon<false, COUNT>(d.sys_nodes, d.sys_num_nodes, d.sys_post, b.code_sys, b.groupable,
+        uint32_t cs = walk_lexicon<false, false>(d.sys_nodes, d.sys_num_nodes, d.sys_post, b.code_sys, b.groupable,
                                                  sw, nullptr, nullptr, st, &hb, 0);
         matched = (cu + cs) != 0;
         uint32_t ck = gen_unknown<false>(d, sw, ci, g, matched, nullptr, nullptr, &hb);
-        if (COUNT) st.w += ck;
         cnt = cu + cs + ck;
     }
     // Block-aggregated allocation from the candidate pool: a scan inside each warp, the eight warp totals through
@@ -492,7 +482,7 @@ __global__ void __launch_bounds__(256) k_candidates(DictView d, Batch b) {
 // Side array for counted runs: per slot {M, T, P, W} so that k_viterbi can sum them over the
 // positions the reference actually visits.  Filled by a second, counting-only kernel.
 __global__ void __launch_bounds__(256) k_candidate_stats(DictView d, Batch b, uint4* stats) {
-    VBT_STAND_DOWN_IF_REJECTED(b);
+    if (stand_down(*b.flags)) return;
     const uint32_t slot = blockIdx.x * blockDim.x + threadIdx.x;
     if (slot >= b.slot_off[b.n_sent]) return;
     uint32_t g0 = b.groupable[slot];
@@ -540,14 +530,107 @@ __device__ __forceinline__ uint4 load_info(const Batch& b, uint32_t slot) {
     return r;
 }
 
-// Build-time switches of k_viterbi, kept for A/B builds (tools/build_variants.sh; profiles/r01e_k3_variants_ab.md):
-// VBT_K3_PF_DIST = how many candidates ahead one lane per group hints into L1 (0 = no hint), VBT_K3_PIPE = fetch a
-// position's row metadata and candidate header one position early.
+// The lattice bookkeeping shared by k_viterbi and k_viterbi2.  Every lane of the warp calls these helpers; `sidx` is
+// the group's sentence in launch order and the group's lane 0 (gl == 0) writes the per-sentence records.
+
+// Start of the sweep of sentence `sidx`: returns its slots {first, sentinel} (both 0 without a sentence).  An empty
+// sentence gets its EOS record here; any other gets its BOS node.
+__device__ __forceinline__ uint2 begin_sentence(const Batch& b, uint32_t sidx, uint32_t gl) {
+    uint32_t slot = 0, slot_end = 0;
+    if (sidx < b.n_sent) {
+        const uint32_t s = b.order ? b.order[sidx] : sidx;
+        slot = b.slot_off[s];
+        slot_end = b.slot_off[s + 1] - 1;
+        if (gl == 0) {
+            if (slot == slot_end) {  // Worker::tokenize returns early on an empty sentence (worker.rs:50-52)
+                b.eos[s] = make_uint4(kNone, 0, 0, 0);
+            } else {  // Lattice::insert_bos (lattice.rs:72-83): right_id 0, cost 0
+                const uint32_t eo = b.ends_meta[slot].x;
+                b.ends_hot[eo] = make_int2(0, 0);
+                b.ends_cold[eo] = make_uint4(kNone, kNone, kNone, 0);
+                b.ends_meta[slot].y = eo + 1;
+            }
+        }
+    }
+    __syncwarp();
+    return make_uint2(slot, slot_end);
+}
+
+// Lattice::insert_node (lattice.rs:103-127): every valid lane pushes its candidate `cd` {left | right << 16, word
+// cost in the low half, word idx, end slot} into ends[end_word], whose next free entry is `fill`, in candidate order.
+// Its best total is `best`, reached from start slot `slot` through predecessor `bestk` of the row at entry `eo`.
+// End slots of different sentences never coincide, so one warp-wide match suffices.  Returns the row's new fill on
+// the lane that stored it (rank 0 among the lanes ending there), 0 on every other lane.
+__device__ __forceinline__ uint32_t insert_node(const Batch& b, bool valid, const uint4& cd, int32_t best, uint32_t slot,
+                                                uint32_t eo, uint32_t bestk, uint32_t fill) {
+    const uint32_t vmask = __ballot_sync(kFull, valid);
+    uint32_t new_fill = 0;
+    if (valid) {
+        const uint32_t peers = __match_any_sync(vmask, cd.w);
+        const uint32_t rank = __popc(peers & lanemask_lt());
+        const uint32_t idx = fill + rank;
+        const int32_t cost = int32_t(uint32_t(best) + uint32_t(int32_t(int16_t(cd.y & 0xFFFFu))));
+        b.ends_hot[idx] = make_int2(cost, int32_t(cd.x >> 16));
+        // lattice.rs:144 keeps the predecessor index as u16
+        b.ends_cold[idx] = make_uint4(slot, eo + (bestk & 0xFFFFu), cd.z, uint32_t(cost));
+        if (rank == 0) {
+            new_fill = fill + __popc(peers);
+            b.ends_meta[cd.w].y = new_fill;
+        }
+    }
+    __syncwarp();
+    return new_fill;
+}
+
+// What k_viterbi's counters need of a finished sentence: the size of its EOS row, its base slot and its length.
+struct SentenceEnd {
+    uint32_t K, base, n;
+};
+
+// Lattice::insert_eos (lattice.rs:85-101): left_id 0, no word cost; the G lanes of the group take the predecessors
+// in the row of `slot_end` and lane 0 writes b.eos.  Conn is the kernel's connector (ConnRow or ConnCol).
+template <int G, class Conn>
+__device__ __forceinline__ SentenceEnd insert_eos(const DictView& d, const Batch& b, uint32_t sidx, uint32_t slot_end,
+                                                  uint32_t gl) {
+    const bool has_sentence = sidx < b.n_sent;
+    const uint32_t s = has_sentence ? (b.order ? b.order[sidx] : sidx) : 0;
+    const uint32_t base = has_sentence ? b.slot_off[s] : 0;
+    const uint32_t n = has_sentence ? b.slot_off[s + 1] - 1 - base : 0;
+    const uint32_t eos_start = slot_end - base;  // n, or the start of the trailing space run
+    uint32_t K = 0, eo = 0;
+    if (n > 0) {
+        const uint2 m = b.ends_meta[slot_end];
+        eo = m.x;
+        K = m.y - m.x;
+    }
+    // minimise the signed 64-bit key (cost << 32 | ~index): smallest cost, then the LARGEST index
+    // among ties — the `<=` rule of search_min_node
+    long long bestkey = LLONG_MAX;
+    const Conn conn_eos(d, 0);  // BOS_EOS_CONNECTION_ID (common.rs:18)
+    const uint32_t max_k = __reduce_max_sync(kFull, K);
+    for (uint32_t k0 = 0; k0 < max_k; k0 += G) {
+        long long key = LLONG_MAX;
+        if (k0 + gl < K) {
+            int2 pr = b.ends_hot[eo + k0 + gl];
+            int32_t v = int32_t(uint32_t(pr.x) + uint32_t(conn_eos.cost(d, uint32_t(pr.y))));
+            key = (long long)(((unsigned long long)uint32_t(v) << 32) | (unsigned long long)(~(k0 + gl)));
+        }
+#pragma unroll
+        for (int o = G / 2; o > 0; o >>= 1) key = min(key, __shfl_xor_sync(kFull, key, o, G));
+        bestkey = min(bestkey, key);
+    }
+    if (n > 0 && gl == 0) {
+        const bool none = K == 0;
+        const uint32_t bestk = (~uint32_t(bestkey)) & 0xFFFFu;  // lattice.rs:144 `i as u16`
+        b.eos[s] = make_uint4(none ? kNone : eo + bestk, eos_start, uint32_t(int32_t(bestkey >> 32)), 0);
+    }
+    return {K, base, n};
+}
+
+// Tuning knobs of k_viterbi, swept with A/B builds (tools/build_variants.sh, tools/ab_multi.py): VBT_K3_MIN_BLOCKS
+// (above) and VBT_K3_PF_DIST = how many candidates ahead one lane per group hints into L1 (0 = no hint).
 #ifndef VBT_K3_PF_DIST
 #define VBT_K3_PF_DIST 8
-#endif
-#ifndef VBT_K3_PIPE
-#define VBT_K3_PIPE 1
 #endif
 
 // ConnectorCost::cost(right_id, left_id) for one fixed left id (one candidate).
@@ -613,38 +696,20 @@ struct ConnRow<2> {  // DualConnector::cost (dual_connector.rs:269-280): reduced
 
 template <int G, bool COUNT, int CONN>
 __global__ void __launch_bounds__(128, (CONN == 0 && !COUNT) ? VBT_K3_MIN_BLOCKS : 8) k_viterbi(DictView d, Batch b, const uint4* __restrict__ stats) {
-    VBT_STAND_DOWN_IF_REJECTED(b);
+    if (stand_down(*b.flags)) return;
     constexpr uint32_t SPW = 32 / G;  // sentences per warp
     const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const uint32_t lane = threadIdx.x & 31;
     const uint32_t sub = lane / G, gl = lane % G;
     const uint32_t sidx = warp * SPW + sub;
-    const bool has_sentence = sidx < b.n_sent;
     unsigned long long cntE = 0, cntN = 2, cM = 0, cT = 0, cP = 0, cW = 0, cWalks = 0;
 
     // Loop state is kept slot-absolute (current slot, the slot whose row EOS connects to, first slot after a
     // skipped space run) so that nothing but these three words lives across the gather loop; the sentence
     // index, its base slot and its length are looked up again where the sweep ends.
-    uint32_t slot = 0, slot_end = 0;
-    if (has_sentence) {
-        const uint32_t s = b.order ? b.order[sidx] : sidx;
-        slot = b.slot_off[s];
-        slot_end = b.slot_off[s + 1] - 1;
-        if (gl == 0) {
-            if (slot == slot_end) {  // Worker::tokenize returns early on an empty sentence (worker.rs:50-52)
-                b.eos[s] = make_uint4(kNone, 0, 0, 0);
-            } else {  // Lattice::insert_bos (lattice.rs:72-83): right_id 0, cost 0
-                const uint32_t eo = b.ends_meta[slot].x;
-                b.ends_hot[eo] = make_int2(0, 0);
-                b.ends_cold[eo] = make_uint4(kNone, kNone, kNone, 0);
-                b.ends_meta[slot].y = eo + 1;
-            }
-        }
-    }
-    __syncwarp();
-
+    const uint2 range = begin_sentence(b, sidx, gl);
+    uint32_t slot = range.x, slot_end = range.y;
     uint32_t skip_slot = slot;
-#if VBT_K3_PIPE
     // Row metadata and candidate header of a position are fetched one position early, so that its candidates and
     // predecessors can be requested as soon as the position starts (one round trip less on the chain).
     uint2 m_cur = make_uint2(0, 0);
@@ -654,12 +719,10 @@ __global__ void __launch_bounds__(128, (CONN == 0 && !COUNT) ? VBT_K3_MIN_BLOCKS
         info_cur = load_info(b, slot);
     }
     const uint32_t group_mask = G == 32 ? kFull : (((1u << (G & 31)) - 1u) << (sub * G));
-#endif
     while (__any_sync(kFull, slot < slot_end)) {
         const bool active = slot < slot_end;
         uint32_t K = 0, eo = 0;
         uint4 info = make_uint4(0, 0, 0, 0);
-#if VBT_K3_PIPE
         if (active) {
             eo = m_cur.x;
             K = m_cur.y - m_cur.x;
@@ -674,14 +737,6 @@ __global__ void __launch_bounds__(128, (CONN == 0 && !COUNT) ? VBT_K3_MIN_BLOCKS
             m_nx = b.ends_meta[slot + 1];
             info_nx = load_info(b, slot + 1);
         }
-#else
-        if (active) {  // two independent loads, one round trip
-            const uint2 m = b.ends_meta[slot];
-            info = load_info(b, slot);
-            eo = m.x;
-            K = m.y - m.x;
-        }
-#endif
         // positions inside a skipped space run are never start_node; K == 0: has_previous_node fails
         bool visit = active && slot >= skip_slot && K != 0;  // (lattice.rs:155-157, tokenizer.rs:110-114)
         if (visit && (info.w & kInfoTrailing)) {  // tokenizer.rs:128-130: EOS starts here, the sweep ends
@@ -705,11 +760,7 @@ __global__ void __launch_bounds__(128, (CONN == 0 && !COUNT) ? VBT_K3_MIN_BLOCKS
         // this position's; K2 wrote them long ago (evicted from L2), pull the line ahead while this position works
         if (visit && gl == 0 && info.x + ncand + VBT_K3_PF_DIST < b.cand_cap) {
             const uint4* nx = b.cand + info.x + ncand + VBT_K3_PF_DIST;
-#if VBT_K3_PF_L2
-            asm volatile("prefetch.global.L2 [%0];" ::"l"(nx));
-#else
             asm volatile("prefetch.global.L1 [%0];" ::"l"(nx));
-#endif
         }
 #endif
         const uint32_t max_cand = __reduce_max_sync(kFull, ncand);
@@ -726,7 +777,7 @@ __global__ void __launch_bounds__(128, (CONN == 0 && !COUNT) ? VBT_K3_MIN_BLOCKS
                 const uint2 me = b.ends_meta[cd.w];
                 fill = me.y;  // next free entry of that row (absolute)
             }
-            const uint32_t left = cd.x & 0xFFFFu, right = cd.x >> 16;
+            const uint32_t left = cd.x & 0xFFFFu;
             const ConnRow<CONN> conn(d, left);
             // Lattice::add_connid_counts (lattice.rs:170-176): one (left, pred.right) edge per predecessor
             if (COUNT && b.lid_count && valid) atomicAdd(&b.lid_count[left], (unsigned long long)K);
@@ -758,73 +809,25 @@ __global__ void __launch_bounds__(128, (CONN == 0 && !COUNT) ? VBT_K3_MIN_BLOCKS
                     }
                 }
             }
-            // Lattice::insert_node (lattice.rs:103-127): push into ends[end_word] in candidate order.
-            // End slots of different sentences never coincide, so one warp-wide match suffices.
-            const uint32_t vmask = __ballot_sync(kFull, valid);
-            if (valid) {
-                const uint32_t peers = __match_any_sync(vmask, cd.w);
-                const uint32_t rank = __popc(peers & lanemask_lt());
-                const uint32_t idx = fill + rank;
-                const int32_t cost = int32_t(uint32_t(best) + uint32_t(int32_t(int16_t(cd.y & 0xFFFFu))));
-                b.ends_hot[idx] = make_int2(cost, int32_t(right));
-                // lattice.rs:144 keeps the predecessor index as u16
-                b.ends_cold[idx] = make_uint4(slot, eo + (bestk & 0xFFFFu), cd.z, uint32_t(cost));
-                if (rank == 0) b.ends_meta[cd.w].y = fill + __popc(peers);
-#if VBT_K3_PIPE
-                if (rank == 0 && cd.w == slot + 1) k_fix = fill + __popc(peers);
-#endif
-            }
-            __syncwarp();
+            const uint32_t row_fill = insert_node(b, valid, cd, best, slot, eo, bestk, fill);
+            if (row_fill && cd.w == slot + 1) k_fix = row_fill;
         }
-#if VBT_K3_PIPE
         k_fix = __reduce_max_sync(group_mask, k_fix);  // fills only grow: the last chunk's count is the largest
         m_cur = make_uint2(m_nx.x, max(m_nx.y, k_fix));
         info_cur = info_nx;
-#endif
         if (slot < slot_end) ++slot;
     }
 
-    // Lattice::insert_eos (lattice.rs:85-101): left_id 0, no word cost; lanes of the group = predecessors
-    {
-        const uint32_t s = has_sentence ? (b.order ? b.order[sidx] : sidx) : 0;
-        const uint32_t base = has_sentence ? b.slot_off[s] : 0;
-        const uint32_t n = has_sentence ? b.slot_off[s + 1] - 1 - base : 0;
-        const uint32_t eos_start = slot_end - base;  // n, or the start of the trailing space run
-        uint32_t K = 0, eo = 0;
-        if (n > 0) {
-            const uint2 m = b.ends_meta[slot_end];
-            eo = m.x;
-            K = m.y - m.x;
-        }
-        // minimise the signed 64-bit key (cost << 32 | ~index): smallest cost, then the LARGEST index
-        // among ties — the `<=` rule of search_min_node
-        long long bestkey = LLONG_MAX;
-        const ConnRow<CONN> conn_eos(d, 0);  // BOS_EOS_CONNECTION_ID (common.rs:18)
-        const uint32_t max_k = __reduce_max_sync(kFull, K);
-        for (uint32_t k0 = 0; k0 < max_k; k0 += G) {
-            long long key = LLONG_MAX;
-            if (k0 + gl < K) {
-                int2 pr = b.ends_hot[eo + k0 + gl];
-                int32_t v = int32_t(uint32_t(pr.x) + uint32_t(conn_eos.cost(d, uint32_t(pr.y))));
-                key = (long long)(((unsigned long long)uint32_t(v) << 32) | (unsigned long long)(~(k0 + gl)));
-            }
-#pragma unroll
-            for (int o = G / 2; o > 0; o >>= 1) key = min(key, __shfl_xor_sync(kFull, key, o, G));
-            bestkey = min(bestkey, key);
-        }
-        if (COUNT) cntE += K;
-        if (COUNT && b.lid_count && n > 0) {  // lattice.rs:178-181: the EOS edges are counted over ends[len_char]
-            const uint2 ml = b.ends_meta[base + n];
+    const SentenceEnd e = insert_eos<G, ConnRow<CONN>>(d, b, sidx, slot_end, gl);
+    if (COUNT) {
+        cntE += e.K;
+        if (b.lid_count && e.n > 0) {  // lattice.rs:178-181: the EOS edges are counted over ends[len_char]
+            const uint2 ml = b.ends_meta[e.base + e.n];
             const uint32_t nl = ml.y - ml.x;
             for (uint32_t k = gl; k < nl; k += G) atomicAdd(&b.rid_count[uint32_t(b.ends_hot[ml.x + k].y)], 1ull);
             if (gl == 0 && nl) atomicAdd(&b.lid_count[0], (unsigned long long)nl);
         }
-        if (n > 0 && gl == 0) {
-            const bool none = K == 0;
-            const uint32_t bestk = (~uint32_t(bestkey)) & 0xFFFFu;  // lattice.rs:144 `i as u16`
-            b.eos[s] = make_uint4(none ? kNone : eo + bestk, eos_start, uint32_t(int32_t(bestkey >> 32)), 0);
-        }
-        if (COUNT && b.counters && n > 0 && gl == 0) {
+        if (b.counters && e.n > 0 && gl == 0) {
             atomicAdd(&b.counters[kCntE], cntE);
             atomicAdd(&b.counters[kCntN], cntN);
             atomicAdd(&b.counters[kCntM], cM);
@@ -862,22 +865,10 @@ __global__ void __launch_bounds__(128, (CONN == 0 && !COUNT) ? VBT_K3_MIN_BLOCKS
 // 14.8 ms).
 #define VBT_K3V2_MIN_BLOCKS (48 / VBT_K3V2_WARPS)
 #endif
-#ifndef VBT_K3V2_BATCH
-#define VBT_K3V2_BATCH 2  // predecessors whose gathers are issued together (2 or 4); 4 spills at 32 registers
-#endif
-#ifndef VBT_K3V2_FIRST
-#define VBT_K3V2_FIRST 0  // 1 = the first predecessor of a row is evaluated alone, ahead of the batches
-#endif
 #ifndef VBT_K3V2_PF_DIST
 #define VBT_K3V2_PF_DIST 8
 #endif
 
-#ifndef VBT_K3V2_BULK
-#define VBT_K3V2_BULK 0
-#endif
-#if VBT_K3V2_BULK
-constexpr uint32_t kCandWin = 8;  // candidates per sentence in the bulk-copied window
-#endif
 constexpr int kPredCap = 32;                             // predecessors staged per pass
 constexpr int32_t kPredSentinel = INT32_MAX - 70000;     // + any i16 stays below INT32_MAX and above every real best
 
@@ -908,11 +899,11 @@ struct ConnCol<0> {
             : "r"(right), "r"(stride2), "r"(colbase), "r"(hi));
         return m;
     }
-    // U predecessors of Lattice::search_min_node, staged at shared address `pp` as {cost, right} pairs.  Phase 1
-    // tests every one of them (PRUNE: cost + lb <= best, lb = cost_word >> 16; otherwise: its address lies below
-    // `plim`, the end of this lane's row) and issues the surviving 2-byte gathers together; phase 2 folds them in
-    // row order with `<=`, so the LAST minimum wins.  A bound that is one batch old is still a bound: `best` only
-    // falls.  The shared address of the winner is its token (`besttok`).
+    // Two predecessors of Lattice::search_min_node, staged at shared address `pp` as {cost, right} pairs.  Phase 1
+    // tests both (PRUNE: cost + lb <= best, lb = cost_word >> 16; otherwise: its address lies below `plim`, the end
+    // of this lane's row) and issues the surviving 2-byte gathers together; phase 2 folds them in row order with
+    // `<=`, so the LAST minimum wins.  A bound that is one batch old is still a bound: `best` only falls.  The shared
+    // address of the winner is its token (`besttok`).
 #define VBT_V2_DECL(i) ".reg .pred p" #i ";\n\t.reg .s32 c" #i ", m" #i ";\n\t.reg .u32 r" #i ", l" #i ";\n\t.reg .u64 a" #i ";\n\t"
 #define VBT_V2_TEST_PRUNE(i) "add.s32 t, c" #i ", lb;\n\tsetp.le.s32 p" #i ", t, %0;\n\t"
 #define VBT_V2_TEST_PLAIN(i) "add.u32 l" #i ", %2, " #i "*8;\n\tsetp.lt.u32 p" #i ", l" #i ", %3;\n\t"
@@ -924,21 +915,11 @@ struct ConnCol<0> {
 #define VBT_V2_HEAD "{\n\t.reg .pred q;\n\t.reg .s32 t, lb;\n\t.reg .u32 k;\n\t"
 #define VBT_V2_OPERANDS \
     : "+r"(best), "+r"(besttok) : "r"(pp), "r"(PRUNE ? cost_word : plim), "r"(stride2), "r"(colbase), "r"(hi)
-    template <bool PRUNE>
-    __device__ __forceinline__ void batch1(uint32_t pp, uint32_t cost_word, uint32_t plim, int32_t& best,
-                                           uint32_t& besttok) const {
-        if (PRUNE)
-            asm volatile(VBT_V2_HEAD VBT_V2_DECL(0) "ld.shared.v2.b32 {c0, r0}, [%2];\n\tshr.s32 lb, %3, 16;\n\t"  //
-                         VBT_V2_TEST_PRUNE(0) VBT_V2_LOAD(0) VBT_V2_FOLD(0) "}" VBT_V2_OPERANDS);
-        else
-            asm volatile(VBT_V2_HEAD VBT_V2_DECL(0) "ld.shared.v2.b32 {c0, r0}, [%2];\n\t"  //
-                         VBT_V2_TEST_PLAIN(0) VBT_V2_LOAD(0) VBT_V2_FOLD(0) "}" VBT_V2_OPERANDS);
-    }
     // `zero` is a run-time zero the compiler cannot see through: the first fold reads m0 | (m1 & zero) = m0, one
     // LOP3 that needs BOTH gathers, so the two loads are issued back to back (left alone, ptxas at 32 registers
     // sinks the second load below the first fold and the two round trips serialise).
-#define VBT_V2_FOLD0_JOIN(j) \
-    "lop3.b32 k, m0, m" #j ", %7, 0xF8;\n\t@p0 add.s32 t, c0, k;\n\tsetp.le.and.s32 q, t, %0, p0;\n\t" \
+#define VBT_V2_FOLD0_JOIN \
+    "lop3.b32 k, m0, m1, %7, 0xF8;\n\t@p0 add.s32 t, c0, k;\n\tsetp.le.and.s32 q, t, %0, p0;\n\t" \
     "selp.s32 %0, t, %0, q;\n\tselp.u32 %1, %2, %1, q;\n\t"
     template <bool PRUNE>
     __device__ __forceinline__ void batch2(uint32_t pp, uint32_t cost_word, uint32_t plim, int32_t& best,
@@ -946,28 +927,11 @@ struct ConnCol<0> {
         if (PRUNE)
             asm volatile(VBT_V2_HEAD VBT_V2_DECL(0) VBT_V2_DECL(1) "ld.shared.v4.b32 {c0, r0, c1, r1}, [%2];\n\tshr.s32 lb, %3, 16;\n\t"
                          VBT_V2_TEST_PRUNE(0) VBT_V2_TEST_PRUNE(1) VBT_V2_LOAD(0) VBT_V2_LOAD(1)  //
-                         VBT_V2_FOLD0_JOIN(1) VBT_V2_FOLD(1) "}" VBT_V2_OPERANDS, "r"(zero));
+                         VBT_V2_FOLD0_JOIN VBT_V2_FOLD(1) "}" VBT_V2_OPERANDS, "r"(zero));
         else
             asm volatile(VBT_V2_HEAD VBT_V2_DECL(0) VBT_V2_DECL(1) "ld.shared.v4.b32 {c0, r0, c1, r1}, [%2];\n\t"
                          VBT_V2_TEST_PLAIN(0) VBT_V2_TEST_PLAIN(1) VBT_V2_LOAD(0) VBT_V2_LOAD(1)  //
-                         VBT_V2_FOLD0_JOIN(1) VBT_V2_FOLD(1) "}" VBT_V2_OPERANDS, "r"(zero));
-    }
-    template <bool PRUNE>
-    __device__ __forceinline__ void batch4(uint32_t pp, uint32_t cost_word, uint32_t plim, int32_t& best,
-                                           uint32_t& besttok) const {
-#define VBT_V2_LDS4 "ld.shared.v4.b32 {c0, r0, c1, r1}, [%2];\n\tld.shared.v4.b32 {c2, r2, c3, r3}, [%2+16];\n\t"
-        if (PRUNE)
-            asm volatile(VBT_V2_HEAD VBT_V2_DECL(0) VBT_V2_DECL(1) VBT_V2_DECL(2) VBT_V2_DECL(3) VBT_V2_LDS4 "shr.s32 lb, %3, 16;\n\t"
-                         VBT_V2_TEST_PRUNE(0) VBT_V2_TEST_PRUNE(1) VBT_V2_TEST_PRUNE(2) VBT_V2_TEST_PRUNE(3)  //
-                         VBT_V2_LOAD(0) VBT_V2_LOAD(1) VBT_V2_LOAD(2) VBT_V2_LOAD(3)                          //
-                         "lop3.b32 m1, m1, m2, m3, 0xF0;\n\t" /* = m1, after all three arrived */                     //
-                         VBT_V2_FOLD0_JOIN(1) VBT_V2_FOLD(1) VBT_V2_FOLD(2) VBT_V2_FOLD(3) "}" VBT_V2_OPERANDS, "r"(zero));
-        else
-            asm volatile(VBT_V2_HEAD VBT_V2_DECL(0) VBT_V2_DECL(1) VBT_V2_DECL(2) VBT_V2_DECL(3) VBT_V2_LDS4
-                         VBT_V2_TEST_PLAIN(0) VBT_V2_TEST_PLAIN(1) VBT_V2_TEST_PLAIN(2) VBT_V2_TEST_PLAIN(3)  //
-                         VBT_V2_LOAD(0) VBT_V2_LOAD(1) VBT_V2_LOAD(2) VBT_V2_LOAD(3)                          //
-                         "lop3.b32 m1, m1, m2, m3, 0xF0;\n\t"                                                         //
-                         VBT_V2_FOLD0_JOIN(1) VBT_V2_FOLD(1) VBT_V2_FOLD(2) VBT_V2_FOLD(3) "}" VBT_V2_OPERANDS, "r"(zero));
+                         VBT_V2_FOLD0_JOIN VBT_V2_FOLD(1) "}" VBT_V2_OPERANDS, "r"(zero));
     }
 };
 
@@ -977,26 +941,20 @@ struct ConnCol : ConnRow<CONN> {
     const DictView& dv;
     __device__ __forceinline__ ConnCol(const DictView& d, uint32_t left) : ConnRow<CONN>(d, left), dv(d) {}
     template <bool PRUNE>
-    __device__ __forceinline__ void batch1(uint32_t pp, uint32_t, uint32_t plim, int32_t& best, uint32_t& besttok) const {
-        if (pp < plim) {
-            int2 pr;
-            asm volatile("ld.shared.v2.b32 {%0, %1}, [%2];" : "=r"(pr.x), "=r"(pr.y) : "r"(pp));
-            const int32_t v = int32_t(uint32_t(pr.x) + uint32_t(this->cost(dv, uint32_t(pr.y))));  // i32 wrapping add
-            if (v <= best) {
-                best = v;
-                besttok = pp;
+    __device__ __forceinline__ void batch2(uint32_t pp, uint32_t, uint32_t plim, int32_t& best, uint32_t& besttok) const {
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            const uint32_t p = pp + 8 * i;
+            if (p < plim) {
+                int2 pr;
+                asm volatile("ld.shared.v2.b32 {%0, %1}, [%2];" : "=r"(pr.x), "=r"(pr.y) : "r"(p));
+                const int32_t v = int32_t(uint32_t(pr.x) + uint32_t(this->cost(dv, uint32_t(pr.y))));  // i32 wrapping add
+                if (v <= best) {
+                    best = v;
+                    besttok = p;
+                }
             }
         }
-    }
-    template <bool PRUNE>
-    __device__ __forceinline__ void batch2(uint32_t pp, uint32_t cw, uint32_t plim, int32_t& best, uint32_t& besttok) const {
-#pragma unroll
-        for (int i = 0; i < 2; ++i) batch1<PRUNE>(pp + 8 * i, cw, plim, best, besttok);
-    }
-    template <bool PRUNE>
-    __device__ __forceinline__ void batch4(uint32_t pp, uint32_t cw, uint32_t plim, int32_t& best, uint32_t& besttok) const {
-#pragma unroll
-        for (int i = 0; i < 4; ++i) batch1<PRUNE>(pp + 8 * i, cw, plim, best, besttok);
     }
 };
 
@@ -1010,12 +968,6 @@ struct V2Shared {
     int2 rows[SPW][kPredCap + 4];
     uint4 desc[SPW];
     uint32_t cnt[8];
-#if VBT_K3V2_BULK
-    // candidate windows: the first kCandWin candidates of every sentence's NEXT position, fetched one position ahead
-    // by a bulk asynchronous copy (cp.async.bulk, completion counted on an mbarrier); two buffers alternate
-    uint4 cwin[2][SPW][kCandWin];
-    unsigned long long mbar[2];
-#endif
 };
 
 template <int G, int CONN, bool PRUNE, bool SPACE>
@@ -1026,63 +978,11 @@ __device__ __forceinline__ void viterbi2_sweep(const DictView& d, const Batch& b
     const uint32_t lane = threadIdx.x & 31;
     const uint32_t gl = lane % G, sub = lane / G;
     const uint32_t sidx = ((blockIdx.x * blockDim.x + threadIdx.x) >> 5) * SPW + sub;
-#if VBT_K3V2_BULK
-    constexpr uint32_t kWinOff = kCntOff + 32, kWinBytes = SPW * kCandWin * 16, kBarOff = kWinOff + 2 * kWinBytes;
-    // issues the bulk copy of the first candidates of position `at` into window `buf` (leaders only) and arrives on
-    // that window's barrier; a position without candidates (or past the end) arrives without a copy
-    auto prefetch_candidates = [&](uint32_t at, bool in_sentence, uint32_t buf) {
-        uint32_t nb = 0;
-        uint2 inx = make_uint2(0, 0);
-        if (in_sentence) inx = b.info[at];
-        nb = min(inx.y & ~kInfoSpecial, kCandWin) * 16u;
-        const uint32_t bar = sw + kBarOff + buf * 8u;
-        if (nb) {
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(nb) : "memory");
-            asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                             sw + kWinOff + buf * kWinBytes + sub * (kCandWin * 16u)),
-                         "l"(b.cand + inx.x), "r"(nb), "r"(bar)
-                         : "memory");
-        } else {
-            asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-        }
-    };
-#endif
 
-    uint32_t slot = 0, slot_end = 0;
-    if (sidx < b.n_sent) {
-        const uint32_t s = b.order ? b.order[sidx] : sidx;
-        slot = b.slot_off[s];
-        slot_end = b.slot_off[s + 1] - 1;
-        if (gl == 0) {
-            if (slot == slot_end) {  // Worker::tokenize returns early on an empty sentence (worker.rs:50-52)
-                b.eos[s] = make_uint4(kNone, 0, 0, 0);
-            } else {  // Lattice::insert_bos (lattice.rs:72-83): right_id 0, cost 0
-                const uint32_t eo = b.ends_meta[slot].x;
-                b.ends_hot[eo] = make_int2(0, 0);
-                b.ends_cold[eo] = make_uint4(kNone, kNone, kNone, 0);
-                b.ends_meta[slot].y = eo + 1;
-            }
-        }
-    }
-    __syncwarp();
-#if VBT_K3V2_BULK
-    if (lane == 0) {
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(sw + kBarOff), "r"(SPW) : "memory");
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(sw + kBarOff + 8u), "r"(SPW) : "memory");
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncwarp();
-    uint32_t it = 0;  // iteration of the lockstep walk: window it & 1, barrier parity (it >> 1) & 1
-    if (gl == 0) prefetch_candidates(slot, slot < slot_end, 0);
-#endif
-
+    const uint2 range = begin_sentence(b, sidx, gl);
+    uint32_t slot = range.x, slot_end = range.y;
     uint32_t skip_slot = slot;
     while (__any_sync(kFull, slot < slot_end)) {
-#if VBT_K3V2_BULK
-        // the candidates of the NEXT position start travelling now, into the other window
-        if (gl == 0) prefetch_candidates(slot + 1, slot + 1 < slot_end, (it + 1) & 1);
-#endif
         uint32_t K = 0, eo = 0, cptr = 0, ncand = 0;
         if (slot < slot_end) {  // two independent loads, one round trip
             const uint2 m = b.ends_meta[slot];
@@ -1127,11 +1027,10 @@ __device__ __forceinline__ void viterbi2_sweep(const DictView& d, const Batch& b
         // global -> shared without a register or a scoreboard entry in between) so that it overlaps the loads of
         // the candidates below; the copies are awaited right before the first batch.  Rows are 8-byte aligned only,
         // which rules out the 16-byte granular bulk copies (cp.async.bulk).
-        constexpr uint32_t B = VBT_K3V2_BATCH, F = VBT_K3V2_FIRST;
         const bool one_pass = max_k <= uint32_t(kPredCap);
         if (one_pass && total) {
-            const uint32_t n_stage = F + ((max_k - F + (B - 1u)) & ~(B - 1u));
-            const uint32_t own = sw + sub * kRowBytes + 8u * F;
+            const uint32_t n_stage = (max_k + 1u) & ~1u;
+            const uint32_t own = sw + sub * kRowBytes;
 #pragma unroll 1
             for (uint32_t k = gl; k < n_stage; k += G) {
                 if (k < K)
@@ -1141,15 +1040,6 @@ __device__ __forceinline__ void viterbi2_sweep(const DictView& d, const Batch& b
             }
         }
         __syncwarp();
-#if VBT_K3V2_BULK
-        {  // this position's window: every lane waits every iteration, which also keeps the barrier phases in step
-            const uint32_t bar = sw + kBarOff + (it & 1u) * 8u, parity = (it >> 1) & 1u;
-            asm volatile(
-                "{\n\t.reg .pred p;\n\tWAIT_%=:\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t@p bra DONE_%=;\n\tbra WAIT_%=;\n\tDONE_%=:\n\t}" ::"r"(bar),
-                "r"(parity)
-                : "memory");
-        }
-#endif
         for (uint32_t q0 = 0; q0 < total; q0 += 32) {
             const uint32_t q = q0 + lane;
             const bool valid = q < total;
@@ -1174,14 +1064,7 @@ __device__ __forceinline__ void viterbi2_sweep(const DictView& d, const Batch& b
             uint4 cd = make_uint4(0, 0, 0, 0);
             uint32_t nxt = 0;
             if (valid) {
-#if VBT_K3V2_BULK
-                if (q - before < kCandWin)  // arrived with the window (awaited above)
-                    asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];"
-                                 : "=r"(cd.x), "=r"(cd.y), "=r"(cd.z), "=r"(cd.w)
-                                 : "r"(sw + kWinOff + (it & 1u) * kWinBytes + (s2 * kCandWin + (q - before)) * 16u));
-                else
-#endif
-                    cd = b.cand[ds.x + (q - before)];
+                cd = b.cand[ds.x + (q - before)];
                 nxt = b.ends_meta[cd.w].y;  // next free entry of the row the node ends in: independent of the search
             }
             const ConnCol<CONN> conn(d, cd.x & 0xFFFFu);
@@ -1191,10 +1074,9 @@ __device__ __forceinline__ void viterbi2_sweep(const DictView& d, const Batch& b
 #pragma unroll 1
             for (uint32_t k0 = 0; k0 < max_k; k0 += kPredCap) {
                 // This pass covers predecessors [k0, k0 + kc) of every row, staged by the row's own group and padded
-                // with sentinels to whole batches.  With VBT_K3V2_FIRST the first one is evaluated alone (its total is
-                // the bound the batches start from) and sits one entry in, so that the batches stay 16-byte aligned.
+                // with sentinels to whole batches of two.
                 const uint32_t kc = min(uint32_t(kPredCap), max_k - k0);
-                const uint32_t n_stage = F + ((kc - F + (B - 1u)) & ~(B - 1u));
+                const uint32_t n_stage = (kc + 1u) & ~1u;
                 if (one_pass) {
                     if (q0 == 0) {  // the copies started above have had the candidates' round trip to arrive
                         asm volatile("cp.async.wait_all;" ::: "memory");
@@ -1202,7 +1084,7 @@ __device__ __forceinline__ void viterbi2_sweep(const DictView& d, const Batch& b
                     }
                 } else {  // rows longer than kPredCap: pass after pass, staged synchronously
                     __syncwarp();
-                    const uint32_t own = sw + sub * kRowBytes + 8u * F;
+                    const uint32_t own = sw + sub * kRowBytes;
 #pragma unroll 1
                     for (uint32_t k = gl; k < n_stage; k += G) {
                         int2 pr = make_int2(kPredSentinel, 0);
@@ -1212,75 +1094,19 @@ __device__ __forceinline__ void viterbi2_sweep(const DictView& d, const Batch& b
                     __syncwarp();
                 }
                 // the shared address of a predecessor doubles as its token: index = k0 + (token - row) / 8
-                const uint32_t row = sw + s2 * kRowBytes + 8u * F;
+                const uint32_t row = sw + s2 * kRowBytes;
                 const uint32_t plim = row + (valid ? min(ds.w - min(ds.w, k0), kc) : 0u) * 8u;  // end of this lane's row
                 uint32_t besttok = kNone;
-                if (F) conn.template batch1<PRUNE>(row, cd.y, plim, best, besttok);
                 const uint32_t pend = row + n_stage * 8u;
 #pragma unroll 1
-                for (uint32_t pp = row + 8u * F; pp < pend; pp += 8u * B) {
-                    if (B == 2)
-                        conn.template batch2<PRUNE>(pp, cd.y, plim, best, besttok);
-                    else
-                        conn.template batch4<PRUNE>(pp, cd.y, plim, best, besttok);
-                }
+                for (uint32_t pp = row; pp < pend; pp += 16u) conn.template batch2<PRUNE>(pp, cd.y, plim, best, besttok);
                 if (besttok != kNone) bestk = k0 + ((besttok - row) >> 3);
             }
-            // Lattice::insert_node (lattice.rs:103-127): push into ends[end_word] in candidate order.
-            // End slots of different sentences never coincide, so one warp-wide match suffices.
-            const uint32_t vmask = __ballot_sync(kFull, valid);
-            if (valid) {
-                const uint32_t peers = __match_any_sync(vmask, cd.w);
-                const uint32_t idx = nxt + __popc(peers & lanemask_lt());
-                const int32_t cost = int32_t(uint32_t(best) + uint32_t(int32_t(int16_t(cd.y & 0xFFFFu))));
-                b.ends_hot[idx] = make_int2(cost, int32_t(cd.x >> 16));
-                // lattice.rs:144 keeps the predecessor index as u16
-                b.ends_cold[idx] = make_uint4(ds.y, ds.z + (bestk & 0xFFFFu), cd.z, uint32_t(cost));
-                if (idx == nxt) b.ends_meta[cd.w].y = nxt + __popc(peers);
-            }
-            __syncwarp();
+            insert_node(b, valid, cd, best, ds.y, ds.z, bestk, nxt);
         }
         if (slot < slot_end) ++slot;
-#if VBT_K3V2_BULK
-        ++it;
-#endif
     }
-
-    // Lattice::insert_eos (lattice.rs:85-101): left_id 0, no word cost; lanes of the group = predecessors
-    {
-        const bool has_sentence = sidx < b.n_sent;
-        const uint32_t s = has_sentence ? (b.order ? b.order[sidx] : sidx) : 0;
-        const uint32_t base = has_sentence ? b.slot_off[s] : 0;
-        const uint32_t n = has_sentence ? b.slot_off[s + 1] - 1 - base : 0;
-        const uint32_t eos_start = slot_end - base;  // n, or the start of the trailing space run
-        uint32_t K = 0, eo = 0;
-        if (n > 0) {
-            const uint2 m = b.ends_meta[slot_end];
-            eo = m.x;
-            K = m.y - m.x;
-        }
-        // minimise the signed 64-bit key (cost << 32 | ~index): smallest cost, then the LARGEST index
-        // among ties — the `<=` rule of search_min_node
-        long long bestkey = LLONG_MAX;
-        const ConnCol<CONN> conn_eos(d, 0);  // BOS_EOS_CONNECTION_ID (common.rs:18)
-        const uint32_t max_k = __reduce_max_sync(kFull, K);
-        for (uint32_t k0 = 0; k0 < max_k; k0 += G) {
-            long long key = LLONG_MAX;
-            if (k0 + gl < K) {
-                int2 pr = b.ends_hot[eo + k0 + gl];
-                int32_t v = int32_t(uint32_t(pr.x) + uint32_t(conn_eos.cost(d, uint32_t(pr.y))));
-                key = (long long)(((unsigned long long)uint32_t(v) << 32) | (unsigned long long)(~(k0 + gl)));
-            }
-#pragma unroll
-            for (int o = G / 2; o > 0; o >>= 1) key = min(key, __shfl_xor_sync(kFull, key, o, G));
-            bestkey = min(bestkey, key);
-        }
-        if (n > 0 && gl == 0) {
-            const bool none = K == 0;
-            const uint32_t bestk = (~uint32_t(bestkey)) & 0xFFFFu;  // lattice.rs:144 `i as u16`
-            b.eos[s] = make_uint4(none ? kNone : eo + bestk, eos_start, uint32_t(int32_t(bestkey >> 32)), 0);
-        }
-    }
+    insert_eos<G, ConnCol<CONN>>(d, b, sidx, slot_end, gl);
 }
 
 // PRUNE and its unpruned twin are separate kernels launched back to back (each keeps its own register allocation);
@@ -1289,7 +1115,7 @@ __device__ __forceinline__ void viterbi2_sweep(const DictView& d, const Batch& b
 template <int G, int CONN, bool PRUNE, bool SPACE, bool TWIN>
 __global__ void __launch_bounds__(32 * VBT_K3V2_WARPS, CONN == 0 ? VBT_K3V2_MIN_BLOCKS : (32 / VBT_K3V2_WARPS)) k_viterbi2(DictView d, Batch b) {
     const uint32_t batch_flags = *b.flags;
-    if (batch_flags & kFlagsStandDown) return;
+    if (stand_down(batch_flags)) return;
     if (TWIN && PRUNE == ((batch_flags & kFlagLongSentence) != 0)) return;
     __shared__ __align__(16) V2Shared<G> s_warp[VBT_K3V2_WARPS];
     const uint32_t sp = uint32_t(__cvta_generic_to_shared(&s_warp[threadIdx.x >> 5]));
@@ -1306,7 +1132,7 @@ __global__ void __launch_bounds__(32 * VBT_K3V2_WARPS, CONN == 0 ? VBT_K3V2_MIN_
 // into token records with a warp per sentence — the pointer chase is not repeated and the 24-byte records of a
 // sentence are written by neighbouring lanes.
 __global__ void __launch_bounds__(256) k_backtrack_count(Batch b) {
-    VBT_STAND_DOWN_IF_REJECTED(b);
+    if (stand_down(*b.flags)) return;
     uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= b.n_sent) return;
     uint4 e = b.eos[s];
@@ -1327,7 +1153,7 @@ __global__ void __launch_bounds__(256) k_backtrack_count(Batch b) {
 }
 
 __global__ void __launch_bounds__(256) k_backtrack_write(Batch b) {
-    VBT_STAND_DOWN_IF_REJECTED(b);
+    if (stand_down(*b.flags)) return;
     const uint32_t w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const uint32_t lane = threadIdx.x & 31;
 #pragma unroll 1
