@@ -167,9 +167,9 @@ int32_t vbt_tokenizer_new_from_device_blob(uint64_t d_blob, uint64_t n_bytes, in
  * uploaded once, to devices[0], and broadcast to the others (ncclBroadcast when libnccl.so.2 can be loaded, peer
  * copies otherwise).  vbt_tokenize_batch cuts the batch into contiguous shards of about equal bytes, runs one
  * engine per device on its own host thread (pinned to the GPU's NUMA node) and returns ONE result in input order,
- * identical to a single-device one.  vbt_tokenize_batch_device expects its input on devices[0] and gathers the
- * token records back to it over NVLink (ncclSend / ncclRecv).  Not available on such a tokenizer: a caller-owned
- * stream and the output stage ("output_mode"). */
+ * identical to a single-device one, the text of the output stage ("output_mode") included: each device formats its
+ * shard.  vbt_tokenize_batch_device expects its input on devices[0] and gathers the token records back to it over
+ * NVLink (ncclSend / ncclRecv).  Not available on such a tokenizer: a caller-owned stream. */
 int32_t vbt_tokenizer_new_multi(const vbt_dict *d, int32_t ignore_space, uint64_t max_grouping_len,
                                 const int32_t *devices, int32_t n_devices, vbt_tokenizer **out);
 /* JSON description of how the tokenizer is laid out: {"devices": [...], "dictionary_transport": "nccl 22703" |
@@ -201,7 +201,9 @@ int32_t vbt_result_view_compact(const vbt_result *r, const uint64_t **tok_offset
 /* The output loop of `tokenize` (tokenize/src/main.rs:83-127) for the whole batch, formatted on the device when the
  * tokenizer option "output_mode" was 1 (mecab: `surface\tfeature\n`.. `EOS\n`), 2 (wakati: surfaces joined by ' ',
  * `\n`) or 3 (detail: mecab + lex_type/left_id/right_id/word_cost/total_cost) during vbt_tokenize_batch: sentence i's
- * lines are text[text_offsets[i] .. text_offsets[i+1]).  VBT_ERR_INVALID_ARGUMENT when the option was off. */
+ * lines are text[text_offsets[i] .. text_offsets[i+1]).  Available on every host route: whole batches, the chunked
+ * pipeline of large batches and multi-device tokenizers, with the same bytes on each.  VBT_ERR_INVALID_ARGUMENT when
+ * the option was off.  vbt_tokenize_batch_device produces tokens only, on single- and multi-device tokenizers. */
 int32_t vbt_result_text(const vbt_result *r, const uint64_t **text_offsets, const char **text, uint64_t *n_bytes);
 /* The loop of the `evaluate` tool (evaluate/src/main.rs:61-138): corpus = `surface\tfeature` lines with `EOS`
  * between sentences (Corpus::from_reader, trainer/corpus.rs:78-121); every sentence (its surfaces concatenated) is

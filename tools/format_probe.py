@@ -21,7 +21,7 @@ d = vb.SystemDictionaryBuilder.from_readers(sd.lex_csv, sd.matrix, sd.char_def, 
 tok = vb.Tokenizer.new(d)
 h_utf8 = torch.from_numpy(utf8).pin_memory().numpy()
 h_off = torch.from_numpy(off.astype(np.int64)).pin_memory().numpy().view(np.uint64)
-tok.set_option("chunk_sentences", 0)  # the output stage formats whole batches; compare like with like
+tok.set_option("chunk_sentences", 0)  # the whole-batch route throughout (tools/output_bench.py compares the routes)
 base = None
 for mode in (None, "wakati", "mecab", "detail"):
     tok.output_mode(mode)

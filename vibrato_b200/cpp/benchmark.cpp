@@ -32,15 +32,7 @@ int main(int argc, char** argv) {
     for (int i = 1; i < argc; ++i) {
         std::string a = argv[i];
         if ((a == "-i" || a == "--sysdic") && i + 1 < argc) sysdic = argv[++i];
-        else if (a == "--devices" && i + 1 < argc) {
-            std::string list = argv[++i];
-            for (size_t p = 0; p < list.size();) {
-                size_t q = list.find(',', p);
-                if (q == std::string::npos) q = list.size();
-                devices.push_back(int32_t(std::stol(list.substr(p, q - p))));
-                p = q + 1;
-            }
-        }
+        else if (a == "--devices" && i + 1 < argc) devices = cli::parse_devices(argv[++i]);
         else if (a == "-S" || a == "--ignore-space") ignore_space = true;
         else if ((a == "-M" || a == "--max-grouping-len") && i + 1 < argc) max_grouping_len = std::stoull(argv[++i]);
         else {

@@ -41,6 +41,19 @@ inline bool read_line(std::istream& in, std::string& line) {
     return true;
 }
 
+// --devices 0,1,..: the GPUs one tokenizer spreads every batch over (Tokenizer::devices); an empty list keeps the
+// single-device tokenizer.
+inline std::vector<int32_t> parse_devices(const std::string& list) {
+    std::vector<int32_t> devices;
+    for (size_t p = 0; p < list.size();) {
+        size_t q = list.find(',', p);
+        if (q == std::string::npos) q = list.size();
+        devices.push_back(int32_t(std::stol(list.substr(p, q - p))));
+        p = q + 1;
+    }
+    return devices;
+}
+
 struct Packed {
     std::string utf8;
     std::vector<uint64_t> off{0};

@@ -12,13 +12,16 @@ using namespace vibrato_b200;
 static void usage() {
     std::fprintf(stderr,
                  "tokenize -i <system.dic.zst | mecab-source-dir> [-u user.csv] [-O mecab|wakati|detail] [-S] [-M n]\n"
-                 "         [--format-on device|host]   (where the output text is built; default device)\n");
+                 "         [--format-on device|host]   (where the output text is built; default device)\n"
+                 "         [--devices 0,1,..]          (spread every batch over these GPUs)\n"
+                 "         [--batch-lines N]           (lines per batch when stdin is not a terminal; default 65536)\n");
 }
 
 int main(int argc, char** argv) {
     std::string sysdic, userlex, mode = "mecab", format_on = "device";
     bool ignore_space = false;
-    size_t max_grouping_len = 0;
+    size_t max_grouping_len = 0, batch_lines_arg = 65536;
+    std::vector<int32_t> devices;
     for (int i = 1; i < argc; ++i) {
         std::string a = argv[i];
         auto next = [&]() -> std::string {
@@ -34,10 +37,16 @@ int main(int argc, char** argv) {
         else if (a == "--format-on") format_on = next();
         else if (a == "-S" || a == "--ignore-space") ignore_space = true;
         else if (a == "-M" || a == "--max-grouping-len") max_grouping_len = std::stoull(next());
+        else if (a == "--devices") devices = cli::parse_devices(next());
+        else if (a == "--batch-lines") batch_lines_arg = std::stoull(next());
         else {
             usage();
             return 2;
         }
+    }
+    if (batch_lines_arg == 0) {
+        usage();
+        return 2;
     }
     if (sysdic.empty() || (mode != "mecab" && mode != "wakati" && mode != "detail") ||
         (format_on != "device" && format_on != "host")) {
@@ -52,11 +61,12 @@ int main(int argc, char** argv) {
             std::string csv = cli::slurp(userlex);
             dict = std::move(dict).reset_user_lexicon_from_reader(&csv);
         }
-        Tokenizer tokenizer = Tokenizer(std::move(dict)).ignore_space(ignore_space).max_grouping_len(max_grouping_len);
+        Tokenizer tokenizer =
+            Tokenizer(std::move(dict)).ignore_space(ignore_space).max_grouping_len(max_grouping_len).devices(devices);
         if (format_on == "device") tokenizer.output_mode(mode);  // k_format_len / k_format_write build the text
         std::fprintf(stderr, "Ready to tokenize\n");
         const bool tty_out = isatty(STDOUT_FILENO), tty_in = isatty(STDIN_FILENO);
-        const size_t batch_lines = tty_in ? 1 : 65536;
+        const size_t batch_lines = tty_in ? 1 : batch_lines_arg;
         std::string out;
         cli::Packed pk;
         std::string line;

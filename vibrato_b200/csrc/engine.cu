@@ -55,6 +55,7 @@ struct Control {  // one small block zeroed per batch and read back once
     unsigned long long pool_ctr;
     unsigned long long n_tokens;
     unsigned long long counters[kNumCounters];
+    unsigned long long text_bytes;  // output stage: the text total of the batch (or chunk)
     uint32_t flags;
     uint32_t total_slots;
 };
@@ -129,13 +130,13 @@ __global__ void k_publish_totals(const uint32_t* slot_off, const unsigned long l
     c->n_tokens = tok_off[n_sent];
 }
 
-// Chunked host batches: token offsets of a chunk become global by adding the tokens of all earlier
-// chunks (kept in a device-resident running total so the host never has to wait for it).
+// Chunked host batches: token (and text) offsets of a chunk become global by adding the tokens (text bytes) of all
+// earlier chunks (kept in a device-resident running total so the host never has to wait for it).
 __global__ void k_add_base(unsigned long long* tok_off, uint32_t n_plus_1, const unsigned long long* base) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n_plus_1) tok_off[i] += *base;
 }
-__global__ void k_bump_base(unsigned long long* base, const Control* c) { *base += c->n_tokens; }
+__global__ void k_bump_base(unsigned long long* base, const unsigned long long* by) { *base += *by; }
 __global__ void k_add_value(unsigned long long* tok_off, uint32_t n_plus_1, unsigned long long base) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n_plus_1) tok_off[i] += base;
@@ -155,6 +156,7 @@ struct Workspace {  // every per-(chunk of a)-batch device array; two of them le
 
 struct OutSlot {  // where one (chunk of a) batch leaves its results; two of them alternate in chunked runs
     DevBuf tok_off, tokens, ctrl;
+    DevBuf sent_len, text_off, text;  // output stage (k_format_*)
     Control* h_ctrl = nullptr;
     cudaEvent_t ev[kNumStages + 1];
     cudaEvent_t done = nullptr, drained = nullptr;
@@ -188,6 +190,7 @@ class EngineImpl final : public Engine {
         CK(cudaStreamCreateWithFlags(&aux_stream_, cudaStreamNonBlocking));
         for (auto& e : base_ready_) CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
         tok_base_.ensure(8);
+        text_base_.ensure(8);
         BlobHeader h;
         if (host_blob) {
             if (n_bytes < sizeof(BlobHeader)) throw Error(kInvalidArgument, "dictionary image too small");
@@ -305,9 +308,7 @@ class EngineImpl final : public Engine {
         cudaStreamSynchronize(in_stream_);
         cudaStreamSynchronize(out_stream_);
         for (auto& o : out_) {
-            o.tok_off.release();
-            o.tokens.release();
-            o.ctrl.release();
+            for (DevBuf* b : {&o.tok_off, &o.tokens, &o.ctrl, &o.sent_len, &o.text_off, &o.text}) b->release();
             pinned_free(o.h_ctrl);
             for (auto& ev : o.ev) cudaEventDestroy(ev);
             cudaEventDestroy(o.done);
@@ -321,7 +322,8 @@ class EngineImpl final : public Engine {
         cudaStreamDestroy(in_stream_);
         cudaStreamDestroy(out_stream_);
         tok_base_.release();
-        for (auto* b : {&blob_own_, &in_utf8_, &in_off_, &connid_, &connid_try_, &fmt_len_, &fmt_off_, &fmt_text_off_, &fmt_text_}) b->release();
+        text_base_.release();
+        for (auto* b : {&blob_own_, &in_utf8_, &in_off_, &connid_, &connid_try_}) b->release();
         for (auto& w : ws_) w.release();
         cudaStreamSynchronize(aux_stream_);
         cudaStreamDestroy(aux_stream_);
@@ -441,8 +443,8 @@ class EngineImpl final : public Engine {
         const bool off_pinned = off != byte_off || is_pinned(byte_off);  // rebased_ is ours (pageable, small)
         staged_bytes_ = 0;
         const uint32_t chunk = chunk_sentences_;
-        // the output stage formats the whole batch at once from the device-resident tokens
-        const bool chunked = chunk > 0 && n_sent > chunk + chunk / 2 && output_mode_ == kOutNone;
+        const bool chunked = chunk > 0 && n_sent > chunk + chunk / 2;
+        const bool fmt = output_mode_ != kOutNone;
         for (int attempt = 0;; ++attempt) {
             if (!chunked) {
                 h2d(in_off_.p, off, (size_t(n_sent) + 1) * 8, stream_, off_pinned && off == byte_off);
@@ -471,7 +473,7 @@ class EngineImpl final : public Engine {
                 CK(cudaMemcpyAsync(r->tok_off, o.tok_off.p, (size_t(n_sent) + 1) * 8, cudaMemcpyDeviceToHost, stream_));
                 if (r->n_tokens) CK(cudaMemcpyAsync(r->tokens, o.tokens.p, r->n_tokens * tok_bytes_, cudaMemcpyDeviceToHost, stream_));
                 r->has_text = false;
-                if (output_mode_ != kOutNone) format_text(d_utf8, d_off, n_sent, o, r);
+                if (fmt) format_text(d_utf8, d_off, n_sent, r);
                 CK(cudaStreamSynchronize(stream_));
                 return r;
             }
@@ -507,6 +509,18 @@ class EngineImpl final : public Engine {
             }
             // a pinned result sized from the learned tokens-per-byte ratio (grown below if short)
             HostResult* r = acquire(n_sent, uint64_t(double(n_bytes) * tok_per_byte_) + 1024);
+            // output stage: each slot's text buffer holds the text a chunk is expected to produce (at most 4 bytes per
+            // sentence plus the learned ratio per input byte); a chunk with more text flags itself and the batch is
+            // re-run with the ratio it measured
+            const double text_ratio = text_per_byte_[output_mode_];
+            if (fmt) {
+                for (int i = 0; i < 2; ++i) {
+                    ensure_format(out_[i], ws_[dual_stream_ ? i : 0], max_chunk_sent);
+                    out_[i].text.ensure(size_t(double(max_chunk_bytes) * text_ratio) + size_t(max_chunk_sent) * 4 + 4096);
+                }
+                ensure_text(r, n_sent, uint64_t(double(n_bytes) * text_ratio) + uint64_t(n_sent) * 4 + 1024);
+                CK(cudaMemsetAsync(text_base_.p, 0, 8, stream_));
+            }
             CK(cudaMemsetAsync(tok_base_.p, 0, 8, stream_));
             connid_begin(stream_);
             h2d(in_off_.p, off, (size_t(n_sent) + 1) * 8, stream_, off_pinned && off == byte_off);
@@ -516,9 +530,10 @@ class EngineImpl final : public Engine {
             std::memset(stage_ms_, 0, sizeof(stage_ms_));
             std::memset(counters_, 0, sizeof(counters_));
             launches_ = 0;
-            uint64_t tok_total = 0;
+            uint64_t tok_total = 0, text_total = 0;
+            double text_need = 0;  // text bytes per input byte beyond 4 per sentence, largest over the sound chunks
             uint32_t route = kRouteNone;
-            bool overflow = false, bad_utf8 = false, bad_offsets = false, slots_overflow = false;
+            bool overflow = false, bad_utf8 = false, bad_offsets = false, slots_overflow = false, text_overflow = false;
             uint64_t slots_seen = 0;
             batch_total_bytes_ = n_bytes;
             std::vector<cudaEvent_t>& h2d_ev = h2d_events(n_chunks);
@@ -542,6 +557,7 @@ class EngineImpl final : public Engine {
                 if (o.h_ctrl->flags & kFlagBadOffsets) bad_offsets = true;
                 if (o.h_ctrl->flags & kFlagPoolOverflow) overflow = true;
                 if (o.h_ctrl->flags & kFlagSlotsOverflow) overflow = slots_overflow = true;
+                if (o.h_ctrl->flags & kFlagTextOverflow) text_overflow = true;
                 slots_seen += o.h_ctrl->total_slots;
                 for (int i = 0; i < kNumStages; ++i) {
                     float ms = 0;
@@ -554,8 +570,10 @@ class EngineImpl final : public Engine {
                 if (counting_)
                     for (int i = 0; i < kNumCounters; ++i) counters_[i] += o.h_ctrl->counters[i];
                 pool_need_ = std::max<uint64_t>(pool_need_, o.h_ctrl->pool_ctr);
-                const uint64_t nt = o.h_ctrl->n_tokens;
-                if (!overflow && !bad_utf8 && !bad_offsets) {
+                const uint64_t nt = o.h_ctrl->n_tokens, nx = fmt ? o.h_ctrl->text_bytes : 0;
+                if (fmt && !(o.h_ctrl->flags & (kFlagsStandDown | kFlagUtf8Error | kFlagPoolOverflow)))
+                    text_need = std::max(text_need, (double(nx) - 4.0 * (s1 - s0)) / double(std::max<uint64_t>(1, off[s1] - off[s0])));
+                if (!overflow && !text_overflow && !bad_utf8 && !bad_offsets) {
                     if ((tok_total + nt) * tok_bytes_ > r->cap_tok) {  // rare: grow the pinned buffer, keep what is there
                         CK(cudaStreamSynchronize(out_stream_));
                         size_t cap = size_t(double((tok_total + nt) * 24) * 1.5) + 4096;
@@ -571,9 +589,24 @@ class EngineImpl final : public Engine {
                     if (nt)
                         CK(cudaMemcpyAsync(static_cast<uint8_t*>(r->tokens) + tok_total * tok_bytes_, o.tokens.p, nt * tok_bytes_,
                                            cudaMemcpyDeviceToHost, out_stream_));
+                    if (fmt) {
+                        if (text_total + nx + 1 > r->cap_text) {  // grown like the token buffer
+                            CK(cudaStreamSynchronize(out_stream_));
+                            size_t cap = size_t(double(text_total + nx) * 1.5) + 4096;
+                            char* bigger = static_cast<char*>(pinned_alloc(cap));
+                            std::memcpy(bigger, r->text, text_total);
+                            pinned_free(r->text);
+                            r->text = bigger;
+                            r->cap_text = cap;
+                        }
+                        CK(cudaMemcpyAsync(r->text_off + s0, o.text_off.p, (size_t(s1 - s0) + (last ? 1 : 0)) * 8,
+                                           cudaMemcpyDeviceToHost, out_stream_));
+                        if (nx) CK(cudaMemcpyAsync(r->text + text_total, o.text.p, nx, cudaMemcpyDeviceToHost, out_stream_));
+                    }
                 }
                 CK(cudaEventRecord(o.drained, out_stream_));
                 tok_total += nt;
+                text_total += nx;
             };
             pool_need_ = 0;
             for (uint32_t c = 0; c < n_chunks; ++c) {
@@ -586,7 +619,8 @@ class EngineImpl final : public Engine {
                 CK(cudaStreamWaitEvent(w.stream, h2d_ev[c], 0));
                 if (c >= 2) CK(cudaStreamWaitEvent(w.stream, o.drained, 0));  // slot reused: its D2H must be done
                 enqueue(w, d_utf8, d_off + s0, s1 - s0, off[s1] - off[s0], o, tok_base_.as<unsigned long long>(),
-                        c >= 1 ? base_ready_[(c - 1) & 1] : nullptr, base_ready_[c & 1]);
+                        fmt ? text_base_.as<unsigned long long>() : nullptr, c >= 1 ? base_ready_[(c - 1) & 1] : nullptr,
+                        base_ready_[c & 1]);
                 if (!utf8_pinned && c + 1 < n_chunks) issue_h2d(c + 1);
                 if (c >= 1) drain(c - 1);
             }
@@ -603,20 +637,25 @@ class EngineImpl final : public Engine {
                 release(r);
                 throw Error(kUtf8, "stream did not contain valid UTF-8");
             }
-            if (overflow) {
+            if (overflow || text_overflow) {
                 release(r);
-                if (attempt >= 3) throw Error(kInternal, "candidate pool overflow persists");
+                if (attempt >= 3) throw Error(kInternal, overflow ? "candidate pool overflow persists" : "text buffer overflow persists");
                 if (slots_overflow) chars_per_byte_ = 1.0;
-                cand_per_byte_ = std::max(cand_per_byte_ * 1.5, double(pool_need_) / double(std::max<uint64_t>(1, max_chunk_bytes)) * 1.2);
+                if (overflow)
+                    cand_per_byte_ = std::max(cand_per_byte_ * 1.5, double(pool_need_) / double(std::max<uint64_t>(1, max_chunk_bytes)) * 1.2);
+                if (text_overflow) text_per_byte_[output_mode_] = std::max(text_ratio * 1.5, text_need * 1.05);
                 continue;
             }
             if (max_chunk_bytes)
                 cand_per_byte_ = std::max(0.25, double(pool_need_) / double(max_chunk_bytes) * 1.25);
             if (n_bytes) tok_per_byte_ = std::max(0.02, double(tok_total) / double(n_bytes) * 1.1);
             if (n_bytes) chars_per_byte_ = std::min(1.0, double(slots_seen - n_sent) / double(n_bytes) * 1.10);
+            if (fmt) text_per_byte_[output_mode_] = std::max(0.5, text_need * 1.25);
             connid_commit(stream_);
             last_route_ = route;
             r->n_tokens = tok_total;
+            r->has_text = fmt;
+            r->text_bytes = text_total;
             return r;
         }
     }
@@ -626,7 +665,7 @@ class EngineImpl final : public Engine {
     }
 
     // ---- shard-level entry points (multi_engine.cu) -------------------------------------------------
-    uint64_t run_shard(const char* utf8, const uint64_t* byte_off, uint64_t n_sent64, int src_device) override {
+    uint64_t run_shard(const char* utf8, const uint64_t* byte_off, uint64_t n_sent64, int src_device, uint64_t* text_bytes) override {
         CK(cudaSetDevice(device_));
         const uint64_t first = n_sent64 ? byte_off[0] : 0;
         const uint64_t n_bytes = n_sent64 ? byte_off[n_sent64] - first : 0;
@@ -651,6 +690,9 @@ class EngineImpl final : public Engine {
         }
         run_whole(in_utf8_.as<uint8_t>(), in_off_.as<unsigned long long>(), n_sent, n_bytes);
         shard_n_sent_ = n_sent;
+        shard_text_ = text_bytes && output_mode_ != kOutNone;
+        shard_text_bytes_ = shard_text_ ? format_whole(in_utf8_.as<uint8_t>(), in_off_.as<unsigned long long>(), n_sent) : 0;
+        if (text_bytes) *text_bytes = shard_text_bytes_;
         return out_[0].h_ctrl->n_tokens;
     }
     void rebase_shard(uint64_t tok_base) override {
@@ -660,7 +702,8 @@ class EngineImpl final : public Engine {
                                                                          shard_n_sent_ + 1, tok_base);
         CK(cudaStreamSynchronize(stream_));
     }
-    void fetch_shard(uint64_t* h_tok_off, void* h_tokens, uint64_t tok_base, bool last) override {
+    void fetch_shard(uint64_t* h_tok_off, void* h_tokens, uint64_t tok_base, bool last, uint64_t* h_text_off, char* h_text,
+                     uint64_t text_base) override {
         CK(cudaSetDevice(device_));
         OutSlot& o = out_[0];
         if (tok_base)
@@ -669,6 +712,14 @@ class EngineImpl final : public Engine {
         CK(cudaMemcpyAsync(h_tok_off, o.tok_off.p, (size_t(shard_n_sent_) + (last ? 1 : 0)) * 8, cudaMemcpyDeviceToHost, stream_));
         if (o.h_ctrl->n_tokens)
             CK(cudaMemcpyAsync(h_tokens, o.tokens.p, o.h_ctrl->n_tokens * tok_bytes_, cudaMemcpyDeviceToHost, stream_));
+        if (h_text_off) {
+            if (!shard_text_) throw Error(kInternal, "the shard was run without its text");
+            unsigned long long* text_off = o.text_off.as<unsigned long long>();
+            const uint64_t n_text = shard_text_bytes_;
+            if (text_base) k_add_value<<<(shard_n_sent_ + 256) / 256, 256, 0, stream_>>>(text_off, shard_n_sent_ + 1, text_base);
+            CK(cudaMemcpyAsync(h_text_off, text_off, (size_t(shard_n_sent_) + (last ? 1 : 0)) * 8, cudaMemcpyDeviceToHost, stream_));
+            if (n_text) CK(cudaMemcpyAsync(h_text, o.text.p, n_text, cudaMemcpyDeviceToHost, stream_));
+        }
         CK(cudaStreamSynchronize(stream_));
     }
     void shard_outputs(uint64_t* d_tok_off, uint64_t* d_tokens) const override {
@@ -772,54 +823,76 @@ class EngineImpl final : public Engine {
         return r;
     }
 
-    // Output stage: size every token's text, scan, copy bytes (k_format_len / k_format_write), D2H into `r`.
-    void format_text(const uint8_t* d_utf8, const unsigned long long* d_off, uint32_t n_sent, OutSlot& o, HostResult* r) {
-        const uint64_t n_tok = r->n_tokens;
-        fmt_len_.ensure((n_tok + 1) * 4, 1.25);
-        fmt_off_.ensure((n_tok + 1) * 8, 1.25);
-        fmt_text_off_.ensure((size_t(n_sent) + 1) * 8, 1.25);
+    // Output stage buffers of slot `o` and scan storage of `w` for (chunks of) up to n_sent sentences.
+    void ensure_format(OutSlot& o, Workspace& w, uint32_t n_sent) {
+        o.sent_len.ensure((size_t(n_sent) + 1) * 8, 1.25);
+        o.text_off.ensure((size_t(n_sent) + 1) * 8, 1.25);
+        size_t tmp = 0;
+        CK(cub::DeviceScan::ExclusiveSum(nullptr, tmp, static_cast<unsigned long long*>(nullptr),
+                                         static_cast<unsigned long long*>(nullptr), size_t(n_sent) + 1, w.stream));
+        w.scan_tmp.ensure(tmp + 1024, 1.5);
+    }
+
+    // Output stage, pass 1 and the scan on w.stream: o.text_off = where each sentence's text starts in o.text
+    // (n_sent + 1 entries, relative to the batch or chunk in `o`).  Returns the arguments of pass 2.
+    FormatArgs format_offsets(Workspace& w, const uint8_t* d_utf8, const unsigned long long* d_off, uint32_t n_sent, OutSlot& o) {
         FormatArgs f{};
         f.utf8 = d_utf8;
         f.byte_off = d_off;
         f.n_sent = n_sent;
         f.tok_off = o.tok_off.as<unsigned long long>();
         f.tokens = o.tokens.as<uint2>();
-        f.tok_len = fmt_len_.as<uint32_t>();
-        f.tok_text_off = fmt_off_.as<unsigned long long>();
-        f.text_off = fmt_text_off_.as<unsigned long long>();
+        f.sent_len = o.sent_len.as<unsigned long long>();
+        f.text_off = o.text_off.as<unsigned long long>();
+        f.text = o.text.as<uint8_t>();
+        f.text_cap = o.text.cap;
+        Control* dc = o.ctrl.as<Control>();
+        f.flags = &dc->flags;
+        f.text_total = &dc->text_bytes;
         f.mode = output_mode_;
-        CK(cudaMemsetAsync(fmt_len_.as<uint32_t>() + n_tok, 0, 4, stream_));
-        launch_format_len(dv_, f, stream_);
-        {
-            cub::TransformInputIterator<unsigned long long, CastU64, const uint32_t*> it(fmt_len_.as<uint32_t>(), CastU64());
-            size_t tmp = 0;
-            CK(cub::DeviceScan::ExclusiveSum(nullptr, tmp, it, fmt_off_.as<unsigned long long>(), n_tok + 1, stream_));
-            ws_[0].scan_tmp.ensure(tmp + 1024, 1.5);
-            ws_[0].stream = stream_;
-            exclusive_scan(ws_[0], it, fmt_off_.as<unsigned long long>(), n_tok + 1);
-        }
-        unsigned long long tok_bytes = 0;
-        CK(cudaMemcpyAsync(&tok_bytes, fmt_off_.as<unsigned long long>() + n_tok, 8, cudaMemcpyDeviceToHost, stream_));
+        CK(cudaMemsetAsync(f.sent_len + n_sent, 0, 8, w.stream));
+        launch_format_len(dv_, f, w.stream);
+        exclusive_scan(w, f.sent_len, f.text_off, size_t(n_sent) + 1);
+        return f;
+    }
+
+    // Output stage of a whole batch (or shard) that run_whole left in out_[0]: the text buffer is sized from the
+    // exact total, read back with one synchronisation.  Returns the text's bytes.
+    uint64_t format_whole(const uint8_t* d_utf8, const unsigned long long* d_off, uint32_t n_sent) {
+        OutSlot& o = out_[0];
+        ensure_format(o, ws_[0], n_sent);
+        FormatArgs f = format_offsets(ws_[0], d_utf8, d_off, n_sent, o);
+        unsigned long long total = 0;
+        CK(cudaMemcpyAsync(&total, f.text_off + n_sent, 8, cudaMemcpyDeviceToHost, stream_));
         CK(cudaStreamSynchronize(stream_));
-        const uint64_t term = output_mode_ == kOutWakati ? 1 : 4;
-        const uint64_t total = tok_bytes + term * n_sent;
-        fmt_text_.ensure(total + 16, 1.25);
-        f.text = fmt_text_.as<uint8_t>();
-        if (n_sent == 0) CK(cudaMemsetAsync(fmt_text_off_.p, 0, 8, stream_));
+        o.text.ensure(total + 16, 1.25);
+        f.text = o.text.as<uint8_t>();
+        f.text_cap = o.text.cap;
         launch_format_write(dv_, f, stream_);
         launches_ += 2;
-        if ((size_t(n_sent) + 1) * 8 > r->cap_text_off) {
+        return total;
+    }
+
+    // Pinned text arrays of `r` for n_sent sentences and text_bytes bytes (contents not kept).
+    static void ensure_text(HostResult* r, uint64_t n_sent, uint64_t text_bytes) {
+        if ((n_sent + 1) * 8 > r->cap_text_off) {
             pinned_free(r->text_off);
-            r->cap_text_off = size_t(double((size_t(n_sent) + 1) * 8) * 1.25) + 64;
+            r->cap_text_off = size_t(double((n_sent + 1) * 8) * 1.25) + 64;
             r->text_off = static_cast<uint64_t*>(pinned_alloc(r->cap_text_off));
         }
-        if (total + 1 > r->cap_text) {
+        if (text_bytes + 1 > r->cap_text) {
             pinned_free(r->text);
-            r->cap_text = size_t(double(total + 1) * 1.25) + 64;
+            r->cap_text = size_t(double(text_bytes + 1) * 1.25) + 64;
             r->text = static_cast<char*>(pinned_alloc(r->cap_text));
         }
-        CK(cudaMemcpyAsync(r->text_off, fmt_text_off_.p, (size_t(n_sent) + 1) * 8, cudaMemcpyDeviceToHost, stream_));
-        if (total) CK(cudaMemcpyAsync(r->text, fmt_text_.p, total, cudaMemcpyDeviceToHost, stream_));
+    }
+
+    // Output stage of the whole-batch host path: format, then D2H into `r` on stream_.
+    void format_text(const uint8_t* d_utf8, const unsigned long long* d_off, uint32_t n_sent, HostResult* r) {
+        const uint64_t total = format_whole(d_utf8, d_off, n_sent);
+        ensure_text(r, n_sent, total);
+        CK(cudaMemcpyAsync(r->text_off, out_[0].text_off.p, (size_t(n_sent) + 1) * 8, cudaMemcpyDeviceToHost, stream_));
+        if (total) CK(cudaMemcpyAsync(r->text, out_[0].text.p, total, cudaMemcpyDeviceToHost, stream_));
         r->text_bytes = total;
         r->has_text = true;
     }
@@ -880,7 +953,7 @@ class EngineImpl final : public Engine {
             o.tok_off.ensure((size_t(n_sent) + 1) * 8, 1.25);
             o.tokens.ensure(size_t(n_bytes) * 24 + 24, 1.25);  // a token spans >= 1 character >= 1 byte
             connid_begin(stream_);
-            enqueue(ws_[0], d_utf8, d_off, n_sent, n_bytes, o, nullptr, nullptr, nullptr);
+            enqueue(ws_[0], d_utf8, d_off, n_sent, n_bytes, o, nullptr, nullptr, nullptr, nullptr);
             CK(cudaEventSynchronize(o.done));
             CK(cudaGetLastError());
             if (o.h_ctrl->flags & kFlagBadOffsets)
@@ -911,9 +984,12 @@ class EngineImpl final : public Engine {
     }
 
     // Queues the whole kernel sequence for one (chunk of a) batch on stream_; no host synchronisation.
-    // `tok_base` (device) makes the chunk's token offsets global and is advanced by its token count.
+    // `tok_base` (device) makes the chunk's token offsets global and is advanced by its token count.  `text_base`
+    // (device, chunked runs with the output stage only) does the same for the chunk's text, which is formatted into
+    // o.text up to its capacity (kFlagTextOverflow beyond).
     void enqueue(Workspace& w, const uint8_t* d_utf8, const unsigned long long* d_off, uint32_t n_sent, uint64_t n_bytes,
-                 OutSlot& o, unsigned long long* tok_base, cudaEvent_t base_wait, cudaEvent_t base_signal) {
+                 OutSlot& o, unsigned long long* tok_base, unsigned long long* text_base, cudaEvent_t base_wait,
+                 cudaEvent_t base_signal) {
         cudaStream_t st = w.stream;
         // characters <= bytes is the hard bound; the per-character launches are sized from the ratio learned on
         // earlier batches (plus slack), and a batch that exceeds it flags itself and is re-run with the hard bound
@@ -1004,12 +1080,22 @@ class EngineImpl final : public Engine {
         CK(cudaEventRecord(o.ev[8], st));
         launch_backtrack_write(b, st);
         k_publish_totals<<<1, 1, 0, st>>>(b.slot_off, b.tok_off, n_sent, dc);
+        if (text_base) {  // output stage of a chunk: formatted while its token offsets are still chunk-local
+            FormatArgs f = format_offsets(w, d_utf8, d_off, n_sent, o);
+            launch_format_write(dv_, f, st);
+            o.launches += 2;
+        }
         if (tok_base) {
             if (base_wait) CK(cudaStreamWaitEvent(st, base_wait, 0));  // the previous chunk (other stream) bumped it
             k_add_base<<<(n_sent + 256) / 256, 256, 0, st>>>(b.tok_off, n_sent + 1, tok_base);
-            k_bump_base<<<1, 1, 0, st>>>(tok_base, dc);
-            if (base_signal) CK(cudaEventRecord(base_signal, st));
+            k_bump_base<<<1, 1, 0, st>>>(tok_base, &dc->n_tokens);
             o.launches += 2;
+            if (text_base) {
+                k_add_base<<<(n_sent + 256) / 256, 256, 0, st>>>(o.text_off.as<unsigned long long>(), n_sent + 1, text_base);
+                k_bump_base<<<1, 1, 0, st>>>(text_base, &dc->text_bytes);
+                o.launches += 2;
+            }
+            if (base_signal) CK(cudaEventRecord(base_signal, st));
         }
         CK(cudaEventRecord(o.ev[9], st));
         CK(cudaMemcpyAsync(o.h_ctrl, dc, sizeof(Control), cudaMemcpyDeviceToHost, st));
@@ -1030,11 +1116,13 @@ class EngineImpl final : public Engine {
     HostResult* eager_sink_ = nullptr;
     uint64_t staged_bytes_ = 0;  // bytes of pageable caller memory that went through the ring (last batch)
     uint32_t shard_n_sent_ = 0;
+    bool shard_text_ = false;  // the last shard was formatted: shard_text_bytes_ of text in out_[0].text
+    uint64_t shard_text_bytes_ = 0;
     cudaStream_t stream_ = nullptr, own_stream_ = nullptr, in_stream_ = nullptr, out_stream_ = nullptr;
     cudaEvent_t in_done_ = nullptr;
     std::vector<cudaEvent_t> h2d_ev_;
     OutSlot out_[2];
-    DevBuf tok_base_;
+    DevBuf tok_base_, text_base_;
     uint32_t chunk_sentences_ = 262144;
     uint64_t pool_need_ = 0;
     double tok_per_byte_ = 0.2;
@@ -1055,7 +1143,9 @@ class EngineImpl final : public Engine {
     int order_mode_ = 0;  // K3's sentence order: 0 input order, 1 whole batch by length, 2 by length inside tiles
     uint32_t output_mode_ = 0;
     uint64_t batch_total_bytes_ = 0;  // size of the input buffer of the batch in flight (bounds check in K1a)
-    DevBuf fmt_len_, fmt_off_, fmt_text_off_, fmt_text_;
+    // output text bytes expected per input byte (beyond 4 per sentence), by output mode: sizes the text buffers of
+    // the chunked host pipeline, learned like cand_per_byte_
+    double text_per_byte_[4] = {0.0, 8.0, 2.0, 16.0};
     bool dual_stream_ = false;
     int lanes_ = 16;  // fastest on H100 for ~40-character and 512-character sentences alike (DESIGN.md §4)
     uint32_t tok_bytes_ = 24;

@@ -50,11 +50,15 @@ class Engine {
     // Building blocks of the multi-device engine (multi_engine.cu); a single-device caller never needs them.
     // run_shard: host sentences in, tokens left in this device's memory; returns their number (synchronises).
     // With src_device >= 0 `utf8` is a DEVICE address on that device (peer copy over NVLink) while byte_off is
-    // still a host array.
-    virtual uint64_t run_shard(const char* utf8, const uint64_t* byte_off, uint64_t n_sent, int src_device) = 0;
+    // still a host array.  With text_bytes != nullptr the shard's output text is formatted too ("output_mode";
+    // *text_bytes = its size, 0 when the option is off).
+    virtual uint64_t run_shard(const char* utf8, const uint64_t* byte_off, uint64_t n_sent, int src_device,
+                               uint64_t* text_bytes) = 0;
     // fetch_shard: the last shard's token offsets (+ tok_base, n_sent entries, one more when `last`) and token
-    // records into host memory (pinned, or it is slow).
-    virtual void fetch_shard(uint64_t* h_tok_off, void* h_tokens, uint64_t tok_base, bool last) = 0;
+    // records into host memory (pinned, or it is slow); with h_text_off != nullptr also its text offsets
+    // (+ text_base, same count) and text, which run_shard must have formatted.
+    virtual void fetch_shard(uint64_t* h_tok_off, void* h_tokens, uint64_t tok_base, bool last, uint64_t* h_text_off,
+                             char* h_text, uint64_t text_base) = 0;
     // Device addresses of the last shard's token offsets (uint64[n_sent + 1], already + tok_base after
     // rebase_shard) and token records.
     virtual void rebase_shard(uint64_t tok_base) = 0;
@@ -66,7 +70,7 @@ class Engine {
     virtual void set_counting(bool on) = 0;
     // Knobs: "lanes_per_sentence" (4/8/16/32), "sort_by_length" (0/1), "counting" (0/1), "chunk_sentences",
     // "dual_stream", "connid_counting", "output_mode" (0 none, 1 mecab, 2 wakati, 3 detail: run_host also
-    // produces HostResult::text).
+    // produces HostResult::text, on every host route; run_device stays token-only).
     virtual void set_option(const std::string& name, long long value) = 0;
     // Launch on a caller-owned CUDA stream (0 restores the engine's own stream).
     virtual void set_stream(uint64_t stream) = 0;

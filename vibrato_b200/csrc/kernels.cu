@@ -1190,7 +1190,9 @@ __global__ void __launch_bounds__(256) k_backtrack_write(Batch b) {
 //   mecab : {surface}\t{feature}\n per token, then EOS\n
 //   wakati: surfaces joined by one space, then \n
 //   detail: {surface}\t{feature}\tlex_type={:?}\tleft_id={}\tright_id={}\tword_cost={}\ttotal_cost={}\n, then EOS\n
-// One warp per sentence.  Pass 1 sizes every token, a scan places it, pass 2 copies bytes.
+// One warp per sentence.  Pass 1 sizes every sentence, a scan over sentences places it, pass 2 places the tokens
+// inside their sentence with a warp scan and copies bytes.  Both passes need only the tokens of their own sentence,
+// so a chunk of a batch formats with chunk-local token offsets.
 // ---------------------------------------------------------------------------------------------
 
 __device__ __forceinline__ uint32_t dec_len(uint32_t v) {
@@ -1261,21 +1263,27 @@ __device__ __forceinline__ uint32_t detail_tail_len(const DictView& d, const Tok
            dec_len_signed(int32_t(int16_t(pr.y & 0xFFFFu))) + 12 + dec_len_signed(x.total_cost);
 }
 
+// Bytes token t contributes to its sentence's text (separators included, the sentence terminator not).
+__device__ __forceinline__ uint32_t token_text_len(const DictView& d, const TokenText& x, uint32_t mode, bool first) {
+    if (mode == kOutWakati) return x.surf_len + (first ? 0u : 1u);
+    if (mode == kOutMecab) return x.surf_len + 1 + x.feat_len + 1;
+    return x.surf_len + 1 + x.feat_len + detail_tail_len(d, x) + 1;
+}
+
+// The stage runs only on a batch whose tokens are sound: after an input error or an overflow the engine drops or
+// re-runs the batch anyway, and its token records may then point anywhere.
+__device__ __forceinline__ bool format_stands_down(const FormatArgs& f) {
+    return *f.flags & (kFlagsStandDown | kFlagUtf8Error | kFlagPoolOverflow);
+}
+
 __global__ void __launch_bounds__(256) k_format_len(DictView d, FormatArgs f) {
     const uint32_t s = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-    if (s >= f.n_sent) return;
+    if (s >= f.n_sent || format_stands_down(f)) return;
     const unsigned long long t0 = f.tok_off[s], t1 = f.tok_off[s + 1];
-    for (unsigned long long t = t0 + lane; t < t1; t += 32) {
-        const TokenText x = token_text(d, f.tokens, t);
-        uint32_t len;
-        if (f.mode == kOutWakati)
-            len = x.surf_len + (t != t0 ? 1u : 0u);
-        else if (f.mode == kOutMecab)
-            len = x.surf_len + 1 + x.feat_len + 1;
-        else
-            len = x.surf_len + 1 + x.feat_len + detail_tail_len(d, x) + 1;
-        f.tok_len[t] = len;
-    }
+    unsigned long long len = 0;
+    for (unsigned long long t = t0 + lane; t < t1; t += 32) len += token_text_len(d, token_text(d, f.tokens, t), f.mode, t == t0);
+    for (int k = 16; k > 0; k >>= 1) len += __shfl_xor_sync(kFull, len, k);
+    if (lane == 0) f.sent_len[s] = len + (f.mode == kOutWakati ? 1 : 4);  // "\n" or "EOS\n"
 }
 
 __device__ __forceinline__ void warp_copy(uint8_t* __restrict__ dst, const uint8_t* __restrict__ src, uint32_t n, uint32_t lane) {
@@ -1284,24 +1292,32 @@ __device__ __forceinline__ void warp_copy(uint8_t* __restrict__ dst, const uint8
 
 __global__ void __launch_bounds__(256) k_format_write(DictView d, FormatArgs f) {
     const uint32_t s = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-    if (s >= f.n_sent) return;
-    const unsigned long long t0 = f.tok_off[s], t1 = f.tok_off[s + 1];
-    const uint32_t term = f.mode == kOutWakati ? 1 : 4;  // "\n" or "EOS\n"
-    const unsigned long long shift = (unsigned long long)term * s;  // terminators of the sentences before
-    const uint8_t* __restrict__ sent = f.utf8 + f.byte_off[s];
-    if (lane == 0) {
-        f.text_off[s] = f.tok_text_off[t0] + shift;
-        if (s + 1 == f.n_sent) f.text_off[s + 1] = f.tok_text_off[t1] + shift + term;
+    if (s >= f.n_sent || format_stands_down(f)) return;
+    const unsigned long long total = f.text_off[f.n_sent];
+    if (s == 0 && lane == 0) {
+        *f.text_total = total;
+        if (total > f.text_cap) atomicOr(f.flags, kFlagTextOverflow);
     }
+    if (total > f.text_cap) return;  // every warp sees the same total: nothing is written
+    const unsigned long long t0 = f.tok_off[s], t1 = f.tok_off[s + 1];
+    const uint8_t* __restrict__ sent = f.utf8 + f.byte_off[s];
+    unsigned long long base = f.text_off[s];  // where the next group of 32 tokens starts
     for (unsigned long long c = t0; c < t1; c += 32) {
         // lane i stages token c + i; the copies below take one token at a time with all 32 lanes
         const uint32_t cnt = uint32_t(min(32ull, t1 - c));
         TokenText mine = {0, 0, 0, 0, 0, 0, 0};
-        unsigned long long at = 0;
+        uint32_t len = 0;
         if (lane < cnt) {
             mine = token_text(d, f.tokens, c + lane);
-            at = f.tok_text_off[c + lane] + shift;
+            len = token_text_len(d, mine, f.mode, c + lane == t0);
         }
+        unsigned long long incl = len;  // inclusive warp scan of the group's lengths
+        for (int k = 1; k < 32; k <<= 1) {
+            const unsigned long long v = __shfl_up_sync(kFull, incl, k);
+            if (lane >= uint32_t(k)) incl += v;
+        }
+        const unsigned long long at = base + incl - len;
+        base += __shfl_sync(kFull, incl, 31);
         for (uint32_t j = 0; j < cnt; ++j) {
             TokenText x;
             x.start_byte = __shfl_sync(kFull, mine.start_byte, j);
@@ -1345,7 +1361,7 @@ __global__ void __launch_bounds__(256) k_format_write(DictView d, FormatArgs f) 
         }
     }
     if (lane == 0) {
-        uint8_t* dst = f.text + f.tok_text_off[t1] + shift;
+        uint8_t* dst = f.text + base;
         if (f.mode != kOutWakati) dst = put_str(dst, "EOS");
         *dst = '\n';
     }

@@ -62,6 +62,9 @@ enum : uint32_t {
     // the batch has more characters than the per-character kernels were launched for (the engine sizes those
     // launches from a learned characters-per-byte ratio): later kernels stand down, the engine re-runs the batch
     kFlagSlotsOverflow = 16u,
+    // the batch's output text is larger than the text buffer (sized from a learned text-per-byte ratio in the
+    // chunked host pipeline): k_format_write wrote nothing, the engine re-runs the batch with a larger buffer
+    kFlagTextOverflow = 32u,
 };
 constexpr uint32_t kFlagsStandDown = kFlagBadOffsets | kFlagSlotsOverflow;
 constexpr uint32_t kPruneMaxChars = 16000;  // (chars + 1) nodes x 65 535 per node < 2^30
@@ -124,12 +127,14 @@ struct FormatArgs {
     const uint8_t* utf8;
     const unsigned long long* byte_off;  // n_sent + 1
     uint32_t n_sent;
-    const unsigned long long* tok_off;   // n_sent + 1
+    const unsigned long long* tok_off;   // n_sent + 1, indices into `tokens`
     const uint2* tokens;                 // vbt_token as 3 x uint2
-    uint32_t* tok_len;                   // bytes each token contributes (separators included, terminators not)
-    const unsigned long long* tok_text_off;  // exclusive scan of tok_len, n_tokens + 1
-    unsigned long long* text_off;        // n_sent + 1: where each sentence's text starts
+    unsigned long long* sent_len;        // n_sent + 1: bytes of each sentence's text, terminator included
+    unsigned long long* text_off;        // n_sent + 1: exclusive scan of sent_len, where each sentence's text starts
     uint8_t* text;
+    unsigned long long text_cap;         // bytes behind `text`: a larger total sets kFlagTextOverflow instead
+    uint32_t* flags;                     // the batch's flags: the stage stands down after an input error or overflow
+    unsigned long long* text_total;      // receives text_off[n_sent] (also when it does not fit)
     uint32_t mode;
 };
 void launch_format_len(const DictView& d, const FormatArgs& f, cudaStream_t st);

@@ -12,7 +12,8 @@
 //     D2H copies of different devices overlap and use their own PCIe links.
 //   * Host results: once every shard's token count is known the shards' token records are copied straight into
 //     ONE pinned result at their final positions (no host-side merge pass); token offsets are made global on
-//     the device before they leave it.  The result is indistinguishable from a single-device one.
+//     the device before they leave it.  The output stage ("output_mode") formats each shard's text on its device
+//     and places it the same way.  The result is indistinguishable from a single-device one.
 //   * Device-resident batches (vbt_tokenize_batch_device): the input sits on the first device, shards reach the
 //     other devices by peer copies, and the token records come back to the first device with grouped
 //     ncclSend / ncclRecv (the "gather of token spans over NVLink"; peer copies without NCCL).
@@ -217,6 +218,8 @@ class MultiEngine final : public Engine {
         for (auto* r : pool_) {
             pinned_free(r->tok_off);
             pinned_free(r->tokens);
+            pinned_free(r->text_off);
+            pinned_free(r->text);
             delete r;
         }
         pinned_free(h_off_);
@@ -234,16 +237,22 @@ class MultiEngine final : public Engine {
             return r;
         }
         const std::vector<uint64_t> cut = split_by_bytes(byte_off, n_sent, n);
-        std::vector<uint64_t> n_tok(n, 0);
-        run_on_all([&](int i) { n_tok[i] = eng_[i]->run_shard(utf8, byte_off + cut[i], cut[i + 1] - cut[i], -1); });
-        std::vector<uint64_t> base(n + 1, 0);
-        for (int i = 0; i < n; ++i) base[i + 1] = base[i] + n_tok[i];
-        HostResult* r = acquire(n_sent, base[n]);
+        std::vector<uint64_t> n_tok(n, 0), n_text(n, 0);
+        run_on_all([&](int i) {
+            n_tok[i] = eng_[i]->run_shard(utf8, byte_off + cut[i], cut[i + 1] - cut[i], -1, text_ ? &n_text[i] : nullptr);
+        });
+        std::vector<uint64_t> base(n + 1, 0), text_base(n + 1, 0);
+        for (int i = 0; i < n; ++i) {
+            base[i + 1] = base[i] + n_tok[i];
+            text_base[i + 1] = text_base[i] + n_text[i];
+        }
+        HostResult* r = acquire(n_sent, base[n], text_ ? &text_base[n] : nullptr);
         const uint64_t tb = eng_[0]->token_bytes();
         r->token_bytes = uint32_t(tb);
         int last = n - 1;  // the shard that also delivers the closing offset: the last one, even when it is empty
         run_on_all([&](int i) {
-            eng_[i]->fetch_shard(r->tok_off + cut[i], static_cast<uint8_t*>(r->tokens) + base[i] * tb, base[i], i == last);
+            eng_[i]->fetch_shard(r->tok_off + cut[i], static_cast<uint8_t*>(r->tokens) + base[i] * tb, base[i], i == last,
+                                 text_ ? r->text_off + cut[i] : nullptr, r->text + text_base[i], text_base[i]);
         });
         collect_stats();
         return r;
@@ -279,7 +288,7 @@ class MultiEngine final : public Engine {
         std::vector<uint64_t> n_tok(n, 0);
         run_on_all([&](int i) {
             n_tok[i] = eng_[i]->run_shard(reinterpret_cast<const char*>(d_utf8), h_off_ + cut[i], cut[i + 1] - cut[i],
-                                          dev_[0]);
+                                          dev_[0], nullptr);  // token-only, like the single-device entry point
         });
         std::vector<uint64_t> base(n + 1, 0);
         for (int i = 0; i < n; ++i) base[i + 1] = base[i] + n_tok[i];
@@ -337,10 +346,9 @@ class MultiEngine final : public Engine {
         for (auto& e : eng_) e->set_counting(on);
     }
     void set_option(const std::string& name, long long value) override {
-        if (name == "output_mode" && value != 0)
-            throw Error(kUnsupported, "the output stage runs on single-device tokenizers only");
         if (name == "chunk_sentences") return;  // shards are not chunked (see the constructor)
         for (auto& e : eng_) e->set_option(name, value);
+        if (name == "output_mode") text_ = value != 0;
     }
     void set_stream(uint64_t stream) override {
         if (stream) throw Error(kUnsupported, "a multi-device tokenizer runs on its own streams");
@@ -363,8 +371,10 @@ class MultiEngine final : public Engine {
             for (uint32_t i = 0; i < nr; ++i) rid[i] += r[i];
         }
     }
-    uint64_t run_shard(const char*, const uint64_t*, uint64_t, int) override { throw Error(kInternal, "not a shard engine"); }
-    void fetch_shard(uint64_t*, void*, uint64_t, bool) override { throw Error(kInternal, "not a shard engine"); }
+    uint64_t run_shard(const char*, const uint64_t*, uint64_t, int, uint64_t*) override { throw Error(kInternal, "not a shard engine"); }
+    void fetch_shard(uint64_t*, void*, uint64_t, bool, uint64_t*, char*, uint64_t) override {
+        throw Error(kInternal, "not a shard engine");
+    }
     void rebase_shard(uint64_t) override { throw Error(kInternal, "not a shard engine"); }
     void shard_outputs(uint64_t*, uint64_t*) const override { throw Error(kInternal, "not a shard engine"); }
     int device() const override { return dev_[0]; }
@@ -434,7 +444,8 @@ class MultiEngine final : public Engine {
         }
     }
 
-    HostResult* acquire(uint64_t n_sent, uint64_t n_tokens) {
+    // A pooled pinned result for n_sent sentences and n_tokens tokens, and *text_bytes bytes of text when given.
+    HostResult* acquire(uint64_t n_sent, uint64_t n_tokens, const uint64_t* text_bytes) {
         HostResult* r = nullptr;
         if (!free_.empty()) {
             r = free_.back();
@@ -455,8 +466,22 @@ class MultiEngine final : public Engine {
         }
         r->n_sent = n_sent;
         r->n_tokens = n_tokens;
-        r->has_text = false;
+        r->has_text = text_bytes != nullptr;
+        r->text_bytes = text_bytes ? *text_bytes : 0;
+        if (text_bytes) {
+            if ((n_sent + 1) * 8 > r->cap_text_off) {
+                pinned_free(r->text_off);
+                r->cap_text_off = size_t(double((n_sent + 1) * 8) * 1.25) + 64;
+                r->text_off = static_cast<uint64_t*>(pinned_alloc(r->cap_text_off));
+            }
+            if (*text_bytes + 1 > r->cap_text) {
+                pinned_free(r->text);
+                r->cap_text = size_t(double(*text_bytes + 1) * 1.25) + 64;
+                r->text = static_cast<char*>(pinned_alloc(r->cap_text));
+            }
+        }
         if (n_sent == 0) r->tok_off[0] = 0;
+        if (n_sent == 0 && text_bytes) r->text_off[0] = 0;
         return r;
     }
 
@@ -469,6 +494,7 @@ class MultiEngine final : public Engine {
     std::vector<std::unique_ptr<Engine>> eng_;
     std::string transport_;
     std::vector<HostResult*> pool_, free_;
+    bool text_ = false;  // "output_mode" is on: host results carry the formatted text
     uint64_t* h_off_ = nullptr;  // pinned
     size_t h_off_cap_ = 0;
     void* gather_tokens_ = nullptr;
