@@ -107,6 +107,12 @@ int32_t vbt_scorer_accumulate(const int32_t *triples, size_t n_triples, const ui
                               size_t n_keys, int32_t *cost);
 /* Dictionary::write (dictionary.rs:142-150). *out is released with vbt_bytes_free. */
 int32_t vbt_dict_write(const vbt_dict *d, uint8_t **out, size_t *n);
+/* zstd::Encoder::new(File::create(path), level) + Dictionary::write + finish (compile/src/main.rs:98-100): the
+ * `system.dic.zst` every tool reads with -i.  One zstd frame whose header carries the content size; only the
+ * decompressed bytes are specified (they equal vbt_dict_write's), not the compressed ones.  Needs libzstd.so.1 at run
+ * time.  VBT_ERR_IO when the library is missing, the file cannot be created or a write fails; a partly written file
+ * is removed. */
+int32_t vbt_dict_write_zstd_file(const vbt_dict *d, const char *path, int32_t level);
 void vbt_bytes_free(uint8_t *p);
 /* Dictionary::reset_user_lexicon_from_reader (dictionary.rs:209-229); csv == NULL clears it. */
 int32_t vbt_dict_set_user_lexicon_csv(vbt_dict *d, const char *csv, size_t n);

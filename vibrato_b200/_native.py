@@ -66,6 +66,7 @@ def lib():
     sig("vbt_dict_from_bigram", i32, [vp, sz, vp, sz, vp, sz, vp, sz, vp, sz, vp, sz, i32, pp])
     sig("vbt_scorer_accumulate", i32, [vp, sz, vp, vp, sz, C.POINTER(i32)])
     sig("vbt_dict_write", i32, [vp, pp, C.POINTER(sz)])
+    sig("vbt_dict_write_zstd_file", i32, [vp, cp, i32])
     sig("vbt_bytes_free", None, [vp])
     sig("vbt_dict_set_user_lexicon_csv", i32, [vp, vp, sz])
     sig("vbt_dict_free", None, [vp])

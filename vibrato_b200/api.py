@@ -93,6 +93,12 @@ class Dictionary:
         finally:
             lib().vbt_bytes_free(p)
 
+    def write_zstd_file(self, path, level=19):
+        """Dictionary::write into zstd::Encoder::new(File::create(path), level) (compile/src/main.rs:98-100): the
+        `system.dic.zst` that from_zstd_file and every tool's -i read.  A failed write leaves no file behind."""
+        check(lib().vbt_dict_write_zstd_file(self._h, str(path).encode(), int(level)))
+        return self
+
     def reset_user_lexicon_from_reader(self, user_lexicon):
         """Dictionary::reset_user_lexicon_from_reader (dictionary.rs:209-229); None clears it."""
         if user_lexicon is None:

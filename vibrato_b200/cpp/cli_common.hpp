@@ -1,8 +1,10 @@
-// Shared bits of the `tokenize` / `benchmark` look-alike CLIs.
+// Shared bits of the look-alike CLIs (`tokenize`, `benchmark`, `evaluate`, `compile`, `reorder`, `map`).
 #pragma once
 
 #include <sys/stat.h>
 
+#include <charconv>
+#include <cmath>
 #include <cstdio>
 #include <fstream>
 #include <iostream>
@@ -67,5 +69,72 @@ struct Packed {
         off.assign(1, 0);
     }
 };
+
+// Rust's `{}` for f64: shortest digits that round-trip, never an exponent, "NaN" / "inf"
+inline std::string rust_f64(double v) {
+    if (std::isnan(v)) return "NaN";
+    if (std::isinf(v)) return v < 0 ? "-inf" : "inf";
+    char buf[512];
+    auto r = std::to_chars(buf, buf + sizeof(buf), v, std::chars_format::fixed);
+    return std::string(buf, r.ptr);
+}
+
+// A `.lmap` / `.rmap` file of `reorder`: `{id}\t{p}\n` per id (map/src/reorder.rs:50-52)
+inline std::string mapping_text(const vibrato_b200::ConnIdProbs& probs) {
+    std::string text;
+    for (const auto& [id, p] : probs) text.append(std::to_string(id)).append("\t").append(rust_f64(p)).append("\n");
+    return text;
+}
+
+// Rust's `{:?}` for a path: quoted, with `\`, `"` and control characters escaped (char::escape_debug)
+inline std::string rust_debug_path(const std::string& path) {
+    std::string out = "\"";
+    for (unsigned char c : path) {
+        if (c == '\\' || c == '"') out += '\\', out += char(c);
+        else if (c == '\t') out += "\\t";
+        else if (c == '\r') out += "\\r";
+        else if (c == '\n') out += "\\n";
+        else if (c == 0) out += "\\0";
+        else if (c < 0x20 || c == 0x7F) {
+            char b[16];
+            std::snprintf(b, sizeof(b), "\\u{%x}", c);
+            out += b;
+        } else out += char(c);
+    }
+    return out + "\"";
+}
+
+// PathBuf::set_extension: the extension of the last component is replaced, or added when it has none (".hidden" has
+// none).  A path without a last file name ("", "/", ".", "..", "a/..") stays as it is.  Like Rust, everything after
+// the file stem goes, trailing "/" and "/." included.
+inline std::string set_extension(const std::string& path, const std::string& ext) {
+    size_t end = path.size();
+    for (;;) {  // Path::components() drops trailing separators and "." components
+        while (end > 1 && path[end - 1] == '/') --end;
+        if (end > 1 && path[end - 1] == '.' && path[end - 2] == '/') end -= 2;
+        else break;
+    }
+    size_t start = path.rfind('/', end ? end - 1 : 0);
+    start = (start == std::string::npos || end == 0) ? 0 : start + 1;
+    if (end > 0 && start == end) return path;  // the root
+    const std::string name = path.substr(start, end - start);
+    if (name.empty() || name == "." || name == "..") return path;
+    const size_t dot = name.rfind('.');
+    const size_t stem = (dot == std::string::npos || dot == 0) ? name.size() : dot;
+    return path.substr(0, start + stem) + "." + ext;
+}
+
+// u16::from_str: an optional '+', then ASCII digits only, at most 65535 (no sign, space or empty string)
+inline uint16_t parse_u16(std::string_view s) {
+    if (s.empty()) throw std::runtime_error("cannot parse integer from empty string");
+    if (s[0] == '+' && s.size() > 1) s.remove_prefix(1);
+    uint32_t v = 0;
+    for (char c : s) {
+        if (c < '0' || c > '9') throw std::runtime_error("invalid digit found in string");
+        v = v * 10 + uint32_t(c - '0');
+        if (v > 0xFFFF) throw std::runtime_error("number too large to fit in target type");
+    }
+    return uint16_t(v);
+}
 
 }  // namespace cli

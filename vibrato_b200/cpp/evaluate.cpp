@@ -1,26 +1,16 @@
 // `evaluate` look-alike: same flags and output as the reference tool (/root/reference/evaluate/src/main.rs:13-38
 // flags, :61-138 loop, :132-136 output), with the whole test corpus tokenised as one batch on the GPU.
-#include <charconv>
-#include <cmath>
 #include <cstring>
 
 #include "cli_common.hpp"
 
 using namespace vibrato_b200;
+using cli::rust_f64;
 
 static void usage() {
     std::fprintf(stderr,
                  "evaluate -t <test corpus> -i <system.dic.zst | mecab-source-dir> [-u user.csv] [-M n]\n"
                  "         [--feature-indices i,j,...]\n");
-}
-
-// Rust's `{}` for f64: shortest digits that round-trip, never an exponent, "NaN" / "inf"
-static std::string rust_f64(double v) {
-    if (std::isnan(v)) return "NaN";
-    if (std::isinf(v)) return v < 0 ? "-inf" : "inf";
-    char buf[512];
-    auto r = std::to_chars(buf, buf + sizeof(buf), v, std::chars_format::fixed);
-    return std::string(buf, r.ptr);
 }
 
 int main(int argc, char** argv) {

@@ -1,6 +1,8 @@
 // Header-only C++17 mirror of vibrato's public API over the C ABI (include/vibrato_b200.h).
 //
-//   vibrato::Dictionary::read / reset_user_lexicon_from_reader   dictionary.rs:173,209
+//   vibrato::Dictionary::read / reset_user_lexicon_from_reader / map_connection_ids_from_iter   dictionary.rs:173,209,245
+//   SystemDictionaryBuilder::from_readers / from_readers_with_bigram_info   dictionary/builder.rs:64,111
+//   ConnIdCounter::compute_probs   dictionary/mapper.rs:108-146
 //   vibrato::Tokenizer::new / ignore_space / max_grouping_len / new_worker   tokenizer.rs:26-84
 //   vibrato::tokenizer::worker::Worker::reset_sentence / tokenize / num_tokens / token   worker.rs:34-74
 //   vibrato::token::Token accessors   token.rs:21-92
@@ -8,6 +10,7 @@
 // (paths relative to /root/reference/vibrato/src/)
 #pragma once
 
+#include <algorithm>
 #include <cstdint>
 #include <memory>
 #include <stdexcept>
@@ -59,8 +62,27 @@ class Dictionary {
                                   unk.data(), unk.size(), &h));
         return Dictionary(h);
     }
+    static Dictionary from_readers_with_bigram_info(std::string_view lex, std::string_view bigram_right,
+                                                    std::string_view bigram_left, std::string_view bigram_cost,
+                                                    std::string_view chr, std::string_view unk,
+                                                    bool dual_connector) {  // builder.rs:111-148
+        vbt_dict* h = nullptr;
+        check(vbt_dict_from_bigram(lex.data(), lex.size(), bigram_right.data(), bigram_right.size(), bigram_left.data(),
+                                   bigram_left.size(), bigram_cost.data(), bigram_cost.size(), chr.data(), chr.size(),
+                                   unk.data(), unk.size(), dual_connector ? 1 : 0, &h));
+        return Dictionary(h);
+    }
+    // Dictionary::write into zstd::Encoder::new(File::create(path), level) (compile/src/main.rs:98-100)
+    void write_zstd_file(const std::string& path, int32_t level = 19) const {
+        check(vbt_dict_write_zstd_file(h_.get(), path.c_str(), level));
+    }
     Dictionary reset_user_lexicon_from_reader(const std::string* csv) && {  // dictionary.rs:209; consumes self
         check(vbt_dict_set_user_lexicon_csv(h_.get(), csv ? csv->data() : nullptr, csv ? csv->size() : 0));
+        return std::move(*this);
+    }
+    Dictionary map_connection_ids_from_iter(const std::vector<uint16_t>& lmap,
+                                            const std::vector<uint16_t>& rmap) && {  // dictionary.rs:245-259
+        check(vbt_dict_map_connection_ids(h_.get(), lmap.data(), lmap.size(), rmap.data(), rmap.size()));
         return std::move(*this);
     }
     std::string_view word_feature(WordIdx w) const {  // dictionary.rs:108
@@ -109,6 +131,24 @@ class BatchResult {
     uint64_t n_sent_ = 0, n_tokens_ = 0;
 };
 
+// ConnIdProbs (mapper.rs:84): (id, occurrence probability) pairs
+using ConnIdProbs = std::vector<std::pair<uint32_t, double>>;
+
+// ConnIdCounter::compute_probs (mapper.rs:108-146) for one side: each count over the sum, id 0 dropped, by descending
+// probability then ascending id.  With a zero sum every probability is NaN, no two compare, and the order is by id.
+inline ConnIdProbs compute_connid_probs(const std::vector<uint64_t>& counts) {
+    uint64_t sum = 0;
+    for (uint64_t c : counts) sum += c;
+    ConnIdProbs probs;
+    for (uint32_t i = 1; i < counts.size(); ++i) probs.emplace_back(i, double(counts[i]) / double(sum));
+    std::sort(probs.begin(), probs.end(), [](const auto& a, const auto& b) {
+        if (a.second > b.second) return true;
+        if (a.second < b.second) return false;
+        return a.first < b.first;  // equal, or incomparable (NaN)
+    });
+    return probs;
+}
+
 class Worker;
 
 class Tokenizer {
@@ -147,6 +187,16 @@ class Tokenizer {
         const int64_t m = mode.empty() ? 0 : mode == "mecab" ? 1 : mode == "wakati" ? 2 : mode == "detail" ? 3 : -1;
         if (m < 0) throw VibratoError(VBT_ERR_INVALID_ARGUMENT, "Could not parse a mode");
         check(vbt_tokenizer_set_option(handle(), "output_mode", m));
+    }
+    // Worker::init_connid_counter / update_connid_counts / compute_connid_probs (worker.rs:77-103): after
+    // init_connid_counter() every batch is counted, an empty sentence counting nothing
+    void init_connid_counter() const { check(vbt_tokenizer_set_option(handle(), "connid_counting", 1)); }
+    std::pair<ConnIdProbs, ConnIdProbs> compute_connid_probs() const {
+        uint32_t nl = 0, nr = 0;
+        check(vbt_connid_counts(handle(), nullptr, nullptr, &nl, &nr));
+        std::vector<uint64_t> lid(nl), rid(nr);
+        check(vbt_connid_counts(handle(), lid.data(), rid.data(), nullptr, nullptr));
+        return {vibrato_b200::compute_connid_probs(lid), vibrato_b200::compute_connid_probs(rid)};
     }
 
     BatchResult tokenize_batch(const char* utf8, const uint64_t* byte_offsets, uint64_t n_sent) const {

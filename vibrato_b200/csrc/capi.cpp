@@ -146,6 +146,16 @@ int32_t vbt_dict_write(const vbt_dict* d, uint8_t** out, size_t* n) {
     });
 }
 
+int32_t vbt_dict_write_zstd_file(const vbt_dict* d, const char* path, int32_t level) {
+    return guarded([&] {
+        need(d, "d");
+        need(path, "path");
+        std::vector<uint8_t> buf;
+        d->d.write(buf);
+        vbt::zstd_compress_to_file(buf, path, level);
+    });
+}
+
 void vbt_bytes_free(uint8_t* p) { std::free(p); }
 
 int32_t vbt_dict_set_user_lexicon_csv(vbt_dict* d, const char* csv, size_t n) {

@@ -5,11 +5,13 @@
 #include <dlfcn.h>
 
 #include <algorithm>
+#include <cerrno>
 #include <cstdio>
 #include <cstring>
 #include <limits>
 #include <map>
 #include <numeric>
+#include <thread>
 #include <unordered_map>
 #include <unordered_set>
 #include <type_traits>
@@ -1576,6 +1578,70 @@ std::vector<uint8_t> zstd_decompress_file(const char* path) {
     }
     destroy(ds);
     return out;
+}
+
+void zstd_compress_to_file(const std::vector<uint8_t>& data, const char* path, int level) {
+    void* h = dlopen("libzstd.so.1", RTLD_NOW | RTLD_LOCAL);
+    if (!h) throw Error(kIo, "libzstd.so.1 is not available: write the stream of vbt_dict_write and compress it yourself");
+    struct Buf {
+        const void* p;
+        size_t size, pos;
+    };
+    struct OBuf {
+        void* p;
+        size_t size, pos;
+    };
+    enum { kLevel = 100, kWorkers = 400, kEnd = 2 };  // ZSTD_c_compressionLevel, ZSTD_c_nbWorkers, ZSTD_e_end
+    using CreateFn = void* (*)();
+    using FreeFn = size_t (*)(void*);
+    using SetParamFn = size_t (*)(void*, int, int);
+    using PledgeFn = size_t (*)(void*, unsigned long long);
+    using StepFn = size_t (*)(void*, OBuf*, Buf*, int);
+    using IsErrFn = unsigned (*)(size_t);
+    using ErrNameFn = const char* (*)(size_t);
+    auto create = reinterpret_cast<CreateFn>(dlsym(h, "ZSTD_createCCtx"));
+    auto destroy = reinterpret_cast<FreeFn>(dlsym(h, "ZSTD_freeCCtx"));
+    auto set_param = reinterpret_cast<SetParamFn>(dlsym(h, "ZSTD_CCtx_setParameter"));
+    auto pledge = reinterpret_cast<PledgeFn>(dlsym(h, "ZSTD_CCtx_setPledgedSrcSize"));
+    auto step = reinterpret_cast<StepFn>(dlsym(h, "ZSTD_compressStream2"));
+    auto is_err = reinterpret_cast<IsErrFn>(dlsym(h, "ZSTD_isError"));
+    auto err_name = reinterpret_cast<ErrNameFn>(dlsym(h, "ZSTD_getErrorName"));
+    if (!create || !destroy || !set_param || !pledge || !step || !is_err || !err_name)
+        throw Error(kIo, "libzstd.so.1 lacks the streaming compression API");
+    FILE* f = std::fopen(path, "wb");
+    if (!f) throw Error(kIo, std::string("cannot create ") + path + ": " + std::strerror(errno));
+    void* cs = create();
+    // On any failure the partly written file is removed, so a failed write never leaves a truncated dictionary.
+    auto fail = [&](const std::string& msg) {
+        if (cs) destroy(cs);
+        std::fclose(f);
+        std::remove(path);
+        throw Error(kIo, msg);
+    };
+    if (!cs) fail("zstd: cannot create a compression context");
+    size_t rc = set_param(cs, kLevel, level);
+    if (is_err(rc)) fail(std::string("zstd: compression level ") + std::to_string(level) + ": " + err_name(rc));
+    // Worker threads only change how fast the frame is made, not what it decodes to; a libzstd built without them
+    // refuses the parameter and compresses on this thread.  Each worker holds its own match tables (tens of MB at
+    // the high levels), hence the cap.
+    set_param(cs, kWorkers, int(std::min(std::thread::hardware_concurrency(), 16u)));
+    rc = pledge(cs, data.size());  // the frame header then carries the content size
+    if (is_err(rc)) fail(std::string("zstd: ") + err_name(rc));
+    std::vector<uint8_t> chunk(1 << 20);
+    Buf ib{data.data(), data.size(), 0};
+    do {
+        OBuf ob{chunk.data(), chunk.size(), 0};
+        rc = step(cs, &ob, &ib, kEnd);
+        if (is_err(rc)) fail(std::string("zstd: ") + err_name(rc));
+        if (std::fwrite(chunk.data(), 1, ob.pos, f) != ob.pos) fail(std::string("cannot write ") + path + ": " + std::strerror(errno));
+    } while (rc != 0);
+    destroy(cs);
+    cs = nullptr;
+    if (std::fclose(f) != 0) {
+        const std::string msg = std::string("cannot write ") + path + ": " + std::strerror(errno);
+        std::remove(path);
+        throw Error(kIo, msg);
+    }
 }
 
 }  // namespace vbt

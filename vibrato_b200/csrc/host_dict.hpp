@@ -217,5 +217,8 @@ std::u32string utf8_to_u32(std::string_view s);
 
 // zstd frame decoding through the runtime libzstd.so.1 (no headers in this image).
 std::vector<uint8_t> zstd_decompress_file(const char* path);
+// zstd::Encoder::new(File::create(path), level) + write_all + finish (compile/src/main.rs:98-100): one frame that
+// carries its content size.  Fails with kIo and removes the partly written file.
+void zstd_compress_to_file(const std::vector<uint8_t>& data, const char* path, int level);
 
 }  // namespace vbt
