@@ -6,7 +6,7 @@
  * item it stands behind (paths relative to /root/reference/vibrato/src/); INTEGRATION.md shows the
  * Rust shim (`extern "C"` block + Dictionary/Tokenizer/Worker/Token wrappers) that binds them.
  *
- * Conventions: every function returns an int32 status (VBT_OK = 0; 1..9 mirror the VibratoError
+ * Conventions: every function returns an int32 status (VBT_OK = 0; 1..8 and 10 mirror the VibratoError
  * variants of errors.rs:11-42); out-parameters come last; handles are opaque and released with the
  * matching *_free; vbt_last_error() returns the calling thread's last message (UTF-8, NUL-ended).
  * No torch / CUDA types appear in any signature: device memory is passed as plain addresses.
@@ -40,6 +40,7 @@ enum {
     VBT_ERR_IO = 7,               /* VibratoError::StdIo           */
     VBT_ERR_UTF8 = 8,             /* VibratoError::Utf8            */
     VBT_ERR_UNSUPPORTED = 9,      /* reserved: a recognised input this build cannot run */
+    VBT_ERR_PARSE_FLOAT = 10,     /* VibratoError::ParseFloat      */
     VBT_ERR_CUDA = 100,
     VBT_ERR_NO_DEVICE = 101,
     VBT_ERR_INTERNAL = 102
@@ -105,6 +106,17 @@ int32_t vbt_dict_from_bigram(const char *lex_csv, size_t lex_len, const char *bi
  * (raw_connector/scorer.rs:110-168, 255-267); triples = n x (key1, key2, cost). */
 int32_t vbt_scorer_accumulate(const int32_t *triples, size_t n_triples, const uint32_t *keys1, const uint32_t *keys2,
                               size_t n_keys, int32_t *cost);
+/* mecab::generate_bigram_info (mecab.rs:31-181): converts a trained MeCab model (feature.def, right-id.def,
+ * left-id.def, model.def; note the reference's argument order) into the bigram.right / bigram.left / bigram.cost
+ * files that vbt_dict_from_bigram reads.  right-id.def supplies bigram.right and left-id.def bigram.left.  A model.def
+ * weight w becomes the cost -(w * cost_factor) truncated toward zero and saturated to i32 (NaN gives 0); zero costs
+ * are dropped.  A weight f64::from_str rejects fails with VBT_ERR_PARSE_FLOAT.  The three buffers are released with
+ * vbt_bytes_free; on error nothing is allocated. */
+int32_t vbt_mecab_generate_bigram_info(const char *feature_def, size_t feature_len, const char *right_id_def,
+                                       size_t right_id_len, const char *left_id_def, size_t left_id_len,
+                                       const char *model_def, size_t model_len, double cost_factor,
+                                       uint8_t **bigram_right, size_t *right_n, uint8_t **bigram_left,
+                                       size_t *left_n, uint8_t **bigram_cost, size_t *cost_n);
 /* Dictionary::write (dictionary.rs:142-150). *out is released with vbt_bytes_free. */
 int32_t vbt_dict_write(const vbt_dict *d, uint8_t **out, size_t *n);
 /* zstd::Encoder::new(File::create(path), level) + Dictionary::write + finish (compile/src/main.rs:98-100): the

@@ -40,6 +40,12 @@ extern "C" {
                             left: *const c_char, left_len: usize, cost: *const c_char, cost_len: usize,
                             chr: *const c_char, chr_len: usize, unk: *const c_char, unk_len: usize,
                             dual_connector: i32, out: *mut *mut vbt_dict) -> i32;
+    fn vbt_mecab_generate_bigram_info(feature_def: *const c_char, feature_len: usize, right_id_def: *const c_char,
+                                      right_id_len: usize, left_id_def: *const c_char, left_id_len: usize,
+                                      model_def: *const c_char, model_len: usize, cost_factor: f64,
+                                      bigram_right: *mut *mut u8, right_n: *mut usize, bigram_left: *mut *mut u8,
+                                      left_n: *mut usize, bigram_cost: *mut *mut u8, cost_n: *mut usize) -> i32;
+    fn vbt_bytes_free(p: *mut u8);
     fn vbt_dict_map_connection_ids(d: *mut vbt_dict, lmap: *const u16, n_lmap: usize, rmap: *const u16,
                                    n_rmap: usize) -> i32;
     fn vbt_tokenizer_set_option(t: *mut vbt_tokenizer, name: *const c_char, value: i64) -> i32;
@@ -134,6 +140,39 @@ impl SystemDictionaryBuilder {
                                             k.as_ptr() as _, k.len(), c.as_ptr() as _, c.len(), d.as_ptr() as _, d.len(),
                                             dual_connector as i32, &mut h) })?;
         Ok(Dictionary { h })
+    }
+}
+
+/// mecab.rs: utilities for MeCab models.
+pub mod mecab {
+    use super::*;
+    use std::io::Write;
+
+    /// mecab.rs:31-181: writes the bigram.right / bigram.left / bigram.cost files of a compact dictionary made from a
+    /// trained MeCab model.  Same argument order as the reference: right-id.def feeds `bigram_right_wtr`.
+    #[allow(clippy::too_many_arguments)]
+    pub fn generate_bigram_info(feature_def_rdr: impl Read, right_id_def_rdr: impl Read, left_id_def_rdr: impl Read,
+                                model_def_rdr: impl Read, cost_factor: f64, mut bigram_right_wtr: impl Write,
+                                mut bigram_left_wtr: impl Write, mut bigram_cost_wtr: impl Write) -> Result<()> {
+        let (f, r, l, m) = (slurp(feature_def_rdr)?, slurp(right_id_def_rdr)?, slurp(left_id_def_rdr)?,
+                            slurp(model_def_rdr)?);
+        let mut p = [std::ptr::null_mut(); 3];
+        let mut n = [0usize; 3];
+        let [p0, p1, p2] = &mut p;
+        let [n0, n1, n2] = &mut n;
+        check(unsafe { vbt_mecab_generate_bigram_info(f.as_ptr() as _, f.len(), r.as_ptr() as _, r.len(),
+                                                      l.as_ptr() as _, l.len(), m.as_ptr() as _, m.len(), cost_factor,
+                                                      p0, n0, p1, n1, p2, n2) })?;
+        let mut res = Ok(());
+        let writers: [&mut dyn Write; 3] = [&mut bigram_right_wtr, &mut bigram_left_wtr, &mut bigram_cost_wtr];
+        for (i, w) in writers.into_iter().enumerate() {
+            let bytes = unsafe { std::slice::from_raw_parts(p[i], n[i]) };
+            if res.is_ok() {
+                res = w.write_all(bytes).map_err(|e| VibratoError { code: 7, msg: e.to_string() });
+            }
+            unsafe { vbt_bytes_free(p[i]) };
+        }
+        res
     }
 }
 

@@ -5,6 +5,7 @@ libvibrato_b200.so), `api` (host-side mirror of the reference's Rust API over th
 `synth` (seeded synthetic dictionaries / corpora for tests and benchmarks).
 """
 from .api import (BatchResult, Dictionary, SystemDictionaryBuilder, Token, Tokenizer, VibratoError, WordIdx,  # noqa: F401
-                  Worker, TOKEN_DTYPE, COMPACT_TOKEN_DTYPE, LEX_TYPE_NAMES, expand_compact_tokens)
+                  Worker, TOKEN_DTYPE, COMPACT_TOKEN_DTYPE, LEX_TYPE_NAMES, expand_compact_tokens,
+                  generate_bigram_info)
 
 __version__ = "0.1.0"

@@ -14,7 +14,7 @@ HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "vibrato_b200.h")
 VBT_OK = 0
 ERR_NAMES = {
     1: "InvalidArgument", 2: "InvalidFormat", 3: "TryFromInt", 4: "ParseInt", 5: "BincodeDecode", 6: "BincodeEncode",
-    7: "StdIo", 8: "Utf8", 9: "Unsupported", 100: "Cuda", 101: "NoDevice", 102: "Internal",
+    7: "StdIo", 8: "Utf8", 9: "Unsupported", 10: "ParseFloat", 100: "Cuda", 101: "NoDevice", 102: "Internal",
 }
 
 
@@ -65,6 +65,7 @@ def lib():
     sig("vbt_dict_from_parts", i32, [vp, sz, vp, u32, u32, vp, sz, vp, sz, pp])
     sig("vbt_dict_from_bigram", i32, [vp, sz, vp, sz, vp, sz, vp, sz, vp, sz, vp, sz, i32, pp])
     sig("vbt_scorer_accumulate", i32, [vp, sz, vp, vp, sz, C.POINTER(i32)])
+    sig("vbt_mecab_generate_bigram_info", i32, [vp, sz, vp, sz, vp, sz, vp, sz, C.c_double] + [pp, C.POINTER(sz)] * 3)
     sig("vbt_dict_write", i32, [vp, pp, C.POINTER(sz)])
     sig("vbt_dict_write_zstd_file", i32, [vp, cp, i32])
     sig("vbt_bytes_free", None, [vp])

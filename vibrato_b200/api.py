@@ -9,6 +9,7 @@ here (paths relative to /root/reference/vibrato/src/):
     Worker.reset_sentence / tokenize / num_tokens / token / token_iter worker.rs:34-74
     Token.surface / feature / range_char / range_byte / word_idx / lex_type /
           left_id / right_id / word_cost / total_cost                  token.rs:21-92
+    generate_bigram_info                                               mecab.rs:31-181
 
 plus the batched entry point the GPU wants: Tokenizer.tokenize_batch(list_of_str) -> BatchResult.
 All tokenisation runs in the CUDA library; nothing here computes a lattice.
@@ -212,6 +213,27 @@ class SystemDictionaryBuilder:
         h = C.c_void_p()
         check(lib().vbt_dict_from_bigram(*args, int(dual_connector), C.byref(h)))
         return Dictionary(h)
+
+
+def generate_bigram_info(feature_def, right_id_def, left_id_def, model_def, cost_factor):
+    """mecab::generate_bigram_info (mecab.rs:31-181): a trained MeCab model (feature.def, right-id.def, left-id.def,
+    model.def, in the reference's order) -> (bigram_right, bigram_left, bigram_cost) as bytes, the sources of
+    SystemDictionaryBuilder.from_readers_with_bigram_info.  right-id.def gives bigram.right, left-id.def bigram.left."""
+    bufs = [_buf(x) for x in (feature_def, right_id_def, left_id_def, model_def)]
+    args = []
+    for _, p, n in bufs:
+        args += [p, n]
+    ptrs = [C.c_void_p() for _ in range(3)]
+    lens = [C.c_size_t() for _ in range(3)]
+    out = []
+    for p, n in zip(ptrs, lens):
+        out += [C.byref(p), C.byref(n)]
+    check(lib().vbt_mecab_generate_bigram_info(*args, float(cost_factor), *out))
+    try:
+        return tuple(C.string_at(p, n.value) for p, n in zip(ptrs, lens))
+    finally:
+        for p in ptrs:
+            lib().vbt_bytes_free(p)
 
 
 def scorer_accumulate(triples, keys1, keys2):

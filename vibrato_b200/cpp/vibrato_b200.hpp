@@ -3,6 +3,7 @@
 //   vibrato::Dictionary::read / reset_user_lexicon_from_reader / map_connection_ids_from_iter   dictionary.rs:173,209,245
 //   SystemDictionaryBuilder::from_readers / from_readers_with_bigram_info   dictionary/builder.rs:64,111
 //   ConnIdCounter::compute_probs   dictionary/mapper.rs:108-146
+//   mecab::generate_bigram_info   mecab.rs:31-181
 //   vibrato::Tokenizer::new / ignore_space / max_grouping_len / new_worker   tokenizer.rs:26-84
 //   vibrato::tokenizer::worker::Worker::reset_sentence / tokenize / num_tokens / token   worker.rs:34-74
 //   vibrato::token::Token accessors   token.rs:21-92
@@ -105,6 +106,31 @@ class Dictionary {
     explicit Dictionary(vbt_dict* h) : h_(h, &vbt_dict_free) {}
     std::unique_ptr<vbt_dict, void (*)(vbt_dict*)> h_;
 };
+
+namespace mecab {
+
+// The three files mecab::generate_bigram_info writes (bigram.right, bigram.left, bigram.cost), the sources of
+// Dictionary::from_readers_with_bigram_info
+struct BigramInfo {
+    std::string right, left, cost;
+};
+
+// mecab::generate_bigram_info (mecab.rs:31-181): a trained MeCab model -> bigram.* files.  The reference's argument
+// order: right-id.def supplies bigram.right, left-id.def bigram.left.
+inline BigramInfo generate_bigram_info(std::string_view feature_def, std::string_view right_id_def,
+                                       std::string_view left_id_def, std::string_view model_def, double cost_factor) {
+    uint8_t* p[3] = {};
+    size_t n[3] = {};
+    check(vbt_mecab_generate_bigram_info(feature_def.data(), feature_def.size(), right_id_def.data(), right_id_def.size(),
+                                         left_id_def.data(), left_id_def.size(), model_def.data(), model_def.size(),
+                                         cost_factor, &p[0], &n[0], &p[1], &n[1], &p[2], &n[2]));
+    using Bytes = std::unique_ptr<uint8_t, void (*)(uint8_t*)>;
+    Bytes own[3] = {{p[0], &vbt_bytes_free}, {p[1], &vbt_bytes_free}, {p[2], &vbt_bytes_free}};
+    auto text = [&](int i) { return std::string(reinterpret_cast<const char*>(own[i].get()), n[i]); };
+    return {text(0), text(1), text(2)};
+}
+
+}  // namespace mecab
 
 class BatchResult {
    public:

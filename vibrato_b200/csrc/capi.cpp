@@ -131,6 +131,36 @@ int32_t vbt_scorer_accumulate(const int32_t* triples, size_t n_triples, const ui
     });
 }
 
+int32_t vbt_mecab_generate_bigram_info(const char* feature_def, size_t feature_len, const char* right_id_def,
+                                       size_t right_id_len, const char* left_id_def, size_t left_id_len,
+                                       const char* model_def, size_t model_len, double cost_factor,
+                                       uint8_t** bigram_right, size_t* right_n, uint8_t** bigram_left,
+                                       size_t* left_n, uint8_t** bigram_cost, size_t* cost_n) {
+    return guarded([&] {
+        need(bigram_right, "bigram_right");
+        need(right_n, "right_n");
+        need(bigram_left, "bigram_left");
+        need(left_n, "left_n");
+        need(bigram_cost, "bigram_cost");
+        need(cost_n, "cost_n");
+        vbt::BigramInfoText t = vbt::generate_bigram_info({feature_def, feature_len}, {right_id_def, right_id_len},
+                                                          {left_id_def, left_id_len}, {model_def, model_len}, cost_factor);
+        const std::string* src[3] = {&t.right, &t.left, &t.cost};
+        uint8_t* p[3] = {};
+        for (int i = 0; i < 3; ++i) {
+            p[i] = static_cast<uint8_t*>(std::malloc(src[i]->size() ? src[i]->size() : 1));
+            if (!p[i]) {
+                for (int k = 0; k < i; ++k) std::free(p[k]);
+                throw std::bad_alloc();
+            }
+            std::memcpy(p[i], src[i]->data(), src[i]->size());
+        }
+        *bigram_right = p[0], *right_n = t.right.size();
+        *bigram_left = p[1], *left_n = t.left.size();
+        *bigram_cost = p[2], *cost_n = t.cost.size();
+    });
+}
+
 int32_t vbt_dict_write(const vbt_dict* d, uint8_t** out, size_t* n) {
     return guarded([&] {
         need(d, "d");

@@ -16,7 +16,7 @@
 
 namespace vbt {
 
-// Status codes crossing the C ABI (include/vibrato_b200.h). 1..9 mirror VibratoError's variants
+// Status codes crossing the C ABI (include/vibrato_b200.h). 1..8 and 10 mirror VibratoError's variants
 // (errors.rs:11-42).
 enum Status : int32_t {
     kOk = 0,
@@ -29,6 +29,7 @@ enum Status : int32_t {
     kIo = 7,      // StdIo
     kUtf8 = 8,
     kUnsupported = 9,  // a recognised input this build cannot run (unused since the Dual connector landed)
+    kParseFloat = 10,
     kCuda = 100,
     kNoDevice = 101,
     kInternal = 102,
@@ -205,6 +206,14 @@ struct Dictionary {  // dictionary.rs:43-51
    private:
     void finish_build(std::string_view lex_csv, std::string_view char_def, std::string_view unk_def);
 };
+
+// mecab::generate_bigram_info (mecab.rs:31-181), in mecab_model.cpp: the three bigram.* files of a MeCab model
+// (feature.def, right-id.def, left-id.def, model.def), in the reference's argument order.
+struct BigramInfoText {
+    std::string right, left, cost;
+};
+BigramInfoText generate_bigram_info(std::string_view feature_def, std::string_view right_id_def,
+                                    std::string_view left_id_def, std::string_view model_def, double cost_factor);
 
 // utils::parse_csv_row (utils.rs:41-61): the fields of one CSV row
 std::vector<std::string> parse_csv_row(std::string_view row);

@@ -404,3 +404,133 @@ def make_bigram_files(d, n_templates=6, vocab=24, pairs_per_template=260, seed=2
             lines.append(f"R{t}:a,b/L{t}:v1\t555")
     lines.append("R0:v0/L0:v0\t42")  # a repeated pair: the later cost replaces the earlier one
     return right, left, "\n".join(lines) + "\n"
+
+
+def make_mecab_model(num_left, num_right, n_templates=16, n_model_lines=20000, seed=20261015):
+    """The files of a trained MeCab model shaped like unidic's (docs/small-dic.md of the reference): `feature.def`,
+    `left-id.def` (ids 0..num_left-1), `right-id.def` (ids 0..num_right-1) and `model.def`, as a dict of str, for
+    mecab::generate_bigram_info.  Every id gets a CSV feature row: one of 150 POS / conjugation tuples (six fields),
+    then three lexical fields, often "*", sometimes a quoted field holding a comma, and some rows stop early.  The
+    BIGRAM templates combine one to three fields, with `?` on the lexical ones; at most eight templates touch the
+    lexical fields, so a Dual connector's matrix part stays POS-sized, as it does for unidic.  model.def has MeCab's
+    header, UNIGRAM lines (skipped by the conversion), BOS/EOS sides, feature strings the ids never produce, and
+    weights that truncate to a zero cost."""
+    rng = np.random.default_rng(seed)
+    pos1 = ["名詞", "動詞", "助詞", "形容詞", "副詞", "助動詞", "接尾辞", "補助記号", "代名詞", "連体詞", "接頭辞", "感動詞"]
+    pos = []
+    for k in range(150):
+        p = [pos1[min(int(rng.geometric(0.3)) - 1, len(pos1) - 1)], f"細{int(rng.integers(0, 10))}",
+             "*" if rng.random() < 0.5 else f"類{int(rng.integers(0, 8))}", "*" if rng.random() < 0.8 else "一般"]
+        conj = rng.random() < 0.4
+        p += [f"活用型{int(rng.integers(0, 24))}" if conj else "*", f"活用形{int(rng.integers(0, 12))}" if conj else "*"]
+        pos.append(p)
+
+    def rows(side, n_ids):
+        out = ["0 BOS/EOS,*,*,*,*,*,*,*,*,*"]
+        tup = _zipf_choice(rng, len(pos), n_ids, 1.1)
+        lex = rng.integers(0, 4000, (n_ids, 3))
+        star = rng.random((n_ids, 3)) < [0.3, 0.5, 0.7]
+        quoted = rng.random(n_ids) < 0.03
+        short = rng.random(n_ids) < 0.05
+        for i in range(1, n_ids):
+            f = list(pos[int(tup[i])]) + ["*" if star[i, j] else f"{side}語{int(lex[i, j])}" for j in range(3)]
+            if quoted[i]:
+                f[6] = f'"{f[6]},{int(lex[i, 0]) % 7}"'
+            if short[i]:
+                f = f[:7]
+            out.append(f"{i} " + ",".join(f))
+        return "\n".join(out) + "\n"
+
+    templates = []  # (left template, right template)
+    n_lex = min(8, max(1, n_templates // 3))
+    for k in range(n_templates):
+        if k < n_lex:
+            idx = [int(rng.integers(0, 6)), 6 + k % 3]
+        else:
+            idx = sorted(set(rng.integers(0, 6, int(rng.integers(1, 4))).tolist()))
+        if k == n_templates - 1:
+            idx = idx + [10]  # past the end of every row: always "*"
+        opt = [i >= 6 and i != 10 for i in idx]
+        lt = f"B{k:02}:" + ",".join(f"%L{'?' if o else ''}[{i}]" for i, o in zip(idx, opt))
+        rt = ",".join(f"%R{'?' if o else ''}[{i}]" for i, o in zip(idx, opt))
+        templates.append((lt, rt))
+    feature_def = "# synthetic feature.def\nUNIGRAM U00:%F[0]\nUNIGRAM U01:%F[0],%F?[1]\n\n" + "".join(
+        f"BIGRAM {lt}/{rt}\n" for lt, rt in templates)
+    left_id_def, right_id_def = rows("L", num_left), rows("R", num_right)
+
+    def expansions(id_def, k, side):
+        """The feature strings template k makes on one side (its map keys), for the model's weights to name."""
+        tmpl = templates[k][side]
+        out = set()
+        for line in id_def.splitlines()[1:]:
+            f = _split_csv(line.split(" ", 1)[1])
+            s, ok, pos_ = [], True, 0
+            while True:
+                a = tmpl.find("%", pos_)
+                if a < 0:
+                    s.append(tmpl[pos_:])
+                    break
+                b = tmpl.index("]", a)
+                i = int(tmpl[tmpl.index("[", a) + 1:b])
+                v = f[i] if i < len(f) else "*"
+                if tmpl[a + 2] == "?" and v == "*":
+                    ok = False
+                    break
+                s.append(tmpl[pos_:a] + v)
+                pos_ = b + 1
+            if ok:
+                out.add("".join(s))
+        return sorted(out)
+
+    # right-id.def names the left features (the left context's right ids), left-id.def the right ones
+    lefts = [expansions(right_id_def, k, 0) for k in range(n_templates)]
+    rights = [expansions(left_id_def, k, 1) for k in range(n_templates)]
+    kind = rng.random(n_model_lines)
+    tk = rng.integers(0, n_templates, n_model_lines)
+    pick = rng.integers(0, 1 << 30, (n_model_lines, 2))
+    w = rng.normal(0.0, 1.5, n_model_lines)
+    w[rng.random(n_model_lines) < 0.02] = 1e-5  # |w| * 700 < 1: a zero cost
+    lines = ["version: 102", "charset: UTF-8", "cost-factor: 700", "eval-size: 10", "unk-eval-size: 4", "bias: 0", ""]
+    for n in range(n_model_lines):
+        k, r = int(tk[n]), kind[n]
+        ls, rs = lefts[k], rights[k]
+        lf = ls[int(pick[n, 0]) % len(ls)] if ls else f"B{k:02}:"
+        rf = rs[int(pick[n, 1]) % len(rs)] if rs else ""
+        if r < 0.05:
+            feat = f"U{k:02}:{rf}"  # a unigram feature: no '/' once BOS/EOS is gone
+        elif r < 0.10:
+            feat = f"BOS/EOS/{rf}"
+        elif r < 0.15:
+            feat = f"{lf}/BOS/EOS"
+        elif r < 0.20:
+            feat = f"{lf}/未知{int(pick[n, 1]) % 97}"
+        else:
+            feat = f"{lf}/{rf}"
+        lines.append(f"{w[n]:.6f}\t{feat}")
+    return {"feature.def": feature_def, "left-id.def": left_id_def, "right-id.def": right_id_def,
+            "model.def": "\n".join(lines) + "\n"}
+
+
+def _split_csv(row):
+    """Fields of one CSV row with '"' quoting (the rows make_mecab_model writes)."""
+    out, cur, q, i = [], [], False, 0
+    while i < len(row):
+        c = row[i]
+        if q:
+            if c == '"' and i + 1 < len(row) and row[i + 1] == '"':
+                cur.append('"')
+                i += 1
+            elif c == '"':
+                q = False
+            else:
+                cur.append(c)
+        elif c == '"' and not cur:
+            q = True
+        elif c == ",":
+            out.append("".join(cur))
+            cur = []
+        else:
+            cur.append(c)
+        i += 1
+    out.append("".join(cur))
+    return out
