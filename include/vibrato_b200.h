@@ -194,7 +194,8 @@ int32_t vbt_tokenizer_new_multi(const vbt_dict *d, int32_t ignore_space, uint64_
  * "cudaMemcpyPeer" | "single device", "token_gather": ..., "numa_pinned": [...]}.  A single-device tokenizer also
  * names the Viterbi kernel that did the work in its last call: "last_viterbi": "k_viterbi" (round 1; every counted
  * run) | "k_viterbi2" (with lower-bound pruning) | "k_viterbi2_unpruned" (viterbi_kernel 2, the Raw and Dual
- * connectors, or a batch holding a sentence of more than 16 000 characters) | "none" (no call yet, or no sentence). */
+ * connectors, or a batch holding a sentence of more than 16 000 characters) | "k_small_batch" (the whole call in one
+ * kernel, see the option "small_batch") | "none" (no call yet, or no sentence). */
 int32_t vbt_tokenizer_describe(const vbt_tokenizer *t, char *buf, size_t cap);
 /* Restricts the calling thread to the CPUs of the NUMA node `device` hangs off (host-side copies of a rank then
  * stay on its socket); never widens the process's own affinity mask. */
@@ -252,7 +253,14 @@ int32_t vbt_tokenizer_set_counting(vbt_tokenizer *t, int32_t on);
  * Viterbi kernel (default 16), "sort_by_length" = 0|1 (default 0: process sentences in input order),
  * "chunk_sentences" = sentences per chunk of the pipelined host path (default 262144, 0 = off),
  * "dual_stream" = 0|1 (default 0: chunks share one compute stream), "counting" = 0|1,
- * "connid_counting" = 0|1 (see vbt_connid_counts), "output_mode" = 0|1|2|3 (see vbt_result_text; default 0). */
+ * "connid_counting" = 0|1 (see vbt_connid_counts), "output_mode" = 0|1|2|3 (see vbt_result_text; default 0),
+ * "small_batch" = N in 0..65536 (default 0 = off): a vbt_tokenize_batch call of at most N sentences and 16 KiB of
+ * input, without "counting" or "connid_counting", runs every stage, the text of "output_mode" included, in ONE
+ * kernel launch (k_small_batch) with one copy each way and one synchronisation; tokens and text are the same as on
+ * the usual route.  vbt_last_launch_count then gives 1 and vbt_last_stage_ms books the whole kernel under
+ * "viterbi".  A batch whose candidates or text outgrow the route's fixed scratch runs again on the usual route
+ * (describe() names the route that ran).  vbt_tokenize_batch_device and the shards of a multi-device tokenizer
+ * keep the usual route. */
 int32_t vbt_tokenizer_set_option(vbt_tokenizer *t, const char *name, int64_t value);
 /* Worker::init_connid_counter / update_connid_counts / compute_connid_probs (worker.rs:77-103): switch
  * the option "connid_counting" on (this zeroes the counters), tokenise the corpus, then read the edge

@@ -227,6 +227,11 @@ impl Tokenizer {
         check(unsafe { vbt_tokenizer_set_option(self.handle(), b"output_mode\0".as_ptr() as *const c_char,
                                                 mode.map_or(0, |m| m as i64)) })
     }
+    /// Batches of at most `n` sentences and 16 KiB tokenised afterwards run in one kernel launch (`k_small_batch`),
+    /// with the same tokens and text: the per-sentence `Worker` loop pays one launch per call.  0 = off (the default).
+    pub fn small_batch(&self, n: u32) -> Result<()> {
+        check(unsafe { vbt_tokenizer_set_option(self.handle(), b"small_batch\0".as_ptr() as *const c_char, n as i64) })
+    }
     /// The loop of the `evaluate` tool (evaluate/src/main.rs:61-138): (num_ref, num_sys, num_cor).
     pub fn evaluate(&self, corpus: &str, feature_indices: &[usize]) -> Result<(u64, u64, u64)> {
         let idx: Vec<u64> = feature_indices.iter().map(|&i| i as u64).collect();

@@ -502,6 +502,13 @@ class Tokenizer:
         self.set_option("output_mode", OUTPUT_MODES[mode])
         return self
 
+    def small_batch(self, n=64):
+        """Batches of at most `n` sentences and 16 KiB tokenised afterwards run in one kernel launch (k_small_batch):
+        one copy up, one launch, one copy down, one synchronisation, with the same tokens and text.  Counted runs
+        keep the usual route.  0 switches the route off (the default)."""
+        self.set_option("small_batch", int(n))
+        return self
+
     def describe(self):
         """dict: devices, how the dictionary image travelled ("nccl <version>" / "cudaMemcpyPeer" / "single device"), ..."""
         import json

@@ -67,6 +67,7 @@ int main(int argc, char** argv) {
         std::fprintf(stderr, "Ready to tokenize\n");
         const bool tty_out = isatty(STDOUT_FILENO), tty_in = isatty(STDIN_FILENO);
         const size_t batch_lines = tty_in ? 1 : batch_lines_arg;
+        if (batch_lines == 1) tokenizer.small_batch(1);  // a line at a time: one kernel launch per line
         std::string out;
         cli::Packed pk;
         std::string line;

@@ -214,6 +214,9 @@ class Tokenizer {
         if (m < 0) throw VibratoError(VBT_ERR_INVALID_ARGUMENT, "Could not parse a mode");
         check(vbt_tokenizer_set_option(handle(), "output_mode", m));
     }
+    // Batches of at most n sentences and 16 KiB run in one kernel launch (k_small_batch), with the same tokens and
+    // text; counted runs keep the usual route.  0 = off (the default).
+    void small_batch(uint32_t n = 64) const { check(vbt_tokenizer_set_option(handle(), "small_batch", int64_t(n))); }
     // Worker::init_connid_counter / update_connid_counts / compute_connid_probs (worker.rs:77-103): after
     // init_connid_counter() every batch is counted, an empty sentence counting nothing
     void init_connid_counter() const { check(vbt_tokenizer_set_option(handle(), "connid_counting", 1)); }

@@ -325,6 +325,11 @@ class EngineImpl final : public Engine {
         text_base_.release();
         for (auto* b : {&blob_own_, &in_utf8_, &in_off_, &connid_, &connid_try_}) b->release();
         for (auto& w : ws_) w.release();
+        ws_small_.release();
+        small_in_.release();
+        small_out_.release();
+        pinned_free(small_in_h_);
+        pinned_free(small_out_h_);
         cudaStreamSynchronize(aux_stream_);
         cudaStreamDestroy(aux_stream_);
         for (auto& e : base_ready_) cudaEventDestroy(e);
@@ -386,6 +391,10 @@ class EngineImpl final : public Engine {
             viterbi_kernel_ = int(value);
         } else if (name == "counting") {
             counting_ = value != 0;
+        } else if (name == "small_batch") {
+            // host batches of at most `value` sentences and kEagerBytes bytes take k_small_batch (0 = never)
+            if (value < 0 || value > kSmallBatchMax) throw Error(kInvalidArgument, "small_batch must be between 0 and 65536");
+            small_batch_ = uint32_t(value);
         } else {
             throw Error(kInvalidArgument, "unknown option: " + name);
         }
@@ -445,6 +454,10 @@ class EngineImpl final : public Engine {
         const uint32_t chunk = chunk_sentences_;
         const bool chunked = chunk > 0 && n_sent > chunk + chunk / 2;
         const bool fmt = output_mode_ != kOutNone;
+        if (small_batch_ && n_sent <= small_batch_ && !chunked && n_bytes <= kEagerBytes && !counting_ && !connid_on_) {
+            if (HostResult* r = run_small(utf8 + first, off, n_sent, n_bytes)) return r;
+            // the batch outgrew the scratch of k_small_batch: it runs again on the route below
+        }
         for (int attempt = 0;; ++attempt) {
             if (!chunked) {
                 h2d(in_off_.p, off, (size_t(n_sent) + 1) * 8, stream_, off_pinned && off == byte_off);
@@ -729,7 +742,7 @@ class EngineImpl final : public Engine {
     int device() const override { return device_; }
     uint32_t token_bytes() const override { return tok_bytes_; }
     std::string describe() const override {
-        static const char* const kRouteNames[] = {"none", "k_viterbi", "k_viterbi2", "k_viterbi2_unpruned"};
+        static const char* const kRouteNames[] = {"none", "k_viterbi", "k_viterbi2", "k_viterbi2_unpruned", "k_small_batch"};
         return "{\"devices\": [" + std::to_string(device_) + "], \"dictionary_transport\": \"single device\", \"token_gather\": \"none\", " +
                "\"last_viterbi\": \"" + kRouteNames[last_route_] + "\"}";
     }
@@ -895,6 +908,149 @@ class EngineImpl final : public Engine {
         if (total) CK(cudaMemcpyAsync(r->text, out_[0].text.p, total, cudaMemcpyDeviceToHost, stream_));
         r->text_bytes = total;
         r->has_text = true;
+    }
+
+    // ---- k_small_batch route -------------------------------------------------------------------------------
+    // Its scratch is sized once for the largest batch the route accepts: per-slot arrays for the hard bound of
+    // kEagerBytes + small_batch_ + 1 slots and a pool of kSmallCands candidates (about 5 MiB with the lattice rows,
+    // so it stays in L2).  A batch with more candidates, or more text than kSmallText, flags itself and is run again
+    // on the usual route; nothing grows on the device.  Input and output each travel in ONE copy: offsets + text up
+    // through a pinned staging block, and the output region [SmallBatchOut | tok_off | text_off | tokens | text] back
+    // into another, from which the result is copied into the pooled HostResult.
+    static constexpr uint32_t kSmallCands = 131072;
+    static constexpr size_t kSmallText = size_t(2) << 20;
+    static constexpr long long kSmallBatchMax = 65536;
+    static constexpr size_t kSmallHead = 64;  // SmallBatchOut, padded
+
+    void ensure_small() {
+        Workspace& w = ws_small_;
+        const size_t ns = size_t(small_batch_) + 1, ms = kEagerBytes + ns;
+        w.n_slots.ensure(ns * 4);
+        w.slot_off.ensure(ns * 4);
+        w.eos.ensure(ns * 16);
+        w.n_tok.ensure(ns * 4);
+        w.stats.ensure(ns * 8);  // sent_len of the output stage
+        w.code_sys.ensure(ms * 4);
+        if (dv_.usr_table) w.code_usr.ensure(ms * 4);
+        w.cinfo.ensure(ms * 4);
+        w.groupable.ensure(ms * 4);
+        w.byte_pos.ensure(ms * 4);
+        w.info.ensure(ms * 8);
+        w.info_ex.ensure(ms * 8);
+        w.ends_cnt.ensure(ms * 4);
+        w.ends_meta.ensure(ms * 8);
+        w.cand.ensure(size_t(kSmallCands) * 16);
+        w.ends_hot.ensure((kSmallCands + ns) * 8);
+        w.ends_cold.ensure((kSmallCands + ns) * 16);
+        const size_t in_cap = ns * 8 + kEagerBytes;
+        const size_t out_cap = kSmallHead + 2 * ns * 8 + 16 + kEagerBytes * 24 + kSmallText;
+        small_in_.ensure(in_cap);
+        small_out_.ensure(out_cap);
+        if (small_in_cap_ < in_cap) {
+            pinned_free(small_in_h_);
+            small_in_h_ = static_cast<uint8_t*>(pinned_alloc(in_cap));
+            small_in_cap_ = in_cap;
+        }
+        if (small_out_cap_ < out_cap) {
+            pinned_free(small_out_h_);
+            small_out_h_ = static_cast<uint8_t*>(pinned_alloc(out_cap));
+            small_out_cap_ = out_cap;
+        }
+    }
+
+    // One host batch through k_small_batch: one copy up, one launch, one copy down, one synchronisation (a second
+    // copy only when the text outgrew the part of the region the first one brought back).  Returns nullptr when the
+    // batch overflowed the scratch; input errors throw like on the usual route.
+    HostResult* run_small(const char* utf8, const uint64_t* off, uint32_t n_sent, uint64_t n_bytes) {
+        ensure_small();
+        const size_t off_bytes = (size_t(n_sent) + 1) * 8;
+        std::memcpy(small_in_h_, off, off_bytes);
+        if (n_bytes) std::memcpy(small_in_h_ + off_bytes, utf8, n_bytes);
+        CK(cudaMemcpyAsync(small_in_.p, small_in_h_, off_bytes + n_bytes, cudaMemcpyHostToDevice, stream_));
+
+        const bool fmt = output_mode_ != kOutNone;
+        const size_t tb = tok_bytes_;
+        const size_t at_tok_off = kSmallHead, at_text_off = at_tok_off + off_bytes;
+        const size_t at_tokens = (at_text_off + (fmt ? off_bytes : 0) + 15) & ~size_t(15);
+        const size_t at_text = at_tokens + n_bytes * tb;
+        uint8_t* region = small_out_.as<uint8_t>();
+        Workspace& w = ws_small_;
+        Batch b{};
+        b.utf8 = small_in_.as<uint8_t>() + off_bytes;
+        b.byte_off = small_in_.as<unsigned long long>();
+        b.total_bytes = n_bytes;
+        b.n_sent = n_sent;
+        b.n_slots = w.n_slots.as<uint32_t>();
+        b.slot_off = w.slot_off.as<uint32_t>();
+        b.eos = w.eos.as<uint4>();
+        b.n_tok = w.n_tok.as<uint32_t>();
+        b.tok_off = reinterpret_cast<unsigned long long*>(region + at_tok_off);
+        b.code_sys = w.code_sys.as<uint32_t>();
+        b.code_usr = w.code_usr.as<uint32_t>();
+        b.cinfo = w.cinfo.as<uint32_t>();
+        b.groupable = w.groupable.as<uint32_t>();
+        b.byte_pos = w.byte_pos.as<uint32_t>();
+        b.info = w.info.as<uint2>();
+        b.info_ex = w.info_ex.as<uint2>();
+        b.ends_cnt = w.ends_cnt.as<uint32_t>();
+        b.ends_meta = w.ends_meta.as<uint2>();
+        b.cand = w.cand.as<uint4>();
+        b.cand_cap = kSmallCands;
+        b.ends_hot = w.ends_hot.as<int2>();
+        b.ends_cold = w.ends_cold.as<uint4>();
+        b.tokens = region + at_tokens;
+        b.compact = tb == 16 ? 1u : 0u;
+        FormatArgs f{};
+        f.utf8 = b.utf8;
+        f.byte_off = b.byte_off;
+        f.n_sent = n_sent;
+        f.tok_off = b.tok_off;
+        f.tokens = static_cast<const uint2*>(b.tokens);
+        f.sent_len = w.stats.as<unsigned long long>();
+        f.text_off = reinterpret_cast<unsigned long long*>(region + at_text_off);
+        f.text = region + at_text;
+        f.text_cap = small_out_cap_ - at_text;  // the device region and its pinned twin have (at least) this size
+        f.mode = output_mode_;
+
+        // the first copy brings the text expected from the learned ratio; more comes in a second one
+        const size_t text_guess = fmt ? std::min<size_t>(f.text_cap, size_t(double(n_bytes) * text_per_byte_[output_mode_]) +
+                                                                         size_t(n_sent) * 4 + 256)
+                                      : 0;
+        OutSlot& o = out_[0];
+        CK(cudaEventRecord(o.ev[0], stream_));
+        launch_small_batch(dv_, b, f, reinterpret_cast<SmallBatchOut*>(region), stream_);
+        CK(cudaGetLastError());
+        CK(cudaEventRecord(o.ev[1], stream_));
+        CK(cudaMemcpyAsync(small_out_h_, region, at_text + text_guess, cudaMemcpyDeviceToHost, stream_));
+        CK(cudaStreamSynchronize(stream_));
+        SmallBatchOut h;
+        std::memcpy(&h, small_out_h_, sizeof h);
+        if (h.flags & kFlagBadOffsets)
+            throw Error(kInvalidArgument, "byte_offsets must be non-decreasing and end within the input buffer");
+        if (h.flags & kFlagUtf8Error) throw Error(kUtf8, "stream did not contain valid UTF-8");
+        if (h.flags & (kFlagPoolOverflow | kFlagTextOverflow)) return nullptr;
+        if (fmt && h.text_bytes > text_guess) {
+            CK(cudaMemcpyAsync(small_out_h_ + at_text + text_guess, region + at_text + text_guess, h.text_bytes - text_guess,
+                               cudaMemcpyDeviceToHost, stream_));
+            CK(cudaStreamSynchronize(stream_));
+            if (n_bytes)
+                text_per_byte_[output_mode_] = std::max(text_per_byte_[output_mode_] * 1.5, double(h.text_bytes) / double(n_bytes) * 1.25);
+        }
+        HostResult* r = acquire(n_sent, h.n_tokens);
+        std::memcpy(r->tok_off, small_out_h_ + at_tok_off, off_bytes);
+        if (h.n_tokens) std::memcpy(r->tokens, small_out_h_ + at_tokens, h.n_tokens * tb);
+        if (fmt) {
+            ensure_text(r, n_sent, h.text_bytes);
+            std::memcpy(r->text_off, small_out_h_ + at_text_off, off_bytes);
+            if (h.text_bytes) std::memcpy(r->text, small_out_h_ + at_text, h.text_bytes);
+            r->text_bytes = h.text_bytes;
+            r->has_text = true;
+        }
+        std::memset(stage_ms_, 0, sizeof(stage_ms_));
+        CK(cudaEventElapsedTime(&stage_ms_[kSmallBatchStage], o.ev[0], o.ev[1]));
+        launches_ = 1;
+        last_route_ = kRouteSmallBatch;
+        return r;
     }
 
     template <typename In, typename Out>
@@ -1114,6 +1270,12 @@ class EngineImpl final : public Engine {
     int ring_next_ = 0;
     static constexpr uint64_t kEagerBytes = 16384;
     HostResult* eager_sink_ = nullptr;
+    uint32_t small_batch_ = 0;  // "small_batch": the most sentences k_small_batch takes (0 = the route is off)
+    Workspace ws_small_;        // scratch of k_small_batch (its stream is unused)
+    DevBuf small_in_, small_out_;
+    uint8_t* small_in_h_ = nullptr;  // pinned staging of the input / output region (ensure_small)
+    uint8_t* small_out_h_ = nullptr;
+    size_t small_in_cap_ = 0, small_out_cap_ = 0;
     uint64_t staged_bytes_ = 0;  // bytes of pageable caller memory that went through the ring (last batch)
     uint32_t shard_n_sent_ = 0;
     bool shard_text_ = false;  // the last shard was formatted: shard_text_bytes_ of text in out_[0].text

@@ -27,6 +27,9 @@ struct HostResult {  // pinned host memory holding one batch's tokens
 
 constexpr int kNumStages = 9;
 extern const char* const kStageNames;  // comma-separated, kNumStages entries
+// A call on the k_small_batch route ("small_batch" option) runs every stage in one kernel: its whole time is booked
+// under "viterbi" and the other stages read 0.
+constexpr int kSmallBatchStage = 5;
 
 class Engine {
    public:
@@ -70,7 +73,9 @@ class Engine {
     virtual void set_counting(bool on) = 0;
     // Knobs: "lanes_per_sentence" (4/8/16/32), "sort_by_length" (0/1), "counting" (0/1), "chunk_sentences",
     // "dual_stream", "connid_counting", "output_mode" (0 none, 1 mecab, 2 wakati, 3 detail: run_host also
-    // produces HostResult::text, on every host route; run_device stays token-only).
+    // produces HostResult::text, on every host route; run_device stays token-only), "small_batch" (N > 0: run_host
+    // takes k_small_batch for batches of at most N sentences and 16 KiB without counting; run_device and the shards
+    // of a multi-device engine keep the usual route).
     virtual void set_option(const std::string& name, long long value) = 0;
     // Launch on a caller-owned CUDA stream (0 restores the engine's own stream).
     virtual void set_stream(uint64_t stream) = 0;

@@ -343,6 +343,67 @@ __device__ __forceinline__ uint32_t gen_unknown(const DictView& d, uint32_t sw, 
     return count;
 }
 
+// Where the word of start position `slot` begins (tokenizer.rs:117-130); g0 = groupable[slot], 0 for the sentinel.
+// At a space (ignore_space) the groupable run is skipped; a skip that reaches the end of the sentence leaves the
+// trailing flag and no candidates.
+struct StartWord {
+    uint32_t sw, skip, flags, ci, g;
+    bool active;
+};
+__device__ __forceinline__ StartWord start_word(const DictView& d, const Batch& b, uint32_t slot, uint32_t g0) {
+    StartWord w{slot, 0, 0, 0, 0, g0 != 0};
+    if (w.active) {
+        uint32_t ci0 = b.cinfo[slot];
+        if (ci_cate(ci0) & d.space_mask) {  // tokenizer.rs:117-125: skip the groupable run at a space
+            w.skip = g0;
+            w.sw = slot + w.skip;
+        }
+        w.g = w.skip ? b.groupable[w.sw] : g0;
+        if (w.g == 0) {  // start_word == len: tokenizer.rs:128-130
+            w.flags = kInfoTrailing;
+            w.active = false;
+        } else {
+            w.ci = w.skip ? b.cinfo[w.sw] : ci0;
+        }
+    }
+    return w;
+}
+
+// Candidate count of an active start position: user lexicon, system lexicon, then unknown words, the order of
+// Tokenizer::add_lattice_edges.  `matched` = some lexicon word starts here.  With hb the sources are kept for a fill.
+__device__ __forceinline__ uint32_t count_candidates(const DictView& d, const Batch& b, const StartWord& w, bool& matched,
+                                                     HitBuf* hb) {
+    WalkStats st{0, 0, 0, 0, 0};
+    uint32_t cu = 0;
+    if (d.usr_table)
+        cu = walk_lexicon<false, false>(d.usr_nodes, d.usr_num_nodes, d.usr_post, b.code_usr, b.groupable, w.sw, nullptr,
+                                        nullptr, st, hb, kSegUser);
+    uint32_t cs = walk_lexicon<false, false>(d.sys_nodes, d.sys_num_nodes, d.sys_post, b.code_sys, b.groupable, w.sw,
+                                             nullptr, nullptr, st, hb, 0);
+    matched = (cu + cs) != 0;
+    return cu + cs + gen_unknown<false>(d, w.sw, w.ci, w.g, matched, nullptr, nullptr, hb);
+}
+
+// Writes the candidates count_candidates counted to `out`, in the same order, and adds them to ends_cnt.
+__device__ __forceinline__ void fill_candidates(const DictView& d, const Batch& b, const StartWord& w, bool matched,
+                                                uint4* out) {
+    WalkStats st{0, 0, 0, 0, 0};
+    uint32_t n = 0;
+    if (d.usr_table)
+        n += walk_lexicon<true, false>(d.usr_nodes, d.usr_num_nodes, d.usr_post, b.code_usr, b.groupable, w.sw, out + n,
+                                       b.ends_cnt, st);
+    n += walk_lexicon<true, false>(d.sys_nodes, d.sys_num_nodes, d.sys_post, b.code_sys, b.groupable, w.sw, out + n,
+                                   b.ends_cnt, st);
+    gen_unknown<true>(d, w.sw, w.ci, w.g, matched, out + n, b.ends_cnt);
+}
+
+// Candidate header of a start position with g0 != 0: {cand_ptr, count}, plus the skip / flags side entry.
+__device__ __forceinline__ void store_info(const Batch& b, uint32_t slot, uint32_t ptr, uint32_t cnt, const StartWord& w) {
+    const bool special = (w.skip | w.flags) != 0;
+    b.info[slot] = make_uint2(ptr, cnt | (special ? kInfoSpecial : 0u));
+    if (special) b.info_ex[slot] = make_uint2(w.skip, w.flags);
+}
+
 __global__ void __launch_bounds__(256) k_candidates(DictView d, Batch b) {
     const uint32_t slot = blockIdx.x * blockDim.x + threadIdx.x;
     const uint32_t lane = threadIdx.x & 31;
@@ -354,39 +415,14 @@ __global__ void __launch_bounds__(256) k_candidates(DictView d, Batch b) {
     if (slot == 0 && total_slots > b.launch_slots) atomicOr(b.flags, kFlagSlotsOverflow);
     const bool in_range = slot < total_slots && !(batch_flags & kFlagBadOffsets);
     uint32_t g0 = in_range ? b.groupable[slot] : 0;
-    bool active = in_range && g0 != 0;
-    uint32_t sw = slot, skip = 0, flags = 0, ci = 0, g = 0;
-    WalkStats st{0, 0, 0, 0, 0};
-    if (active) {
-        uint32_t ci0 = b.cinfo[slot];
-        if (ci_cate(ci0) & d.space_mask) {  // tokenizer.rs:117-125: skip the groupable run at a space
-            skip = g0;
-            sw = slot + skip;
-        }
-        g = skip ? b.groupable[sw] : g0;
-        if (g == 0) {  // start_word == len: tokenizer.rs:128-130
-            flags = kInfoTrailing;
-            active = false;
-        } else {
-            ci = skip ? b.cinfo[sw] : ci0;
-        }
-    }
+    const StartWord sw = start_word(d, b, slot, g0);
+    const bool active = sw.active;
     uint32_t cnt = 0;
     bool matched = false;
     __shared__ uint2 s_hits[kMaxHits][256];
     __shared__ uint8_t s_seg_cnt[kMaxHits][256];
     HitBuf hb{&s_hits[0][threadIdx.x], &s_seg_cnt[0][threadIdx.x], 256, 0};
-    if (active) {
-        uint32_t cu = 0;
-        if (d.usr_table)
-            cu = walk_lexicon<false, false>(d.usr_nodes, d.usr_num_nodes, d.usr_post, b.code_usr, b.groupable, sw,
-                                            nullptr, nullptr, st, &hb, kSegUser);
-        uint32_t cs = walk_lexicon<false, false>(d.sys_nodes, d.sys_num_nodes, d.sys_post, b.code_sys, b.groupable,
-                                                 sw, nullptr, nullptr, st, &hb, 0);
-        matched = (cu + cs) != 0;
-        uint32_t ck = gen_unknown<false>(d, sw, ci, g, matched, nullptr, nullptr, &hb);
-        cnt = cu + cs + ck;
-    }
+    if (active) cnt = count_candidates(d, b, sw, matched, &hb);
     // Block-aggregated allocation from the candidate pool: a scan inside each warp, the eight warp totals through
     // shared memory, ONE atomicAdd per block.  (One atomic per warp was 1.3 M same-address atomics per batch, and
     // every warp sat on the round trip of its own; the pool also comes out in slot order block by block.)
@@ -416,11 +452,7 @@ __global__ void __launch_bounds__(256) k_candidates(DictView d, Batch b) {
     const uint32_t warp_total = __shfl_sync(kFull, incl, 31);
     const bool fits = wbase + warp_total <= (unsigned long long)b.cand_cap;
     uint32_t ptr = uint32_t(wbase) + (incl - cnt);
-    if (in_range && g0 != 0) {
-        const bool special = (skip | flags) != 0;
-        b.info[slot] = make_uint2(ptr, (fits ? cnt : 0) | (special ? kInfoSpecial : 0u));
-        if (special) b.info_ex[slot] = make_uint2(skip, flags);
-    }
+    if (in_range && g0 != 0) store_info(b, slot, ptr, fits ? cnt : 0, sw);
     // Fill.  Usual case: every position of the warp kept its sources in the segment buffer; the warp's candidates
     // (contiguous in the pool, in position order) are then dealt to the 32 lanes as ONE list — lane i writes entries
     // i, i + 32, ...: full-width, coalesced stores and loads that walk postings lists side by side, instead of
@@ -467,16 +499,8 @@ __global__ void __launch_bounds__(256) k_candidates(DictView d, Batch b) {
             }
         }
     } else if (active && fits && cnt) {  // some position has more sources than the buffer holds: regenerate per thread
-        uint4* out = b.cand + ptr;
-        uint32_t w = 0;
-        if (d.usr_table)
-            w += walk_lexicon<true, false>(d.usr_nodes, d.usr_num_nodes, d.usr_post, b.code_usr, b.groupable, sw,
-                                           out + w, b.ends_cnt, st);
-        w += walk_lexicon<true, false>(d.sys_nodes, d.sys_num_nodes, d.sys_post, b.code_sys, b.groupable, sw,
-                                       out + w, b.ends_cnt, st);
-        gen_unknown<true>(d, sw, ci, g, matched, out + w, b.ends_cnt);
+        fill_candidates(d, b, sw, matched, b.cand + ptr);
     }
-    (void)st;
 }
 
 // Side array for counted runs: per slot {M, T, P, W} so that k_viterbi can sum them over the
@@ -694,14 +718,11 @@ struct ConnRow<2> {  // DualConnector::cost (dual_connector.rs:269-280): reduced
     }
 };
 
+// The sweep of k_viterbi over sentence `sidx` of each G-lane group of the calling warp (every lane calls it).
 template <int G, bool COUNT, int CONN>
-__global__ void __launch_bounds__(128, (CONN == 0 && !COUNT) ? VBT_K3_MIN_BLOCKS : 8) k_viterbi(DictView d, Batch b, const uint4* __restrict__ stats) {
-    if (stand_down(*b.flags)) return;
-    constexpr uint32_t SPW = 32 / G;  // sentences per warp
-    const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+__device__ __forceinline__ void viterbi_sweep(const DictView& d, const Batch& b, const uint4* __restrict__ stats, uint32_t sidx) {
     const uint32_t lane = threadIdx.x & 31;
     const uint32_t sub = lane / G, gl = lane % G;
-    const uint32_t sidx = warp * SPW + sub;
     unsigned long long cntE = 0, cntN = 2, cM = 0, cT = 0, cP = 0, cW = 0, cWalks = 0;
 
     // Loop state is kept slot-absolute (current slot, the slot whose row EOS connects to, first slot after a
@@ -837,6 +858,14 @@ __global__ void __launch_bounds__(128, (CONN == 0 && !COUNT) ? VBT_K3_MIN_BLOCKS
             atomicAdd(&b.counters[kCntWalks], cWalks);
         }
     }
+}
+
+template <int G, bool COUNT, int CONN>
+__global__ void __launch_bounds__(128, (CONN == 0 && !COUNT) ? VBT_K3_MIN_BLOCKS : 8) k_viterbi(DictView d, Batch b, const uint4* __restrict__ stats) {
+    if (stand_down(*b.flags)) return;
+    constexpr uint32_t SPW = 32 / G;  // sentences per warp
+    const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    viterbi_sweep<G, COUNT, CONN>(d, b, stats, warp * SPW + (threadIdx.x & 31) / G);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1131,10 +1160,7 @@ __global__ void __launch_bounds__(32 * VBT_K3V2_WARPS, CONN == 0 ? VBT_K3V2_MIN_
 // character, and a path has at most one node per character).  After the token-offset scan K4b turns those entries
 // into token records with a warp per sentence — the pointer chase is not repeated and the 24-byte records of a
 // sentence are written by neighbouring lanes.
-__global__ void __launch_bounds__(256) k_backtrack_count(Batch b) {
-    if (stand_down(*b.flags)) return;
-    uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
-    if (s >= b.n_sent) return;
+__device__ __forceinline__ void backtrack_count_one(const Batch& b, uint32_t s) {
     uint4 e = b.eos[s];
     uint32_t k = 0;
     if (e.x != kNone) {
@@ -1152,14 +1178,15 @@ __global__ void __launch_bounds__(256) k_backtrack_count(Batch b) {
     if (b.counters && k) atomicAdd(&b.counters[kCntK], (unsigned long long)k);
 }
 
-__global__ void __launch_bounds__(256) k_backtrack_write(Batch b) {
+__global__ void __launch_bounds__(256) k_backtrack_count(Batch b) {
     if (stand_down(*b.flags)) return;
-    const uint32_t w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    const uint32_t lane = threadIdx.x & 31;
-#pragma unroll 1
-    for (uint32_t r = 0; r < VBT_SENT_PER_WARP; ++r) {
-    const uint32_t s = w * VBT_SENT_PER_WARP + r;
+    uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= b.n_sent) return;
+    backtrack_count_one(b, s);
+}
+
+// Token records of sentence s at tok_off[s], from the path entries backtrack_count_one left (a warp per sentence).
+__device__ __forceinline__ void backtrack_write_one(const Batch& b, uint32_t s, uint32_t lane) {
     const uint32_t base = b.slot_off[s];
     const unsigned long long t0 = b.tok_off[s];
     const uint32_t n = uint32_t(b.tok_off[s + 1] - t0);
@@ -1181,6 +1208,17 @@ __global__ void __launch_bounds__(256) k_backtrack_write(Batch b) {
         t[1] = bytes;
         t[2] = make_uint2(c.z, c.w);  // word_idx, total_cost
     }
+}
+
+__global__ void __launch_bounds__(256) k_backtrack_write(Batch b) {
+    if (stand_down(*b.flags)) return;
+    const uint32_t w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const uint32_t lane = threadIdx.x & 31;
+#pragma unroll 1
+    for (uint32_t r = 0; r < VBT_SENT_PER_WARP; ++r) {
+        const uint32_t s = w * VBT_SENT_PER_WARP + r;
+        if (s >= b.n_sent) return;
+        backtrack_write_one(b, s, lane);
     }
 }
 
@@ -1276,9 +1314,8 @@ __device__ __forceinline__ bool format_stands_down(const FormatArgs& f) {
     return *f.flags & (kFlagsStandDown | kFlagUtf8Error | kFlagPoolOverflow);
 }
 
-__global__ void __launch_bounds__(256) k_format_len(DictView d, FormatArgs f) {
-    const uint32_t s = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-    if (s >= f.n_sent || format_stands_down(f)) return;
+// Pass 1 for sentence s (a warp per sentence): lane 0 stores its text length in sent_len[s].
+__device__ __forceinline__ void format_len_one(const DictView& d, const FormatArgs& f, uint32_t s, uint32_t lane) {
     const unsigned long long t0 = f.tok_off[s], t1 = f.tok_off[s + 1];
     unsigned long long len = 0;
     for (unsigned long long t = t0 + lane; t < t1; t += 32) len += token_text_len(d, token_text(d, f.tokens, t), f.mode, t == t0);
@@ -1286,19 +1323,18 @@ __global__ void __launch_bounds__(256) k_format_len(DictView d, FormatArgs f) {
     if (lane == 0) f.sent_len[s] = len + (f.mode == kOutWakati ? 1 : 4);  // "\n" or "EOS\n"
 }
 
+__global__ void __launch_bounds__(256) k_format_len(DictView d, FormatArgs f) {
+    const uint32_t s = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (s >= f.n_sent || format_stands_down(f)) return;
+    format_len_one(d, f, s, lane);
+}
+
 __device__ __forceinline__ void warp_copy(uint8_t* __restrict__ dst, const uint8_t* __restrict__ src, uint32_t n, uint32_t lane) {
     for (uint32_t i = lane; i < n; i += 32) dst[i] = src[i];
 }
 
-__global__ void __launch_bounds__(256) k_format_write(DictView d, FormatArgs f) {
-    const uint32_t s = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-    if (s >= f.n_sent || format_stands_down(f)) return;
-    const unsigned long long total = f.text_off[f.n_sent];
-    if (s == 0 && lane == 0) {
-        *f.text_total = total;
-        if (total > f.text_cap) atomicOr(f.flags, kFlagTextOverflow);
-    }
-    if (total > f.text_cap) return;  // every warp sees the same total: nothing is written
+// Pass 2 for sentence s (a warp per sentence): its text at text_off[s], which must fit in text_cap.
+__device__ __forceinline__ void format_write_one(const DictView& d, const FormatArgs& f, uint32_t s, uint32_t lane) {
     const unsigned long long t0 = f.tok_off[s], t1 = f.tok_off[s + 1];
     const uint8_t* __restrict__ sent = f.utf8 + f.byte_off[s];
     unsigned long long base = f.text_off[s];  // where the next group of 32 tokens starts
@@ -1367,7 +1403,164 @@ __global__ void __launch_bounds__(256) k_format_write(DictView d, FormatArgs f) 
     }
 }
 
+__global__ void __launch_bounds__(256) k_format_write(DictView d, FormatArgs f) {
+    const uint32_t s = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (s >= f.n_sent || format_stands_down(f)) return;
+    const unsigned long long total = f.text_off[f.n_sent];
+    if (s == 0 && lane == 0) {
+        *f.text_total = total;
+        if (total > f.text_cap) atomicOr(f.flags, kFlagTextOverflow);
+    }
+    if (total > f.text_cap) return;  // every warp sees the same total: nothing is written
+    format_write_one(d, f, s, lane);
+}
+
+// ---------------------------------------------------------------------------------------------
+// k_small_batch: the whole pipeline above for a small host batch in ONE thread block, so that a call costs one
+// launch.  The device-wide scans between the kernels become block scans between __syncthreads(); each stage calls
+// the per-sentence / per-position bodies of its kernel:
+//   count_chars_one -> scan -> decode_one -> start_word / count_candidates / fill_candidates -> scan -> viterbi_sweep
+//   (k_viterbi's sweep, 32 lanes per sentence, no pruning) -> backtrack_count_one -> scan -> backtrack_write_one
+//   [-> format_len_one -> scan -> format_write_one].
+// A warp takes one sentence at a time, a thread one start position.  The batch flags live in shared memory and
+// go out with the totals in SmallBatchOut.  A candidate pool or text larger than the buffers the engine gave sets
+// kFlagPoolOverflow / kFlagTextOverflow and ends the kernel: the engine then runs the batch on the usual route.
+// ---------------------------------------------------------------------------------------------
+
+constexpr uint32_t kSmallThreads = 1024;
+
+// Exclusive prefix of v over the block's threads in thread order; *total = the block's sum.  Every thread calls it.
+__device__ __forceinline__ unsigned long long block_exclusive(unsigned long long v, unsigned long long& total,
+                                                              unsigned long long* s_warp /* [32] */) {
+    const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
+    unsigned long long incl = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const unsigned long long t = __shfl_up_sync(kFull, incl, o);
+        if (lane >= uint32_t(o)) incl += t;
+    }
+    if (lane == 31) s_warp[wid] = incl;
+    __syncthreads();
+    unsigned long long before = 0, sum = 0;
+    for (uint32_t i = 0; i < nw; ++i) {
+        const unsigned long long t = s_warp[i];
+        if (i < wid) before += t;
+        sum += t;
+    }
+    __syncthreads();  // s_warp is free again
+    total = sum;
+    return before + incl - v;
+}
+
+// out(i, exclusive prefix of get(0..i)) for i in [0, n]; out(n) = the total, which is returned.  Every thread calls
+// it; everything written is visible to the whole block on return.
+template <class Get, class Put>
+__device__ __forceinline__ unsigned long long block_scan(uint32_t n, Get get, Put put, unsigned long long* s_warp) {
+    unsigned long long carry = 0;
+    for (uint32_t base = 0; base < n; base += blockDim.x) {
+        const uint32_t i = base + threadIdx.x;
+        unsigned long long tile;
+        const unsigned long long ex = block_exclusive(i < n ? (unsigned long long)get(i) : 0ull, tile, s_warp);
+        if (i < n) put(i, carry + ex);
+        carry += tile;
+    }
+    if (threadIdx.x == 0) put(n, carry);
+    __syncthreads();
+    return carry;
+}
+
+template <int CONN>
+__global__ void __launch_bounds__(kSmallThreads, 1) k_small_batch(DictView d, Batch b, FormatArgs f, SmallBatchOut* out) {
+    __shared__ uint32_t s_flags;
+    __shared__ unsigned long long s_warp[32];
+    const uint32_t tid = threadIdx.x, lane = tid & 31, wid = tid >> 5, nw = blockDim.x >> 5;
+    const uint32_t n = b.n_sent;
+    if (tid == 0) s_flags = 0;
+    __syncthreads();
+    b.flags = &s_flags;
+    f.flags = &s_flags;
+    uint32_t total_slots = 0;
+    unsigned long long n_tokens = 0, text_bytes = 0;
+    // K1a, then the slot scan.  `s_flags` is read right after a barrier and written again only after the next one,
+    // so every decision taken on it below is the same in all threads.
+    for (uint32_t s = wid; s < n; s += nw) count_chars_one(b, s, lane);
+    __syncthreads();
+    bool ok = !(s_flags & (kFlagsStandDown | kFlagUtf8Error));  // the engine reports the error; nothing else to do
+    if (ok) {
+        total_slots = uint32_t(block_scan(
+            n, [&](uint32_t i) { return b.n_slots[i]; }, [&](uint32_t i, unsigned long long v) { b.slot_off[i] = uint32_t(v); },
+            s_warp));
+        for (uint32_t s = wid; s < n; s += nw) {  // K1b
+            decode_one(d, b, s, lane);
+            __syncwarp();
+        }
+        __syncthreads();
+        // K2: a thread per start position; the pool is handed out in position order by a scan per block-wide tile
+        unsigned long long carry = 0;
+        for (uint32_t base = 0; base < total_slots; base += blockDim.x) {
+            const uint32_t slot = base + tid;
+            const uint32_t g0 = slot < total_slots ? b.groupable[slot] : 0;
+            const StartWord w = start_word(d, b, slot, g0);
+            bool matched = false;
+            const uint32_t cnt = w.active ? count_candidates(d, b, w, matched, nullptr) : 0;
+            unsigned long long tile;
+            const unsigned long long ptr = carry + block_exclusive(cnt, tile, s_warp);
+            carry += tile;
+            if (ptr + cnt > b.cand_cap) {
+                atomicOr(&s_flags, kFlagPoolOverflow);
+            } else if (g0 != 0) {
+                store_info(b, slot, uint32_t(ptr), cnt, w);
+                if (cnt) fill_candidates(d, b, w, matched, b.cand + ptr);
+            }
+        }
+        __syncthreads();
+        ok = !(s_flags & kFlagPoolOverflow);
+    }
+    if (ok) {
+        // lattice rows: ends_meta = {row offset, next free entry} from the node counts per end position
+        block_scan(
+            total_slots, [&](uint32_t i) { return b.ends_cnt[i]; },
+            [&](uint32_t i, unsigned long long v) { b.ends_meta[i] = make_uint2(uint32_t(v), uint32_t(v)); }, s_warp);
+        for (uint32_t s = wid; s < n; s += nw) viterbi_sweep<32, false, CONN>(d, b, nullptr, s);  // K3
+        __syncthreads();
+        for (uint32_t s = tid; s < n; s += blockDim.x) backtrack_count_one(b, s);  // K4a
+        __syncthreads();
+        n_tokens = block_scan(
+            n, [&](uint32_t i) { return b.n_tok[i]; }, [&](uint32_t i, unsigned long long v) { b.tok_off[i] = v; }, s_warp);
+        for (uint32_t s = wid; s < n; s += nw) backtrack_write_one(b, s, lane);  // K4b
+        if (f.mode != kOutNone) {  // output stage
+            __syncthreads();
+            for (uint32_t s = wid; s < n; s += nw) format_len_one(d, f, s, lane);
+            __syncthreads();
+            text_bytes = block_scan(
+                n, [&](uint32_t i) { return f.sent_len[i]; }, [&](uint32_t i, unsigned long long v) { f.text_off[i] = v; },
+                s_warp);
+            if (text_bytes > f.text_cap) {
+                if (tid == 0) atomicOr(&s_flags, kFlagTextOverflow);
+            } else {
+                for (uint32_t s = wid; s < n; s += nw) format_write_one(d, f, s, lane);
+            }
+        }
+    }
+    __syncthreads();
+    if (tid == 0) {
+        out->flags = s_flags;
+        out->total_slots = total_slots;
+        out->n_tokens = n_tokens;
+        out->text_bytes = text_bytes;
+    }
+}
+
 }  // namespace
+
+void launch_small_batch(const DictView& d, const Batch& b, const FormatArgs& f, SmallBatchOut* out, cudaStream_t st) {
+    if (d.connector_kind == 1)
+        k_small_batch<1><<<1, kSmallThreads, 0, st>>>(d, b, f, out);
+    else if (d.connector_kind == 2)
+        k_small_batch<2><<<1, kSmallThreads, 0, st>>>(d, b, f, out);
+    else
+        k_small_batch<0><<<1, kSmallThreads, 0, st>>>(d, b, f, out);
+}
 
 void launch_format_len(const DictView& d, const FormatArgs& f, cudaStream_t st) {
     if (!f.n_sent) return;

@@ -155,6 +155,7 @@ enum ViterbiRoute : uint32_t {
     kRouteV1,              // k_viterbi
     kRouteV2,              // k_viterbi2 with pruning
     kRouteV2Unpruned,      // k_viterbi2 without pruning (kernel 2, the Raw / Dual connectors, or the pruned one's twin)
+    kRouteSmallBatch,      // k_small_batch: the whole batch in one kernel (launch_small_batch)
     kRouteV2PrunedOrTwin,  // the pruned k_viterbi2 and its twin are both launched: kFlagLongSentence picks one
 };
 // The kernel that did the work, once the batch's flags are known on the host.
@@ -166,5 +167,22 @@ int launch_viterbi(const DictView& d, const Batch& b, const uint4* stats, int la
                    cudaStream_t st, uint32_t* route);
 void launch_backtrack_count(const Batch& b, cudaStream_t st);
 void launch_backtrack_write(const Batch& b, cudaStream_t st);
+
+// What k_small_batch reports besides its outputs: the batch flags and the totals of its scans.
+struct SmallBatchOut {
+    uint32_t flags;
+    uint32_t total_slots;
+    unsigned long long n_tokens;
+    unsigned long long text_bytes;  // 0 unless f.mode != kOutNone
+    unsigned long long reserved;
+};
+// Every stage from count_chars to backtrack_write, and the output stage when f.mode != kOutNone, for a whole batch
+// in ONE launch of one thread block.  Inputs as for the separate kernels except: b.flags and f.flags are ignored
+// (the kernel keeps the flags in shared memory and reports them in *out), b.order / counters / lid_count must be
+// null, b.launch_slots and b.pool_ctr are unused, and the per-slot arrays must hold n_bytes + n_sent + 1 entries
+// (the hard bound), so only the candidate pool (b.cand_cap; ends_hot / ends_cold need cand_cap + n_sent + 1
+// entries) and the text (f.text_cap) can overflow: kFlagPoolOverflow / kFlagTextOverflow, the outputs are then void.
+// f.tok_off / f.tokens must equal b.tok_off / b.tokens; f.sent_len needs n_sent entries, f.text_off n_sent + 1.
+void launch_small_batch(const DictView& d, const Batch& b, const FormatArgs& f, SmallBatchOut* out, cudaStream_t st);
 
 }  // namespace vbt
