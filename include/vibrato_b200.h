@@ -262,6 +262,27 @@ int32_t vbt_tokenizer_set_counting(vbt_tokenizer *t, int32_t on);
  * (describe() names the route that ran).  vbt_tokenize_batch_device and the shards of a multi-device tokenizer
  * keep the usual route. */
 int32_t vbt_tokenizer_set_option(vbt_tokenizer *t, const char *name, int64_t value);
+/* MeCab-style output formats, rendered on the device in place of the option "output_mode": batches tokenised
+ * afterwards carry the text of the format in vbt_result_text, on every host route (whole batch, chunked pipeline,
+ * "small_batch", multi-device).  `node` is printed per System / User token, `unk` per Unknown token (NULL: the same
+ * as node), `bos` before and `eos` after every sentence (NULL: "" and "EOS\n").  Strings are taken by length, not
+ * NUL-terminated.  Directives ("prev" = the previous token of the sentence, or BOS with cost 0 and end byte 0):
+ *   %m surface, %M bytes from prev's end to this token's end (skipped spaces + surface), %pS the skipped spaces
+ *   only, %H the feature string, %f[N1,N2,..] feature fields joined by TAB, %F<c>[N1,..] joined by the byte or
+ *   escape <c> (fields split as the evaluate tool splits them, quotes removed; a field whose text begins with '*',
+ *   or that the feature does not have, is left out with its separator), %c / %pw word cost, %pc total cost,
+ *   %pn total cost - prev's, %pC total cost - prev's - word cost (both wrapping i32), %ps / %pe start / end byte,
+ *   %pl surface bytes, %pL end byte - prev's end byte, %phl / %phr left / right id, %s 0 for System / User and 1 for
+ *   Unknown, %S / %L the sentence and its byte length, %% a '%'.  Escapes: \0 \a \b \t \n \v \f \r \s (space)
+ *   \\.  bos / eos take only literals, escapes, %%, %S and %L.  An unknown or malformed directive or escape, a
+ *   MeCab directive without a value on the best path (%h %t %P %pP %pA %pB %pi %pb %pp), more than 16 distinct field
+ *   indices or one above 255 give VBT_ERR_INVALID_ARGUMENT with the directive and its byte position in
+ *   vbt_last_error().  A format that references fields builds a table of them on each device (once per call of this
+ *   function).  Setting "output_mode" replaces the format; node == NULL switches it off.  Excludes
+ *   "compact_tokens". */
+int32_t vbt_tokenizer_set_output_format(vbt_tokenizer *t, const char *node, size_t node_len, const char *unk,
+                                        size_t unk_len, const char *bos, size_t bos_len, const char *eos,
+                                        size_t eos_len);
 /* Worker::init_connid_counter / update_connid_counts / compute_connid_probs (worker.rs:77-103): switch
  * the option "connid_counting" on (this zeroes the counters), tokenise the corpus, then read the edge
  * counts of every lattice (Lattice::add_connid_counts, lattice.rs:170-183) in the dictionary's own ids:

@@ -49,6 +49,9 @@ extern "C" {
     fn vbt_dict_map_connection_ids(d: *mut vbt_dict, lmap: *const u16, n_lmap: usize, rmap: *const u16,
                                    n_rmap: usize) -> i32;
     fn vbt_tokenizer_set_option(t: *mut vbt_tokenizer, name: *const c_char, value: i64) -> i32;
+    fn vbt_tokenizer_set_output_format(t: *mut vbt_tokenizer, node: *const c_char, node_len: usize,
+                                       unk: *const c_char, unk_len: usize, bos: *const c_char, bos_len: usize,
+                                       eos: *const c_char, eos_len: usize) -> i32;
     fn vbt_result_text(r: *const vbt_result, text_offsets: *mut *const u64, text: *mut *const c_char,
                        n_bytes: *mut u64) -> i32;
     fn vbt_evaluate(d: *const vbt_dict, t: *mut vbt_tokenizer, corpus: *const c_char, len: usize,
@@ -226,6 +229,15 @@ impl Tokenizer {
     pub fn output_mode(&self, mode: Option<OutputMode>) -> Result<()> {
         check(unsafe { vbt_tokenizer_set_option(self.handle(), b"output_mode\0".as_ptr() as *const c_char,
                                                 mode.map_or(0, |m| m as i64)) })
+    }
+    /// MeCab-style output formats (node / unk / BOS / EOS format strings, as `tokenize -F`), rendered on the device
+    /// in place of `output_mode`: `BatchResult::text`.  `node == None` switches the format off; `unk == None` prints
+    /// Unknown tokens with `node`, `bos` / `eos == None` print "" / "EOS\n".
+    pub fn output_format(&self, node: Option<&str>, unk: Option<&str>, bos: Option<&str>, eos: Option<&str>)
+                         -> Result<()> {
+        let p = |x: Option<&str>| x.map_or((std::ptr::null(), 0), |s| (s.as_ptr() as *const c_char, s.len()));
+        let (n, u, b, e) = (p(node), p(unk), p(bos), p(eos));
+        check(unsafe { vbt_tokenizer_set_output_format(self.handle(), n.0, n.1, u.0, u.1, b.0, b.1, e.0, e.1) })
     }
     /// Batches of at most `n` sentences and 16 KiB tokenised afterwards run in one kernel launch (`k_small_batch`),
     /// with the same tokens and text: the per-sentence `Worker` loop pays one launch per call.  0 = off (the default).

@@ -344,6 +344,7 @@ class Tokenizer:
         self._device = device
         self._h = None
         self._options = {}  # engine options set so far: replayed when the engine is rebuilt (ignore_space / max_grouping_len)
+        self._format = None  # (node, unk, bos, eos) of output_format(), replayed after the options
         self._stream = 0
         self._counting = False
         self._free = lib().vbt_tokenizer_free
@@ -403,6 +404,8 @@ class Tokenizer:
             # a rebuilt engine starts from defaults: put back what the caller had configured
             for name, value in self._options.items():
                 check(lib().vbt_tokenizer_set_option(h, name.encode(), int(value)))
+            if self._format is not None:
+                self._set_format(h, self._format)
             if self._counting:
                 check(lib().vbt_tokenizer_set_counting(h, 1))
             if self._stream:
@@ -472,6 +475,8 @@ class Tokenizer:
         check(lib().vbt_tokenizer_set_option(self.handle(), name.encode(), int(value)))
         if name != "connid_counting":  # accumulated counts cannot be carried into a rebuilt engine
             self._options[name] = int(value)
+        if name == "output_mode":  # a fixed mode replaces an output format
+            self._format = None
 
     def evaluate(self, corpus, feature_indices=()):
         """The loop of the `evaluate` tool (evaluate/src/main.rs:61-138) over a `surface\\tfeature` / `EOS` corpus:
@@ -501,6 +506,30 @@ class Tokenizer:
             raise VibratoError(1, "Could not parse a mode")  # tokenize/src/main.rs:26
         self.set_option("output_mode", OUTPUT_MODES[mode])
         return self
+
+    def output_format(self, node, unk=None, bos="", eos="EOS\n"):
+        """MeCab-style output formats (`-F` / `--unk-format` / `--bos-format` / `--eos-format`), rendered on the
+        device: batches tokenised afterwards carry the text in BatchResult.text().  `node` is printed per System / User
+        token, `unk` per Unknown token (None: as node), `bos` / `eos` before / after every sentence.  The directives
+        are listed in README.md and include/vibrato_b200.h.  Replaces output_mode(); output_format(None) switches the
+        format off.  str or bytes."""
+        if node is None:
+            check(lib().vbt_tokenizer_set_output_format(self.handle(), None, 0, None, 0, None, 0, None, 0))
+            self._format = None
+            return self
+        enc = lambda x: None if x is None else (x.encode("utf-8") if isinstance(x, str) else bytes(x))  # noqa: E731
+        fmt = (enc(node), enc(unk), enc(bos), enc(eos))
+        self._set_format(self.handle(), fmt)
+        self._format = fmt
+        self._options.pop("output_mode", None)
+        return self
+
+    @staticmethod
+    def _set_format(h, fmt):
+        args = []
+        for x in fmt:
+            args += [x, len(x)] if x is not None else [None, 0]
+        check(lib().vbt_tokenizer_set_output_format(h, *args))
 
     def small_batch(self, n=64):
         """Batches of at most `n` sentences and 16 KiB tokenised afterwards run in one kernel launch (k_small_batch):

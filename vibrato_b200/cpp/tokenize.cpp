@@ -12,7 +12,10 @@ using namespace vibrato_b200;
 static void usage() {
     std::fprintf(stderr,
                  "tokenize -i <system.dic.zst | mecab-source-dir> [-u user.csv] [-O mecab|wakati|detail] [-S] [-M n]\n"
-                 "         [--format-on device|host]   (where the output text is built; default device)\n"
+                 "         [-F|--node-format FMT] [--unk-format FMT] [--bos-format FMT] [--eos-format FMT]\n"
+                 "                                     (MeCab-style formats, built on the device; -F takes precedence over -O;\n"
+                 "                                      unk defaults to the node format, bos to \"\", eos to \"EOS\\n\")\n"
+                 "         [--format-on device|host]   (where the output text is built; default device; -F needs device)\n"
                  "         [--devices 0,1,..]          (spread every batch over these GPUs)\n"
                  "         [--batch-lines N]           (lines per batch when stdin is not a terminal; default 65536)\n");
 }
@@ -22,6 +25,8 @@ int main(int argc, char** argv) {
     bool ignore_space = false;
     size_t max_grouping_len = 0, batch_lines_arg = 65536;
     std::vector<int32_t> devices;
+    std::string node_format, unk_format, bos_format, eos_format;
+    bool has_node = false, has_unk = false, has_bos = false, has_eos = false;
     for (int i = 1; i < argc; ++i) {
         std::string a = argv[i];
         auto next = [&]() -> std::string {
@@ -39,12 +44,17 @@ int main(int argc, char** argv) {
         else if (a == "-M" || a == "--max-grouping-len") max_grouping_len = std::stoull(next());
         else if (a == "--devices") devices = cli::parse_devices(next());
         else if (a == "--batch-lines") batch_lines_arg = std::stoull(next());
+        else if (a == "-F" || a == "--node-format") node_format = next(), has_node = true;
+        else if (a == "--unk-format") unk_format = next(), has_unk = true;
+        else if (a == "--bos-format") bos_format = next(), has_bos = true;
+        else if (a == "--eos-format") eos_format = next(), has_eos = true;
         else {
             usage();
             return 2;
         }
     }
-    if (batch_lines_arg == 0) {
+    // the formats are rendered by the device only; --unk/bos/eos-format complete -F
+    if (batch_lines_arg == 0 || (has_node && format_on == "host") || (!has_node && (has_unk || has_bos || has_eos))) {
         usage();
         return 2;
     }
@@ -63,7 +73,12 @@ int main(int argc, char** argv) {
         }
         Tokenizer tokenizer =
             Tokenizer(std::move(dict)).ignore_space(ignore_space).max_grouping_len(max_grouping_len).devices(devices);
-        if (format_on == "device") tokenizer.output_mode(mode);  // k_format_len / k_format_write build the text
+        if (has_node) {
+            const std::string_view node = node_format, unk = unk_format, bos = bos_format, eos = eos_format;
+            tokenizer.output_format(&node, has_unk ? &unk : nullptr, has_bos ? &bos : nullptr, has_eos ? &eos : nullptr);
+        } else if (format_on == "device") {
+            tokenizer.output_mode(mode);  // k_format_len / k_format_write build the text
+        }
         std::fprintf(stderr, "Ready to tokenize\n");
         const bool tty_out = isatty(STDOUT_FILENO), tty_in = isatty(STDIN_FILENO);
         const size_t batch_lines = tty_in ? 1 : batch_lines_arg;

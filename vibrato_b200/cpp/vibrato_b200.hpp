@@ -214,6 +214,16 @@ class Tokenizer {
         if (m < 0) throw VibratoError(VBT_ERR_INVALID_ARGUMENT, "Could not parse a mode");
         check(vbt_tokenizer_set_option(handle(), "output_mode", m));
     }
+    // MeCab-style output formats (node / unk / BOS / EOS format strings, see vbt_tokenizer_set_output_format),
+    // rendered on the device in place of output_mode(): BatchResult::text().  A null node switches the format off; a
+    // null unk prints Unknown tokens with node; null bos / eos print "" / "EOS\n".
+    void output_format(const std::string_view* node, const std::string_view* unk = nullptr,
+                       const std::string_view* bos = nullptr, const std::string_view* eos = nullptr) const {
+        // data() of an empty view may be null, which would read as "not given"
+        auto p = [](const std::string_view* s) -> const char* { return !s ? nullptr : s->empty() ? "" : s->data(); };
+        auto n = [](const std::string_view* s) { return s ? s->size() : size_t(0); };
+        check(vbt_tokenizer_set_output_format(handle(), p(node), n(node), p(unk), n(unk), p(bos), n(bos), p(eos), n(eos)));
+    }
     // Batches of at most n sentences and 16 KiB run in one kernel launch (k_small_batch), with the same tokens and
     // text; counted runs keep the usual route.  0 = off (the default).
     void small_batch(uint32_t n = 64) const { check(vbt_tokenizer_set_option(handle(), "small_batch", int64_t(n))); }

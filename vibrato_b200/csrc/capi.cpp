@@ -11,6 +11,7 @@
 #include "device_blob.hpp"
 #include "engine.hpp"
 #include "evaluate.hpp"
+#include "format.hpp"
 #include "host_dict.hpp"
 
 struct vbt_dict {
@@ -517,6 +518,20 @@ int32_t vbt_tokenizer_set_option(vbt_tokenizer* t, const char* name, int64_t val
         need(t, "t");
         need(name, "name");
         t->e->set_option(name, value);
+    });
+}
+
+int32_t vbt_tokenizer_set_output_format(vbt_tokenizer* t, const char* node, size_t node_len, const char* unk, size_t unk_len,
+                                        const char* bos, size_t bos_len, const char* eos, size_t eos_len) {
+    return guarded([&] {
+        need(t, "t");
+        if (!node) {
+            t->e->set_format(nullptr);
+            return;
+        }
+        // an empty string may come with any pointer: only NULL means "not given"
+        const vbt::FormatProgram p = vbt::compile_format({node, node_len}, {unk, unk_len}, {bos, bos_len}, {eos, eos_len});
+        t->e->set_format(&p);
     });
 }
 

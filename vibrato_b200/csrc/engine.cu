@@ -323,6 +323,7 @@ class EngineImpl final : public Engine {
         cudaStreamDestroy(out_stream_);
         tok_base_.release();
         text_base_.release();
+        for (DevBuf* b : {&fmt_prog_, &ft_keep_, &ft_off_, &ft_bytes_}) b->release();
         for (auto* b : {&blob_own_, &in_utf8_, &in_off_, &connid_, &connid_try_}) b->release();
         for (auto& w : ws_) w.release();
         ws_small_.release();
@@ -371,6 +372,7 @@ class EngineImpl final : public Engine {
         } else if (name == "output_mode") {
             if (value < 0 || value > 3) throw Error(kInvalidArgument, "output_mode must be 0 (off), 1 mecab, 2 wakati or 3 detail");
             if (value != 0 && tok_bytes_ != 24) throw Error(kInvalidArgument, "compact_tokens and output_mode exclude each other");
+            clear_format();  // a fixed mode replaces an output format
             output_mode_ = uint32_t(value);
         } else if (name == "dual_stream") {
             dual_stream_ = value != 0;
@@ -398,6 +400,23 @@ class EngineImpl final : public Engine {
         } else {
             throw Error(kInvalidArgument, "unknown option: " + name);
         }
+    }
+    void set_format(const FormatProgram* p) override {
+        CK(cudaSetDevice(device_));
+        clear_format();
+        if (!p) return;
+        if (tok_bytes_ != 24) throw Error(kInvalidArgument, "compact_tokens and output formats exclude each other");
+        try {
+            fmt_prog_.ensure(sizeof(FormatProgram));
+            CK(cudaMemcpy(fmt_prog_.p, p, sizeof(FormatProgram), cudaMemcpyHostToDevice));
+            if (p->n_fields) build_field_table(*p);
+        } catch (...) {
+            clear_format();
+            throw;
+        }
+        output_mode_ = kOutFormat;
+        text_per_sent_ = p->per_sentence;
+        text_per_byte_[kOutFormat] = kFormatTextPerByte;  // learned anew for every format
     }
     void set_stream(uint64_t stream) override {
         cudaStreamSynchronize(stream_);
@@ -529,9 +548,9 @@ class EngineImpl final : public Engine {
             if (fmt) {
                 for (int i = 0; i < 2; ++i) {
                     ensure_format(out_[i], ws_[dual_stream_ ? i : 0], max_chunk_sent);
-                    out_[i].text.ensure(size_t(double(max_chunk_bytes) * text_ratio) + size_t(max_chunk_sent) * 4 + 4096);
+                    out_[i].text.ensure(size_t(double(max_chunk_bytes) * text_ratio) + size_t(max_chunk_sent) * text_per_sent_ + 4096);
                 }
-                ensure_text(r, n_sent, uint64_t(double(n_bytes) * text_ratio) + uint64_t(n_sent) * 4 + 1024);
+                ensure_text(r, n_sent, uint64_t(double(n_bytes) * text_ratio) + uint64_t(n_sent) * text_per_sent_ + 1024);
                 CK(cudaMemsetAsync(text_base_.p, 0, 8, stream_));
             }
             CK(cudaMemsetAsync(tok_base_.p, 0, 8, stream_));
@@ -544,7 +563,7 @@ class EngineImpl final : public Engine {
             std::memset(counters_, 0, sizeof(counters_));
             launches_ = 0;
             uint64_t tok_total = 0, text_total = 0;
-            double text_need = 0;  // text bytes per input byte beyond 4 per sentence, largest over the sound chunks
+            double text_need = 0;  // text bytes per input byte beyond text_per_sent_ per sentence, largest over the sound chunks
             uint32_t route = kRouteNone;
             bool overflow = false, bad_utf8 = false, bad_offsets = false, slots_overflow = false, text_overflow = false;
             uint64_t slots_seen = 0;
@@ -585,7 +604,7 @@ class EngineImpl final : public Engine {
                 pool_need_ = std::max<uint64_t>(pool_need_, o.h_ctrl->pool_ctr);
                 const uint64_t nt = o.h_ctrl->n_tokens, nx = fmt ? o.h_ctrl->text_bytes : 0;
                 if (fmt && !(o.h_ctrl->flags & (kFlagsStandDown | kFlagUtf8Error | kFlagPoolOverflow)))
-                    text_need = std::max(text_need, (double(nx) - 4.0 * (s1 - s0)) / double(std::max<uint64_t>(1, off[s1] - off[s0])));
+                    text_need = std::max(text_need, (double(nx) - double(text_per_sent_) * (s1 - s0)) / double(std::max<uint64_t>(1, off[s1] - off[s0])));
                 if (!overflow && !text_overflow && !bad_utf8 && !bad_offsets) {
                     if ((tok_total + nt) * tok_bytes_ > r->cap_tok) {  // rare: grow the pinned buffer, keep what is there
                         CK(cudaStreamSynchronize(out_stream_));
@@ -743,8 +762,11 @@ class EngineImpl final : public Engine {
     uint32_t token_bytes() const override { return tok_bytes_; }
     std::string describe() const override {
         static const char* const kRouteNames[] = {"none", "k_viterbi", "k_viterbi2", "k_viterbi2_unpruned", "k_small_batch"};
+        std::string ft;
+        if (output_mode_ == kOutFormat)  // the field table of the output format: device bytes and build time
+            ft = ", \"field_table\": {\"bytes\": " + std::to_string(ft_size_) + ", \"build_ms\": " + std::to_string(ft_ms_) + "}";
         return "{\"devices\": [" + std::to_string(device_) + "], \"dictionary_transport\": \"single device\", \"token_gather\": \"none\", " +
-               "\"last_viterbi\": \"" + kRouteNames[last_route_] + "\"}";
+               "\"last_viterbi\": \"" + kRouteNames[last_route_] + "\"" + ft + "}";
     }
 
    private:
@@ -862,7 +884,7 @@ class EngineImpl final : public Engine {
         Control* dc = o.ctrl.as<Control>();
         f.flags = &dc->flags;
         f.text_total = &dc->text_bytes;
-        f.mode = output_mode_;
+        set_mode(f);
         CK(cudaMemsetAsync(f.sent_len + n_sent, 0, 8, w.stream));
         launch_format_len(dv_, f, w.stream);
         exclusive_scan(w, f.sent_len, f.text_off, size_t(n_sent) + 1);
@@ -1010,11 +1032,11 @@ class EngineImpl final : public Engine {
         f.text_off = reinterpret_cast<unsigned long long*>(region + at_text_off);
         f.text = region + at_text;
         f.text_cap = small_out_cap_ - at_text;  // the device region and its pinned twin have (at least) this size
-        f.mode = output_mode_;
+        set_mode(f);
 
         // the first copy brings the text expected from the learned ratio; more comes in a second one
         const size_t text_guess = fmt ? std::min<size_t>(f.text_cap, size_t(double(n_bytes) * text_per_byte_[output_mode_]) +
-                                                                         size_t(n_sent) * 4 + 256)
+                                                                         size_t(n_sent) * text_per_sent_ + 256)
                                       : 0;
         OutSlot& o = out_[0];
         CK(cudaEventRecord(o.ev[0], stream_));
@@ -1051,6 +1073,85 @@ class EngineImpl final : public Engine {
         launches_ = 1;
         last_route_ = kRouteSmallBatch;
         return r;
+    }
+
+    // The output mode of the stage, with the program and field table of an output format.
+    void set_mode(FormatArgs& f) const {
+        f.mode = output_mode_;
+        f.prog = fmt_prog_.as<FormatProgram>();
+        f.ft_keep = ft_keep_.as<uint32_t>();
+        f.ft_off = ft_off_.as<uint32_t>();
+        f.ft_bytes = ft_bytes_.as<uint8_t>();
+    }
+
+    void clear_format() {
+        CK(cudaStreamSynchronize(stream_));
+        for (DevBuf* b : {&fmt_prog_, &ft_keep_, &ft_off_, &ft_bytes_}) b->release();
+        ft_size_ = 0;
+        ft_ms_ = 0;
+        text_per_sent_ = 4;
+        if (output_mode_ == kOutFormat) output_mode_ = kOutNone;
+    }
+
+    // The field table of format `p` (FormatArgs::ft_*): per word of the three lexicons, the unquoted text of every
+    // field p references, split on the device from the feature strings of the image (k_field_table_*).
+    void build_field_table(const FormatProgram& p) {
+        const uint64_t n_words = uint64_t(dv_.n_words[0]) + dv_.n_words[1] + dv_.n_words[2];
+        const uint64_t n_entries = n_words * p.n_fields;
+        uint64_t feat_bytes = 0;  // a field is part of its feature string: the table holds at most this many bytes
+        for (int li = 0; li < 3; ++li) {
+            uint32_t end = 0;
+            if (dv_.n_words[li]) CK(cudaMemcpy(&end, dv_.feat_off[li] + dv_.n_words[li], 4, cudaMemcpyDeviceToHost));
+            feat_bytes += end;
+        }
+        if (n_entries + 1 > 0xFFFFFFFFull || feat_bytes > 0xFFFFFFFFull)
+            throw Error(kUnsupported, "the field table of this format exceeds 2^32 entries or bytes: reference fewer fields");
+        FieldTableArgs a{};
+        std::memset(a.slot_of, 0xFF, sizeof a.slot_of);
+        for (uint32_t k = 0; k < p.n_fields; ++k) {
+            a.slot_of[p.fields[k]] = uint8_t(k);
+            a.fields[k] = p.fields[k];
+        }
+        a.n_fields = p.n_fields;
+        a.n_words = uint32_t(n_words);
+        DevBuf lens, tmp;
+        cudaEvent_t ev[2] = {nullptr, nullptr};
+        try {
+            for (auto& e : ev) CK(cudaEventCreate(&e));
+            CK(cudaEventRecord(ev[0], stream_));
+            lens.ensure((n_entries + 1) * 4);
+            ft_keep_.ensure(n_words * 4);
+            ft_off_.ensure((n_entries + 1) * 4);
+            a.lens = lens.as<uint32_t>();
+            a.keep = ft_keep_.as<uint32_t>();
+            launch_field_table_len(dv_, a, stream_);
+            CK(cudaMemsetAsync(a.lens + n_entries, 0, 4, stream_));
+            size_t tmp_bytes = 0;
+            CK(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, a.lens, ft_off_.as<uint32_t>(), n_entries + 1, stream_));
+            tmp.ensure(tmp_bytes);
+            CK(cub::DeviceScan::ExclusiveSum(tmp.p, tmp_bytes, a.lens, ft_off_.as<uint32_t>(), n_entries + 1, stream_));
+            uint32_t total = 0;
+            CK(cudaMemcpyAsync(&total, ft_off_.as<uint32_t>() + n_entries, 4, cudaMemcpyDeviceToHost, stream_));
+            CK(cudaStreamSynchronize(stream_));
+            ft_bytes_.ensure(size_t(total) + 16);
+            a.off = ft_off_.as<uint32_t>();
+            a.bytes = ft_bytes_.as<uint8_t>();
+            launch_field_table_write(dv_, a, stream_);
+            CK(cudaGetLastError());
+            CK(cudaEventRecord(ev[1], stream_));
+            CK(cudaEventSynchronize(ev[1]));
+            CK(cudaEventElapsedTime(&ft_ms_, ev[0], ev[1]));
+            ft_size_ = ft_keep_.cap + ft_off_.cap + ft_bytes_.cap;
+        } catch (...) {
+            lens.release();
+            tmp.release();
+            for (auto& e : ev)
+                if (e) cudaEventDestroy(e);
+            throw;
+        }
+        lens.release();
+        tmp.release();
+        for (auto& e : ev) cudaEventDestroy(e);
     }
 
     template <typename In, typename Out>
@@ -1305,9 +1406,15 @@ class EngineImpl final : public Engine {
     int order_mode_ = 0;  // K3's sentence order: 0 input order, 1 whole batch by length, 2 by length inside tiles
     uint32_t output_mode_ = 0;
     uint64_t batch_total_bytes_ = 0;  // size of the input buffer of the batch in flight (bounds check in K1a)
-    // output text bytes expected per input byte (beyond 4 per sentence), by output mode: sizes the text buffers of
-    // the chunked host pipeline, learned like cand_per_byte_
-    double text_per_byte_[4] = {0.0, 8.0, 2.0, 16.0};
+    // output text bytes expected per input byte (beyond text_per_sent_ per sentence), by output mode: sizes the text
+    // buffers of the chunked host pipeline, learned like cand_per_byte_
+    static constexpr double kFormatTextPerByte = 8.0;
+    double text_per_byte_[5] = {0.0, 8.0, 2.0, 16.0, kFormatTextPerByte};
+    uint32_t text_per_sent_ = 4;  // "EOS\n"; an output format: what its BOS and EOS print (FormatProgram::per_sentence)
+    // output format (set_format): the compiled program and its field table, with the table's size and build time
+    DevBuf fmt_prog_, ft_keep_, ft_off_, ft_bytes_;
+    size_t ft_size_ = 0;
+    float ft_ms_ = 0;
     bool dual_stream_ = false;
     int lanes_ = 16;  // fastest on H100 for ~40-character and 512-character sentences alike (DESIGN.md §4)
     uint32_t tok_bytes_ = 24;

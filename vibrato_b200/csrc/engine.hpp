@@ -6,6 +6,7 @@
 #include <string>
 #include <vector>
 
+#include "format.hpp"
 #include "host_dict.hpp"
 
 namespace vbt {
@@ -77,6 +78,9 @@ class Engine {
     // takes k_small_batch for batches of at most N sentences and 16 KiB without counting; run_device and the shards
     // of a multi-device engine keep the usual route).
     virtual void set_option(const std::string& name, long long value) = 0;
+    // An output format (format.hpp) in place of "output_mode" 1-3, on every host route; nullptr switches it off.
+    // Setting "output_mode" replaces it.  Builds the format's field table on the device.
+    virtual void set_format(const FormatProgram* p) = 0;
     // Launch on a caller-owned CUDA stream (0 restores the engine's own stream).
     virtual void set_stream(uint64_t stream) = 0;
     virtual const float* stage_ms() const = 0;

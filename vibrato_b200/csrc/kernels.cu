@@ -1308,42 +1308,336 @@ __device__ __forceinline__ uint32_t token_text_len(const DictView& d, const Toke
     return x.surf_len + 1 + x.feat_len + detail_tail_len(d, x) + 1;
 }
 
+// ---- kOutFormat: a format program (format.hpp) interpreted per token --------------------------------------------
+
+// Words of the three lexicons numbered in one range (system, user, unknown): the index of the field table.
+__device__ __forceinline__ uint32_t word_global(const DictView& d, uint32_t lex, uint32_t id) {
+    return (lex >= 1 ? d.n_words[0] : 0u) + (lex >= 2 ? d.n_words[1] : 0u) + id;
+}
+
+// What a format program may print of token t (prev = token t - 1 of the sentence, or BOS: end byte 0, cost 0).
+struct FmtTok {
+    TokenText x;
+    uint32_t end, prev_end;
+    int32_t prev_total, word_cost;
+    uint32_t ids;          // left | right << 16
+    uint32_t keep, entry;  // field table: the fields printed, and the word's first entry
+};
+
+__device__ __forceinline__ FmtTok fmt_tok(const DictView& d, const FormatArgs& f, const FormatProgram& P,
+                                          unsigned long long t, unsigned long long t0) {
+    const uint32_t uses = P.uses;
+    FmtTok v;
+    v.x = token_text(d, f.tokens, t);
+    v.end = v.x.start_byte + v.x.surf_len;
+    v.prev_end = 0;
+    v.prev_total = 0;
+    if ((uses & kUsesPrev) && t > t0) {
+        const uint2 pb = f.tokens[(t - 1) * 3 + 1], pc = f.tokens[(t - 1) * 3 + 2];
+        v.prev_end = pb.y;
+        v.prev_total = int32_t(pc.y);
+    }
+    const bool known = v.x.word_id < d.n_words[v.x.lex];
+    v.ids = 0;
+    v.word_cost = 0;
+    if ((uses & kUsesParams) && known) {
+        const uint2 pr = __ldg(d.params[v.x.lex] + v.x.word_id);
+        v.ids = pr.x;
+        v.word_cost = int32_t(int16_t(pr.y & 0xFFFFu));
+    }
+    v.keep = 0;
+    v.entry = 0;
+    if ((uses & kUsesFields) && known) {
+        const uint32_t wg = word_global(d, v.x.lex, v.x.word_id);
+        v.keep = __ldg(f.ft_keep + wg);
+        v.entry = wg * P.n_fields;
+    }
+    return v;
+}
+
+// The value of a numeric op (every op but literals, copies and fields).
+__device__ __forceinline__ long long fmt_number(uint32_t kind, const FmtTok& v, uint32_t sent_len) {
+    switch (kind) {
+        case kOpWordCost: return v.word_cost;
+        case kOpTotalCost: return v.x.total_cost;
+        case kOpCostDiff: return int32_t(uint32_t(v.x.total_cost) - uint32_t(v.prev_total));
+        case kOpConnCost: return int32_t(uint32_t(v.x.total_cost) - uint32_t(v.prev_total) - uint32_t(v.word_cost));
+        case kOpStart: return v.x.start_byte;
+        case kOpEnd: return v.end;
+        case kOpSurfLen: return v.x.surf_len;
+        case kOpSurfLenWs: return v.end - v.prev_end;
+        case kOpLeftId: return v.ids & 0xFFFFu;
+        case kOpRightId: return v.ids >> 16;
+        case kOpStat: return v.x.lex == 2 ? 1 : 0;
+        default: return sent_len;  // kOpSentLen
+    }
+}
+__device__ __forceinline__ uint32_t num_len(long long x) { return x < 0 ? 1 + dec_len(uint32_t(-x)) : dec_len(uint32_t(x)); }
+
+// Bytes the ops [a, b) of the program write for one token (or for BOS / EOS, with v unused).
+__device__ __forceinline__ unsigned long long fmt_len(const FormatProgram& P, uint32_t a, uint32_t b, const FormatArgs& f,
+                                                      const FmtTok& v, uint32_t sent_len) {
+    unsigned long long n = 0;
+    for (uint32_t i = a; i < b; ++i) {
+        const FormatOp o = P.ops[i];
+        switch (o.kind) {
+            case kOpLit: n += o.n; break;
+            case kOpSurface: n += v.x.surf_len; break;
+            case kOpSurfaceWs: n += v.end - v.prev_end; break;
+            case kOpWs: n += v.x.start_byte - v.prev_end; break;
+            case kOpFeature: n += v.x.feat_len; break;
+            case kOpSentence: n += sent_len; break;
+            case kOpFields: {
+                bool first = true;
+                for (uint32_t j = 0; j < o.n; ++j) {
+                    const uint32_t k = P.slot[o.at + j];
+                    if (!((v.keep >> k) & 1u)) continue;
+                    n += (first ? 0u : 1u) + __ldg(f.ft_off + v.entry + k + 1) - __ldg(f.ft_off + v.entry + k);
+                    first = false;
+                }
+                break;
+            }
+            default: n += num_len(fmt_number(o.kind, v, sent_len));
+        }
+    }
+    return n;
+}
+
 // The stage runs only on a batch whose tokens are sound: after an input error or an overflow the engine drops or
 // re-runs the batch anyway, and its token records may then point anywhere.
 __device__ __forceinline__ bool format_stands_down(const FormatArgs& f) {
     return *f.flags & (kFlagsStandDown | kFlagUtf8Error | kFlagPoolOverflow);
 }
 
-// Pass 1 for sentence s (a warp per sentence): lane 0 stores its text length in sent_len[s].
-__device__ __forceinline__ void format_len_one(const DictView& d, const FormatArgs& f, uint32_t s, uint32_t lane) {
-    const unsigned long long t0 = f.tok_off[s], t1 = f.tok_off[s + 1];
-    unsigned long long len = 0;
-    for (unsigned long long t = t0 + lane; t < t1; t += 32) len += token_text_len(d, token_text(d, f.tokens, t), f.mode, t == t0);
-    for (int k = 16; k > 0; k >>= 1) len += __shfl_xor_sync(kFull, len, k);
-    if (lane == 0) f.sent_len[s] = len + (f.mode == kOutWakati ? 1 : 4);  // "\n" or "EOS\n"
+// kOutFormat: every block stages the program in (dynamic) shared memory; all its threads call this.
+__device__ __forceinline__ const FormatProgram* stage_program(const FormatArgs& f, FormatProgram* s_prog) {
+    if (f.mode != kOutFormat) return nullptr;
+    const FormatProgram* g = f.prog;
+    const uint32_t n_ops = g->n_ops, n_slots = g->n_slots, n_lit = g->n_lit;
+    auto copy = [&](void* dst, const void* src, uint32_t bytes) {
+        for (uint32_t i = threadIdx.x; i < (bytes + 3) / 4; i += blockDim.x)
+            static_cast<uint32_t*>(dst)[i] = static_cast<const uint32_t*>(src)[i];
+    };
+    copy(s_prog, g, kFmtHeaderBytes);
+    copy(s_prog->ops, g->ops, n_ops * uint32_t(sizeof(FormatOp)));
+    copy(s_prog->slot, g->slot, n_slots);
+    copy(s_prog->lit, g->lit, n_lit);
+    __syncthreads();
+    return s_prog;
 }
 
+// Pass 1 for sentence s (a warp per sentence): lane 0 stores its text length in sent_len[s].  PROG: f.mode is
+// kOutFormat (a separate instantiation, so that the fixed modes keep their registers).
+template <bool PROG>
+__device__ __forceinline__ void format_len_one(const DictView& d, const FormatArgs& f, const FormatProgram* P, uint32_t s,
+                                               uint32_t lane) {
+    const unsigned long long t0 = f.tok_off[s], t1 = f.tok_off[s + 1];
+    unsigned long long len = 0;
+    if constexpr (PROG) {
+        const uint32_t sl = uint32_t(f.byte_off[s + 1] - f.byte_off[s]);
+        for (unsigned long long t = t0 + lane; t < t1; t += 32) {
+            const FmtTok v = fmt_tok(d, f, *P, t, t0);
+            const uint32_t sec = v.x.lex == 2 ? kSecUnk : kSecNode;
+            len += fmt_len(*P, P->sec[sec][0], P->sec[sec][1], f, v, sl);
+        }
+        for (int k = 16; k > 0; k >>= 1) len += __shfl_xor_sync(kFull, len, k);
+        if (lane == 0) {
+            FmtTok none{};
+            len += fmt_len(*P, P->sec[kSecBos][0], P->sec[kSecBos][1], f, none, sl);
+            f.sent_len[s] = len + fmt_len(*P, P->sec[kSecEos][0], P->sec[kSecEos][1], f, none, sl);
+        }
+    } else {
+        for (unsigned long long t = t0 + lane; t < t1; t += 32) len += token_text_len(d, token_text(d, f.tokens, t), f.mode, t == t0);
+        for (int k = 16; k > 0; k >>= 1) len += __shfl_xor_sync(kFull, len, k);
+        if (lane == 0) f.sent_len[s] = len + (f.mode == kOutWakati ? 1 : 4);  // "\n" or "EOS\n"
+    }
+}
+
+template <bool PROG>
 __global__ void __launch_bounds__(256) k_format_len(DictView d, FormatArgs f) {
+    extern __shared__ uint4 s_dyn[];
+    const FormatProgram* P = PROG ? stage_program(f, reinterpret_cast<FormatProgram*>(s_dyn)) : nullptr;
     const uint32_t s = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     if (s >= f.n_sent || format_stands_down(f)) return;
-    format_len_one(d, f, s, lane);
+    format_len_one<PROG>(d, f, P, s, lane);
 }
 
 __device__ __forceinline__ void warp_copy(uint8_t* __restrict__ dst, const uint8_t* __restrict__ src, uint32_t n, uint32_t lane) {
     for (uint32_t i = lane; i < n; i += 32) dst[i] = src[i];
 }
 
+// Writes the ops [a, b) at dst with the whole warp (every lane passes the same arguments); returns the end.
+__device__ __forceinline__ uint8_t* fmt_write(const DictView& d, const FormatProgram& P, uint32_t a, uint32_t b,
+                                              const FormatArgs& f, const FmtTok& v, const uint8_t* __restrict__ sent,
+                                              uint32_t sent_len, uint8_t* dst, uint32_t lane) {
+    for (uint32_t i = a; i < b; ++i) {
+        const FormatOp o = P.ops[i];
+        switch (o.kind) {
+            case kOpLit:
+                warp_copy(dst, P.lit + o.at, o.n, lane);
+                dst += o.n;
+                break;
+            case kOpSurface:
+                warp_copy(dst, sent + v.x.start_byte, v.x.surf_len, lane);
+                dst += v.x.surf_len;
+                break;
+            case kOpSurfaceWs:
+                warp_copy(dst, sent + v.prev_end, v.end - v.prev_end, lane);
+                dst += v.end - v.prev_end;
+                break;
+            case kOpWs:
+                warp_copy(dst, sent + v.prev_end, v.x.start_byte - v.prev_end, lane);
+                dst += v.x.start_byte - v.prev_end;
+                break;
+            case kOpFeature:
+                if (v.x.feat_len) warp_copy(dst, d.feat[v.x.lex] + v.x.feat_at, v.x.feat_len, lane);
+                dst += v.x.feat_len;
+                break;
+            case kOpSentence:
+                warp_copy(dst, sent, sent_len, lane);
+                dst += sent_len;
+                break;
+            case kOpFields: {
+                bool first = true;
+                for (uint32_t j = 0; j < o.n; ++j) {
+                    const uint32_t k = P.slot[o.at + j];
+                    if (!((v.keep >> k) & 1u)) continue;
+                    if (!first) {
+                        if (lane == 0) *dst = o.sep;
+                        ++dst;
+                    }
+                    const uint32_t at = __ldg(f.ft_off + v.entry + k), n = __ldg(f.ft_off + v.entry + k + 1) - at;
+                    warp_copy(dst, f.ft_bytes + at, n, lane);
+                    dst += n;
+                    first = false;
+                }
+                break;
+            }
+            default: {
+                const long long x = fmt_number(o.kind, v, sent_len);
+                if (lane == 0) {
+                    if (x < 0) {
+                        *dst = '-';
+                        put_dec(dst + 1, uint32_t(-x));
+                    } else {
+                        put_dec(dst, uint32_t(x));
+                    }
+                }
+                dst += num_len(x);
+            }
+        }
+    }
+    return dst;
+}
+
+// The unquoted text of the fields of a feature string, split as the evaluate tool's parse_csv_row splits it
+// (csv-core: a field that begins with '"' is quoted, "" inside it stands for '"', a ',' outside quotes ends the
+// field): out(field, byte) for every byte of field text.  Returns the number of fields.
+template <class Out>
+__device__ __forceinline__ uint32_t csv_fields(const uint8_t* __restrict__ p, uint32_t n, Out out) {
+    uint32_t field = 0;
+    bool quoted = false, at_start = true;
+    for (uint32_t i = 0; i < n; ++i) {
+        const uint8_t c = p[i];
+        if (quoted) {
+            if (c != '"') {
+                out(field, c);
+            } else if (i + 1 < n && p[i + 1] == '"') {
+                out(field, c);
+                ++i;
+            } else {
+                quoted = false;
+            }
+        } else if (c == '"' && at_start) {
+            quoted = true;
+        } else if (c == ',') {
+            ++field;
+            at_start = true;
+            continue;
+        } else {
+            out(field, c);
+        }
+        at_start = false;
+    }
+    return field + 1;
+}
+
+__device__ __forceinline__ void word_feature(const DictView& d, uint32_t wg, const uint8_t*& p, uint32_t& n) {
+    uint32_t lex = 0;
+    while (lex < 2 && wg >= d.n_words[lex]) wg -= d.n_words[lex++];
+    const uint32_t a = d.feat_off[lex][wg];
+    p = d.feat[lex] + a;
+    n = d.feat_off[lex][wg + 1] - a;
+}
+
+// Field table, pass 1: a thread per word stores which referenced fields it prints and their lengths.
+__global__ void __launch_bounds__(256) k_field_table_len(DictView d, FieldTableArgs a) {
+    const uint32_t wg = blockIdx.x * blockDim.x + threadIdx.x;
+    if (wg >= a.n_words) return;
+    const uint8_t* p;
+    uint32_t n;
+    word_feature(d, wg, p, n);
+    uint32_t len[kFmtMaxFields];
+    for (uint32_t k = 0; k < kFmtMaxFields; ++k) len[k] = 0;
+    uint32_t seen = 0, star = 0;
+    const uint32_t nf = csv_fields(p, n, [&](uint32_t field, uint8_t c) {
+        const uint32_t k = field <= kFmtMaxFieldIndex ? a.slot_of[field] : 0xFFu;
+        if (k == 0xFFu) return;
+        if (!((seen >> k) & 1u)) {
+            seen |= 1u << k;
+            if (c == '*') star |= 1u << k;
+        }
+        ++len[k];
+    });
+    uint32_t keep = 0;
+    for (uint32_t k = 0; k < a.n_fields; ++k) {
+        const bool kept = a.fields[k] < nf && !((star >> k) & 1u);  // a field past the last one counts as '*'
+        keep |= uint32_t(kept) << k;
+        a.lens[size_t(wg) * a.n_fields + k] = kept ? len[k] : 0u;
+    }
+    a.keep[wg] = keep;
+}
+
+// Field table, pass 2: the same split writes the printed fields at their offsets.
+__global__ void __launch_bounds__(256) k_field_table_write(DictView d, FieldTableArgs a) {
+    const uint32_t wg = blockIdx.x * blockDim.x + threadIdx.x;
+    if (wg >= a.n_words) return;
+    const uint32_t keep = a.keep[wg];
+    if (!keep) return;
+    const uint8_t* p;
+    uint32_t n;
+    word_feature(d, wg, p, n);
+    uint32_t at[kFmtMaxFields];
+    for (uint32_t k = 0; k < a.n_fields; ++k) at[k] = a.off[size_t(wg) * a.n_fields + k];
+    csv_fields(p, n, [&](uint32_t field, uint8_t c) {
+        const uint32_t k = field <= kFmtMaxFieldIndex ? a.slot_of[field] : 0xFFu;
+        if (k != 0xFFu && ((keep >> k) & 1u)) a.bytes[at[k]++] = c;
+    });
+}
+
 // Pass 2 for sentence s (a warp per sentence): its text at text_off[s], which must fit in text_cap.
-__device__ __forceinline__ void format_write_one(const DictView& d, const FormatArgs& f, uint32_t s, uint32_t lane) {
+template <bool PROG>
+__device__ __forceinline__ void format_write_one(const DictView& d, const FormatArgs& f, const FormatProgram* P, uint32_t s,
+                                                 uint32_t lane) {
     const unsigned long long t0 = f.tok_off[s], t1 = f.tok_off[s + 1];
     const uint8_t* __restrict__ sent = f.utf8 + f.byte_off[s];
     unsigned long long base = f.text_off[s];  // where the next group of 32 tokens starts
+    const bool prog = PROG;
+    const uint32_t sl = prog ? uint32_t(f.byte_off[s + 1] - f.byte_off[s]) : 0u;
+    if (prog) {
+        const FmtTok none{};
+        base = fmt_write(d, *P, P->sec[kSecBos][0], P->sec[kSecBos][1], f, none, sent, sl, f.text + base, lane) - f.text;
+    }
     for (unsigned long long c = t0; c < t1; c += 32) {
         // lane i stages token c + i; the copies below take one token at a time with all 32 lanes
         const uint32_t cnt = uint32_t(min(32ull, t1 - c));
         TokenText mine = {0, 0, 0, 0, 0, 0, 0};
-        uint32_t len = 0;
-        if (lane < cnt) {
+        unsigned long long len = 0;
+        if (lane < cnt && prog) {
+            const FmtTok v = fmt_tok(d, f, *P, c + lane, t0);
+            const uint32_t sec = v.x.lex == 2 ? kSecUnk : kSecNode;
+            len = fmt_len(*P, P->sec[sec][0], P->sec[sec][1], f, v, sl);
+        } else if (lane < cnt) {
             mine = token_text(d, f.tokens, c + lane);
             len = token_text_len(d, mine, f.mode, c + lane == t0);
         }
@@ -1355,6 +1649,12 @@ __device__ __forceinline__ void format_write_one(const DictView& d, const Format
         const unsigned long long at = base + incl - len;
         base += __shfl_sync(kFull, incl, 31);
         for (uint32_t j = 0; j < cnt; ++j) {
+            if (prog) {  // every lane loads token c + j again: one broadcast load per record
+                const FmtTok v = fmt_tok(d, f, *P, c + j, t0);
+                const uint32_t sec = v.x.lex == 2 ? kSecUnk : kSecNode;
+                fmt_write(d, *P, P->sec[sec][0], P->sec[sec][1], f, v, sent, sl, f.text + __shfl_sync(kFull, at, j), lane);
+                continue;
+            }
             TokenText x;
             x.start_byte = __shfl_sync(kFull, mine.start_byte, j);
             x.surf_len = __shfl_sync(kFull, mine.surf_len, j);
@@ -1396,14 +1696,20 @@ __device__ __forceinline__ void format_write_one(const DictView& d, const Format
             }
         }
     }
-    if (lane == 0) {
+    if (prog) {
+        const FmtTok none{};
+        fmt_write(d, *P, P->sec[kSecEos][0], P->sec[kSecEos][1], f, none, sent, sl, f.text + base, lane);
+    } else if (lane == 0) {
         uint8_t* dst = f.text + base;
         if (f.mode != kOutWakati) dst = put_str(dst, "EOS");
         *dst = '\n';
     }
 }
 
+template <bool PROG>
 __global__ void __launch_bounds__(256) k_format_write(DictView d, FormatArgs f) {
+    extern __shared__ uint4 s_dyn[];
+    const FormatProgram* P = PROG ? stage_program(f, reinterpret_cast<FormatProgram*>(s_dyn)) : nullptr;
     const uint32_t s = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     if (s >= f.n_sent || format_stands_down(f)) return;
     const unsigned long long total = f.text_off[f.n_sent];
@@ -1412,7 +1718,7 @@ __global__ void __launch_bounds__(256) k_format_write(DictView d, FormatArgs f) 
         if (total > f.text_cap) atomicOr(f.flags, kFlagTextOverflow);
     }
     if (total > f.text_cap) return;  // every warp sees the same total: nothing is written
-    format_write_one(d, f, s, lane);
+    format_write_one<PROG>(d, f, P, s, lane);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1473,6 +1779,7 @@ template <int CONN>
 __global__ void __launch_bounds__(kSmallThreads, 1) k_small_batch(DictView d, Batch b, FormatArgs f, SmallBatchOut* out) {
     __shared__ uint32_t s_flags;
     __shared__ unsigned long long s_warp[32];
+    extern __shared__ uint4 s_dyn[];
     const uint32_t tid = threadIdx.x, lane = tid & 31, wid = tid >> 5, nw = blockDim.x >> 5;
     const uint32_t n = b.n_sent;
     if (tid == 0) s_flags = 0;
@@ -1530,7 +1837,13 @@ __global__ void __launch_bounds__(kSmallThreads, 1) k_small_batch(DictView d, Ba
         for (uint32_t s = wid; s < n; s += nw) backtrack_write_one(b, s, lane);  // K4b
         if (f.mode != kOutNone) {  // output stage
             __syncthreads();
-            for (uint32_t s = wid; s < n; s += nw) format_len_one(d, f, s, lane);
+            const FormatProgram* P = stage_program(f, reinterpret_cast<FormatProgram*>(s_dyn));
+            for (uint32_t s = wid; s < n; s += nw) {
+                if (P)
+                    format_len_one<true>(d, f, P, s, lane);
+                else
+                    format_len_one<false>(d, f, P, s, lane);
+            }
             __syncthreads();
             text_bytes = block_scan(
                 n, [&](uint32_t i) { return f.sent_len[i]; }, [&](uint32_t i, unsigned long long v) { f.text_off[i] = v; },
@@ -1538,7 +1851,12 @@ __global__ void __launch_bounds__(kSmallThreads, 1) k_small_batch(DictView d, Ba
             if (text_bytes > f.text_cap) {
                 if (tid == 0) atomicOr(&s_flags, kFlagTextOverflow);
             } else {
-                for (uint32_t s = wid; s < n; s += nw) format_write_one(d, f, s, lane);
+                for (uint32_t s = wid; s < n; s += nw) {
+                    if (P)
+                        format_write_one<true>(d, f, P, s, lane);
+                    else
+                        format_write_one<false>(d, f, P, s, lane);
+                }
             }
         }
     }
@@ -1554,22 +1872,37 @@ __global__ void __launch_bounds__(kSmallThreads, 1) k_small_batch(DictView d, Ba
 }  // namespace
 
 void launch_small_batch(const DictView& d, const Batch& b, const FormatArgs& f, SmallBatchOut* out, cudaStream_t st) {
+    const size_t smem = f.mode == kOutFormat ? sizeof(FormatProgram) : 0;
     if (d.connector_kind == 1)
-        k_small_batch<1><<<1, kSmallThreads, 0, st>>>(d, b, f, out);
+        k_small_batch<1><<<1, kSmallThreads, smem, st>>>(d, b, f, out);
     else if (d.connector_kind == 2)
-        k_small_batch<2><<<1, kSmallThreads, 0, st>>>(d, b, f, out);
+        k_small_batch<2><<<1, kSmallThreads, smem, st>>>(d, b, f, out);
     else
-        k_small_batch<0><<<1, kSmallThreads, 0, st>>>(d, b, f, out);
+        k_small_batch<0><<<1, kSmallThreads, smem, st>>>(d, b, f, out);
 }
 
 void launch_format_len(const DictView& d, const FormatArgs& f, cudaStream_t st) {
     if (!f.n_sent) return;
-    k_format_len<<<(f.n_sent + 7) / 8, 256, 0, st>>>(d, f);
+    if (f.mode == kOutFormat)
+        k_format_len<true><<<(f.n_sent + 7) / 8, 256, sizeof(FormatProgram), st>>>(d, f);
+    else
+        k_format_len<false><<<(f.n_sent + 7) / 8, 256, 0, st>>>(d, f);
 }
 
 void launch_format_write(const DictView& d, const FormatArgs& f, cudaStream_t st) {
     if (!f.n_sent) return;
-    k_format_write<<<(f.n_sent + 7) / 8, 256, 0, st>>>(d, f);
+    if (f.mode == kOutFormat)
+        k_format_write<true><<<(f.n_sent + 7) / 8, 256, sizeof(FormatProgram), st>>>(d, f);
+    else
+        k_format_write<false><<<(f.n_sent + 7) / 8, 256, 0, st>>>(d, f);
+}
+
+void launch_field_table_len(const DictView& d, const FieldTableArgs& a, cudaStream_t st) {
+    if (a.n_words) k_field_table_len<<<(a.n_words + 255) / 256, 256, 0, st>>>(d, a);
+}
+
+void launch_field_table_write(const DictView& d, const FieldTableArgs& a, cudaStream_t st) {
+    if (a.n_words) k_field_table_write<<<(a.n_words + 255) / 256, 256, 0, st>>>(d, a);
 }
 
 void launch_count_chars(const Batch& b, cudaStream_t st) {

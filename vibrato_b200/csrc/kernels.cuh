@@ -8,6 +8,8 @@
 #include <cstdint>
 #include <cuda_runtime.h>
 
+#include "format.hpp"
+
 namespace vbt {
 
 struct DictView {
@@ -121,8 +123,9 @@ struct Batch {
     unsigned long long* rid_count;
 };
 
-// Output stage: what `tokenize` prints per sentence (tokenize/src/main.rs:83-127), produced on the device.
-enum : uint32_t { kOutNone = 0, kOutMecab = 1, kOutWakati = 2, kOutDetail = 3 };
+// Output stage: what `tokenize` prints per sentence (tokenize/src/main.rs:83-127), produced on the device;
+// kOutFormat: a MeCab-style format program (format.hpp).
+enum : uint32_t { kOutNone = 0, kOutMecab = 1, kOutWakati = 2, kOutDetail = 3, kOutFormat = 4 };
 struct FormatArgs {
     const uint8_t* utf8;
     const unsigned long long* byte_off;  // n_sent + 1
@@ -136,9 +139,29 @@ struct FormatArgs {
     uint32_t* flags;                     // the batch's flags: the stage stands down after an input error or overflow
     unsigned long long* text_total;      // receives text_off[n_sent] (also when it does not fit)
     uint32_t mode;
+    // kOutFormat: the compiled program (device memory; every block stages it in shared memory) and the field table
+    // of the fields it references.  Words are numbered system, user, unknown in turn (word_global).
+    const FormatProgram* prog;
+    const uint32_t* ft_keep;  // per word: bit k set = field prog->fields[k] is printed (present, not '*')
+    const uint32_t* ft_off;   // per word and k (n_fields per word), + 1: where the field's unquoted text starts
+    const uint8_t* ft_bytes;
 };
 void launch_format_len(const DictView& d, const FormatArgs& f, cudaStream_t st);
 void launch_format_write(const DictView& d, const FormatArgs& f, cudaStream_t st);
+
+// Field table of a format program, built once per format and device from the feature strings of the image.
+struct FieldTableArgs {
+    uint8_t slot_of[kFmtMaxFieldIndex + 1];  // field index -> position k in fields[], 0xFF when not referenced
+    uint8_t fields[kFmtMaxFields];
+    uint32_t n_fields;
+    uint32_t n_words;  // all three lexicons
+    uint32_t* lens;    // n_words * n_fields + 1: bytes of each printed field (pass 1)
+    uint32_t* keep;    // n_words
+    const uint32_t* off;  // exclusive scan of lens (pass 2)
+    uint8_t* bytes;
+};
+void launch_field_table_len(const DictView& d, const FieldTableArgs& a, cudaStream_t st);
+void launch_field_table_write(const DictView& d, const FieldTableArgs& a, cudaStream_t st);
 
 void launch_count_chars(const Batch& b, cudaStream_t st);
 void launch_decode(const DictView& d, const Batch& b, cudaStream_t st);

@@ -348,7 +348,18 @@ class MultiEngine final : public Engine {
     void set_option(const std::string& name, long long value) override {
         if (name == "chunk_sentences") return;  // shards are not chunked (see the constructor)
         for (auto& e : eng_) e->set_option(name, value);
-        if (name == "output_mode") text_ = value != 0;
+        if (name == "output_mode") text_ = fixed_mode_ = value != 0;
+    }
+    void set_format(const FormatProgram* p) override {
+        try {
+            for (auto& e : eng_) e->set_format(p);  // each device builds its own field table
+        } catch (...) {
+            for (auto& e : eng_) e->set_format(nullptr);
+            text_ = fixed_mode_;
+            throw;
+        }
+        if (p) fixed_mode_ = false;  // the format replaced it
+        text_ = p != nullptr || fixed_mode_;
     }
     void set_stream(uint64_t stream) override {
         if (stream) throw Error(kUnsupported, "a multi-device tokenizer runs on its own streams");
@@ -494,7 +505,8 @@ class MultiEngine final : public Engine {
     std::vector<std::unique_ptr<Engine>> eng_;
     std::string transport_;
     std::vector<HostResult*> pool_, free_;
-    bool text_ = false;  // "output_mode" is on: host results carry the formatted text
+    bool text_ = false;  // "output_mode" or an output format is on: host results carry the formatted text
+    bool fixed_mode_ = false;  // "output_mode" 1-3 is on
     uint64_t* h_off_ = nullptr;  // pinned
     size_t h_off_cap_ = 0;
     void* gather_tokens_ = nullptr;
