@@ -209,6 +209,28 @@ void vbt_tokenizer_free(vbt_tokenizer *t);
  * An empty sentence yields zero tokens (worker.rs:50-52). */
 int32_t vbt_tokenize_batch(vbt_tokenizer *t, const char *utf8, const uint64_t *byte_offsets, uint64_t n_sent,
                            vbt_result **out);
+/* As vbt_tokenize_batch, with required token boundaries (no reference counterpart; MeCab's partial analysis, -p,
+ * answers the same need).  Sentence i's required boundaries are bnd[bnd_offsets[i] .. bnd_offsets[i+1]): byte offsets
+ * into the sentence, sentence-relative like vbt_token.start_byte.
+ * Guarantee: no token t of sentence i has t.start_byte < b < t.end_byte for any of its boundaries b.  Apart from that
+ * the result is the minimum-cost path of the constrained lattice, chosen and tie-broken as vbt_tokenize_batch does.
+ * Definition, in character positions: for a start position sw let lim(sw) be the first boundary after sw (or the
+ * sentence's length).  (1) A lexicon word (system or user) that ends after lim(sw) is no candidate and does not
+ * count as a match for the unknown-word rule; (2) in gen_unk_words (dictionary/unknown.rs:69-116) the groupable
+ * length g becomes min(g, lim(sw) - sw) everywhere, so a boundary ends a character group; (3) the space skip of
+ * ignore_space is unchanged: a boundary inside a skipped run of spaces holds trivially; (4) nothing else changes, so
+ * the one-character unknown word keeps a path wherever unk.def has entries for the category.  A sentence without
+ * boundaries, or with only 0 and its length, gives exactly the tokens of vbt_tokenize_batch, and a batch whose lists
+ * are all empty runs the kernels of vbt_tokenize_batch.
+ * Input rules: each list is non-decreasing (duplicates count once), every value is <= the sentence's byte length and
+ * a value below it sits on a UTF-8 lead byte; bnd_offsets is non-decreasing.  Anything else fails the call with
+ * VBT_ERR_INVALID_ARGUMENT; the errors of vbt_tokenize_batch (VBT_ERR_UTF8, bad byte_offsets) take precedence.
+ * Works on single- and multi-device tokenizers, on every host route ("chunk_sentences", "small_batch") and with
+ * "compact_tokens", "output_mode", output formats and "connid_counting" (which then counts the constrained
+ * lattices).  With the measurement hook "counting" on the call fails with VBT_ERR_INVALID_ARGUMENT: its counters
+ * describe the unconstrained walk. */
+int32_t vbt_tokenize_batch_bounded(vbt_tokenizer *t, const char *utf8, const uint64_t *byte_offsets, uint64_t n_sent,
+                                   const uint64_t *bnd_offsets, const uint32_t *bnd, vbt_result **out);
 /* Worker::num_tokens / token(i) / token_iter (worker.rs:59-74) for the whole batch:
  * tokens of sentence i are toks[tok_offsets[i] .. tok_offsets[i+1]), in sentence order. */
 int32_t vbt_result_view(const vbt_result *r, const uint64_t **tok_offsets, const vbt_token **toks,
@@ -239,6 +261,12 @@ void vbt_result_free(vbt_result *r);
 int32_t vbt_tokenize_batch_device(vbt_tokenizer *t, uint64_t d_utf8, uint64_t d_byte_offsets, uint64_t n_sent,
                                   uint64_t n_bytes, uint64_t *d_tok_offsets, uint64_t *d_tokens,
                                   uint64_t *n_tokens);
+/* As vbt_tokenize_batch_device with the required boundaries of vbt_tokenize_batch_bounded; d_bnd_offsets
+ * (uint64[n_sent+1]) and d_bnd (uint32[n_bnd]) are DEVICE addresses, and every offset must be <= n_bnd.  A
+ * multi-device tokenizer copies the two arrays to the host to cut them into shards. */
+int32_t vbt_tokenize_batch_device_bounded(vbt_tokenizer *t, uint64_t d_utf8, uint64_t d_byte_offsets, uint64_t n_sent,
+                                          uint64_t n_bytes, uint64_t d_bnd_offsets, uint64_t d_bnd, uint64_t n_bnd,
+                                          uint64_t *d_tok_offsets, uint64_t *d_tokens, uint64_t *n_tokens);
 
 /* Pinned host memory for callers that want full-speed host<->device copies. */
 int32_t vbt_host_alloc(size_t n_bytes, void **out);

@@ -96,6 +96,9 @@ def lib():
     sig("vbt_evaluate", i32, [vp, vp, vp, sz, vp, sz, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64)])
     sig("vbt_result_free", None, [vp])
     sig("vbt_tokenize_batch_device", i32, [vp, u64, u64, u64, u64, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64)])
+    sig("vbt_tokenize_batch_bounded", i32, [vp, vp, vp, u64, vp, vp, pp])
+    sig("vbt_tokenize_batch_device_bounded", i32,
+        [vp, u64, u64, u64, u64, u64, u64, u64, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64)])
     sig("vbt_host_alloc", i32, [sz, pp])
     sig("vbt_host_free", None, [vp])
     sig("vbt_tokenizer_set_counting", i32, [vp, i32])

@@ -421,23 +421,52 @@ class Tokenizer:
             off[1:] = np.cumsum([len(b) for b in blobs], dtype=np.uint64)
         return np.frombuffer(b"".join(blobs), dtype=np.uint8), off
 
-    def tokenize_batch(self, sentences=None, utf8=None, byte_offsets=None):
-        """reset_sentence + tokenize for every sentence of the batch on the GPU (host in, host out)."""
+    @staticmethod
+    def pack_bounds(boundaries):
+        """list[list[int]] (per-sentence byte offsets) -> (bnd_offsets uint64[n+1], bnd uint32[])"""
+        off = np.zeros(len(boundaries) + 1, dtype=np.uint64)
+        if boundaries:
+            off[1:] = np.cumsum([len(b) for b in boundaries], dtype=np.uint64)
+        flat = [v for b in boundaries for v in b]
+        return off, np.array(flat, dtype=np.uint32)
+
+    def tokenize_batch(self, sentences=None, utf8=None, byte_offsets=None, boundaries=None, bnd_offsets=None, bnd=None):
+        """reset_sentence + tokenize for every sentence of the batch on the GPU (host in, host out).
+
+        Required boundaries (vbt_tokenize_batch_bounded): `boundaries` = one list of sentence-relative byte offsets
+        per sentence, or the packed form bnd_offsets (uint64[n+1]) / bnd (uint32[]).  No token of a sentence crosses
+        one of its boundaries; the library validates them."""
         if sentences is not None:
             utf8, byte_offsets = self.pack(sentences)
+        if boundaries is not None:
+            bnd_offsets, bnd = self.pack_bounds(boundaries)
         utf8 = np.ascontiguousarray(utf8, dtype=np.uint8)
         byte_offsets = np.ascontiguousarray(byte_offsets, dtype=np.uint64)
         n = len(byte_offsets) - 1
         h = C.c_void_p()
-        check(lib().vbt_tokenize_batch(self.handle(), utf8.ctypes.data if utf8.size else None,
-                                       byte_offsets.ctypes.data, n, C.byref(h)))
+        if bnd_offsets is None:
+            check(lib().vbt_tokenize_batch(self.handle(), utf8.ctypes.data if utf8.size else None,
+                                           byte_offsets.ctypes.data, n, C.byref(h)))
+        else:
+            bnd_offsets = np.ascontiguousarray(bnd_offsets, dtype=np.uint64)
+            bnd = np.ascontiguousarray(bnd if bnd is not None else [], dtype=np.uint32)
+            check(lib().vbt_tokenize_batch_bounded(self.handle(), utf8.ctypes.data if utf8.size else None,
+                                                   byte_offsets.ctypes.data, n, bnd_offsets.ctypes.data,
+                                                   bnd.ctypes.data if bnd.size else None, C.byref(h)))
         return BatchResult(self, h, utf8, byte_offsets, compact=bool(self._options.get("compact_tokens", 0)))
 
-    def tokenize_batch_device(self, d_utf8, d_byte_offsets, n_sent, n_bytes):
-        """Device-resident variant: addresses in, (d_tok_offsets, d_tokens, n_tokens) out."""
+    def tokenize_batch_device(self, d_utf8, d_byte_offsets, n_sent, n_bytes, d_bnd_offsets=None, d_bnd=None, n_bnd=0):
+        """Device-resident variant: addresses in, (d_tok_offsets, d_tokens, n_tokens) out.  With d_bnd_offsets
+        (uint64[n_sent+1]) and d_bnd (uint32[n_bnd]), also device addresses: required boundaries as in
+        tokenize_batch."""
         a, b, n = C.c_uint64(), C.c_uint64(), C.c_uint64()
-        check(lib().vbt_tokenize_batch_device(self.handle(), int(d_utf8), int(d_byte_offsets), int(n_sent),
-                                              int(n_bytes), C.byref(a), C.byref(b), C.byref(n)))
+        if d_bnd_offsets is None:
+            check(lib().vbt_tokenize_batch_device(self.handle(), int(d_utf8), int(d_byte_offsets), int(n_sent),
+                                                  int(n_bytes), C.byref(a), C.byref(b), C.byref(n)))
+        else:
+            check(lib().vbt_tokenize_batch_device_bounded(self.handle(), int(d_utf8), int(d_byte_offsets), int(n_sent),
+                                                          int(n_bytes), int(d_bnd_offsets), int(d_bnd or 0),
+                                                          int(n_bnd), C.byref(a), C.byref(b), C.byref(n)))
         return a.value, b.value, n.value
 
     # connection-id statistics (worker.rs:77-103) ---------------------------------------------------
@@ -616,16 +645,19 @@ class Worker:
     def __init__(self, tokenizer):
         self._tok = tokenizer
         self._sent = b""
+        self._bounds = None
         self._tokens = []
 
-    def reset_sentence(self, text):
+    def reset_sentence(self, text, boundaries=None):
+        """boundaries: required token boundaries, byte offsets into the sentence (see Tokenizer.tokenize_batch)."""
         self._sent = text.encode("utf-8") if isinstance(text, str) else bytes(text)
+        self._bounds = None if boundaries is None else list(boundaries)
         self._tokens = []
 
     def tokenize(self):
         if not self._sent:  # worker.rs:50-52
             return
-        res = self._tok.tokenize_batch([self._sent])
+        res = self._tok.tokenize_batch([self._sent], boundaries=None if self._bounds is None else [self._bounds])
         self._tokens = [Token(self._tok, self._sent, r.copy()) for r in res.tokens]
         res.close()
 

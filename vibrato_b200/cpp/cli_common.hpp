@@ -56,17 +56,43 @@ inline std::vector<int32_t> parse_devices(const std::string& list) {
     return devices;
 }
 
+// tokenize --boundary-marker C: removes every occurrence of the ASCII byte `marker` from `line` and returns the byte
+// offsets, in the line without markers, where they stood: required token boundaries.  Adjacent markers give one
+// boundary; markers at either end give 0 / the length, which constrain nothing.
+inline std::vector<uint32_t> strip_boundary_markers(std::string& line, char marker) {
+    std::vector<uint32_t> bnd;
+    size_t w = 0;
+    for (size_t r = 0; r < line.size(); ++r) {
+        if (line[r] == marker) {
+            if (bnd.empty() || bnd.back() != w) bnd.push_back(uint32_t(w));
+        } else {
+            line[w++] = line[r];
+        }
+    }
+    line.resize(w);
+    return bnd;
+}
+
 struct Packed {
     std::string utf8;
     std::vector<uint64_t> off{0};
+    std::vector<uint64_t> bnd_off{0};  // required boundaries per line (--boundary-marker), bnd_off / bnd as CSR
+    std::vector<uint32_t> bnd;
     void add(const std::string& s) {
         utf8 += s;
         off.push_back(utf8.size());
+        bnd_off.push_back(bnd.size());
+    }
+    void add(const std::string& s, const std::vector<uint32_t>& b) {
+        bnd.insert(bnd.end(), b.begin(), b.end());
+        add(s);
     }
     uint64_t size() const { return off.size() - 1; }
     void clear() {
         utf8.clear();
         off.assign(1, 0);
+        bnd_off.assign(1, 0);
+        bnd.clear();
     }
 };
 

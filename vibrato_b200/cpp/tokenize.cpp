@@ -17,7 +17,9 @@ static void usage() {
                  "                                      unk defaults to the node format, bos to \"\", eos to \"EOS\\n\")\n"
                  "         [--format-on device|host]   (where the output text is built; default device; -F needs device)\n"
                  "         [--devices 0,1,..]          (spread every batch over these GPUs)\n"
-                 "         [--batch-lines N]           (lines per batch when stdin is not a terminal; default 65536)\n");
+                 "         [--batch-lines N]           (lines per batch when stdin is not a terminal; default 65536)\n"
+                 "         [--boundary-marker C]       (an ASCII byte other than newline: removed from every line, it\n"
+                 "                                      marks a required token boundary where it stood)\n");
 }
 
 int main(int argc, char** argv) {
@@ -27,6 +29,7 @@ int main(int argc, char** argv) {
     std::vector<int32_t> devices;
     std::string node_format, unk_format, bos_format, eos_format;
     bool has_node = false, has_unk = false, has_bos = false, has_eos = false;
+    std::string marker;
     for (int i = 1; i < argc; ++i) {
         std::string a = argv[i];
         auto next = [&]() -> std::string {
@@ -48,13 +51,16 @@ int main(int argc, char** argv) {
         else if (a == "--unk-format") unk_format = next(), has_unk = true;
         else if (a == "--bos-format") bos_format = next(), has_bos = true;
         else if (a == "--eos-format") eos_format = next(), has_eos = true;
+        else if (a == "--boundary-marker") marker = next();
         else {
             usage();
             return 2;
         }
     }
     // the formats are rendered by the device only; --unk/bos/eos-format complete -F
-    if (batch_lines_arg == 0 || (has_node && format_on == "host") || (!has_node && (has_unk || has_bos || has_eos))) {
+    const bool bounded = !marker.empty();
+    if (batch_lines_arg == 0 || (has_node && format_on == "host") || (!has_node && (has_unk || has_bos || has_eos)) ||
+        (bounded && (marker.size() != 1 || marker[0] == '\n' || (marker[0] & 0x80)))) {
         usage();
         return 2;
     }
@@ -88,7 +94,9 @@ int main(int argc, char** argv) {
         std::string line;
         auto flush_batch = [&]() {
             if (pk.size() == 0) return;
-            BatchResult r = tokenizer.tokenize_batch(pk.utf8.data(), pk.off.data(), pk.size());
+            BatchResult r = bounded ? tokenizer.tokenize_batch(pk.utf8.data(), pk.off.data(), pk.size(), pk.bnd_off.data(),
+                                                               pk.bnd.data())
+                                    : tokenizer.tokenize_batch(pk.utf8.data(), pk.off.data(), pk.size());
             if (format_on == "device") {
                 std::string_view text = r.text();
                 std::fwrite(text.data(), 1, text.size(), stdout);
@@ -125,7 +133,12 @@ int main(int argc, char** argv) {
             pk.clear();
         };
         while (cli::read_line(std::cin, line)) {
-            pk.add(line);
+            if (bounded) {
+                const std::vector<uint32_t> bnd = cli::strip_boundary_markers(line, marker[0]);
+                pk.add(line, bnd);
+            } else {
+                pk.add(line);
+            }
             if (pk.size() >= batch_lines) flush_batch();
         }
         flush_batch();

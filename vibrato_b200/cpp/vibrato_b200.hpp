@@ -243,6 +243,25 @@ class Tokenizer {
         check(vbt_tokenize_batch(handle(), utf8, byte_offsets, n_sent, &r));
         return BatchResult(r);
     }
+    // With required boundaries: sentence i's are the byte offsets bnd[bnd_offsets[i] .. bnd_offsets[i+1]).
+    BatchResult tokenize_batch(const char* utf8, const uint64_t* byte_offsets, uint64_t n_sent, const uint64_t* bnd_offsets,
+                               const uint32_t* bnd) const {
+        vbt_result* r = nullptr;
+        check(vbt_tokenize_batch_bounded(handle(), utf8, byte_offsets, n_sent, bnd_offsets, bnd, &r));
+        return BatchResult(r);
+    }
+    // Device-resident batches (device addresses in, device addresses of the results out; see vibrato_b200.h).
+    void tokenize_batch_device(uint64_t d_utf8, uint64_t d_byte_offsets, uint64_t n_sent, uint64_t n_bytes,
+                               uint64_t& d_tok_offsets, uint64_t& d_tokens, uint64_t& n_tokens) const {
+        check(vbt_tokenize_batch_device(handle(), d_utf8, d_byte_offsets, n_sent, n_bytes, &d_tok_offsets, &d_tokens,
+                                        &n_tokens));
+    }
+    void tokenize_batch_device(uint64_t d_utf8, uint64_t d_byte_offsets, uint64_t n_sent, uint64_t n_bytes,
+                               uint64_t d_bnd_offsets, uint64_t d_bnd, uint64_t n_bnd, uint64_t& d_tok_offsets,
+                               uint64_t& d_tokens, uint64_t& n_tokens) const {
+        check(vbt_tokenize_batch_device_bounded(handle(), d_utf8, d_byte_offsets, n_sent, n_bytes, d_bnd_offsets, d_bnd,
+                                                n_bnd, &d_tok_offsets, &d_tokens, &n_tokens));
+    }
 
    private:
     vbt_tokenizer* handle() const {
@@ -299,12 +318,22 @@ class Worker {  // worker.rs:13-74
     explicit Worker(const Tokenizer* t) : t_(t) {}
     void reset_sentence(std::string_view s) {
         sent_.assign(s);
+        bnd_.clear();
+        bounded_ = false;
         toks_.clear();
+    }
+    // With required boundaries (byte offsets into s; see Tokenizer::tokenize_batch).
+    void reset_sentence(std::string_view s, std::vector<uint32_t> boundaries) {
+        reset_sentence(s);
+        bnd_ = std::move(boundaries);
+        bounded_ = true;
     }
     void tokenize() {
         if (sent_.empty()) return;  // worker.rs:50-52
         uint64_t off[2] = {0, sent_.size()};
-        BatchResult r = t_->tokenize_batch(sent_.data(), off, 1);
+        uint64_t boff[2] = {0, bnd_.size()};
+        BatchResult r = bounded_ ? t_->tokenize_batch(sent_.data(), off, 1, boff, bnd_.data())
+                                 : t_->tokenize_batch(sent_.data(), off, 1);
         toks_.assign(r.tokens(), r.tokens() + r.n_tokens());
     }
     size_t num_tokens() const { return toks_.size(); }
@@ -313,6 +342,8 @@ class Worker {  // worker.rs:13-74
    private:
     const Tokenizer* t_;
     std::string sent_;
+    std::vector<uint32_t> bnd_;
+    bool bounded_ = false;
     std::vector<vbt_token> toks_;
 };
 

@@ -428,6 +428,23 @@ int32_t vbt_tokenize_batch(vbt_tokenizer* t, const char* utf8, const uint64_t* b
     });
 }
 
+int32_t vbt_tokenize_batch_bounded(vbt_tokenizer* t, const char* utf8, const uint64_t* byte_offsets, uint64_t n_sent,
+                                   const uint64_t* bnd_offsets, const uint32_t* bnd, vbt_result** out) {
+    return guarded([&] {
+        need(t, "t");
+        need(out, "out");
+        need(byte_offsets, "byte_offsets");
+        need(bnd_offsets, "bnd_offsets");
+        if (n_sent && byte_offsets[n_sent] > byte_offsets[0]) need(utf8, "utf8");
+        if (bnd_offsets[n_sent] > bnd_offsets[0]) need(bnd, "bnd");
+        for (uint64_t i = 0; i < n_sent; ++i)
+            if (byte_offsets[i] > byte_offsets[i + 1]) throw vbt::Error(vbt::kInvalidArgument, "byte_offsets must be non-decreasing");
+        const vbt::Bounds b{bnd_offsets, bnd, bnd_offsets[n_sent]};  // the boundary lists are checked on the device
+        vbt::HostResult* r = t->e->run_host(utf8, byte_offsets, n_sent, &b);
+        *out = new vbt_result{t->e, r};
+    });
+}
+
 int32_t vbt_result_view(const vbt_result* r, const uint64_t** tok_offsets, const vbt_token** toks, uint64_t* n_sent,
                         uint64_t* n_tokens) {
     return guarded([&] {
@@ -494,6 +511,21 @@ int32_t vbt_tokenize_batch_device(vbt_tokenizer* t, uint64_t d_utf8, uint64_t d_
         need(d_tokens, "d_tokens");
         need(n_tokens, "n_tokens");
         t->e->run_device(d_utf8, d_byte_offsets, n_sent, n_bytes, d_tok_offsets, d_tokens, n_tokens);
+    });
+}
+
+int32_t vbt_tokenize_batch_device_bounded(vbt_tokenizer* t, uint64_t d_utf8, uint64_t d_byte_offsets, uint64_t n_sent,
+                                          uint64_t n_bytes, uint64_t d_bnd_offsets, uint64_t d_bnd, uint64_t n_bnd,
+                                          uint64_t* d_tok_offsets, uint64_t* d_tokens, uint64_t* n_tokens) {
+    return guarded([&] {
+        need(t, "t");
+        need(d_tok_offsets, "d_tok_offsets");
+        need(d_tokens, "d_tokens");
+        need(n_tokens, "n_tokens");
+        if (!d_bnd_offsets) throw vbt::Error(vbt::kInvalidArgument, "d_bnd_offsets is null");
+        if (n_bnd && !d_bnd) throw vbt::Error(vbt::kInvalidArgument, "d_bnd is null");
+        const vbt::Bounds b{reinterpret_cast<const uint64_t*>(d_bnd_offsets), reinterpret_cast<const uint32_t*>(d_bnd), n_bnd};
+        t->e->run_device(d_utf8, d_byte_offsets, n_sent, n_bytes, d_tok_offsets, d_tokens, n_tokens, &b);
     });
 }
 

@@ -145,13 +145,22 @@ __global__ void k_add_value(unsigned long long* tok_off, uint32_t n_plus_1, unsi
 struct Workspace {  // every per-(chunk of a)-batch device array; two of them let consecutive chunks overlap
     DevBuf n_slots, slot_off, eos, n_tok, code_sys, code_usr, cinfo, groupable, byte_pos, info, info_ex, ends_cnt,
         ends_meta, cand, ends_hot, ends_cold, scan_tmp, stats, iota, sort_keys, order;
+    DevBuf bnd_dist;  // bounded batches only: Batch::bnd_dist
     cudaStream_t stream = nullptr;
     void release() {
         for (DevBuf* b : {&n_slots, &slot_off, &eos, &n_tok, &code_sys, &code_usr, &cinfo, &groupable, &byte_pos, &info,
                           &info_ex, &ends_cnt, &ends_meta, &cand, &ends_hot, &ends_cold, &scan_tmp, &stats, &iota,
-                          &sort_keys, &order})
+                          &sort_keys, &order, &bnd_dist})
             b->release();
     }
+};
+
+// The required boundaries of a batch (or chunk) in device memory: bnd_off[n_sent + 1] into bnd[n]; off == nullptr
+// for an unbounded batch.
+struct DevBounds {
+    const unsigned long long* off = nullptr;
+    const uint32_t* bnd = nullptr;
+    uint64_t n = 0;
 };
 
 struct OutSlot {  // where one (chunk of a) batch leaves its results; two of them alternate in chunked runs
@@ -324,13 +333,14 @@ class EngineImpl final : public Engine {
         tok_base_.release();
         text_base_.release();
         for (DevBuf* b : {&fmt_prog_, &ft_keep_, &ft_off_, &ft_bytes_}) b->release();
-        for (auto* b : {&blob_own_, &in_utf8_, &in_off_, &connid_, &connid_try_}) b->release();
+        for (auto* b : {&blob_own_, &in_utf8_, &in_off_, &in_bnd_off_, &in_bnd_, &connid_, &connid_try_}) b->release();
         for (auto& w : ws_) w.release();
         ws_small_.release();
         small_in_.release();
         small_out_.release();
         pinned_free(small_in_h_);
         pinned_free(small_out_h_);
+        pinned_free(bnd_stage_);
         cudaStreamSynchronize(aux_stream_);
         cudaStreamDestroy(aux_stream_);
         for (auto& e : base_ready_) cudaEventDestroy(e);
@@ -438,11 +448,15 @@ class EngineImpl final : public Engine {
     }
 
     void run_device(uint64_t d_utf8, uint64_t d_byte_off, uint64_t n_sent, uint64_t n_bytes, uint64_t* d_tok_off,
-                    uint64_t* d_tokens, uint64_t* n_tokens) override {
+                    uint64_t* d_tokens, uint64_t* n_tokens, const Bounds* bnd) override {
         CK(cudaSetDevice(device_));
         check_size(n_sent, n_bytes);
+        check_bounded(bnd);
+        if (bnd && bnd->n == 0 && device_offsets_zero(bnd->off, n_sent)) bnd = nullptr;  // no boundary at all
+        DevBounds bd;
+        if (bnd) bd = DevBounds{reinterpret_cast<const unsigned long long*>(bnd->off), bnd->bnd, bnd->n};
         run_whole(reinterpret_cast<const uint8_t*>(d_utf8), reinterpret_cast<const unsigned long long*>(d_byte_off),
-                  uint32_t(n_sent), n_bytes);
+                  uint32_t(n_sent), n_bytes, bd);
         *d_tok_off = reinterpret_cast<uint64_t>(out_[0].tok_off.p);
         *d_tokens = reinterpret_cast<uint64_t>(out_[0].tokens.p);
         *n_tokens = out_[0].h_ctrl->n_tokens;
@@ -450,12 +464,14 @@ class EngineImpl final : public Engine {
 
     // Host path.  Large batches are cut into chunks that flow through three streams: the H2D copy of
     // chunk i+1 and the D2H copy of chunk i-1 overlap the kernels of chunk i (PCIe is full duplex).
-    HostResult* run_host(const char* utf8, const uint64_t* byte_off, uint64_t n_sent64) override {
+    HostResult* run_host(const char* utf8, const uint64_t* byte_off, uint64_t n_sent64, const Bounds* bnd) override {
         CK(cudaSetDevice(device_));
         // offsets may start anywhere in the caller's buffer; ship only the used window
         const uint64_t first = n_sent64 ? byte_off[0] : 0;
         const uint64_t n_bytes = n_sent64 ? byte_off[n_sent64] - first : 0;
         check_size(n_sent64, n_bytes);
+        check_bounded(bnd);
+        if (bnd && host_lists_empty(*bnd, n_sent64)) bnd = nullptr;  // no boundary at all: the unbounded kernels
         const uint32_t n_sent = uint32_t(n_sent64);
         in_utf8_.ensure(n_bytes + 16, 1.25);
         in_off_.ensure((size_t(n_sent) + 1) * 8, 1.25);
@@ -473,10 +489,12 @@ class EngineImpl final : public Engine {
         const uint32_t chunk = chunk_sentences_;
         const bool chunked = chunk > 0 && n_sent > chunk + chunk / 2;
         const bool fmt = output_mode_ != kOutNone;
-        if (small_batch_ && n_sent <= small_batch_ && !chunked && n_bytes <= kEagerBytes && !counting_ && !connid_on_) {
-            if (HostResult* r = run_small(utf8 + first, off, n_sent, n_bytes)) return r;
+        if (small_batch_ && n_sent <= small_batch_ && !chunked && n_bytes <= kEagerBytes && !counting_ && !connid_on_ &&
+            (!bnd || small_bounds_fit(*bnd, n_sent))) {
+            if (HostResult* r = run_small(utf8 + first, off, n_sent, n_bytes, bnd)) return r;
             // the batch outgrew the scratch of k_small_batch: it runs again on the route below
         }
+        const DevBounds bd = bnd ? upload_bounds(*bnd, n_sent, stream_) : DevBounds{};
         for (int attempt = 0;; ++attempt) {
             if (!chunked) {
                 h2d(in_off_.p, off, (size_t(n_sent) + 1) * 8, stream_, off_pinned && off == byte_off);
@@ -488,7 +506,7 @@ class EngineImpl final : public Engine {
                     HostResult* r = acquire(n_sent, n_bytes);
                     eager_sink_ = r;
                     try {
-                        run_whole(d_utf8, d_off, n_sent, n_bytes);
+                        run_whole(d_utf8, d_off, n_sent, n_bytes, bd);
                     } catch (...) {
                         eager_sink_ = nullptr;
                         release(r);
@@ -499,7 +517,7 @@ class EngineImpl final : public Engine {
                     r->has_text = false;
                     return r;
                 }
-                run_whole(d_utf8, d_off, n_sent, n_bytes);
+                run_whole(d_utf8, d_off, n_sent, n_bytes, bd);
                 OutSlot& o = out_[0];
                 HostResult* r = acquire(n_sent, o.h_ctrl->n_tokens);
                 CK(cudaMemcpyAsync(r->tok_off, o.tok_off.p, (size_t(n_sent) + 1) * 8, cudaMemcpyDeviceToHost, stream_));
@@ -534,7 +552,7 @@ class EngineImpl final : public Engine {
             ws_[1].stream = aux_stream_;
             const uint32_t n_ws = dual_stream_ ? 2 : 1;
             for (uint32_t i = 0; i < n_ws; ++i)
-                ensure_workspace(ws_[i], max_chunk_sent, max_chunk_bytes);  // sized once: no cudaMalloc in the pipeline
+                ensure_workspace(ws_[i], max_chunk_sent, max_chunk_bytes, bd.off != nullptr);  // sized once: no cudaMalloc in the pipeline
             for (auto& o : out_) {
                 o.tok_off.ensure((size_t(max_chunk_sent) + 1) * 8, 1.25);
                 o.tokens.ensure(size_t(max_chunk_bytes) * 24 + 24, 1.25);
@@ -566,6 +584,7 @@ class EngineImpl final : public Engine {
             double text_need = 0;  // text bytes per input byte beyond text_per_sent_ per sentence, largest over the sound chunks
             uint32_t route = kRouteNone;
             bool overflow = false, bad_utf8 = false, bad_offsets = false, slots_overflow = false, text_overflow = false;
+            bool bad_bounds = false;
             uint64_t slots_seen = 0;
             batch_total_bytes_ = n_bytes;
             std::vector<cudaEvent_t>& h2d_ev = h2d_events(n_chunks);
@@ -587,6 +606,7 @@ class EngineImpl final : public Engine {
                 CK(cudaEventSynchronize(o.done));
                 if (o.h_ctrl->flags & kFlagUtf8Error) bad_utf8 = true;
                 if (o.h_ctrl->flags & kFlagBadOffsets) bad_offsets = true;
+                if (o.h_ctrl->flags & kFlagBadBoundary) bad_bounds = true;
                 if (o.h_ctrl->flags & kFlagPoolOverflow) overflow = true;
                 if (o.h_ctrl->flags & kFlagSlotsOverflow) overflow = slots_overflow = true;
                 if (o.h_ctrl->flags & kFlagTextOverflow) text_overflow = true;
@@ -605,7 +625,7 @@ class EngineImpl final : public Engine {
                 const uint64_t nt = o.h_ctrl->n_tokens, nx = fmt ? o.h_ctrl->text_bytes : 0;
                 if (fmt && !(o.h_ctrl->flags & (kFlagsStandDown | kFlagUtf8Error | kFlagPoolOverflow)))
                     text_need = std::max(text_need, (double(nx) - double(text_per_sent_) * (s1 - s0)) / double(std::max<uint64_t>(1, off[s1] - off[s0])));
-                if (!overflow && !text_overflow && !bad_utf8 && !bad_offsets) {
+                if (!overflow && !text_overflow && !bad_utf8 && !bad_offsets && !bad_bounds) {
                     if ((tok_total + nt) * tok_bytes_ > r->cap_tok) {  // rare: grow the pinned buffer, keep what is there
                         CK(cudaStreamSynchronize(out_stream_));
                         size_t cap = size_t(double((tok_total + nt) * 24) * 1.5) + 4096;
@@ -650,9 +670,11 @@ class EngineImpl final : public Engine {
                 Workspace& w = ws_[dual_stream_ ? (c & 1) : 0];
                 CK(cudaStreamWaitEvent(w.stream, h2d_ev[c], 0));
                 if (c >= 2) CK(cudaStreamWaitEvent(w.stream, o.drained, 0));  // slot reused: its D2H must be done
+                DevBounds cb = bd;  // the chunk's slice of the boundary offsets (they index the whole bnd array)
+                if (cb.off) cb.off += s0;
                 enqueue(w, d_utf8, d_off + s0, s1 - s0, off[s1] - off[s0], o, tok_base_.as<unsigned long long>(),
                         fmt ? text_base_.as<unsigned long long>() : nullptr, c >= 1 ? base_ready_[(c - 1) & 1] : nullptr,
-                        base_ready_[c & 1]);
+                        base_ready_[c & 1], cb);
                 if (!utf8_pinned && c + 1 < n_chunks) issue_h2d(c + 1);
                 if (c >= 1) drain(c - 1);
             }
@@ -668,6 +690,10 @@ class EngineImpl final : public Engine {
             if (bad_utf8) {
                 release(r);
                 throw Error(kUtf8, "stream did not contain valid UTF-8");
+            }
+            if (bad_bounds) {
+                release(r);
+                throw Error(kInvalidArgument, kBadBoundsMsg);
             }
             if (overflow || text_overflow) {
                 release(r);
@@ -697,12 +723,16 @@ class EngineImpl final : public Engine {
     }
 
     // ---- shard-level entry points (multi_engine.cu) -------------------------------------------------
-    uint64_t run_shard(const char* utf8, const uint64_t* byte_off, uint64_t n_sent64, int src_device, uint64_t* text_bytes) override {
+    uint64_t run_shard(const char* utf8, const uint64_t* byte_off, uint64_t n_sent64, int src_device, uint64_t* text_bytes,
+                       const Bounds* bnd) override {
         CK(cudaSetDevice(device_));
         const uint64_t first = n_sent64 ? byte_off[0] : 0;
         const uint64_t n_bytes = n_sent64 ? byte_off[n_sent64] - first : 0;
         check_size(n_sent64, n_bytes);
+        check_bounded(bnd);
+        if (bnd && host_lists_empty(*bnd, n_sent64)) bnd = nullptr;
         const uint32_t n_sent = uint32_t(n_sent64);
+        const DevBounds bd = bnd ? upload_bounds(*bnd, n_sent, stream_) : DevBounds{};
         in_utf8_.ensure(n_bytes + 16, 1.25);
         in_off_.ensure((size_t(n_sent) + 1) * 8, 1.25);
         const uint64_t* off = byte_off;
@@ -720,7 +750,7 @@ class EngineImpl final : public Engine {
             else
                 h2d(in_utf8_.p, utf8 + first, n_bytes, stream_, is_pinned(utf8 + first));
         }
-        run_whole(in_utf8_.as<uint8_t>(), in_off_.as<unsigned long long>(), n_sent, n_bytes);
+        run_whole(in_utf8_.as<uint8_t>(), in_off_.as<unsigned long long>(), n_sent, n_bytes, bd);
         shard_n_sent_ = n_sent;
         shard_text_ = text_bytes && output_mode_ != kOutNone;
         shard_text_bytes_ = shard_text_ ? format_whole(in_utf8_.as<uint8_t>(), in_off_.as<unsigned long long>(), n_sent) : 0;
@@ -821,6 +851,53 @@ class EngineImpl final : public Engine {
         // warp-per-sentence kernels derive the sentence from a 32-bit global thread index (>> 5): 2^27 is the bound
         if (n_sent >= 0x07FFFFFFull || n_bytes + n_sent >= 0xFFFFFF00ull)
             throw Error(kInvalidArgument, "batch too large: split it (at most 2^27 sentences / 2^32 characters per call)");
+    }
+
+    static constexpr const char* kBadBoundsMsg =
+        "required boundaries must be non-decreasing, at most the sentence's byte length and on a UTF-8 lead byte, "
+        "and their offsets non-decreasing and within the boundary array";
+
+    void check_bounded(const Bounds* bnd) const {
+        if (bnd && counting_)
+            throw Error(kInvalidArgument, "the \"counting\" hook measures the unconstrained lattice: it refuses bounded batches");
+    }
+
+    // A batch whose boundary lists are all empty (every offset the same) runs the unbounded kernels.  Broken offsets
+    // are not empty: they take the bounded route, which reports them after the errors that take precedence.
+    static bool host_lists_empty(const Bounds& hb, uint64_t n_sent) {
+        for (uint64_t i = 0; i < n_sent; ++i)
+            if (hb.off[i + 1] != hb.off[0]) return false;
+        return true;
+    }
+    // The same for device-resident lists with n_bnd == 0: valid offsets are then all 0 (one copy of them to the host).
+    bool device_offsets_zero(const uint64_t* d_off, uint64_t n_sent) {
+        const size_t bytes = (size_t(n_sent) + 1) * 8;
+        if (bnd_stage_cap_ < bytes) {
+            pinned_free(bnd_stage_);
+            bnd_stage_ = static_cast<uint64_t*>(pinned_alloc(bytes));
+            bnd_stage_cap_ = bytes;
+        }
+        CK(cudaMemcpyAsync(bnd_stage_, d_off, bytes, cudaMemcpyDeviceToHost, stream_));
+        CK(cudaStreamSynchronize(stream_));
+        for (uint64_t i = 0; i <= n_sent; ++i)
+            if (bnd_stage_[i] != 0) return false;
+        return true;
+    }
+
+    // Host boundary lists -> in_bnd_off_ / in_bnd_ on `st`.  The offsets are rebased to the window that is copied,
+    // bnd[off[0] .. off[n_sent]).  A list whose window is inverted or leaves bnd ships no boundaries and keeps
+    // offsets that k_mark_bounds refuses (some sentence's end offset then lies below its start or beyond 0).
+    DevBounds upload_bounds(const Bounds& hb, uint32_t n_sent, cudaStream_t st) {
+        const uint64_t first = hb.off[0], last = hb.off[n_sent];
+        const bool sound = first <= last && last <= hb.n;
+        const uint64_t lo = sound ? first : 0, n = sound ? last - first : 0;
+        bnd_rebased_.resize(size_t(n_sent) + 1);
+        for (uint32_t i = 0; i <= n_sent; ++i) bnd_rebased_[i] = hb.off[i] - lo;  // wraps for a broken list: refused
+        in_bnd_off_.ensure((size_t(n_sent) + 1) * 8, 1.25);
+        in_bnd_.ensure(n * 4 + 4, 1.25);
+        h2d(in_bnd_off_.p, bnd_rebased_.data(), (size_t(n_sent) + 1) * 8, st, false);
+        if (n) h2d(in_bnd_.p, hb.bnd + lo, n * 4, st, is_pinned(hb.bnd + lo));
+        return DevBounds{in_bnd_off_.as<unsigned long long>(), in_bnd_.as<uint32_t>(), n};
     }
 
     std::vector<cudaEvent_t>& h2d_events(uint32_t n) {
@@ -943,6 +1020,14 @@ class EngineImpl final : public Engine {
     static constexpr size_t kSmallText = size_t(2) << 20;
     static constexpr long long kSmallBatchMax = 65536;
     static constexpr size_t kSmallHead = 64;  // SmallBatchOut, padded
+    static constexpr uint64_t kSmallBounds = 16384;  // boundaries a bounded batch may bring (more take the usual route)
+
+    // A bounded host batch takes k_small_batch when its boundaries fit the upload; a broken list is left to the usual
+    // route, which reports it.
+    bool small_bounds_fit(const Bounds& hb, uint32_t n_sent) const {
+        const uint64_t first = hb.off[0], last = hb.off[n_sent];
+        return first <= last && last <= hb.n && last - first <= kSmallBounds;
+    }
 
     void ensure_small() {
         Workspace& w = ws_small_;
@@ -961,10 +1046,11 @@ class EngineImpl final : public Engine {
         w.info_ex.ensure(ms * 8);
         w.ends_cnt.ensure(ms * 4);
         w.ends_meta.ensure(ms * 8);
+        w.bnd_dist.ensure(ms * 4);
         w.cand.ensure(size_t(kSmallCands) * 16);
         w.ends_hot.ensure((kSmallCands + ns) * 8);
         w.ends_cold.ensure((kSmallCands + ns) * 16);
-        const size_t in_cap = ns * 8 + kEagerBytes;
+        const size_t in_cap = ns * 8 + kEagerBytes + 8 + ns * 8 + kSmallBounds * 4;  // [off | utf8 | bnd_off | bnd]
         const size_t out_cap = kSmallHead + 2 * ns * 8 + 16 + kEagerBytes * 24 + kSmallText;
         small_in_.ensure(in_cap);
         small_out_.ensure(out_cap);
@@ -983,12 +1069,23 @@ class EngineImpl final : public Engine {
     // One host batch through k_small_batch: one copy up, one launch, one copy down, one synchronisation (a second
     // copy only when the text outgrew the part of the region the first one brought back).  Returns nullptr when the
     // batch overflowed the scratch; input errors throw like on the usual route.
-    HostResult* run_small(const char* utf8, const uint64_t* off, uint32_t n_sent, uint64_t n_bytes) {
+    HostResult* run_small(const char* utf8, const uint64_t* off, uint32_t n_sent, uint64_t n_bytes, const Bounds* bnd) {
         ensure_small();
         const size_t off_bytes = (size_t(n_sent) + 1) * 8;
         std::memcpy(small_in_h_, off, off_bytes);
         if (n_bytes) std::memcpy(small_in_h_ + off_bytes, utf8, n_bytes);
-        CK(cudaMemcpyAsync(small_in_.p, small_in_h_, off_bytes + n_bytes, cudaMemcpyHostToDevice, stream_));
+        size_t in_bytes = off_bytes + n_bytes;
+        const size_t at_bnd_off = (in_bytes + 7) & ~size_t(7), at_bnd = at_bnd_off + off_bytes;
+        uint64_t n_bnd = 0;
+        if (bnd) {  // the boundaries travel in the same copy, their offsets rebased to the part that is copied
+            const uint64_t first = bnd->off[0];
+            n_bnd = bnd->off[n_sent] - first;
+            uint64_t* o = reinterpret_cast<uint64_t*>(small_in_h_ + at_bnd_off);
+            for (uint32_t i = 0; i <= n_sent; ++i) o[i] = bnd->off[i] - first;
+            if (n_bnd) std::memcpy(small_in_h_ + at_bnd, bnd->bnd + first, n_bnd * 4);
+            in_bytes = at_bnd + n_bnd * 4;
+        }
+        CK(cudaMemcpyAsync(small_in_.p, small_in_h_, in_bytes, cudaMemcpyHostToDevice, stream_));
 
         const bool fmt = output_mode_ != kOutNone;
         const size_t tb = tok_bytes_;
@@ -1022,6 +1119,12 @@ class EngineImpl final : public Engine {
         b.ends_cold = w.ends_cold.as<uint4>();
         b.tokens = region + at_tokens;
         b.compact = tb == 16 ? 1u : 0u;
+        if (bnd) {
+            b.bnd_off = reinterpret_cast<const unsigned long long*>(small_in_.as<uint8_t>() + at_bnd_off);
+            b.bnd = reinterpret_cast<const uint32_t*>(small_in_.as<uint8_t>() + at_bnd);
+            b.n_bnd = n_bnd;
+            b.bnd_dist = w.bnd_dist.as<uint32_t>();
+        }
         FormatArgs f{};
         f.utf8 = b.utf8;
         f.byte_off = b.byte_off;
@@ -1050,6 +1153,7 @@ class EngineImpl final : public Engine {
         if (h.flags & kFlagBadOffsets)
             throw Error(kInvalidArgument, "byte_offsets must be non-decreasing and end within the input buffer");
         if (h.flags & kFlagUtf8Error) throw Error(kUtf8, "stream did not contain valid UTF-8");
+        if (h.flags & kFlagBadBoundary) throw Error(kInvalidArgument, kBadBoundsMsg);
         if (h.flags & (kFlagPoolOverflow | kFlagTextOverflow)) return nullptr;
         if (fmt && h.text_bytes > text_guess) {
             CK(cudaMemcpyAsync(small_out_h_ + at_text + text_guess, region + at_text + text_guess, h.text_bytes - text_guess,
@@ -1162,7 +1266,7 @@ class EngineImpl final : public Engine {
 
     // Sizes every workspace array for batches of up to n_sent sentences / n_bytes bytes (upper
     // bounds: characters <= bytes, one sentinel slot per sentence).
-    void ensure_workspace(Workspace& w, uint32_t n_sent, uint64_t n_bytes) {
+    void ensure_workspace(Workspace& w, uint32_t n_sent, uint64_t n_bytes, bool bounded) {
         const size_t ns = size_t(n_sent) + 1;
         w.n_slots.ensure(ns * 4, 1.25);
         w.slot_off.ensure(ns * 4, 1.25);
@@ -1183,6 +1287,7 @@ class EngineImpl final : public Engine {
         w.info_ex.ensure(ms * 8, 1.25);
         w.ends_cnt.ensure(ms * 4, 1.25);
         w.ends_meta.ensure(ms * 8, 1.25);
+        if (bounded) w.bnd_dist.ensure(ms * 4, 1.25);
         if (counting_) w.stats.ensure(ms * 16, 1.25);
         size_t want_cand = std::max<size_t>(1 << 16, size_t(double(n_bytes) * cand_per_byte_) + 4096);
         want_cand = std::min<size_t>(want_cand, 0xFFFFFFF0ull);
@@ -1201,22 +1306,24 @@ class EngineImpl final : public Engine {
     }
 
     // One whole batch from device-resident input into out_[0]; synchronises, retries on pool overflow.
-    void run_whole(const uint8_t* d_utf8, const unsigned long long* d_off, uint32_t n_sent, uint64_t n_bytes) {
+    void run_whole(const uint8_t* d_utf8, const unsigned long long* d_off, uint32_t n_sent, uint64_t n_bytes,
+                   const DevBounds& bd) {
         OutSlot& o = out_[0];
         ws_[0].stream = stream_;
         batch_total_bytes_ = n_bytes;
         for (int attempt = 0;; ++attempt) {
-            ensure_workspace(ws_[0], n_sent, n_bytes);
+            ensure_workspace(ws_[0], n_sent, n_bytes, bd.off != nullptr);
             o.tok_off.ensure((size_t(n_sent) + 1) * 8, 1.25);
             o.tokens.ensure(size_t(n_bytes) * 24 + 24, 1.25);  // a token spans >= 1 character >= 1 byte
             connid_begin(stream_);
-            enqueue(ws_[0], d_utf8, d_off, n_sent, n_bytes, o, nullptr, nullptr, nullptr, nullptr);
+            enqueue(ws_[0], d_utf8, d_off, n_sent, n_bytes, o, nullptr, nullptr, nullptr, nullptr, bd);
             CK(cudaEventSynchronize(o.done));
             CK(cudaGetLastError());
             if (o.h_ctrl->flags & kFlagBadOffsets)
                 throw Error(kInvalidArgument, "byte_offsets must be non-decreasing and end within the input buffer");
             if (o.h_ctrl->flags & kFlagUtf8Error)
                 throw Error(kUtf8, "stream did not contain valid UTF-8");  // what `stdin.lines()` reports
+            if (o.h_ctrl->flags & kFlagBadBoundary) throw Error(kInvalidArgument, kBadBoundsMsg);
             if (o.h_ctrl->flags & kFlagSlotsOverflow) {  // more characters per byte than any batch before: hard bound
                 if (attempt >= 3) throw Error(kInternal, "slot overflow persists");
                 chars_per_byte_ = 1.0;
@@ -1246,7 +1353,7 @@ class EngineImpl final : public Engine {
     // o.text up to its capacity (kFlagTextOverflow beyond).
     void enqueue(Workspace& w, const uint8_t* d_utf8, const unsigned long long* d_off, uint32_t n_sent, uint64_t n_bytes,
                  OutSlot& o, unsigned long long* tok_base, unsigned long long* text_base, cudaEvent_t base_wait,
-                 cudaEvent_t base_signal) {
+                 cudaEvent_t base_signal, const DevBounds& bd) {
         cudaStream_t st = w.stream;
         // characters <= bytes is the hard bound; the per-character launches are sized from the ratio learned on
         // earlier batches (plus slack), and a batch that exceeds it flags itself and is re-run with the hard bound
@@ -1289,6 +1396,12 @@ class EngineImpl final : public Engine {
         // or dropped, and must not leave its partial counts behind (lattice.rs:170-181 counts a lattice once)
         b.lid_count = connid_on_ ? connid_try_.as<unsigned long long>() : nullptr;
         b.rid_count = connid_on_ ? connid_try_.as<unsigned long long>() + num_left_ : nullptr;
+        if (bd.off) {
+            b.bnd_off = bd.off;
+            b.bnd = bd.bnd;
+            b.n_bnd = bd.n;
+            b.bnd_dist = w.bnd_dist.as<uint32_t>();
+        }
 
         o.launches = 0;
         CK(cudaMemsetAsync(dc, 0, sizeof(Control), st));
@@ -1316,6 +1429,10 @@ class EngineImpl final : public Engine {
         }
         CK(cudaEventRecord(o.ev[2], st));
         launch_decode(dv_, b, st);
+        if (b.bnd_dist && n_sent) {  // the bounded batch's boundaries, booked with the decode stage
+            launch_mark_bounds(b, st);
+            ++o.launches;
+        }
         CK(cudaEventRecord(o.ev[3], st));
         launch_candidates(dv_, b, max_slots, st);
         if (counting_) {
@@ -1392,6 +1509,10 @@ class EngineImpl final : public Engine {
     DictView dv_{};
     const uint8_t* blob_ = nullptr;
     DevBuf blob_own_, in_utf8_, in_off_, connid_, connid_try_;
+    DevBuf in_bnd_off_, in_bnd_;           // boundary lists of a bounded host batch (upload_bounds)
+    std::vector<uint64_t> bnd_rebased_;
+    uint64_t* bnd_stage_ = nullptr;  // pinned: device-resident boundary offsets checked for emptiness
+    size_t bnd_stage_cap_ = 0;
     bool connid_on_ = false;
     uint32_t num_left_ = 0, num_right_ = 0;
     std::vector<uint16_t> left_ids_, right_ids_;

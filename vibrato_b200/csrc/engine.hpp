@@ -26,6 +26,15 @@ struct HostResult {  // pinned host memory holding one batch's tokens
     bool has_text = false;
 };
 
+// Required token boundaries of a batch (vbt_tokenize_batch_bounded): sentence i's boundaries are the
+// sentence-relative byte offsets bnd[off[i] .. off[i+1]), and bnd holds n entries.  Host or device addresses, as the
+// call that takes them says.  A null pointer to Bounds = an unbounded batch.
+struct Bounds {
+    const uint64_t* off = nullptr;  // n_sent + 1
+    const uint32_t* bnd = nullptr;
+    uint64_t n = 0;
+};
+
 constexpr int kNumStages = 9;
 extern const char* const kStageNames;  // comma-separated, kNumStages entries
 // A call on the k_small_batch route ("small_batch" option) runs every stage in one kernel: its whole time is booked
@@ -45,10 +54,11 @@ class Engine {
     virtual ~Engine() = default;
 
     // Inputs/outputs in device memory; outputs owned by the engine until the next call.
+    // With bnd: a bounded batch, its boundary arrays in device memory too.  Bounded batches refuse "counting".
     virtual void run_device(uint64_t d_utf8, uint64_t d_byte_off, uint64_t n_sent, uint64_t n_bytes,
-                            uint64_t* d_tok_off, uint64_t* d_tokens, uint64_t* n_tokens) = 0;
-    // Inputs/outputs in host memory (copies inside).
-    virtual HostResult* run_host(const char* utf8, const uint64_t* byte_off, uint64_t n_sent) = 0;
+                            uint64_t* d_tok_off, uint64_t* d_tokens, uint64_t* n_tokens, const Bounds* bnd = nullptr) = 0;
+    // Inputs/outputs in host memory (copies inside); bnd in host memory.
+    virtual HostResult* run_host(const char* utf8, const uint64_t* byte_off, uint64_t n_sent, const Bounds* bnd = nullptr) = 0;
     virtual void release(HostResult* r) = 0;
 
     // Building blocks of the multi-device engine (multi_engine.cu); a single-device caller never needs them.
@@ -56,8 +66,9 @@ class Engine {
     // With src_device >= 0 `utf8` is a DEVICE address on that device (peer copy over NVLink) while byte_off is
     // still a host array.  With text_bytes != nullptr the shard's output text is formatted too ("output_mode";
     // *text_bytes = its size, 0 when the option is off).
+    // bnd (host memory, may be null) holds the shard's n_sent + 1 boundary offsets.
     virtual uint64_t run_shard(const char* utf8, const uint64_t* byte_off, uint64_t n_sent, int src_device,
-                               uint64_t* text_bytes) = 0;
+                               uint64_t* text_bytes, const Bounds* bnd = nullptr) = 0;
     // fetch_shard: the last shard's token offsets (+ tok_base, n_sent entries, one more when `last`) and token
     // records into host memory (pinned, or it is slow); with h_text_off != nullptr also its text offsets
     // (+ text_base, same count) and text, which run_shard must have formatted.

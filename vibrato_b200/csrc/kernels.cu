@@ -255,18 +255,21 @@ struct HitBuf {
 
 // Lexicon::common_prefix_iterator (lexicon.rs:33-46): crawdad common-prefix search over the double
 // array (trie.rs:49-56), then the postings of every hit (posting.rs:18-21) with their WordParams.
-template <bool FILL, bool COUNT>
+// BND (bounded batches): the walk stops at q_end = lim(sw), the first required boundary after sw, so no word that
+// crosses it is a candidate or counts as a match.
+template <bool FILL, bool COUNT, bool BND = false>
 __device__ __forceinline__ uint32_t walk_lexicon(const uint4* __restrict__ nodes, uint32_t num_nodes,
                                                  const uint4* __restrict__ post,
                                                  const uint32_t* __restrict__ codes,
                                                  const uint32_t* __restrict__ groupable, uint32_t sw, uint4* out,
                                                  uint32_t* ends_cnt, WalkStats& st, HitBuf* hb = nullptr,
-                                                 uint32_t lex_flag = 0) {
+                                                 uint32_t lex_flag = 0, uint32_t q_end = 0) {
     if (num_nodes == 0) return 0;
     uint32_t count = 0, node = 0, d = 0, hits = 0;
     uint32_t nbase = __ldg(&nodes[0].x);
     uint32_t q = sw;
     for (;; ++q) {
+        if (BND && q >= q_end) break;
         uint32_t code = codes[q];
         if (code == kInvalidCode) break;  // unmapped character or the sentence's sentinel
         if (nbase & kFlag) break;         // a leaf has no children
@@ -349,9 +352,14 @@ __device__ __forceinline__ uint32_t gen_unknown(const DictView& d, uint32_t sw, 
 struct StartWord {
     uint32_t sw, skip, flags, ci, g;
     bool active;
+    uint32_t lim;  // BND only: lim(sw) - sw
 };
+//
+// BND: w.lim = lim(sw) - sw (bnd_dist), and g is clipped to it wherever gen_unknown uses it, so that a boundary ends a
+// character group.  The space skip is not affected.
+template <bool BND = false>
 __device__ __forceinline__ StartWord start_word(const DictView& d, const Batch& b, uint32_t slot, uint32_t g0) {
-    StartWord w{slot, 0, 0, 0, 0, g0 != 0};
+    StartWord w{slot, 0, 0, 0, 0, g0 != 0, 0};
     if (w.active) {
         uint32_t ci0 = b.cinfo[slot];
         if (ci_cate(ci0) & d.space_mask) {  // tokenizer.rs:117-125: skip the groupable run at a space
@@ -364,6 +372,10 @@ __device__ __forceinline__ StartWord start_word(const DictView& d, const Batch& 
             w.active = false;
         } else {
             w.ci = w.skip ? b.cinfo[w.sw] : ci0;
+            if (BND) {
+                w.lim = b.bnd_dist[w.sw];
+                w.g = min(w.g, w.lim);
+            }
         }
     }
     return w;
@@ -371,29 +383,31 @@ __device__ __forceinline__ StartWord start_word(const DictView& d, const Batch& 
 
 // Candidate count of an active start position: user lexicon, system lexicon, then unknown words, the order of
 // Tokenizer::add_lattice_edges.  `matched` = some lexicon word starts here.  With hb the sources are kept for a fill.
+template <bool BND = false>
 __device__ __forceinline__ uint32_t count_candidates(const DictView& d, const Batch& b, const StartWord& w, bool& matched,
                                                      HitBuf* hb) {
     WalkStats st{0, 0, 0, 0, 0};
     uint32_t cu = 0;
     if (d.usr_table)
-        cu = walk_lexicon<false, false>(d.usr_nodes, d.usr_num_nodes, d.usr_post, b.code_usr, b.groupable, w.sw, nullptr,
-                                        nullptr, st, hb, kSegUser);
-    uint32_t cs = walk_lexicon<false, false>(d.sys_nodes, d.sys_num_nodes, d.sys_post, b.code_sys, b.groupable, w.sw,
-                                             nullptr, nullptr, st, hb, 0);
+        cu = walk_lexicon<false, false, BND>(d.usr_nodes, d.usr_num_nodes, d.usr_post, b.code_usr, b.groupable, w.sw,
+                                             nullptr, nullptr, st, hb, kSegUser, w.sw + w.lim);
+    uint32_t cs = walk_lexicon<false, false, BND>(d.sys_nodes, d.sys_num_nodes, d.sys_post, b.code_sys, b.groupable, w.sw,
+                                                  nullptr, nullptr, st, hb, 0, w.sw + w.lim);
     matched = (cu + cs) != 0;
     return cu + cs + gen_unknown<false>(d, w.sw, w.ci, w.g, matched, nullptr, nullptr, hb);
 }
 
 // Writes the candidates count_candidates counted to `out`, in the same order, and adds them to ends_cnt.
+template <bool BND = false>
 __device__ __forceinline__ void fill_candidates(const DictView& d, const Batch& b, const StartWord& w, bool matched,
                                                 uint4* out) {
     WalkStats st{0, 0, 0, 0, 0};
     uint32_t n = 0;
     if (d.usr_table)
-        n += walk_lexicon<true, false>(d.usr_nodes, d.usr_num_nodes, d.usr_post, b.code_usr, b.groupable, w.sw, out + n,
-                                       b.ends_cnt, st);
-    n += walk_lexicon<true, false>(d.sys_nodes, d.sys_num_nodes, d.sys_post, b.code_sys, b.groupable, w.sw, out + n,
-                                   b.ends_cnt, st);
+        n += walk_lexicon<true, false, BND>(d.usr_nodes, d.usr_num_nodes, d.usr_post, b.code_usr, b.groupable, w.sw,
+                                            out + n, b.ends_cnt, st, nullptr, 0, w.sw + w.lim);
+    n += walk_lexicon<true, false, BND>(d.sys_nodes, d.sys_num_nodes, d.sys_post, b.code_sys, b.groupable, w.sw, out + n,
+                                        b.ends_cnt, st, nullptr, 0, w.sw + w.lim);
     gen_unknown<true>(d, w.sw, w.ci, w.g, matched, out + n, b.ends_cnt);
 }
 
@@ -404,6 +418,8 @@ __device__ __forceinline__ void store_info(const Batch& b, uint32_t slot, uint32
     if (special) b.info_ex[slot] = make_uint2(w.skip, w.flags);
 }
 
+// BND: the bounded instantiation (required boundaries in b.bnd_dist); the unbounded one is the code as it was.
+template <bool BND>
 __global__ void __launch_bounds__(256) k_candidates(DictView d, Batch b) {
     const uint32_t slot = blockIdx.x * blockDim.x + threadIdx.x;
     const uint32_t lane = threadIdx.x & 31;
@@ -415,14 +431,14 @@ __global__ void __launch_bounds__(256) k_candidates(DictView d, Batch b) {
     if (slot == 0 && total_slots > b.launch_slots) atomicOr(b.flags, kFlagSlotsOverflow);
     const bool in_range = slot < total_slots && !(batch_flags & kFlagBadOffsets);
     uint32_t g0 = in_range ? b.groupable[slot] : 0;
-    const StartWord sw = start_word(d, b, slot, g0);
+    const StartWord sw = start_word<BND>(d, b, slot, g0);
     const bool active = sw.active;
     uint32_t cnt = 0;
     bool matched = false;
     __shared__ uint2 s_hits[kMaxHits][256];
     __shared__ uint8_t s_seg_cnt[kMaxHits][256];
     HitBuf hb{&s_hits[0][threadIdx.x], &s_seg_cnt[0][threadIdx.x], 256, 0};
-    if (active) cnt = count_candidates(d, b, sw, matched, &hb);
+    if (active) cnt = count_candidates<BND>(d, b, sw, matched, &hb);
     // Block-aggregated allocation from the candidate pool: a scan inside each warp, the eight warp totals through
     // shared memory, ONE atomicAdd per block.  (One atomic per warp was 1.3 M same-address atomics per batch, and
     // every warp sat on the round trip of its own; the pool also comes out in slot order block by block.)
@@ -499,7 +515,65 @@ __global__ void __launch_bounds__(256) k_candidates(DictView d, Batch b) {
             }
         }
     } else if (active && fits && cnt) {  // some position has more sources than the buffer holds: regenerate per thread
-        fill_candidates(d, b, sw, matched, b.cand + ptr);
+        fill_candidates<BND>(d, b, sw, matched, b.cand + ptr);
+    }
+}
+
+// Required boundaries of sentence s -> bnd_dist, in two passes of the warp.  (1) One lane per boundary: a boundary b
+// (sentence-relative byte offset) with 0 < b < len marks the character that starts at byte b (binary search of
+// byte_pos over the sentence's slots; the slots are cleared first).  (2) Right to left over 32-character chunks, as
+// decode_one solves groupable: bnd_dist[c] = the first marked position after c (or n) - c.  Runs after decode_one of
+// the same sentence.
+// Validates the list on the way: offsets in order and inside bnd, values non-decreasing, <= len and on a UTF-8 lead
+// byte; anything else raises kFlagBadBoundary.  A boundary at 0 or len marks nothing: every token already ends there.
+__device__ __forceinline__ void mark_bounds_one(const Batch& b, uint32_t s, uint32_t lane) {
+    const unsigned long long j0 = b.bnd_off[s], j1 = b.bnd_off[s + 1];
+    const bool listed = !(j1 < j0 || j1 > b.n_bnd);
+    const unsigned long long bo = b.byte_off[s], len = b.byte_off[s + 1] - bo;
+    const uint32_t base = b.slot_off[s], n = b.slot_off[s + 1] - base - 1;
+    uint32_t* mark = b.bnd_dist + base;
+    for (uint32_t i = lane; i <= n; i += 32) mark[i] = 0;
+    __syncwarp();
+    bool bad = !listed;
+    for (unsigned long long j = j0 + lane; listed && j < j1; j += 32) {
+        const uint32_t v = b.bnd[j];
+        if (v > len || (j > j0 && b.bnd[j - 1] > v) || (v < len && (b.utf8[bo + v] & 0xC0) == 0x80)) {
+            bad = true;
+            continue;
+        }
+        if (v == 0 || v == len) continue;
+        uint32_t lo = 0, hi = n;  // byte_pos[base + n] == len > v
+        while (lo < hi) {
+            const uint32_t mid = (lo + hi) >> 1;
+            if (b.byte_pos[base + mid] < v)
+                lo = mid + 1;
+            else
+                hi = mid;
+        }
+        mark[lo] = 1;
+    }
+    if (__any_sync(kFull, bad) && lane == 0) atomicOr(b.flags, kFlagBadBoundary);
+    __syncwarp();
+    uint32_t next = n;  // the first marked position right of the chunks done so far
+    for (int k = int((n + 31) / 32) - 1; k >= 0; --k) {
+        const uint32_t c = uint32_t(k) * 32 + lane;
+        const uint32_t m = __ballot_sync(kFull, c < n && mark[c] != 0);
+        const uint32_t above = lane == 31 ? 0u : m >> (lane + 1);
+        if (c < n) mark[c] = (above ? c + uint32_t(__ffs(above)) : next) - c;
+        if (m) next = uint32_t(k) * 32 + uint32_t(__ffs(m)) - 1;
+    }
+    if (lane == 0) mark[n] = 0;
+}
+
+__global__ void __launch_bounds__(256) k_mark_bounds(Batch b) {
+    if (stand_down(*b.flags)) return;
+    const uint32_t w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const uint32_t lane = threadIdx.x & 31;
+#pragma unroll 1
+    for (uint32_t r = 0; r < VBT_SENT_PER_WARP; ++r) {
+        const uint32_t s = w * VBT_SENT_PER_WARP + r;
+        if (s >= b.n_sent) return;
+        mark_bounds_one(b, s, lane);
     }
 }
 
@@ -1775,7 +1849,7 @@ __device__ __forceinline__ unsigned long long block_scan(uint32_t n, Get get, Pu
     return carry;
 }
 
-template <int CONN>
+template <int CONN, bool BND>
 __global__ void __launch_bounds__(kSmallThreads, 1) k_small_batch(DictView d, Batch b, FormatArgs f, SmallBatchOut* out) {
     __shared__ uint32_t s_flags;
     __shared__ unsigned long long s_warp[32];
@@ -1800,6 +1874,10 @@ __global__ void __launch_bounds__(kSmallThreads, 1) k_small_batch(DictView d, Ba
         for (uint32_t s = wid; s < n; s += nw) {  // K1b
             decode_one(d, b, s, lane);
             __syncwarp();
+            if (BND) {  // required boundaries: a bad list only raises its flag, the engine reports it
+                mark_bounds_one(b, s, lane);
+                __syncwarp();
+            }
         }
         __syncthreads();
         // K2: a thread per start position; the pool is handed out in position order by a scan per block-wide tile
@@ -1807,9 +1885,9 @@ __global__ void __launch_bounds__(kSmallThreads, 1) k_small_batch(DictView d, Ba
         for (uint32_t base = 0; base < total_slots; base += blockDim.x) {
             const uint32_t slot = base + tid;
             const uint32_t g0 = slot < total_slots ? b.groupable[slot] : 0;
-            const StartWord w = start_word(d, b, slot, g0);
+            const StartWord w = start_word<BND>(d, b, slot, g0);
             bool matched = false;
-            const uint32_t cnt = w.active ? count_candidates(d, b, w, matched, nullptr) : 0;
+            const uint32_t cnt = w.active ? count_candidates<BND>(d, b, w, matched, nullptr) : 0;
             unsigned long long tile;
             const unsigned long long ptr = carry + block_exclusive(cnt, tile, s_warp);
             carry += tile;
@@ -1817,7 +1895,7 @@ __global__ void __launch_bounds__(kSmallThreads, 1) k_small_batch(DictView d, Ba
                 atomicOr(&s_flags, kFlagPoolOverflow);
             } else if (g0 != 0) {
                 store_info(b, slot, uint32_t(ptr), cnt, w);
-                if (cnt) fill_candidates(d, b, w, matched, b.cand + ptr);
+                if (cnt) fill_candidates<BND>(d, b, w, matched, b.cand + ptr);
             }
         }
         __syncthreads();
@@ -1871,14 +1949,22 @@ __global__ void __launch_bounds__(kSmallThreads, 1) k_small_batch(DictView d, Ba
 
 }  // namespace
 
-void launch_small_batch(const DictView& d, const Batch& b, const FormatArgs& f, SmallBatchOut* out, cudaStream_t st) {
+template <bool BND>
+static void launch_small_batch_b(const DictView& d, const Batch& b, const FormatArgs& f, SmallBatchOut* out, cudaStream_t st) {
     const size_t smem = f.mode == kOutFormat ? sizeof(FormatProgram) : 0;
     if (d.connector_kind == 1)
-        k_small_batch<1><<<1, kSmallThreads, smem, st>>>(d, b, f, out);
+        k_small_batch<1, BND><<<1, kSmallThreads, smem, st>>>(d, b, f, out);
     else if (d.connector_kind == 2)
-        k_small_batch<2><<<1, kSmallThreads, smem, st>>>(d, b, f, out);
+        k_small_batch<2, BND><<<1, kSmallThreads, smem, st>>>(d, b, f, out);
     else
-        k_small_batch<0><<<1, kSmallThreads, smem, st>>>(d, b, f, out);
+        k_small_batch<0, BND><<<1, kSmallThreads, smem, st>>>(d, b, f, out);
+}
+
+void launch_small_batch(const DictView& d, const Batch& b, const FormatArgs& f, SmallBatchOut* out, cudaStream_t st) {
+    if (b.bnd_dist)
+        launch_small_batch_b<true>(d, b, f, out, st);
+    else
+        launch_small_batch_b<false>(d, b, f, out, st);
 }
 
 void launch_format_len(const DictView& d, const FormatArgs& f, cudaStream_t st) {
@@ -1917,10 +2003,19 @@ void launch_decode(const DictView& d, const Batch& b, cudaStream_t st) {
     k_decode<<<blocks, 256, 0, st>>>(d, b);
 }
 
+void launch_mark_bounds(const Batch& b, cudaStream_t st) {
+    if (!b.n_sent) return;
+    uint32_t blocks = (b.n_sent + 8 * VBT_SENT_PER_WARP - 1) / (8 * VBT_SENT_PER_WARP);
+    k_mark_bounds<<<blocks, 256, 0, st>>>(b);
+}
+
 void launch_candidates(const DictView& d, const Batch& b, uint32_t max_slots, cudaStream_t st) {
     if (!max_slots) return;
     uint32_t blocks = (max_slots + 255) / 256;
-    k_candidates<<<blocks, 256, 0, st>>>(d, b);
+    if (b.bnd_dist)
+        k_candidates<true><<<blocks, 256, 0, st>>>(d, b);
+    else
+        k_candidates<false><<<blocks, 256, 0, st>>>(d, b);
 }
 
 void launch_candidate_stats(const DictView& d, const Batch& b, uint32_t max_slots, uint4* stats, cudaStream_t st) {

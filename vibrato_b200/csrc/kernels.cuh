@@ -67,6 +67,9 @@ enum : uint32_t {
     // the batch's output text is larger than the text buffer (sized from a learned text-per-byte ratio in the
     // chunked host pipeline): k_format_write wrote nothing, the engine re-runs the batch with a larger buffer
     kFlagTextOverflow = 32u,
+    // a required boundary list is out of order, past its sentence's end or inside a multi-byte character, or the
+    // boundary offsets themselves are out of order or past n_bnd (k_mark_bounds)
+    kFlagBadBoundary = 64u,
 };
 constexpr uint32_t kFlagsStandDown = kFlagBadOffsets | kFlagSlotsOverflow;
 constexpr uint32_t kPruneMaxChars = 16000;  // (chars + 1) nodes x 65 535 per node < 2^30
@@ -121,6 +124,14 @@ struct Batch {
     // ConnIdCounter (mapper.rs:87-104) over internal ids, or nullptr: lid_count[num_left], rid_count[num_right]
     unsigned long long* lid_count;
     unsigned long long* rid_count;
+    // Required boundaries (bounded batches only; bnd_dist == nullptr otherwise).  Sentence s's boundaries are the
+    // sentence-relative byte offsets bnd[bnd_off[s] .. bnd_off[s+1]); k_mark_bounds turns them into bnd_dist[slot] =
+    // (character position of the first boundary after this one, or the sentence's length) - this position, the
+    // lim(sw) - sw that k_candidates<true> obeys.
+    const unsigned long long* bnd_off;  // n_sent + 1
+    const uint32_t* bnd;
+    unsigned long long n_bnd;  // entries behind bnd: no offset may exceed it
+    uint32_t* bnd_dist;        // per slot, written by k_mark_bounds
 };
 
 // Output stage: what `tokenize` prints per sentence (tokenize/src/main.rs:83-127), produced on the device;
@@ -165,6 +176,10 @@ void launch_field_table_write(const DictView& d, const FieldTableArgs& a, cudaSt
 
 void launch_count_chars(const Batch& b, cudaStream_t st);
 void launch_decode(const DictView& d, const Batch& b, cudaStream_t st);
+// Bounded batches (b.bnd_dist != nullptr): writes bnd_dist from the boundary lists after launch_decode and
+// validates them (kFlagBadBoundary).
+void launch_mark_bounds(const Batch& b, cudaStream_t st);
+// b.bnd_dist != nullptr selects the bounded instantiation of k_candidates: no candidate crosses a marked boundary.
 void launch_candidates(const DictView& d, const Batch& b, uint32_t max_slots, cudaStream_t st);
 // Counted runs only: per-slot {M | walks << 24, T, P, W} of SURVEY.md §8(d), summed by K3 over visited positions.
 void launch_candidate_stats(const DictView& d, const Batch& b, uint32_t max_slots, uint4* stats, cudaStream_t st);
@@ -206,6 +221,7 @@ struct SmallBatchOut {
 // (the hard bound), so only the candidate pool (b.cand_cap; ends_hot / ends_cold need cand_cap + n_sent + 1
 // entries) and the text (f.text_cap) can overflow: kFlagPoolOverflow / kFlagTextOverflow, the outputs are then void.
 // f.tok_off / f.tokens must equal b.tok_off / b.tokens; f.sent_len needs n_sent entries, f.text_off n_sent + 1.
+// A bounded batch (b.bnd_dist != nullptr, per-slot like the other arrays) is marked and validated inside the block.
 void launch_small_batch(const DictView& d, const Batch& b, const FormatArgs& f, SmallBatchOut* out, cudaStream_t st);
 
 }  // namespace vbt

@@ -223,23 +223,27 @@ class MultiEngine final : public Engine {
             delete r;
         }
         pinned_free(h_off_);
+        pinned_free(h_bnd_off_);
+        pinned_free(h_bnd_);
         cudaSetDevice(dev_[0]);
         if (gather_tokens_) cudaFree(gather_tokens_);
         if (gather_off_) cudaFree(gather_off_);
     }
 
     // ---- host batches --------------------------------------------------------------------------------
-    HostResult* run_host(const char* utf8, const uint64_t* byte_off, uint64_t n_sent) override {
+    HostResult* run_host(const char* utf8, const uint64_t* byte_off, uint64_t n_sent, const Bounds* bnd) override {
         const int n = int(dev_.size());
         if (n == 1) {  // nothing to split: the device's own chunked, overlapped host pipeline
-            HostResult* r = eng_[0]->run_host(utf8, byte_off, n_sent);
+            HostResult* r = eng_[0]->run_host(utf8, byte_off, n_sent, bnd);
             collect_stats();
             return r;
         }
         const std::vector<uint64_t> cut = split_by_bytes(byte_off, n_sent, n);
         std::vector<uint64_t> n_tok(n, 0), n_text(n, 0);
         run_on_all([&](int i) {
-            n_tok[i] = eng_[i]->run_shard(utf8, byte_off + cut[i], cut[i + 1] - cut[i], -1, text_ ? &n_text[i] : nullptr);
+            const Bounds sb = shard_bounds(bnd, cut[i]);
+            n_tok[i] = eng_[i]->run_shard(utf8, byte_off + cut[i], cut[i + 1] - cut[i], -1, text_ ? &n_text[i] : nullptr,
+                                          bnd ? &sb : nullptr);
         });
         std::vector<uint64_t> base(n + 1, 0), text_base(n + 1, 0);
         for (int i = 0; i < n; ++i) {
@@ -267,10 +271,10 @@ class MultiEngine final : public Engine {
 
     // ---- device-resident batches: input on the first device, results gathered back to it ------------------
     void run_device(uint64_t d_utf8, uint64_t d_byte_off, uint64_t n_sent, uint64_t n_bytes, uint64_t* d_tok_off,
-                    uint64_t* d_tokens, uint64_t* n_tokens) override {
+                    uint64_t* d_tokens, uint64_t* n_tokens, const Bounds* bnd) override {
         const int n = int(dev_.size());
         if (n == 1) {
-            eng_[0]->run_device(d_utf8, d_byte_off, n_sent, n_bytes, d_tok_off, d_tokens, n_tokens);
+            eng_[0]->run_device(d_utf8, d_byte_off, n_sent, n_bytes, d_tok_off, d_tokens, n_tokens, bnd);
             collect_stats();
             return;
         }
@@ -284,11 +288,23 @@ class MultiEngine final : public Engine {
         }
         CK(cudaMemcpyAsync(h_off_, reinterpret_cast<const void*>(d_byte_off), (n_sent + 1) * 8, cudaMemcpyDeviceToHost, stream_[0]));
         CK(cudaStreamSynchronize(stream_[0]));
+        // boundary lists: to the host as well, and from there to every shard like those of a host batch (they are
+        // validated on the devices)
+        Bounds hb;
+        if (bnd) {
+            grow_pinned(h_bnd_off_, h_bnd_off_cap_, (n_sent + 1) * 8);
+            grow_pinned(h_bnd_, h_bnd_cap_, bnd->n * 4 + 4);
+            CK(cudaMemcpyAsync(h_bnd_off_, bnd->off, (n_sent + 1) * 8, cudaMemcpyDeviceToHost, stream_[0]));
+            if (bnd->n) CK(cudaMemcpyAsync(h_bnd_, bnd->bnd, bnd->n * 4, cudaMemcpyDeviceToHost, stream_[0]));
+            CK(cudaStreamSynchronize(stream_[0]));
+            hb = Bounds{static_cast<const uint64_t*>(h_bnd_off_), static_cast<const uint32_t*>(h_bnd_), bnd->n};
+        }
         const std::vector<uint64_t> cut = split_by_bytes(h_off_, n_sent, n);
         std::vector<uint64_t> n_tok(n, 0);
         run_on_all([&](int i) {
+            const Bounds sb = shard_bounds(bnd ? &hb : nullptr, cut[i]);
             n_tok[i] = eng_[i]->run_shard(reinterpret_cast<const char*>(d_utf8), h_off_ + cut[i], cut[i + 1] - cut[i],
-                                          dev_[0], nullptr);  // token-only, like the single-device entry point
+                                          dev_[0], nullptr, bnd ? &sb : nullptr);  // token-only, like the single-device entry point
         });
         std::vector<uint64_t> base(n + 1, 0);
         for (int i = 0; i < n; ++i) base[i + 1] = base[i] + n_tok[i];
@@ -382,7 +398,9 @@ class MultiEngine final : public Engine {
             for (uint32_t i = 0; i < nr; ++i) rid[i] += r[i];
         }
     }
-    uint64_t run_shard(const char*, const uint64_t*, uint64_t, int, uint64_t*) override { throw Error(kInternal, "not a shard engine"); }
+    uint64_t run_shard(const char*, const uint64_t*, uint64_t, int, uint64_t*, const Bounds*) override {
+        throw Error(kInternal, "not a shard engine");
+    }
     void fetch_shard(uint64_t*, void*, uint64_t, bool, uint64_t*, char*, uint64_t) override {
         throw Error(kInternal, "not a shard engine");
     }
@@ -411,6 +429,18 @@ class MultiEngine final : public Engine {
             cut[i] = std::max<uint64_t>(cut[i - 1], std::min<uint64_t>(uint64_t(p - off), n_sent));
         }
         return cut;
+    }
+
+    static void grow_pinned(void*& p, size_t& cap, size_t bytes) {
+        if (bytes <= cap) return;
+        pinned_free(p);
+        cap = size_t(double(bytes) * 1.25) + 64;
+        p = pinned_alloc(cap);
+    }
+
+    // The boundary lists of the shard that starts at sentence `first` (host memory): its slice of the offsets.
+    static Bounds shard_bounds(const Bounds* bnd, uint64_t first) {
+        return bnd ? Bounds{bnd->off + first, bnd->bnd, bnd->n} : Bounds{};
     }
 
     // One host thread per device (the calling thread takes the first): each call blocks on its own device.
@@ -509,6 +539,9 @@ class MultiEngine final : public Engine {
     bool fixed_mode_ = false;  // "output_mode" 1-3 is on
     uint64_t* h_off_ = nullptr;  // pinned
     size_t h_off_cap_ = 0;
+    void* h_bnd_off_ = nullptr;  // pinned: the boundary lists of a device-resident batch, cut into shards on the host
+    void* h_bnd_ = nullptr;
+    size_t h_bnd_off_cap_ = 0, h_bnd_cap_ = 0;
     void* gather_tokens_ = nullptr;
     void* gather_off_ = nullptr;
     size_t gather_tok_cap_ = 0, gather_off_cap_ = 0;
