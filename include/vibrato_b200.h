@@ -317,6 +317,27 @@ int32_t vbt_tokenizer_set_output_format(vbt_tokenizer *t, const char *node, size
  * lid_count[num_left], rid_count[num_right].  Pass NULL arrays to query the sizes only. */
 int32_t vbt_connid_counts(vbt_tokenizer *t, uint64_t *lid_count, uint64_t *rid_count, uint32_t *num_left,
                           uint32_t *num_right);
+/* Marginal probabilities, computed on the device by forward-backward over each sentence's lattice: the nodes the
+ * tokenizer inserts (ignore_space, max_grouping_len, the user lexicon and required boundaries included) plus BOS and
+ * EOS.  Node k of row ends[p] has an edge to every candidate c starting at p, of cost conn(k.right, c.left) +
+ * word_cost(c), and every node of the last row an edge to EOS of cost conn(k.right, 0) (conn: the dictionary's
+ * connector value, the matrix i16 or the Raw / Dual i32 sum).  A path's cost is the exact (unwrapped) sum of its
+ * edges; P(path) = exp(-theta * cost) / Z over all BOS -> EOS paths.  A token's marginal is the sum of P over the
+ * paths through its lattice node; a sentence's path_prob = exp(-theta * min cost) / Z, the probability of one
+ * minimum-cost path (1 for an empty sentence).  Nodes without a path to EOS have probability 0.
+ * Where the tokenizer's own i32 path costs wrap (very long sentences, extreme Raw / Dual dictionaries) the tokens
+ * keep the reference's arithmetic while the probabilities stay the exact-cost ones above.  Whether this theta has
+ * the scale of MeCab's -theta is not verified.
+ * theta > 0 switches them on, 0 off; negative, NaN or infinite: VBT_ERR_INVALID_ARGUMENT.  While on, batches take
+ * two more kernel launches (booked under the "viterbi" stage) and the "small_batch" route steps aside.  The
+ * probabilities are bit-identical across routes, chunking, sentence order and K3 variants. */
+int32_t vbt_tokenizer_set_marginals(vbt_tokenizer *t, double theta);
+/* token_prob[n_tokens] (at the tokens' own indices) and path_prob[n_sent] of a result tokenised with marginals on;
+ * owned by the result.  VBT_ERR_INVALID_ARGUMENT for a result made without them. */
+int32_t vbt_result_marginals(const vbt_result *r, const float **token_prob, const float **path_prob);
+/* Device addresses (float32) of the marginals of the last vbt_tokenize_batch_device{,_bounded} call, valid until the
+ * next call; VBT_ERR_INVALID_ARGUMENT when it ran without marginals. */
+int32_t vbt_last_device_marginals(const vbt_tokenizer *t, uint64_t *d_token_prob, uint64_t *d_path_prob);
 /* Launch the kernels on a caller-owned CUDA stream (a cudaStream_t passed as an integer; 0 restores
  * the tokenizer's own stream), so callers can bracket batches with their own events. */
 int32_t vbt_tokenizer_set_stream(vbt_tokenizer *t, uint64_t stream);

@@ -54,6 +54,8 @@ extern "C" {
                                        eos: *const c_char, eos_len: usize) -> i32;
     fn vbt_result_text(r: *const vbt_result, text_offsets: *mut *const u64, text: *mut *const c_char,
                        n_bytes: *mut u64) -> i32;
+    fn vbt_tokenizer_set_marginals(t: *mut vbt_tokenizer, theta: f64) -> i32;
+    fn vbt_result_marginals(r: *const vbt_result, token_prob: *mut *const f32, path_prob: *mut *const f32) -> i32;
     fn vbt_evaluate(d: *const vbt_dict, t: *mut vbt_tokenizer, corpus: *const c_char, len: usize,
                     feature_indices: *const u64, n_indices: usize, num_ref: *mut u64, num_sys: *mut u64,
                     num_cor: *mut u64) -> i32;
@@ -244,6 +246,11 @@ impl Tokenizer {
     pub fn small_batch(&self, n: u32) -> Result<()> {
         check(unsafe { vbt_tokenizer_set_option(self.handle(), b"small_batch\0".as_ptr() as *const c_char, n as i64) })
     }
+    /// Marginal probabilities at temperature `theta` > 0 (0 = off; see `vbt_tokenizer_set_marginals`): batches
+    /// tokenised afterwards carry `BatchResult::marginals`.  Set it before an output format that prints `%pP`.
+    pub fn marginals(&self, theta: f64) -> Result<()> {
+        check(unsafe { vbt_tokenizer_set_marginals(self.handle(), theta) })
+    }
     /// The loop of the `evaluate` tool (evaluate/src/main.rs:61-138): (num_ref, num_sys, num_cor).
     pub fn evaluate(&self, corpus: &str, feature_indices: &[usize]) -> Result<(u64, u64, u64)> {
         let idx: Vec<u64> = feature_indices.iter().map(|&i| i as u64).collect();
@@ -276,6 +283,17 @@ impl BatchResult {
             vbt_result_view(self.r, &mut to, &mut tt, &mut ns, &mut nt);
             Ok((std::slice::from_raw_parts(o, ns as usize + 1),
                 std::str::from_utf8_unchecked(std::slice::from_raw_parts(t as *const u8, n as usize))))
+        }
+    }
+    /// (per-token marginal, per-sentence best-path probability); an error for a batch tokenised without marginals.
+    pub fn marginals(&self) -> Result<(&[f32], &[f32])> {
+        let (mut tp, mut pp) = (std::ptr::null(), std::ptr::null());
+        check(unsafe { vbt_result_marginals(self.r, &mut tp, &mut pp) })?;
+        let (mut o, mut t, mut ns, mut nt) = (std::ptr::null(), std::ptr::null(), 0u64, 0u64);
+        unsafe {
+            vbt_result_view(self.r, &mut o, &mut t, &mut ns, &mut nt);
+            let s = |p: *const f32, n: u64| if n == 0 { &[][..] } else { std::slice::from_raw_parts(p, n as usize) };
+            Ok((s(tp, nt), s(pp, ns)))
         }
     }
     pub fn view(&self) -> (&[u64], &[vbt_token]) {

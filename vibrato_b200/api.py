@@ -273,9 +273,11 @@ def expand_compact_tokens(compact, tok_offsets, utf8, byte_offsets):
 class BatchResult:
     """Tokens of a batch: `tok_offsets[i]..tok_offsets[i+1]` index `tokens` (TOKEN_DTYPE) for sentence i.  With the
     tokenizer option compact_tokens the device returns 16-byte records (`compact`); `tokens` is then rebuilt on the
-    host from them and the sentences' UTF-8."""
+    host from them and the sentences' UTF-8.  With Tokenizer.marginals(theta) on, `token_probs` (float32[n_tokens])
+    and `path_probs` (float32[n_sent]) hold the marginal of every token and the probability of each sentence's best
+    path; both are None otherwise."""
 
-    def __init__(self, tokenizer, handle, sentences_utf8, byte_offsets, compact=False):
+    def __init__(self, tokenizer, handle, sentences_utf8, byte_offsets, compact=False, marginals=False):
         self._tok = tokenizer
         self._h = handle
         self._free = lib().vbt_result_free
@@ -292,6 +294,15 @@ class BatchResult:
             toks = np.empty(0, dtype=dt)
         self.compact = toks if compact else None
         self.tokens = expand_compact_tokens(toks, self.tok_offsets, sentences_utf8, byte_offsets) if compact else toks
+        self.token_probs = self.path_probs = None
+        if marginals:
+            tp, pp = C.c_void_p(), C.c_void_p()
+            check(lib().vbt_result_marginals(handle, C.byref(tp), C.byref(pp)))
+            f32 = C.POINTER(C.c_float)
+            self.token_probs = (np.ctypeslib.as_array(C.cast(tp, f32), shape=(self.n_tokens,)) if self.n_tokens
+                                else np.empty(0, dtype=np.float32))
+            self.path_probs = (np.ctypeslib.as_array(C.cast(pp, f32), shape=(self.n_sent,)) if self.n_sent
+                               else np.empty(0, dtype=np.float32))
         self._utf8 = sentences_utf8
         self._off = byte_offsets
 
@@ -302,6 +313,9 @@ class BatchResult:
             self.tokens = self.tokens.copy()
             if self.compact is not None:
                 self.compact = self.compact.copy()
+            if self.token_probs is not None:
+                self.token_probs = self.token_probs.copy()
+                self.path_probs = self.path_probs.copy()
             self._free(h)
 
     def __del__(self):
@@ -327,7 +341,8 @@ class BatchResult:
         """Token views of sentence i, in order (Worker::token_iter)."""
         s = bytes(self._utf8[int(self._off[i]):int(self._off[i + 1])])
         a, b = int(self.tok_offsets[i]), int(self.tok_offsets[i + 1])
-        return [Token(self._tok, s, self.tokens[k]) for k in range(a, b)]
+        tp = self.token_probs
+        return [Token(self._tok, s, self.tokens[k], None if tp is None else float(tp[k])) for k in range(a, b)]
 
 
 OUTPUT_MODES = {None: 0, "none": 0, "mecab": 1, "wakati": 2, "detail": 3}  # tokenize/src/main.rs:12-29
@@ -345,6 +360,7 @@ class Tokenizer:
         self._h = None
         self._options = {}  # engine options set so far: replayed when the engine is rebuilt (ignore_space / max_grouping_len)
         self._format = None  # (node, unk, bos, eos) of output_format(), replayed after the options
+        self._theta = 0.0  # marginals(), replayed before the format
         self._stream = 0
         self._counting = False
         self._free = lib().vbt_tokenizer_free
@@ -404,6 +420,8 @@ class Tokenizer:
             # a rebuilt engine starts from defaults: put back what the caller had configured
             for name, value in self._options.items():
                 check(lib().vbt_tokenizer_set_option(h, name.encode(), int(value)))
+            if self._theta:
+                check(lib().vbt_tokenizer_set_marginals(h, self._theta))
             if self._format is not None:
                 self._set_format(h, self._format)
             if self._counting:
@@ -453,7 +471,8 @@ class Tokenizer:
             check(lib().vbt_tokenize_batch_bounded(self.handle(), utf8.ctypes.data if utf8.size else None,
                                                    byte_offsets.ctypes.data, n, bnd_offsets.ctypes.data,
                                                    bnd.ctypes.data if bnd.size else None, C.byref(h)))
-        return BatchResult(self, h, utf8, byte_offsets, compact=bool(self._options.get("compact_tokens", 0)))
+        return BatchResult(self, h, utf8, byte_offsets, compact=bool(self._options.get("compact_tokens", 0)),
+                           marginals=self._theta > 0)
 
     def tokenize_batch_device(self, d_utf8, d_byte_offsets, n_sent, n_bytes, d_bnd_offsets=None, d_bnd=None, n_bnd=0):
         """Device-resident variant: addresses in, (d_tok_offsets, d_tokens, n_tokens) out.  With d_bnd_offsets
@@ -468,6 +487,23 @@ class Tokenizer:
                                                           int(n_bytes), int(d_bnd_offsets), int(d_bnd or 0),
                                                           int(n_bnd), C.byref(a), C.byref(b), C.byref(n)))
         return a.value, b.value, n.value
+
+    def last_device_marginals(self):
+        """-> (d_token_probs, d_path_probs): device addresses (float32[n_tokens], float32[n_sent]) of the marginals of
+        the last tokenize_batch_device call, valid until the next call."""
+        a, b = C.c_uint64(), C.c_uint64()
+        check(lib().vbt_last_device_marginals(self.handle(), C.byref(a), C.byref(b)))
+        return a.value, b.value
+
+    def marginals(self, theta):
+        """Marginal probabilities at temperature `theta` (> 0; None or 0 switches them off): P(path) is proportional
+        to exp(-theta * cost(path)) over every BOS -> EOS path of the lattice, a token's marginal sums P over the
+        paths through its node.  Results then carry BatchResult.token_probs / path_probs and Token.prob().  The tokens
+        do not change; the "small_batch" route steps aside while they are on.  Definition: include/vibrato_b200.h."""
+        theta = 0.0 if theta is None else float(theta)
+        check(lib().vbt_tokenizer_set_marginals(self.handle(), theta))
+        self._theta = theta
+        return self
 
     # connection-id statistics (worker.rs:77-103) ---------------------------------------------------
     def init_connid_counter(self):
@@ -599,12 +635,13 @@ class Tokenizer:
 class Token:
     """vibrato::token::Token (token.rs:8-92)."""
 
-    __slots__ = ("_tok", "_sent", "_r")
+    __slots__ = ("_tok", "_sent", "_r", "_p")
 
-    def __init__(self, tokenizer, sentence_bytes, rec):
+    def __init__(self, tokenizer, sentence_bytes, rec, prob=None):
         self._tok = tokenizer
         self._sent = sentence_bytes
         self._r = rec
+        self._p = prob
 
     def range_char(self):
         return range(int(self._r["start_char"]), int(self._r["end_char"]))
@@ -637,6 +674,12 @@ class Token:
     def total_cost(self):
         return int(self._r["total_cost"])
 
+    def prob(self):
+        """The token's marginal probability (Tokenizer.marginals)."""
+        if self._p is None:
+            raise VibratoError(1, "no marginals: switch them on with Tokenizer.marginals(theta) before tokenising")
+        return self._p
+
 
 class Worker:
     """vibrato::tokenizer::worker::Worker (worker.rs:13-74): the one-sentence loop of
@@ -658,7 +701,9 @@ class Worker:
         if not self._sent:  # worker.rs:50-52
             return
         res = self._tok.tokenize_batch([self._sent], boundaries=None if self._bounds is None else [self._bounds])
-        self._tokens = [Token(self._tok, self._sent, r.copy()) for r in res.tokens]
+        tp = res.token_probs
+        self._tokens = [Token(self._tok, self._sent, r.copy(), None if tp is None else float(tp[k]))
+                        for k, r in enumerate(res.tokens)]
         res.close()
 
     def num_tokens(self):

@@ -3,6 +3,7 @@
 // Lines are shipped in batches; output order and content equal the per-line loop of main.rs:78-128.
 #include <unistd.h>
 
+#include <cstdlib>
 #include <cstring>
 
 #include "cli_common.hpp"
@@ -19,7 +20,9 @@ static void usage() {
                  "         [--devices 0,1,..]          (spread every batch over these GPUs)\n"
                  "         [--batch-lines N]           (lines per batch when stdin is not a terminal; default 65536)\n"
                  "         [--boundary-marker C]       (an ASCII byte other than newline: removed from every line, it\n"
-                 "                                      marks a required token boundary where it stood)\n");
+                 "                                      marks a required token boundary where it stood)\n"
+                 "         [-m|--marginal -t|--theta F] (marginal probabilities at temperature F > 0: -F may print\n"
+                 "                                      each token's with %%pP; -O output is unchanged)\n");
 }
 
 int main(int argc, char** argv) {
@@ -30,6 +33,8 @@ int main(int argc, char** argv) {
     std::string node_format, unk_format, bos_format, eos_format;
     bool has_node = false, has_unk = false, has_bos = false, has_eos = false;
     std::string marker;
+    bool marginal = false, has_theta = false;
+    double theta = 0;
     for (int i = 1; i < argc; ++i) {
         std::string a = argv[i];
         auto next = [&]() -> std::string {
@@ -52,6 +57,17 @@ int main(int argc, char** argv) {
         else if (a == "--bos-format") bos_format = next(), has_bos = true;
         else if (a == "--eos-format") eos_format = next(), has_eos = true;
         else if (a == "--boundary-marker") marker = next();
+        else if (a == "-m" || a == "--marginal") marginal = true;
+        else if (a == "-t" || a == "--theta") {
+            const std::string v = next();
+            char* end = nullptr;
+            theta = std::strtod(v.c_str(), &end);
+            if (v.empty() || *end) {
+                usage();
+                return 2;
+            }
+            has_theta = true;
+        }
         else {
             usage();
             return 2;
@@ -59,7 +75,9 @@ int main(int argc, char** argv) {
     }
     // the formats are rendered by the device only; --unk/bos/eos-format complete -F
     const bool bounded = !marker.empty();
+    // -m needs --theta, and --theta belongs to -m
     if (batch_lines_arg == 0 || (has_node && format_on == "host") || (!has_node && (has_unk || has_bos || has_eos)) ||
+        marginal != has_theta ||
         (bounded && (marker.size() != 1 || marker[0] == '\n' || (marker[0] & 0x80)))) {
         usage();
         return 2;
@@ -79,6 +97,7 @@ int main(int argc, char** argv) {
         }
         Tokenizer tokenizer =
             Tokenizer(std::move(dict)).ignore_space(ignore_space).max_grouping_len(max_grouping_len).devices(devices);
+        if (marginal) tokenizer.marginals(theta);  // before -F, which may print %pP
         if (has_node) {
             const std::string_view node = node_format, unk = unk_format, bos = bos_format, eos = eos_format;
             tokenizer.output_format(&node, has_unk ? &unk : nullptr, has_bos ? &bos : nullptr, has_eos ? &eos : nullptr);

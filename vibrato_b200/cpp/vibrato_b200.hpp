@@ -13,6 +13,7 @@
 
 #include <algorithm>
 #include <cstdint>
+#include <limits>
 #include <memory>
 #include <stdexcept>
 #include <string>
@@ -149,6 +150,18 @@ class BatchResult {
         check(vbt_result_text(r_.get(), text_offsets, &p, &n));
         return {p, size_t(n)};
     }
+    // Marginal probabilities (Tokenizer::marginals before the batch): float per token, at the tokens' indices, and
+    // the best path's probability per sentence.  Throws on a result made without them.
+    const float* token_probs() const {
+        const float* tp = nullptr;
+        check(vbt_result_marginals(r_.get(), &tp, nullptr));
+        return tp;
+    }
+    const float* path_probs() const {
+        const float* pp = nullptr;
+        check(vbt_result_marginals(r_.get(), nullptr, &pp));
+        return pp;
+    }
 
    private:
     std::unique_ptr<vbt_result, void (*)(vbt_result*)> r_;
@@ -227,6 +240,19 @@ class Tokenizer {
     // Batches of at most n sentences and 16 KiB run in one kernel launch (k_small_batch), with the same tokens and
     // text; counted runs keep the usual route.  0 = off (the default).
     void small_batch(uint32_t n = 64) const { check(vbt_tokenizer_set_option(handle(), "small_batch", int64_t(n))); }
+    // Marginal probabilities at temperature theta > 0 (0 = off; see vbt_tokenizer_set_marginals): BatchResult::
+    // token_probs / path_probs, Token::prob().  Set it before an output format that prints %pP.
+    void marginals(double theta) const {
+        check(vbt_tokenizer_set_marginals(handle(), theta));
+        marginals_ = theta > 0;
+    }
+    // Device addresses {token_prob, path_prob} (float) of the last tokenize_batch_device call, valid until the next.
+    std::pair<uint64_t, uint64_t> last_device_marginals() const {
+        uint64_t tp = 0, pp = 0;
+        check(vbt_last_device_marginals(handle(), &tp, &pp));
+        return {tp, pp};
+    }
+    bool has_marginals() const { return marginals_; }
     // Worker::init_connid_counter / update_connid_counts / compute_connid_probs (worker.rs:77-103): after
     // init_connid_counter() every batch is counted, an empty sentence counting nothing
     void init_connid_counter() const { check(vbt_tokenizer_set_option(handle(), "connid_counting", 1)); }
@@ -281,12 +307,15 @@ class Tokenizer {
     std::vector<int32_t> devices_;
     bool ignore_space_ = false;
     uint64_t max_grouping_len_ = 0;
+    mutable bool marginals_ = false;
     mutable std::shared_ptr<vbt_tokenizer> h_;
 };
 
 class Token {  // token.rs:8-92
    public:
-    Token(const Tokenizer* t, std::string_view sentence, vbt_token rec) : t_(t), s_(sentence), r_(rec) {}
+    // prob: the token's marginal probability, or NaN when the tokenizer computes none
+    Token(const Tokenizer* t, std::string_view sentence, vbt_token rec, float prob = std::numeric_limits<float>::quiet_NaN())
+        : t_(t), s_(sentence), r_(rec), p_(prob) {}
     std::pair<size_t, size_t> range_char() const { return {r_.start_char, r_.end_char}; }
     std::pair<size_t, size_t> range_byte() const { return {r_.start_byte, r_.end_byte}; }
     std::string_view surface() const { return s_.substr(r_.start_byte, r_.end_byte - r_.start_byte); }
@@ -297,6 +326,11 @@ class Token {  // token.rs:8-92
     uint16_t right_id() const { return param().r; }
     int16_t word_cost() const { return param().c; }
     int32_t total_cost() const { return r_.total_cost; }
+    float prob() const {  // Tokenizer::marginals
+        if (p_ != p_)
+            throw VibratoError(VBT_ERR_INVALID_ARGUMENT, "no marginals: switch them on with Tokenizer::marginals before tokenising");
+        return p_;
+    }
 
    private:
     struct P {
@@ -311,6 +345,7 @@ class Token {  // token.rs:8-92
     const Tokenizer* t_;
     std::string_view s_;
     vbt_token r_;
+    float p_;
 };
 
 class Worker {  // worker.rs:13-74
@@ -335,9 +370,13 @@ class Worker {  // worker.rs:13-74
         BatchResult r = bounded_ ? t_->tokenize_batch(sent_.data(), off, 1, boff, bnd_.data())
                                  : t_->tokenize_batch(sent_.data(), off, 1);
         toks_.assign(r.tokens(), r.tokens() + r.n_tokens());
+        probs_.clear();
+        if (t_->has_marginals() && r.n_tokens()) probs_.assign(r.token_probs(), r.token_probs() + r.n_tokens());
     }
     size_t num_tokens() const { return toks_.size(); }
-    Token token(size_t i) const { return Token(t_, sent_, toks_[i]); }
+    Token token(size_t i) const {
+        return probs_.empty() ? Token(t_, sent_, toks_[i]) : Token(t_, sent_, toks_[i], probs_[i]);
+    }
 
    private:
     const Tokenizer* t_;
@@ -345,6 +384,7 @@ class Worker {  // worker.rs:13-74
     std::vector<uint32_t> bnd_;
     bool bounded_ = false;
     std::vector<vbt_token> toks_;
+    std::vector<float> probs_;
 };
 
 inline Worker Tokenizer::new_worker() const { return Worker(this); }

@@ -562,8 +562,34 @@ int32_t vbt_tokenizer_set_output_format(vbt_tokenizer* t, const char* node, size
             return;
         }
         // an empty string may come with any pointer: only NULL means "not given"
-        const vbt::FormatProgram p = vbt::compile_format({node, node_len}, {unk, unk_len}, {bos, bos_len}, {eos, eos_len});
+        // %pP has a value only while the tokenizer computes marginals
+        const vbt::FormatProgram p = vbt::compile_format({node, node_len}, {unk, unk_len}, {bos, bos_len}, {eos, eos_len},
+                                                         t->e->marginals() > 0);
         t->e->set_format(&p);
+    });
+}
+
+int32_t vbt_tokenizer_set_marginals(vbt_tokenizer* t, double theta) {
+    return guarded([&] {
+        need(t, "t");
+        t->e->set_marginals(theta);
+    });
+}
+
+int32_t vbt_result_marginals(const vbt_result* r, const float** token_prob, const float** path_prob) {
+    return guarded([&] {
+        need(r, "r");
+        if (!r->r->has_marg)
+            throw vbt::Error(vbt::kInvalidArgument, "no marginals: switch them on with vbt_tokenizer_set_marginals before tokenising");
+        if (token_prob) *token_prob = r->r->token_prob;
+        if (path_prob) *path_prob = r->r->path_prob;
+    });
+}
+
+int32_t vbt_last_device_marginals(const vbt_tokenizer* t, uint64_t* d_token_prob, uint64_t* d_path_prob) {
+    return guarded([&] {
+        need(t, "t");
+        t->e->device_marginals(d_token_prob, d_path_prob);
     });
 }
 

@@ -6,6 +6,7 @@
 #include <cub/iterator/transform_input_iterator.cuh>
 
 #include <algorithm>
+#include <cmath>
 #include <iterator>
 #include <cstring>
 #include <string>
@@ -146,11 +147,12 @@ struct Workspace {  // every per-(chunk of a)-batch device array; two of them le
     DevBuf n_slots, slot_off, eos, n_tok, code_sys, code_usr, cinfo, groupable, byte_pos, info, info_ex, ends_cnt,
         ends_meta, cand, ends_hot, ends_cold, scan_tmp, stats, iota, sort_keys, order;
     DevBuf bnd_dist;  // bounded batches only: Batch::bnd_dist
+    DevBuf m_fill, m_ncand, m_cand_entry, m_R, m_ab, m_r_eos, m_a_eos;  // marginals only: MargArgs
     cudaStream_t stream = nullptr;
     void release() {
         for (DevBuf* b : {&n_slots, &slot_off, &eos, &n_tok, &code_sys, &code_usr, &cinfo, &groupable, &byte_pos, &info,
                           &info_ex, &ends_cnt, &ends_meta, &cand, &ends_hot, &ends_cold, &scan_tmp, &stats, &iota,
-                          &sort_keys, &order, &bnd_dist})
+                          &sort_keys, &order, &bnd_dist, &m_fill, &m_ncand, &m_cand_entry, &m_R, &m_ab, &m_r_eos, &m_a_eos})
             b->release();
     }
 };
@@ -166,6 +168,8 @@ struct DevBounds {
 struct OutSlot {  // where one (chunk of a) batch leaves its results; two of them alternate in chunked runs
     DevBuf tok_off, tokens, ctrl;
     DevBuf sent_len, text_off, text;  // output stage (k_format_*)
+    DevBuf token_prob, path_prob;     // marginals
+    bool marg = false;                // the (chunk of a) batch in this slot was run with marginals
     Control* h_ctrl = nullptr;
     cudaEvent_t ev[kNumStages + 1];
     cudaEvent_t done = nullptr, drained = nullptr;
@@ -317,7 +321,8 @@ class EngineImpl final : public Engine {
         cudaStreamSynchronize(in_stream_);
         cudaStreamSynchronize(out_stream_);
         for (auto& o : out_) {
-            for (DevBuf* b : {&o.tok_off, &o.tokens, &o.ctrl, &o.sent_len, &o.text_off, &o.text}) b->release();
+            for (DevBuf* b : {&o.tok_off, &o.tokens, &o.ctrl, &o.sent_len, &o.text_off, &o.text, &o.token_prob, &o.path_prob})
+                b->release();
             pinned_free(o.h_ctrl);
             for (auto& ev : o.ev) cudaEventDestroy(ev);
             cudaEventDestroy(o.done);
@@ -349,6 +354,8 @@ class EngineImpl final : public Engine {
             pinned_free(r->tokens);
             pinned_free(r->text_off);
             pinned_free(r->text);
+            pinned_free(r->token_prob);
+            pinned_free(r->path_prob);
             delete r;
         }
         cudaStreamDestroy(own_stream_);
@@ -416,6 +423,8 @@ class EngineImpl final : public Engine {
         clear_format();
         if (!p) return;
         if (tok_bytes_ != 24) throw Error(kInvalidArgument, "compact_tokens and output formats exclude each other");
+        if ((p->uses & kUsesProb) && theta_ == 0)
+            throw Error(kInvalidArgument, "%pP needs marginals: switch them on before setting the format");
         try {
             fmt_prog_.ensure(sizeof(FormatProgram));
             CK(cudaMemcpy(fmt_prog_.p, p, sizeof(FormatProgram), cudaMemcpyHostToDevice));
@@ -425,8 +434,23 @@ class EngineImpl final : public Engine {
             throw;
         }
         output_mode_ = kOutFormat;
+        fmt_uses_ = p->uses;
         text_per_sent_ = p->per_sentence;
         text_per_byte_[kOutFormat] = kFormatTextPerByte;  // learned anew for every format
+    }
+    void set_marginals(double theta) override {
+        if (!(theta >= 0) || !std::isfinite(theta))
+            throw Error(kInvalidArgument, "the marginals' theta must be a finite number >= 0 (0 switches them off)");
+        if (theta == 0 && output_mode_ == kOutFormat && (fmt_uses_ & kUsesProb))
+            throw Error(kInvalidArgument, "the output format prints %pP: change the format before switching marginals off");
+        cudaStreamSynchronize(stream_);
+        theta_ = theta;
+    }
+    double marginals() const override { return theta_; }
+    void device_marginals(uint64_t* d_token_prob, uint64_t* d_path_prob) const override {
+        if (!dev_marg_) throw Error(kInvalidArgument, "the last device-resident call ran without marginals");
+        if (d_token_prob) *d_token_prob = reinterpret_cast<uint64_t>(out_[0].token_prob.p);
+        if (d_path_prob) *d_path_prob = reinterpret_cast<uint64_t>(out_[0].path_prob.p);
     }
     void set_stream(uint64_t stream) override {
         cudaStreamSynchronize(stream_);
@@ -455,11 +479,13 @@ class EngineImpl final : public Engine {
         if (bnd && bnd->n == 0 && device_offsets_zero(bnd->off, n_sent)) bnd = nullptr;  // no boundary at all
         DevBounds bd;
         if (bnd) bd = DevBounds{reinterpret_cast<const unsigned long long*>(bnd->off), bnd->bnd, bnd->n};
+        dev_marg_ = false;
         run_whole(reinterpret_cast<const uint8_t*>(d_utf8), reinterpret_cast<const unsigned long long*>(d_byte_off),
                   uint32_t(n_sent), n_bytes, bd);
         *d_tok_off = reinterpret_cast<uint64_t>(out_[0].tok_off.p);
         *d_tokens = reinterpret_cast<uint64_t>(out_[0].tokens.p);
         *n_tokens = out_[0].h_ctrl->n_tokens;
+        dev_marg_ = out_[0].marg;
     }
 
     // Host path.  Large batches are cut into chunks that flow through three streams: the H2D copy of
@@ -489,7 +515,8 @@ class EngineImpl final : public Engine {
         const uint32_t chunk = chunk_sentences_;
         const bool chunked = chunk > 0 && n_sent > chunk + chunk / 2;
         const bool fmt = output_mode_ != kOutNone;
-        if (small_batch_ && n_sent <= small_batch_ && !chunked && n_bytes <= kEagerBytes && !counting_ && !connid_on_ &&
+        // k_small_batch computes no marginals: with them on, small batches take the usual route
+        if (small_batch_ && n_sent <= small_batch_ && !chunked && n_bytes <= kEagerBytes && !counting_ && !connid_on_ && theta_ == 0 &&
             (!bnd || small_bounds_fit(*bnd, n_sent))) {
             if (HostResult* r = run_small(utf8 + first, off, n_sent, n_bytes, bnd)) return r;
             // the batch outgrew the scratch of k_small_batch: it runs again on the route below
@@ -522,6 +549,11 @@ class EngineImpl final : public Engine {
                 HostResult* r = acquire(n_sent, o.h_ctrl->n_tokens);
                 CK(cudaMemcpyAsync(r->tok_off, o.tok_off.p, (size_t(n_sent) + 1) * 8, cudaMemcpyDeviceToHost, stream_));
                 if (r->n_tokens) CK(cudaMemcpyAsync(r->tokens, o.tokens.p, r->n_tokens * tok_bytes_, cudaMemcpyDeviceToHost, stream_));
+                if (r->has_marg) {
+                    if (r->n_tokens)
+                        CK(cudaMemcpyAsync(r->token_prob, o.token_prob.p, r->n_tokens * 4, cudaMemcpyDeviceToHost, stream_));
+                    if (n_sent) CK(cudaMemcpyAsync(r->path_prob, o.path_prob.p, size_t(n_sent) * 4, cudaMemcpyDeviceToHost, stream_));
+                }
                 r->has_text = false;
                 if (fmt) format_text(d_utf8, d_off, n_sent, r);
                 CK(cudaStreamSynchronize(stream_));
@@ -556,6 +588,7 @@ class EngineImpl final : public Engine {
             for (auto& o : out_) {
                 o.tok_off.ensure((size_t(max_chunk_sent) + 1) * 8, 1.25);
                 o.tokens.ensure(size_t(max_chunk_bytes) * 24 + 24, 1.25);
+                ensure_marg_out(o, max_chunk_sent, max_chunk_bytes);
             }
             // a pinned result sized from the learned tokens-per-byte ratio (grown below if short)
             HostResult* r = acquire(n_sent, uint64_t(double(n_bytes) * tok_per_byte_) + 1024);
@@ -635,12 +668,26 @@ class EngineImpl final : public Engine {
                         r->tokens = bigger;
                         r->cap_tok = cap;
                     }
+                    if (r->has_marg && (tok_total + nt) * 4 > r->cap_tprob) {  // the same for the token marginals
+                        CK(cudaStreamSynchronize(out_stream_));
+                        size_t cap = size_t(double((tok_total + nt) * 4) * 1.5) + 4096;
+                        float* bigger = static_cast<float*>(pinned_alloc(cap));
+                        std::memcpy(bigger, r->token_prob, tok_total * 4);
+                        pinned_free(r->token_prob);
+                        r->token_prob = bigger;
+                        r->cap_tprob = cap;
+                    }
                     const bool last = s1 == n_sent;
                     CK(cudaMemcpyAsync(r->tok_off + s0, o.tok_off.p, (size_t(s1 - s0) + (last ? 1 : 0)) * 8,
                                        cudaMemcpyDeviceToHost, out_stream_));
                     if (nt)
                         CK(cudaMemcpyAsync(static_cast<uint8_t*>(r->tokens) + tok_total * tok_bytes_, o.tokens.p, nt * tok_bytes_,
                                            cudaMemcpyDeviceToHost, out_stream_));
+                    if (r->has_marg) {  // at the same offsets as the token records
+                        if (nt) CK(cudaMemcpyAsync(r->token_prob + tok_total, o.token_prob.p, nt * 4, cudaMemcpyDeviceToHost, out_stream_));
+                        if (s1 > s0)
+                            CK(cudaMemcpyAsync(r->path_prob + s0, o.path_prob.p, size_t(s1 - s0) * 4, cudaMemcpyDeviceToHost, out_stream_));
+                    }
                     if (fmt) {
                         if (text_total + nx + 1 > r->cap_text) {  // grown like the token buffer
                             CK(cudaStreamSynchronize(out_stream_));
@@ -765,7 +812,7 @@ class EngineImpl final : public Engine {
         CK(cudaStreamSynchronize(stream_));
     }
     void fetch_shard(uint64_t* h_tok_off, void* h_tokens, uint64_t tok_base, bool last, uint64_t* h_text_off, char* h_text,
-                     uint64_t text_base) override {
+                     uint64_t text_base, float* h_token_prob, float* h_path_prob) override {
         CK(cudaSetDevice(device_));
         OutSlot& o = out_[0];
         if (tok_base)
@@ -774,6 +821,12 @@ class EngineImpl final : public Engine {
         CK(cudaMemcpyAsync(h_tok_off, o.tok_off.p, (size_t(shard_n_sent_) + (last ? 1 : 0)) * 8, cudaMemcpyDeviceToHost, stream_));
         if (o.h_ctrl->n_tokens)
             CK(cudaMemcpyAsync(h_tokens, o.tokens.p, o.h_ctrl->n_tokens * tok_bytes_, cudaMemcpyDeviceToHost, stream_));
+        if (h_token_prob) {
+            if (!o.marg) throw Error(kInternal, "the shard was run without marginals");
+            if (o.h_ctrl->n_tokens)
+                CK(cudaMemcpyAsync(h_token_prob, o.token_prob.p, o.h_ctrl->n_tokens * 4, cudaMemcpyDeviceToHost, stream_));
+            if (shard_n_sent_) CK(cudaMemcpyAsync(h_path_prob, o.path_prob.p, size_t(shard_n_sent_) * 4, cudaMemcpyDeviceToHost, stream_));
+        }
         if (h_text_off) {
             if (!shard_text_) throw Error(kInternal, "the shard was run without its text");
             unsigned long long* text_off = o.text_off.as<unsigned long long>();
@@ -787,6 +840,11 @@ class EngineImpl final : public Engine {
     void shard_outputs(uint64_t* d_tok_off, uint64_t* d_tokens) const override {
         *d_tok_off = reinterpret_cast<uint64_t>(out_[0].tok_off.p);
         *d_tokens = reinterpret_cast<uint64_t>(out_[0].tokens.p);
+    }
+    void shard_marginals(uint64_t* d_token_prob, uint64_t* d_path_prob) const override {
+        if (!out_[0].marg) throw Error(kInternal, "the shard was run without marginals");
+        *d_token_prob = reinterpret_cast<uint64_t>(out_[0].token_prob.p);
+        *d_path_prob = reinterpret_cast<uint64_t>(out_[0].path_prob.p);
     }
     int device() const override { return device_; }
     uint32_t token_bytes() const override { return tok_bytes_; }
@@ -932,7 +990,30 @@ class EngineImpl final : public Engine {
         r->n_tokens = n_tokens;
         r->has_text = false;
         r->token_bytes = tok_bytes_;
+        r->has_marg = theta_ > 0;
+        if (r->has_marg) ensure_marg_host(r, n_sent, n_tokens);
         return r;
+    }
+
+    // Pinned marginal arrays of `r` for n_sent sentences and n_tokens tokens (contents not kept).
+    static void ensure_marg_host(HostResult* r, uint64_t n_sent, uint64_t n_tokens) {
+        if (n_tokens * 4 > r->cap_tprob) {
+            pinned_free(r->token_prob);
+            r->cap_tprob = size_t(double(n_tokens * 4) * 1.25) + 64;
+            r->token_prob = static_cast<float*>(pinned_alloc(r->cap_tprob));
+        }
+        if (n_sent * 4 > r->cap_pprob) {
+            pinned_free(r->path_prob);
+            r->cap_pprob = size_t(double(n_sent * 4) * 1.25) + 64;
+            r->path_prob = static_cast<float*>(pinned_alloc(r->cap_pprob));
+        }
+    }
+
+    // Device marginal outputs of slot `o` for (chunks of) up to n_sent sentences and n_bytes bytes.
+    void ensure_marg_out(OutSlot& o, uint32_t n_sent, uint64_t n_bytes) {
+        if (theta_ == 0) return;
+        o.token_prob.ensure(size_t(n_bytes) * 4 + 4, 1.25);  // a token spans >= 1 byte
+        o.path_prob.ensure((size_t(n_sent) + 1) * 4, 1.25);
     }
 
     // Output stage buffers of slot `o` and scan storage of `w` for (chunks of) up to n_sent sentences.
@@ -962,6 +1043,7 @@ class EngineImpl final : public Engine {
         f.flags = &dc->flags;
         f.text_total = &dc->text_bytes;
         set_mode(f);
+        f.token_prob = (o.marg && (fmt_uses_ & kUsesProb)) ? o.token_prob.as<float>() : nullptr;  // %pP
         CK(cudaMemsetAsync(f.sent_len + n_sent, 0, 8, w.stream));
         launch_format_len(dv_, f, w.stream);
         exclusive_scan(w, f.sent_len, f.text_off, size_t(n_sent) + 1);
@@ -1193,6 +1275,7 @@ class EngineImpl final : public Engine {
         for (DevBuf* b : {&fmt_prog_, &ft_keep_, &ft_off_, &ft_bytes_}) b->release();
         ft_size_ = 0;
         ft_ms_ = 0;
+        fmt_uses_ = 0;
         text_per_sent_ = 4;
         if (output_mode_ == kOutFormat) output_mode_ = kOutNone;
     }
@@ -1288,12 +1371,23 @@ class EngineImpl final : public Engine {
         w.ends_cnt.ensure(ms * 4, 1.25);
         w.ends_meta.ensure(ms * 8, 1.25);
         if (bounded) w.bnd_dist.ensure(ms * 4, 1.25);
+        if (theta_ > 0) {
+            w.m_fill.ensure(ms * 4, 1.25);
+            w.m_ncand.ensure(ms * 4, 1.25);
+            w.m_r_eos.ensure(ns * 8, 1.25);
+            w.m_a_eos.ensure(ns * 8, 1.25);
+        }
         if (counting_) w.stats.ensure(ms * 16, 1.25);
         size_t want_cand = std::max<size_t>(1 << 16, size_t(double(n_bytes) * cand_per_byte_) + 4096);
         want_cand = std::min<size_t>(want_cand, 0xFFFFFFF0ull);
         w.cand.ensure(want_cand * 16);
         w.ends_hot.ensure((want_cand + ns) * 8);
         w.ends_cold.ensure((want_cand + ns) * 16);
+        if (theta_ > 0) {
+            w.m_cand_entry.ensure(want_cand * 4);
+            w.m_R.ensure((want_cand + ns) * 8);
+            w.m_ab.ensure((want_cand + ns) * 16);
+        }
         size_t tmp = 0;  // cub temp storage for the largest scan / sort of this size
         cub::DeviceScan::ExclusiveSum(nullptr, tmp, static_cast<uint32_t*>(nullptr), static_cast<uint32_t*>(nullptr), ms, w.stream);
         w.scan_tmp.ensure(tmp + 1024, 1.5);
@@ -1315,6 +1409,7 @@ class EngineImpl final : public Engine {
             ensure_workspace(ws_[0], n_sent, n_bytes, bd.off != nullptr);
             o.tok_off.ensure((size_t(n_sent) + 1) * 8, 1.25);
             o.tokens.ensure(size_t(n_bytes) * 24 + 24, 1.25);  // a token spans >= 1 character >= 1 byte
+            ensure_marg_out(o, n_sent, n_bytes);
             connid_begin(stream_);
             enqueue(ws_[0], d_utf8, d_off, n_sent, n_bytes, o, nullptr, nullptr, nullptr, nullptr, bd);
             CK(cudaEventSynchronize(o.done));
@@ -1359,8 +1454,12 @@ class EngineImpl final : public Engine {
         // earlier batches (plus slack), and a batch that exceeds it flags itself and is re-run with the hard bound
         const uint32_t hard_slots = uint32_t(n_bytes + n_sent);
         const uint32_t max_slots = uint32_t(std::min<uint64_t>(hard_slots, uint64_t(double(n_bytes) * chars_per_byte_) + n_sent + 4096));
-        const uint32_t cand_cap = uint32_t(std::min<size_t>(
-            w.cand.cap / 16, std::min<size_t>(w.ends_hot.cap / 8 - n_sent - 1, w.ends_cold.cap / 16 - n_sent - 1)));
+        size_t cap_all = std::min<size_t>(w.cand.cap / 16, std::min<size_t>(w.ends_hot.cap / 8 - n_sent - 1, w.ends_cold.cap / 16 - n_sent - 1));
+        const bool marg = theta_ > 0;
+        if (marg)
+            cap_all = std::min<size_t>(cap_all, std::min<size_t>(w.m_cand_entry.cap / 4,
+                                                                 std::min<size_t>(w.m_R.cap / 8, w.m_ab.cap / 16) - n_sent - 1));
+        const uint32_t cand_cap = uint32_t(cap_all);
         Batch b{};
         b.utf8 = d_utf8;
         b.byte_off = d_off;
@@ -1443,6 +1542,22 @@ class EngineImpl final : public Engine {
         exclusive_scan(w, b.ends_cnt, RowMetaOut{b.ends_meta}, size_t(max_slots) + 1);
         CK(cudaEventRecord(o.ev[5], st));
         o.launches += launch_viterbi(dv_, b, counting_ ? w.stats.as<uint4>() : nullptr, lanes_, viterbi_kernel_, st, &o.route);
+        MargArgs m{};
+        o.marg = marg;
+        if (marg) {  // booked with the Viterbi stage; must run before K4a reuses ends_meta
+            m.theta = theta_;
+            m.fill = w.m_fill.as<uint32_t>();
+            m.ncand = w.m_ncand.as<uint32_t>();
+            m.cand_entry = w.m_cand_entry.as<uint32_t>();
+            m.R = w.m_R.as<long long>();
+            m.ab = w.m_ab.as<double2>();
+            m.r_eos = w.m_r_eos.as<long long>();
+            m.a_eos = w.m_a_eos.as<double>();
+            m.path_prob = o.path_prob.as<float>();
+            m.token_prob = o.token_prob.as<float>();
+            launch_marginals(dv_, b, m, st);
+            if (n_sent) o.launches += 2;
+        }
         CK(cudaEventRecord(o.ev[6], st));
         launch_backtrack_count(b, st);
         CK(cudaEventRecord(o.ev[7], st));
@@ -1452,7 +1567,10 @@ class EngineImpl final : public Engine {
             exclusive_scan(w, it, b.tok_off, size_t(n_sent) + 1);
         }
         CK(cudaEventRecord(o.ev[8], st));
-        launch_backtrack_write(b, st);
+        if (marg)
+            launch_backtrack_write_marg(b, m, st);
+        else
+            launch_backtrack_write(b, st);
         k_publish_totals<<<1, 1, 0, st>>>(b.slot_off, b.tok_off, n_sent, dc);
         if (text_base) {  // output stage of a chunk: formatted while its token offsets are still chunk-local
             FormatArgs f = format_offsets(w, d_utf8, d_off, n_sent, o);
@@ -1476,6 +1594,8 @@ class EngineImpl final : public Engine {
         if (eager_sink_) {  // small batch: results leave in the same breath (sized by their upper bound)
             CK(cudaMemcpyAsync(eager_sink_->tok_off, o.tok_off.p, (size_t(n_sent) + 1) * 8, cudaMemcpyDeviceToHost, st));
             if (n_bytes) CK(cudaMemcpyAsync(eager_sink_->tokens, o.tokens.p, size_t(n_bytes) * tok_bytes_, cudaMemcpyDeviceToHost, st));
+            if (marg && n_bytes) CK(cudaMemcpyAsync(eager_sink_->token_prob, o.token_prob.p, size_t(n_bytes) * 4, cudaMemcpyDeviceToHost, st));
+            if (marg && n_sent) CK(cudaMemcpyAsync(eager_sink_->path_prob, o.path_prob.p, size_t(n_sent) * 4, cudaMemcpyDeviceToHost, st));
         }
         CK(cudaEventRecord(o.done, st));
     }
@@ -1534,12 +1654,15 @@ class EngineImpl final : public Engine {
     uint32_t text_per_sent_ = 4;  // "EOS\n"; an output format: what its BOS and EOS print (FormatProgram::per_sentence)
     // output format (set_format): the compiled program and its field table, with the table's size and build time
     DevBuf fmt_prog_, ft_keep_, ft_off_, ft_bytes_;
+    uint32_t fmt_uses_ = 0;  // FormatProgram::uses of the output format
     size_t ft_size_ = 0;
     float ft_ms_ = 0;
     bool dual_stream_ = false;
     int lanes_ = 16;  // fastest on H100 for ~40-character and 512-character sentences alike (DESIGN.md §4)
     uint32_t tok_bytes_ = 24;
     int viterbi_kernel_ = 1;  // 1 = k_viterbi2 with pruning (kernels.cuh)
+    double theta_ = 0;        // marginals' theta, 0 = off (set_marginals)
+    bool dev_marg_ = false;   // the last run_device computed marginals (device_marginals)
     float stage_ms_[kNumStages];
     uint64_t launches_ = 0;
     uint32_t last_route_ = kRouteNone;  // ViterbiRoute of the last successful call (describe())

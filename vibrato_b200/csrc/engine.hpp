@@ -24,6 +24,11 @@ struct HostResult {  // pinned host memory holding one batch's tokens
     char* text = nullptr;
     size_t cap_text_off = 0, cap_text = 0;
     bool has_text = false;
+    // marginals (set_marginals): per token and per sentence, has_marg == false when they are off
+    float* token_prob = nullptr;  // n_tokens
+    float* path_prob = nullptr;   // n_sent
+    size_t cap_tprob = 0, cap_pprob = 0;
+    bool has_marg = false;
 };
 
 // Required token boundaries of a batch (vbt_tokenize_batch_bounded): sentence i's boundaries are the
@@ -71,13 +76,16 @@ class Engine {
                                uint64_t* text_bytes, const Bounds* bnd = nullptr) = 0;
     // fetch_shard: the last shard's token offsets (+ tok_base, n_sent entries, one more when `last`) and token
     // records into host memory (pinned, or it is slow); with h_text_off != nullptr also its text offsets
-    // (+ text_base, same count) and text, which run_shard must have formatted.
+    // (+ text_base, same count) and text, which run_shard must have formatted; with h_token_prob != nullptr also its
+    // marginals (n_tokens and n_sent floats), which it must have computed.
     virtual void fetch_shard(uint64_t* h_tok_off, void* h_tokens, uint64_t tok_base, bool last, uint64_t* h_text_off,
-                             char* h_text, uint64_t text_base) = 0;
+                             char* h_text, uint64_t text_base, float* h_token_prob = nullptr, float* h_path_prob = nullptr) = 0;
     // Device addresses of the last shard's token offsets (uint64[n_sent + 1], already + tok_base after
     // rebase_shard) and token records.
     virtual void rebase_shard(uint64_t tok_base) = 0;
     virtual void shard_outputs(uint64_t* d_tok_off, uint64_t* d_tokens) const = 0;
+    // Device addresses of the last shard's marginals: float token_prob[n_tokens], path_prob[n_sent].
+    virtual void shard_marginals(uint64_t* d_token_prob, uint64_t* d_path_prob) const = 0;
     virtual int device() const = 0;
     virtual uint32_t token_bytes() const = 0;  // 24, or 16 with the "compact_tokens" option
     virtual std::string describe() const = 0;  // JSON: devices, how the dictionary travelled, ...
@@ -92,6 +100,14 @@ class Engine {
     // An output format (format.hpp) in place of "output_mode" 1-3, on every host route; nullptr switches it off.
     // Setting "output_mode" replaces it.  Builds the format's field table on the device.
     virtual void set_format(const FormatProgram* p) = 0;
+    // Marginal probabilities (kernels.cuh MargArgs) at temperature theta > 0 on every route except k_small_batch,
+    // which steps aside while they are on; 0 switches them off.  Results then carry HostResult::token_prob /
+    // path_prob, and run_device leaves them in device memory (device_marginals).
+    virtual void set_marginals(double theta) = 0;
+    virtual double marginals() const = 0;
+    // Device addresses of the last run_device's float token_prob[n_tokens] and path_prob[n_sent]; valid until the
+    // next call.  Throws when that call ran without marginals.
+    virtual void device_marginals(uint64_t* d_token_prob, uint64_t* d_path_prob) const = 0;
     // Launch on a caller-owned CUDA stream (0 restores the engine's own stream).
     virtual void set_stream(uint64_t stream) = 0;
     virtual const float* stage_ms() const = 0;

@@ -14,7 +14,7 @@ namespace {
 
 class Compiler {
    public:
-    explicit Compiler(FormatProgram& p) : p_(p) {}
+    Compiler(FormatProgram& p, bool marginals) : p_(p), marginals_(marginals) {}
 
     // Appends the ops of one format string as section `sec`; `tokens` = false admits only what BOS / EOS can print.
     void section(uint32_t sec, const char* name, const char* s, size_t n, bool tokens) {
@@ -53,6 +53,12 @@ class Compiler {
                 if (i >= n) fail(at, "unknown directive %p");
                 dir += s[i++];
                 if (dir == "%ph" && i < n && (s[i] == 'l' || s[i] == 'r')) dir += s[i++];
+            }
+            if (dir == "%pP" && marginals_) {
+                if (!tokens) fail(at, dir + " is not allowed here (only literals, %%, %S and %L)");
+                op(kOpProb, at);
+                p_.uses |= kUsesProb;
+                continue;
             }
             static const char* const kNoValue[] = {"%h", "%t", "%P", "%pP", "%pA", "%pB", "%pi", "%pb", "%pp"};
             for (const char* nv : kNoValue)
@@ -188,6 +194,7 @@ class Compiler {
 
     FormatProgram& p_;
     const char* name_ = "";
+    bool marginals_ = false;
     bool open_lit_ = false;
     std::vector<uint32_t> raw_;
 };
@@ -201,10 +208,10 @@ uint32_t fixed_bytes(const FormatProgram& p, uint32_t a, uint32_t b) {
 
 }  // namespace
 
-FormatProgram compile_format(FormatText node, FormatText unk, FormatText bos, FormatText eos) {
+FormatProgram compile_format(FormatText node, FormatText unk, FormatText bos, FormatText eos, bool marginals) {
     FormatProgram p;
     std::memset(&p, 0, sizeof p);
-    Compiler c(p);
+    Compiler c(p, marginals);
     if (!node.ptr) throw Error(kInvalidArgument, "format: the node format must be given");
     c.section(kSecNode, "node", node.ptr, node.len, true);
     if (unk.ptr) {

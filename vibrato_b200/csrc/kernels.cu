@@ -659,6 +659,10 @@ __device__ __forceinline__ uint2 begin_sentence(const Batch& b, uint32_t sidx, u
 // Its best total is `best`, reached from start slot `slot` through predecessor `bestk` of the row at entry `eo`.
 // End slots of different sentences never coincide, so one warp-wide match suffices.  Returns the row's new fill on
 // the lane that stored it (rank 0 among the lanes ending there), 0 on every other lane.
+// k_marg_forward depends on this numbering: it assigns every candidate the same lattice entry again (BOS first, then
+// positions in order, candidates in candidate order) and follows the sweep's position rules (a non-empty row, the
+// space skip, the trailing break).  A change to either in k_viterbi / k_viterbi2 must be made there too; the
+// marginal tests against tests/marginal_oracle.py catch a mismatch.
 __device__ __forceinline__ uint32_t insert_node(const Batch& b, bool valid, const uint4& cd, int32_t best, uint32_t slot,
                                                 uint32_t eo, uint32_t bestk, uint32_t fill) {
     const uint32_t vmask = __ballot_sync(kFull, valid);
@@ -1296,6 +1300,180 @@ __global__ void __launch_bounds__(256) k_backtrack_write(Batch b) {
     }
 }
 
+// ---------------------------------------------------------------------------------------------
+// Marginals (MargArgs in kernels.cuh): one warp per sentence, positions left to right (forward) and right to left
+// (backward).  A lane owns one node at a time and folds that node's terms sequentially.
+// ---------------------------------------------------------------------------------------------
+
+// log(exp(a) + exp(b)) with -inf as the empty sum
+__device__ __forceinline__ double lse2(double a, double b) {
+    const double hi = fmax(a, b), lo = fmin(a, b);
+    return lo == -INFINITY ? hi : hi + log1p(exp(lo - hi));
+}
+
+// Folds the path of cost x that reaches a node with log weight `a` (relative to its own prefix minimum) into the
+// running {rmin, L}: rmin = the least cost so far, L = log-sum-exp relative to rmin.
+__device__ __forceinline__ void marg_push(long long x, double a, double theta, long long& rmin, double& L) {
+    if (x < rmin) {
+        if (rmin != LLONG_MAX) L -= theta * double(rmin - x);
+        rmin = x;
+    }
+    L = lse2(L, a - theta * double(x - rmin));
+}
+
+// The sentence of warp `sidx` as {first slot, sentinel slot}, or false without one.
+__device__ __forceinline__ bool marg_sentence(const Batch& b, uint32_t sidx, uint32_t& s, uint32_t& base, uint32_t& last) {
+    if (sidx >= b.n_sent) return false;
+    s = b.order ? b.order[sidx] : sidx;
+    base = b.slot_off[s];
+    last = b.slot_off[s + 1] - 1;
+    return true;
+}
+
+template <int CONN>
+__global__ void __launch_bounds__(256) k_marg_forward(DictView d, Batch b, MargArgs m) {
+    if (stand_down(*b.flags)) return;
+    const uint32_t lane = threadIdx.x & 31;
+    uint32_t s, base, last;
+    if (!marg_sentence(b, (blockIdx.x * blockDim.x + threadIdx.x) >> 5, s, base, last)) return;
+    if (base == last) {  // an empty sentence: one (empty) path
+        if (lane == 0) {
+            m.r_eos[s] = 0;
+            m.a_eos[s] = 0.0;
+            m.path_prob[s] = 1.f;
+        }
+        return;
+    }
+    for (uint32_t i = lane; i <= last - base; i += 32) m.fill[base + i] = b.ends_meta[base + i].x + (i == 0 ? 1u : 0u);
+    if (lane == 0) {  // BOS
+        const uint32_t bos = b.ends_meta[base].x;
+        m.R[bos] = 0;
+        m.ab[bos] = make_double2(0.0, -INFINITY);
+    }
+    __syncwarp();
+    const double th = m.theta;
+    uint32_t slot_end = last, skip_slot = base;
+    // the positions K3 visits, by the rules of its sweep (tokenizer.rs:110-135): a non-empty row, outside a skipped
+    // space run, and the trailing flag ends the sweep
+    for (uint32_t slot = base; slot < slot_end; ++slot) {
+        const uint2 me = b.ends_meta[slot];  // final after K3: every node ending here came from an earlier position
+        const uint32_t eo = me.x, K = me.y - me.x;
+        const uint4 info = load_info(b, slot);
+        const bool visit = slot >= skip_slot && K != 0;
+        if (visit && (info.w & kInfoTrailing)) {
+            slot_end = slot;
+            break;
+        }
+        if (visit && info.z) skip_slot = slot + info.z + 1;
+        const uint32_t ncand = visit ? info.y : 0;
+        if (lane == 0) m.ncand[slot] = ncand;
+        for (uint32_t c0 = 0; c0 < ncand; c0 += 32) {
+            const uint32_t c = c0 + lane;
+            const bool valid = c < ncand;
+            uint4 cd = make_uint4(0, 0, 0, 0);
+            uint32_t peers = 0, f = 0;
+            const uint32_t vmask = __ballot_sync(kFull, valid);
+            if (valid) {
+                cd = b.cand[info.x + c];
+                peers = __match_any_sync(vmask, cd.w);
+                f = m.fill[cd.w];
+            }
+            __syncwarp();
+            if (valid) {  // the entry insert_node gave this candidate
+                const uint32_t rank = __popc(peers & lanemask_lt());
+                const uint32_t idx = f + rank;
+                m.cand_entry[info.x + c] = idx;
+                if (rank == 0) m.fill[cd.w] = f + __popc(peers);
+                const ConnRow<CONN> conn(d, cd.x & 0xFFFFu);
+                const long long wc = int16_t(cd.y & 0xFFFFu);
+                long long rmin = LLONG_MAX;
+                double L = -INFINITY;
+                for (uint32_t k = 0; k < K; ++k) {
+                    const long long x = m.R[eo + k] + conn.cost(d, uint32_t(b.ends_hot[eo + k].y)) + wc;
+                    marg_push(x, m.ab[eo + k].x, th, rmin, L);
+                }
+                m.R[idx] = rmin;
+                m.ab[idx].x = L;
+            }
+            __syncwarp();
+        }
+    }
+    if (lane == 0) {  // EOS: left id 0, no word cost
+        const uint2 me = b.ends_meta[slot_end];
+        const uint32_t K = me.y - me.x;
+        const ConnRow<CONN> conn(d, 0);
+        long long rmin = LLONG_MAX;
+        double L = -INFINITY;
+        for (uint32_t k = 0; k < K; ++k)
+            marg_push(m.R[me.x + k] + conn.cost(d, uint32_t(b.ends_hot[me.x + k].y)), m.ab[me.x + k].x, th, rmin, L);
+        m.r_eos[s] = rmin;
+        m.a_eos[s] = L;
+        m.path_prob[s] = K ? float(exp(-L)) : 0.f;
+    }
+}
+
+template <int CONN>
+__global__ void __launch_bounds__(256) k_marg_backward(DictView d, Batch b, MargArgs m) {
+    if (stand_down(*b.flags)) return;
+    const uint32_t lane = threadIdx.x & 31;
+    uint32_t s, base, last;
+    if (!marg_sentence(b, (blockIdx.x * blockDim.x + threadIdx.x) >> 5, s, base, last) || base == last) return;
+    const uint32_t slot_end = base + b.eos[s].y;  // the row EOS connects to
+    const long long r_eos = m.r_eos[s];
+    const double th = m.theta;
+    for (uint32_t slot = last + 1; slot-- > base;) {
+        const uint2 me = b.ends_meta[slot];
+        const uint32_t eo = me.x, K = me.y - me.x;
+        if (slot == slot_end) {
+            const ConnRow<CONN> conn(d, 0);
+            for (uint32_t k = lane; k < K; k += 32) {
+                const long long x = m.R[eo + k] + conn.cost(d, uint32_t(b.ends_hot[eo + k].y));
+                m.ab[eo + k].y = -th * double(x - r_eos);
+            }
+        } else {  // no successor at all beyond EOS's row or at a position the sweep skips: -inf
+            const uint32_t nc = slot < slot_end ? m.ncand[slot] : 0u;
+            const uint32_t cptr = nc ? b.info[slot].x : 0u;
+            for (uint32_t k = lane; k < K; k += 32) {
+                double L = -INFINITY;
+                if (nc) {
+                    const long long rk = m.R[eo + k];
+                    const uint32_t right = uint32_t(b.ends_hot[eo + k].y);
+                    for (uint32_t c = 0; c < nc; ++c) {
+                        const uint4 cd = b.cand[cptr + c];
+                        const uint32_t e = m.cand_entry[cptr + c];
+                        const ConnRow<CONN> conn(d, cd.x & 0xFFFFu);
+                        const long long x = rk + conn.cost(d, right) + int16_t(cd.y & 0xFFFFu);
+                        L = lse2(L, m.ab[e].y - th * double(x - m.R[e]));
+                    }
+                }
+                m.ab[eo + k].y = L;
+            }
+        }
+        __syncwarp();
+    }
+}
+
+// K4b with the marginal of every token: prob = exp(â + b̂ - â(EOS)) of its lattice entry.
+__global__ void __launch_bounds__(256) k_backtrack_write_marg(Batch b, MargArgs m) {
+    if (stand_down(*b.flags)) return;
+    const uint32_t w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const uint32_t lane = threadIdx.x & 31;
+#pragma unroll 1
+    for (uint32_t r = 0; r < VBT_SENT_PER_WARP; ++r) {
+        const uint32_t s = w * VBT_SENT_PER_WARP + r;
+        if (s >= b.n_sent) return;
+        backtrack_write_one(b, s, lane);
+        const uint32_t base = b.slot_off[s];
+        const unsigned long long t0 = b.tok_off[s];
+        const uint32_t n = uint32_t(b.tok_off[s + 1] - t0);
+        const double a_eos = n ? m.a_eos[s] : 0.0;
+        for (uint32_t k = lane; k < n; k += 32) {
+            const double2 ab = m.ab[b.ends_meta[base + k].x];
+            m.token_prob[t0 + (n - 1 - k)] = float(exp(ab.x + ab.y - a_eos));
+        }
+    }
+}
+
 
 // ---------------------------------------------------------------------------------------------
 // Output stage: the text `tokenize` writes per sentence (tokenize/src/main.rs:83-127):
@@ -1396,8 +1574,10 @@ struct FmtTok {
     int32_t prev_total, word_cost;
     uint32_t ids;          // left | right << 16
     uint32_t keep, entry;  // field table: the fields printed, and the word's first entry
+    uint32_t prob_micro;   // %pP: round(marginal * 1e6), in [0, 1e6]
 };
 
+template <bool PROB = false>
 __device__ __forceinline__ FmtTok fmt_tok(const DictView& d, const FormatArgs& f, const FormatProgram& P,
                                           unsigned long long t, unsigned long long t0) {
     const uint32_t uses = P.uses;
@@ -1426,6 +1606,13 @@ __device__ __forceinline__ FmtTok fmt_tok(const DictView& d, const FormatArgs& f
         v.keep = __ldg(f.ft_keep + wg);
         v.entry = wg * P.n_fields;
     }
+    v.prob_micro = 0;
+    if constexpr (PROB) {
+        if (uses & kUsesProb) {
+            const double pm = rint(double(f.token_prob[t]) * 1e6);
+            v.prob_micro = uint32_t(fmin(fmax(pm, 0.0), 1e6));
+        }
+    }
     return v;
 }
 
@@ -1448,7 +1635,9 @@ __device__ __forceinline__ long long fmt_number(uint32_t kind, const FmtTok& v, 
 }
 __device__ __forceinline__ uint32_t num_len(long long x) { return x < 0 ? 1 + dec_len(uint32_t(-x)) : dec_len(uint32_t(x)); }
 
-// Bytes the ops [a, b) of the program write for one token (or for BOS / EOS, with v unused).
+// Bytes the ops [a, b) of the program write for one token (or for BOS / EOS, with v unused).  PROB: the program may
+// print %pP (a separate instantiation, so that the other formats keep their code).
+template <bool PROB = false>
 __device__ __forceinline__ unsigned long long fmt_len(const FormatProgram& P, uint32_t a, uint32_t b, const FormatArgs& f,
                                                       const FmtTok& v, uint32_t sent_len) {
     unsigned long long n = 0;
@@ -1471,7 +1660,14 @@ __device__ __forceinline__ unsigned long long fmt_len(const FormatProgram& P, ui
                 }
                 break;
             }
-            default: n += num_len(fmt_number(o.kind, v, sent_len));
+            default:
+                if constexpr (PROB) {
+                    if (o.kind == kOpProb) {
+                        n += 8;  // d.dddddd
+                        break;
+                    }
+                }
+                n += num_len(fmt_number(o.kind, v, sent_len));
         }
     }
     return n;
@@ -1502,7 +1698,7 @@ __device__ __forceinline__ const FormatProgram* stage_program(const FormatArgs& 
 
 // Pass 1 for sentence s (a warp per sentence): lane 0 stores its text length in sent_len[s].  PROG: f.mode is
 // kOutFormat (a separate instantiation, so that the fixed modes keep their registers).
-template <bool PROG>
+template <bool PROG, bool PROB = false>
 __device__ __forceinline__ void format_len_one(const DictView& d, const FormatArgs& f, const FormatProgram* P, uint32_t s,
                                                uint32_t lane) {
     const unsigned long long t0 = f.tok_off[s], t1 = f.tok_off[s + 1];
@@ -1510,15 +1706,15 @@ __device__ __forceinline__ void format_len_one(const DictView& d, const FormatAr
     if constexpr (PROG) {
         const uint32_t sl = uint32_t(f.byte_off[s + 1] - f.byte_off[s]);
         for (unsigned long long t = t0 + lane; t < t1; t += 32) {
-            const FmtTok v = fmt_tok(d, f, *P, t, t0);
+            const FmtTok v = fmt_tok<PROB>(d, f, *P, t, t0);
             const uint32_t sec = v.x.lex == 2 ? kSecUnk : kSecNode;
-            len += fmt_len(*P, P->sec[sec][0], P->sec[sec][1], f, v, sl);
+            len += fmt_len<PROB>(*P, P->sec[sec][0], P->sec[sec][1], f, v, sl);
         }
         for (int k = 16; k > 0; k >>= 1) len += __shfl_xor_sync(kFull, len, k);
         if (lane == 0) {
             FmtTok none{};
-            len += fmt_len(*P, P->sec[kSecBos][0], P->sec[kSecBos][1], f, none, sl);
-            f.sent_len[s] = len + fmt_len(*P, P->sec[kSecEos][0], P->sec[kSecEos][1], f, none, sl);
+            len += fmt_len<PROB>(*P, P->sec[kSecBos][0], P->sec[kSecBos][1], f, none, sl);
+            f.sent_len[s] = len + fmt_len<PROB>(*P, P->sec[kSecEos][0], P->sec[kSecEos][1], f, none, sl);
         }
     } else {
         for (unsigned long long t = t0 + lane; t < t1; t += 32) len += token_text_len(d, token_text(d, f.tokens, t), f.mode, t == t0);
@@ -1527,13 +1723,13 @@ __device__ __forceinline__ void format_len_one(const DictView& d, const FormatAr
     }
 }
 
-template <bool PROG>
+template <bool PROG, bool PROB = false>
 __global__ void __launch_bounds__(256) k_format_len(DictView d, FormatArgs f) {
     extern __shared__ uint4 s_dyn[];
     const FormatProgram* P = PROG ? stage_program(f, reinterpret_cast<FormatProgram*>(s_dyn)) : nullptr;
     const uint32_t s = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     if (s >= f.n_sent || format_stands_down(f)) return;
-    format_len_one<PROG>(d, f, P, s, lane);
+    format_len_one<PROG, PROB>(d, f, P, s, lane);
 }
 
 __device__ __forceinline__ void warp_copy(uint8_t* __restrict__ dst, const uint8_t* __restrict__ src, uint32_t n, uint32_t lane) {
@@ -1541,6 +1737,7 @@ __device__ __forceinline__ void warp_copy(uint8_t* __restrict__ dst, const uint8
 }
 
 // Writes the ops [a, b) at dst with the whole warp (every lane passes the same arguments); returns the end.
+template <bool PROB = false>
 __device__ __forceinline__ uint8_t* fmt_write(const DictView& d, const FormatProgram& P, uint32_t a, uint32_t b,
                                               const FormatArgs& f, const FmtTok& v, const uint8_t* __restrict__ sent,
                                               uint32_t sent_len, uint8_t* dst, uint32_t lane) {
@@ -1588,6 +1785,18 @@ __device__ __forceinline__ uint8_t* fmt_write(const DictView& d, const FormatPro
                 break;
             }
             default: {
+                if constexpr (PROB) {
+                    if (o.kind == kOpProb) {  // round(p * 1e6) as d.dddddd
+                        if (lane == 0) {
+                            dst[0] = uint8_t('0' + v.prob_micro / 1000000u);
+                            dst[1] = '.';
+                            uint32_t frac = v.prob_micro % 1000000u;
+                            for (int k = 7; k >= 2; --k, frac /= 10) dst[k] = uint8_t('0' + frac % 10);
+                        }
+                        dst += 8;
+                        break;
+                    }
+                }
                 const long long x = fmt_number(o.kind, v, sent_len);
                 if (lane == 0) {
                     if (x < 0) {
@@ -1690,7 +1899,7 @@ __global__ void __launch_bounds__(256) k_field_table_write(DictView d, FieldTabl
 }
 
 // Pass 2 for sentence s (a warp per sentence): its text at text_off[s], which must fit in text_cap.
-template <bool PROG>
+template <bool PROG, bool PROB = false>
 __device__ __forceinline__ void format_write_one(const DictView& d, const FormatArgs& f, const FormatProgram* P, uint32_t s,
                                                  uint32_t lane) {
     const unsigned long long t0 = f.tok_off[s], t1 = f.tok_off[s + 1];
@@ -1700,7 +1909,7 @@ __device__ __forceinline__ void format_write_one(const DictView& d, const Format
     const uint32_t sl = prog ? uint32_t(f.byte_off[s + 1] - f.byte_off[s]) : 0u;
     if (prog) {
         const FmtTok none{};
-        base = fmt_write(d, *P, P->sec[kSecBos][0], P->sec[kSecBos][1], f, none, sent, sl, f.text + base, lane) - f.text;
+        base = fmt_write<PROB>(d, *P, P->sec[kSecBos][0], P->sec[kSecBos][1], f, none, sent, sl, f.text + base, lane) - f.text;
     }
     for (unsigned long long c = t0; c < t1; c += 32) {
         // lane i stages token c + i; the copies below take one token at a time with all 32 lanes
@@ -1708,9 +1917,9 @@ __device__ __forceinline__ void format_write_one(const DictView& d, const Format
         TokenText mine = {0, 0, 0, 0, 0, 0, 0};
         unsigned long long len = 0;
         if (lane < cnt && prog) {
-            const FmtTok v = fmt_tok(d, f, *P, c + lane, t0);
+            const FmtTok v = fmt_tok<PROB>(d, f, *P, c + lane, t0);
             const uint32_t sec = v.x.lex == 2 ? kSecUnk : kSecNode;
-            len = fmt_len(*P, P->sec[sec][0], P->sec[sec][1], f, v, sl);
+            len = fmt_len<PROB>(*P, P->sec[sec][0], P->sec[sec][1], f, v, sl);
         } else if (lane < cnt) {
             mine = token_text(d, f.tokens, c + lane);
             len = token_text_len(d, mine, f.mode, c + lane == t0);
@@ -1724,9 +1933,9 @@ __device__ __forceinline__ void format_write_one(const DictView& d, const Format
         base += __shfl_sync(kFull, incl, 31);
         for (uint32_t j = 0; j < cnt; ++j) {
             if (prog) {  // every lane loads token c + j again: one broadcast load per record
-                const FmtTok v = fmt_tok(d, f, *P, c + j, t0);
+                const FmtTok v = fmt_tok<PROB>(d, f, *P, c + j, t0);
                 const uint32_t sec = v.x.lex == 2 ? kSecUnk : kSecNode;
-                fmt_write(d, *P, P->sec[sec][0], P->sec[sec][1], f, v, sent, sl, f.text + __shfl_sync(kFull, at, j), lane);
+                fmt_write<PROB>(d, *P, P->sec[sec][0], P->sec[sec][1], f, v, sent, sl, f.text + __shfl_sync(kFull, at, j), lane);
                 continue;
             }
             TokenText x;
@@ -1772,7 +1981,7 @@ __device__ __forceinline__ void format_write_one(const DictView& d, const Format
     }
     if (prog) {
         const FmtTok none{};
-        fmt_write(d, *P, P->sec[kSecEos][0], P->sec[kSecEos][1], f, none, sent, sl, f.text + base, lane);
+        fmt_write<PROB>(d, *P, P->sec[kSecEos][0], P->sec[kSecEos][1], f, none, sent, sl, f.text + base, lane);
     } else if (lane == 0) {
         uint8_t* dst = f.text + base;
         if (f.mode != kOutWakati) dst = put_str(dst, "EOS");
@@ -1780,7 +1989,7 @@ __device__ __forceinline__ void format_write_one(const DictView& d, const Format
     }
 }
 
-template <bool PROG>
+template <bool PROG, bool PROB = false>
 __global__ void __launch_bounds__(256) k_format_write(DictView d, FormatArgs f) {
     extern __shared__ uint4 s_dyn[];
     const FormatProgram* P = PROG ? stage_program(f, reinterpret_cast<FormatProgram*>(s_dyn)) : nullptr;
@@ -1792,7 +2001,7 @@ __global__ void __launch_bounds__(256) k_format_write(DictView d, FormatArgs f) 
         if (total > f.text_cap) atomicOr(f.flags, kFlagTextOverflow);
     }
     if (total > f.text_cap) return;  // every warp sees the same total: nothing is written
-    format_write_one<PROG>(d, f, P, s, lane);
+    format_write_one<PROG, PROB>(d, f, P, s, lane);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1970,7 +2179,8 @@ void launch_small_batch(const DictView& d, const Batch& b, const FormatArgs& f, 
 void launch_format_len(const DictView& d, const FormatArgs& f, cudaStream_t st) {
     if (!f.n_sent) return;
     if (f.mode == kOutFormat)
-        k_format_len<true><<<(f.n_sent + 7) / 8, 256, sizeof(FormatProgram), st>>>(d, f);
+        f.token_prob ? k_format_len<true, true><<<(f.n_sent + 7) / 8, 256, sizeof(FormatProgram), st>>>(d, f)
+                     : k_format_len<true><<<(f.n_sent + 7) / 8, 256, sizeof(FormatProgram), st>>>(d, f);
     else
         k_format_len<false><<<(f.n_sent + 7) / 8, 256, 0, st>>>(d, f);
 }
@@ -1978,7 +2188,8 @@ void launch_format_len(const DictView& d, const FormatArgs& f, cudaStream_t st) 
 void launch_format_write(const DictView& d, const FormatArgs& f, cudaStream_t st) {
     if (!f.n_sent) return;
     if (f.mode == kOutFormat)
-        k_format_write<true><<<(f.n_sent + 7) / 8, 256, sizeof(FormatProgram), st>>>(d, f);
+        f.token_prob ? k_format_write<true, true><<<(f.n_sent + 7) / 8, 256, sizeof(FormatProgram), st>>>(d, f)
+                     : k_format_write<true><<<(f.n_sent + 7) / 8, 256, sizeof(FormatProgram), st>>>(d, f);
     else
         k_format_write<false><<<(f.n_sent + 7) / 8, 256, 0, st>>>(d, f);
 }
@@ -2097,6 +2308,26 @@ void launch_backtrack_count(const Batch& b, cudaStream_t st) {
 void launch_backtrack_write(const Batch& b, cudaStream_t st) {
     if (!b.n_sent) return;
     k_backtrack_write<<<(b.n_sent + 8 * VBT_SENT_PER_WARP - 1) / (8 * VBT_SENT_PER_WARP), 256, 0, st>>>(b);  // warps over sentences
+}
+
+void launch_marginals(const DictView& d, const Batch& b, const MargArgs& m, cudaStream_t st) {
+    if (!b.n_sent) return;
+    const uint32_t blocks = (b.n_sent + 7) / 8;  // a warp per sentence
+    if (d.connector_kind == 1) {
+        k_marg_forward<1><<<blocks, 256, 0, st>>>(d, b, m);
+        k_marg_backward<1><<<blocks, 256, 0, st>>>(d, b, m);
+    } else if (d.connector_kind == 2) {
+        k_marg_forward<2><<<blocks, 256, 0, st>>>(d, b, m);
+        k_marg_backward<2><<<blocks, 256, 0, st>>>(d, b, m);
+    } else {
+        k_marg_forward<0><<<blocks, 256, 0, st>>>(d, b, m);
+        k_marg_backward<0><<<blocks, 256, 0, st>>>(d, b, m);
+    }
+}
+
+void launch_backtrack_write_marg(const Batch& b, const MargArgs& m, cudaStream_t st) {
+    if (!b.n_sent) return;
+    k_backtrack_write_marg<<<(b.n_sent + 8 * VBT_SENT_PER_WARP - 1) / (8 * VBT_SENT_PER_WARP), 256, 0, st>>>(b, m);
 }
 
 }  // namespace vbt

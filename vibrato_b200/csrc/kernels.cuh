@@ -156,6 +156,9 @@ struct FormatArgs {
     const uint32_t* ft_keep;  // per word: bit k set = field prog->fields[k] is printed (present, not '*')
     const uint32_t* ft_off;   // per word and k (n_fields per word), + 1: where the field's unquoted text starts
     const uint8_t* ft_bytes;
+    // the batch's token marginals (at the token indices of tok_off) when the program prints %pP, else nullptr (this
+    // selects the kernels' %pP instantiation; k_small_batch, which never runs with marginals, ignores it)
+    const float* token_prob;
 };
 void launch_format_len(const DictView& d, const FormatArgs& f, cudaStream_t st);
 void launch_format_write(const DictView& d, const FormatArgs& f, cudaStream_t st);
@@ -205,6 +208,31 @@ int launch_viterbi(const DictView& d, const Batch& b, const uint4* stats, int la
                    cudaStream_t st, uint32_t* route);
 void launch_backtrack_count(const Batch& b, cudaStream_t st);
 void launch_backtrack_write(const Batch& b, cudaStream_t st);
+
+// Marginal probabilities: forward-backward over the lattice K3 left in ends_hot / ends_meta, between K3 and K4a
+// (K4a overwrites ends_meta).  Per lattice entry n, with R(n) the exact (64-bit) minimum cost from BOS to n:
+//   ab[n].x = â(n) = log alpha(n) + theta R(n),   ab[n].y = b̂(n) = log beta(n) + theta (R(EOS) - R(n)),
+// so prob(n) = exp(â(n) + b̂(n) - â(EOS)) and path_prob = exp(-â(EOS)).  Every term of the log-sum-exps is
+// â - theta * (an exact non-negative integer excess), so the values stay within [-inf, log #paths].  Each node sums
+// its terms in one lane in a fixed order (predecessors in row order, candidates in candidate order): the results do
+// not depend on the route, the chunking or the sentence order.  The forward pass numbers the candidates' lattice
+// entries itself, in the order every K3 variant inserts them (position order, then candidate order).
+struct MargArgs {
+    double theta;            // > 0
+    uint32_t* fill;          // per slot: the row's next free entry while the forward pass numbers the nodes
+    uint32_t* ncand;         // per slot: the candidates of a position the sweep visits, 0 elsewhere
+    uint32_t* cand_entry;    // per candidate of a visited position: its lattice entry
+    long long* R;            // per lattice entry
+    double2* ab;             // per lattice entry: {â, b̂}
+    long long* r_eos;        // per sentence: R(EOS)
+    double* a_eos;           // per sentence: â(EOS)
+    float* path_prob;        // per sentence: exp(-â(EOS)); 1 for an empty sentence
+    float* token_prob;       // per token, at the token's index (tok_off)
+};
+// k_marg_forward and k_marg_backward (two launches).
+void launch_marginals(const DictView& d, const Batch& b, const MargArgs& m, cudaStream_t st);
+// launch_backtrack_write plus MargArgs::token_prob of every token (one launch, in its place).
+void launch_backtrack_write_marg(const Batch& b, const MargArgs& m, cudaStream_t st);
 
 // What k_small_batch reports besides its outputs: the batch flags and the totals of its scans.
 struct SmallBatchOut {

@@ -220,6 +220,8 @@ class MultiEngine final : public Engine {
             pinned_free(r->tokens);
             pinned_free(r->text_off);
             pinned_free(r->text);
+            pinned_free(r->token_prob);
+            pinned_free(r->path_prob);
             delete r;
         }
         pinned_free(h_off_);
@@ -228,6 +230,8 @@ class MultiEngine final : public Engine {
         cudaSetDevice(dev_[0]);
         if (gather_tokens_) cudaFree(gather_tokens_);
         if (gather_off_) cudaFree(gather_off_);
+        if (gather_tprob_) cudaFree(gather_tprob_);
+        if (gather_pprob_) cudaFree(gather_pprob_);
     }
 
     // ---- host batches --------------------------------------------------------------------------------
@@ -256,7 +260,8 @@ class MultiEngine final : public Engine {
         int last = n - 1;  // the shard that also delivers the closing offset: the last one, even when it is empty
         run_on_all([&](int i) {
             eng_[i]->fetch_shard(r->tok_off + cut[i], static_cast<uint8_t*>(r->tokens) + base[i] * tb, base[i], i == last,
-                                 text_ ? r->text_off + cut[i] : nullptr, r->text + text_base[i], text_base[i]);
+                                 text_ ? r->text_off + cut[i] : nullptr, r->text + text_base[i], text_base[i],
+                                 r->has_marg ? r->token_prob + base[i] : nullptr, r->has_marg ? r->path_prob + cut[i] : nullptr);
         });
         collect_stats();
         return r;
@@ -278,6 +283,7 @@ class MultiEngine final : public Engine {
             collect_stats();
             return;
         }
+        dev_marg_ = false;
         CK(cudaSetDevice(dev_[0]));
         // the split needs the offsets on the host (pinned staging buffer, one copy); their validity is checked on
         // the devices like for any device-resident batch (k_count_chars)
@@ -321,8 +327,19 @@ class MultiEngine final : public Engine {
             gather_off_cap_ = size_t(double((n_sent + 1) * 8) * 1.25) + 4096;
             CK(cudaMalloc(&gather_off_, gather_off_cap_));
         }
-        std::vector<uint64_t> src_off(n), src_tok(n);
-        for (int i = 0; i < n; ++i) eng_[i]->shard_outputs(&src_off[i], &src_tok[i]);
+        const bool marg = marginals() > 0;
+        if (marg) {  // the marginals travel with the token records: float per token, float per sentence
+            grow_device(gather_tprob_, gather_tprob_cap_, base[n] * 4 + 4);
+            grow_device(gather_pprob_, gather_pprob_cap_, n_sent * 4 + 4);
+        }
+        std::vector<uint64_t> src_off(n), src_tok(n), src_tp(n), src_pp(n);
+        for (int i = 0; i < n; ++i) {
+            eng_[i]->shard_outputs(&src_off[i], &src_tok[i]);
+            if (marg) eng_[i]->shard_marginals(&src_tp[i], &src_pp[i]);
+        }
+        auto dst_tp = [&](int i) { return static_cast<uint8_t*>(gather_tprob_) + base[i] * 4; };
+        auto dst_pp = [&](int i) { return static_cast<uint8_t*>(gather_pprob_) + cut[i] * 4; };
+        auto n_sh = [&](int i) { return cut[i + 1] - cut[i]; };
         const uint64_t tb = eng_[0]->token_bytes();
         auto dst_tok = [&](int i) { return static_cast<uint8_t*>(gather_tokens_) + base[i] * tb; };
         auto dst_off = [&](int i) { return static_cast<uint8_t*>(gather_off_) + cut[i] * 8; };
@@ -330,21 +347,33 @@ class MultiEngine final : public Engine {
         // shard 0 is already on the first device
         CK(cudaMemcpyAsync(dst_tok(0), reinterpret_cast<const void*>(src_tok[0]), n_tok[0] * tb, cudaMemcpyDeviceToDevice, stream_[0]));
         CK(cudaMemcpyAsync(dst_off(0), reinterpret_cast<const void*>(src_off[0]), off_bytes(0), cudaMemcpyDeviceToDevice, stream_[0]));
+        if (marg) {
+            if (n_tok[0]) CK(cudaMemcpyAsync(dst_tp(0), reinterpret_cast<const void*>(src_tp[0]), n_tok[0] * 4, cudaMemcpyDeviceToDevice, stream_[0]));
+            if (n_sh(0)) CK(cudaMemcpyAsync(dst_pp(0), reinterpret_cast<const void*>(src_pp[0]), n_sh(0) * 4, cudaMemcpyDeviceToDevice, stream_[0]));
+        }
         if (n > 1 && nccl_) {
             NK(nccl_->GroupStart());
             for (int i = 1; i < n; ++i) {
                 CK(cudaSetDevice(dev_[i]));
                 if (n_tok[i]) NK(nccl_->Send(reinterpret_cast<const void*>(src_tok[i]), n_tok[i] * tb, ncclUint8, 0, comm_[i], stream_[i]));
                 NK(nccl_->Send(reinterpret_cast<const void*>(src_off[i]), off_bytes(i), ncclUint8, 0, comm_[i], stream_[i]));
+                if (marg && n_tok[i]) NK(nccl_->Send(reinterpret_cast<const void*>(src_tp[i]), n_tok[i] * 4, ncclUint8, 0, comm_[i], stream_[i]));
+                if (marg && n_sh(i)) NK(nccl_->Send(reinterpret_cast<const void*>(src_pp[i]), n_sh(i) * 4, ncclUint8, 0, comm_[i], stream_[i]));
                 CK(cudaSetDevice(dev_[0]));
                 if (n_tok[i]) NK(nccl_->Recv(dst_tok(i), n_tok[i] * tb, ncclUint8, i, comm_[0], stream_[0]));
                 NK(nccl_->Recv(dst_off(i), off_bytes(i), ncclUint8, i, comm_[0], stream_[0]));
+                if (marg && n_tok[i]) NK(nccl_->Recv(dst_tp(i), n_tok[i] * 4, ncclUint8, i, comm_[0], stream_[0]));
+                if (marg && n_sh(i)) NK(nccl_->Recv(dst_pp(i), n_sh(i) * 4, ncclUint8, i, comm_[0], stream_[0]));
             }
             NK(nccl_->GroupEnd());
         } else {
             for (int i = 1; i < n; ++i) {
                 if (n_tok[i]) CK(cudaMemcpyPeerAsync(dst_tok(i), dev_[0], reinterpret_cast<const void*>(src_tok[i]), dev_[i], n_tok[i] * tb, stream_[0]));
                 CK(cudaMemcpyPeerAsync(dst_off(i), dev_[0], reinterpret_cast<const void*>(src_off[i]), dev_[i], off_bytes(i), stream_[0]));
+                if (marg && n_tok[i])
+                    CK(cudaMemcpyPeerAsync(dst_tp(i), dev_[0], reinterpret_cast<const void*>(src_tp[i]), dev_[i], n_tok[i] * 4, stream_[0]));
+                if (marg && n_sh(i))
+                    CK(cudaMemcpyPeerAsync(dst_pp(i), dev_[0], reinterpret_cast<const void*>(src_pp[i]), dev_[i], n_sh(i) * 4, stream_[0]));
             }
         }
         for (int i = 0; i < n; ++i) {
@@ -355,6 +384,7 @@ class MultiEngine final : public Engine {
         *d_tok_off = reinterpret_cast<uint64_t>(gather_off_);
         *d_tokens = reinterpret_cast<uint64_t>(gather_tokens_);
         *n_tokens = base[n];
+        dev_marg_ = marg;
     }
 
     // ---- everything else is forwarded ------------------------------------------------------------------
@@ -376,6 +406,16 @@ class MultiEngine final : public Engine {
         }
         if (p) fixed_mode_ = false;  // the format replaced it
         text_ = p != nullptr || fixed_mode_;
+    }
+    void set_marginals(double theta) override {
+        for (auto& e : eng_) e->set_marginals(theta);
+    }
+    double marginals() const override { return eng_[0]->marginals(); }
+    void device_marginals(uint64_t* d_token_prob, uint64_t* d_path_prob) const override {
+        if (dev_.size() == 1) return eng_[0]->device_marginals(d_token_prob, d_path_prob);
+        if (!dev_marg_) throw Error(kInvalidArgument, "the last device-resident call ran without marginals");
+        if (d_token_prob) *d_token_prob = reinterpret_cast<uint64_t>(gather_tprob_);
+        if (d_path_prob) *d_path_prob = reinterpret_cast<uint64_t>(gather_pprob_);
     }
     void set_stream(uint64_t stream) override {
         if (stream) throw Error(kUnsupported, "a multi-device tokenizer runs on its own streams");
@@ -401,9 +441,10 @@ class MultiEngine final : public Engine {
     uint64_t run_shard(const char*, const uint64_t*, uint64_t, int, uint64_t*, const Bounds*) override {
         throw Error(kInternal, "not a shard engine");
     }
-    void fetch_shard(uint64_t*, void*, uint64_t, bool, uint64_t*, char*, uint64_t) override {
+    void fetch_shard(uint64_t*, void*, uint64_t, bool, uint64_t*, char*, uint64_t, float*, float*) override {
         throw Error(kInternal, "not a shard engine");
     }
+    void shard_marginals(uint64_t*, uint64_t*) const override { throw Error(kInternal, "not a shard engine"); }
     void rebase_shard(uint64_t) override { throw Error(kInternal, "not a shard engine"); }
     void shard_outputs(uint64_t*, uint64_t*) const override { throw Error(kInternal, "not a shard engine"); }
     int device() const override { return dev_[0]; }
@@ -429,6 +470,14 @@ class MultiEngine final : public Engine {
             cut[i] = std::max<uint64_t>(cut[i - 1], std::min<uint64_t>(uint64_t(p - off), n_sent));
         }
         return cut;
+    }
+
+    static void grow_device(void*& p, size_t& cap, size_t bytes) {
+        if (bytes <= cap) return;
+        if (p) CK(cudaFree(p));
+        p = nullptr;
+        cap = size_t(double(bytes) * 1.25) + 4096;
+        CK(cudaMalloc(&p, cap));
     }
 
     static void grow_pinned(void*& p, size_t& cap, size_t bytes) {
@@ -521,6 +570,15 @@ class MultiEngine final : public Engine {
                 r->text = static_cast<char*>(pinned_alloc(r->cap_text));
             }
         }
+        r->has_marg = marginals() > 0;
+        if (r->has_marg) {
+            void* tp = r->token_prob;
+            void* pp = r->path_prob;
+            grow_pinned(tp, r->cap_tprob, n_tokens * 4);
+            grow_pinned(pp, r->cap_pprob, n_sent * 4);
+            r->token_prob = static_cast<float*>(tp);
+            r->path_prob = static_cast<float*>(pp);
+        }
         if (n_sent == 0) r->tok_off[0] = 0;
         if (n_sent == 0 && text_bytes) r->text_off[0] = 0;
         return r;
@@ -545,6 +603,10 @@ class MultiEngine final : public Engine {
     void* gather_tokens_ = nullptr;
     void* gather_off_ = nullptr;
     size_t gather_tok_cap_ = 0, gather_off_cap_ = 0;
+    void* gather_tprob_ = nullptr;  // marginals of a gathered device-resident batch
+    void* gather_pprob_ = nullptr;
+    size_t gather_tprob_cap_ = 0, gather_pprob_cap_ = 0;
+    bool dev_marg_ = false;
     float stage_ms_[kNumStages];
     uint64_t counters_[10];
     uint64_t launches_ = 0;
