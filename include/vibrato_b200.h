@@ -72,6 +72,14 @@ typedef struct vbt_token16 {
     int32_t total_cost;  /* Token::total_cost()                           token.rs:89-92 */
 } vbt_token16;
 
+/* Lattice output (option "lattice"): per lattice node, next to its vbt_token record. */
+typedef struct vbt_lattice_link {
+    int32_t prev;   /* the node's best predecessor (Node::min_idx, u16-truncated as the backtrack reads it) as an index
+                       into the sentence's own node list; -1 for BOS */
+    uint32_t flags; /* VBT_NODE_BEST: the node is on the best path; every other bit is 0 */
+} vbt_lattice_link;
+#define VBT_NODE_BEST 1u
+
 #define VBT_WORD_ID(word_idx) ((word_idx) & 0x3FFFFFFFu)
 #define VBT_LEX_TYPE(word_idx) ((word_idx) >> 30)
 
@@ -338,6 +346,29 @@ int32_t vbt_result_marginals(const vbt_result *r, const float **token_prob, cons
 /* Device addresses (float32) of the marginals of the last vbt_tokenize_batch_device{,_bounded} call, valid until the
  * next call; VBT_ERR_INVALID_ARGUMENT when it ran without marginals. */
 int32_t vbt_last_device_marginals(const vbt_tokenizer *t, uint64_t *d_token_prob, uint64_t *d_path_prob);
+/* Lattice output, the option "lattice" of vbt_tokenizer_set_option: 0 off (default); 1 every result also carries
+ * every node of each sentence's lattice; 2 the same, and the output text ("output_mode" 1-3 or a format) renders the
+ * nodes in place of the tokens, like MeCab's -a (BOS / EOS formats still print once per sentence).  Single-device
+ * tokenizers only (a multi-device one refuses it with VBT_ERR_UNSUPPORTED).
+ *   Nodes: the entries of the reference's Lattice::ends once build_lattice has finished, without BOS and EOS; exactly
+ *   the nodes the tokenizer inserts (ignore_space, max_grouping_len, the user lexicon and required boundaries
+ *   included), dead ends and nodes ending inside a trailing space run included.  An empty sentence has none.
+ *   Order: by end character position, then in insertion order (Lattice::ends[e]).  This is not MeCab's start order.
+ *   Record: a vbt_token record, always 24 bytes (also under "compact_tokens"), with start_char = the node's start_word,
+ *   total_cost = Node::min_cost (the tokenizer's wrapping i32), and a vbt_lattice_link.
+ *   Guarantee: the nodes with VBT_NODE_BEST set, in node order, equal the sentence's token records byte for byte.
+ *   With marginals on, node_prob[k] is the node's marginal (vbt_tokenizer_set_marginals); on the best path it equals
+ *   token_prob bit for bit.
+ * While on, batches take three more kernel launches and a scan (booked under "viterbi"), "small_batch" steps aside,
+ * and with 2 a format may not print the "prev" directives %M %pS %pn %pC %pL (setting either order fails). */
+/* node_offsets[n_sent + 1] into nodes / links / node_prob (NULL without marginals) of a result made with the lattice;
+ * owned by the result.  VBT_ERR_INVALID_ARGUMENT for a result made without it. */
+int32_t vbt_result_lattice(const vbt_result *r, const uint64_t **node_offsets, const vbt_token **nodes,
+                           const vbt_lattice_link **links, const float **node_prob, uint64_t *n_nodes);
+/* Device addresses of the lattice of the last vbt_tokenize_batch_device{,_bounded} call (d_node_prob 0 without
+ * marginals), valid until the next call; VBT_ERR_INVALID_ARGUMENT when it ran without the lattice. */
+int32_t vbt_last_device_lattice(const vbt_tokenizer *t, uint64_t *d_node_offsets, uint64_t *d_nodes, uint64_t *d_links,
+                                uint64_t *d_node_prob, uint64_t *n_nodes);
 /* Launch the kernels on a caller-owned CUDA stream (a cudaStream_t passed as an integer; 0 restores
  * the tokenizer's own stream), so callers can bracket batches with their own events. */
 int32_t vbt_tokenizer_set_stream(vbt_tokenizer *t, uint64_t stream);

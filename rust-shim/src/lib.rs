@@ -14,6 +14,12 @@ pub struct vbt_token {
     pub word_idx: u32, pub total_cost: i32,
 }
 
+/// Per lattice node (option "lattice"): its best predecessor in the sentence's node list (-1 for BOS) and flags.
+#[repr(C)]
+#[derive(Clone, Copy, Debug)]
+pub struct vbt_lattice_link { pub prev: i32, pub flags: u32 }
+pub const VBT_NODE_BEST: u32 = 1;
+
 #[link(name = "vibrato_b200")]
 extern "C" {
     fn vbt_last_error() -> *const c_char;
@@ -56,6 +62,8 @@ extern "C" {
                        n_bytes: *mut u64) -> i32;
     fn vbt_tokenizer_set_marginals(t: *mut vbt_tokenizer, theta: f64) -> i32;
     fn vbt_result_marginals(r: *const vbt_result, token_prob: *mut *const f32, path_prob: *mut *const f32) -> i32;
+    fn vbt_result_lattice(r: *const vbt_result, node_offsets: *mut *const u64, nodes: *mut *const vbt_token,
+                          links: *mut *const vbt_lattice_link, node_prob: *mut *const f32, n_nodes: *mut u64) -> i32;
     fn vbt_evaluate(d: *const vbt_dict, t: *mut vbt_tokenizer, corpus: *const c_char, len: usize,
                     feature_indices: *const u64, n_indices: usize, num_ref: *mut u64, num_sys: *mut u64,
                     num_cor: *mut u64) -> i32;
@@ -251,6 +259,12 @@ impl Tokenizer {
     pub fn marginals(&self, theta: f64) -> Result<()> {
         check(unsafe { vbt_tokenizer_set_marginals(self.handle(), theta) })
     }
+    /// Lattice output (option "lattice"): batches tokenised afterwards carry `BatchResult::lattice`; `text` also
+    /// renders the nodes in place of the tokens in the output text (MeCab -a).  Set it before a format that prints `%pb`.
+    pub fn lattice(&self, on: bool, text: bool) -> Result<()> {
+        let v = if !on { 0 } else if text { 2 } else { 1 };
+        check(unsafe { vbt_tokenizer_set_option(self.handle(), b"lattice\0".as_ptr() as *const c_char, v) })
+    }
     /// The loop of the `evaluate` tool (evaluate/src/main.rs:61-138): (num_ref, num_sys, num_cor).
     pub fn evaluate(&self, corpus: &str, feature_indices: &[usize]) -> Result<(u64, u64, u64)> {
         let idx: Vec<u64> = feature_indices.iter().map(|&i| i as u64).collect();
@@ -294,6 +308,21 @@ impl BatchResult {
             vbt_result_view(self.r, &mut o, &mut t, &mut ns, &mut nt);
             let s = |p: *const f32, n: u64| if n == 0 { &[][..] } else { std::slice::from_raw_parts(p, n as usize) };
             Ok((s(tp, nt), s(pp, ns)))
+        }
+    }
+    /// (node offsets, nodes, links, node marginals or None without marginals); an error for a batch tokenised
+    /// without the lattice.
+    pub fn lattice(&self) -> Result<(&[u64], &[vbt_token], &[vbt_lattice_link], Option<&[f32]>)> {
+        let (mut o, mut nd, mut l, mut p, mut nn) = (std::ptr::null(), std::ptr::null(), std::ptr::null(), std::ptr::null(), 0u64);
+        check(unsafe { vbt_result_lattice(self.r, &mut o, &mut nd, &mut l, &mut p, &mut nn) })?;
+        let (mut to, mut t, mut ns, mut nt) = (std::ptr::null(), std::ptr::null(), 0u64, 0u64);
+        unsafe {
+            vbt_result_view(self.r, &mut to, &mut t, &mut ns, &mut nt);
+            let n = nn as usize;
+            let nodes: &[vbt_token] = if n == 0 { &[] } else { std::slice::from_raw_parts(nd, n) };
+            let links: &[vbt_lattice_link] = if n == 0 { &[] } else { std::slice::from_raw_parts(l, n) };
+            let probs = if p.is_null() { None } else if n == 0 { Some(&[][..]) } else { Some(std::slice::from_raw_parts(p, n)) };
+            Ok((std::slice::from_raw_parts(o, ns as usize + 1), nodes, links, probs))
         }
     }
     pub fn view(&self) -> (&[u64], &[vbt_token]) {

@@ -25,6 +25,8 @@ TOKEN_DTYPE = np.dtype(
     [("start_char", "<u4"), ("end_char", "<u4"), ("start_byte", "<u4"), ("end_byte", "<u4"),
      ("word_idx", "<u4"), ("total_cost", "<i4")]
 )
+LINK_DTYPE = np.dtype([("prev", "<i4"), ("flags", "<u4")])  # vbt_lattice_link
+NODE_BEST = 1  # VBT_NODE_BEST
 LEX_TYPE_NAMES = ("System", "User", "Unknown")  # dictionary.rs:30-40 (Debug names used by tokenize -O detail)
 
 
@@ -275,9 +277,11 @@ class BatchResult:
     tokenizer option compact_tokens the device returns 16-byte records (`compact`); `tokens` is then rebuilt on the
     host from them and the sentences' UTF-8.  With Tokenizer.marginals(theta) on, `token_probs` (float32[n_tokens])
     and `path_probs` (float32[n_sent]) hold the marginal of every token and the probability of each sentence's best
-    path; both are None otherwise."""
+    path; both are None otherwise.  With Tokenizer.lattice() on, `node_offsets[i]..node_offsets[i+1]` index `nodes`
+    (TOKEN_DTYPE), `node_links` (LINK_DTYPE) and `node_probs` (float32, None without marginals): every node of sentence
+    i's lattice (include/vibrato_b200.h); all four are None otherwise."""
 
-    def __init__(self, tokenizer, handle, sentences_utf8, byte_offsets, compact=False, marginals=False):
+    def __init__(self, tokenizer, handle, sentences_utf8, byte_offsets, compact=False, marginals=False, lattice=False):
         self._tok = tokenizer
         self._h = handle
         self._free = lib().vbt_result_free
@@ -303,6 +307,20 @@ class BatchResult:
                                 else np.empty(0, dtype=np.float32))
             self.path_probs = (np.ctypeslib.as_array(C.cast(pp, f32), shape=(self.n_sent,)) if self.n_sent
                                else np.empty(0, dtype=np.float32))
+        self.node_offsets = self.nodes = self.node_links = self.node_probs = None
+        if lattice:
+            po, pn, pl, pp, nn = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_uint64()
+            check(lib().vbt_result_lattice(handle, C.byref(po), C.byref(pn), C.byref(pl), C.byref(pp), C.byref(nn)))
+            n = nn.value
+            self.node_offsets = np.ctypeslib.as_array(C.cast(po, C.POINTER(C.c_uint64)), shape=(self.n_sent + 1,))
+            u8 = C.POINTER(C.c_uint8)
+            self.nodes = (np.ctypeslib.as_array(C.cast(pn, u8), shape=(n * TOKEN_DTYPE.itemsize,)).view(TOKEN_DTYPE)
+                          if n else np.empty(0, dtype=TOKEN_DTYPE))
+            self.node_links = (np.ctypeslib.as_array(C.cast(pl, u8), shape=(n * LINK_DTYPE.itemsize,)).view(LINK_DTYPE)
+                               if n else np.empty(0, dtype=LINK_DTYPE))
+            if pp.value:
+                self.node_probs = (np.ctypeslib.as_array(C.cast(pp, C.POINTER(C.c_float)), shape=(n,)) if n
+                                   else np.empty(0, dtype=np.float32))
         self._utf8 = sentences_utf8
         self._off = byte_offsets
 
@@ -316,6 +334,9 @@ class BatchResult:
             if self.token_probs is not None:
                 self.token_probs = self.token_probs.copy()
                 self.path_probs = self.path_probs.copy()
+            for name in ("node_offsets", "nodes", "node_links", "node_probs"):
+                if getattr(self, name) is not None:
+                    setattr(self, name, getattr(self, name).copy())
             self._free(h)
 
     def __del__(self):
@@ -344,6 +365,19 @@ class BatchResult:
         tp = self.token_probs
         return [Token(self._tok, s, self.tokens[k], None if tp is None else float(tp[k])) for k in range(a, b)]
 
+    def num_nodes(self, i):
+        return int(self.node_offsets[i + 1] - self.node_offsets[i])
+
+    def sentence_nodes(self, i):
+        """LatticeNode views of sentence i's lattice, in node order (needs Tokenizer.lattice())."""
+        if self.nodes is None:
+            raise VibratoError(1, "no lattice: switch it on with Tokenizer.lattice() before tokenising")
+        s = bytes(self._utf8[int(self._off[i]):int(self._off[i + 1])])
+        a, b = int(self.node_offsets[i]), int(self.node_offsets[i + 1])
+        npb = self.node_probs
+        return [LatticeNode(self._tok, s, self.nodes[k], self.node_links[k], None if npb is None else float(npb[k]))
+                for k in range(a, b)]
+
 
 OUTPUT_MODES = {None: 0, "none": 0, "mecab": 1, "wakati": 2, "detail": 3}  # tokenize/src/main.rs:12-29
 
@@ -361,6 +395,7 @@ class Tokenizer:
         self._options = {}  # engine options set so far: replayed when the engine is rebuilt (ignore_space / max_grouping_len)
         self._format = None  # (node, unk, bos, eos) of output_format(), replayed after the options
         self._theta = 0.0  # marginals(), replayed before the format
+        self._lattice = 0  # lattice(), replayed before the format
         self._stream = 0
         self._counting = False
         self._free = lib().vbt_tokenizer_free
@@ -422,6 +457,8 @@ class Tokenizer:
                 check(lib().vbt_tokenizer_set_option(h, name.encode(), int(value)))
             if self._theta:
                 check(lib().vbt_tokenizer_set_marginals(h, self._theta))
+            if self._lattice:
+                check(lib().vbt_tokenizer_set_option(h, b"lattice", self._lattice))
             if self._format is not None:
                 self._set_format(h, self._format)
             if self._counting:
@@ -472,7 +509,7 @@ class Tokenizer:
                                                    byte_offsets.ctypes.data, n, bnd_offsets.ctypes.data,
                                                    bnd.ctypes.data if bnd.size else None, C.byref(h)))
         return BatchResult(self, h, utf8, byte_offsets, compact=bool(self._options.get("compact_tokens", 0)),
-                           marginals=self._theta > 0)
+                           marginals=self._theta > 0, lattice=self._lattice > 0)
 
     def tokenize_batch_device(self, d_utf8, d_byte_offsets, n_sent, n_bytes, d_bnd_offsets=None, d_bnd=None, n_bnd=0):
         """Device-resident variant: addresses in, (d_tok_offsets, d_tokens, n_tokens) out.  With d_bnd_offsets
@@ -494,6 +531,24 @@ class Tokenizer:
         a, b = C.c_uint64(), C.c_uint64()
         check(lib().vbt_last_device_marginals(self.handle(), C.byref(a), C.byref(b)))
         return a.value, b.value
+
+    def last_device_lattice(self):
+        """-> (d_node_offsets, d_nodes, d_links, d_node_probs, n_nodes): device addresses (uint64[n_sent + 1],
+        vbt_token[n_nodes], vbt_lattice_link[n_nodes], float32[n_nodes] or 0 without marginals) of the lattice of the
+        last tokenize_batch_device call, valid until the next call."""
+        v = [C.c_uint64() for _ in range(5)]
+        check(lib().vbt_last_device_lattice(self.handle(), *[C.byref(x) for x in v]))
+        return tuple(x.value for x in v)
+
+    def lattice(self, on=True, text=False):
+        """Lattice output: results then carry every node of each sentence's lattice (BatchResult.nodes /
+        node_links / node_probs, sentence_nodes()), with its best predecessor, a best-path flag and, with marginals,
+        its marginal.  text=True also renders the nodes in place of the tokens in the output text (MeCab -a).
+        Single-device tokenizers only; the "small_batch" route steps aside.  Definition: include/vibrato_b200.h."""
+        value = (2 if text else 1) if on else 0
+        check(lib().vbt_tokenizer_set_option(self.handle(), b"lattice", value))
+        self._lattice = value
+        return self
 
     def marginals(self, theta):
         """Marginal probabilities at temperature `theta` (> 0; None or 0 switches them off): P(path) is proportional
@@ -538,6 +593,9 @@ class Tokenizer:
 
     def set_option(self, name, value):
         check(lib().vbt_tokenizer_set_option(self.handle(), name.encode(), int(value)))
+        if name == "lattice":  # replayed with lattice()'s state, after the marginals
+            self._lattice = int(value)
+            return
         if name != "connid_counting":  # accumulated counts cannot be carried into a rebuilt engine
             self._options[name] = int(value)
         if name == "output_mode":  # a fixed mode replaces an output format
@@ -681,6 +739,25 @@ class Token:
         return self._p
 
 
+class LatticeNode(Token):
+    """One node of a sentence's lattice (Tokenizer.lattice): Token's accessors (start_char is the node's start_word,
+    total_cost its min_cost), plus its best predecessor, best-path flag and marginal."""
+
+    __slots__ = ("_link",)
+
+    def __init__(self, tokenizer, sentence_bytes, rec, link, prob=None):
+        super().__init__(tokenizer, sentence_bytes, rec, prob)
+        self._link = link
+
+    def prev(self):
+        """Index of the best predecessor in the sentence's node list, or None for BOS."""
+        p = int(self._link["prev"])
+        return None if p < 0 else p
+
+    def is_best(self):
+        return bool(int(self._link["flags"]) & NODE_BEST)
+
+
 class Worker:
     """vibrato::tokenizer::worker::Worker (worker.rs:13-74): the one-sentence loop of
     tokenize/src/main.rs:78-81 keeps working unmodified (one tiny batch per call)."""
@@ -690,12 +767,14 @@ class Worker:
         self._sent = b""
         self._bounds = None
         self._tokens = []
+        self._nodes = []
 
     def reset_sentence(self, text, boundaries=None):
         """boundaries: required token boundaries, byte offsets into the sentence (see Tokenizer.tokenize_batch)."""
         self._sent = text.encode("utf-8") if isinstance(text, str) else bytes(text)
         self._bounds = None if boundaries is None else list(boundaries)
         self._tokens = []
+        self._nodes = []
 
     def tokenize(self):
         if not self._sent:  # worker.rs:50-52
@@ -704,6 +783,9 @@ class Worker:
         tp = res.token_probs
         self._tokens = [Token(self._tok, self._sent, r.copy(), None if tp is None else float(tp[k]))
                         for k, r in enumerate(res.tokens)]
+        self._nodes = res.sentence_nodes(0) if res.nodes is not None else []
+        for nd in self._nodes:
+            nd._r, nd._link = nd._r.copy(), nd._link.copy()
         res.close()
 
     def num_tokens(self):
@@ -714,3 +796,13 @@ class Worker:
 
     def token_iter(self):
         return iter(self._tokens)
+
+    def num_nodes(self):
+        """Nodes of the sentence's lattice (Tokenizer.lattice())."""
+        return len(self._nodes)
+
+    def node(self, i):
+        return self._nodes[i]
+
+    def node_iter(self):
+        return iter(self._nodes)

@@ -22,7 +22,9 @@ static void usage() {
                  "         [--boundary-marker C]       (an ASCII byte other than newline: removed from every line, it\n"
                  "                                      marks a required token boundary where it stood)\n"
                  "         [-m|--marginal -t|--theta F] (marginal probabilities at temperature F > 0: -F may print\n"
-                 "                                      each token's with %%pP; -O output is unchanged)\n");
+                 "                                      each token's with %%pP; -O output is unchanged)\n"
+                 "         [-a|--all-morphs]           (every lattice node in place of the tokens, like MeCab -a: -O and\n"
+                 "                                      -F render nodes, -F may print %%pb; needs --format-on device)\n");
 }
 
 int main(int argc, char** argv) {
@@ -33,7 +35,7 @@ int main(int argc, char** argv) {
     std::string node_format, unk_format, bos_format, eos_format;
     bool has_node = false, has_unk = false, has_bos = false, has_eos = false;
     std::string marker;
-    bool marginal = false, has_theta = false;
+    bool marginal = false, has_theta = false, all_morphs = false;
     double theta = 0;
     for (int i = 1; i < argc; ++i) {
         std::string a = argv[i];
@@ -58,6 +60,7 @@ int main(int argc, char** argv) {
         else if (a == "--eos-format") eos_format = next(), has_eos = true;
         else if (a == "--boundary-marker") marker = next();
         else if (a == "-m" || a == "--marginal") marginal = true;
+        else if (a == "-a" || a == "--all-morphs") all_morphs = true;
         else if (a == "-t" || a == "--theta") {
             const std::string v = next();
             char* end = nullptr;
@@ -77,7 +80,7 @@ int main(int argc, char** argv) {
     const bool bounded = !marker.empty();
     // -m needs --theta, and --theta belongs to -m
     if (batch_lines_arg == 0 || (has_node && format_on == "host") || (!has_node && (has_unk || has_bos || has_eos)) ||
-        marginal != has_theta ||
+        marginal != has_theta || (all_morphs && format_on == "host") ||
         (bounded && (marker.size() != 1 || marker[0] == '\n' || (marker[0] & 0x80)))) {
         usage();
         return 2;
@@ -98,6 +101,7 @@ int main(int argc, char** argv) {
         Tokenizer tokenizer =
             Tokenizer(std::move(dict)).ignore_space(ignore_space).max_grouping_len(max_grouping_len).devices(devices);
         if (marginal) tokenizer.marginals(theta);  // before -F, which may print %pP
+        if (all_morphs) tokenizer.lattice(true, true);  // before -F, which may print %pb
         if (has_node) {
             const std::string_view node = node_format, unk = unk_format, bos = bos_format, eos = eos_format;
             tokenizer.output_format(&node, has_unk ? &unk : nullptr, has_bos ? &bos : nullptr, has_eos ? &eos : nullptr);
@@ -107,7 +111,8 @@ int main(int argc, char** argv) {
         std::fprintf(stderr, "Ready to tokenize\n");
         const bool tty_out = isatty(STDOUT_FILENO), tty_in = isatty(STDIN_FILENO);
         const size_t batch_lines = tty_in ? 1 : batch_lines_arg;
-        if (batch_lines == 1) tokenizer.small_batch(1);  // a line at a time: one kernel launch per line
+        // a line at a time: one kernel launch per line (k_small_batch has no lattice: -a takes the usual route)
+        if (batch_lines == 1 && !all_morphs) tokenizer.small_batch(1);
         std::string out;
         cli::Packed pk;
         std::string line;

@@ -162,6 +162,21 @@ class BatchResult {
         check(vbt_result_marginals(r_.get(), nullptr, &pp));
         return pp;
     }
+    // Lattice output (Tokenizer::lattice before the batch, see vbt_result_lattice): node_offsets()[i] ..
+    // node_offsets()[i + 1] index sentence i's nodes, links and (with marginals, else nullptr) node probabilities.
+    // Throws on a result made without the lattice.
+    struct Lattice {
+        const uint64_t* node_offsets = nullptr;
+        const vbt_token* nodes = nullptr;
+        const vbt_lattice_link* links = nullptr;
+        const float* node_probs = nullptr;
+        uint64_t n_nodes = 0;
+    };
+    Lattice lattice() const {
+        Lattice l;
+        check(vbt_result_lattice(r_.get(), &l.node_offsets, &l.nodes, &l.links, &l.node_probs, &l.n_nodes));
+        return l;
+    }
 
    private:
     std::unique_ptr<vbt_result, void (*)(vbt_result*)> r_;
@@ -253,6 +268,22 @@ class Tokenizer {
         return {tp, pp};
     }
     bool has_marginals() const { return marginals_; }
+    // Lattice output (the option "lattice", see vbt_result_lattice): BatchResult::lattice(); text = true also renders
+    // the nodes in place of the tokens in the output text (MeCab -a).  Set text before a format that prints %pb.
+    void lattice(bool on = true, bool text = false) const {
+        check(vbt_tokenizer_set_option(handle(), "lattice", on ? (text ? 2 : 1) : 0));
+        lattice_ = on;
+    }
+    bool has_lattice() const { return lattice_; }
+    // Device addresses of the last tokenize_batch_device call's lattice (node_prob 0 without marginals).
+    struct DeviceLattice {
+        uint64_t node_offsets = 0, nodes = 0, links = 0, node_probs = 0, n_nodes = 0;
+    };
+    DeviceLattice last_device_lattice() const {
+        DeviceLattice d;
+        check(vbt_last_device_lattice(handle(), &d.node_offsets, &d.nodes, &d.links, &d.node_probs, &d.n_nodes));
+        return d;
+    }
     // Worker::init_connid_counter / update_connid_counts / compute_connid_probs (worker.rs:77-103): after
     // init_connid_counter() every batch is counted, an empty sentence counting nothing
     void init_connid_counter() const { check(vbt_tokenizer_set_option(handle(), "connid_counting", 1)); }
@@ -308,6 +339,7 @@ class Tokenizer {
     bool ignore_space_ = false;
     uint64_t max_grouping_len_ = 0;
     mutable bool marginals_ = false;
+    mutable bool lattice_ = false;
     mutable std::shared_ptr<vbt_tokenizer> h_;
 };
 
@@ -348,6 +380,20 @@ class Token {  // token.rs:8-92
     float p_;
 };
 
+// One node of a sentence's lattice (Tokenizer::lattice): Token's accessors (start_char = start_word, total_cost =
+// min_cost), plus its best predecessor, best-path flag and marginal.
+class LatticeNode : public Token {
+   public:
+    LatticeNode(const Tokenizer* t, std::string_view sentence, vbt_token rec, vbt_lattice_link link,
+                float prob = std::numeric_limits<float>::quiet_NaN())
+        : Token(t, sentence, rec, prob), link_(link) {}
+    int32_t prev() const { return link_.prev; }  // index in the sentence's node list, -1 for BOS
+    bool is_best() const { return (link_.flags & VBT_NODE_BEST) != 0; }
+
+   private:
+    vbt_lattice_link link_;
+};
+
 class Worker {  // worker.rs:13-74
    public:
     explicit Worker(const Tokenizer* t) : t_(t) {}
@@ -356,6 +402,9 @@ class Worker {  // worker.rs:13-74
         bnd_.clear();
         bounded_ = false;
         toks_.clear();
+        nodes_.clear();
+        links_.clear();
+        nprobs_.clear();
     }
     // With required boundaries (byte offsets into s; see Tokenizer::tokenize_batch).
     void reset_sentence(std::string_view s, std::vector<uint32_t> boundaries) {
@@ -372,6 +421,19 @@ class Worker {  // worker.rs:13-74
         toks_.assign(r.tokens(), r.tokens() + r.n_tokens());
         probs_.clear();
         if (t_->has_marginals() && r.n_tokens()) probs_.assign(r.token_probs(), r.token_probs() + r.n_tokens());
+        nodes_.clear();
+        links_.clear();
+        nprobs_.clear();
+        if (t_->has_lattice()) {
+            const BatchResult::Lattice l = r.lattice();
+            nodes_.assign(l.nodes, l.nodes + l.n_nodes);
+            links_.assign(l.links, l.links + l.n_nodes);
+            if (l.node_probs) nprobs_.assign(l.node_probs, l.node_probs + l.n_nodes);
+        }
+    }
+    size_t num_nodes() const { return nodes_.size(); }
+    LatticeNode node(size_t i) const {
+        return nprobs_.empty() ? LatticeNode(t_, sent_, nodes_[i], links_[i]) : LatticeNode(t_, sent_, nodes_[i], links_[i], nprobs_[i]);
     }
     size_t num_tokens() const { return toks_.size(); }
     Token token(size_t i) const {
@@ -385,6 +447,9 @@ class Worker {  // worker.rs:13-74
     bool bounded_ = false;
     std::vector<vbt_token> toks_;
     std::vector<float> probs_;
+    std::vector<vbt_token> nodes_;  // Tokenizer::lattice
+    std::vector<vbt_lattice_link> links_;
+    std::vector<float> nprobs_;
 };
 
 inline Worker Tokenizer::new_worker() const { return Worker(this); }

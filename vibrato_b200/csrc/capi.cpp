@@ -562,9 +562,10 @@ int32_t vbt_tokenizer_set_output_format(vbt_tokenizer* t, const char* node, size
             return;
         }
         // an empty string may come with any pointer: only NULL means "not given"
-        // %pP has a value only while the tokenizer computes marginals
+        // %pP has a value only while the tokenizer computes marginals, %pb only in lattice text (where the "prev"
+        // directives have none)
         const vbt::FormatProgram p = vbt::compile_format({node, node_len}, {unk, unk_len}, {bos, bos_len}, {eos, eos_len},
-                                                         t->e->marginals() > 0);
+                                                         t->e->marginals() > 0, t->e->lattice() == 2);
         t->e->set_format(&p);
     });
 }
@@ -590,6 +591,28 @@ int32_t vbt_last_device_marginals(const vbt_tokenizer* t, uint64_t* d_token_prob
     return guarded([&] {
         need(t, "t");
         t->e->device_marginals(d_token_prob, d_path_prob);
+    });
+}
+
+int32_t vbt_result_lattice(const vbt_result* r, const uint64_t** node_offsets, const vbt_token** nodes,
+                           const vbt_lattice_link** links, const float** node_prob, uint64_t* n_nodes) {
+    return guarded([&] {
+        need(r, "r");
+        if (!r->r->has_lat)
+            throw vbt::Error(vbt::kInvalidArgument, "no lattice: set the tokenizer option \"lattice\" before tokenising");
+        if (node_offsets) *node_offsets = r->r->node_off;
+        if (nodes) *nodes = static_cast<const vbt_token*>(r->r->nodes);
+        if (links) *links = static_cast<const vbt_lattice_link*>(r->r->links);
+        if (node_prob) *node_prob = r->r->has_marg ? r->r->node_prob : nullptr;
+        if (n_nodes) *n_nodes = r->r->n_nodes;
+    });
+}
+
+int32_t vbt_last_device_lattice(const vbt_tokenizer* t, uint64_t* d_node_offsets, uint64_t* d_nodes, uint64_t* d_links,
+                                uint64_t* d_node_prob, uint64_t* n_nodes) {
+    return guarded([&] {
+        need(t, "t");
+        t->e->device_lattice(d_node_offsets, d_nodes, d_links, d_node_prob, n_nodes);
     });
 }
 

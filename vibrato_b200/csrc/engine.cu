@@ -57,6 +57,7 @@ struct Control {  // one small block zeroed per batch and read back once
     unsigned long long n_tokens;
     unsigned long long counters[kNumCounters];
     unsigned long long text_bytes;  // output stage: the text total of the batch (or chunk)
+    unsigned long long n_nodes;     // lattice output: the node total of the batch (or chunk)
     uint32_t flags;
     uint32_t total_slots;
 };
@@ -148,11 +149,13 @@ struct Workspace {  // every per-(chunk of a)-batch device array; two of them le
         ends_meta, cand, ends_hot, ends_cold, scan_tmp, stats, iota, sort_keys, order;
     DevBuf bnd_dist;  // bounded batches only: Batch::bnd_dist
     DevBuf m_fill, m_ncand, m_cand_entry, m_R, m_ab, m_r_eos, m_a_eos;  // marginals only: MargArgs
+    DevBuf l_row_base, l_n_nodes;  // lattice output only: LatticeArgs
     cudaStream_t stream = nullptr;
     void release() {
         for (DevBuf* b : {&n_slots, &slot_off, &eos, &n_tok, &code_sys, &code_usr, &cinfo, &groupable, &byte_pos, &info,
                           &info_ex, &ends_cnt, &ends_meta, &cand, &ends_hot, &ends_cold, &scan_tmp, &stats, &iota,
-                          &sort_keys, &order, &bnd_dist, &m_fill, &m_ncand, &m_cand_entry, &m_R, &m_ab, &m_r_eos, &m_a_eos})
+                          &sort_keys, &order, &bnd_dist, &m_fill, &m_ncand, &m_cand_entry, &m_R, &m_ab, &m_r_eos, &m_a_eos,
+                          &l_row_base, &l_n_nodes})
             b->release();
     }
 };
@@ -170,6 +173,8 @@ struct OutSlot {  // where one (chunk of a) batch leaves its results; two of the
     DevBuf sent_len, text_off, text;  // output stage (k_format_*)
     DevBuf token_prob, path_prob;     // marginals
     bool marg = false;                // the (chunk of a) batch in this slot was run with marginals
+    DevBuf node_off, nodes, links, node_prob;  // lattice output (LatticeArgs)
+    bool lat = false;                          // the (chunk of a) batch in this slot was run with the lattice
     Control* h_ctrl = nullptr;
     cudaEvent_t ev[kNumStages + 1];
     cudaEvent_t done = nullptr, drained = nullptr;
@@ -204,6 +209,7 @@ class EngineImpl final : public Engine {
         for (auto& e : base_ready_) CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
         tok_base_.ensure(8);
         text_base_.ensure(8);
+        node_base_.ensure(8);
         BlobHeader h;
         if (host_blob) {
             if (n_bytes < sizeof(BlobHeader)) throw Error(kInvalidArgument, "dictionary image too small");
@@ -321,7 +327,8 @@ class EngineImpl final : public Engine {
         cudaStreamSynchronize(in_stream_);
         cudaStreamSynchronize(out_stream_);
         for (auto& o : out_) {
-            for (DevBuf* b : {&o.tok_off, &o.tokens, &o.ctrl, &o.sent_len, &o.text_off, &o.text, &o.token_prob, &o.path_prob})
+            for (DevBuf* b : {&o.tok_off, &o.tokens, &o.ctrl, &o.sent_len, &o.text_off, &o.text, &o.token_prob, &o.path_prob,
+                              &o.node_off, &o.nodes, &o.links, &o.node_prob})
                 b->release();
             pinned_free(o.h_ctrl);
             for (auto& ev : o.ev) cudaEventDestroy(ev);
@@ -337,6 +344,7 @@ class EngineImpl final : public Engine {
         cudaStreamDestroy(out_stream_);
         tok_base_.release();
         text_base_.release();
+        node_base_.release();
         for (DevBuf* b : {&fmt_prog_, &ft_keep_, &ft_off_, &ft_bytes_}) b->release();
         for (auto* b : {&blob_own_, &in_utf8_, &in_off_, &in_bnd_off_, &in_bnd_, &connid_, &connid_try_}) b->release();
         for (auto& w : ws_) w.release();
@@ -356,6 +364,7 @@ class EngineImpl final : public Engine {
             pinned_free(r->text);
             pinned_free(r->token_prob);
             pinned_free(r->path_prob);
+            for (void* p : {static_cast<void*>(r->node_off), r->nodes, r->links, static_cast<void*>(r->node_prob)}) pinned_free(p);
             delete r;
         }
         cudaStreamDestroy(own_stream_);
@@ -410,6 +419,17 @@ class EngineImpl final : public Engine {
             viterbi_kernel_ = int(value);
         } else if (name == "counting") {
             counting_ = value != 0;
+        } else if (name == "lattice") {
+            // every lattice node next to the tokens (1), and in place of them in the output text (2)
+            if (value < 0 || value > 2) throw Error(kInvalidArgument, "lattice must be 0 (off), 1 (nodes) or 2 (nodes, and the text renders them)");
+            if (value == 2 && output_mode_ == kOutFormat && (fmt_uses_ & kUsesPrev))
+                throw Error(kInvalidArgument,
+                            "the output format prints a \"prev\" directive (%M %pS %pn %pC %pL), which lattice text has no value for: "
+                            "change the format before setting lattice = 2");
+            if (value != 2 && output_mode_ == kOutFormat && (fmt_uses_ & kUsesBest))
+                throw Error(kInvalidArgument, "the output format prints %pb, which only lattice text has: change the format before setting lattice below 2");
+            cudaStreamSynchronize(stream_);
+            lattice_ = int(value);
         } else if (name == "small_batch") {
             // host batches of at most `value` sentences and kEagerBytes bytes take k_small_batch (0 = never)
             if (value < 0 || value > kSmallBatchMax) throw Error(kInvalidArgument, "small_batch must be between 0 and 65536");
@@ -425,6 +445,10 @@ class EngineImpl final : public Engine {
         if (tok_bytes_ != 24) throw Error(kInvalidArgument, "compact_tokens and output formats exclude each other");
         if ((p->uses & kUsesProb) && theta_ == 0)
             throw Error(kInvalidArgument, "%pP needs marginals: switch them on before setting the format");
+        if ((p->uses & kUsesBest) && lattice_ != 2)
+            throw Error(kInvalidArgument, "%pb needs lattice text: set the option \"lattice\" to 2 before setting the format");
+        if ((p->uses & kUsesPrev) && lattice_ == 2)  // compile_format names the directive; this guards other callers
+            throw Error(kInvalidArgument, "lattice text has no previous token: the format may not print %M %pS %pn %pC %pL");
         try {
             fmt_prog_.ensure(sizeof(FormatProgram));
             CK(cudaMemcpy(fmt_prog_.p, p, sizeof(FormatProgram), cudaMemcpyHostToDevice));
@@ -437,6 +461,7 @@ class EngineImpl final : public Engine {
         fmt_uses_ = p->uses;
         text_per_sent_ = p->per_sentence;
         text_per_byte_[kOutFormat] = kFormatTextPerByte;  // learned anew for every format
+        text_per_byte_lat_[kOutFormat] = kFormatTextPerByte * kLatticeTextFactor;
     }
     void set_marginals(double theta) override {
         if (!(theta >= 0) || !std::isfinite(theta))
@@ -447,10 +472,21 @@ class EngineImpl final : public Engine {
         theta_ = theta;
     }
     double marginals() const override { return theta_; }
+    int lattice() const override { return lattice_; }
     void device_marginals(uint64_t* d_token_prob, uint64_t* d_path_prob) const override {
         if (!dev_marg_) throw Error(kInvalidArgument, "the last device-resident call ran without marginals");
         if (d_token_prob) *d_token_prob = reinterpret_cast<uint64_t>(out_[0].token_prob.p);
         if (d_path_prob) *d_path_prob = reinterpret_cast<uint64_t>(out_[0].path_prob.p);
+    }
+    void device_lattice(uint64_t* d_node_off, uint64_t* d_nodes, uint64_t* d_links, uint64_t* d_node_prob,
+                        uint64_t* n_nodes) const override {
+        if (!dev_lat_) throw Error(kInvalidArgument, "the last device-resident call ran without the lattice");
+        const OutSlot& o = out_[0];
+        if (d_node_off) *d_node_off = reinterpret_cast<uint64_t>(o.node_off.p);
+        if (d_nodes) *d_nodes = reinterpret_cast<uint64_t>(o.nodes.p);
+        if (d_links) *d_links = reinterpret_cast<uint64_t>(o.links.p);
+        if (d_node_prob) *d_node_prob = o.marg ? reinterpret_cast<uint64_t>(o.node_prob.p) : 0;
+        if (n_nodes) *n_nodes = o.h_ctrl->n_nodes;
     }
     void set_stream(uint64_t stream) override {
         cudaStreamSynchronize(stream_);
@@ -479,13 +515,14 @@ class EngineImpl final : public Engine {
         if (bnd && bnd->n == 0 && device_offsets_zero(bnd->off, n_sent)) bnd = nullptr;  // no boundary at all
         DevBounds bd;
         if (bnd) bd = DevBounds{reinterpret_cast<const unsigned long long*>(bnd->off), bnd->bnd, bnd->n};
-        dev_marg_ = false;
+        dev_marg_ = dev_lat_ = false;
         run_whole(reinterpret_cast<const uint8_t*>(d_utf8), reinterpret_cast<const unsigned long long*>(d_byte_off),
                   uint32_t(n_sent), n_bytes, bd);
         *d_tok_off = reinterpret_cast<uint64_t>(out_[0].tok_off.p);
         *d_tokens = reinterpret_cast<uint64_t>(out_[0].tokens.p);
         *n_tokens = out_[0].h_ctrl->n_tokens;
         dev_marg_ = out_[0].marg;
+        dev_lat_ = out_[0].lat;
     }
 
     // Host path.  Large batches are cut into chunks that flow through three streams: the H2D copy of
@@ -515,8 +552,8 @@ class EngineImpl final : public Engine {
         const uint32_t chunk = chunk_sentences_;
         const bool chunked = chunk > 0 && n_sent > chunk + chunk / 2;
         const bool fmt = output_mode_ != kOutNone;
-        // k_small_batch computes no marginals: with them on, small batches take the usual route
-        if (small_batch_ && n_sent <= small_batch_ && !chunked && n_bytes <= kEagerBytes && !counting_ && !connid_on_ && theta_ == 0 &&
+        // k_small_batch computes no marginals and no lattice: with either on, small batches take the usual route
+        if (small_batch_ && n_sent <= small_batch_ && !chunked && n_bytes <= kEagerBytes && !counting_ && !connid_on_ && theta_ == 0 && !lattice_ &&
             (!bnd || small_bounds_fit(*bnd, n_sent))) {
             if (HostResult* r = run_small(utf8 + first, off, n_sent, n_bytes, bnd)) return r;
             // the batch outgrew the scratch of k_small_batch: it runs again on the route below
@@ -526,7 +563,7 @@ class EngineImpl final : public Engine {
             if (!chunked) {
                 h2d(in_off_.p, off, (size_t(n_sent) + 1) * 8, stream_, off_pinned && off == byte_off);
                 h2d(in_utf8_.p, utf8 + first, n_bytes, stream_, utf8_pinned);
-                if (n_bytes <= kEagerBytes && output_mode_ == kOutNone) {
+                if (n_bytes <= kEagerBytes && output_mode_ == kOutNone && !lattice_) {
                     // Small batches (a per-sentence Worker loop ends up here) are all latency: the result copies are
                     // queued behind the kernels with an upper bound for the token count (a token spans >= 1 byte), so
                     // that the call makes ONE host synchronisation instead of two.
@@ -553,6 +590,11 @@ class EngineImpl final : public Engine {
                     if (r->n_tokens)
                         CK(cudaMemcpyAsync(r->token_prob, o.token_prob.p, r->n_tokens * 4, cudaMemcpyDeviceToHost, stream_));
                     if (n_sent) CK(cudaMemcpyAsync(r->path_prob, o.path_prob.p, size_t(n_sent) * 4, cudaMemcpyDeviceToHost, stream_));
+                }
+                if (r->has_lat) {
+                    r->n_nodes = o.h_ctrl->n_nodes;
+                    ensure_lat_host(r, n_sent, r->n_nodes);
+                    copy_lattice(o, r, 0, 0, n_sent, true, stream_);
                 }
                 r->has_text = false;
                 if (fmt) format_text(d_utf8, d_off, n_sent, r);
@@ -589,13 +631,15 @@ class EngineImpl final : public Engine {
                 o.tok_off.ensure((size_t(max_chunk_sent) + 1) * 8, 1.25);
                 o.tokens.ensure(size_t(max_chunk_bytes) * 24 + 24, 1.25);
                 ensure_marg_out(o, max_chunk_sent, max_chunk_bytes);
+                ensure_lat_out(o, ws_[0], max_chunk_sent);
             }
             // a pinned result sized from the learned tokens-per-byte ratio (grown below if short)
             HostResult* r = acquire(n_sent, uint64_t(double(n_bytes) * tok_per_byte_) + 1024);
+            if (r->has_lat) ensure_lat_host(r, n_sent, uint64_t(double(n_bytes) * node_per_byte_) + 1024);
             // output stage: each slot's text buffer holds the text a chunk is expected to produce (at most 4 bytes per
             // sentence plus the learned ratio per input byte); a chunk with more text flags itself and the batch is
             // re-run with the ratio it measured
-            const double text_ratio = text_per_byte_[output_mode_];
+            const double text_ratio = text_ratio_ref();
             if (fmt) {
                 for (int i = 0; i < 2; ++i) {
                     ensure_format(out_[i], ws_[dual_stream_ ? i : 0], max_chunk_sent);
@@ -605,6 +649,7 @@ class EngineImpl final : public Engine {
                 CK(cudaMemsetAsync(text_base_.p, 0, 8, stream_));
             }
             CK(cudaMemsetAsync(tok_base_.p, 0, 8, stream_));
+            if (lattice_) CK(cudaMemsetAsync(node_base_.p, 0, 8, stream_));
             connid_begin(stream_);
             h2d(in_off_.p, off, (size_t(n_sent) + 1) * 8, stream_, off_pinned && off == byte_off);
             CK(cudaEventRecord(in_done_, stream_));
@@ -613,7 +658,7 @@ class EngineImpl final : public Engine {
             std::memset(stage_ms_, 0, sizeof(stage_ms_));
             std::memset(counters_, 0, sizeof(counters_));
             launches_ = 0;
-            uint64_t tok_total = 0, text_total = 0;
+            uint64_t tok_total = 0, text_total = 0, node_total = 0;
             double text_need = 0;  // text bytes per input byte beyond text_per_sent_ per sentence, largest over the sound chunks
             uint32_t route = kRouteNone;
             bool overflow = false, bad_utf8 = false, bad_offsets = false, slots_overflow = false, text_overflow = false;
@@ -656,6 +701,7 @@ class EngineImpl final : public Engine {
                     for (int i = 0; i < kNumCounters; ++i) counters_[i] += o.h_ctrl->counters[i];
                 pool_need_ = std::max<uint64_t>(pool_need_, o.h_ctrl->pool_ctr);
                 const uint64_t nt = o.h_ctrl->n_tokens, nx = fmt ? o.h_ctrl->text_bytes : 0;
+                const uint64_t nn = lattice_ ? o.h_ctrl->n_nodes : 0;
                 if (fmt && !(o.h_ctrl->flags & (kFlagsStandDown | kFlagUtf8Error | kFlagPoolOverflow)))
                     text_need = std::max(text_need, (double(nx) - double(text_per_sent_) * (s1 - s0)) / double(std::max<uint64_t>(1, off[s1] - off[s0])));
                 if (!overflow && !text_overflow && !bad_utf8 && !bad_offsets && !bad_bounds) {
@@ -688,6 +734,13 @@ class EngineImpl final : public Engine {
                         if (s1 > s0)
                             CK(cudaMemcpyAsync(r->path_prob + s0, o.path_prob.p, size_t(s1 - s0) * 4, cudaMemcpyDeviceToHost, out_stream_));
                     }
+                    if (r->has_lat) {  // node offsets are global already (node_base_); the arrays grow like the tokens
+                        if (!lat_fits(r, node_total + nn)) {
+                            CK(cudaStreamSynchronize(out_stream_));
+                            grow_lat_host(r, size_t(double(node_total + nn) * 1.5) + 4096, node_total);
+                        }
+                        copy_lattice(o, r, node_total, s0, s1 - s0, last, out_stream_);
+                    }
                     if (fmt) {
                         if (text_total + nx + 1 > r->cap_text) {  // grown like the token buffer
                             CK(cudaStreamSynchronize(out_stream_));
@@ -706,6 +759,7 @@ class EngineImpl final : public Engine {
                 CK(cudaEventRecord(o.drained, out_stream_));
                 tok_total += nt;
                 text_total += nx;
+                node_total += nn;
             };
             pool_need_ = 0;
             for (uint32_t c = 0; c < n_chunks; ++c) {
@@ -748,17 +802,19 @@ class EngineImpl final : public Engine {
                 if (slots_overflow) chars_per_byte_ = 1.0;
                 if (overflow)
                     cand_per_byte_ = std::max(cand_per_byte_ * 1.5, double(pool_need_) / double(std::max<uint64_t>(1, max_chunk_bytes)) * 1.2);
-                if (text_overflow) text_per_byte_[output_mode_] = std::max(text_ratio * 1.5, text_need * 1.05);
+                if (text_overflow) text_ratio_ref() = std::max(text_ratio * 1.5, text_need * 1.05);
                 continue;
             }
             if (max_chunk_bytes)
                 cand_per_byte_ = std::max(0.25, double(pool_need_) / double(max_chunk_bytes) * 1.25);
             if (n_bytes) tok_per_byte_ = std::max(0.02, double(tok_total) / double(n_bytes) * 1.1);
             if (n_bytes) chars_per_byte_ = std::min(1.0, double(slots_seen - n_sent) / double(n_bytes) * 1.10);
-            if (fmt) text_per_byte_[output_mode_] = std::max(0.5, text_need * 1.25);
+            if (fmt) text_ratio_ref() = std::max(0.5, text_need * 1.25);
+            if (n_bytes && lattice_) node_per_byte_ = std::max(0.1, double(node_total) / double(n_bytes) * 1.1);
             connid_commit(stream_);
             last_route_ = route;
             r->n_tokens = tok_total;
+            r->n_nodes = node_total;
             r->has_text = fmt;
             r->text_bytes = text_total;
             return r;
@@ -845,6 +901,45 @@ class EngineImpl final : public Engine {
         if (!out_[0].marg) throw Error(kInternal, "the shard was run without marginals");
         *d_token_prob = reinterpret_cast<uint64_t>(out_[0].token_prob.p);
         *d_path_prob = reinterpret_cast<uint64_t>(out_[0].path_prob.p);
+    }
+    uint64_t shard_nodes() const override {
+        if (!out_[0].lat) throw Error(kInternal, "the shard was run without the lattice");
+        return out_[0].h_ctrl->n_nodes;
+    }
+    void fetch_shard_lattice(uint64_t* h_node_off, void* h_nodes, void* h_links, float* h_node_prob, uint64_t node_base,
+                             bool last) override {
+        CK(cudaSetDevice(device_));
+        OutSlot& o = out_[0];
+        if (!o.lat) throw Error(kInternal, "the shard was run without the lattice");
+        if (node_base)
+            k_add_value<<<(shard_n_sent_ + 256) / 256, 256, 0, stream_>>>(o.node_off.as<unsigned long long>(), shard_n_sent_ + 1,
+                                                                         node_base);
+        const uint64_t nn = o.h_ctrl->n_nodes;
+        CK(cudaMemcpyAsync(h_node_off, o.node_off.p, (size_t(shard_n_sent_) + (last ? 1 : 0)) * 8, cudaMemcpyDeviceToHost, stream_));
+        if (nn) {
+            CK(cudaMemcpyAsync(h_nodes, o.nodes.p, nn * 24, cudaMemcpyDeviceToHost, stream_));
+            CK(cudaMemcpyAsync(h_links, o.links.p, nn * 8, cudaMemcpyDeviceToHost, stream_));
+            if (h_node_prob) {
+                if (!o.marg) throw Error(kInternal, "the shard was run without marginals");
+                CK(cudaMemcpyAsync(h_node_prob, o.node_prob.p, nn * 4, cudaMemcpyDeviceToHost, stream_));
+            }
+        }
+        CK(cudaStreamSynchronize(stream_));
+    }
+    void rebase_shard_lattice(uint64_t node_base) override {
+        CK(cudaSetDevice(device_));
+        if (node_base)
+            k_add_value<<<(shard_n_sent_ + 256) / 256, 256, 0, stream_>>>(out_[0].node_off.as<unsigned long long>(),
+                                                                         shard_n_sent_ + 1, node_base);
+        CK(cudaStreamSynchronize(stream_));
+    }
+    void shard_lattice(uint64_t* d_node_off, uint64_t* d_nodes, uint64_t* d_links, uint64_t* d_node_prob) const override {
+        const OutSlot& o = out_[0];
+        if (!o.lat) throw Error(kInternal, "the shard was run without the lattice");
+        *d_node_off = reinterpret_cast<uint64_t>(o.node_off.p);
+        *d_nodes = reinterpret_cast<uint64_t>(o.nodes.p);
+        *d_links = reinterpret_cast<uint64_t>(o.links.p);
+        *d_node_prob = o.marg ? reinterpret_cast<uint64_t>(o.node_prob.p) : 0;
     }
     int device() const override { return device_; }
     uint32_t token_bytes() const override { return tok_bytes_; }
@@ -992,8 +1087,70 @@ class EngineImpl final : public Engine {
         r->token_bytes = tok_bytes_;
         r->has_marg = theta_ > 0;
         if (r->has_marg) ensure_marg_host(r, n_sent, n_tokens);
+        r->has_lat = lattice_ != 0;
+        r->n_nodes = 0;
         return r;
     }
+
+    // Pinned lattice arrays of `r` for n_sent sentences and n_nodes nodes (contents not kept).
+    void ensure_lat_host(HostResult* r, uint64_t n_sent, uint64_t n_nodes) {
+        if ((n_sent + 1) * 8 > r->cap_node_off) {
+            pinned_free(r->node_off);
+            r->cap_node_off = size_t(double((n_sent + 1) * 8) * 1.25) + 64;
+            r->node_off = static_cast<uint64_t*>(pinned_alloc(r->cap_node_off));
+        }
+        if (!lat_fits(r, n_nodes)) grow_lat_host(r, size_t(double(n_nodes) * 1.25) + 64, 0);
+    }
+    static bool lat_fits(const HostResult* r, uint64_t n_nodes) {
+        return n_nodes * 24 <= r->cap_nodes && n_nodes * 8 <= r->cap_links && (!r->has_marg || n_nodes * 4 <= r->cap_nprob);
+    }
+    // Grows the node arrays of `r` to `nodes` entries, keeping the first `keep`.
+    static void grow_lat_host(HostResult* r, size_t nodes, uint64_t keep) {
+        auto grow = [&](void*& p, size_t& cap, size_t rec) {
+            if (nodes * rec <= cap) return;
+            void* bigger = pinned_alloc(nodes * rec);
+            if (keep) std::memcpy(bigger, p, keep * rec);
+            pinned_free(p);
+            p = bigger;
+            cap = nodes * rec;
+        };
+        grow(r->nodes, r->cap_nodes, 24);
+        grow(r->links, r->cap_links, 8);
+        if (r->has_marg) {
+            void* np = r->node_prob;
+            grow(np, r->cap_nprob, 4);
+            r->node_prob = static_cast<float*>(np);
+        }
+    }
+    // D2H of the lattice of slot `o` (n sentences, h_ctrl->n_nodes nodes) to sentence s0 / node `at` of `r`.
+    void copy_lattice(const OutSlot& o, HostResult* r, uint64_t at, uint64_t s0, uint64_t n, bool last, cudaStream_t st) {
+        const uint64_t nn = o.h_ctrl->n_nodes;
+        CK(cudaMemcpyAsync(r->node_off + s0, o.node_off.p, (size_t(n) + (last ? 1 : 0)) * 8, cudaMemcpyDeviceToHost, st));
+        if (!nn) return;
+        CK(cudaMemcpyAsync(static_cast<uint8_t*>(r->nodes) + at * 24, o.nodes.p, nn * 24, cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(static_cast<uint8_t*>(r->links) + at * 8, o.links.p, nn * 8, cudaMemcpyDeviceToHost, st));
+        if (r->has_marg) CK(cudaMemcpyAsync(r->node_prob + at, o.node_prob.p, nn * 4, cudaMemcpyDeviceToHost, st));
+    }
+
+    // Device lattice outputs of slot `o` for (chunks of) up to n_sent sentences: a node is a candidate placed in the
+    // pool, so the node arrays hold as many entries as the candidate pool of `w` (enqueue clips cand_cap to them and
+    // a larger batch takes the pool-overflow retry).
+    void ensure_lat_out(OutSlot& o, const Workspace& w, uint32_t n_sent) {
+        if (!lattice_) return;
+        const size_t n = w.cand.cap / 16 + 1;
+        o.node_off.ensure((size_t(n_sent) + 1) * 8, 1.25);
+        o.nodes.ensure(n * 24);
+        o.links.ensure(n * 8);
+        if (theta_ > 0) o.node_prob.ensure(n * 4);
+    }
+
+    // The nodes' links when lattice text prints %pb (the %pb instantiation of the format kernels), else nullptr.
+    const int2* fmt_links(const OutSlot& o) const {
+        return (lattice_ == 2 && output_mode_ == kOutFormat && (fmt_uses_ & kUsesBest)) ? o.links.as<int2>() : nullptr;
+    }
+
+    // Text bytes per input byte expected for the output mode; lattice text is learned apart (about 17x larger).
+    double& text_ratio_ref() { return lattice_ == 2 ? text_per_byte_lat_[output_mode_] : text_per_byte_[output_mode_]; }
 
     // Pinned marginal arrays of `r` for n_sent sentences and n_tokens tokens (contents not kept).
     static void ensure_marg_host(HostResult* r, uint64_t n_sent, uint64_t n_tokens) {
@@ -1033,8 +1190,9 @@ class EngineImpl final : public Engine {
         f.utf8 = d_utf8;
         f.byte_off = d_off;
         f.n_sent = n_sent;
-        f.tok_off = o.tok_off.as<unsigned long long>();
-        f.tokens = o.tokens.as<uint2>();
+        const bool nodes = lattice_ == 2;  // lattice text: the nodes are rendered as tokens
+        f.tok_off = nodes ? o.node_off.as<unsigned long long>() : o.tok_off.as<unsigned long long>();
+        f.tokens = nodes ? o.nodes.as<uint2>() : o.tokens.as<uint2>();
         f.sent_len = o.sent_len.as<unsigned long long>();
         f.text_off = o.text_off.as<unsigned long long>();
         f.text = o.text.as<uint8_t>();
@@ -1043,9 +1201,9 @@ class EngineImpl final : public Engine {
         f.flags = &dc->flags;
         f.text_total = &dc->text_bytes;
         set_mode(f);
-        f.token_prob = (o.marg && (fmt_uses_ & kUsesProb)) ? o.token_prob.as<float>() : nullptr;  // %pP
+        f.token_prob = (o.marg && (fmt_uses_ & kUsesProb)) ? (nodes ? o.node_prob.as<float>() : o.token_prob.as<float>()) : nullptr;  // %pP
         CK(cudaMemsetAsync(f.sent_len + n_sent, 0, 8, w.stream));
-        launch_format_len(dv_, f, w.stream);
+        launch_format_len(dv_, f, w.stream, fmt_links(o));
         exclusive_scan(w, f.sent_len, f.text_off, size_t(n_sent) + 1);
         return f;
     }
@@ -1062,7 +1220,7 @@ class EngineImpl final : public Engine {
         o.text.ensure(total + 16, 1.25);
         f.text = o.text.as<uint8_t>();
         f.text_cap = o.text.cap;
-        launch_format_write(dv_, f, stream_);
+        launch_format_write(dv_, f, stream_, fmt_links(o));
         launches_ += 2;
         return total;
     }
@@ -1377,6 +1535,10 @@ class EngineImpl final : public Engine {
             w.m_r_eos.ensure(ns * 8, 1.25);
             w.m_a_eos.ensure(ns * 8, 1.25);
         }
+        if (lattice_) {
+            w.l_row_base.ensure(ms * 4, 1.25);
+            w.l_n_nodes.ensure(ns * 4, 1.25);
+        }
         if (counting_) w.stats.ensure(ms * 16, 1.25);
         size_t want_cand = std::max<size_t>(1 << 16, size_t(double(n_bytes) * cand_per_byte_) + 4096);
         want_cand = std::min<size_t>(want_cand, 0xFFFFFFF0ull);
@@ -1410,6 +1572,7 @@ class EngineImpl final : public Engine {
             o.tok_off.ensure((size_t(n_sent) + 1) * 8, 1.25);
             o.tokens.ensure(size_t(n_bytes) * 24 + 24, 1.25);  // a token spans >= 1 character >= 1 byte
             ensure_marg_out(o, n_sent, n_bytes);
+            ensure_lat_out(o, ws_[0], n_sent);
             connid_begin(stream_);
             enqueue(ws_[0], d_utf8, d_off, n_sent, n_bytes, o, nullptr, nullptr, nullptr, nullptr, bd);
             CK(cudaEventSynchronize(o.done));
@@ -1459,6 +1622,11 @@ class EngineImpl final : public Engine {
         if (marg)
             cap_all = std::min<size_t>(cap_all, std::min<size_t>(w.m_cand_entry.cap / 4,
                                                                  std::min<size_t>(w.m_R.cap / 8, w.m_ab.cap / 16) - n_sent - 1));
+        const bool lat = lattice_ != 0;
+        if (lat) {  // nodes <= candidates placed: the node arrays bound the pool too
+            cap_all = std::min<size_t>(cap_all, std::min<size_t>(o.nodes.cap / 24, o.links.cap / 8));
+            if (marg) cap_all = std::min<size_t>(cap_all, o.node_prob.cap / 4);
+        }
         const uint32_t cand_cap = uint32_t(cap_all);
         Batch b{};
         b.utf8 = d_utf8;
@@ -1558,6 +1726,23 @@ class EngineImpl final : public Engine {
             launch_marginals(dv_, b, m, st);
             if (n_sent) o.launches += 2;
         }
+        o.lat = lat;
+        if (lat) {  // booked with the Viterbi stage too, and also before K4a
+            LatticeArgs l{};
+            l.row_base = w.l_row_base.as<uint32_t>();
+            l.n_nodes = w.l_n_nodes.as<uint32_t>();
+            l.node_off = o.node_off.as<unsigned long long>();
+            l.nodes = o.nodes.as<uint2>();
+            l.links = o.links.as<int2>();
+            l.node_prob = marg ? o.node_prob.as<float>() : nullptr;
+            launch_lattice_count(b, l, st);
+            cub::TransformInputIterator<unsigned long long, CastU64, const uint32_t*> it(l.n_nodes, CastU64());
+            if (n_sent == 0) CK(cudaMemsetAsync(l.n_nodes, 0, 4, st));
+            exclusive_scan(w, it, l.node_off, size_t(n_sent) + 1);
+            launch_lattice_write(b, l, m, st);
+            CK(cudaMemcpyAsync(&dc->n_nodes, l.node_off + n_sent, 8, cudaMemcpyDeviceToDevice, st));
+            if (n_sent) o.launches += 2;
+        }
         CK(cudaEventRecord(o.ev[6], st));
         launch_backtrack_count(b, st);
         CK(cudaEventRecord(o.ev[7], st));
@@ -1574,7 +1759,7 @@ class EngineImpl final : public Engine {
         k_publish_totals<<<1, 1, 0, st>>>(b.slot_off, b.tok_off, n_sent, dc);
         if (text_base) {  // output stage of a chunk: formatted while its token offsets are still chunk-local
             FormatArgs f = format_offsets(w, d_utf8, d_off, n_sent, o);
-            launch_format_write(dv_, f, st);
+            launch_format_write(dv_, f, st, fmt_links(o));
             o.launches += 2;
         }
         if (tok_base) {
@@ -1582,6 +1767,11 @@ class EngineImpl final : public Engine {
             k_add_base<<<(n_sent + 256) / 256, 256, 0, st>>>(b.tok_off, n_sent + 1, tok_base);
             k_bump_base<<<1, 1, 0, st>>>(tok_base, &dc->n_tokens);
             o.launches += 2;
+            if (lat) {  // the same for the node offsets
+                k_add_base<<<(n_sent + 256) / 256, 256, 0, st>>>(o.node_off.as<unsigned long long>(), n_sent + 1, node_base_.as<unsigned long long>());
+                k_bump_base<<<1, 1, 0, st>>>(node_base_.as<unsigned long long>(), &dc->n_nodes);
+                o.launches += 2;
+            }
             if (text_base) {
                 k_add_base<<<(n_sent + 256) / 256, 256, 0, st>>>(o.text_off.as<unsigned long long>(), n_sent + 1, text_base);
                 k_bump_base<<<1, 1, 0, st>>>(text_base, &dc->text_bytes);
@@ -1622,7 +1812,7 @@ class EngineImpl final : public Engine {
     cudaEvent_t in_done_ = nullptr;
     std::vector<cudaEvent_t> h2d_ev_;
     OutSlot out_[2];
-    DevBuf tok_base_, text_base_;
+    DevBuf tok_base_, text_base_, node_base_;
     uint32_t chunk_sentences_ = 262144;
     uint64_t pool_need_ = 0;
     double tok_per_byte_ = 0.2;
@@ -1651,6 +1841,11 @@ class EngineImpl final : public Engine {
     // buffers of the chunked host pipeline, learned like cand_per_byte_
     static constexpr double kFormatTextPerByte = 8.0;
     double text_per_byte_[5] = {0.0, 8.0, 2.0, 16.0, kFormatTextPerByte};
+    // the same for lattice text ("lattice" = 2), which renders ~17 nodes per token
+    static constexpr double kLatticeTextFactor = 17.0;
+    double text_per_byte_lat_[5] = {0.0, 8.0 * kLatticeTextFactor, 2.0 * kLatticeTextFactor, 16.0 * kLatticeTextFactor,
+                                    kFormatTextPerByte * kLatticeTextFactor};
+    double node_per_byte_ = 2.0;  // lattice nodes per input byte: sizes the host result of the chunked pipeline
     uint32_t text_per_sent_ = 4;  // "EOS\n"; an output format: what its BOS and EOS print (FormatProgram::per_sentence)
     // output format (set_format): the compiled program and its field table, with the table's size and build time
     DevBuf fmt_prog_, ft_keep_, ft_off_, ft_bytes_;
@@ -1663,6 +1858,8 @@ class EngineImpl final : public Engine {
     int viterbi_kernel_ = 1;  // 1 = k_viterbi2 with pruning (kernels.cuh)
     double theta_ = 0;        // marginals' theta, 0 = off (set_marginals)
     bool dev_marg_ = false;   // the last run_device computed marginals (device_marginals)
+    int lattice_ = 0;         // option "lattice": 0 off, 1 nodes, 2 nodes and lattice text
+    bool dev_lat_ = false;    // the last run_device produced the lattice (device_lattice)
     float stage_ms_[kNumStages];
     uint64_t launches_ = 0;
     uint32_t last_route_ = kRouteNone;  // ViterbiRoute of the last successful call (describe())

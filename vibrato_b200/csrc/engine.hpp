@@ -29,6 +29,15 @@ struct HostResult {  // pinned host memory holding one batch's tokens
     float* path_prob = nullptr;   // n_sent
     size_t cap_tprob = 0, cap_pprob = 0;
     bool has_marg = false;
+    // lattice output (option "lattice" >= 1): every node of each sentence's lattice, has_lat == false when it is off.
+    // node_off[i] .. node_off[i + 1] index sentence i's nodes (kernels.cuh LatticeArgs).
+    uint64_t n_nodes = 0;
+    uint64_t* node_off = nullptr;  // n_sent + 1
+    void* nodes = nullptr;         // vbt_token[n_nodes], always 24 bytes
+    void* links = nullptr;         // vbt_lattice_link[n_nodes]
+    float* node_prob = nullptr;    // n_nodes, with marginals only (has_marg)
+    size_t cap_node_off = 0, cap_nodes = 0, cap_links = 0, cap_nprob = 0;
+    bool has_lat = false;
 };
 
 // Required token boundaries of a batch (vbt_tokenize_batch_bounded): sentence i's boundaries are the
@@ -86,6 +95,15 @@ class Engine {
     virtual void shard_outputs(uint64_t* d_tok_off, uint64_t* d_tokens) const = 0;
     // Device addresses of the last shard's marginals: float token_prob[n_tokens], path_prob[n_sent].
     virtual void shard_marginals(uint64_t* d_token_prob, uint64_t* d_path_prob) const = 0;
+    // The last shard's lattice (option "lattice"): its node count; fetch_shard_lattice copies its node offsets
+    // (+ node_base, n_sent entries, one more when `last`), nodes, links and, with h_node_prob != nullptr, node marginals
+    // into host memory; rebase_shard_lattice adds node_base to the offsets on the device and shard_lattice gives the
+    // device addresses of the four arrays.
+    virtual uint64_t shard_nodes() const = 0;
+    virtual void fetch_shard_lattice(uint64_t* h_node_off, void* h_nodes, void* h_links, float* h_node_prob,
+                                     uint64_t node_base, bool last) = 0;
+    virtual void rebase_shard_lattice(uint64_t node_base) = 0;
+    virtual void shard_lattice(uint64_t* d_node_off, uint64_t* d_nodes, uint64_t* d_links, uint64_t* d_node_prob) const = 0;
     virtual int device() const = 0;
     virtual uint32_t token_bytes() const = 0;  // 24, or 16 with the "compact_tokens" option
     virtual std::string describe() const = 0;  // JSON: devices, how the dictionary travelled, ...
@@ -95,7 +113,8 @@ class Engine {
     // "dual_stream", "connid_counting", "output_mode" (0 none, 1 mecab, 2 wakati, 3 detail: run_host also
     // produces HostResult::text, on every host route; run_device stays token-only), "small_batch" (N > 0: run_host
     // takes k_small_batch for batches of at most N sentences and 16 KiB without counting; run_device and the shards
-    // of a multi-device engine keep the usual route).
+    // of a multi-device engine keep the usual route), "lattice" (0 off, 1 results also carry every lattice node,
+    // 2 the same and the output text renders the nodes in place of the tokens).
     virtual void set_option(const std::string& name, long long value) = 0;
     // An output format (format.hpp) in place of "output_mode" 1-3, on every host route; nullptr switches it off.
     // Setting "output_mode" replaces it.  Builds the format's field table on the device.
@@ -105,9 +124,15 @@ class Engine {
     // path_prob, and run_device leaves them in device memory (device_marginals).
     virtual void set_marginals(double theta) = 0;
     virtual double marginals() const = 0;
+    virtual int lattice() const = 0;  // the option "lattice"
     // Device addresses of the last run_device's float token_prob[n_tokens] and path_prob[n_sent]; valid until the
     // next call.  Throws when that call ran without marginals.
     virtual void device_marginals(uint64_t* d_token_prob, uint64_t* d_path_prob) const = 0;
+    // Device addresses of the last run_device's lattice (option "lattice" >= 1): uint64 node_off[n_sent + 1],
+    // vbt_token nodes[n_nodes], vbt_lattice_link links[n_nodes] and float node_prob[n_nodes] (0 without marginals);
+    // valid until the next call.  Throws when that call ran without the lattice.
+    virtual void device_lattice(uint64_t* d_node_off, uint64_t* d_nodes, uint64_t* d_links, uint64_t* d_node_prob,
+                                uint64_t* n_nodes) const = 0;
     // Launch on a caller-owned CUDA stream (0 restores the engine's own stream).
     virtual void set_stream(uint64_t stream) = 0;
     virtual const float* stage_ms() const = 0;

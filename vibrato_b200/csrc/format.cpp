@@ -14,7 +14,7 @@ namespace {
 
 class Compiler {
    public:
-    Compiler(FormatProgram& p, bool marginals) : p_(p), marginals_(marginals) {}
+    Compiler(FormatProgram& p, bool marginals, bool lattice_text) : p_(p), marginals_(marginals), lattice_text_(lattice_text) {}
 
     // Appends the ops of one format string as section `sec`; `tokens` = false admits only what BOS / EOS can print.
     void section(uint32_t sec, const char* name, const char* s, size_t n, bool tokens) {
@@ -60,6 +60,14 @@ class Compiler {
                 p_.uses |= kUsesProb;
                 continue;
             }
+            if (dir == "%pb" && lattice_text_) {
+                if (!tokens) fail(at, dir + " is not allowed here (only literals, %%, %S and %L)");
+                op(kOpBest, at);
+                p_.uses |= kUsesBest;
+                continue;
+            }
+            if (lattice_text_ && (dir == "%M" || dir == "%pS" || dir == "%pn" || dir == "%pC" || dir == "%pL"))
+                fail(at, dir + " has no value in lattice text (option \"lattice\" = 2): a node has no previous token");
             static const char* const kNoValue[] = {"%h", "%t", "%P", "%pP", "%pA", "%pB", "%pi", "%pb", "%pp"};
             for (const char* nv : kNoValue)
                 if (dir == nv) fail(at, dir + " has no value for the tokens of the best path");
@@ -195,6 +203,7 @@ class Compiler {
     FormatProgram& p_;
     const char* name_ = "";
     bool marginals_ = false;
+    bool lattice_text_ = false;
     bool open_lit_ = false;
     std::vector<uint32_t> raw_;
 };
@@ -208,10 +217,11 @@ uint32_t fixed_bytes(const FormatProgram& p, uint32_t a, uint32_t b) {
 
 }  // namespace
 
-FormatProgram compile_format(FormatText node, FormatText unk, FormatText bos, FormatText eos, bool marginals) {
+FormatProgram compile_format(FormatText node, FormatText unk, FormatText bos, FormatText eos, bool marginals,
+                             bool lattice_text) {
     FormatProgram p;
     std::memset(&p, 0, sizeof p);
-    Compiler c(p, marginals);
+    Compiler c(p, marginals, lattice_text);
     if (!node.ptr) throw Error(kInvalidArgument, "format: the node format must be given");
     c.section(kSecNode, "node", node.ptr, node.len, true);
     if (unk.ptr) {

@@ -9,6 +9,8 @@
 //   %ps %pe %pl %pL start byte, end byte, surface bytes, end byte - prev's end byte   %phl %phr left / right id
 //   %s 0 for System / User words, 1 for Unknown   %S %L the whole sentence, its byte length   %% '%'
 //   %pP the token's marginal probability as d.dddddd (only while marginals are on)
+//   %pb '*' for a node of the best path, ' ' otherwise (only in lattice text, option "lattice" = 2, where the "prev"
+//   directives %M %pS %pn %pC %pL are refused: a node has no previous token)
 // Escapes \0 \a \b \t \n \v \f \r \s(space) \\ are replaced by the compiler.  BOS / EOS take literals, %%, %S, %L.
 #pragma once
 
@@ -38,6 +40,7 @@ enum FormatOpKind : uint8_t {
     kOpSentence,     // %S
     kOpSentLen,      // %L
     kOpProb,         // %pP
+    kOpBest,         // %pb (lattice text)
 };
 
 struct FormatOp {
@@ -50,7 +53,7 @@ struct FormatOp {
 constexpr uint32_t kFmtMaxOps = 256, kFmtMaxSlots = 256, kFmtMaxLit = 2048, kFmtMaxFields = 16, kFmtMaxFieldIndex = 255;
 enum : uint32_t { kSecNode = 0, kSecUnk = 1, kSecBos = 2, kSecEos = 3 };
 // what a token's values must be loaded for (FormatProgram::uses)
-enum : uint32_t { kUsesPrev = 1u, kUsesParams = 2u, kUsesFeature = 4u, kUsesFields = 8u, kUsesProb = 16u };
+enum : uint32_t { kUsesPrev = 1u, kUsesParams = 2u, kUsesFeature = 4u, kUsesFields = 8u, kUsesProb = 16u, kUsesBest = 32u };
 
 // Laid out so that the used part is a prefix of each array: the kernels stage the header, ops[0 .. n_ops),
 // slot[0 .. n_slots) and lit[0 .. n_lit) in shared memory.
@@ -74,7 +77,9 @@ struct FormatText {  // one format string: ptr == nullptr means "not given"
 // Compiles node / unk / bos / eos (unk not given = node, bos = "", eos = "EOS\n").  Throws
 // Error(kInvalidArgument, "<which> format, byte <pos>: ...") naming the offending directive or escape.
 // `marginals`: the tokenizer computes marginal probabilities, so %pP has a value (otherwise it is refused).
-FormatProgram compile_format(FormatText node, FormatText unk, FormatText bos, FormatText eos, bool marginals = false);
+// `lattice_text`: the text renders lattice nodes ("lattice" = 2), so %pb has a value and the "prev" directives do not.
+FormatProgram compile_format(FormatText node, FormatText unk, FormatText bos, FormatText eos, bool marginals = false,
+                             bool lattice_text = false);
 #endif
 
 }  // namespace vbt

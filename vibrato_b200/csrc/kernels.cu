@@ -1474,6 +1474,92 @@ __global__ void __launch_bounds__(256) k_backtrack_write_marg(Batch b, MargArgs 
     }
 }
 
+// ---------------------------------------------------------------------------------------------
+// Lattice output (LatticeArgs in kernels.cuh): one warp per sentence over the rows K3 filled, ends_meta[slot] =
+// {row offset, fill}.  The first slot's row holds only BOS, which is not a node.
+// ---------------------------------------------------------------------------------------------
+
+// Nodes of the row of `slot` (i = slot - base); 0 for every row of an empty sentence
+__device__ __forceinline__ uint32_t lattice_row_nodes(const Batch& b, uint32_t slot, uint32_t i, bool empty) {
+    const uint2 me = b.ends_meta[slot];
+    return me.y - me.x - ((i == 0 && !empty) ? 1u : 0u);
+}
+
+__global__ void __launch_bounds__(256) k_lattice_count(Batch b, LatticeArgs l) {
+    const uint32_t s = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const uint32_t lane = threadIdx.x & 31;
+    if (s >= b.n_sent) return;
+    // a batch that is re-run or refused: its rows cannot be trusted, and nothing is read from it
+    if (*b.flags & (kFlagsStandDown | kFlagPoolOverflow)) {
+        if (lane == 0) l.n_nodes[s] = 0;
+        return;
+    }
+    const uint32_t base = b.slot_off[s], rows = b.slot_off[s + 1] - base;  // the sentinel's row included
+    const bool empty = rows == 1;
+    uint32_t run = 0;
+    for (uint32_t i0 = 0; i0 < rows; i0 += 32) {
+        const uint32_t i = i0 + lane;
+        const uint32_t c = i < rows ? lattice_row_nodes(b, base + i, i, empty) : 0u;
+        uint32_t x = c;  // inclusive warp scan
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+            const uint32_t y = __shfl_up_sync(kFull, x, d);
+            if (lane >= uint32_t(d)) x += y;
+        }
+        if (i < rows) l.row_base[base + i] = run + x - c;
+        run += __shfl_sync(kFull, x, 31);
+    }
+    if (lane == 0) l.n_nodes[s] = run;
+}
+
+__global__ void __launch_bounds__(256) k_lattice_write(Batch b, LatticeArgs l, MargArgs m) {
+    const uint32_t s = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const uint32_t lane = threadIdx.x & 31;
+    if (s >= b.n_sent || (*b.flags & (kFlagsStandDown | kFlagPoolOverflow))) return;
+    const uint32_t base = b.slot_off[s], last = b.slot_off[s + 1] - 1;
+    if (base == last) return;  // an empty sentence has no nodes
+    const unsigned long long n0 = l.node_off[s];
+    const double a_eos = l.node_prob ? m.a_eos[s] : 0.0;
+    for (uint32_t slot = base; slot <= last; ++slot) {
+        const uint2 me = b.ends_meta[slot];
+        const uint32_t skip_bos = slot == base ? 1u : 0u;
+        const uint32_t rb = l.row_base[slot];
+        for (uint32_t e = me.x + skip_bos + lane; e < me.y; e += 32) {
+            const uint4 c = b.ends_cold[e];  // {start_node slot, best prev entry, word_idx, min_cost}
+            const unsigned long long k = n0 + rb + (e - me.x - skip_bos);
+            const uint32_t end_node = slot - base;
+            const uint32_t start_node = c.x - base;
+            const uint2 i8 = b.info[c.x];
+            const uint32_t start_word = start_node + ((i8.y & kInfoSpecial) ? b.info_ex[c.x].x : 0u);  // as backtrack_write_one
+            uint2* t = l.nodes + k * 3;
+            t[0] = make_uint2(start_word, end_node);
+            t[1] = make_uint2(b.byte_pos[base + start_word], b.byte_pos[slot]);
+            t[2] = make_uint2(c.z, c.w);
+            // the predecessor's row starts at ends_meta[c.x].x; the first slot's row holds only BOS
+            const int32_t prev = c.x == base ? -1 : int32_t(l.row_base[c.x] + (c.y - b.ends_meta[c.x].x));
+            l.links[k] = make_int2(prev, 0);
+            if (l.node_prob) {
+                const double2 ab = m.ab[e];
+                l.node_prob[k] = float(exp(ab.x + ab.y - a_eos));  // the expression of k_backtrack_write_marg
+            }
+        }
+    }
+    __syncwarp();
+    if (lane == 0) {  // the chain backtrack_count_one walks
+        const uint4 eo = b.eos[s];
+        if (eo.x != kNone) {
+            uint32_t cur = eo.x, end_node = eo.y;
+            while (end_node != 0) {
+                const uint32_t slot = base + end_node;
+                const uint4 c = b.ends_cold[cur];
+                l.links[n0 + l.row_base[slot] + (cur - b.ends_meta[slot].x)].y = int32_t(kNodeBest);  // never the BOS row
+                end_node = c.x - base;
+                cur = c.y;
+            }
+        }
+    }
+}
+
 
 // ---------------------------------------------------------------------------------------------
 // Output stage: the text `tokenize` writes per sentence (tokenize/src/main.rs:83-127):
@@ -1575,11 +1661,12 @@ struct FmtTok {
     uint32_t ids;          // left | right << 16
     uint32_t keep, entry;  // field table: the fields printed, and the word's first entry
     uint32_t prob_micro;   // %pP: round(marginal * 1e6), in [0, 1e6]
+    uint32_t best;         // %pb (lattice text): the node is on the best path
 };
 
-template <bool PROB = false>
+template <bool PROB = false, bool BEST = false>
 __device__ __forceinline__ FmtTok fmt_tok(const DictView& d, const FormatArgs& f, const FormatProgram& P,
-                                          unsigned long long t, unsigned long long t0) {
+                                          unsigned long long t, unsigned long long t0, const int2* links = nullptr) {
     const uint32_t uses = P.uses;
     FmtTok v;
     v.x = token_text(d, f.tokens, t);
@@ -1613,6 +1700,7 @@ __device__ __forceinline__ FmtTok fmt_tok(const DictView& d, const FormatArgs& f
             v.prob_micro = uint32_t(fmin(fmax(pm, 0.0), 1e6));
         }
     }
+    if constexpr (BEST) v.best = (uses & kUsesBest) ? (uint32_t(links[t].y) & kNodeBest) : 0u;
     return v;
 }
 
@@ -1637,7 +1725,7 @@ __device__ __forceinline__ uint32_t num_len(long long x) { return x < 0 ? 1 + de
 
 // Bytes the ops [a, b) of the program write for one token (or for BOS / EOS, with v unused).  PROB: the program may
 // print %pP (a separate instantiation, so that the other formats keep their code).
-template <bool PROB = false>
+template <bool PROB = false, bool BEST = false>
 __device__ __forceinline__ unsigned long long fmt_len(const FormatProgram& P, uint32_t a, uint32_t b, const FormatArgs& f,
                                                       const FmtTok& v, uint32_t sent_len) {
     unsigned long long n = 0;
@@ -1664,6 +1752,12 @@ __device__ __forceinline__ unsigned long long fmt_len(const FormatProgram& P, ui
                 if constexpr (PROB) {
                     if (o.kind == kOpProb) {
                         n += 8;  // d.dddddd
+                        break;
+                    }
+                }
+                if constexpr (BEST) {
+                    if (o.kind == kOpBest) {
+                        n += 1;  // '*' or ' '
                         break;
                     }
                 }
@@ -1698,23 +1792,23 @@ __device__ __forceinline__ const FormatProgram* stage_program(const FormatArgs& 
 
 // Pass 1 for sentence s (a warp per sentence): lane 0 stores its text length in sent_len[s].  PROG: f.mode is
 // kOutFormat (a separate instantiation, so that the fixed modes keep their registers).
-template <bool PROG, bool PROB = false>
+template <bool PROG, bool PROB = false, bool BEST = false>
 __device__ __forceinline__ void format_len_one(const DictView& d, const FormatArgs& f, const FormatProgram* P, uint32_t s,
-                                               uint32_t lane) {
+                                               uint32_t lane, const int2* links = nullptr) {
     const unsigned long long t0 = f.tok_off[s], t1 = f.tok_off[s + 1];
     unsigned long long len = 0;
     if constexpr (PROG) {
         const uint32_t sl = uint32_t(f.byte_off[s + 1] - f.byte_off[s]);
         for (unsigned long long t = t0 + lane; t < t1; t += 32) {
-            const FmtTok v = fmt_tok<PROB>(d, f, *P, t, t0);
+            const FmtTok v = fmt_tok<PROB, BEST>(d, f, *P, t, t0, links);
             const uint32_t sec = v.x.lex == 2 ? kSecUnk : kSecNode;
-            len += fmt_len<PROB>(*P, P->sec[sec][0], P->sec[sec][1], f, v, sl);
+            len += fmt_len<PROB, BEST>(*P, P->sec[sec][0], P->sec[sec][1], f, v, sl);
         }
         for (int k = 16; k > 0; k >>= 1) len += __shfl_xor_sync(kFull, len, k);
         if (lane == 0) {
             FmtTok none{};
-            len += fmt_len<PROB>(*P, P->sec[kSecBos][0], P->sec[kSecBos][1], f, none, sl);
-            f.sent_len[s] = len + fmt_len<PROB>(*P, P->sec[kSecEos][0], P->sec[kSecEos][1], f, none, sl);
+            len += fmt_len<PROB, BEST>(*P, P->sec[kSecBos][0], P->sec[kSecBos][1], f, none, sl);
+            f.sent_len[s] = len + fmt_len<PROB, BEST>(*P, P->sec[kSecEos][0], P->sec[kSecEos][1], f, none, sl);
         }
     } else {
         for (unsigned long long t = t0 + lane; t < t1; t += 32) len += token_text_len(d, token_text(d, f.tokens, t), f.mode, t == t0);
@@ -1737,7 +1831,7 @@ __device__ __forceinline__ void warp_copy(uint8_t* __restrict__ dst, const uint8
 }
 
 // Writes the ops [a, b) at dst with the whole warp (every lane passes the same arguments); returns the end.
-template <bool PROB = false>
+template <bool PROB = false, bool BEST = false>
 __device__ __forceinline__ uint8_t* fmt_write(const DictView& d, const FormatProgram& P, uint32_t a, uint32_t b,
                                               const FormatArgs& f, const FmtTok& v, const uint8_t* __restrict__ sent,
                                               uint32_t sent_len, uint8_t* dst, uint32_t lane) {
@@ -1794,6 +1888,13 @@ __device__ __forceinline__ uint8_t* fmt_write(const DictView& d, const FormatPro
                             for (int k = 7; k >= 2; --k, frac /= 10) dst[k] = uint8_t('0' + frac % 10);
                         }
                         dst += 8;
+                        break;
+                    }
+                }
+                if constexpr (BEST) {
+                    if (o.kind == kOpBest) {  // MeCab's %pb: '*' on the best path, ' ' elsewhere
+                        if (lane == 0) *dst = v.best ? '*' : ' ';
+                        dst += 1;
                         break;
                     }
                 }
@@ -1899,9 +2000,9 @@ __global__ void __launch_bounds__(256) k_field_table_write(DictView d, FieldTabl
 }
 
 // Pass 2 for sentence s (a warp per sentence): its text at text_off[s], which must fit in text_cap.
-template <bool PROG, bool PROB = false>
+template <bool PROG, bool PROB = false, bool BEST = false>
 __device__ __forceinline__ void format_write_one(const DictView& d, const FormatArgs& f, const FormatProgram* P, uint32_t s,
-                                                 uint32_t lane) {
+                                                 uint32_t lane, const int2* links = nullptr) {
     const unsigned long long t0 = f.tok_off[s], t1 = f.tok_off[s + 1];
     const uint8_t* __restrict__ sent = f.utf8 + f.byte_off[s];
     unsigned long long base = f.text_off[s];  // where the next group of 32 tokens starts
@@ -1909,7 +2010,7 @@ __device__ __forceinline__ void format_write_one(const DictView& d, const Format
     const uint32_t sl = prog ? uint32_t(f.byte_off[s + 1] - f.byte_off[s]) : 0u;
     if (prog) {
         const FmtTok none{};
-        base = fmt_write<PROB>(d, *P, P->sec[kSecBos][0], P->sec[kSecBos][1], f, none, sent, sl, f.text + base, lane) - f.text;
+        base = fmt_write<PROB, BEST>(d, *P, P->sec[kSecBos][0], P->sec[kSecBos][1], f, none, sent, sl, f.text + base, lane) - f.text;
     }
     for (unsigned long long c = t0; c < t1; c += 32) {
         // lane i stages token c + i; the copies below take one token at a time with all 32 lanes
@@ -1917,9 +2018,9 @@ __device__ __forceinline__ void format_write_one(const DictView& d, const Format
         TokenText mine = {0, 0, 0, 0, 0, 0, 0};
         unsigned long long len = 0;
         if (lane < cnt && prog) {
-            const FmtTok v = fmt_tok<PROB>(d, f, *P, c + lane, t0);
+            const FmtTok v = fmt_tok<PROB, BEST>(d, f, *P, c + lane, t0, links);
             const uint32_t sec = v.x.lex == 2 ? kSecUnk : kSecNode;
-            len = fmt_len<PROB>(*P, P->sec[sec][0], P->sec[sec][1], f, v, sl);
+            len = fmt_len<PROB, BEST>(*P, P->sec[sec][0], P->sec[sec][1], f, v, sl);
         } else if (lane < cnt) {
             mine = token_text(d, f.tokens, c + lane);
             len = token_text_len(d, mine, f.mode, c + lane == t0);
@@ -1933,9 +2034,9 @@ __device__ __forceinline__ void format_write_one(const DictView& d, const Format
         base += __shfl_sync(kFull, incl, 31);
         for (uint32_t j = 0; j < cnt; ++j) {
             if (prog) {  // every lane loads token c + j again: one broadcast load per record
-                const FmtTok v = fmt_tok<PROB>(d, f, *P, c + j, t0);
+                const FmtTok v = fmt_tok<PROB, BEST>(d, f, *P, c + j, t0, links);
                 const uint32_t sec = v.x.lex == 2 ? kSecUnk : kSecNode;
-                fmt_write<PROB>(d, *P, P->sec[sec][0], P->sec[sec][1], f, v, sent, sl, f.text + __shfl_sync(kFull, at, j), lane);
+                fmt_write<PROB, BEST>(d, *P, P->sec[sec][0], P->sec[sec][1], f, v, sent, sl, f.text + __shfl_sync(kFull, at, j), lane);
                 continue;
             }
             TokenText x;
@@ -1981,7 +2082,7 @@ __device__ __forceinline__ void format_write_one(const DictView& d, const Format
     }
     if (prog) {
         const FmtTok none{};
-        fmt_write<PROB>(d, *P, P->sec[kSecEos][0], P->sec[kSecEos][1], f, none, sent, sl, f.text + base, lane);
+        fmt_write<PROB, BEST>(d, *P, P->sec[kSecEos][0], P->sec[kSecEos][1], f, none, sent, sl, f.text + base, lane);
     } else if (lane == 0) {
         uint8_t* dst = f.text + base;
         if (f.mode != kOutWakati) dst = put_str(dst, "EOS");
@@ -2002,6 +2103,32 @@ __global__ void __launch_bounds__(256) k_format_write(DictView d, FormatArgs f) 
     }
     if (total > f.text_cap) return;  // every warp sees the same total: nothing is written
     format_write_one<PROG, PROB>(d, f, P, s, lane);
+}
+
+// Lattice text with %pb: the nodes' links give the best-path flag (separate kernels, so that the instantiations
+// above keep their code).
+template <bool PROB>
+__global__ void __launch_bounds__(256) k_format_len_best(DictView d, FormatArgs f, const int2* links) {
+    extern __shared__ uint4 s_dyn[];
+    const FormatProgram* P = stage_program(f, reinterpret_cast<FormatProgram*>(s_dyn));
+    const uint32_t s = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (s >= f.n_sent || format_stands_down(f)) return;
+    format_len_one<true, PROB, true>(d, f, P, s, lane, links);
+}
+
+template <bool PROB>
+__global__ void __launch_bounds__(256) k_format_write_best(DictView d, FormatArgs f, const int2* links) {
+    extern __shared__ uint4 s_dyn[];
+    const FormatProgram* P = stage_program(f, reinterpret_cast<FormatProgram*>(s_dyn));
+    const uint32_t s = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (s >= f.n_sent || format_stands_down(f)) return;
+    const unsigned long long total = f.text_off[f.n_sent];
+    if (s == 0 && lane == 0) {
+        *f.text_total = total;
+        if (total > f.text_cap) atomicOr(f.flags, kFlagTextOverflow);
+    }
+    if (total > f.text_cap) return;
+    format_write_one<true, PROB, true>(d, f, P, s, lane, links);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -2176,18 +2303,24 @@ void launch_small_batch(const DictView& d, const Batch& b, const FormatArgs& f, 
         launch_small_batch_b<false>(d, b, f, out, st);
 }
 
-void launch_format_len(const DictView& d, const FormatArgs& f, cudaStream_t st) {
+void launch_format_len(const DictView& d, const FormatArgs& f, cudaStream_t st, const int2* links) {
     if (!f.n_sent) return;
-    if (f.mode == kOutFormat)
+    if (links && f.mode == kOutFormat)
+        f.token_prob ? k_format_len_best<true><<<(f.n_sent + 7) / 8, 256, sizeof(FormatProgram), st>>>(d, f, links)
+                     : k_format_len_best<false><<<(f.n_sent + 7) / 8, 256, sizeof(FormatProgram), st>>>(d, f, links);
+    else if (f.mode == kOutFormat)
         f.token_prob ? k_format_len<true, true><<<(f.n_sent + 7) / 8, 256, sizeof(FormatProgram), st>>>(d, f)
                      : k_format_len<true><<<(f.n_sent + 7) / 8, 256, sizeof(FormatProgram), st>>>(d, f);
     else
         k_format_len<false><<<(f.n_sent + 7) / 8, 256, 0, st>>>(d, f);
 }
 
-void launch_format_write(const DictView& d, const FormatArgs& f, cudaStream_t st) {
+void launch_format_write(const DictView& d, const FormatArgs& f, cudaStream_t st, const int2* links) {
     if (!f.n_sent) return;
-    if (f.mode == kOutFormat)
+    if (links && f.mode == kOutFormat)
+        f.token_prob ? k_format_write_best<true><<<(f.n_sent + 7) / 8, 256, sizeof(FormatProgram), st>>>(d, f, links)
+                     : k_format_write_best<false><<<(f.n_sent + 7) / 8, 256, sizeof(FormatProgram), st>>>(d, f, links);
+    else if (f.mode == kOutFormat)
         f.token_prob ? k_format_write<true, true><<<(f.n_sent + 7) / 8, 256, sizeof(FormatProgram), st>>>(d, f)
                      : k_format_write<true><<<(f.n_sent + 7) / 8, 256, sizeof(FormatProgram), st>>>(d, f);
     else
@@ -2328,6 +2461,16 @@ void launch_marginals(const DictView& d, const Batch& b, const MargArgs& m, cuda
 void launch_backtrack_write_marg(const Batch& b, const MargArgs& m, cudaStream_t st) {
     if (!b.n_sent) return;
     k_backtrack_write_marg<<<(b.n_sent + 8 * VBT_SENT_PER_WARP - 1) / (8 * VBT_SENT_PER_WARP), 256, 0, st>>>(b, m);
+}
+
+void launch_lattice_count(const Batch& b, const LatticeArgs& l, cudaStream_t st) {
+    if (!b.n_sent) return;
+    k_lattice_count<<<(b.n_sent + 7) / 8, 256, 0, st>>>(b, l);  // a warp per sentence
+}
+
+void launch_lattice_write(const Batch& b, const LatticeArgs& l, const MargArgs& m, cudaStream_t st) {
+    if (!b.n_sent) return;
+    k_lattice_write<<<(b.n_sent + 7) / 8, 256, 0, st>>>(b, l, m);
 }
 
 }  // namespace vbt

@@ -160,8 +160,9 @@ struct FormatArgs {
     // selects the kernels' %pP instantiation; k_small_batch, which never runs with marginals, ignores it)
     const float* token_prob;
 };
-void launch_format_len(const DictView& d, const FormatArgs& f, cudaStream_t st);
-void launch_format_write(const DictView& d, const FormatArgs& f, cudaStream_t st);
+// links != nullptr (lattice text whose program prints %pb; f.tokens are then the nodes): the %pb instantiation.
+void launch_format_len(const DictView& d, const FormatArgs& f, cudaStream_t st, const int2* links = nullptr);
+void launch_format_write(const DictView& d, const FormatArgs& f, cudaStream_t st, const int2* links = nullptr);
 
 // Field table of a format program, built once per format and device from the feature strings of the image.
 struct FieldTableArgs {
@@ -233,6 +234,26 @@ struct MargArgs {
 void launch_marginals(const DictView& d, const Batch& b, const MargArgs& m, cudaStream_t st);
 // launch_backtrack_write plus MargArgs::token_prob of every token (one launch, in its place).
 void launch_backtrack_write_marg(const Batch& b, const MargArgs& m, cudaStream_t st);
+
+// Lattice output: every node K3 inserted (the entries of ends[1..=len] without BOS and EOS), after K3 and the
+// marginal kernels and before K4a (which overwrites ends_meta).  A sentence's nodes are listed by end position, and
+// within a row in insertion order.  Each node gets a vbt_token record (start_char = its start_word, total_cost = its
+// min_cost) and a link {prev, flags}: prev = the sentence-relative node index of the predecessor ends_cold names
+// (the u16-truncated min_idx, as the backtrack follows it), -1 for BOS; flags bit 0 (kNodeBest) = on the best path.
+enum : uint32_t { kNodeBest = 1u };
+struct LatticeArgs {
+    uint32_t* row_base;           // per slot: sentence-relative node index of the row's first node (BOS left out)
+    uint32_t* n_nodes;            // per sentence (scan input)
+    unsigned long long* node_off; // n_sent + 1: exclusive scan of n_nodes
+    uint2* nodes;                 // vbt_token as 3 x uint2, always 24 bytes
+    int2* links;                  // {prev, flags}
+    float* node_prob;             // per node, or nullptr without marginals (then MargArgs is not read)
+};
+// k_lattice_count: row_base and n_nodes (a warp per sentence).
+void launch_lattice_count(const Batch& b, const LatticeArgs& l, cudaStream_t st);
+// k_lattice_write: the records, links and, with l.node_prob, prob = exp(â + b̂ - â(EOS)) as k_backtrack_write_marg
+// computes it (a warp per sentence), after node_off has been scanned.
+void launch_lattice_write(const Batch& b, const LatticeArgs& l, const MargArgs& m, cudaStream_t st);
 
 // What k_small_batch reports besides its outputs: the batch flags and the totals of its scans.
 struct SmallBatchOut {

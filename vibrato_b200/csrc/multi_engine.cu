@@ -222,6 +222,7 @@ class MultiEngine final : public Engine {
             pinned_free(r->text);
             pinned_free(r->token_prob);
             pinned_free(r->path_prob);
+            for (void* p : {static_cast<void*>(r->node_off), r->nodes, r->links, static_cast<void*>(r->node_prob)}) pinned_free(p);
             delete r;
         }
         pinned_free(h_off_);
@@ -232,6 +233,8 @@ class MultiEngine final : public Engine {
         if (gather_off_) cudaFree(gather_off_);
         if (gather_tprob_) cudaFree(gather_tprob_);
         if (gather_pprob_) cudaFree(gather_pprob_);
+        for (void* p : {gather_noff_, gather_nodes_, gather_links_, gather_nprob_})
+            if (p) cudaFree(p);
     }
 
     // ---- host batches --------------------------------------------------------------------------------
@@ -254,7 +257,10 @@ class MultiEngine final : public Engine {
             base[i + 1] = base[i] + n_tok[i];
             text_base[i + 1] = text_base[i] + n_text[i];
         }
-        HostResult* r = acquire(n_sent, base[n], text_ ? &text_base[n] : nullptr);
+        std::vector<uint64_t> node_base(n + 1, 0);  // lattice nodes: merged at their final positions like the tokens
+        if (lattice_)
+            for (int i = 0; i < n; ++i) node_base[i + 1] = node_base[i] + eng_[i]->shard_nodes();
+        HostResult* r = acquire(n_sent, base[n], text_ ? &text_base[n] : nullptr, node_base[n]);
         const uint64_t tb = eng_[0]->token_bytes();
         r->token_bytes = uint32_t(tb);
         int last = n - 1;  // the shard that also delivers the closing offset: the last one, even when it is empty
@@ -262,6 +268,10 @@ class MultiEngine final : public Engine {
             eng_[i]->fetch_shard(r->tok_off + cut[i], static_cast<uint8_t*>(r->tokens) + base[i] * tb, base[i], i == last,
                                  text_ ? r->text_off + cut[i] : nullptr, r->text + text_base[i], text_base[i],
                                  r->has_marg ? r->token_prob + base[i] : nullptr, r->has_marg ? r->path_prob + cut[i] : nullptr);
+            if (r->has_lat)
+                eng_[i]->fetch_shard_lattice(r->node_off + cut[i], static_cast<uint8_t*>(r->nodes) + node_base[i] * 24,
+                                             static_cast<uint8_t*>(r->links) + node_base[i] * 8,
+                                             r->has_marg ? r->node_prob + node_base[i] : nullptr, node_base[i], i == last);
         });
         collect_stats();
         return r;
@@ -283,7 +293,7 @@ class MultiEngine final : public Engine {
             collect_stats();
             return;
         }
-        dev_marg_ = false;
+        dev_marg_ = dev_lat_ = false;
         CK(cudaSetDevice(dev_[0]));
         // the split needs the offsets on the host (pinned staging buffer, one copy); their validity is checked on
         // the devices like for any device-resident batch (k_count_chars)
@@ -315,6 +325,13 @@ class MultiEngine final : public Engine {
         std::vector<uint64_t> base(n + 1, 0);
         for (int i = 0; i < n; ++i) base[i + 1] = base[i] + n_tok[i];
         run_on_all([&](int i) { eng_[i]->rebase_shard(base[i]); });
+        const bool lat = lattice_ != 0;
+        std::vector<uint64_t> nbase(n + 1, 0), src_noff(n), src_nodes(n), src_links(n), src_nprob(n);
+        if (lat) {  // the lattice travels like the tokens: nodes at their final positions, offsets rebased
+            for (int i = 0; i < n; ++i) nbase[i + 1] = nbase[i] + eng_[i]->shard_nodes();
+            run_on_all([&](int i) { eng_[i]->rebase_shard_lattice(nbase[i]); });
+            for (int i = 0; i < n; ++i) eng_[i]->shard_lattice(&src_noff[i], &src_nodes[i], &src_links[i], &src_nprob[i]);
+        }
         // gather on the first device: token records and offsets of every shard at their final positions
         CK(cudaSetDevice(dev_[0]));
         if (base[n] * 24 + 24 > gather_tok_cap_) {
@@ -332,6 +349,29 @@ class MultiEngine final : public Engine {
             grow_device(gather_tprob_, gather_tprob_cap_, base[n] * 4 + 4);
             grow_device(gather_pprob_, gather_pprob_cap_, n_sent * 4 + 4);
         }
+        if (lat) {
+            grow_device(gather_noff_, gather_noff_cap_, (n_sent + 1) * 8);
+            grow_device(gather_nodes_, gather_nodes_cap_, nbase[n] * 24 + 24);
+            grow_device(gather_links_, gather_links_cap_, nbase[n] * 8 + 8);
+            if (marg) grow_device(gather_nprob_, gather_nprob_cap_, nbase[n] * 4 + 4);
+        }
+        // the lattice pieces of shard i: {destination on the first device, source on device i, bytes}
+        struct Piece {
+            void* dst;
+            uint64_t src, bytes;
+        };
+        auto lat_pieces = [&](int i) {
+            std::vector<Piece> v;
+            if (!lat) return v;
+            const uint64_t nn = nbase[i + 1] - nbase[i];
+            v.push_back({static_cast<uint8_t*>(gather_noff_) + cut[i] * 8, src_noff[i], (cut[i + 1] - cut[i] + (i == n - 1 ? 1 : 0)) * 8});
+            if (nn) {
+                v.push_back({static_cast<uint8_t*>(gather_nodes_) + nbase[i] * 24, src_nodes[i], nn * 24});
+                v.push_back({static_cast<uint8_t*>(gather_links_) + nbase[i] * 8, src_links[i], nn * 8});
+                if (marg) v.push_back({static_cast<uint8_t*>(gather_nprob_) + nbase[i] * 4, src_nprob[i], nn * 4});
+            }
+            return v;
+        };
         std::vector<uint64_t> src_off(n), src_tok(n), src_tp(n), src_pp(n);
         for (int i = 0; i < n; ++i) {
             eng_[i]->shard_outputs(&src_off[i], &src_tok[i]);
@@ -351,6 +391,8 @@ class MultiEngine final : public Engine {
             if (n_tok[0]) CK(cudaMemcpyAsync(dst_tp(0), reinterpret_cast<const void*>(src_tp[0]), n_tok[0] * 4, cudaMemcpyDeviceToDevice, stream_[0]));
             if (n_sh(0)) CK(cudaMemcpyAsync(dst_pp(0), reinterpret_cast<const void*>(src_pp[0]), n_sh(0) * 4, cudaMemcpyDeviceToDevice, stream_[0]));
         }
+        for (const Piece& p : lat_pieces(0))
+            CK(cudaMemcpyAsync(p.dst, reinterpret_cast<const void*>(p.src), p.bytes, cudaMemcpyDeviceToDevice, stream_[0]));
         if (n > 1 && nccl_) {
             NK(nccl_->GroupStart());
             for (int i = 1; i < n; ++i) {
@@ -359,11 +401,14 @@ class MultiEngine final : public Engine {
                 NK(nccl_->Send(reinterpret_cast<const void*>(src_off[i]), off_bytes(i), ncclUint8, 0, comm_[i], stream_[i]));
                 if (marg && n_tok[i]) NK(nccl_->Send(reinterpret_cast<const void*>(src_tp[i]), n_tok[i] * 4, ncclUint8, 0, comm_[i], stream_[i]));
                 if (marg && n_sh(i)) NK(nccl_->Send(reinterpret_cast<const void*>(src_pp[i]), n_sh(i) * 4, ncclUint8, 0, comm_[i], stream_[i]));
+                const std::vector<Piece> lp = lat_pieces(i);
+                for (const Piece& p : lp) NK(nccl_->Send(reinterpret_cast<const void*>(p.src), p.bytes, ncclUint8, 0, comm_[i], stream_[i]));
                 CK(cudaSetDevice(dev_[0]));
                 if (n_tok[i]) NK(nccl_->Recv(dst_tok(i), n_tok[i] * tb, ncclUint8, i, comm_[0], stream_[0]));
                 NK(nccl_->Recv(dst_off(i), off_bytes(i), ncclUint8, i, comm_[0], stream_[0]));
                 if (marg && n_tok[i]) NK(nccl_->Recv(dst_tp(i), n_tok[i] * 4, ncclUint8, i, comm_[0], stream_[0]));
                 if (marg && n_sh(i)) NK(nccl_->Recv(dst_pp(i), n_sh(i) * 4, ncclUint8, i, comm_[0], stream_[0]));
+                for (const Piece& p : lp) NK(nccl_->Recv(p.dst, p.bytes, ncclUint8, i, comm_[0], stream_[0]));
             }
             NK(nccl_->GroupEnd());
         } else {
@@ -374,6 +419,8 @@ class MultiEngine final : public Engine {
                     CK(cudaMemcpyPeerAsync(dst_tp(i), dev_[0], reinterpret_cast<const void*>(src_tp[i]), dev_[i], n_tok[i] * 4, stream_[0]));
                 if (marg && n_sh(i))
                     CK(cudaMemcpyPeerAsync(dst_pp(i), dev_[0], reinterpret_cast<const void*>(src_pp[i]), dev_[i], n_sh(i) * 4, stream_[0]));
+                for (const Piece& p : lat_pieces(i))
+                    CK(cudaMemcpyPeerAsync(p.dst, dev_[0], reinterpret_cast<const void*>(p.src), dev_[i], p.bytes, stream_[0]));
             }
         }
         for (int i = 0; i < n; ++i) {
@@ -385,6 +432,8 @@ class MultiEngine final : public Engine {
         *d_tokens = reinterpret_cast<uint64_t>(gather_tokens_);
         *n_tokens = base[n];
         dev_marg_ = marg;
+        dev_lat_ = lat;
+        dev_nodes_ = nbase[n];
     }
 
     // ---- everything else is forwarded ------------------------------------------------------------------
@@ -394,6 +443,7 @@ class MultiEngine final : public Engine {
     void set_option(const std::string& name, long long value) override {
         if (name == "chunk_sentences") return;  // shards are not chunked (see the constructor)
         for (auto& e : eng_) e->set_option(name, value);
+        if (name == "lattice") lattice_ = int(value);
         if (name == "output_mode") text_ = fixed_mode_ = value != 0;
     }
     void set_format(const FormatProgram* p) override {
@@ -411,11 +461,22 @@ class MultiEngine final : public Engine {
         for (auto& e : eng_) e->set_marginals(theta);
     }
     double marginals() const override { return eng_[0]->marginals(); }
+    int lattice() const override { return lattice_; }
     void device_marginals(uint64_t* d_token_prob, uint64_t* d_path_prob) const override {
         if (dev_.size() == 1) return eng_[0]->device_marginals(d_token_prob, d_path_prob);
         if (!dev_marg_) throw Error(kInvalidArgument, "the last device-resident call ran without marginals");
         if (d_token_prob) *d_token_prob = reinterpret_cast<uint64_t>(gather_tprob_);
         if (d_path_prob) *d_path_prob = reinterpret_cast<uint64_t>(gather_pprob_);
+    }
+    void device_lattice(uint64_t* d_node_off, uint64_t* d_nodes, uint64_t* d_links, uint64_t* d_node_prob,
+                        uint64_t* n_nodes) const override {
+        if (dev_.size() == 1) return eng_[0]->device_lattice(d_node_off, d_nodes, d_links, d_node_prob, n_nodes);
+        if (!dev_lat_) throw Error(kInvalidArgument, "the last device-resident call ran without the lattice");
+        if (d_node_off) *d_node_off = reinterpret_cast<uint64_t>(gather_noff_);
+        if (d_nodes) *d_nodes = reinterpret_cast<uint64_t>(gather_nodes_);
+        if (d_links) *d_links = reinterpret_cast<uint64_t>(gather_links_);
+        if (d_node_prob) *d_node_prob = dev_marg_ ? reinterpret_cast<uint64_t>(gather_nprob_) : 0;
+        if (n_nodes) *n_nodes = dev_nodes_;
     }
     void set_stream(uint64_t stream) override {
         if (stream) throw Error(kUnsupported, "a multi-device tokenizer runs on its own streams");
@@ -445,6 +506,10 @@ class MultiEngine final : public Engine {
         throw Error(kInternal, "not a shard engine");
     }
     void shard_marginals(uint64_t*, uint64_t*) const override { throw Error(kInternal, "not a shard engine"); }
+    uint64_t shard_nodes() const override { throw Error(kInternal, "not a shard engine"); }
+    void fetch_shard_lattice(uint64_t*, void*, void*, float*, uint64_t, bool) override { throw Error(kInternal, "not a shard engine"); }
+    void rebase_shard_lattice(uint64_t) override { throw Error(kInternal, "not a shard engine"); }
+    void shard_lattice(uint64_t*, uint64_t*, uint64_t*, uint64_t*) const override { throw Error(kInternal, "not a shard engine"); }
     void rebase_shard(uint64_t) override { throw Error(kInternal, "not a shard engine"); }
     void shard_outputs(uint64_t*, uint64_t*) const override { throw Error(kInternal, "not a shard engine"); }
     int device() const override { return dev_[0]; }
@@ -535,7 +600,7 @@ class MultiEngine final : public Engine {
     }
 
     // A pooled pinned result for n_sent sentences and n_tokens tokens, and *text_bytes bytes of text when given.
-    HostResult* acquire(uint64_t n_sent, uint64_t n_tokens, const uint64_t* text_bytes) {
+    HostResult* acquire(uint64_t n_sent, uint64_t n_tokens, const uint64_t* text_bytes, uint64_t n_nodes = 0) {
         HostResult* r = nullptr;
         if (!free_.empty()) {
             r = free_.back();
@@ -579,6 +644,19 @@ class MultiEngine final : public Engine {
             r->token_prob = static_cast<float*>(tp);
             r->path_prob = static_cast<float*>(pp);
         }
+        r->has_lat = lattice_ != 0;
+        r->n_nodes = n_nodes;
+        if (r->has_lat) {
+            void* no = r->node_off;
+            void* np = r->node_prob;
+            grow_pinned(no, r->cap_node_off, (n_sent + 1) * 8);
+            grow_pinned(r->nodes, r->cap_nodes, n_nodes * 24);
+            grow_pinned(r->links, r->cap_links, n_nodes * 8);
+            if (r->has_marg) grow_pinned(np, r->cap_nprob, n_nodes * 4);
+            r->node_off = static_cast<uint64_t*>(no);
+            r->node_prob = static_cast<float*>(np);
+            if (n_sent == 0) r->node_off[0] = 0;
+        }
         if (n_sent == 0) r->tok_off[0] = 0;
         if (n_sent == 0 && text_bytes) r->text_off[0] = 0;
         return r;
@@ -607,6 +685,14 @@ class MultiEngine final : public Engine {
     void* gather_pprob_ = nullptr;
     size_t gather_tprob_cap_ = 0, gather_pprob_cap_ = 0;
     bool dev_marg_ = false;
+    void* gather_noff_ = nullptr;  // lattice of a gathered device-resident batch
+    void* gather_nodes_ = nullptr;
+    void* gather_links_ = nullptr;
+    void* gather_nprob_ = nullptr;
+    size_t gather_noff_cap_ = 0, gather_nodes_cap_ = 0, gather_links_cap_ = 0, gather_nprob_cap_ = 0;
+    int lattice_ = 0;  // option "lattice"
+    bool dev_lat_ = false;
+    uint64_t dev_nodes_ = 0;
     float stage_ms_[kNumStages];
     uint64_t counters_[10];
     uint64_t launches_ = 0;
