@@ -26,12 +26,13 @@ LexSizes measure(const Lexicon& lx) {
     for (size_t i = 0; i < lx.postings.size();) {
         uint64_t len = lx.postings[i];
         if (i + 1 + len > lx.postings.size()) throw Error(kDecode, "postings overrun");
-        if (dev > 0x7FFFFFFFull) throw Error(kTryFromInt, "postings too large for the device layout");
+        // k_candidates names a postings list by a 30-bit index (its segments keep two bits for the kind)
+        if (dev > 0x3FFFFFFFull) throw Error(kTryFromInt, "postings too large for the device layout");
         s.post_map[i] = uint32_t(dev);
         dev += 1 + len;  // in 16-byte units: one header, one record per word
         i += 1 + len;
     }
-    if (dev > 0x7FFFFFFFull) throw Error(kTryFromInt, "postings too large for the device layout");
+    if (dev > 0x3FFFFFFFull) throw Error(kTryFromInt, "postings too large for the device layout");
     s.post_len = uint32_t(dev);
     s.post_bytes = dev * 16;
     return s;
@@ -138,6 +139,7 @@ void pack_device_blob(const Dictionary& d, std::vector<uint8_t>& out) {
     for (size_t i = 0; i + 1 < d.unk.offsets.size(); ++i)
         if (d.unk.offsets[i] > d.unk.offsets[i + 1] || d.unk.offsets[i + 1] > d.unk.entries.size())
             throw Error(kDecode, "unk offsets out of range");
+    if (d.unk.entries.size() > 0x3FFFFFFFull) throw Error(kTryFromInt, "unk.def too large for the device layout");
 
     LexSizes ss = measure(d.system), us{};
     if (d.user) us = measure(*d.user);

@@ -53,7 +53,8 @@ struct DevBuf {
 };
 
 struct Control {  // one small block zeroed per batch and read back once
-    unsigned long long pool_ctr;
+    unsigned long long pool_ctr;  // candidates
+    unsigned long long seg_ctr;   // segments of the candidate pool
     unsigned long long n_tokens;
     unsigned long long counters[kNumCounters];
     unsigned long long text_bytes;  // output stage: the text total of the batch (or chunk)
@@ -61,6 +62,10 @@ struct Control {  // one small block zeroed per batch and read back once
     uint32_t flags;
     uint32_t total_slots;
 };
+
+// Entries the workspace must hold per batch: the segment pool and the lattice rows are sized from one learned count,
+// and a batch needs it to cover both its candidates and its segments (almost always fewer).
+static uint64_t pool_need(const Control& c) { return std::max<uint64_t>(c.pool_ctr, c.seg_ctr); }
 
 // Output iterator for the row-offset scan: writes {offset, offset} (an empty row) into the 8-byte row metadata so that
 // no separate initialisation pass is needed.
@@ -146,14 +151,14 @@ __global__ void k_add_value(unsigned long long* tok_off, uint32_t n_plus_1, unsi
 
 struct Workspace {  // every per-(chunk of a)-batch device array; two of them let consecutive chunks overlap
     DevBuf n_slots, slot_off, eos, n_tok, code_sys, code_usr, cinfo, groupable, byte_pos, info, info_ex, ends_cnt,
-        ends_meta, cand, ends_hot, ends_cold, scan_tmp, stats, iota, sort_keys, order;
+        ends_meta, seg, ends_hot, ends_cold, scan_tmp, stats, iota, sort_keys, order;
     DevBuf bnd_dist;  // bounded batches only: Batch::bnd_dist
     DevBuf m_fill, m_ncand, m_cand_entry, m_R, m_ab, m_r_eos, m_a_eos;  // marginals only: MargArgs
     DevBuf l_row_base, l_n_nodes;  // lattice output only: LatticeArgs
     cudaStream_t stream = nullptr;
     void release() {
         for (DevBuf* b : {&n_slots, &slot_off, &eos, &n_tok, &code_sys, &code_usr, &cinfo, &groupable, &byte_pos, &info,
-                          &info_ex, &ends_cnt, &ends_meta, &cand, &ends_hot, &ends_cold, &scan_tmp, &stats, &iota,
+                          &info_ex, &ends_cnt, &ends_meta, &seg, &ends_hot, &ends_cold, &scan_tmp, &stats, &iota,
                           &sort_keys, &order, &bnd_dist, &m_fill, &m_ncand, &m_cand_entry, &m_R, &m_ab, &m_r_eos, &m_a_eos,
                           &l_row_base, &l_n_nodes})
             b->release();
@@ -699,7 +704,7 @@ class EngineImpl final : public Engine {
                 route = std::max<uint32_t>(route, resolve_viterbi_route(o.route, o.h_ctrl->flags));
                 if (counting_)
                     for (int i = 0; i < kNumCounters; ++i) counters_[i] += o.h_ctrl->counters[i];
-                pool_need_ = std::max<uint64_t>(pool_need_, o.h_ctrl->pool_ctr);
+                pool_need_ = std::max<uint64_t>(pool_need_, pool_need(*o.h_ctrl));
                 const uint64_t nt = o.h_ctrl->n_tokens, nx = fmt ? o.h_ctrl->text_bytes : 0;
                 const uint64_t nn = lattice_ ? o.h_ctrl->n_nodes : 0;
                 if (fmt && !(o.h_ctrl->flags & (kFlagsStandDown | kFlagUtf8Error | kFlagPoolOverflow)))
@@ -1133,11 +1138,11 @@ class EngineImpl final : public Engine {
     }
 
     // Device lattice outputs of slot `o` for (chunks of) up to n_sent sentences: a node is a candidate placed in the
-    // pool, so the node arrays hold as many entries as the candidate pool of `w` (enqueue clips cand_cap to them and
+    // pool, so the node arrays hold as many entries as the lattice rows of `w` (enqueue clips cand_cap to them and
     // a larger batch takes the pool-overflow retry).
     void ensure_lat_out(OutSlot& o, const Workspace& w, uint32_t n_sent) {
         if (!lattice_) return;
-        const size_t n = w.cand.cap / 16 + 1;
+        const size_t n = w.ends_cold.cap / 16 + 1;
         o.node_off.ensure((size_t(n_sent) + 1) * 8, 1.25);
         o.nodes.ensure(n * 24);
         o.links.ensure(n * 8);
@@ -1287,7 +1292,7 @@ class EngineImpl final : public Engine {
         w.ends_cnt.ensure(ms * 4);
         w.ends_meta.ensure(ms * 8);
         w.bnd_dist.ensure(ms * 4);
-        w.cand.ensure(size_t(kSmallCands) * 16);
+        w.seg.ensure(size_t(kSmallCands) * 8);  // a position has at least as many candidates as segments
         w.ends_hot.ensure((kSmallCands + ns) * 8);
         w.ends_cold.ensure((kSmallCands + ns) * 16);
         const size_t in_cap = ns * 8 + kEagerBytes + 8 + ns * 8 + kSmallBounds * 4;  // [off | utf8 | bnd_off | bnd]
@@ -1353,7 +1358,8 @@ class EngineImpl final : public Engine {
         b.info_ex = w.info_ex.as<uint2>();
         b.ends_cnt = w.ends_cnt.as<uint32_t>();
         b.ends_meta = w.ends_meta.as<uint2>();
-        b.cand = w.cand.as<uint4>();
+        b.seg = w.seg.as<uint2>();
+        b.seg_cap = kSmallCands;
         b.cand_cap = kSmallCands;
         b.ends_hot = w.ends_hot.as<int2>();
         b.ends_cold = w.ends_cold.as<uint4>();
@@ -1542,11 +1548,11 @@ class EngineImpl final : public Engine {
         if (counting_) w.stats.ensure(ms * 16, 1.25);
         size_t want_cand = std::max<size_t>(1 << 16, size_t(double(n_bytes) * cand_per_byte_) + 4096);
         want_cand = std::min<size_t>(want_cand, 0xFFFFFFF0ull);
-        w.cand.ensure(want_cand * 16);
+        w.seg.ensure(want_cand * 8);  // sized like the candidates: a source has one or more of them
         w.ends_hot.ensure((want_cand + ns) * 8);
         w.ends_cold.ensure((want_cand + ns) * 16);
         if (theta_ > 0) {
-            w.m_cand_entry.ensure(want_cand * 4);
+            w.m_cand_entry.ensure((want_cand + ns) * 4);
             w.m_R.ensure((want_cand + ns) * 8);
             w.m_ab.ensure((want_cand + ns) * 16);
         }
@@ -1589,12 +1595,12 @@ class EngineImpl final : public Engine {
             }
             if (o.h_ctrl->flags & kFlagPoolOverflow) {
                 if (attempt >= 3) throw Error(kInternal, "candidate pool overflow persists");
-                if (double(o.h_ctrl->pool_ctr) * 1.05 + 4096 >= double(0xFFFFFFF0ull))
+                if (double(pool_need(*o.h_ctrl)) * 1.05 + 4096 >= double(0xFFFFFFF0ull))
                     throw Error(kInvalidArgument, "batch produces more than 2^32 lattice nodes: split it");
-                cand_per_byte_ = double(o.h_ctrl->pool_ctr) / double(std::max<uint64_t>(1, n_bytes)) * 1.05 + 1e-3;
+                cand_per_byte_ = double(pool_need(*o.h_ctrl)) / double(std::max<uint64_t>(1, n_bytes)) * 1.05 + 1e-3;
                 continue;
             }
-            if (n_bytes) cand_per_byte_ = std::max(0.25, double(o.h_ctrl->pool_ctr) / double(n_bytes) * 1.15);
+            if (n_bytes) cand_per_byte_ = std::max(0.25, double(pool_need(*o.h_ctrl)) / double(n_bytes) * 1.15);
             if (n_bytes) chars_per_byte_ = std::min(1.0, double(o.h_ctrl->total_slots - n_sent) / double(n_bytes) * 1.10);
             connid_commit(stream_);
             break;
@@ -1617,11 +1623,11 @@ class EngineImpl final : public Engine {
         // earlier batches (plus slack), and a batch that exceeds it flags itself and is re-run with the hard bound
         const uint32_t hard_slots = uint32_t(n_bytes + n_sent);
         const uint32_t max_slots = uint32_t(std::min<uint64_t>(hard_slots, uint64_t(double(n_bytes) * chars_per_byte_) + n_sent + 4096));
-        size_t cap_all = std::min<size_t>(w.cand.cap / 16, std::min<size_t>(w.ends_hot.cap / 8 - n_sent - 1, w.ends_cold.cap / 16 - n_sent - 1));
+        size_t cap_all = std::min<size_t>(0xFFFFFFF0ull, std::min<size_t>(w.ends_hot.cap / 8 - n_sent - 1, w.ends_cold.cap / 16 - n_sent - 1));
         const bool marg = theta_ > 0;
         if (marg)
             cap_all = std::min<size_t>(cap_all, std::min<size_t>(w.m_cand_entry.cap / 4,
-                                                                 std::min<size_t>(w.m_R.cap / 8, w.m_ab.cap / 16) - n_sent - 1));
+                                                                 std::min<size_t>(w.m_R.cap / 8, w.m_ab.cap / 16)) - n_sent - 1);
         const bool lat = lattice_ != 0;
         if (lat) {  // nodes <= candidates placed: the node arrays bound the pool too
             cap_all = std::min<size_t>(cap_all, std::min<size_t>(o.nodes.cap / 24, o.links.cap / 8));
@@ -1649,7 +1655,8 @@ class EngineImpl final : public Engine {
         b.info_ex = w.info_ex.as<uint2>();
         b.ends_cnt = w.ends_cnt.as<uint32_t>();
         b.ends_meta = w.ends_meta.as<uint2>();
-        b.cand = w.cand.as<uint4>();
+        b.seg = w.seg.as<uint2>();
+        b.seg_cap = uint32_t(std::min<size_t>(w.seg.cap / 8, 0xFFFFFFF0ull));
         b.cand_cap = cand_cap;
         b.ends_hot = w.ends_hot.as<int2>();
         b.ends_cold = w.ends_cold.as<uint4>();
@@ -1657,6 +1664,7 @@ class EngineImpl final : public Engine {
         b.compact = tok_bytes_ == 16 ? 1u : 0u;
         Control* dc = o.ctrl.as<Control>();
         b.pool_ctr = &dc->pool_ctr;
+        b.seg_ctr = &dc->seg_ctr;
         b.flags = &dc->flags;
         b.counters = counting_ ? dc->counters : nullptr;
         // counts go to a per-attempt scratch: an attempt that ends in a pool overflow or an input error is re-run

@@ -230,40 +230,94 @@ struct WalkStats {
     uint32_t m, t, p, w, walks;
 };
 
-// Candidate sources of one start position — trie hits (a postings list each) and unknown-word spans (a run of
-// unk.def entries each) — kept in shared memory between the counting walk and the fill, so that the dependent
-// pointer chase through the double array is done once and the fill can deal the candidates of a whole warp to its
-// lanes.  A segment = {kind | index, end slot} + its candidate count.  Column-major ([segment][thread]) keeps the
-// accesses of a warp conflict-free.
-constexpr uint32_t kMaxHits = 8;
+// The candidate pool holds, per start position, its candidate SOURCES rather than the candidates: every candidate
+// is one record of a postings list (trie hit) or of the unk.def entries of a character category (unknown-word span),
+// and the candidates of one source are a contiguous run of it.  A segment (8 bytes) names such a run:
+//   x = kind | index   kind: 0 system postings, kSegUser user postings (index = the key's header, the records follow
+//                      it), kSegUnk unknown words (index = the first unk_ent entry)
+//   y = delta << 16 | count   count: candidates in the run (< 2^16); delta (signed 16 bits): end slot of the run
+//                      minus that of the segment before it, or minus the position's own slot for the first one.
+// A source with 2^16 candidates or more becomes several segments; an end slot more than 32 767 away from the one
+// before is reached through count-0 segments that only move it.  The segments of a position follow the candidate
+// order of Tokenizer::add_lattice_edges (user, system, unknown; ascending length; CSV order inside a postings list),
+// so candidate j of a position is found by walking its segments (cand_at).  The device image keeps both arrays
+// below 2^30 entries, so that index + count never reaches the kind bits.
 constexpr uint32_t kSegUser = 0x80000000u, kSegUnk = 0x40000000u, kSegIndex = 0x3FFFFFFFu;
-struct HitBuf {
-    uint2* col;    // &hits[0][threadIdx.x]; stride blockDim.x
-    uint8_t* cnt;  // &counts[0][threadIdx.x]; stride blockDim.x
-    uint32_t stride;
-    uint32_t n;  // segments seen; kMaxHits + 1 and beyond = does not fit (the fill then regenerates per thread)
+constexpr int32_t kSegMaxDelta = 32767;
+
+// Candidate j of segment s, whose run ends at slot `end`: {left | right << 16, cost word, word_idx, end slot}.
+__device__ __forceinline__ uint4 seg_record(const DictView& d, uint2 s, uint32_t j, uint32_t end) {
+    if (s.x & kSegUnk) {  // unknown.rs:133 `word_id as u16`, LexType::Unknown
+        const uint32_t id = (s.x & kSegIndex) + j;
+        const uint2 ue = __ldg(&d.unk_ent[id]);
+        return make_uint4(ue.x, ue.y, (2u << 30) | (id & 0xFFFFu), end);
+    }
+    const uint4* __restrict__ post = (s.x & kSegUser) ? d.usr_post : d.sys_post;
+    uint4 r = __ldg(&post[(s.x & kSegIndex) + 1 + j]);  // the candidate record, end slot still open
+    r.w = end;
+    return r;
+}
+
+// Candidate j (< the position's candidate count) of the start position at `slot`, whose segments are seg(0),
+// seg(1), ...: a walk over the segments before it.
+template <class SegAt>
+__device__ __forceinline__ uint4 cand_at(const DictView& d, SegAt seg, uint32_t slot, uint32_t j) {
+    uint32_t h = 0, end = slot;
+    uint2 s = seg(0u);
+    for (;;) {
+        end += uint32_t(int32_t(s.y) >> 16);
+        const uint32_t c = s.y & 0xFFFFu;
+        if (j < c) break;
+        j -= c;
+        s = seg(++h);
+    }
+    return seg_record(d, s, j, end);
+}
+
+// Segment encoder of one start position.  The count pass of k_candidates keeps up to kMaxSegs segments in shared
+// memory (column-major, [segment][thread], so the accesses of a warp are conflict-free) and counts the rest; a
+// position with more is walked again after the allocation, straight into the pool, with ends_cnt set.
+constexpr uint32_t kMaxSegs = 8;
+struct SegOut {
+    uint2* dst;          // segment h goes to dst[h * stride] while h < cap
+    uint32_t stride, cap;
+    uint32_t n;          // segments so far, also those past cap
+    uint32_t last;       // end slot of the segment before; the position's slot at first
+    uint32_t* ends_cnt;  // non-null: every candidate is also counted into its end row
+    __device__ __forceinline__ void put(uint32_t x, uint32_t y) {
+        if (n < cap) dst[n * stride] = make_uint2(x, y);
+        ++n;
+    }
     __device__ __forceinline__ void push(uint32_t v, uint32_t end, uint32_t count) {
-        if (n < kMaxHits && count < 256u && (v & kSegIndex) == (v & ~(kSegUser | kSegUnk))) {
-            col[n * stride] = make_uint2(v, end);
-            cnt[n * stride] = uint8_t(count);
-            ++n;
-        } else {
-            n = kMaxHits + 1;
+        if (count == 0) return;
+        if (ends_cnt) atomicAdd(&ends_cnt[end], count);
+        int32_t delta = int32_t(end - last);
+        while (delta > kSegMaxDelta || delta < -kSegMaxDelta) {
+            const int32_t step = delta > 0 ? kSegMaxDelta : -kSegMaxDelta;
+            put(v, uint32_t(step) << 16);
+            delta -= step;
+        }
+        last = end;
+        for (;;) {
+            const uint32_t c = min(count, 0xFFFFu);
+            put(v, (uint32_t(delta) << 16) | c);
+            count -= c;
+            if (count == 0) break;
+            v += c;  // the next run starts c records further; for postings `index` stays one before the run
+            delta = 0;
         }
     }
 };
 
 // Lexicon::common_prefix_iterator (lexicon.rs:33-46): crawdad common-prefix search over the double
-// array (trie.rs:49-56), then the postings of every hit (posting.rs:18-21) with their WordParams.
+// array (trie.rs:49-56); every hit is one segment, the postings list of its key (posting.rs:18-21).
 // BND (bounded batches): the walk stops at q_end = lim(sw), the first required boundary after sw, so no word that
 // crosses it is a candidate or counts as a match.
-template <bool FILL, bool COUNT, bool BND = false>
+template <bool COUNT, bool BND = false>
 __device__ __forceinline__ uint32_t walk_lexicon(const uint4* __restrict__ nodes, uint32_t num_nodes,
-                                                 const uint4* __restrict__ post,
                                                  const uint32_t* __restrict__ codes,
-                                                 const uint32_t* __restrict__ groupable, uint32_t sw, uint4* out,
-                                                 uint32_t* ends_cnt, WalkStats& st, HitBuf* hb = nullptr,
-                                                 uint32_t lex_flag = 0, uint32_t q_end = 0) {
+                                                 const uint32_t* __restrict__ groupable, uint32_t sw, WalkStats& st,
+                                                 SegOut* so = nullptr, uint32_t lex_flag = 0, uint32_t q_end = 0) {
     if (num_nodes == 0) return 0;
     uint32_t count = 0, node = 0, d = 0, hits = 0;
     uint32_t nbase = __ldg(&nodes[0].x);
@@ -283,15 +337,7 @@ __device__ __forceinline__ uint32_t walk_lexicon(const uint4* __restrict__ nodes
         if (nd.z == kNone) continue;
         const uint32_t v = nd.z;
         const uint32_t plen = nd.w;
-        if (!FILL && hb) hb->push(v | lex_flag, q + 1, plen);
-        if (FILL) {
-            for (uint32_t j = 0; j < plen; ++j) {
-                uint4 e = __ldg(&post[v + 1 + j]);
-                e.w = q + 1;
-                out[count + j] = e;
-            }
-            atomicAdd(&ends_cnt[q + 1], plen);
-        }
+        if (so) so->push(v | lex_flag, q + 1, plen);
         count += plen;
         ++hits;
         if (COUNT) {
@@ -308,24 +354,15 @@ __device__ __forceinline__ uint32_t walk_lexicon(const uint4* __restrict__ nodes
     return count;
 }
 
-// UnkHandler::gen_unk_words (unknown.rs:69-116) with scan_entries (:119-137).
-template <bool FILL>
+// UnkHandler::gen_unk_words (unknown.rs:69-116) with scan_entries (:119-137): every span is one segment.
 __device__ __forceinline__ uint32_t gen_unknown(const DictView& d, uint32_t sw, uint32_t ci, uint32_t g,
-                                                bool has_matched, uint4* out, uint32_t* ends_cnt, HitBuf* hb = nullptr) {
+                                                bool has_matched, SegOut* so = nullptr) {
     if (has_matched && !ci_invoke(ci)) return 0;
     const uint32_t e0 = __ldg(&d.unk_off[ci_base(ci)]), e1 = __ldg(&d.unk_off[ci_base(ci) + 1]);
     const uint32_t ne = e1 - e0;
     uint32_t count = 0;
     auto span = [&](uint32_t end) {
-        if (FILL) {
-            for (uint32_t j = 0; j < ne; ++j) {
-                uint2 e = __ldg(&d.unk_ent[e0 + j]);
-                // unknown.rs:133 `word_id as u16`, LexType::Unknown
-                out[count + j] = make_uint4(e.x, e.y, (2u << 30) | ((e0 + j) & 0xFFFFu), end);
-            }
-            if (ne) atomicAdd(&ends_cnt[end], ne);
-        }
-        if (!FILL && hb && ne) hb->push(kSegUnk | e0, end, ne);
+        if (so) so->push(kSegUnk | e0, end, ne);
         count += ne;
     };
     bool grouped = false;
@@ -382,36 +419,20 @@ __device__ __forceinline__ StartWord start_word(const DictView& d, const Batch& 
 }
 
 // Candidate count of an active start position: user lexicon, system lexicon, then unknown words, the order of
-// Tokenizer::add_lattice_edges.  `matched` = some lexicon word starts here.  With hb the sources are kept for a fill.
+// Tokenizer::add_lattice_edges.  Its segments go to `so` (so.last = the position's slot).
 template <bool BND = false>
-__device__ __forceinline__ uint32_t count_candidates(const DictView& d, const Batch& b, const StartWord& w, bool& matched,
-                                                     HitBuf* hb) {
+__device__ __forceinline__ uint32_t count_candidates(const DictView& d, const Batch& b, const StartWord& w, SegOut& so) {
     WalkStats st{0, 0, 0, 0, 0};
     uint32_t cu = 0;
     if (d.usr_table)
-        cu = walk_lexicon<false, false, BND>(d.usr_nodes, d.usr_num_nodes, d.usr_post, b.code_usr, b.groupable, w.sw,
-                                             nullptr, nullptr, st, hb, kSegUser, w.sw + w.lim);
-    uint32_t cs = walk_lexicon<false, false, BND>(d.sys_nodes, d.sys_num_nodes, d.sys_post, b.code_sys, b.groupable, w.sw,
-                                                  nullptr, nullptr, st, hb, 0, w.sw + w.lim);
-    matched = (cu + cs) != 0;
-    return cu + cs + gen_unknown<false>(d, w.sw, w.ci, w.g, matched, nullptr, nullptr, hb);
+        cu = walk_lexicon<false, BND>(d.usr_nodes, d.usr_num_nodes, b.code_usr, b.groupable, w.sw, st, &so, kSegUser,
+                                      w.sw + w.lim);
+    uint32_t cs = walk_lexicon<false, BND>(d.sys_nodes, d.sys_num_nodes, b.code_sys, b.groupable, w.sw, st, &so, 0,
+                                           w.sw + w.lim);
+    return cu + cs + gen_unknown(d, w.sw, w.ci, w.g, (cu + cs) != 0, &so);  // (cu + cs) != 0: a lexicon word starts here
 }
 
-// Writes the candidates count_candidates counted to `out`, in the same order, and adds them to ends_cnt.
-template <bool BND = false>
-__device__ __forceinline__ void fill_candidates(const DictView& d, const Batch& b, const StartWord& w, bool matched,
-                                                uint4* out) {
-    WalkStats st{0, 0, 0, 0, 0};
-    uint32_t n = 0;
-    if (d.usr_table)
-        n += walk_lexicon<true, false, BND>(d.usr_nodes, d.usr_num_nodes, d.usr_post, b.code_usr, b.groupable, w.sw,
-                                            out + n, b.ends_cnt, st, nullptr, 0, w.sw + w.lim);
-    n += walk_lexicon<true, false, BND>(d.sys_nodes, d.sys_num_nodes, d.sys_post, b.code_sys, b.groupable, w.sw, out + n,
-                                        b.ends_cnt, st, nullptr, 0, w.sw + w.lim);
-    gen_unknown<true>(d, w.sw, w.ci, w.g, matched, out + n, b.ends_cnt);
-}
-
-// Candidate header of a start position with g0 != 0: {cand_ptr, count}, plus the skip / flags side entry.
+// Candidate header of a start position with g0 != 0: {segment ptr, candidate count}, plus the skip / flags side entry.
 __device__ __forceinline__ void store_info(const Batch& b, uint32_t slot, uint32_t ptr, uint32_t cnt, const StartWord& w) {
     const bool special = (w.skip | w.flags) != 0;
     b.info[slot] = make_uint2(ptr, cnt | (special ? kInfoSpecial : 0u));
@@ -434,88 +455,64 @@ __global__ void __launch_bounds__(256) k_candidates(DictView d, Batch b) {
     const StartWord sw = start_word<BND>(d, b, slot, g0);
     const bool active = sw.active;
     uint32_t cnt = 0;
-    bool matched = false;
-    __shared__ uint2 s_hits[kMaxHits][256];
-    __shared__ uint8_t s_seg_cnt[kMaxHits][256];
-    HitBuf hb{&s_hits[0][threadIdx.x], &s_seg_cnt[0][threadIdx.x], 256, 0};
-    if (active) cnt = count_candidates<BND>(d, b, sw, matched, &hb);
-    // Block-aggregated allocation from the candidate pool: a scan inside each warp, the eight warp totals through
+    __shared__ uint2 s_segs[kMaxSegs][256];
+    SegOut so{&s_segs[0][threadIdx.x], 256, kMaxSegs, 0, slot, nullptr};
+    if (active) cnt = count_candidates<BND>(d, b, sw, so);
+    const uint32_t nseg = so.n;
+    // Block-aggregated allocation from the segment pool: a scan inside each warp, the eight warp totals through
     // shared memory, ONE atomicAdd per block.  (One atomic per warp was 1.3 M same-address atomics per batch, and
-    // every warp sat on the round trip of its own; the pool also comes out in slot order block by block.)
-    uint32_t incl = cnt;
+    // every warp sat on the round trip of its own; the pool also comes out in slot order block by block.)  The
+    // candidates are counted alongside: they are the lattice nodes, and the rows must hold them.
+    uint32_t incl = cnt, sincl = nseg;
 #pragma unroll
     for (int o = 1; o < 32; o <<= 1) {
-        uint32_t v = __shfl_up_sync(kFull, incl, o);
-        if (lane >= uint32_t(o)) incl += v;
+        const uint32_t v = __shfl_up_sync(kFull, incl, o), sv = __shfl_up_sync(kFull, sincl, o);
+        if (lane >= uint32_t(o)) {
+            incl += v;
+            sincl += sv;
+        }
     }
-    __shared__ uint32_t s_warp_total[8];
-    __shared__ unsigned long long s_block_base;
+    __shared__ uint32_t s_warp_total[8], s_warp_segs[8];
+    __shared__ unsigned long long s_block_base, s_block_cand;
     const uint32_t wid = threadIdx.x >> 5;
-    if (lane == 31) s_warp_total[wid] = incl;
+    if (lane == 31) {
+        s_warp_total[wid] = incl;
+        s_warp_segs[wid] = sincl;
+    }
     __syncthreads();
     if (threadIdx.x == 0) {
-        uint32_t run = 0;
+        uint32_t run = 0, srun = 0;
         for (int i = 0; i < 8; ++i) {  // warp totals -> exclusive offsets inside the block
-            const uint32_t t = s_warp_total[i];
+            const uint32_t t = s_warp_total[i], st = s_warp_segs[i];
             s_warp_total[i] = run;
+            s_warp_segs[i] = srun;
             run += t;
+            srun += st;
         }
-        s_block_base = run ? atomicAdd(b.pool_ctr, (unsigned long long)run) : 0ull;
-        if (s_block_base + run > (unsigned long long)b.cand_cap) atomicOr(b.flags, kFlagPoolOverflow);
+        s_block_base = srun ? atomicAdd(b.seg_ctr, (unsigned long long)srun) : 0ull;
+        s_block_cand = run ? atomicAdd(b.pool_ctr, (unsigned long long)run) : 0ull;
+        if (s_block_base + srun > (unsigned long long)b.seg_cap || s_block_cand + run > (unsigned long long)b.cand_cap)
+            atomicOr(b.flags, kFlagPoolOverflow);
     }
     __syncthreads();
-    const unsigned long long wbase = s_block_base + s_warp_total[wid];
-    const uint32_t warp_total = __shfl_sync(kFull, incl, 31);
-    const bool fits = wbase + warp_total <= (unsigned long long)b.cand_cap;
-    uint32_t ptr = uint32_t(wbase) + (incl - cnt);
+    const unsigned long long wbase = s_block_base + s_warp_segs[wid], cbase = s_block_cand + s_warp_total[wid];
+    const bool fits = wbase + __shfl_sync(kFull, sincl, 31) <= (unsigned long long)b.seg_cap &&
+                      cbase + __shfl_sync(kFull, incl, 31) <= (unsigned long long)b.cand_cap;
+    const uint32_t ptr = uint32_t(wbase) + (sincl - nseg);
     if (in_range && g0 != 0) store_info(b, slot, ptr, fits ? cnt : 0, sw);
-    // Fill.  Usual case: every position of the warp kept its sources in the segment buffer; the warp's candidates
-    // (contiguous in the pool, in position order) are then dealt to the 32 lanes as ONE list — lane i writes entries
-    // i, i + 32, ...: full-width, coalesced stores and loads that walk postings lists side by side, instead of
-    // every lane copying its own run of ~7 candidates with the others idle.  An entry finds its position by a
-    // binary search over the warp's inclusive counts (shuffles) and its segment by a short scan of that position's
-    // segment counts.
-    const bool pooled = !__any_sync(kFull, hb.n > kMaxHits);
-    if (pooled) {
-        if (fits) {
-            if (active)
-                for (uint32_t h = 0; h < hb.n; ++h) atomicAdd(&b.ends_cnt[hb.col[h * hb.stride].y], uint32_t(hb.cnt[h * hb.stride]));
-            const uint32_t col0 = threadIdx.x & ~31u;
-            for (uint32_t e0 = 0; e0 < warp_total; e0 += 32) {
-                const uint32_t e = e0 + lane;
-                uint32_t t = 0;  // owner = number of positions whose inclusive count is <= e
-#pragma unroll
-                for (uint32_t step = 16; step; step >>= 1) {
-                    const uint32_t v = __shfl_sync(kFull, incl, t + step - 1);
-                    if (v <= e) t += step;
-                }
-                t = min(t, 31u);
-                uint32_t local = e - __shfl_sync(kFull, incl - cnt, t);
-                if (e < warp_total) {
-                    uint32_t h = 0;
-                    uint32_t c = s_seg_cnt[0][col0 + t];
-                    while (local >= c) {  // e < warp_total: the owner has a segment that holds it
-                        local -= c;
-                        ++h;
-                        c = s_seg_cnt[h][col0 + t];
-                    }
-                    const uint2 seg = s_hits[h][col0 + t];
-                    uint4 rec;
-                    if (seg.x & kSegUnk) {  // unknown.rs:133 `word_id as u16`, LexType::Unknown
-                        const uint32_t id = (seg.x & kSegIndex) + local;
-                        const uint2 ue = __ldg(&d.unk_ent[id]);
-                        rec = make_uint4(ue.x, ue.y, (2u << 30) | (id & 0xFFFFu), seg.y);
-                    } else {
-                        const uint4* __restrict__ post = (seg.x & kSegUser) ? d.usr_post : d.sys_post;
-                        rec = __ldg(&post[(seg.x & kSegIndex) + 1 + local]);  // the candidate record, end slot still open
-                        rec.w = seg.y;
-                    }
-                    b.cand[uint32_t(wbase) + e] = rec;
-                }
-            }
+    // Fill: the position's segments go to the pool as they are, and its candidates into their end rows.
+    if (!(active && fits && cnt)) return;
+    if (nseg <= kMaxSegs) {
+        uint32_t end = slot;
+        for (uint32_t h = 0; h < nseg; ++h) {
+            const uint2 s = s_segs[h][threadIdx.x];
+            end += uint32_t(int32_t(s.y) >> 16);
+            if (s.y & 0xFFFFu) atomicAdd(&b.ends_cnt[end], s.y & 0xFFFFu);
+            b.seg[ptr + h] = s;
         }
-    } else if (active && fits && cnt) {  // some position has more sources than the buffer holds: regenerate per thread
-        fill_candidates<BND>(d, b, sw, matched, b.cand + ptr);
+    } else {  // more segments than the buffer holds: walk again, straight into the pool
+        SegOut out{b.seg + ptr, 1, nseg, 0, slot, b.ends_cnt};
+        count_candidates<BND>(d, b, sw, out);
     }
 }
 
@@ -593,11 +590,9 @@ __global__ void __launch_bounds__(256) k_candidate_stats(DictView d, Batch b, ui
             WalkStats st{0, 0, 0, 0, 0};
             uint32_t cu = 0;
             if (d.usr_table)
-                cu = walk_lexicon<false, true>(d.usr_nodes, d.usr_num_nodes, d.usr_post, b.code_usr, b.groupable, sw,
-                                               nullptr, nullptr, st);
-            uint32_t cs = walk_lexicon<false, true>(d.sys_nodes, d.sys_num_nodes, d.sys_post, b.code_sys, b.groupable,
-                                                    sw, nullptr, nullptr, st);
-            uint32_t ck = gen_unknown<false>(d, sw, b.cinfo[sw], g, (cu + cs) != 0, nullptr, nullptr);
+                cu = walk_lexicon<true>(d.usr_nodes, d.usr_num_nodes, b.code_usr, b.groupable, sw, st);
+            uint32_t cs = walk_lexicon<true>(d.sys_nodes, d.sys_num_nodes, b.code_sys, b.groupable, sw, st);
+            uint32_t ck = gen_unknown(d, sw, b.cinfo[sw], g, (cu + cs) != 0);
             out = make_uint4(st.m, st.t, st.p, st.w + ck);
             out.x |= st.walks << 24;  // <= 2 walks; M stays far below 2^24 per position
         }
@@ -615,7 +610,7 @@ __global__ void __launch_bounds__(256) k_candidate_stats(DictView d, Batch b, ui
 // and ~8 predecessors, so G = 8 keeps most lanes busy where one warp per sentence left 3/4 idle.
 // ---------------------------------------------------------------------------------------------
 
-// Candidate header of one start position as {cand_ptr, cand_cnt, skip, flags}; the last two live in a side array
+// Candidate header of one start position as {seg_ptr, cand_cnt, skip, flags}; the last two live in a side array
 // that only the few positions with a skipped space run or the trailing flag ever touch.
 __device__ __forceinline__ uint4 load_info(const Batch& b, uint32_t slot) {
     const uint2 i8 = b.info[slot];
@@ -728,12 +723,6 @@ __device__ __forceinline__ SentenceEnd insert_eos(const DictView& d, const Batch
     }
     return {K, base, n};
 }
-
-// Tuning knobs of k_viterbi, swept with A/B builds (tools/build_variants.sh, tools/ab_multi.py): VBT_K3_MIN_BLOCKS
-// (above) and VBT_K3_PF_DIST = how many candidates ahead one lane per group hints into L1 (0 = no hint).
-#ifndef VBT_K3_PF_DIST
-#define VBT_K3_PF_DIST 8
-#endif
 
 // ConnectorCost::cost(right_id, left_id) for one fixed left id (one candidate).
 template <int CONN>
@@ -854,14 +843,6 @@ __device__ __forceinline__ void viterbi_sweep(const DictView& d, const Batch& b,
             cntE += (unsigned long long)K * ncand;
             cntN += ncand;
         }
-#if VBT_K3_PF_DIST
-        // K2 hands out the candidate pool in position order, so the candidates of the positions ahead follow
-        // this position's; K2 wrote them long ago (evicted from L2), pull the line ahead while this position works
-        if (visit && gl == 0 && info.x + ncand + VBT_K3_PF_DIST < b.cand_cap) {
-            const uint4* nx = b.cand + info.x + ncand + VBT_K3_PF_DIST;
-            asm volatile("prefetch.global.L1 [%0];" ::"l"(nx));
-        }
-#endif
         const uint32_t max_cand = __reduce_max_sync(kFull, ncand);
         // first chunk of predecessors: independent of the candidates, so issue it alongside their load
         int2 pr_first = make_int2(0, 0);
@@ -871,7 +852,7 @@ __device__ __forceinline__ void viterbi_sweep(const DictView& d, const Batch& b,
             uint4 cd = make_uint4(0, 0, 0, 0);
             uint32_t fill = 0;
             if (valid) {
-                cd = b.cand[info.x + c0 + gl];
+                cd = cand_at(d, [&](uint32_t h) { return __ldg(&b.seg[info.x + h]); }, slot, c0 + gl);
                 // row metadata of the node's end position: independent of the minimum search, fetch now
                 const uint2 me = b.ends_meta[cd.w];
                 fill = me.y;  // next free entry of that row (absolute)
@@ -972,9 +953,6 @@ __global__ void __launch_bounds__(128, (CONN == 0 && !COUNT) ? VBT_K3_MIN_BLOCKS
 // 14.8 ms).
 #define VBT_K3V2_MIN_BLOCKS (48 / VBT_K3V2_WARPS)
 #endif
-#ifndef VBT_K3V2_PF_DIST
-#define VBT_K3V2_PF_DIST 8
-#endif
 
 constexpr int kPredCap = 32;                             // predecessors staged per pass
 constexpr int32_t kPredSentinel = INT32_MAX - 70000;     // + any i16 stays below INT32_MAX and above every real best
@@ -1067,7 +1045,8 @@ struct ConnCol : ConnRow<CONN> {
 
 // Shared-memory window of one warp of k_viterbi2: a staging row per sentence ({cost, right} of the predecessors, up
 // to kPredCap per pass plus padding to whole batches; the odd multiple of 32 bytes skews the rows across the banks),
-// and per sentence the descriptor of its current position {cand_ptr, slot, row offset, K} and its candidate count.
+// and per sentence the descriptor of its current position {seg_ptr, slot, row offset, K}, its candidate count and
+// its first G segments.
 template <int G>
 struct V2Shared {
     static constexpr uint32_t SPW = 32 / G;
@@ -1075,13 +1054,15 @@ struct V2Shared {
     int2 rows[SPW][kPredCap + 4];
     uint4 desc[SPW];
     uint32_t cnt[8];
+    uint2 segs[SPW][G];
 };
 
 template <int G, int CONN, bool PRUNE, bool SPACE>
 __device__ __forceinline__ void viterbi2_sweep(const DictView& d, const Batch& b, const uint32_t sw /* shared-window address of this warp's V2Shared */) {
     constexpr uint32_t SPW = 32 / G;  // sentences per warp
     constexpr uint32_t kRowBytes = V2Shared<G>::kRowBytes;
-    constexpr uint32_t kDescOff = SPW * kRowBytes, kCntOff = kDescOff + SPW * 16;
+    constexpr uint32_t kDescOff = SPW * kRowBytes, kCntOff = kDescOff + SPW * 16, kSegOff = kCntOff + 8 * 4;
+    static_assert(kSegOff == offsetof(V2Shared<G>, segs), "V2Shared layout");
     const uint32_t lane = threadIdx.x & 31;
     const uint32_t gl = lane % G, sub = lane / G;
     const uint32_t sidx = ((blockIdx.x * blockDim.x + threadIdx.x) >> 5) * SPW + sub;
@@ -1113,12 +1094,13 @@ __device__ __forceinline__ void viterbi2_sweep(const DictView& d, const Batch& b
             }
         }
         if (ncand == 0) K = 0;
+        // The position's first G segments, one per lane of the group, for the lanes that take its candidates below
+        // (a position rarely has more; those are read from the pool).  Loaded now, stored to shared memory after the
+        // predecessor copies are under way.  Past the position's own segments a lane loads a neighbour's: unused.
+        const bool stage = ncand != 0 && cptr + gl < b.seg_cap;
+        uint2 sg = make_uint2(0, 0);
+        if (stage) sg = __ldg(&b.seg[cptr + gl]);
         const uint32_t max_k = __reduce_max_sync(kFull, K);
-#if VBT_K3V2_PF_DIST
-        // K2 hands out the candidate pool in position order: pull the line of the positions ahead towards L1
-        if (ncand && gl == 0 && cptr + ncand + VBT_K3V2_PF_DIST < b.cand_cap)
-            asm volatile("prefetch.global.L1 [%0];" ::"l"(b.cand + cptr + ncand + VBT_K3V2_PF_DIST));
-#endif
         // The candidates of the warp's sentences are dealt to the 32 lanes as ONE pool (sentence after sentence):
         // a position with 3 candidates next to one with 13 fills half a warp, not two rounds of 8-lane groups.
         // Every group publishes its position; a lane then finds which sentence its pool index falls into.
@@ -1146,6 +1128,8 @@ __device__ __forceinline__ void viterbi2_sweep(const DictView& d, const Batch& b
                     asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(own + k * 8u), "r"(kPredSentinel), "r"(0) : "memory");
             }
         }
+        if (stage)
+            asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(sw + kSegOff + lane * 8u), "r"(sg.x), "r"(sg.y) : "memory");
         __syncwarp();
         for (uint32_t q0 = 0; q0 < total; q0 += 32) {
             const uint32_t q = q0 + lane;
@@ -1164,15 +1148,27 @@ __device__ __forceinline__ void viterbi2_sweep(const DictView& d, const Batch& b
                     }
                 }
             }
-            uint4 ds;  // {cand_ptr, slot, row offset, K} of the sentence this lane's candidate belongs to
+            uint4 ds;  // {seg_ptr, slot, row offset, K} of the sentence this lane's candidate belongs to
             asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];"
                          : "=r"(ds.x), "=r"(ds.y), "=r"(ds.z), "=r"(ds.w)
                          : "r"(sw + kDescOff + s2 * 16u));
             uint4 cd = make_uint4(0, 0, 0, 0);
             uint32_t nxt = 0;
             if (valid) {
-                cd = b.cand[ds.x + (q - before)];
-                nxt = b.ends_meta[cd.w].y;  // next free entry of the row the node ends in: independent of the search
+                const uint32_t segs = sw + kSegOff + s2 * (G * 8u);  // lane (s2, h) staged segment h
+                cd = cand_at(
+                    d,
+                    [&](uint32_t h) {
+                        uint2 s;
+                        if (h < uint32_t(G))
+                            asm volatile("ld.shared.v2.b32 {%0, %1}, [%2];" : "=r"(s.x), "=r"(s.y) : "r"(segs + h * 8u));
+                        else
+                            s = __ldg(&b.seg[ds.x + h]);
+                        return s;
+                    },
+                    ds.y, q - before);
+                // next free entry of the row the node ends in: independent of the search, and of the record's load
+                nxt = b.ends_meta[cd.w].y;
             }
             const ConnCol<CONN> conn(d, cd.x & 0xFFFFu);
             // Lattice::search_min_node (lattice.rs:129-151): `<=` keeps the LAST minimum
@@ -1352,6 +1348,9 @@ __global__ void __launch_bounds__(256) k_marg_forward(DictView d, Batch b, MargA
     }
     __syncwarp();
     const double th = m.theta;
+    // the lattice entries of the candidates of the visited positions, numbered in position order from the sentence's
+    // first row offset: there are fewer of them than the sentence's rows hold (BOS is one more)
+    uint32_t centry = b.ends_meta[base].x;
     uint32_t slot_end = last, skip_slot = base;
     // the positions K3 visits, by the rules of its sweep (tokenizer.rs:110-135): a non-empty row, outside a skipped
     // space run, and the trailing flag ends the sweep
@@ -1374,7 +1373,7 @@ __global__ void __launch_bounds__(256) k_marg_forward(DictView d, Batch b, MargA
             uint32_t peers = 0, f = 0;
             const uint32_t vmask = __ballot_sync(kFull, valid);
             if (valid) {
-                cd = b.cand[info.x + c];
+                cd = cand_at(d, [&](uint32_t h) { return __ldg(&b.seg[info.x + h]); }, slot, c);
                 peers = __match_any_sync(vmask, cd.w);
                 f = m.fill[cd.w];
             }
@@ -1382,7 +1381,7 @@ __global__ void __launch_bounds__(256) k_marg_forward(DictView d, Batch b, MargA
             if (valid) {  // the entry insert_node gave this candidate
                 const uint32_t rank = __popc(peers & lanemask_lt());
                 const uint32_t idx = f + rank;
-                m.cand_entry[info.x + c] = idx;
+                m.cand_entry[centry + c] = idx;
                 if (rank == 0) m.fill[cd.w] = f + __popc(peers);
                 const ConnRow<CONN> conn(d, cd.x & 0xFFFFu);
                 const long long wc = int16_t(cd.y & 0xFFFFu);
@@ -1397,6 +1396,7 @@ __global__ void __launch_bounds__(256) k_marg_forward(DictView d, Batch b, MargA
             }
             __syncwarp();
         }
+        centry += ncand;
     }
     if (lane == 0) {  // EOS: left id 0, no word cost
         const uint2 me = b.ends_meta[slot_end];
@@ -1421,6 +1421,10 @@ __global__ void __launch_bounds__(256) k_marg_backward(DictView d, Batch b, Marg
     const uint32_t slot_end = base + b.eos[s].y;  // the row EOS connects to
     const long long r_eos = m.r_eos[s];
     const double th = m.theta;
+    // one past the last candidate entry k_marg_forward numbered (it counts from the sentence's first row offset)
+    uint32_t centry = 0;
+    for (uint32_t slot = base + lane; slot < slot_end; slot += 32) centry += m.ncand[slot];
+    centry = b.ends_meta[base].x + __reduce_add_sync(kFull, centry);
     for (uint32_t slot = last + 1; slot-- > base;) {
         const uint2 me = b.ends_meta[slot];
         const uint32_t eo = me.x, K = me.y - me.x;
@@ -1432,18 +1436,25 @@ __global__ void __launch_bounds__(256) k_marg_backward(DictView d, Batch b, Marg
             }
         } else {  // no successor at all beyond EOS's row or at a position the sweep skips: -inf
             const uint32_t nc = slot < slot_end ? m.ncand[slot] : 0u;
-            const uint32_t cptr = nc ? b.info[slot].x : 0u;
+            const uint32_t sptr = nc ? b.info[slot].x : 0u;
+            centry -= nc;
             for (uint32_t k = lane; k < K; k += 32) {
                 double L = -INFINITY;
                 if (nc) {
                     const long long rk = m.R[eo + k];
                     const uint32_t right = uint32_t(b.ends_hot[eo + k].y);
-                    for (uint32_t c = 0; c < nc; ++c) {
-                        const uint4 cd = b.cand[cptr + c];
-                        const uint32_t e = m.cand_entry[cptr + c];
-                        const ConnRow<CONN> conn(d, cd.x & 0xFFFFu);
-                        const long long x = rk + conn.cost(d, right) + int16_t(cd.y & 0xFFFFu);
-                        L = lse2(L, m.ab[e].y - th * double(x - m.R[e]));
+                    // the position's candidates in candidate order, segment by segment
+                    uint32_t c = 0, end = slot;
+                    for (uint32_t h = 0; c < nc; ++h) {
+                        const uint2 sg = __ldg(&b.seg[sptr + h]);
+                        end += uint32_t(int32_t(sg.y) >> 16);
+                        for (uint32_t j = 0; j < (sg.y & 0xFFFFu); ++j, ++c) {
+                            const uint4 cd = seg_record(d, sg, j, end);
+                            const uint32_t e = m.cand_entry[centry + c];
+                            const ConnRow<CONN> conn(d, cd.x & 0xFFFFu);
+                            const long long x = rk + conn.cost(d, right) + int16_t(cd.y & 0xFFFFu);
+                            L = lse2(L, m.ab[e].y - th * double(x - m.R[e]));
+                        }
                     }
                 }
                 m.ab[eo + k].y = L;
@@ -2135,7 +2146,7 @@ __global__ void __launch_bounds__(256) k_format_write_best(DictView d, FormatArg
 // k_small_batch: the whole pipeline above for a small host batch in ONE thread block, so that a call costs one
 // launch.  The device-wide scans between the kernels become block scans between __syncthreads(); each stage calls
 // the per-sentence / per-position bodies of its kernel:
-//   count_chars_one -> scan -> decode_one -> start_word / count_candidates / fill_candidates -> scan -> viterbi_sweep
+//   count_chars_one -> scan -> decode_one -> start_word / count_candidates (count, then fill) -> scan -> viterbi_sweep
 //   (k_viterbi's sweep, 32 lanes per sentence, no pruning) -> backtrack_count_one -> scan -> backtrack_write_one
 //   [-> format_len_one -> scan -> format_write_one].
 // A warp takes one sentence at a time, a thread one start position.  The batch flags live in shared memory and
@@ -2216,22 +2227,29 @@ __global__ void __launch_bounds__(kSmallThreads, 1) k_small_batch(DictView d, Ba
             }
         }
         __syncthreads();
-        // K2: a thread per start position; the pool is handed out in position order by a scan per block-wide tile
-        unsigned long long carry = 0;
+        // K2: a thread per start position; the segment pool is handed out in position order by a scan per block-wide
+        // tile, and the candidates are counted the same way (the lattice rows must hold them)
+        unsigned long long carry = 0, seg_carry = 0;
         for (uint32_t base = 0; base < total_slots; base += blockDim.x) {
             const uint32_t slot = base + tid;
             const uint32_t g0 = slot < total_slots ? b.groupable[slot] : 0;
             const StartWord w = start_word<BND>(d, b, slot, g0);
-            bool matched = false;
-            const uint32_t cnt = w.active ? count_candidates<BND>(d, b, w, matched, nullptr) : 0;
+            SegOut so{nullptr, 0, 0, 0, slot, nullptr};
+            const uint32_t cnt = w.active ? count_candidates<BND>(d, b, w, so) : 0;
+            const uint32_t nseg = so.n;
             unsigned long long tile;
-            const unsigned long long ptr = carry + block_exclusive(cnt, tile, s_warp);
+            const unsigned long long cptr = carry + block_exclusive(cnt, tile, s_warp);
             carry += tile;
-            if (ptr + cnt > b.cand_cap) {
+            const unsigned long long ptr = seg_carry + block_exclusive(nseg, tile, s_warp);
+            seg_carry += tile;
+            if (cptr + cnt > b.cand_cap || ptr + nseg > b.seg_cap) {
                 atomicOr(&s_flags, kFlagPoolOverflow);
             } else if (g0 != 0) {
                 store_info(b, slot, uint32_t(ptr), cnt, w);
-                if (cnt) fill_candidates<BND>(d, b, w, matched, b.cand + ptr);
+                if (cnt) {
+                    SegOut out{b.seg + ptr, 1, nseg, 0, slot, b.ends_cnt};
+                    count_candidates<BND>(d, b, w, out);
+                }
             }
         }
         __syncthreads();

@@ -103,22 +103,25 @@ struct Batch {
     uint32_t* cinfo;
     uint32_t* groupable;  // 0 marks the sentinel slot
     uint32_t* byte_pos;   // byte offset of the character inside its sentence (c2b, sentence.rs:40-46)
-    uint2* info;          // {cand_ptr, cand_cnt | kInfoSpecial}
+    uint2* info;          // {seg_ptr (first segment in `seg`), cand_cnt | kInfoSpecial}
     uint2* info_ex;       // {skip (start_word - start_node), flags}; written only where info.y has kInfoSpecial
     uint32_t* ends_cnt;   // upper bound of nodes ending here (+1 for BOS at the first slot)
     uint2* ends_meta;     // {exclusive scan of ends_cnt = row offset, next free entry of the row (absolute index)}
     // candidate pool and lattice rows
-    // {left | right << 16, word_cost (i16, low half) | lower bound of the connection cost into `left` (i16, high
-    //  half; see device_blob.hpp), word_idx, end_slot}
-    uint4* cand;
-    uint32_t cand_cap;
+    // The pool holds per start position the segments of its candidates (kernels.cu, before SegOut): 8 bytes per
+    // postings list or unknown-word span, which stand for the records {left | right << 16, word_cost (i16, low half)
+    // | lower bound of the connection cost into `left` (i16, high half; see device_blob.hpp), word_idx, end_slot}.
+    uint2* seg;
+    uint32_t seg_cap;   // segments behind `seg`
+    uint32_t cand_cap;  // candidates (= lattice nodes) the rows and the per-node arrays hold, BOS entries aside
     int2* ends_hot;       // lattice rows (CSR over end slot): {min_cost, right_id} — all the DP re-reads
     uint4* ends_cold;     // {start_node slot, best prev entry, word_idx, min_cost} — written once, read by the backtrack
     // output
     void* tokens;  // vbt_token[] (24 bytes each), or vbt_token16[] when compact != 0
     uint32_t compact;  // 1: 16-byte records {start_byte, end_byte, word_idx, total_cost} (character ranges left to the host)
     // bookkeeping
-    unsigned long long* pool_ctr;
+    unsigned long long* pool_ctr;  // candidates of the batch
+    unsigned long long* seg_ctr;   // segments of the batch (the pool's allocation counter)
     uint32_t* flags;
     unsigned long long* counters;  // kNumCounters, or nullptr when counting is off
     // ConnIdCounter (mapper.rs:87-104) over internal ids, or nullptr: lid_count[num_left], rid_count[num_right]
@@ -222,7 +225,9 @@ struct MargArgs {
     double theta;            // > 0
     uint32_t* fill;          // per slot: the row's next free entry while the forward pass numbers the nodes
     uint32_t* ncand;         // per slot: the candidates of a position the sweep visits, 0 elsewhere
-    uint32_t* cand_entry;    // per candidate of a visited position: its lattice entry
+    // per candidate of a visited position: its lattice entry; a sentence's are numbered in position order from its
+    // first row offset (ends_meta[first slot].x), so the array is as long as the lattice rows
+    uint32_t* cand_entry;
     long long* R;            // per lattice entry
     double2* ab;             // per lattice entry: {â, b̂}
     long long* r_eos;        // per sentence: R(EOS)
@@ -266,9 +271,10 @@ struct SmallBatchOut {
 // Every stage from count_chars to backtrack_write, and the output stage when f.mode != kOutNone, for a whole batch
 // in ONE launch of one thread block.  Inputs as for the separate kernels except: b.flags and f.flags are ignored
 // (the kernel keeps the flags in shared memory and reports them in *out), b.order / counters / lid_count must be
-// null, b.launch_slots and b.pool_ctr are unused, and the per-slot arrays must hold n_bytes + n_sent + 1 entries
-// (the hard bound), so only the candidate pool (b.cand_cap; ends_hot / ends_cold need cand_cap + n_sent + 1
-// entries) and the text (f.text_cap) can overflow: kFlagPoolOverflow / kFlagTextOverflow, the outputs are then void.
+// null, b.launch_slots, b.pool_ctr and b.seg_ctr are unused, and the per-slot arrays must hold n_bytes + n_sent + 1
+// entries (the hard bound), so only the candidate pool (b.seg_cap segments, b.cand_cap candidates; ends_hot / ends_cold
+// need cand_cap + n_sent + 1 entries) and the text (f.text_cap) can overflow: kFlagPoolOverflow / kFlagTextOverflow,
+// the outputs are then void.
 // f.tok_off / f.tokens must equal b.tok_off / b.tokens; f.sent_len needs n_sent entries, f.text_off n_sent + 1.
 // A bounded batch (b.bnd_dist != nullptr, per-slot like the other arrays) is marked and validated inside the block.
 void launch_small_batch(const DictView& d, const Batch& b, const FormatArgs& f, SmallBatchOut* out, cudaStream_t st);
