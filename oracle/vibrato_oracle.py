@@ -182,13 +182,16 @@ class OracleDictionary:
         return self._L.vo_dict_char_info(self._h, cp)
 
     def common_prefix(self, text, lex_type=0):
-        chars = np.array([ord(c) for c in text], dtype=np.uint32)
+        chars = np.frombuffer(text.encode("utf-32-le"), dtype=np.uint32)
         cap = 4096
-        ids = np.zeros(cap, dtype=np.uint32)
-        ends = np.zeros(cap, dtype=np.uint32)
-        n = self._L.vo_dict_common_prefix(self._h, lex_type, chars.ctypes.data, len(chars), ids.ctypes.data,
-                                        ends.ctypes.data, cap)
-        return [(int(ids[i]), int(ends[i])) for i in range(min(n, cap))]
+        while True:  # the C side returns the full hit count; a postings list may hold more than `cap`
+            ids = np.zeros(cap, dtype=np.uint32)
+            ends = np.zeros(cap, dtype=np.uint32)
+            n = self._L.vo_dict_common_prefix(self._h, lex_type, chars.ctypes.data, len(chars), ids.ctypes.data,
+                                            ends.ctypes.data, cap)
+            if n <= cap:
+                return [(int(ids[i]), int(ends[i])) for i in range(n)]
+            cap = n
 
     def worker(self, ignore_space=False, max_grouping_len=0):
         return OracleWorker(self, ignore_space, max_grouping_len)

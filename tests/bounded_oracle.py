@@ -69,9 +69,11 @@ class BoundedOracle:
             c = self._conn[(right, left)] = self.od.conn_cost(right, left)
         return c
 
-    def lattice(self, sent, bounds):
+    def lattice(self, sent, bounds, trace=None):
         """sent: bytes.  Returns (ends, eos, c2b): ends[i] = nodes ending at character i, a node being
-        [start_node, start_word, word_idx, left, right, min_idx, min_cost]."""
+        [start_node, start_word, word_idx, left, right, min_idx, min_cost, word_cost] (word_cost from the entry
+        itself: an unknown word's word_idx keeps only 16 bits of its entry, unknown.rs:133).  `trace` (a list) receives
+        (start_node, start_word, end, word_idx) for every inserted node, in insertion order."""
         text = sent.decode("utf-8")
         n = len(text)
         c2b = [0] * (n + 1)
@@ -84,7 +86,7 @@ class BoundedOracle:
         for i in range(n - 1, -1, -1):
             grp[i] = 1 if i == n - 1 or (ci[i] & ci[i + 1] & 0x3FFFF) == 0 else grp[i + 1] + 1
         ends = [[] for _ in range(n + 1)]
-        ends[0].append([0, 0, 0xFFFFFFFF, 0, 0, 0, 0])  # BOS
+        ends[0].append([0, 0, 0xFFFFFFFF, 0, 0, 0, 0, 0])  # BOS
 
         def lim(sw):
             for c in brk:
@@ -98,7 +100,9 @@ class BoundedOracle:
                 v = wrap(l[6] + self.conn(l[4], left))
                 if best is None or v <= best:
                     best, bi = v, i
-            ends[ew].append([start_node, sw, widx, left, right, bi, wrap(best + cost)])
+            ends[ew].append([start_node, sw, widx, left, right, bi, wrap(best + cost), cost])
+            if trace is not None:
+                trace.append((start_node, sw, ew, widx))
 
         start_node = start_word = 0
         while start_word < n:
@@ -160,15 +164,18 @@ class BoundedOracle:
         return wrap(ends[end_node][idx][6] + self.conn(ends[end_node][idx][4], 0))
 
     def tokenize(self, sent, bounds=()):
-        """Tokens of one sentence (bytes) as a TOKEN_DTYPE array."""
+        """Tokens of one sentence (bytes) as a TOKEN_DTYPE array.  The reference keeps the best predecessor's row
+        index as u16 (lattice.rs:144, EOS too), so in a row of more than 65 536 nodes the backtrack follows the
+        truncated index."""
         if not sent:
             return np.zeros(0, dtype=TOKEN_DTYPE)
         ends, (end_node, idx), c2b = self.lattice(sent, bounds)
+        idx &= 0xFFFF
         out = []
         while end_node != 0:
             nd = ends[end_node][idx]
             out.append((nd[1], end_node, c2b[nd[1]], c2b[end_node], nd[2], nd[6]))
-            end_node, idx = nd[0], nd[5]
+            end_node, idx = nd[0], nd[5] & 0xFFFF
         return np.array(out[::-1], dtype=TOKEN_DTYPE)
 
     def tokenize_batch(self, sentences, boundaries=None):

@@ -34,11 +34,11 @@ def sentence_lattice(bo, sent, bounds=(), theta=None):
         nd = ends[e][i]
         nodes[k] = (nd[1], e, c2b[nd[1]], c2b[e], nd[2], nd[6])
         links[k] = (-1 if nd[0] == 0 else index[(nd[0], nd[5] & 0xFFFF)], 0)
-    e, i = eos_row, eos_idx
+    e, i = eos_row, eos_idx & 0xFFFF  # the best path follows the u16 indices, as BoundedOracle.tokenize does
     while e != 0:
         links[index[(e, i)]]["flags"] = NODE_BEST
         nd = ends[e][i]
-        e, i = nd[0], nd[5]
+        e, i = nd[0], nd[5] & 0xFFFF
     probs = None
     if theta:
         lat = mo.Lattice(bo, sent, bounds)

@@ -43,7 +43,7 @@ class Lattice:
         if c is None:
             return self.bo.conn(right, 0)
         nd = self.node(c)
-        return self.bo.conn(right, nd[3]) + self.bo.param(nd[2])[2]
+        return self.bo.conn(right, nd[3]) + nd[7]  # the entry's cost, not that of the u16 word_idx
 
     def preds(self, c):
         s = self.node(c)[0]
@@ -52,11 +52,11 @@ class Lattice:
     def best_path(self):
         """The tokenizer's best path (wrapped i32 arithmetic, as the tokens follow it), BOS excluded, in order."""
         out = []
-        e, i = self.eos_row, self.best_idx
+        e, i = self.eos_row, self.best_idx & 0xFFFF  # u16 indices, as BoundedOracle.tokenize follows them
         while e != 0:
             out.append((e, i))
             nd = self.ends[e][i]
-            e, i = nd[0], nd[5]
+            e, i = nd[0], nd[5] & 0xFFFF
         return out[::-1]
 
 

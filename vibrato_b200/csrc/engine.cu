@@ -411,8 +411,9 @@ class EngineImpl final : public Engine {
             if (value < 0 || value > 0x7FFFFFFF) throw Error(kInvalidArgument, "chunk_sentences out of range");
             chunk_sentences_ = uint32_t(value);  // 0 disables the chunked host pipeline
         } else if (name == "pool_estimate_permille") {
-            // candidates expected per input byte (x 1000): the pool is sized from it and a batch that overflows
-            // the pool is re-run with the exact size.  Tests set it low to walk that path.
+            // candidates expected per input byte (x 1000): the pool of segments and the candidate rows are both
+            // sized from it (the larger of the two counts is learned), and a batch that overflows either is re-run
+            // with the exact size.  Tests set it low to walk that path.
             if (value < 1 || value > 1000000) throw Error(kInvalidArgument, "pool_estimate_permille out of range");
             cand_per_byte_ = double(value) / 1000.0;
         } else if (name == "chars_estimate_permille") {
@@ -1292,7 +1293,9 @@ class EngineImpl final : public Engine {
         w.ends_cnt.ensure(ms * 4);
         w.ends_meta.ensure(ms * 8);
         w.bnd_dist.ensure(ms * 4);
-        w.seg.ensure(size_t(kSmallCands) * 8);  // a position has at least as many candidates as segments
+        // Segments outnumber candidates only through move segments (an end slot more than 32 767 away); 16 KiB of
+        // text keeps every move shorter, so each segment holds a candidate here.
+        w.seg.ensure(size_t(kSmallCands) * 8);
         w.ends_hot.ensure((kSmallCands + ns) * 8);
         w.ends_cold.ensure((kSmallCands + ns) * 16);
         const size_t in_cap = ns * 8 + kEagerBytes + 8 + ns * 8 + kSmallBounds * 4;  // [off | utf8 | bnd_off | bnd]
@@ -1548,7 +1551,7 @@ class EngineImpl final : public Engine {
         if (counting_) w.stats.ensure(ms * 16, 1.25);
         size_t want_cand = std::max<size_t>(1 << 16, size_t(double(n_bytes) * cand_per_byte_) + 4096);
         want_cand = std::min<size_t>(want_cand, 0xFFFFFFF0ull);
-        w.seg.ensure(want_cand * 8);  // sized like the candidates: a source has one or more of them
+        w.seg.ensure(want_cand * 8);  // sized like the candidates; move segments can outnumber them (overflow retry)
         w.ends_hot.ensure((want_cand + ns) * 8);
         w.ends_cold.ensure((want_cand + ns) * 16);
         if (theta_ > 0) {
