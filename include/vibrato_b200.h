@@ -369,6 +369,36 @@ int32_t vbt_result_lattice(const vbt_result *r, const uint64_t **node_offsets, c
  * marginals), valid until the next call; VBT_ERR_INVALID_ARGUMENT when it ran without the lattice. */
 int32_t vbt_last_device_lattice(const vbt_tokenizer *t, uint64_t *d_node_offsets, uint64_t *d_nodes, uint64_t *d_links,
                                 uint64_t *d_node_prob, uint64_t *n_nodes);
+/* Segmentation sampling ("subword regularisation"): n paths per sentence drawn independently, with replacement, from
+ * P(path) = exp(-theta * cost(path)) / Z over the lattice, edges and exact int64 path costs of the marginals above.
+ * Forward-filtering backward-sampling on the device: a walk starts at EOS and repeats until BOS.  At the current
+ * node c (EOS: left id 0, word cost 0) the candidates are the entries k = 0..K-1 of the row c starts at, in row
+ * order: x_k = R(k) + conn(right(k), left(c)) + wcost(c) (R the exact least cost from BOS), r = min x_k,
+ * t_k = a(k) - theta * (x_k - r) (a the forward log weight of the marginals), m = max t_k, w_k = exp(t_k - m).  The
+ * walk takes the first k whose running sum w_0 + ... + w_k (float64, in row order) exceeds u * S, S the whole sum,
+ * and the last k with w_k > 0 if rounding leaves none.  u = ((x0 >> 5) * 2^26 + (x1 >> 6)) * 2^-53 from the first
+ * two words of Philox4x32-10 (standard constants) at counter (t, j, i, 0) and key (seed & 0xFFFFFFFF, seed >> 32):
+ * t the draw step (0 at EOS), j the sample, i the sentence's index in the call.  Routes (chunking, devices, the
+ * sentence order) do not change i, so the same call with the same seed gives the same bytes everywhere; callers who
+ * split a corpus over several calls vary the seed per call.
+ *   Records: each sampled token is a 24-byte vbt_token record, also under "compact_tokens"; start_char, bytes, word_idx
+ *   as for tokens, total_cost the sampled path's prefix cost through the token in the tokenizer's wrapping i32
+ *   arithmetic.  A sample whose nodes are the best path's has records byte-identical to the sentence's tokens.
+ *   An empty sentence, or one without a path, gets n empty samples; nodes without a path to EOS are never sampled.
+ * n = 1..1024 switches it on and 0 off; theta must be > 0 and finite; a call with n_sent * n >= 2^32 fails.
+ * Marginals and sampling share one forward pass: setting either while the other is on with a different theta is
+ * VBT_ERR_INVALID_ARGUMENT.  Tokens, marginals, the lattice and the output text do not change.  While on, batches
+ * take three more kernel launches and a scan (the forward pass alone when marginals are off; booked under
+ * "viterbi") with one host wait for the sample total, and "small_batch" steps aside. */
+int32_t vbt_tokenizer_set_sampling(vbt_tokenizer *t, uint32_t n, double theta, uint64_t seed);
+/* sample_offsets[n_sent * n + 1] into samples: sample j of sentence i is samples[sample_offsets[i * n + j] ..
+ * sample_offsets[i * n + j + 1]); owned by the result.  VBT_ERR_INVALID_ARGUMENT for a result made without sampling. */
+int32_t vbt_result_samples(const vbt_result *r, const uint64_t **sample_offsets, const vbt_token **samples,
+                           uint64_t *n_sample_tokens);
+/* Device addresses of the samples of the last vbt_tokenize_batch_device{,_bounded} call, valid until the next call;
+ * VBT_ERR_INVALID_ARGUMENT when it ran without sampling. */
+int32_t vbt_last_device_samples(const vbt_tokenizer *t, uint64_t *d_sample_offsets, uint64_t *d_samples,
+                                uint64_t *n_sample_tokens);
 /* Launch the kernels on a caller-owned CUDA stream (a cudaStream_t passed as an integer; 0 restores
  * the tokenizer's own stream), so callers can bracket batches with their own events. */
 int32_t vbt_tokenizer_set_stream(vbt_tokenizer *t, uint64_t stream);

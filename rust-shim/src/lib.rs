@@ -61,6 +61,9 @@ extern "C" {
     fn vbt_result_text(r: *const vbt_result, text_offsets: *mut *const u64, text: *mut *const c_char,
                        n_bytes: *mut u64) -> i32;
     fn vbt_tokenizer_set_marginals(t: *mut vbt_tokenizer, theta: f64) -> i32;
+    fn vbt_tokenizer_set_sampling(t: *mut vbt_tokenizer, n: u32, theta: f64, seed: u64) -> i32;
+    fn vbt_result_samples(r: *const vbt_result, sample_offsets: *mut *const u64, samples: *mut *const vbt_token,
+                          n_sample_tokens: *mut u64) -> i32;
     fn vbt_result_marginals(r: *const vbt_result, token_prob: *mut *const f32, path_prob: *mut *const f32) -> i32;
     fn vbt_result_lattice(r: *const vbt_result, node_offsets: *mut *const u64, nodes: *mut *const vbt_token,
                           links: *mut *const vbt_lattice_link, node_prob: *mut *const f32, n_nodes: *mut u64) -> i32;
@@ -194,10 +197,11 @@ pub mod mecab {
 pub enum OutputMode { Mecab = 1, Wakati = 2, Detail = 3 }
 
 pub struct Tokenizer { dict: Dictionary, ignore_space: bool, max_grouping_len: usize, devices: Vec<i32>,
-                       h: std::cell::OnceCell<*mut vbt_tokenizer> }
+                       h: std::cell::OnceCell<*mut vbt_tokenizer>, samples: std::cell::Cell<u32> }
 impl Tokenizer {
     pub fn new(dict: Dictionary) -> Self {                                // tokenizer.rs:26
-        Self { dict, ignore_space: false, max_grouping_len: 0, devices: vec![], h: Default::default() }
+        Self { dict, ignore_space: false, max_grouping_len: 0, devices: vec![], h: Default::default(),
+               samples: Default::default() }
     }
     /// Not in the reference (a vibrato Worker is one CPU thread): spread every batch over these GPUs of the node.
     /// The dictionary image is uploaded once and broadcast over NVLink; `tokenize_batch` still returns one result
@@ -265,6 +269,13 @@ impl Tokenizer {
         let v = if !on { 0 } else if text { 2 } else { 1 };
         check(unsafe { vbt_tokenizer_set_option(self.handle(), b"lattice\0".as_ptr() as *const c_char, v) })
     }
+    /// Segmentation sampling (see `vbt_tokenizer_set_sampling`): `n` (1..1024, 0 = off) paths per sentence drawn from
+    /// P(path) at temperature `theta`, keyed by `seed`; batches tokenised afterwards carry `BatchResult::samples`.
+    pub fn sampling(&self, n: u32, theta: f64, seed: u64) -> Result<()> {
+        check(unsafe { vbt_tokenizer_set_sampling(self.handle(), n, theta, seed) })?;
+        self.samples.set(n);
+        Ok(())
+    }
     /// The loop of the `evaluate` tool (evaluate/src/main.rs:61-138): (num_ref, num_sys, num_cor).
     pub fn evaluate(&self, corpus: &str, feature_indices: &[usize]) -> Result<(u64, u64, u64)> {
         let idx: Vec<u64> = feature_indices.iter().map(|&i| i as u64).collect();
@@ -281,11 +292,11 @@ impl Tokenizer {
         let mut r = std::ptr::null_mut();
         check(unsafe { vbt_tokenize_batch(self.handle(), utf8.as_ptr() as *const c_char, off.as_ptr(),
                                           lines.len() as u64, &mut r) })?;
-        Ok(BatchResult { r })
+        Ok(BatchResult { r, n_samples: self.samples.get() })
     }
 }
 
-pub struct BatchResult { r: *mut vbt_result }
+pub struct BatchResult { r: *mut vbt_result, n_samples: u32 }
 impl Drop for BatchResult { fn drop(&mut self) { unsafe { vbt_result_free(self.r) } } }
 impl BatchResult {
     /// What `tokenize` writes for the batch; sentence i is `text[offsets[i]..offsets[i + 1]]`.
@@ -325,6 +336,18 @@ impl BatchResult {
             Ok((std::slice::from_raw_parts(o, ns as usize + 1), nodes, links, probs))
         }
     }
+    /// (sample offsets, sampled tokens): sample j of sentence i is `samples[offsets[i * n + j]..offsets[i * n + j + 1]]`;
+    /// an error for a batch tokenised without sampling.
+    pub fn samples(&self) -> Result<(&[u64], &[vbt_token])> {
+        let (mut o, mut st, mut nst) = (std::ptr::null(), std::ptr::null(), 0u64);
+        check(unsafe { vbt_result_samples(self.r, &mut o, &mut st, &mut nst) })?;
+        let (mut to, mut t, mut ns, mut nt) = (std::ptr::null(), std::ptr::null(), 0u64, 0u64);
+        unsafe {
+            vbt_result_view(self.r, &mut to, &mut t, &mut ns, &mut nt);
+            let recs: &[vbt_token] = if nst == 0 { &[] } else { std::slice::from_raw_parts(st, nst as usize) };
+            Ok((std::slice::from_raw_parts(o, ns as usize * self.n_samples as usize + 1), recs))
+        }
+    }
     pub fn view(&self) -> (&[u64], &[vbt_token]) {
         let (mut o, mut t, mut ns, mut nt) = (std::ptr::null(), std::ptr::null(), 0u64, 0u64);
         unsafe {
@@ -346,7 +369,7 @@ impl<'t> Worker<'t> {
         let rc = unsafe { vbt_tokenize_batch(self.t.handle(), self.sent.as_ptr() as *const c_char,
                                              off.as_ptr(), 1, &mut r) };
         check(rc).expect("vibrato_b200 device error");
-        let b = BatchResult { r };
+        let b = BatchResult { r, n_samples: 0 };
         self.toks = b.view().1.to_vec();
     }
     pub fn num_tokens(&self) -> usize { self.toks.len() }                   // worker.rs:59

@@ -279,9 +279,12 @@ class BatchResult:
     and `path_probs` (float32[n_sent]) hold the marginal of every token and the probability of each sentence's best
     path; both are None otherwise.  With Tokenizer.lattice() on, `node_offsets[i]..node_offsets[i+1]` index `nodes`
     (TOKEN_DTYPE), `node_links` (LINK_DTYPE) and `node_probs` (float32, None without marginals): every node of sentence
-    i's lattice (include/vibrato_b200.h); all four are None otherwise."""
+    i's lattice (include/vibrato_b200.h); all four are None otherwise.  With Tokenizer.sampling(n, theta) on,
+    `sample_offsets[i * n + j]..sample_offsets[i * n + j + 1]` index `samples` (TOKEN_DTYPE): sample j of sentence i
+    (sentence_samples()); both are None otherwise."""
 
-    def __init__(self, tokenizer, handle, sentences_utf8, byte_offsets, compact=False, marginals=False, lattice=False):
+    def __init__(self, tokenizer, handle, sentences_utf8, byte_offsets, compact=False, marginals=False, lattice=False,
+                 samples=0):
         self._tok = tokenizer
         self._h = handle
         self._free = lib().vbt_result_free
@@ -321,6 +324,16 @@ class BatchResult:
             if pp.value:
                 self.node_probs = (np.ctypeslib.as_array(C.cast(pp, C.POINTER(C.c_float)), shape=(n,)) if n
                                    else np.empty(0, dtype=np.float32))
+        self.n_samples = int(samples)  # samples per sentence, 0 without sampling
+        self.sample_offsets = self.samples = None
+        if samples:
+            po, ps, nn = C.c_void_p(), C.c_void_p(), C.c_uint64()
+            check(lib().vbt_result_samples(handle, C.byref(po), C.byref(ps), C.byref(nn)))
+            n = nn.value
+            self.sample_offsets = np.ctypeslib.as_array(C.cast(po, C.POINTER(C.c_uint64)),
+                                                        shape=(self.n_sent * self.n_samples + 1,))
+            self.samples = (np.ctypeslib.as_array(C.cast(ps, C.POINTER(C.c_uint8)), shape=(n * TOKEN_DTYPE.itemsize,))
+                            .view(TOKEN_DTYPE) if n else np.empty(0, dtype=TOKEN_DTYPE))
         self._utf8 = sentences_utf8
         self._off = byte_offsets
 
@@ -334,7 +347,7 @@ class BatchResult:
             if self.token_probs is not None:
                 self.token_probs = self.token_probs.copy()
                 self.path_probs = self.path_probs.copy()
-            for name in ("node_offsets", "nodes", "node_links", "node_probs"):
+            for name in ("node_offsets", "nodes", "node_links", "node_probs", "sample_offsets", "samples"):
                 if getattr(self, name) is not None:
                     setattr(self, name, getattr(self, name).copy())
             self._free(h)
@@ -368,6 +381,16 @@ class BatchResult:
     def num_nodes(self, i):
         return int(self.node_offsets[i + 1] - self.node_offsets[i])
 
+    def sentence_samples(self, i):
+        """The n sampled segmentations of sentence i (Tokenizer.sampling), each a list of Token views; Token.prob()
+        raises on them."""
+        if self.samples is None:
+            raise VibratoError(1, "no samples: switch sampling on with Tokenizer.sampling() before tokenising")
+        s = bytes(self._utf8[int(self._off[i]):int(self._off[i + 1])])
+        n, so = self.n_samples, self.sample_offsets
+        return [[Token(self._tok, s, self.samples[k]) for k in range(int(so[i * n + j]), int(so[i * n + j + 1]))]
+                for j in range(n)]
+
     def sentence_nodes(self, i):
         """LatticeNode views of sentence i's lattice, in node order (needs Tokenizer.lattice())."""
         if self.nodes is None:
@@ -396,6 +419,7 @@ class Tokenizer:
         self._format = None  # (node, unk, bos, eos) of output_format(), replayed after the options
         self._theta = 0.0  # marginals(), replayed before the format
         self._lattice = 0  # lattice(), replayed before the format
+        self._sampling = (0, 0.0, 0)  # sampling() as (n, theta, seed), replayed after the marginals
         self._stream = 0
         self._counting = False
         self._free = lib().vbt_tokenizer_free
@@ -459,6 +483,8 @@ class Tokenizer:
                 check(lib().vbt_tokenizer_set_marginals(h, self._theta))
             if self._lattice:
                 check(lib().vbt_tokenizer_set_option(h, b"lattice", self._lattice))
+            if self._sampling[0]:
+                check(lib().vbt_tokenizer_set_sampling(h, *self._sampling))
             if self._format is not None:
                 self._set_format(h, self._format)
             if self._counting:
@@ -509,7 +535,7 @@ class Tokenizer:
                                                    byte_offsets.ctypes.data, n, bnd_offsets.ctypes.data,
                                                    bnd.ctypes.data if bnd.size else None, C.byref(h)))
         return BatchResult(self, h, utf8, byte_offsets, compact=bool(self._options.get("compact_tokens", 0)),
-                           marginals=self._theta > 0, lattice=self._lattice > 0)
+                           marginals=self._theta > 0, lattice=self._lattice > 0, samples=self._sampling[0])
 
     def tokenize_batch_device(self, d_utf8, d_byte_offsets, n_sent, n_bytes, d_bnd_offsets=None, d_bnd=None, n_bnd=0):
         """Device-resident variant: addresses in, (d_tok_offsets, d_tokens, n_tokens) out.  With d_bnd_offsets
@@ -539,6 +565,30 @@ class Tokenizer:
         v = [C.c_uint64() for _ in range(5)]
         check(lib().vbt_last_device_lattice(self.handle(), *[C.byref(x) for x in v]))
         return tuple(x.value for x in v)
+
+    def last_device_samples(self):
+        """-> (d_sample_offsets, d_samples, n_sample_tokens): device addresses (uint64[n_sent * n + 1],
+        vbt_token[n_sample_tokens]) of the samples of the last tokenize_batch_device call, valid until the next call."""
+        v = [C.c_uint64() for _ in range(3)]
+        check(lib().vbt_last_device_samples(self.handle(), *[C.byref(x) for x in v]))
+        return tuple(x.value for x in v)
+
+    def sampling(self, n, theta=1.0, seed=0):
+        """Segmentation sampling ("subword regularisation"): every result then carries n segmentations per sentence
+        drawn with replacement from P(path) = exp(-theta * cost(path)) / Z, the distribution of marginals()
+        (BatchResult.samples / sample_offsets, sentence_samples()).  theta > 0 and finite; with marginals on it must be
+        theirs.  seed (u64) keys the draws, which depend only on (seed, sentence index in the call, sample, step):
+        vary it per call when a corpus is split over calls.  n = 0 (or None) switches sampling off.  The tokens do not
+        change; the "small_batch" route steps aside.  Definition: include/vibrato_b200.h."""
+        n = 0 if n is None else int(n)
+        theta, seed = float(theta), int(seed)
+        if not 0 <= seed < 2 ** 64:
+            raise VibratoError(1, "sampling: seed must be an unsigned 64-bit integer")
+        if not 0 <= n < 2 ** 32:
+            raise VibratoError(1, "sampling: n must be between 0 (off) and 1024")
+        check(lib().vbt_tokenizer_set_sampling(self.handle(), n, theta, seed))
+        self._sampling = (n, theta, seed) if n else (0, 0.0, 0)
+        return self
 
     def lattice(self, on=True, text=False):
         """Lattice output: results then carry every node of each sentence's lattice (BatchResult.nodes /
@@ -768,6 +818,7 @@ class Worker:
         self._bounds = None
         self._tokens = []
         self._nodes = []
+        self._samples = []
 
     def reset_sentence(self, text, boundaries=None):
         """boundaries: required token boundaries, byte offsets into the sentence (see Tokenizer.tokenize_batch)."""
@@ -775,9 +826,11 @@ class Worker:
         self._bounds = None if boundaries is None else list(boundaries)
         self._tokens = []
         self._nodes = []
+        self._samples = []
 
     def tokenize(self):
         if not self._sent:  # worker.rs:50-52
+            self._samples = [[] for _ in range(self._tok._sampling[0])]
             return
         res = self._tok.tokenize_batch([self._sent], boundaries=None if self._bounds is None else [self._bounds])
         tp = res.token_probs
@@ -786,6 +839,10 @@ class Worker:
         self._nodes = res.sentence_nodes(0) if res.nodes is not None else []
         for nd in self._nodes:
             nd._r, nd._link = nd._r.copy(), nd._link.copy()
+        self._samples = res.sentence_samples(0) if res.samples is not None else []
+        for sample in self._samples:
+            for t in sample:
+                t._r = t._r.copy()
         res.close()
 
     def num_tokens(self):
@@ -806,3 +863,9 @@ class Worker:
 
     def node_iter(self):
         return iter(self._nodes)
+
+    def sample_tokens(self, j):
+        """The tokens of sample j of the sentence (Tokenizer.sampling())."""
+        if not self._tok._sampling[0]:
+            raise VibratoError(1, "no samples: switch sampling on with Tokenizer.sampling() before tokenising")
+        return self._samples[j]

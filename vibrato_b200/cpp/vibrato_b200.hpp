@@ -177,6 +177,19 @@ class BatchResult {
         check(vbt_result_lattice(r_.get(), &l.node_offsets, &l.nodes, &l.links, &l.node_probs, &l.n_nodes));
         return l;
     }
+    // Segmentation sampling (Tokenizer::sampling before the batch, see vbt_tokenizer_set_sampling): sample j of
+    // sentence i is samples[sample_offsets[i * n + j] .. sample_offsets[i * n + j + 1]).  Throws on a result made
+    // without sampling.
+    struct Samples {
+        const uint64_t* sample_offsets = nullptr;
+        const vbt_token* samples = nullptr;
+        uint64_t n_sample_tokens = 0;
+    };
+    Samples samples() const {
+        Samples s;
+        check(vbt_result_samples(r_.get(), &s.sample_offsets, &s.samples, &s.n_sample_tokens));
+        return s;
+    }
 
    private:
     std::unique_ptr<vbt_result, void (*)(vbt_result*)> r_;
@@ -284,6 +297,23 @@ class Tokenizer {
         check(vbt_last_device_lattice(handle(), &d.node_offsets, &d.nodes, &d.links, &d.node_probs, &d.n_nodes));
         return d;
     }
+    // Segmentation sampling (see vbt_tokenizer_set_sampling): n (1..1024, 0 = off) paths per sentence drawn from
+    // P(path) at temperature theta, keyed by seed: BatchResult::samples().  theta must equal the marginals' when both
+    // are on.
+    void sampling(uint32_t n, double theta, uint64_t seed = 0) const {
+        check(vbt_tokenizer_set_sampling(handle(), n, theta, seed));
+        samples_ = n;
+    }
+    uint32_t samples_per_sentence() const { return samples_; }
+    // Device addresses of the last tokenize_batch_device call's samples.
+    struct DeviceSamples {
+        uint64_t sample_offsets = 0, samples = 0, n_sample_tokens = 0;
+    };
+    DeviceSamples last_device_samples() const {
+        DeviceSamples d;
+        check(vbt_last_device_samples(handle(), &d.sample_offsets, &d.samples, &d.n_sample_tokens));
+        return d;
+    }
     // Worker::init_connid_counter / update_connid_counts / compute_connid_probs (worker.rs:77-103): after
     // init_connid_counter() every batch is counted, an empty sentence counting nothing
     void init_connid_counter() const { check(vbt_tokenizer_set_option(handle(), "connid_counting", 1)); }
@@ -340,6 +370,7 @@ class Tokenizer {
     uint64_t max_grouping_len_ = 0;
     mutable bool marginals_ = false;
     mutable bool lattice_ = false;
+    mutable uint32_t samples_ = 0;
     mutable std::shared_ptr<vbt_tokenizer> h_;
 };
 
@@ -405,6 +436,7 @@ class Worker {  // worker.rs:13-74
         nodes_.clear();
         links_.clear();
         nprobs_.clear();
+        samples_.clear();
     }
     // With required boundaries (byte offsets into s; see Tokenizer::tokenize_batch).
     void reset_sentence(std::string_view s, std::vector<uint32_t> boundaries) {
@@ -413,6 +445,7 @@ class Worker {  // worker.rs:13-74
         bounded_ = true;
     }
     void tokenize() {
+        samples_.assign(t_->samples_per_sentence(), {});
         if (sent_.empty()) return;  // worker.rs:50-52
         uint64_t off[2] = {0, sent_.size()};
         uint64_t boff[2] = {0, bnd_.size()};
@@ -430,7 +463,14 @@ class Worker {  // worker.rs:13-74
             links_.assign(l.links, l.links + l.n_nodes);
             if (l.node_probs) nprobs_.assign(l.node_probs, l.node_probs + l.n_nodes);
         }
+        if (!samples_.empty()) {
+            const BatchResult::Samples s = r.samples();
+            for (size_t j = 0; j < samples_.size(); ++j) samples_[j].assign(s.samples + s.sample_offsets[j], s.samples + s.sample_offsets[j + 1]);
+        }
     }
+    // Tokenizer::sampling: the tokens of sample j of the sentence (Token::prob() throws on them).
+    size_t num_sample_tokens(size_t j) const { return samples_.at(j).size(); }
+    Token sample_token(size_t j, size_t i) const { return Token(t_, sent_, samples_.at(j)[i]); }
     size_t num_nodes() const { return nodes_.size(); }
     LatticeNode node(size_t i) const {
         return nprobs_.empty() ? LatticeNode(t_, sent_, nodes_[i], links_[i]) : LatticeNode(t_, sent_, nodes_[i], links_[i], nprobs_[i]);
@@ -450,6 +490,7 @@ class Worker {  // worker.rs:13-74
     std::vector<vbt_token> nodes_;  // Tokenizer::lattice
     std::vector<vbt_lattice_link> links_;
     std::vector<float> nprobs_;
+    std::vector<std::vector<vbt_token>> samples_;  // Tokenizer::sampling
 };
 
 inline Worker Tokenizer::new_worker() const { return Worker(this); }

@@ -616,6 +616,33 @@ int32_t vbt_last_device_lattice(const vbt_tokenizer* t, uint64_t* d_node_offsets
     });
 }
 
+int32_t vbt_tokenizer_set_sampling(vbt_tokenizer* t, uint32_t n, double theta, uint64_t seed) {
+    return guarded([&] {
+        need(t, "t");
+        t->e->set_sampling(n, theta, seed);
+    });
+}
+
+int32_t vbt_result_samples(const vbt_result* r, const uint64_t** sample_offsets, const vbt_token** samples,
+                           uint64_t* n_sample_tokens) {
+    return guarded([&] {
+        need(r, "r");
+        if (!r->r->has_samp)
+            throw vbt::Error(vbt::kInvalidArgument, "no samples: switch sampling on with vbt_tokenizer_set_sampling before tokenising");
+        if (sample_offsets) *sample_offsets = r->r->sample_off;
+        if (samples) *samples = static_cast<const vbt_token*>(r->r->samples);
+        if (n_sample_tokens) *n_sample_tokens = r->r->n_sample_tokens;
+    });
+}
+
+int32_t vbt_last_device_samples(const vbt_tokenizer* t, uint64_t* d_sample_offsets, uint64_t* d_samples,
+                                uint64_t* n_sample_tokens) {
+    return guarded([&] {
+        need(t, "t");
+        t->e->device_samples(d_sample_offsets, d_samples, n_sample_tokens);
+    });
+}
+
 int32_t vbt_tokenizer_set_stream(vbt_tokenizer* t, uint64_t stream) {
     return guarded([&] {
         need(t, "t");

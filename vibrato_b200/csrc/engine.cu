@@ -8,6 +8,8 @@
 #include <algorithm>
 #include <cmath>
 #include <iterator>
+#include <cstdio>
+#include <cstdlib>
 #include <cstring>
 #include <string>
 
@@ -59,6 +61,7 @@ struct Control {  // one small block zeroed per batch and read back once
     unsigned long long counters[kNumCounters];
     unsigned long long text_bytes;  // output stage: the text total of the batch (or chunk)
     unsigned long long n_nodes;     // lattice output: the node total of the batch (or chunk)
+    unsigned long long n_samples;   // sampling: the sample-token total of the batch (or chunk)
     uint32_t flags;
     uint32_t total_slots;
 };
@@ -87,6 +90,16 @@ struct RowMetaOut {
     __host__ __device__ Ref operator*() const { return Ref{p}; }
     __host__ __device__ RowMetaOut operator+(difference_type i) const { return RowMetaOut{p + i}; }
 };
+
+// A theta as an error message prints it: the shortest form that reads back as the same double.
+static std::string num(double v) {
+    char buf[32];
+    for (int prec = 1; prec <= 17; ++prec) {
+        std::snprintf(buf, sizeof buf, "%.*g", prec, v);
+        if (std::strtod(buf, nullptr) == v) break;
+    }
+    return buf;
+}
 
 struct CastU64 {
     __host__ __device__ unsigned long long operator()(uint32_t v) const { return v; }
@@ -155,12 +168,13 @@ struct Workspace {  // every per-(chunk of a)-batch device array; two of them le
     DevBuf bnd_dist;  // bounded batches only: Batch::bnd_dist
     DevBuf m_fill, m_ncand, m_cand_entry, m_R, m_ab, m_r_eos, m_a_eos;  // marginals only: MargArgs
     DevBuf l_row_base, l_n_nodes;  // lattice output only: LatticeArgs
+    DevBuf m_lw, s_cnt, s_total;   // sampling only: MargArgs::lw, SampleArgs::cnt / total
     cudaStream_t stream = nullptr;
     void release() {
         for (DevBuf* b : {&n_slots, &slot_off, &eos, &n_tok, &code_sys, &code_usr, &cinfo, &groupable, &byte_pos, &info,
                           &info_ex, &ends_cnt, &ends_meta, &seg, &ends_hot, &ends_cold, &scan_tmp, &stats, &iota,
                           &sort_keys, &order, &bnd_dist, &m_fill, &m_ncand, &m_cand_entry, &m_R, &m_ab, &m_r_eos, &m_a_eos,
-                          &l_row_base, &l_n_nodes})
+                          &l_row_base, &l_n_nodes, &m_lw, &s_cnt, &s_total})
             b->release();
     }
 };
@@ -180,6 +194,8 @@ struct OutSlot {  // where one (chunk of a) batch leaves its results; two of the
     bool marg = false;                // the (chunk of a) batch in this slot was run with marginals
     DevBuf node_off, nodes, links, node_prob;  // lattice output (LatticeArgs)
     bool lat = false;                          // the (chunk of a) batch in this slot was run with the lattice
+    DevBuf sample_off, samples;                // sampling (SampleArgs)
+    bool samp = false;                         // the (chunk of a) batch in this slot was run with sampling
     Control* h_ctrl = nullptr;
     cudaEvent_t ev[kNumStages + 1];
     cudaEvent_t done = nullptr, drained = nullptr;
@@ -215,6 +231,7 @@ class EngineImpl final : public Engine {
         tok_base_.ensure(8);
         text_base_.ensure(8);
         node_base_.ensure(8);
+        samp_base_.ensure(8);
         BlobHeader h;
         if (host_blob) {
             if (n_bytes < sizeof(BlobHeader)) throw Error(kInvalidArgument, "dictionary image too small");
@@ -333,7 +350,7 @@ class EngineImpl final : public Engine {
         cudaStreamSynchronize(out_stream_);
         for (auto& o : out_) {
             for (DevBuf* b : {&o.tok_off, &o.tokens, &o.ctrl, &o.sent_len, &o.text_off, &o.text, &o.token_prob, &o.path_prob,
-                              &o.node_off, &o.nodes, &o.links, &o.node_prob})
+                              &o.node_off, &o.nodes, &o.links, &o.node_prob, &o.sample_off, &o.samples})
                 b->release();
             pinned_free(o.h_ctrl);
             for (auto& ev : o.ev) cudaEventDestroy(ev);
@@ -350,6 +367,7 @@ class EngineImpl final : public Engine {
         tok_base_.release();
         text_base_.release();
         node_base_.release();
+        samp_base_.release();
         for (DevBuf* b : {&fmt_prog_, &ft_keep_, &ft_off_, &ft_bytes_}) b->release();
         for (auto* b : {&blob_own_, &in_utf8_, &in_off_, &in_bnd_off_, &in_bnd_, &connid_, &connid_try_}) b->release();
         for (auto& w : ws_) w.release();
@@ -370,6 +388,8 @@ class EngineImpl final : public Engine {
             pinned_free(r->token_prob);
             pinned_free(r->path_prob);
             for (void* p : {static_cast<void*>(r->node_off), r->nodes, r->links, static_cast<void*>(r->node_prob)}) pinned_free(p);
+            pinned_free(r->sample_off);
+            pinned_free(r->samples);
             delete r;
         }
         cudaStreamDestroy(own_stream_);
@@ -474,8 +494,30 @@ class EngineImpl final : public Engine {
             throw Error(kInvalidArgument, "the marginals' theta must be a finite number >= 0 (0 switches them off)");
         if (theta == 0 && output_mode_ == kOutFormat && (fmt_uses_ & kUsesProb))
             throw Error(kInvalidArgument, "the output format prints %pP: change the format before switching marginals off");
+        if (theta > 0 && samp_n_ && theta != samp_theta_)
+            throw Error(kInvalidArgument, "marginals and sampling share one forward pass: the marginals' theta " + num(theta) +
+                                              " differs from the sampling theta " + num(samp_theta_));
         cudaStreamSynchronize(stream_);
         theta_ = theta;
+    }
+    void set_sampling(uint32_t n, double theta, uint64_t seed) override {
+        if (n > kMaxSamples) throw Error(kInvalidArgument, "sampling: n must be between 0 (off) and 1024");
+        if (n && (!(theta > 0) || !std::isfinite(theta)))
+            throw Error(kInvalidArgument, "sampling: theta must be a finite number > 0");
+        if (n && theta_ > 0 && theta != theta_)
+            throw Error(kInvalidArgument, "marginals and sampling share one forward pass: the sampling theta " + num(theta) +
+                                              " differs from the marginals' theta " + num(theta_));
+        cudaStreamSynchronize(stream_);
+        samp_n_ = n;
+        samp_theta_ = n ? theta : 0.0;
+        samp_seed_ = seed;
+    }
+    uint32_t sampling() const override { return samp_n_; }
+    void device_samples(uint64_t* d_sample_off, uint64_t* d_samples, uint64_t* n_tokens) const override {
+        if (!dev_samp_) throw Error(kInvalidArgument, "the last device-resident call ran without sampling");
+        if (d_sample_off) *d_sample_off = reinterpret_cast<uint64_t>(out_[0].sample_off.p);
+        if (d_samples) *d_samples = reinterpret_cast<uint64_t>(out_[0].samples.p);
+        if (n_tokens) *n_tokens = out_[0].h_ctrl->n_samples;
     }
     double marginals() const override { return theta_; }
     int lattice() const override { return lattice_; }
@@ -521,7 +563,7 @@ class EngineImpl final : public Engine {
         if (bnd && bnd->n == 0 && device_offsets_zero(bnd->off, n_sent)) bnd = nullptr;  // no boundary at all
         DevBounds bd;
         if (bnd) bd = DevBounds{reinterpret_cast<const unsigned long long*>(bnd->off), bnd->bnd, bnd->n};
-        dev_marg_ = dev_lat_ = false;
+        dev_marg_ = dev_lat_ = dev_samp_ = false;
         run_whole(reinterpret_cast<const uint8_t*>(d_utf8), reinterpret_cast<const unsigned long long*>(d_byte_off),
                   uint32_t(n_sent), n_bytes, bd);
         *d_tok_off = reinterpret_cast<uint64_t>(out_[0].tok_off.p);
@@ -529,6 +571,7 @@ class EngineImpl final : public Engine {
         *n_tokens = out_[0].h_ctrl->n_tokens;
         dev_marg_ = out_[0].marg;
         dev_lat_ = out_[0].lat;
+        dev_samp_ = out_[0].samp;
     }
 
     // Host path.  Large batches are cut into chunks that flow through three streams: the H2D copy of
@@ -558,8 +601,9 @@ class EngineImpl final : public Engine {
         const uint32_t chunk = chunk_sentences_;
         const bool chunked = chunk > 0 && n_sent > chunk + chunk / 2;
         const bool fmt = output_mode_ != kOutNone;
-        // k_small_batch computes no marginals and no lattice: with either on, small batches take the usual route
+        // k_small_batch computes no marginals, no lattice and no samples: with any on, small batches take the usual route
         if (small_batch_ && n_sent <= small_batch_ && !chunked && n_bytes <= kEagerBytes && !counting_ && !connid_on_ && theta_ == 0 && !lattice_ &&
+            !samp_n_ &&
             (!bnd || small_bounds_fit(*bnd, n_sent))) {
             if (HostResult* r = run_small(utf8 + first, off, n_sent, n_bytes, bnd)) return r;
             // the batch outgrew the scratch of k_small_batch: it runs again on the route below
@@ -569,7 +613,7 @@ class EngineImpl final : public Engine {
             if (!chunked) {
                 h2d(in_off_.p, off, (size_t(n_sent) + 1) * 8, stream_, off_pinned && off == byte_off);
                 h2d(in_utf8_.p, utf8 + first, n_bytes, stream_, utf8_pinned);
-                if (n_bytes <= kEagerBytes && output_mode_ == kOutNone && !lattice_) {
+                if (n_bytes <= kEagerBytes && output_mode_ == kOutNone && !lattice_ && !samp_n_) {
                     // Small batches (a per-sentence Worker loop ends up here) are all latency: the result copies are
                     // queued behind the kernels with an upper bound for the token count (a token spans >= 1 byte), so
                     // that the call makes ONE host synchronisation instead of two.
@@ -601,6 +645,11 @@ class EngineImpl final : public Engine {
                     r->n_nodes = o.h_ctrl->n_nodes;
                     ensure_lat_host(r, n_sent, r->n_nodes);
                     copy_lattice(o, r, 0, 0, n_sent, true, stream_);
+                }
+                if (r->has_samp) {
+                    r->n_sample_tokens = o.h_ctrl->n_samples;
+                    ensure_samp_host(r, n_sent, r->n_sample_tokens);
+                    copy_samples(o, r, 0, 0, n_sent, true, stream_);
                 }
                 r->has_text = false;
                 if (fmt) format_text(d_utf8, d_off, n_sent, r);
@@ -638,10 +687,12 @@ class EngineImpl final : public Engine {
                 o.tokens.ensure(size_t(max_chunk_bytes) * 24 + 24, 1.25);
                 ensure_marg_out(o, max_chunk_sent, max_chunk_bytes);
                 ensure_lat_out(o, ws_[0], max_chunk_sent);
+                ensure_samp_out(o, max_chunk_sent);
             }
             // a pinned result sized from the learned tokens-per-byte ratio (grown below if short)
             HostResult* r = acquire(n_sent, uint64_t(double(n_bytes) * tok_per_byte_) + 1024);
             if (r->has_lat) ensure_lat_host(r, n_sent, uint64_t(double(n_bytes) * node_per_byte_) + 1024);
+            if (r->has_samp) ensure_samp_host(r, n_sent, uint64_t(double(n_bytes) * tok_per_byte_ * samp_n_) + 1024);
             // output stage: each slot's text buffer holds the text a chunk is expected to produce (at most 4 bytes per
             // sentence plus the learned ratio per input byte); a chunk with more text flags itself and the batch is
             // re-run with the ratio it measured
@@ -656,6 +707,7 @@ class EngineImpl final : public Engine {
             }
             CK(cudaMemsetAsync(tok_base_.p, 0, 8, stream_));
             if (lattice_) CK(cudaMemsetAsync(node_base_.p, 0, 8, stream_));
+            if (samp_n_) CK(cudaMemsetAsync(samp_base_.p, 0, 8, stream_));
             connid_begin(stream_);
             h2d(in_off_.p, off, (size_t(n_sent) + 1) * 8, stream_, off_pinned && off == byte_off);
             CK(cudaEventRecord(in_done_, stream_));
@@ -664,7 +716,7 @@ class EngineImpl final : public Engine {
             std::memset(stage_ms_, 0, sizeof(stage_ms_));
             std::memset(counters_, 0, sizeof(counters_));
             launches_ = 0;
-            uint64_t tok_total = 0, text_total = 0, node_total = 0;
+            uint64_t tok_total = 0, text_total = 0, node_total = 0, samp_total = 0;
             double text_need = 0;  // text bytes per input byte beyond text_per_sent_ per sentence, largest over the sound chunks
             uint32_t route = kRouteNone;
             bool overflow = false, bad_utf8 = false, bad_offsets = false, slots_overflow = false, text_overflow = false;
@@ -708,6 +760,7 @@ class EngineImpl final : public Engine {
                 pool_need_ = std::max<uint64_t>(pool_need_, pool_need(*o.h_ctrl));
                 const uint64_t nt = o.h_ctrl->n_tokens, nx = fmt ? o.h_ctrl->text_bytes : 0;
                 const uint64_t nn = lattice_ ? o.h_ctrl->n_nodes : 0;
+                const uint64_t ns = samp_n_ ? o.h_ctrl->n_samples : 0;
                 if (fmt && !(o.h_ctrl->flags & (kFlagsStandDown | kFlagUtf8Error | kFlagPoolOverflow)))
                     text_need = std::max(text_need, (double(nx) - double(text_per_sent_) * (s1 - s0)) / double(std::max<uint64_t>(1, off[s1] - off[s0])));
                 if (!overflow && !text_overflow && !bad_utf8 && !bad_offsets && !bad_bounds) {
@@ -747,6 +800,13 @@ class EngineImpl final : public Engine {
                         }
                         copy_lattice(o, r, node_total, s0, s1 - s0, last, out_stream_);
                     }
+                    if (r->has_samp) {  // sample offsets are global already (samp_base_); the records grow like the tokens
+                        if ((samp_total + ns) * 24 > r->cap_samples) {
+                            CK(cudaStreamSynchronize(out_stream_));
+                            grow_samp_host(r, size_t(double(samp_total + ns) * 1.5) + 4096, samp_total);
+                        }
+                        copy_samples(o, r, samp_total, s0, s1 - s0, last, out_stream_);
+                    }
                     if (fmt) {
                         if (text_total + nx + 1 > r->cap_text) {  // grown like the token buffer
                             CK(cudaStreamSynchronize(out_stream_));
@@ -766,6 +826,7 @@ class EngineImpl final : public Engine {
                 tok_total += nt;
                 text_total += nx;
                 node_total += nn;
+                samp_total += ns;
             };
             pool_need_ = 0;
             for (uint32_t c = 0; c < n_chunks; ++c) {
@@ -781,7 +842,7 @@ class EngineImpl final : public Engine {
                 if (cb.off) cb.off += s0;
                 enqueue(w, d_utf8, d_off + s0, s1 - s0, off[s1] - off[s0], o, tok_base_.as<unsigned long long>(),
                         fmt ? text_base_.as<unsigned long long>() : nullptr, c >= 1 ? base_ready_[(c - 1) & 1] : nullptr,
-                        base_ready_[c & 1], cb);
+                        base_ready_[c & 1], cb, s0);
                 if (!utf8_pinned && c + 1 < n_chunks) issue_h2d(c + 1);
                 if (c >= 1) drain(c - 1);
             }
@@ -821,6 +882,7 @@ class EngineImpl final : public Engine {
             last_route_ = route;
             r->n_tokens = tok_total;
             r->n_nodes = node_total;
+            r->n_sample_tokens = samp_total;
             r->has_text = fmt;
             r->text_bytes = text_total;
             return r;
@@ -859,7 +921,7 @@ class EngineImpl final : public Engine {
             else
                 h2d(in_utf8_.p, utf8 + first, n_bytes, stream_, is_pinned(utf8 + first));
         }
-        run_whole(in_utf8_.as<uint8_t>(), in_off_.as<unsigned long long>(), n_sent, n_bytes, bd);
+        run_whole(in_utf8_.as<uint8_t>(), in_off_.as<unsigned long long>(), n_sent, n_bytes, bd, sample_base_);
         shard_n_sent_ = n_sent;
         shard_text_ = text_bytes && output_mode_ != kOutNone;
         shard_text_bytes_ = shard_text_ ? format_whole(in_utf8_.as<uint8_t>(), in_off_.as<unsigned long long>(), n_sent) : 0;
@@ -947,6 +1009,37 @@ class EngineImpl final : public Engine {
         *d_links = reinterpret_cast<uint64_t>(o.links.p);
         *d_node_prob = o.marg ? reinterpret_cast<uint64_t>(o.node_prob.p) : 0;
     }
+    void set_sample_base(uint64_t first_sentence) override { sample_base_ = first_sentence; }
+    uint64_t shard_samples() const override {
+        if (!out_[0].samp) throw Error(kInternal, "the shard was run without sampling");
+        return out_[0].h_ctrl->n_samples;
+    }
+    void fetch_shard_samples(uint64_t* h_sample_off, void* h_samples, uint64_t sample_base, bool last) override {
+        CK(cudaSetDevice(device_));
+        OutSlot& o = out_[0];
+        if (!o.samp) throw Error(kInternal, "the shard was run without sampling");
+        const uint64_t walks = uint64_t(shard_n_sent_) * samp_n_;
+        if (sample_base)
+            k_add_value<<<unsigned((walks + 256) / 256), 256, 0, stream_>>>(o.sample_off.as<unsigned long long>(), uint32_t(walks + 1),
+                                                                            sample_base);
+        CK(cudaMemcpyAsync(h_sample_off, o.sample_off.p, (walks + (last ? 1 : 0)) * 8, cudaMemcpyDeviceToHost, stream_));
+        if (o.h_ctrl->n_samples)
+            CK(cudaMemcpyAsync(h_samples, o.samples.p, o.h_ctrl->n_samples * 24, cudaMemcpyDeviceToHost, stream_));
+        CK(cudaStreamSynchronize(stream_));
+    }
+    void rebase_shard_samples(uint64_t sample_base) override {
+        CK(cudaSetDevice(device_));
+        const uint64_t walks = uint64_t(shard_n_sent_) * samp_n_;
+        if (sample_base)
+            k_add_value<<<unsigned((walks + 256) / 256), 256, 0, stream_>>>(out_[0].sample_off.as<unsigned long long>(),
+                                                                            uint32_t(walks + 1), sample_base);
+        CK(cudaStreamSynchronize(stream_));
+    }
+    void shard_samples_dev(uint64_t* d_sample_off, uint64_t* d_samples) const override {
+        if (!out_[0].samp) throw Error(kInternal, "the shard was run without sampling");
+        *d_sample_off = reinterpret_cast<uint64_t>(out_[0].sample_off.p);
+        *d_samples = reinterpret_cast<uint64_t>(out_[0].samples.p);
+    }
     int device() const override { return device_; }
     uint32_t token_bytes() const override { return tok_bytes_; }
     std::string describe() const override {
@@ -1010,6 +1103,8 @@ class EngineImpl final : public Engine {
         // warp-per-sentence kernels derive the sentence from a 32-bit global thread index (>> 5): 2^27 is the bound
         if (n_sent >= 0x07FFFFFFull || n_bytes + n_sent >= 0xFFFFFF00ull)
             throw Error(kInvalidArgument, "batch too large: split it (at most 2^27 sentences / 2^32 characters per call)");
+        if (n_sent * samp_n_ >= 0xFFFFFFFFull)
+            throw Error(kInvalidArgument, "sampling: n_sent * n must stay below 2^32: split the batch or draw fewer samples");
     }
 
     static constexpr const char* kBadBoundsMsg =
@@ -1095,7 +1190,42 @@ class EngineImpl final : public Engine {
         if (r->has_marg) ensure_marg_host(r, n_sent, n_tokens);
         r->has_lat = lattice_ != 0;
         r->n_nodes = 0;
+        r->has_samp = samp_n_ != 0;
+        r->n_samp = samp_n_;
+        r->n_sample_tokens = 0;
         return r;
+    }
+
+    // Pinned sample arrays of `r` for n_sent sentences and n_tokens sample tokens (contents not kept).
+    void ensure_samp_host(HostResult* r, uint64_t n_sent, uint64_t n_tokens) {
+        const size_t off_bytes = (n_sent * samp_n_ + 1) * 8;
+        if (off_bytes > r->cap_sample_off) {
+            pinned_free(r->sample_off);
+            r->cap_sample_off = size_t(double(off_bytes) * 1.25) + 64;
+            r->sample_off = static_cast<uint64_t*>(pinned_alloc(r->cap_sample_off));
+        }
+        if (n_tokens * 24 > r->cap_samples) grow_samp_host(r, size_t(double(n_tokens) * 1.25) + 64, 0);
+    }
+    // Grows the sample records of `r` to `n` entries, keeping the first `keep`.
+    static void grow_samp_host(HostResult* r, size_t n, uint64_t keep) {
+        if (n * 24 <= r->cap_samples) return;
+        void* bigger = pinned_alloc(n * 24);
+        if (keep) std::memcpy(bigger, r->samples, keep * 24);
+        pinned_free(r->samples);
+        r->samples = bigger;
+        r->cap_samples = n * 24;
+    }
+    // D2H of the samples of slot `o` (n sentences, h_ctrl->n_samples records) to sentence s0 / record `at` of `r`.
+    void copy_samples(const OutSlot& o, HostResult* r, uint64_t at, uint64_t s0, uint64_t n, bool last, cudaStream_t st) {
+        const uint64_t ns = o.h_ctrl->n_samples;
+        CK(cudaMemcpyAsync(r->sample_off + s0 * samp_n_, o.sample_off.p, (n * samp_n_ + (last ? 1 : 0)) * 8,
+                           cudaMemcpyDeviceToHost, st));
+        if (ns) CK(cudaMemcpyAsync(static_cast<uint8_t*>(r->samples) + at * 24, o.samples.p, ns * 24, cudaMemcpyDeviceToHost, st));
+    }
+    // Device sample offsets of slot `o` for (chunks of) up to n_sent sentences; the records are sized by enqueue
+    // from the scanned total.
+    void ensure_samp_out(OutSlot& o, uint32_t n_sent) {
+        if (samp_n_) o.sample_off.ensure((size_t(n_sent) * samp_n_ + 1) * 8, 1.25);
     }
 
     // Pinned lattice arrays of `r` for n_sent sentences and n_nodes nodes (contents not kept).
@@ -1174,9 +1304,8 @@ class EngineImpl final : public Engine {
 
     // Device marginal outputs of slot `o` for (chunks of) up to n_sent sentences and n_bytes bytes.
     void ensure_marg_out(OutSlot& o, uint32_t n_sent, uint64_t n_bytes) {
-        if (theta_ == 0) return;
-        o.token_prob.ensure(size_t(n_bytes) * 4 + 4, 1.25);  // a token spans >= 1 byte
-        o.path_prob.ensure((size_t(n_sent) + 1) * 4, 1.25);
+        if (theta_ > 0) o.token_prob.ensure(size_t(n_bytes) * 4 + 4, 1.25);  // a token spans >= 1 byte
+        if (theta_ > 0 || samp_n_) o.path_prob.ensure((size_t(n_sent) + 1) * 4, 1.25);  // the forward pass writes it
     }
 
     // Output stage buffers of slot `o` and scan storage of `w` for (chunks of) up to n_sent sentences.
@@ -1538,7 +1667,8 @@ class EngineImpl final : public Engine {
         w.ends_cnt.ensure(ms * 4, 1.25);
         w.ends_meta.ensure(ms * 8, 1.25);
         if (bounded) w.bnd_dist.ensure(ms * 4, 1.25);
-        if (theta_ > 0) {
+        const bool fwd = theta_ > 0 || samp_n_;  // the forward pass runs
+        if (fwd) {
             w.m_fill.ensure(ms * 4, 1.25);
             w.m_ncand.ensure(ms * 4, 1.25);
             w.m_r_eos.ensure(ns * 8, 1.25);
@@ -1554,14 +1684,26 @@ class EngineImpl final : public Engine {
         w.seg.ensure(want_cand * 8);  // sized like the candidates; move segments can outnumber them (overflow retry)
         w.ends_hot.ensure((want_cand + ns) * 8);
         w.ends_cold.ensure((want_cand + ns) * 16);
-        if (theta_ > 0) {
+        if (fwd) {
             w.m_cand_entry.ensure((want_cand + ns) * 4);
             w.m_R.ensure((want_cand + ns) * 8);
             w.m_ab.ensure((want_cand + ns) * 16);
         }
+        if (samp_n_) {
+            w.m_lw.ensure((want_cand + ns) * 4);
+            const size_t walks = size_t(n_sent) * samp_n_ + 1;
+            w.s_cnt.ensure(walks * 4, 1.25);
+            w.s_total.ensure(walks * 4, 1.25);
+        }
         size_t tmp = 0;  // cub temp storage for the largest scan / sort of this size
         cub::DeviceScan::ExclusiveSum(nullptr, tmp, static_cast<uint32_t*>(nullptr), static_cast<uint32_t*>(nullptr), ms, w.stream);
         w.scan_tmp.ensure(tmp + 1024, 1.5);
+        if (samp_n_) {  // the scan of the walks' token counts
+            cub::TransformInputIterator<unsigned long long, CastU64, const uint32_t*> it(static_cast<const uint32_t*>(nullptr), CastU64());
+            cub::DeviceScan::ExclusiveSum(nullptr, tmp, it, static_cast<unsigned long long*>(nullptr),
+                                          size_t(n_sent) * samp_n_ + 1, w.stream);
+            w.scan_tmp.ensure(tmp + 1024, 1.5);
+        }
         if (order_mode_ == 1) {
             cub::DeviceRadixSort::SortPairsDescending(nullptr, tmp, static_cast<uint32_t*>(nullptr), static_cast<uint32_t*>(nullptr),
                                                       static_cast<uint32_t*>(nullptr), static_cast<uint32_t*>(nullptr), int(ns), 0,
@@ -1571,8 +1713,9 @@ class EngineImpl final : public Engine {
     }
 
     // One whole batch from device-resident input into out_[0]; synchronises, retries on pool overflow.
+    // sent_base: the caller's index of the first sentence (a shard's place in the batch), for the sampling draws.
     void run_whole(const uint8_t* d_utf8, const unsigned long long* d_off, uint32_t n_sent, uint64_t n_bytes,
-                   const DevBounds& bd) {
+                   const DevBounds& bd, uint64_t sent_base = 0) {
         OutSlot& o = out_[0];
         ws_[0].stream = stream_;
         batch_total_bytes_ = n_bytes;
@@ -1582,8 +1725,9 @@ class EngineImpl final : public Engine {
             o.tokens.ensure(size_t(n_bytes) * 24 + 24, 1.25);  // a token spans >= 1 character >= 1 byte
             ensure_marg_out(o, n_sent, n_bytes);
             ensure_lat_out(o, ws_[0], n_sent);
+            ensure_samp_out(o, n_sent);
             connid_begin(stream_);
-            enqueue(ws_[0], d_utf8, d_off, n_sent, n_bytes, o, nullptr, nullptr, nullptr, nullptr, bd);
+            enqueue(ws_[0], d_utf8, d_off, n_sent, n_bytes, o, nullptr, nullptr, nullptr, nullptr, bd, sent_base);
             CK(cudaEventSynchronize(o.done));
             CK(cudaGetLastError());
             if (o.h_ctrl->flags & kFlagBadOffsets)
@@ -1620,17 +1764,18 @@ class EngineImpl final : public Engine {
     // o.text up to its capacity (kFlagTextOverflow beyond).
     void enqueue(Workspace& w, const uint8_t* d_utf8, const unsigned long long* d_off, uint32_t n_sent, uint64_t n_bytes,
                  OutSlot& o, unsigned long long* tok_base, unsigned long long* text_base, cudaEvent_t base_wait,
-                 cudaEvent_t base_signal, const DevBounds& bd) {
+                 cudaEvent_t base_signal, const DevBounds& bd, uint64_t sent0) {
         cudaStream_t st = w.stream;
         // characters <= bytes is the hard bound; the per-character launches are sized from the ratio learned on
         // earlier batches (plus slack), and a batch that exceeds it flags itself and is re-run with the hard bound
         const uint32_t hard_slots = uint32_t(n_bytes + n_sent);
         const uint32_t max_slots = uint32_t(std::min<uint64_t>(hard_slots, uint64_t(double(n_bytes) * chars_per_byte_) + n_sent + 4096));
         size_t cap_all = std::min<size_t>(0xFFFFFFF0ull, std::min<size_t>(w.ends_hot.cap / 8 - n_sent - 1, w.ends_cold.cap / 16 - n_sent - 1));
-        const bool marg = theta_ > 0;
-        if (marg)
+        const bool marg = theta_ > 0, samp = samp_n_ != 0;
+        if (marg || samp)
             cap_all = std::min<size_t>(cap_all, std::min<size_t>(w.m_cand_entry.cap / 4,
                                                                  std::min<size_t>(w.m_R.cap / 8, w.m_ab.cap / 16)) - n_sent - 1);
+        if (samp) cap_all = std::min<size_t>(cap_all, w.m_lw.cap / 4 - n_sent - 1);
         const bool lat = lattice_ != 0;
         if (lat) {  // nodes <= candidates placed: the node arrays bound the pool too
             cap_all = std::min<size_t>(cap_all, std::min<size_t>(o.nodes.cap / 24, o.links.cap / 8));
@@ -1723,8 +1868,8 @@ class EngineImpl final : public Engine {
         o.launches += launch_viterbi(dv_, b, counting_ ? w.stats.as<uint4>() : nullptr, lanes_, viterbi_kernel_, st, &o.route);
         MargArgs m{};
         o.marg = marg;
-        if (marg) {  // booked with the Viterbi stage; must run before K4a reuses ends_meta
-            m.theta = theta_;
+        if (marg || samp) {  // booked with the Viterbi stage; must run before K4a reuses ends_meta
+            m.theta = marg ? theta_ : samp_theta_;  // equal when both are on (set_marginals / set_sampling)
             m.fill = w.m_fill.as<uint32_t>();
             m.ncand = w.m_ncand.as<uint32_t>();
             m.cand_entry = w.m_cand_entry.as<uint32_t>();
@@ -1733,9 +1878,10 @@ class EngineImpl final : public Engine {
             m.r_eos = w.m_r_eos.as<long long>();
             m.a_eos = w.m_a_eos.as<double>();
             m.path_prob = o.path_prob.as<float>();
-            m.token_prob = o.token_prob.as<float>();
-            launch_marginals(dv_, b, m, st);
-            if (n_sent) o.launches += 2;
+            m.token_prob = marg ? o.token_prob.as<float>() : nullptr;
+            m.lw = samp ? w.m_lw.as<uint32_t>() : nullptr;
+            launch_marginals(dv_, b, m, st, marg);  // sampling alone needs no backward pass
+            if (n_sent) o.launches += marg ? 2 : 1;
         }
         o.lat = lat;
         if (lat) {  // booked with the Viterbi stage too, and also before K4a
@@ -1753,6 +1899,29 @@ class EngineImpl final : public Engine {
             launch_lattice_write(b, l, m, st);
             CK(cudaMemcpyAsync(&dc->n_nodes, l.node_off + n_sent, 8, cudaMemcpyDeviceToDevice, st));
             if (n_sent) o.launches += 2;
+        }
+        o.samp = samp;
+        if (samp) {  // booked with the Viterbi stage too, and also before K4a
+            SampleArgs sa{};
+            sa.n = samp_n_;
+            sa.seed = samp_seed_;
+            sa.sent_base = sent0;
+            sa.cnt = w.s_cnt.as<uint32_t>();
+            sa.total = w.s_total.as<int32_t>();
+            sa.off = o.sample_off.as<unsigned long long>();
+            const size_t walks = size_t(n_sent) * samp_n_;
+            launch_sample_count(dv_, b, m, sa, st);
+            CK(cudaMemsetAsync(sa.cnt + walks, 0, 4, st));
+            cub::TransformInputIterator<unsigned long long, CastU64, const uint32_t*> it(sa.cnt, CastU64());
+            exclusive_scan(w, it, sa.off, walks + 1);
+            CK(cudaMemcpyAsync(&dc->n_samples, sa.off + walks, 8, cudaMemcpyDeviceToDevice, st));
+            // the records are sized from the scanned total: one wait for it here
+            CK(cudaMemcpyAsync(&o.h_ctrl->n_samples, sa.off + walks, 8, cudaMemcpyDeviceToHost, st));
+            CK(cudaStreamSynchronize(st));
+            o.samples.ensure(size_t(o.h_ctrl->n_samples) * 24 + 24, 1.25);
+            sa.out = o.samples.as<uint2>();
+            launch_sample_write(dv_, b, m, sa, st);
+            if (walks) o.launches += 2;
         }
         CK(cudaEventRecord(o.ev[6], st));
         launch_backtrack_count(b, st);
@@ -1781,6 +1950,13 @@ class EngineImpl final : public Engine {
             if (lat) {  // the same for the node offsets
                 k_add_base<<<(n_sent + 256) / 256, 256, 0, st>>>(o.node_off.as<unsigned long long>(), n_sent + 1, node_base_.as<unsigned long long>());
                 k_bump_base<<<1, 1, 0, st>>>(node_base_.as<unsigned long long>(), &dc->n_nodes);
+                o.launches += 2;
+            }
+            if (samp) {  // and for the sample offsets
+                const size_t walks = size_t(n_sent) * samp_n_;
+                k_add_base<<<unsigned((walks + 256) / 256), 256, 0, st>>>(o.sample_off.as<unsigned long long>(), uint32_t(walks + 1),
+                                                                          samp_base_.as<unsigned long long>());
+                k_bump_base<<<1, 1, 0, st>>>(samp_base_.as<unsigned long long>(), &dc->n_samples);
                 o.launches += 2;
             }
             if (text_base) {
@@ -1823,7 +1999,7 @@ class EngineImpl final : public Engine {
     cudaEvent_t in_done_ = nullptr;
     std::vector<cudaEvent_t> h2d_ev_;
     OutSlot out_[2];
-    DevBuf tok_base_, text_base_, node_base_;
+    DevBuf tok_base_, text_base_, node_base_, samp_base_;
     uint32_t chunk_sentences_ = 262144;
     uint64_t pool_need_ = 0;
     double tok_per_byte_ = 0.2;
@@ -1871,6 +2047,12 @@ class EngineImpl final : public Engine {
     bool dev_marg_ = false;   // the last run_device computed marginals (device_marginals)
     int lattice_ = 0;         // option "lattice": 0 off, 1 nodes, 2 nodes and lattice text
     bool dev_lat_ = false;    // the last run_device produced the lattice (device_lattice)
+    static constexpr uint32_t kMaxSamples = 1024;
+    uint32_t samp_n_ = 0;       // sampling: paths per sentence, 0 = off (set_sampling)
+    double samp_theta_ = 0;
+    uint64_t samp_seed_ = 0;
+    uint64_t sample_base_ = 0;  // the caller's index of a shard's first sentence (set_sample_base; 0 outside shards)
+    bool dev_samp_ = false;     // the last run_device drew samples (device_samples)
     float stage_ms_[kNumStages];
     uint64_t launches_ = 0;
     uint32_t last_route_ = kRouteNone;  // ViterbiRoute of the last successful call (describe())

@@ -38,6 +38,14 @@ struct HostResult {  // pinned host memory holding one batch's tokens
     float* node_prob = nullptr;    // n_nodes, with marginals only (has_marg)
     size_t cap_node_off = 0, cap_nodes = 0, cap_links = 0, cap_nprob = 0;
     bool has_lat = false;
+    // segmentation sampling (set_sampling): n_samp paths per sentence, has_samp == false when it is off.
+    // sample_off[i * n_samp + j] .. sample_off[i * n_samp + j + 1] index sample j of sentence i (kernels.cuh SampleArgs).
+    uint32_t n_samp = 0;
+    uint64_t n_sample_tokens = 0;
+    uint64_t* sample_off = nullptr;  // n_sent * n_samp + 1
+    void* samples = nullptr;         // vbt_token[n_sample_tokens], always 24 bytes
+    size_t cap_sample_off = 0, cap_samples = 0;
+    bool has_samp = false;
 };
 
 // Required token boundaries of a batch (vbt_tokenize_batch_bounded): sentence i's boundaries are the
@@ -104,6 +112,15 @@ class Engine {
                                      uint64_t node_base, bool last) = 0;
     virtual void rebase_shard_lattice(uint64_t node_base) = 0;
     virtual void shard_lattice(uint64_t* d_node_off, uint64_t* d_nodes, uint64_t* d_links, uint64_t* d_node_prob) const = 0;
+    // Sampling: set_sample_base gives the caller's index of the next run's first sentence (the i of the draws), so
+    // that a shard draws what the whole batch would.  The last shard's sample-token count; fetch_shard_samples copies
+    // its sample offsets (+ sample_base, n_sent * n entries, one more when `last`) and records into host memory;
+    // rebase_shard_samples adds sample_base on the device and shard_samples_dev gives the two device addresses.
+    virtual void set_sample_base(uint64_t first_sentence) = 0;
+    virtual uint64_t shard_samples() const = 0;
+    virtual void fetch_shard_samples(uint64_t* h_sample_off, void* h_samples, uint64_t sample_base, bool last) = 0;
+    virtual void rebase_shard_samples(uint64_t sample_base) = 0;
+    virtual void shard_samples_dev(uint64_t* d_sample_off, uint64_t* d_samples) const = 0;
     virtual int device() const = 0;
     virtual uint32_t token_bytes() const = 0;  // 24, or 16 with the "compact_tokens" option
     virtual std::string describe() const = 0;  // JSON: devices, how the dictionary travelled, ...
@@ -125,6 +142,15 @@ class Engine {
     virtual void set_marginals(double theta) = 0;
     virtual double marginals() const = 0;
     virtual int lattice() const = 0;  // the option "lattice"
+    // Segmentation sampling (kernels.cuh SampleArgs): n (1..1024) paths per sentence drawn from P(path) at temperature
+    // theta (> 0, finite; the marginals' theta when they are on), with Philox keyed by seed; n = 0 switches it off.
+    // On every route except k_small_batch, which steps aside.  Results then carry HostResult::sample_off / samples,
+    // and run_device leaves them in device memory (device_samples).
+    virtual void set_sampling(uint32_t n, double theta, uint64_t seed) = 0;
+    virtual uint32_t sampling() const = 0;  // n, 0 when off
+    // Device addresses of the last run_device's uint64 sample_off[n_sent * n + 1] and vbt_token samples[n_tokens];
+    // valid until the next call.  Throws when that call ran without sampling.
+    virtual void device_samples(uint64_t* d_sample_off, uint64_t* d_samples, uint64_t* n_tokens) const = 0;
     // Device addresses of the last run_device's float token_prob[n_tokens] and path_prob[n_sent]; valid until the
     // next call.  Throws when that call ran without marginals.
     virtual void device_marginals(uint64_t* d_token_prob, uint64_t* d_path_prob) const = 0;

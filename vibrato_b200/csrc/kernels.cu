@@ -1326,7 +1326,8 @@ __device__ __forceinline__ bool marg_sentence(const Batch& b, uint32_t sidx, uin
     return true;
 }
 
-template <int CONN>
+// LW: the sampling instantiation, which also keeps each entry's {left id, word cost} in m.lw.
+template <int CONN, bool LW = false>
 __global__ void __launch_bounds__(256) k_marg_forward(DictView d, Batch b, MargArgs m) {
     if (stand_down(*b.flags)) return;
     const uint32_t lane = threadIdx.x & 31;
@@ -1393,6 +1394,7 @@ __global__ void __launch_bounds__(256) k_marg_forward(DictView d, Batch b, MargA
                 }
                 m.R[idx] = rmin;
                 m.ab[idx].x = L;
+                if (LW) m.lw[idx] = (cd.x & 0xFFFFu) | (cd.y << 16);
             }
             __syncwarp();
         }
@@ -1569,6 +1571,139 @@ __global__ void __launch_bounds__(256) k_lattice_write(Batch b, LatticeArgs l, M
             }
         }
     }
+}
+
+// ---------------------------------------------------------------------------------------------
+// Segmentation sampling (SampleArgs in kernels.cuh): one lane per (sentence, sample) walk from EOS back to BOS.
+// ---------------------------------------------------------------------------------------------
+
+// Philox4x32-10 (Salmon et al., "Parallel random numbers: as easy as 1, 2, 3", SC'11) with its standard multipliers
+// and Weyl key increments.
+__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k) {
+#pragma unroll
+    for (int r = 0; r < 10; ++r) {
+        if (r) {
+            k.x += 0x9E3779B9u;
+            k.y += 0xBB67AE85u;
+        }
+        const uint32_t lo0 = 0xD2511F53u * c.x, hi0 = __umulhi(0xD2511F53u, c.x);
+        const uint32_t lo1 = 0xCD9E8D57u * c.z, hi1 = __umulhi(0xCD9E8D57u, c.z);
+        c = make_uint4(hi1 ^ c.y ^ k.x, lo1, hi0 ^ c.w ^ k.y, lo0);
+    }
+    return c;
+}
+
+// The uniform of draw step t of sample j of sentence i: 53 bits of the first two output words, in [0, 1).
+__device__ __forceinline__ double sample_uniform(unsigned long long seed, uint32_t t, uint32_t j, uint32_t i) {
+    const uint4 x = philox4x32_10(make_uint4(t, j, i, 0u), make_uint2(uint32_t(seed), uint32_t(seed >> 32)));
+    return (double(x.x >> 5) * 67108864.0 + double(x.y >> 6)) * (1.0 / 9007199254740992.0);
+}
+
+// One walk: count (WRITE = false: its tokens and i32 total into cnt / total) or write (its records, from the end).
+template <int CONN, bool WRITE>
+__device__ __forceinline__ void sample_walk(const DictView& d, const Batch& b, const MargArgs& m, const SampleArgs& sa) {
+    const unsigned long long w = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (w >= (unsigned long long)b.n_sent * sa.n) return;
+    const uint32_t sidx = uint32_t(w / sa.n), j = uint32_t(w % sa.n);
+    const uint32_t s = b.order ? b.order[sidx] : sidx;
+    const unsigned long long walk = (unsigned long long)s * sa.n + j;
+    const bool sound = !(*b.flags & (kFlagsStandDown | kFlagPoolOverflow));  // else the rows cannot be trusted
+    const uint32_t base = sound ? b.slot_off[s] : 0u, last = sound ? b.slot_off[s + 1] - 1 : 0u;
+    const uint4 eos = sound && base != last ? b.eos[s] : make_uint4(kNone, 0, 0, 0);
+    if (eos.x == kNone) {  // an empty sentence, one without a path, or a batch that is re-run or refused
+        if (!WRITE) {
+            sa.cnt[walk] = 0;
+            sa.total[walk] = 0;
+        }
+        return;
+    }
+    const uint32_t i = uint32_t(sa.sent_base + s);
+    const double th = m.theta;
+    uint32_t row = base + eos.y;  // the slot of the row the current node starts at
+    uint32_t left = 0;            // EOS: BOS_EOS_CONNECTION_ID, no word cost
+    int32_t wc = 0;
+    long long r = m.r_eos[s];
+    uint32_t tokens = 0, sum = 0;  // sum: the path's cost so far, wrapping like the tokenizer's i32
+    unsigned long long at = 0;
+    if (WRITE) {
+        sum = uint32_t(sa.total[walk]);
+        at = sa.off[walk] + sa.cnt[walk];
+    }
+    for (uint32_t t = 0; row != base; ++t) {
+        const uint2 me = b.ends_meta[row];
+        const uint32_t eo = me.x, K = me.y - me.x;
+        const ConnRow<CONN> conn(d, left);
+        double mx = -INFINITY;
+        for (uint32_t k = 0; k < K; ++k) {
+            const long long x = m.R[eo + k] + conn.cost(d, uint32_t(b.ends_hot[eo + k].y)) + wc;
+            mx = fmax(mx, m.ab[eo + k].x - th * double(x - r));
+        }
+        double S = 0.0;
+        for (uint32_t k = 0; k < K; ++k) {
+            const long long x = m.R[eo + k] + conn.cost(d, uint32_t(b.ends_hot[eo + k].y)) + wc;
+            S += exp(m.ab[eo + k].x - th * double(x - r) - mx);
+        }
+        const double target = sample_uniform(sa.seed, t, j, i) * S;
+        double cum = 0.0;
+        uint32_t pick = kNone, last_pos = 0;
+        int32_t step = 0, step_last = 0;
+        for (uint32_t k = 0; k < K; ++k) {
+            const int32_t c = conn.cost(d, uint32_t(b.ends_hot[eo + k].y));
+            const long long x = m.R[eo + k] + c + wc;
+            const double wk = exp(m.ab[eo + k].x - th * double(x - r) - mx);
+            cum += wk;
+            const int32_t stp = int32_t(uint32_t(c) + uint32_t(wc));
+            if (wk > 0.0) {
+                last_pos = k;
+                step_last = stp;
+            }
+            if (cum > target) {
+                pick = k;
+                step = stp;
+                break;
+            }
+        }
+        if (pick == kNone) {
+            pick = last_pos;
+            step = step_last;
+        }
+        const uint32_t e = eo + pick;
+        if (WRITE) {  // the token's prefix cost = the path's cost through c minus the edge into c
+            sum -= uint32_t(step);
+            const uint4 c = b.ends_cold[e];
+            const uint32_t start_node = c.x - base;
+            const uint2 i8 = b.info[c.x];
+            const uint32_t start_word = start_node + ((i8.y & kInfoSpecial) ? b.info_ex[c.x].x : 0u);  // as backtrack_write_one
+            uint2* out = sa.out + (--at) * 3;
+            out[0] = make_uint2(start_word, row - base);
+            out[1] = make_uint2(b.byte_pos[base + start_word], b.byte_pos[row]);
+            out[2] = make_uint2(c.z, sum);
+            row = c.x;
+        } else {
+            sum += uint32_t(step);
+            row = b.ends_cold[e].x;
+        }
+        ++tokens;
+        const uint32_t lw = m.lw[e];
+        left = lw & 0xFFFFu;
+        wc = int16_t(lw >> 16);
+        r = m.R[e];
+    }
+    if (!WRITE) {  // the first token's edge from BOS (right id 0, cost 0)
+        sum += uint32_t(ConnRow<CONN>(d, left).cost(d, 0u)) + uint32_t(wc);
+        sa.cnt[walk] = tokens;
+        sa.total[walk] = int32_t(sum);
+    }
+}
+
+template <int CONN>
+__global__ void __launch_bounds__(256) k_sample_count(DictView d, Batch b, MargArgs m, SampleArgs sa) {
+    sample_walk<CONN, false>(d, b, m, sa);
+}
+
+template <int CONN>
+__global__ void __launch_bounds__(256) k_sample_write(DictView d, Batch b, MargArgs m, SampleArgs sa) {
+    sample_walk<CONN, true>(d, b, m, sa);
 }
 
 
@@ -2461,19 +2596,25 @@ void launch_backtrack_write(const Batch& b, cudaStream_t st) {
     k_backtrack_write<<<(b.n_sent + 8 * VBT_SENT_PER_WARP - 1) / (8 * VBT_SENT_PER_WARP), 256, 0, st>>>(b);  // warps over sentences
 }
 
-void launch_marginals(const DictView& d, const Batch& b, const MargArgs& m, cudaStream_t st) {
+// The forward pass's instantiation: with m.lw (sampling) the one that also keeps {left id, word cost}.
+template <int CONN>
+static void launch_marg_conn(const DictView& d, const Batch& b, const MargArgs& m, bool backward, uint32_t blocks, cudaStream_t st) {
+    if (m.lw)
+        k_marg_forward<CONN, true><<<blocks, 256, 0, st>>>(d, b, m);
+    else
+        k_marg_forward<CONN><<<blocks, 256, 0, st>>>(d, b, m);
+    if (backward) k_marg_backward<CONN><<<blocks, 256, 0, st>>>(d, b, m);
+}
+
+void launch_marginals(const DictView& d, const Batch& b, const MargArgs& m, cudaStream_t st, bool backward) {
     if (!b.n_sent) return;
     const uint32_t blocks = (b.n_sent + 7) / 8;  // a warp per sentence
-    if (d.connector_kind == 1) {
-        k_marg_forward<1><<<blocks, 256, 0, st>>>(d, b, m);
-        k_marg_backward<1><<<blocks, 256, 0, st>>>(d, b, m);
-    } else if (d.connector_kind == 2) {
-        k_marg_forward<2><<<blocks, 256, 0, st>>>(d, b, m);
-        k_marg_backward<2><<<blocks, 256, 0, st>>>(d, b, m);
-    } else {
-        k_marg_forward<0><<<blocks, 256, 0, st>>>(d, b, m);
-        k_marg_backward<0><<<blocks, 256, 0, st>>>(d, b, m);
-    }
+    if (d.connector_kind == 1)
+        launch_marg_conn<1>(d, b, m, backward, blocks, st);
+    else if (d.connector_kind == 2)
+        launch_marg_conn<2>(d, b, m, backward, blocks, st);
+    else
+        launch_marg_conn<0>(d, b, m, backward, blocks, st);
 }
 
 void launch_backtrack_write_marg(const Batch& b, const MargArgs& m, cudaStream_t st) {
@@ -2489,6 +2630,30 @@ void launch_lattice_count(const Batch& b, const LatticeArgs& l, cudaStream_t st)
 void launch_lattice_write(const Batch& b, const LatticeArgs& l, const MargArgs& m, cudaStream_t st) {
     if (!b.n_sent) return;
     k_lattice_write<<<(b.n_sent + 7) / 8, 256, 0, st>>>(b, l, m);
+}
+
+void launch_sample_count(const DictView& d, const Batch& b, const MargArgs& m, const SampleArgs& s, cudaStream_t st) {
+    const unsigned long long walks = (unsigned long long)b.n_sent * s.n;
+    if (!walks) return;
+    const uint32_t blocks = uint32_t((walks + 255) / 256);  // a lane per walk
+    if (d.connector_kind == 1)
+        k_sample_count<1><<<blocks, 256, 0, st>>>(d, b, m, s);
+    else if (d.connector_kind == 2)
+        k_sample_count<2><<<blocks, 256, 0, st>>>(d, b, m, s);
+    else
+        k_sample_count<0><<<blocks, 256, 0, st>>>(d, b, m, s);
+}
+
+void launch_sample_write(const DictView& d, const Batch& b, const MargArgs& m, const SampleArgs& s, cudaStream_t st) {
+    const unsigned long long walks = (unsigned long long)b.n_sent * s.n;
+    if (!walks) return;
+    const uint32_t blocks = uint32_t((walks + 255) / 256);
+    if (d.connector_kind == 1)
+        k_sample_write<1><<<blocks, 256, 0, st>>>(d, b, m, s);
+    else if (d.connector_kind == 2)
+        k_sample_write<2><<<blocks, 256, 0, st>>>(d, b, m, s);
+    else
+        k_sample_write<0><<<blocks, 256, 0, st>>>(d, b, m, s);
 }
 
 }  // namespace vbt

@@ -234,9 +234,13 @@ struct MargArgs {
     double* a_eos;           // per sentence: â(EOS)
     float* path_prob;        // per sentence: exp(-â(EOS)); 1 for an empty sentence
     float* token_prob;       // per token, at the token's index (tok_off)
+    // per lattice entry: {left id | word cost (i16) << 16} as the candidate carried them, written by the sampling
+    // instantiation of k_marg_forward only (lw != nullptr selects it); BOS's entry is not written
+    uint32_t* lw;
 };
-// k_marg_forward and k_marg_backward (two launches).
-void launch_marginals(const DictView& d, const Batch& b, const MargArgs& m, cudaStream_t st);
+// k_marg_forward and k_marg_backward (two launches); backward = false runs the forward pass alone (sampling without
+// marginals).  m.lw != nullptr selects the forward pass that also writes MargArgs::lw.
+void launch_marginals(const DictView& d, const Batch& b, const MargArgs& m, cudaStream_t st, bool backward = true);
 // launch_backtrack_write plus MargArgs::token_prob of every token (one launch, in its place).
 void launch_backtrack_write_marg(const Batch& b, const MargArgs& m, cudaStream_t st);
 
@@ -259,6 +263,30 @@ void launch_lattice_count(const Batch& b, const LatticeArgs& l, cudaStream_t st)
 // k_lattice_write: the records, links and, with l.node_prob, prob = exp(â + b̂ - â(EOS)) as k_backtrack_write_marg
 // computes it (a warp per sentence), after node_off has been scanned.
 void launch_lattice_write(const Batch& b, const LatticeArgs& l, const MargArgs& m, cudaStream_t st);
+
+// Segmentation sampling: n paths per sentence drawn with replacement from P(path) = exp(-theta cost) / Z, by
+// forward-filtering backward-sampling over what k_marg_forward left (R, â and MargArgs::lw), after it and before K4a.
+// A walk starts at EOS; at node c (EOS: left id 0, word cost 0) its predecessors are the entries k = 0..K-1 of the
+// row c starts at, in row order, with x_k = R(k) + conn(right(k), left(c)) + wcost(c), r = min x_k = R(c),
+// t_k = â(k) - theta (x_k - r), m = max t_k and w_k = exp(t_k - m).  The walk takes the first k whose running sum
+// (float64, in row order) exceeds u * S, S the whole sum (the last k with w_k > 0 if rounding leaves none), where
+// u = ((x0 >> 5) 2^26 + (x1 >> 6)) 2^-53 of Philox4x32-10 at counter (t, j, i, 0) and key (seed lo, seed hi):
+// t the draw step (0 at EOS), j the sample, i = sent_base + the sentence's index in the batch.  One lane per walk
+// (sentence, sample), launched in b.order; a walk's records are 24-byte vbt_token records built as the backtrack
+// builds them, with total_cost the sampled path's prefix cost in the tokenizer's wrapping i32 arithmetic.
+struct SampleArgs {
+    uint32_t n;                     // samples per sentence, 1..1024
+    unsigned long long seed;
+    unsigned long long sent_base;   // the caller's index of the batch's (chunk's, shard's) first sentence
+    uint32_t* cnt;                  // per walk s * n + j (+ 1 for the scan): its tokens
+    int32_t* total;                 // per walk: the path's total cost (wrapping i32)
+    unsigned long long* off;        // n_sent * n + 1: exclusive scan of cnt
+    uint2* out;                     // vbt_token as 3 x uint2
+};
+// k_sample_count: cnt and total of every walk (an empty sentence, one without a path or a re-run batch: 0).
+void launch_sample_count(const DictView& d, const Batch& b, const MargArgs& m, const SampleArgs& s, cudaStream_t st);
+// k_sample_write: the same walks again, writing each walk's records at off[walk] from its last token back.
+void launch_sample_write(const DictView& d, const Batch& b, const MargArgs& m, const SampleArgs& s, cudaStream_t st);
 
 // What k_small_batch reports besides its outputs: the batch flags and the totals of its scans.
 struct SmallBatchOut {

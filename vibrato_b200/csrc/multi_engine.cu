@@ -223,6 +223,8 @@ class MultiEngine final : public Engine {
             pinned_free(r->token_prob);
             pinned_free(r->path_prob);
             for (void* p : {static_cast<void*>(r->node_off), r->nodes, r->links, static_cast<void*>(r->node_prob)}) pinned_free(p);
+            pinned_free(r->sample_off);
+            pinned_free(r->samples);
             delete r;
         }
         pinned_free(h_off_);
@@ -233,7 +235,7 @@ class MultiEngine final : public Engine {
         if (gather_off_) cudaFree(gather_off_);
         if (gather_tprob_) cudaFree(gather_tprob_);
         if (gather_pprob_) cudaFree(gather_pprob_);
-        for (void* p : {gather_noff_, gather_nodes_, gather_links_, gather_nprob_})
+        for (void* p : {gather_noff_, gather_nodes_, gather_links_, gather_nprob_, gather_soff_, gather_samples_})
             if (p) cudaFree(p);
     }
 
@@ -245,10 +247,12 @@ class MultiEngine final : public Engine {
             collect_stats();
             return r;
         }
+        check_samples(n_sent);
         const std::vector<uint64_t> cut = split_by_bytes(byte_off, n_sent, n);
         std::vector<uint64_t> n_tok(n, 0), n_text(n, 0);
         run_on_all([&](int i) {
             const Bounds sb = shard_bounds(bnd, cut[i]);
+            eng_[i]->set_sample_base(cut[i]);  // the draws of sentence k are those of the whole batch
             n_tok[i] = eng_[i]->run_shard(utf8, byte_off + cut[i], cut[i + 1] - cut[i], -1, text_ ? &n_text[i] : nullptr,
                                           bnd ? &sb : nullptr);
         });
@@ -260,7 +264,11 @@ class MultiEngine final : public Engine {
         std::vector<uint64_t> node_base(n + 1, 0);  // lattice nodes: merged at their final positions like the tokens
         if (lattice_)
             for (int i = 0; i < n; ++i) node_base[i + 1] = node_base[i] + eng_[i]->shard_nodes();
-        HostResult* r = acquire(n_sent, base[n], text_ ? &text_base[n] : nullptr, node_base[n]);
+        const uint64_t ns = sampling();
+        std::vector<uint64_t> samp_base(n + 1, 0);  // sample records: merged at their final positions like the tokens
+        if (ns)
+            for (int i = 0; i < n; ++i) samp_base[i + 1] = samp_base[i] + eng_[i]->shard_samples();
+        HostResult* r = acquire(n_sent, base[n], text_ ? &text_base[n] : nullptr, node_base[n], samp_base[n]);
         const uint64_t tb = eng_[0]->token_bytes();
         r->token_bytes = uint32_t(tb);
         int last = n - 1;  // the shard that also delivers the closing offset: the last one, even when it is empty
@@ -272,6 +280,9 @@ class MultiEngine final : public Engine {
                 eng_[i]->fetch_shard_lattice(r->node_off + cut[i], static_cast<uint8_t*>(r->nodes) + node_base[i] * 24,
                                              static_cast<uint8_t*>(r->links) + node_base[i] * 8,
                                              r->has_marg ? r->node_prob + node_base[i] : nullptr, node_base[i], i == last);
+            if (r->has_samp)
+                eng_[i]->fetch_shard_samples(r->sample_off + cut[i] * ns, static_cast<uint8_t*>(r->samples) + samp_base[i] * 24,
+                                             samp_base[i], i == last);
         });
         collect_stats();
         return r;
@@ -293,7 +304,8 @@ class MultiEngine final : public Engine {
             collect_stats();
             return;
         }
-        dev_marg_ = dev_lat_ = false;
+        check_samples(n_sent);
+        dev_marg_ = dev_lat_ = dev_samp_ = false;
         CK(cudaSetDevice(dev_[0]));
         // the split needs the offsets on the host (pinned staging buffer, one copy); their validity is checked on
         // the devices like for any device-resident batch (k_count_chars)
@@ -319,6 +331,7 @@ class MultiEngine final : public Engine {
         std::vector<uint64_t> n_tok(n, 0);
         run_on_all([&](int i) {
             const Bounds sb = shard_bounds(bnd ? &hb : nullptr, cut[i]);
+            eng_[i]->set_sample_base(cut[i]);
             n_tok[i] = eng_[i]->run_shard(reinterpret_cast<const char*>(d_utf8), h_off_ + cut[i], cut[i + 1] - cut[i],
                                           dev_[0], nullptr, bnd ? &sb : nullptr);  // token-only, like the single-device entry point
         });
@@ -331,6 +344,13 @@ class MultiEngine final : public Engine {
             for (int i = 0; i < n; ++i) nbase[i + 1] = nbase[i] + eng_[i]->shard_nodes();
             run_on_all([&](int i) { eng_[i]->rebase_shard_lattice(nbase[i]); });
             for (int i = 0; i < n; ++i) eng_[i]->shard_lattice(&src_noff[i], &src_nodes[i], &src_links[i], &src_nprob[i]);
+        }
+        const uint64_t ns = sampling();
+        std::vector<uint64_t> sbase(n + 1, 0), src_soff(n), src_samp(n);
+        if (ns) {  // the samples too: records at their final positions, offsets rebased
+            for (int i = 0; i < n; ++i) sbase[i + 1] = sbase[i] + eng_[i]->shard_samples();
+            run_on_all([&](int i) { eng_[i]->rebase_shard_samples(sbase[i]); });
+            for (int i = 0; i < n; ++i) eng_[i]->shard_samples_dev(&src_soff[i], &src_samp[i]);
         }
         // gather on the first device: token records and offsets of every shard at their final positions
         CK(cudaSetDevice(dev_[0]));
@@ -355,6 +375,10 @@ class MultiEngine final : public Engine {
             grow_device(gather_links_, gather_links_cap_, nbase[n] * 8 + 8);
             if (marg) grow_device(gather_nprob_, gather_nprob_cap_, nbase[n] * 4 + 4);
         }
+        if (ns) {
+            grow_device(gather_soff_, gather_soff_cap_, (n_sent * ns + 1) * 8);
+            grow_device(gather_samples_, gather_samples_cap_, sbase[n] * 24 + 24);
+        }
         // the lattice pieces of shard i: {destination on the first device, source on device i, bytes}
         struct Piece {
             void* dst;
@@ -370,6 +394,15 @@ class MultiEngine final : public Engine {
                 v.push_back({static_cast<uint8_t*>(gather_links_) + nbase[i] * 8, src_links[i], nn * 8});
                 if (marg) v.push_back({static_cast<uint8_t*>(gather_nprob_) + nbase[i] * 4, src_nprob[i], nn * 4});
             }
+            return v;
+        };
+        auto samp_pieces = [&](int i) {  // the same for the samples
+            std::vector<Piece> v;
+            if (!ns) return v;
+            v.push_back({static_cast<uint8_t*>(gather_soff_) + cut[i] * ns * 8, src_soff[i],
+                         ((cut[i + 1] - cut[i]) * ns + (i == n - 1 ? 1 : 0)) * 8});
+            if (sbase[i + 1] > sbase[i])
+                v.push_back({static_cast<uint8_t*>(gather_samples_) + sbase[i] * 24, src_samp[i], (sbase[i + 1] - sbase[i]) * 24});
             return v;
         };
         std::vector<uint64_t> src_off(n), src_tok(n), src_tp(n), src_pp(n);
@@ -391,6 +424,8 @@ class MultiEngine final : public Engine {
             if (n_tok[0]) CK(cudaMemcpyAsync(dst_tp(0), reinterpret_cast<const void*>(src_tp[0]), n_tok[0] * 4, cudaMemcpyDeviceToDevice, stream_[0]));
             if (n_sh(0)) CK(cudaMemcpyAsync(dst_pp(0), reinterpret_cast<const void*>(src_pp[0]), n_sh(0) * 4, cudaMemcpyDeviceToDevice, stream_[0]));
         }
+        for (const Piece& p : samp_pieces(0))
+            CK(cudaMemcpyAsync(p.dst, reinterpret_cast<const void*>(p.src), p.bytes, cudaMemcpyDeviceToDevice, stream_[0]));
         for (const Piece& p : lat_pieces(0))
             CK(cudaMemcpyAsync(p.dst, reinterpret_cast<const void*>(p.src), p.bytes, cudaMemcpyDeviceToDevice, stream_[0]));
         if (n > 1 && nccl_) {
@@ -401,7 +436,8 @@ class MultiEngine final : public Engine {
                 NK(nccl_->Send(reinterpret_cast<const void*>(src_off[i]), off_bytes(i), ncclUint8, 0, comm_[i], stream_[i]));
                 if (marg && n_tok[i]) NK(nccl_->Send(reinterpret_cast<const void*>(src_tp[i]), n_tok[i] * 4, ncclUint8, 0, comm_[i], stream_[i]));
                 if (marg && n_sh(i)) NK(nccl_->Send(reinterpret_cast<const void*>(src_pp[i]), n_sh(i) * 4, ncclUint8, 0, comm_[i], stream_[i]));
-                const std::vector<Piece> lp = lat_pieces(i);
+                std::vector<Piece> lp = lat_pieces(i);
+                for (const Piece& p : samp_pieces(i)) lp.push_back(p);
                 for (const Piece& p : lp) NK(nccl_->Send(reinterpret_cast<const void*>(p.src), p.bytes, ncclUint8, 0, comm_[i], stream_[i]));
                 CK(cudaSetDevice(dev_[0]));
                 if (n_tok[i]) NK(nccl_->Recv(dst_tok(i), n_tok[i] * tb, ncclUint8, i, comm_[0], stream_[0]));
@@ -421,6 +457,8 @@ class MultiEngine final : public Engine {
                     CK(cudaMemcpyPeerAsync(dst_pp(i), dev_[0], reinterpret_cast<const void*>(src_pp[i]), dev_[i], n_sh(i) * 4, stream_[0]));
                 for (const Piece& p : lat_pieces(i))
                     CK(cudaMemcpyPeerAsync(p.dst, dev_[0], reinterpret_cast<const void*>(p.src), dev_[i], p.bytes, stream_[0]));
+                for (const Piece& p : samp_pieces(i))
+                    CK(cudaMemcpyPeerAsync(p.dst, dev_[0], reinterpret_cast<const void*>(p.src), dev_[i], p.bytes, stream_[0]));
             }
         }
         for (int i = 0; i < n; ++i) {
@@ -434,6 +472,8 @@ class MultiEngine final : public Engine {
         dev_marg_ = marg;
         dev_lat_ = lat;
         dev_nodes_ = nbase[n];
+        dev_samp_ = ns != 0;
+        dev_samples_ = sbase[n];
     }
 
     // ---- everything else is forwarded ------------------------------------------------------------------
@@ -461,6 +501,17 @@ class MultiEngine final : public Engine {
         for (auto& e : eng_) e->set_marginals(theta);
     }
     double marginals() const override { return eng_[0]->marginals(); }
+    void set_sampling(uint32_t n, double theta, uint64_t seed) override {
+        for (auto& e : eng_) e->set_sampling(n, theta, seed);  // the first refuses what all would
+    }
+    uint32_t sampling() const override { return eng_[0]->sampling(); }
+    void device_samples(uint64_t* d_sample_off, uint64_t* d_samples, uint64_t* n_tokens) const override {
+        if (dev_.size() == 1) return eng_[0]->device_samples(d_sample_off, d_samples, n_tokens);
+        if (!dev_samp_) throw Error(kInvalidArgument, "the last device-resident call ran without sampling");
+        if (d_sample_off) *d_sample_off = reinterpret_cast<uint64_t>(gather_soff_);
+        if (d_samples) *d_samples = reinterpret_cast<uint64_t>(gather_samples_);
+        if (n_tokens) *n_tokens = dev_samples_;
+    }
     int lattice() const override { return lattice_; }
     void device_marginals(uint64_t* d_token_prob, uint64_t* d_path_prob) const override {
         if (dev_.size() == 1) return eng_[0]->device_marginals(d_token_prob, d_path_prob);
@@ -510,6 +561,11 @@ class MultiEngine final : public Engine {
     void fetch_shard_lattice(uint64_t*, void*, void*, float*, uint64_t, bool) override { throw Error(kInternal, "not a shard engine"); }
     void rebase_shard_lattice(uint64_t) override { throw Error(kInternal, "not a shard engine"); }
     void shard_lattice(uint64_t*, uint64_t*, uint64_t*, uint64_t*) const override { throw Error(kInternal, "not a shard engine"); }
+    void set_sample_base(uint64_t) override { throw Error(kInternal, "not a shard engine"); }
+    uint64_t shard_samples() const override { throw Error(kInternal, "not a shard engine"); }
+    void fetch_shard_samples(uint64_t*, void*, uint64_t, bool) override { throw Error(kInternal, "not a shard engine"); }
+    void rebase_shard_samples(uint64_t) override { throw Error(kInternal, "not a shard engine"); }
+    void shard_samples_dev(uint64_t*, uint64_t*) const override { throw Error(kInternal, "not a shard engine"); }
     void rebase_shard(uint64_t) override { throw Error(kInternal, "not a shard engine"); }
     void shard_outputs(uint64_t*, uint64_t*) const override { throw Error(kInternal, "not a shard engine"); }
     int device() const override { return dev_[0]; }
@@ -535,6 +591,12 @@ class MultiEngine final : public Engine {
             cut[i] = std::max<uint64_t>(cut[i - 1], std::min<uint64_t>(uint64_t(p - off), n_sent));
         }
         return cut;
+    }
+
+    // The sample offsets of a whole batch are indexed in 32 bits (every shard checks its own part too).
+    void check_samples(uint64_t n_sent) const {
+        if (n_sent * sampling() >= 0xFFFFFFFFull)
+            throw Error(kInvalidArgument, "sampling: n_sent * n must stay below 2^32: split the batch or draw fewer samples");
     }
 
     static void grow_device(void*& p, size_t& cap, size_t bytes) {
@@ -600,7 +662,8 @@ class MultiEngine final : public Engine {
     }
 
     // A pooled pinned result for n_sent sentences and n_tokens tokens, and *text_bytes bytes of text when given.
-    HostResult* acquire(uint64_t n_sent, uint64_t n_tokens, const uint64_t* text_bytes, uint64_t n_nodes = 0) {
+    HostResult* acquire(uint64_t n_sent, uint64_t n_tokens, const uint64_t* text_bytes, uint64_t n_nodes = 0,
+                        uint64_t n_samples = 0) {
         HostResult* r = nullptr;
         if (!free_.empty()) {
             r = free_.back();
@@ -657,6 +720,16 @@ class MultiEngine final : public Engine {
             r->node_prob = static_cast<float*>(np);
             if (n_sent == 0) r->node_off[0] = 0;
         }
+        r->n_samp = sampling();
+        r->has_samp = r->n_samp != 0;
+        r->n_sample_tokens = n_samples;
+        if (r->has_samp) {
+            void* so = r->sample_off;
+            grow_pinned(so, r->cap_sample_off, (n_sent * r->n_samp + 1) * 8);
+            grow_pinned(r->samples, r->cap_samples, n_samples * 24);
+            r->sample_off = static_cast<uint64_t*>(so);
+            if (n_sent == 0) r->sample_off[0] = 0;
+        }
         if (n_sent == 0) r->tok_off[0] = 0;
         if (n_sent == 0 && text_bytes) r->text_off[0] = 0;
         return r;
@@ -693,6 +766,11 @@ class MultiEngine final : public Engine {
     int lattice_ = 0;  // option "lattice"
     bool dev_lat_ = false;
     uint64_t dev_nodes_ = 0;
+    void* gather_soff_ = nullptr;  // samples of a gathered device-resident batch
+    void* gather_samples_ = nullptr;
+    size_t gather_soff_cap_ = 0, gather_samples_cap_ = 0;
+    bool dev_samp_ = false;
+    uint64_t dev_samples_ = 0;
     float stage_ms_[kNumStages];
     uint64_t counters_[10];
     uint64_t launches_ = 0;
