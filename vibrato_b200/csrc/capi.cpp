@@ -449,12 +449,12 @@ int32_t vbt_result_view(const vbt_result* r, const uint64_t** tok_offsets, const
                         uint64_t* n_tokens) {
     return guarded([&] {
         need(r, "r");
-        if (toks && r->r->token_bytes != sizeof(vbt_token))
+        if (toks && r->r->out.token_bytes != sizeof(vbt_token))
             throw vbt::Error(vbt::kInvalidArgument, "compact result: read it with vbt_result_view_compact");
-        if (tok_offsets) *tok_offsets = r->r->tok_off;
-        if (toks) *toks = static_cast<const vbt_token*>(r->r->tokens);
+        if (tok_offsets) *tok_offsets = r->r->ptr<uint64_t>(vbt::kTokOff);
+        if (toks) *toks = r->r->ptr<const vbt_token>(vbt::kTokens);
         if (n_sent) *n_sent = r->r->n_sent;
-        if (n_tokens) *n_tokens = r->r->n_tokens;
+        if (n_tokens) *n_tokens = r->r->total[vbt::kGroupTokens];
     });
 }
 
@@ -462,23 +462,23 @@ int32_t vbt_result_view_compact(const vbt_result* r, const uint64_t** tok_offset
                                 uint64_t* n_tokens) {
     return guarded([&] {
         need(r, "r");
-        if (toks && r->r->token_bytes != sizeof(vbt_token16))
+        if (toks && r->r->out.token_bytes != sizeof(vbt_token16))
             throw vbt::Error(vbt::kInvalidArgument, "not a compact result: set the tokenizer option \"compact_tokens\" first");
-        if (tok_offsets) *tok_offsets = r->r->tok_off;
-        if (toks) *toks = static_cast<const vbt_token16*>(r->r->tokens);
+        if (tok_offsets) *tok_offsets = r->r->ptr<uint64_t>(vbt::kTokOff);
+        if (toks) *toks = r->r->ptr<const vbt_token16>(vbt::kTokens);
         if (n_sent) *n_sent = r->r->n_sent;
-        if (n_tokens) *n_tokens = r->r->n_tokens;
+        if (n_tokens) *n_tokens = r->r->total[vbt::kGroupTokens];
     });
 }
 
 int32_t vbt_result_text(const vbt_result* r, const uint64_t** text_offsets, const char** text, uint64_t* n_bytes) {
     return guarded([&] {
         need(r, "r");
-        if (!r->r->has_text)
+        if (!r->r->out.text)
             throw vbt::Error(vbt::kInvalidArgument, "no text: set the tokenizer option \"output_mode\" before tokenising");
-        if (text_offsets) *text_offsets = r->r->text_off;
-        if (text) *text = r->r->text;
-        if (n_bytes) *n_bytes = r->r->text_bytes;
+        if (text_offsets) *text_offsets = r->r->ptr<uint64_t>(vbt::kTextOff);
+        if (text) *text = r->r->ptr<const char>(vbt::kText);
+        if (n_bytes) *n_bytes = r->r->total[vbt::kGroupText];
     });
 }
 
@@ -580,10 +580,10 @@ int32_t vbt_tokenizer_set_marginals(vbt_tokenizer* t, double theta) {
 int32_t vbt_result_marginals(const vbt_result* r, const float** token_prob, const float** path_prob) {
     return guarded([&] {
         need(r, "r");
-        if (!r->r->has_marg)
+        if (!r->r->out.marg)
             throw vbt::Error(vbt::kInvalidArgument, "no marginals: switch them on with vbt_tokenizer_set_marginals before tokenising");
-        if (token_prob) *token_prob = r->r->token_prob;
-        if (path_prob) *path_prob = r->r->path_prob;
+        if (token_prob) *token_prob = r->r->ptr<const float>(vbt::kTokenProb);
+        if (path_prob) *path_prob = r->r->ptr<const float>(vbt::kPathProb);
     });
 }
 
@@ -598,13 +598,13 @@ int32_t vbt_result_lattice(const vbt_result* r, const uint64_t** node_offsets, c
                            const vbt_lattice_link** links, const float** node_prob, uint64_t* n_nodes) {
     return guarded([&] {
         need(r, "r");
-        if (!r->r->has_lat)
+        if (!r->r->out.lat)
             throw vbt::Error(vbt::kInvalidArgument, "no lattice: set the tokenizer option \"lattice\" before tokenising");
-        if (node_offsets) *node_offsets = r->r->node_off;
-        if (nodes) *nodes = static_cast<const vbt_token*>(r->r->nodes);
-        if (links) *links = static_cast<const vbt_lattice_link*>(r->r->links);
-        if (node_prob) *node_prob = r->r->has_marg ? r->r->node_prob : nullptr;
-        if (n_nodes) *n_nodes = r->r->n_nodes;
+        if (node_offsets) *node_offsets = r->r->ptr<uint64_t>(vbt::kNodeOff);
+        if (nodes) *nodes = r->r->ptr<const vbt_token>(vbt::kNodes);
+        if (links) *links = r->r->ptr<const vbt_lattice_link>(vbt::kLinks);
+        if (node_prob) *node_prob = r->r->out.marg ? r->r->ptr<const float>(vbt::kNodeProb) : nullptr;
+        if (n_nodes) *n_nodes = r->r->total[vbt::kGroupLattice];
     });
 }
 
@@ -627,11 +627,11 @@ int32_t vbt_result_samples(const vbt_result* r, const uint64_t** sample_offsets,
                            uint64_t* n_sample_tokens) {
     return guarded([&] {
         need(r, "r");
-        if (!r->r->has_samp)
+        if (!r->r->out.n_samp)
             throw vbt::Error(vbt::kInvalidArgument, "no samples: switch sampling on with vbt_tokenizer_set_sampling before tokenising");
-        if (sample_offsets) *sample_offsets = r->r->sample_off;
-        if (samples) *samples = static_cast<const vbt_token*>(r->r->samples);
-        if (n_sample_tokens) *n_sample_tokens = r->r->n_sample_tokens;
+        if (sample_offsets) *sample_offsets = r->r->ptr<uint64_t>(vbt::kSampleOff);
+        if (samples) *samples = r->r->ptr<const vbt_token>(vbt::kSamples);
+        if (n_sample_tokens) *n_sample_tokens = r->r->total[vbt::kGroupSamples];
     });
 }
 

@@ -31,37 +31,11 @@ void cuda_check(cudaError_t e, const char* what) {
 }
 #define CK(x) cuda_check((x), #x)
 
-struct DevBuf {
-    void* p = nullptr;
-    size_t cap = 0;
-    void ensure(size_t bytes, double slack = 1.0) {
-        if (bytes <= cap) return;
-        if (p) CK(cudaFree(p));
-        p = nullptr;
-        cap = 0;
-        size_t want = size_t(double(bytes) * slack) + 256;
-        CK(cudaMalloc(&p, want));
-        cap = want;
-    }
-    void release() {
-        if (p) cudaFree(p);
-        p = nullptr;
-        cap = 0;
-    }
-    template <typename T>
-    T* as() const {
-        return static_cast<T*>(p);
-    }
-};
-
 struct Control {  // one small block zeroed per batch and read back once
     unsigned long long pool_ctr;  // candidates
     unsigned long long seg_ctr;   // segments of the candidate pool
-    unsigned long long n_tokens;
     unsigned long long counters[kNumCounters];
-    unsigned long long text_bytes;  // output stage: the text total of the batch (or chunk)
-    unsigned long long n_nodes;     // lattice output: the node total of the batch (or chunk)
-    unsigned long long n_samples;   // sampling: the sample-token total of the batch (or chunk)
+    unsigned long long total[kNumGroups];  // records of each output group in the batch (or chunk)
     uint32_t flags;
     uint32_t total_slots;
 };
@@ -69,6 +43,12 @@ struct Control {  // one small block zeroed per batch and read back once
 // Entries the workspace must hold per batch: the segment pool and the lattice rows are sized from one learned count,
 // and a batch needs it to cover both its candidates and its segments (almost always fewer).
 static uint64_t pool_need(const Control& c) { return std::max<uint64_t>(c.pool_ctr, c.seg_ctr); }
+
+static Totals totals(const Control& c) {
+    Totals t;
+    for (int g = 0; g < kNumGroups; ++g) t[g] = c.total[g];
+    return t;
+}
 
 // Output iterator for the row-offset scan: writes {offset, offset} (an empty row) into the 8-byte row metadata so that
 // no separate initialisation pass is needed.
@@ -147,11 +127,11 @@ __global__ void k_add_u64(unsigned long long* dst, const unsigned long long* src
 
 __global__ void k_publish_totals(const uint32_t* slot_off, const unsigned long long* tok_off, uint32_t n_sent, Control* c) {
     c->total_slots = slot_off[n_sent];
-    c->n_tokens = tok_off[n_sent];
+    c->total[kGroupTokens] = tok_off[n_sent];
 }
 
-// Chunked host batches: token (and text) offsets of a chunk become global by adding the tokens (text bytes) of all
-// earlier chunks (kept in a device-resident running total so the host never has to wait for it).
+// Chunked host batches: a group's offsets of a chunk become global by adding the group's records of all earlier
+// chunks (kept in a device-resident running total so the host never has to wait for it).
 __global__ void k_add_base(unsigned long long* tok_off, uint32_t n_plus_1, const unsigned long long* base) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n_plus_1) tok_off[i] += *base;
@@ -188,14 +168,9 @@ struct DevBounds {
 };
 
 struct OutSlot {  // where one (chunk of a) batch leaves its results; two of them alternate in chunked runs
-    DevBuf tok_off, tokens, ctrl;
-    DevBuf sent_len, text_off, text;  // output stage (k_format_*)
-    DevBuf token_prob, path_prob;     // marginals
-    bool marg = false;                // the (chunk of a) batch in this slot was run with marginals
-    DevBuf node_off, nodes, links, node_prob;  // lattice output (LatticeArgs)
-    bool lat = false;                          // the (chunk of a) batch in this slot was run with the lattice
-    DevBuf sample_off, samples;                // sampling (SampleArgs)
-    bool samp = false;                         // the (chunk of a) batch in this slot was run with sampling
+    DevBuf buf[kNumArrays];  // the output arrays; path_prob is written by the forward pass of sampling too
+    DevBuf ctrl, sent_len;   // sent_len: output stage (k_format_*)
+    Outputs made;            // the arrays the (chunk of a) batch in this slot produced
     Control* h_ctrl = nullptr;
     cudaEvent_t ev[kNumStages + 1];
     cudaEvent_t done = nullptr, drained = nullptr;
@@ -228,10 +203,7 @@ class EngineImpl final : public Engine {
         CK(cudaEventCreateWithFlags(&in_done_, cudaEventDisableTiming));
         CK(cudaStreamCreateWithFlags(&aux_stream_, cudaStreamNonBlocking));
         for (auto& e : base_ready_) CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-        tok_base_.ensure(8);
-        text_base_.ensure(8);
-        node_base_.ensure(8);
-        samp_base_.ensure(8);
+        base_.ensure(kNumGroups * 8);
         BlobHeader h;
         if (host_blob) {
             if (n_bytes < sizeof(BlobHeader)) throw Error(kInvalidArgument, "dictionary image too small");
@@ -349,9 +321,9 @@ class EngineImpl final : public Engine {
         cudaStreamSynchronize(in_stream_);
         cudaStreamSynchronize(out_stream_);
         for (auto& o : out_) {
-            for (DevBuf* b : {&o.tok_off, &o.tokens, &o.ctrl, &o.sent_len, &o.text_off, &o.text, &o.token_prob, &o.path_prob,
-                              &o.node_off, &o.nodes, &o.links, &o.node_prob, &o.sample_off, &o.samples})
-                b->release();
+            for (DevBuf& b : o.buf) b.release();
+            o.ctrl.release();
+            o.sent_len.release();
             pinned_free(o.h_ctrl);
             for (auto& ev : o.ev) cudaEventDestroy(ev);
             cudaEventDestroy(o.done);
@@ -364,10 +336,7 @@ class EngineImpl final : public Engine {
         cudaEventDestroy(in_done_);
         cudaStreamDestroy(in_stream_);
         cudaStreamDestroy(out_stream_);
-        tok_base_.release();
-        text_base_.release();
-        node_base_.release();
-        samp_base_.release();
+        base_.release();
         for (DevBuf* b : {&fmt_prog_, &ft_keep_, &ft_off_, &ft_bytes_}) b->release();
         for (auto* b : {&blob_own_, &in_utf8_, &in_off_, &in_bnd_off_, &in_bnd_, &connid_, &connid_try_}) b->release();
         for (auto& w : ws_) w.release();
@@ -380,18 +349,6 @@ class EngineImpl final : public Engine {
         cudaStreamSynchronize(aux_stream_);
         cudaStreamDestroy(aux_stream_);
         for (auto& e : base_ready_) cudaEventDestroy(e);
-        for (auto& r : pool_) {
-            pinned_free(r->tok_off);
-            pinned_free(r->tokens);
-            pinned_free(r->text_off);
-            pinned_free(r->text);
-            pinned_free(r->token_prob);
-            pinned_free(r->path_prob);
-            for (void* p : {static_cast<void*>(r->node_off), r->nodes, r->links, static_cast<void*>(r->node_prob)}) pinned_free(p);
-            pinned_free(r->sample_off);
-            pinned_free(r->samples);
-            delete r;
-        }
         cudaStreamDestroy(own_stream_);
     }
 
@@ -514,27 +471,26 @@ class EngineImpl final : public Engine {
     }
     uint32_t sampling() const override { return samp_n_; }
     void device_samples(uint64_t* d_sample_off, uint64_t* d_samples, uint64_t* n_tokens) const override {
-        if (!dev_samp_) throw Error(kInvalidArgument, "the last device-resident call ran without sampling");
-        if (d_sample_off) *d_sample_off = reinterpret_cast<uint64_t>(out_[0].sample_off.p);
-        if (d_samples) *d_samples = reinterpret_cast<uint64_t>(out_[0].samples.p);
-        if (n_tokens) *n_tokens = out_[0].h_ctrl->n_samples;
+        if (!made_.has(kSamples)) throw Error(kInvalidArgument, "the last device-resident call ran without sampling");
+        put_address(d_sample_off, made_, out_[0].buf, kSampleOff);
+        put_address(d_samples, made_, out_[0].buf, kSamples);
+        if (n_tokens) *n_tokens = out_[0].h_ctrl->total[kGroupSamples];
     }
     double marginals() const override { return theta_; }
     int lattice() const override { return lattice_; }
     void device_marginals(uint64_t* d_token_prob, uint64_t* d_path_prob) const override {
-        if (!dev_marg_) throw Error(kInvalidArgument, "the last device-resident call ran without marginals");
-        if (d_token_prob) *d_token_prob = reinterpret_cast<uint64_t>(out_[0].token_prob.p);
-        if (d_path_prob) *d_path_prob = reinterpret_cast<uint64_t>(out_[0].path_prob.p);
+        if (!made_.has(kTokenProb)) throw Error(kInvalidArgument, "the last device-resident call ran without marginals");
+        put_address(d_token_prob, made_, out_[0].buf, kTokenProb);
+        put_address(d_path_prob, made_, out_[0].buf, kPathProb);
     }
     void device_lattice(uint64_t* d_node_off, uint64_t* d_nodes, uint64_t* d_links, uint64_t* d_node_prob,
                         uint64_t* n_nodes) const override {
-        if (!dev_lat_) throw Error(kInvalidArgument, "the last device-resident call ran without the lattice");
-        const OutSlot& o = out_[0];
-        if (d_node_off) *d_node_off = reinterpret_cast<uint64_t>(o.node_off.p);
-        if (d_nodes) *d_nodes = reinterpret_cast<uint64_t>(o.nodes.p);
-        if (d_links) *d_links = reinterpret_cast<uint64_t>(o.links.p);
-        if (d_node_prob) *d_node_prob = o.marg ? reinterpret_cast<uint64_t>(o.node_prob.p) : 0;
-        if (n_nodes) *n_nodes = o.h_ctrl->n_nodes;
+        if (!made_.has(kNodes)) throw Error(kInvalidArgument, "the last device-resident call ran without the lattice");
+        put_address(d_node_off, made_, out_[0].buf, kNodeOff);
+        put_address(d_nodes, made_, out_[0].buf, kNodes);
+        put_address(d_links, made_, out_[0].buf, kLinks);
+        put_address(d_node_prob, made_, out_[0].buf, kNodeProb);
+        if (n_nodes) *n_nodes = out_[0].h_ctrl->total[kGroupLattice];
     }
     void set_stream(uint64_t stream) override {
         cudaStreamSynchronize(stream_);
@@ -563,15 +519,13 @@ class EngineImpl final : public Engine {
         if (bnd && bnd->n == 0 && device_offsets_zero(bnd->off, n_sent)) bnd = nullptr;  // no boundary at all
         DevBounds bd;
         if (bnd) bd = DevBounds{reinterpret_cast<const unsigned long long*>(bnd->off), bnd->bnd, bnd->n};
-        dev_marg_ = dev_lat_ = dev_samp_ = false;
+        made_ = Outputs{};
         run_whole(reinterpret_cast<const uint8_t*>(d_utf8), reinterpret_cast<const unsigned long long*>(d_byte_off),
                   uint32_t(n_sent), n_bytes, bd);
-        *d_tok_off = reinterpret_cast<uint64_t>(out_[0].tok_off.p);
-        *d_tokens = reinterpret_cast<uint64_t>(out_[0].tokens.p);
-        *n_tokens = out_[0].h_ctrl->n_tokens;
-        dev_marg_ = out_[0].marg;
-        dev_lat_ = out_[0].lat;
-        dev_samp_ = out_[0].samp;
+        *d_tok_off = reinterpret_cast<uint64_t>(out_[0].buf[kTokOff].p);
+        *d_tokens = reinterpret_cast<uint64_t>(out_[0].buf[kTokens].p);
+        *n_tokens = out_[0].h_ctrl->total[kGroupTokens];
+        made_ = out_[0].made;
     }
 
     // Host path.  Large batches are cut into chunks that flow through three streams: the H2D copy of
@@ -617,7 +571,7 @@ class EngineImpl final : public Engine {
                     // Small batches (a per-sentence Worker loop ends up here) are all latency: the result copies are
                     // queued behind the kernels with an upper bound for the token count (a token spans >= 1 byte), so
                     // that the call makes ONE host synchronisation instead of two.
-                    HostResult* r = acquire(n_sent, n_bytes);
+                    HostResult* r = pool_.acquire(outputs(), n_sent, Totals{n_bytes, 0, 0, 0});
                     eager_sink_ = r;
                     try {
                         run_whole(d_utf8, d_off, n_sent, n_bytes, bd);
@@ -627,32 +581,14 @@ class EngineImpl final : public Engine {
                         throw;
                     }
                     eager_sink_ = nullptr;
-                    r->n_tokens = out_[0].h_ctrl->n_tokens;
-                    r->has_text = false;
+                    r->total[kGroupTokens] = out_[0].h_ctrl->total[kGroupTokens];
                     return r;
                 }
                 run_whole(d_utf8, d_off, n_sent, n_bytes, bd);
+                if (fmt) format_whole(d_utf8, d_off, n_sent);
                 OutSlot& o = out_[0];
-                HostResult* r = acquire(n_sent, o.h_ctrl->n_tokens);
-                CK(cudaMemcpyAsync(r->tok_off, o.tok_off.p, (size_t(n_sent) + 1) * 8, cudaMemcpyDeviceToHost, stream_));
-                if (r->n_tokens) CK(cudaMemcpyAsync(r->tokens, o.tokens.p, r->n_tokens * tok_bytes_, cudaMemcpyDeviceToHost, stream_));
-                if (r->has_marg) {
-                    if (r->n_tokens)
-                        CK(cudaMemcpyAsync(r->token_prob, o.token_prob.p, r->n_tokens * 4, cudaMemcpyDeviceToHost, stream_));
-                    if (n_sent) CK(cudaMemcpyAsync(r->path_prob, o.path_prob.p, size_t(n_sent) * 4, cudaMemcpyDeviceToHost, stream_));
-                }
-                if (r->has_lat) {
-                    r->n_nodes = o.h_ctrl->n_nodes;
-                    ensure_lat_host(r, n_sent, r->n_nodes);
-                    copy_lattice(o, r, 0, 0, n_sent, true, stream_);
-                }
-                if (r->has_samp) {
-                    r->n_sample_tokens = o.h_ctrl->n_samples;
-                    ensure_samp_host(r, n_sent, r->n_sample_tokens);
-                    copy_samples(o, r, 0, 0, n_sent, true, stream_);
-                }
-                r->has_text = false;
-                if (fmt) format_text(d_utf8, d_off, n_sent, r);
+                HostResult* r = pool_.acquire(outputs(), n_sent, totals(*o.h_ctrl));
+                place(o, r, 0, n_sent, r->total, Totals{}, true, stream_);
                 CK(cudaStreamSynchronize(stream_));
                 return r;
             }
@@ -682,32 +618,23 @@ class EngineImpl final : public Engine {
             const uint32_t n_ws = dual_stream_ ? 2 : 1;
             for (uint32_t i = 0; i < n_ws; ++i)
                 ensure_workspace(ws_[i], max_chunk_sent, max_chunk_bytes, bd.off != nullptr);  // sized once: no cudaMalloc in the pipeline
-            for (auto& o : out_) {
-                o.tok_off.ensure((size_t(max_chunk_sent) + 1) * 8, 1.25);
-                o.tokens.ensure(size_t(max_chunk_bytes) * 24 + 24, 1.25);
-                ensure_marg_out(o, max_chunk_sent, max_chunk_bytes);
-                ensure_lat_out(o, ws_[0], max_chunk_sent);
-                ensure_samp_out(o, max_chunk_sent);
-            }
-            // a pinned result sized from the learned tokens-per-byte ratio (grown below if short)
-            HostResult* r = acquire(n_sent, uint64_t(double(n_bytes) * tok_per_byte_) + 1024);
-            if (r->has_lat) ensure_lat_host(r, n_sent, uint64_t(double(n_bytes) * node_per_byte_) + 1024);
-            if (r->has_samp) ensure_samp_host(r, n_sent, uint64_t(double(n_bytes) * tok_per_byte_ * samp_n_) + 1024);
+            for (auto& o : out_) ensure_out(o, ws_[0], max_chunk_sent, max_chunk_bytes);
             // output stage: each slot's text buffer holds the text a chunk is expected to produce (at most 4 bytes per
             // sentence plus the learned ratio per input byte); a chunk with more text flags itself and the batch is
             // re-run with the ratio it measured
             const double text_ratio = text_ratio_ref();
-            if (fmt) {
+            if (fmt)
                 for (int i = 0; i < 2; ++i) {
                     ensure_format(out_[i], ws_[dual_stream_ ? i : 0], max_chunk_sent);
-                    out_[i].text.ensure(size_t(double(max_chunk_bytes) * text_ratio) + size_t(max_chunk_sent) * text_per_sent_ + 4096);
+                    out_[i].buf[kText].ensure(size_t(double(max_chunk_bytes) * text_ratio) + size_t(max_chunk_sent) * text_per_sent_ + 4096);
                 }
-                ensure_text(r, n_sent, uint64_t(double(n_bytes) * text_ratio) + uint64_t(n_sent) * text_per_sent_ + 1024);
-                CK(cudaMemsetAsync(text_base_.p, 0, 8, stream_));
-            }
-            CK(cudaMemsetAsync(tok_base_.p, 0, 8, stream_));
-            if (lattice_) CK(cudaMemsetAsync(node_base_.p, 0, 8, stream_));
-            if (samp_n_) CK(cudaMemsetAsync(samp_base_.p, 0, 8, stream_));
+            // a pinned result sized from the learned ratios per input byte (grown below if short)
+            HostResult* r = pool_.acquire(outputs(), n_sent,
+                                          Totals{uint64_t(double(n_bytes) * tok_per_byte_) + 1024,
+                                                 uint64_t(double(n_bytes) * text_ratio) + uint64_t(n_sent) * text_per_sent_ + 1024,
+                                                 uint64_t(double(n_bytes) * node_per_byte_) + 1024,
+                                                 uint64_t(double(n_bytes) * tok_per_byte_ * samp_n_) + 1024});
+            CK(cudaMemsetAsync(base_.p, 0, kNumGroups * 8, stream_));
             connid_begin(stream_);
             h2d(in_off_.p, off, (size_t(n_sent) + 1) * 8, stream_, off_pinned && off == byte_off);
             CK(cudaEventRecord(in_done_, stream_));
@@ -716,7 +643,7 @@ class EngineImpl final : public Engine {
             std::memset(stage_ms_, 0, sizeof(stage_ms_));
             std::memset(counters_, 0, sizeof(counters_));
             launches_ = 0;
-            uint64_t tok_total = 0, text_total = 0, node_total = 0, samp_total = 0;
+            Totals sum{};  // records per group of the chunks drained so far
             double text_need = 0;  // text bytes per input byte beyond text_per_sent_ per sentence, largest over the sound chunks
             uint32_t route = kRouteNone;
             bool overflow = false, bad_utf8 = false, bad_offsets = false, slots_overflow = false, text_overflow = false;
@@ -758,75 +685,24 @@ class EngineImpl final : public Engine {
                 if (counting_)
                     for (int i = 0; i < kNumCounters; ++i) counters_[i] += o.h_ctrl->counters[i];
                 pool_need_ = std::max<uint64_t>(pool_need_, pool_need(*o.h_ctrl));
-                const uint64_t nt = o.h_ctrl->n_tokens, nx = fmt ? o.h_ctrl->text_bytes : 0;
-                const uint64_t nn = lattice_ ? o.h_ctrl->n_nodes : 0;
-                const uint64_t ns = samp_n_ ? o.h_ctrl->n_samples : 0;
+                const Totals count = totals(*o.h_ctrl);
                 if (fmt && !(o.h_ctrl->flags & (kFlagsStandDown | kFlagUtf8Error | kFlagPoolOverflow)))
-                    text_need = std::max(text_need, (double(nx) - double(text_per_sent_) * (s1 - s0)) / double(std::max<uint64_t>(1, off[s1] - off[s0])));
+                    text_need = std::max(text_need, (double(count[kGroupText]) - double(text_per_sent_) * (s1 - s0)) /
+                                                        double(std::max<uint64_t>(1, off[s1] - off[s0])));
                 if (!overflow && !text_overflow && !bad_utf8 && !bad_offsets && !bad_bounds) {
-                    if ((tok_total + nt) * tok_bytes_ > r->cap_tok) {  // rare: grow the pinned buffer, keep what is there
+                    // offsets are global already (base_); a record array that is short grows (rare), keeping what it
+                    // holds once the copies into it have landed
+                    for (int a = 0; a < kNumArrays; ++a) {
+                        if (!r->out.has(a) || kArrays[a].kind != kRecords) continue;
+                        const uint64_t keep = r->out.at(a, 0, sum), need = keep + r->out.bytes(a, 0, count, false);
+                        if (need <= r->buf[a].cap) continue;
                         CK(cudaStreamSynchronize(out_stream_));
-                        size_t cap = size_t(double((tok_total + nt) * 24) * 1.5) + 4096;
-                        void* bigger = pinned_alloc(cap);
-                        std::memcpy(bigger, r->tokens, tok_total * tok_bytes_);
-                        pinned_free(r->tokens);
-                        r->tokens = bigger;
-                        r->cap_tok = cap;
+                        r->buf[a].grow(need, keep);
                     }
-                    if (r->has_marg && (tok_total + nt) * 4 > r->cap_tprob) {  // the same for the token marginals
-                        CK(cudaStreamSynchronize(out_stream_));
-                        size_t cap = size_t(double((tok_total + nt) * 4) * 1.5) + 4096;
-                        float* bigger = static_cast<float*>(pinned_alloc(cap));
-                        std::memcpy(bigger, r->token_prob, tok_total * 4);
-                        pinned_free(r->token_prob);
-                        r->token_prob = bigger;
-                        r->cap_tprob = cap;
-                    }
-                    const bool last = s1 == n_sent;
-                    CK(cudaMemcpyAsync(r->tok_off + s0, o.tok_off.p, (size_t(s1 - s0) + (last ? 1 : 0)) * 8,
-                                       cudaMemcpyDeviceToHost, out_stream_));
-                    if (nt)
-                        CK(cudaMemcpyAsync(static_cast<uint8_t*>(r->tokens) + tok_total * tok_bytes_, o.tokens.p, nt * tok_bytes_,
-                                           cudaMemcpyDeviceToHost, out_stream_));
-                    if (r->has_marg) {  // at the same offsets as the token records
-                        if (nt) CK(cudaMemcpyAsync(r->token_prob + tok_total, o.token_prob.p, nt * 4, cudaMemcpyDeviceToHost, out_stream_));
-                        if (s1 > s0)
-                            CK(cudaMemcpyAsync(r->path_prob + s0, o.path_prob.p, size_t(s1 - s0) * 4, cudaMemcpyDeviceToHost, out_stream_));
-                    }
-                    if (r->has_lat) {  // node offsets are global already (node_base_); the arrays grow like the tokens
-                        if (!lat_fits(r, node_total + nn)) {
-                            CK(cudaStreamSynchronize(out_stream_));
-                            grow_lat_host(r, size_t(double(node_total + nn) * 1.5) + 4096, node_total);
-                        }
-                        copy_lattice(o, r, node_total, s0, s1 - s0, last, out_stream_);
-                    }
-                    if (r->has_samp) {  // sample offsets are global already (samp_base_); the records grow like the tokens
-                        if ((samp_total + ns) * 24 > r->cap_samples) {
-                            CK(cudaStreamSynchronize(out_stream_));
-                            grow_samp_host(r, size_t(double(samp_total + ns) * 1.5) + 4096, samp_total);
-                        }
-                        copy_samples(o, r, samp_total, s0, s1 - s0, last, out_stream_);
-                    }
-                    if (fmt) {
-                        if (text_total + nx + 1 > r->cap_text) {  // grown like the token buffer
-                            CK(cudaStreamSynchronize(out_stream_));
-                            size_t cap = size_t(double(text_total + nx) * 1.5) + 4096;
-                            char* bigger = static_cast<char*>(pinned_alloc(cap));
-                            std::memcpy(bigger, r->text, text_total);
-                            pinned_free(r->text);
-                            r->text = bigger;
-                            r->cap_text = cap;
-                        }
-                        CK(cudaMemcpyAsync(r->text_off + s0, o.text_off.p, (size_t(s1 - s0) + (last ? 1 : 0)) * 8,
-                                           cudaMemcpyDeviceToHost, out_stream_));
-                        if (nx) CK(cudaMemcpyAsync(r->text + text_total, o.text.p, nx, cudaMemcpyDeviceToHost, out_stream_));
-                    }
+                    place(o, r, s0, s1 - s0, count, sum, s1 == n_sent, out_stream_);
                 }
                 CK(cudaEventRecord(o.drained, out_stream_));
-                tok_total += nt;
-                text_total += nx;
-                node_total += nn;
-                samp_total += ns;
+                for (int g = 0; g < kNumGroups; ++g) sum[g] += count[g];
             };
             pool_need_ = 0;
             for (uint32_t c = 0; c < n_chunks; ++c) {
@@ -840,9 +716,8 @@ class EngineImpl final : public Engine {
                 if (c >= 2) CK(cudaStreamWaitEvent(w.stream, o.drained, 0));  // slot reused: its D2H must be done
                 DevBounds cb = bd;  // the chunk's slice of the boundary offsets (they index the whole bnd array)
                 if (cb.off) cb.off += s0;
-                enqueue(w, d_utf8, d_off + s0, s1 - s0, off[s1] - off[s0], o, tok_base_.as<unsigned long long>(),
-                        fmt ? text_base_.as<unsigned long long>() : nullptr, c >= 1 ? base_ready_[(c - 1) & 1] : nullptr,
-                        base_ready_[c & 1], cb, s0);
+                enqueue(w, d_utf8, d_off + s0, s1 - s0, off[s1] - off[s0], o, base_.as<unsigned long long>(),
+                        c >= 1 ? base_ready_[(c - 1) & 1] : nullptr, base_ready_[c & 1], cb, s0);
                 if (!utf8_pinned && c + 1 < n_chunks) issue_h2d(c + 1);
                 if (c >= 1) drain(c - 1);
             }
@@ -874,28 +749,22 @@ class EngineImpl final : public Engine {
             }
             if (max_chunk_bytes)
                 cand_per_byte_ = std::max(0.25, double(pool_need_) / double(max_chunk_bytes) * 1.25);
-            if (n_bytes) tok_per_byte_ = std::max(0.02, double(tok_total) / double(n_bytes) * 1.1);
+            if (n_bytes) tok_per_byte_ = std::max(0.02, double(sum[kGroupTokens]) / double(n_bytes) * 1.1);
             if (n_bytes) chars_per_byte_ = std::min(1.0, double(slots_seen - n_sent) / double(n_bytes) * 1.10);
             if (fmt) text_ratio_ref() = std::max(0.5, text_need * 1.25);
-            if (n_bytes && lattice_) node_per_byte_ = std::max(0.1, double(node_total) / double(n_bytes) * 1.1);
+            if (n_bytes && lattice_) node_per_byte_ = std::max(0.1, double(sum[kGroupLattice]) / double(n_bytes) * 1.1);
             connid_commit(stream_);
             last_route_ = route;
-            r->n_tokens = tok_total;
-            r->n_nodes = node_total;
-            r->n_sample_tokens = samp_total;
-            r->has_text = fmt;
-            r->text_bytes = text_total;
+            r->total = sum;
             return r;
         }
     }
 
-    void release(HostResult* r) override {
-        if (r) pool_free_.push_back(r);
-    }
+    void release(HostResult* r) override { pool_.release(r); }
 
     // ---- shard-level entry points (multi_engine.cu) -------------------------------------------------
-    uint64_t run_shard(const char* utf8, const uint64_t* byte_off, uint64_t n_sent64, int src_device, uint64_t* text_bytes,
-                       const Bounds* bnd) override {
+    Totals run_shard(const char* utf8, const uint64_t* byte_off, uint64_t n_sent64, int src_device, uint64_t first_sentence,
+                     bool with_text, const Bounds* bnd) override {
         CK(cudaSetDevice(device_));
         const uint64_t first = n_sent64 ? byte_off[0] : 0;
         const uint64_t n_bytes = n_sent64 ? byte_off[n_sent64] - first : 0;
@@ -921,124 +790,24 @@ class EngineImpl final : public Engine {
             else
                 h2d(in_utf8_.p, utf8 + first, n_bytes, stream_, is_pinned(utf8 + first));
         }
-        run_whole(in_utf8_.as<uint8_t>(), in_off_.as<unsigned long long>(), n_sent, n_bytes, bd, sample_base_);
+        run_whole(in_utf8_.as<uint8_t>(), in_off_.as<unsigned long long>(), n_sent, n_bytes, bd, first_sentence);
         shard_n_sent_ = n_sent;
-        shard_text_ = text_bytes && output_mode_ != kOutNone;
-        shard_text_bytes_ = shard_text_ ? format_whole(in_utf8_.as<uint8_t>(), in_off_.as<unsigned long long>(), n_sent) : 0;
-        if (text_bytes) *text_bytes = shard_text_bytes_;
-        return out_[0].h_ctrl->n_tokens;
+        if (with_text && output_mode_ != kOutNone) format_whole(in_utf8_.as<uint8_t>(), in_off_.as<unsigned long long>(), n_sent);
+        return totals(*out_[0].h_ctrl);
     }
-    void rebase_shard(uint64_t tok_base) override {
+    void rebase_shard(const Totals& base) override {
         CK(cudaSetDevice(device_));
-        if (tok_base)
-            k_add_value<<<(shard_n_sent_ + 256) / 256, 256, 0, stream_>>>(out_[0].tok_off.as<unsigned long long>(),
-                                                                         shard_n_sent_ + 1, tok_base);
+        add_bases(base);
         CK(cudaStreamSynchronize(stream_));
     }
-    void fetch_shard(uint64_t* h_tok_off, void* h_tokens, uint64_t tok_base, bool last, uint64_t* h_text_off, char* h_text,
-                     uint64_t text_base, float* h_token_prob, float* h_path_prob) override {
+    void fetch_shard(HostResult* r, uint64_t first_sentence, const Totals& base, bool last) override {
         CK(cudaSetDevice(device_));
-        OutSlot& o = out_[0];
-        if (tok_base)
-            k_add_value<<<(shard_n_sent_ + 256) / 256, 256, 0, stream_>>>(o.tok_off.as<unsigned long long>(), shard_n_sent_ + 1,
-                                                                         tok_base);
-        CK(cudaMemcpyAsync(h_tok_off, o.tok_off.p, (size_t(shard_n_sent_) + (last ? 1 : 0)) * 8, cudaMemcpyDeviceToHost, stream_));
-        if (o.h_ctrl->n_tokens)
-            CK(cudaMemcpyAsync(h_tokens, o.tokens.p, o.h_ctrl->n_tokens * tok_bytes_, cudaMemcpyDeviceToHost, stream_));
-        if (h_token_prob) {
-            if (!o.marg) throw Error(kInternal, "the shard was run without marginals");
-            if (o.h_ctrl->n_tokens)
-                CK(cudaMemcpyAsync(h_token_prob, o.token_prob.p, o.h_ctrl->n_tokens * 4, cudaMemcpyDeviceToHost, stream_));
-            if (shard_n_sent_) CK(cudaMemcpyAsync(h_path_prob, o.path_prob.p, size_t(shard_n_sent_) * 4, cudaMemcpyDeviceToHost, stream_));
-        }
-        if (h_text_off) {
-            if (!shard_text_) throw Error(kInternal, "the shard was run without its text");
-            unsigned long long* text_off = o.text_off.as<unsigned long long>();
-            const uint64_t n_text = shard_text_bytes_;
-            if (text_base) k_add_value<<<(shard_n_sent_ + 256) / 256, 256, 0, stream_>>>(text_off, shard_n_sent_ + 1, text_base);
-            CK(cudaMemcpyAsync(h_text_off, text_off, (size_t(shard_n_sent_) + (last ? 1 : 0)) * 8, cudaMemcpyDeviceToHost, stream_));
-            if (n_text) CK(cudaMemcpyAsync(h_text, o.text.p, n_text, cudaMemcpyDeviceToHost, stream_));
-        }
+        add_bases(base);
+        place(out_[0], r, first_sentence, shard_n_sent_, totals(*out_[0].h_ctrl), base, last, stream_);
         CK(cudaStreamSynchronize(stream_));
     }
-    void shard_outputs(uint64_t* d_tok_off, uint64_t* d_tokens) const override {
-        *d_tok_off = reinterpret_cast<uint64_t>(out_[0].tok_off.p);
-        *d_tokens = reinterpret_cast<uint64_t>(out_[0].tokens.p);
-    }
-    void shard_marginals(uint64_t* d_token_prob, uint64_t* d_path_prob) const override {
-        if (!out_[0].marg) throw Error(kInternal, "the shard was run without marginals");
-        *d_token_prob = reinterpret_cast<uint64_t>(out_[0].token_prob.p);
-        *d_path_prob = reinterpret_cast<uint64_t>(out_[0].path_prob.p);
-    }
-    uint64_t shard_nodes() const override {
-        if (!out_[0].lat) throw Error(kInternal, "the shard was run without the lattice");
-        return out_[0].h_ctrl->n_nodes;
-    }
-    void fetch_shard_lattice(uint64_t* h_node_off, void* h_nodes, void* h_links, float* h_node_prob, uint64_t node_base,
-                             bool last) override {
-        CK(cudaSetDevice(device_));
-        OutSlot& o = out_[0];
-        if (!o.lat) throw Error(kInternal, "the shard was run without the lattice");
-        if (node_base)
-            k_add_value<<<(shard_n_sent_ + 256) / 256, 256, 0, stream_>>>(o.node_off.as<unsigned long long>(), shard_n_sent_ + 1,
-                                                                         node_base);
-        const uint64_t nn = o.h_ctrl->n_nodes;
-        CK(cudaMemcpyAsync(h_node_off, o.node_off.p, (size_t(shard_n_sent_) + (last ? 1 : 0)) * 8, cudaMemcpyDeviceToHost, stream_));
-        if (nn) {
-            CK(cudaMemcpyAsync(h_nodes, o.nodes.p, nn * 24, cudaMemcpyDeviceToHost, stream_));
-            CK(cudaMemcpyAsync(h_links, o.links.p, nn * 8, cudaMemcpyDeviceToHost, stream_));
-            if (h_node_prob) {
-                if (!o.marg) throw Error(kInternal, "the shard was run without marginals");
-                CK(cudaMemcpyAsync(h_node_prob, o.node_prob.p, nn * 4, cudaMemcpyDeviceToHost, stream_));
-            }
-        }
-        CK(cudaStreamSynchronize(stream_));
-    }
-    void rebase_shard_lattice(uint64_t node_base) override {
-        CK(cudaSetDevice(device_));
-        if (node_base)
-            k_add_value<<<(shard_n_sent_ + 256) / 256, 256, 0, stream_>>>(out_[0].node_off.as<unsigned long long>(),
-                                                                         shard_n_sent_ + 1, node_base);
-        CK(cudaStreamSynchronize(stream_));
-    }
-    void shard_lattice(uint64_t* d_node_off, uint64_t* d_nodes, uint64_t* d_links, uint64_t* d_node_prob) const override {
-        const OutSlot& o = out_[0];
-        if (!o.lat) throw Error(kInternal, "the shard was run without the lattice");
-        *d_node_off = reinterpret_cast<uint64_t>(o.node_off.p);
-        *d_nodes = reinterpret_cast<uint64_t>(o.nodes.p);
-        *d_links = reinterpret_cast<uint64_t>(o.links.p);
-        *d_node_prob = o.marg ? reinterpret_cast<uint64_t>(o.node_prob.p) : 0;
-    }
-    void set_sample_base(uint64_t first_sentence) override { sample_base_ = first_sentence; }
-    uint64_t shard_samples() const override {
-        if (!out_[0].samp) throw Error(kInternal, "the shard was run without sampling");
-        return out_[0].h_ctrl->n_samples;
-    }
-    void fetch_shard_samples(uint64_t* h_sample_off, void* h_samples, uint64_t sample_base, bool last) override {
-        CK(cudaSetDevice(device_));
-        OutSlot& o = out_[0];
-        if (!o.samp) throw Error(kInternal, "the shard was run without sampling");
-        const uint64_t walks = uint64_t(shard_n_sent_) * samp_n_;
-        if (sample_base)
-            k_add_value<<<unsigned((walks + 256) / 256), 256, 0, stream_>>>(o.sample_off.as<unsigned long long>(), uint32_t(walks + 1),
-                                                                            sample_base);
-        CK(cudaMemcpyAsync(h_sample_off, o.sample_off.p, (walks + (last ? 1 : 0)) * 8, cudaMemcpyDeviceToHost, stream_));
-        if (o.h_ctrl->n_samples)
-            CK(cudaMemcpyAsync(h_samples, o.samples.p, o.h_ctrl->n_samples * 24, cudaMemcpyDeviceToHost, stream_));
-        CK(cudaStreamSynchronize(stream_));
-    }
-    void rebase_shard_samples(uint64_t sample_base) override {
-        CK(cudaSetDevice(device_));
-        const uint64_t walks = uint64_t(shard_n_sent_) * samp_n_;
-        if (sample_base)
-            k_add_value<<<unsigned((walks + 256) / 256), 256, 0, stream_>>>(out_[0].sample_off.as<unsigned long long>(),
-                                                                            uint32_t(walks + 1), sample_base);
-        CK(cudaStreamSynchronize(stream_));
-    }
-    void shard_samples_dev(uint64_t* d_sample_off, uint64_t* d_samples) const override {
-        if (!out_[0].samp) throw Error(kInternal, "the shard was run without sampling");
-        *d_sample_off = reinterpret_cast<uint64_t>(out_[0].sample_off.p);
-        *d_samples = reinterpret_cast<uint64_t>(out_[0].samples.p);
+    void shard_arrays(uint64_t addr[kNumArrays]) const override {
+        for (int a = 0; a < kNumArrays; ++a) put_address(&addr[a], out_[0].made, out_[0].buf, a);
     }
     int device() const override { return device_; }
     uint32_t token_bytes() const override { return tok_bytes_; }
@@ -1163,180 +932,89 @@ class EngineImpl final : public Engine {
         return h2d_ev_;
     }
 
-    HostResult* acquire(uint64_t n_sent, uint64_t n_tokens) {
-        HostResult* r = nullptr;
-        if (!pool_free_.empty()) {
-            r = pool_free_.back();
-            pool_free_.pop_back();
-        } else {
-            r = new HostResult();
-            pool_.push_back(r);
+    // The arrays a host result carries under the current options.
+    Outputs outputs() const { return Outputs{tok_bytes_, samp_n_, theta_ > 0, output_mode_ != kOutNone, lattice_ != 0}; }
+
+    // D2H on `st` of every array r carries, from slot `o` holding n sentences and `count` records per group: to
+    // sentence s0 of r and after `base` records per group; `last` brings the closing offsets too.
+    void place(const OutSlot& o, HostResult* r, uint64_t s0, uint64_t n, const Totals& count, const Totals& base, bool last,
+               cudaStream_t st) {
+        for (int a = 0; a < kNumArrays; ++a) {
+            if (!r->out.has(a)) continue;
+            if (!o.made.has(a)) throw Error(kInternal, "the batch was run without an output its result carries");
+            const uint64_t bytes = r->out.bytes(a, n, count, last);
+            if (bytes)
+                CK(cudaMemcpyAsync(r->ptr<uint8_t>(a) + r->out.at(a, s0, base), o.buf[a].p, bytes, cudaMemcpyDeviceToHost, st));
         }
-        if ((n_sent + 1) * 8 > r->cap_off) {
-            pinned_free(r->tok_off);
-            r->cap_off = size_t(double((n_sent + 1) * 8) * 1.25) + 64;
-            r->tok_off = static_cast<uint64_t*>(pinned_alloc(r->cap_off));
-        }
-        if (n_tokens * 24 > r->cap_tok) {
-            pinned_free(r->tokens);
-            r->cap_tok = size_t(double(n_tokens * 24) * 1.25) + 64;
-            r->tokens = pinned_alloc(r->cap_tok);
-        }
-        r->n_sent = n_sent;
-        r->n_tokens = n_tokens;
-        r->has_text = false;
-        r->token_bytes = tok_bytes_;
-        r->has_marg = theta_ > 0;
-        if (r->has_marg) ensure_marg_host(r, n_sent, n_tokens);
-        r->has_lat = lattice_ != 0;
-        r->n_nodes = 0;
-        r->has_samp = samp_n_ != 0;
-        r->n_samp = samp_n_;
-        r->n_sample_tokens = 0;
-        return r;
     }
 
-    // Pinned sample arrays of `r` for n_sent sentences and n_tokens sample tokens (contents not kept).
-    void ensure_samp_host(HostResult* r, uint64_t n_sent, uint64_t n_tokens) {
-        const size_t off_bytes = (n_sent * samp_n_ + 1) * 8;
-        if (off_bytes > r->cap_sample_off) {
-            pinned_free(r->sample_off);
-            r->cap_sample_off = size_t(double(off_bytes) * 1.25) + 64;
-            r->sample_off = static_cast<uint64_t*>(pinned_alloc(r->cap_sample_off));
+    // Adds base[g] to the last shard's offsets of every group g it produced, on stream_.
+    void add_bases(const Totals& base) {
+        const OutSlot& o = out_[0];
+        for (int g = 0; g < kNumGroups; ++g) {
+            const int a = kOffsetsOf[g];
+            if (!o.made.has(a) || !base[g]) continue;
+            const uint64_t n = uint64_t(shard_n_sent_) * o.made.stride(a) + 1;
+            k_add_value<<<unsigned((n + 255) / 256), 256, 0, stream_>>>(o.buf[a].as<unsigned long long>(), uint32_t(n), base[g]);
         }
-        if (n_tokens * 24 > r->cap_samples) grow_samp_host(r, size_t(double(n_tokens) * 1.25) + 64, 0);
-    }
-    // Grows the sample records of `r` to `n` entries, keeping the first `keep`.
-    static void grow_samp_host(HostResult* r, size_t n, uint64_t keep) {
-        if (n * 24 <= r->cap_samples) return;
-        void* bigger = pinned_alloc(n * 24);
-        if (keep) std::memcpy(bigger, r->samples, keep * 24);
-        pinned_free(r->samples);
-        r->samples = bigger;
-        r->cap_samples = n * 24;
-    }
-    // D2H of the samples of slot `o` (n sentences, h_ctrl->n_samples records) to sentence s0 / record `at` of `r`.
-    void copy_samples(const OutSlot& o, HostResult* r, uint64_t at, uint64_t s0, uint64_t n, bool last, cudaStream_t st) {
-        const uint64_t ns = o.h_ctrl->n_samples;
-        CK(cudaMemcpyAsync(r->sample_off + s0 * samp_n_, o.sample_off.p, (n * samp_n_ + (last ? 1 : 0)) * 8,
-                           cudaMemcpyDeviceToHost, st));
-        if (ns) CK(cudaMemcpyAsync(static_cast<uint8_t*>(r->samples) + at * 24, o.samples.p, ns * 24, cudaMemcpyDeviceToHost, st));
-    }
-    // Device sample offsets of slot `o` for (chunks of) up to n_sent sentences; the records are sized by enqueue
-    // from the scanned total.
-    void ensure_samp_out(OutSlot& o, uint32_t n_sent) {
-        if (samp_n_) o.sample_off.ensure((size_t(n_sent) * samp_n_ + 1) * 8, 1.25);
     }
 
-    // Pinned lattice arrays of `r` for n_sent sentences and n_nodes nodes (contents not kept).
-    void ensure_lat_host(HostResult* r, uint64_t n_sent, uint64_t n_nodes) {
-        if ((n_sent + 1) * 8 > r->cap_node_off) {
-            pinned_free(r->node_off);
-            r->cap_node_off = size_t(double((n_sent + 1) * 8) * 1.25) + 64;
-            r->node_off = static_cast<uint64_t*>(pinned_alloc(r->cap_node_off));
+    // Device outputs of slot `o` for (chunks of) up to n_sent sentences and n_bytes bytes, except the text (sized by
+    // the output stage) and the sample records (sized by enqueue from the scanned total).
+    void ensure_out(OutSlot& o, const Workspace& w, uint32_t n_sent, uint64_t n_bytes) {
+        o.buf[kTokOff].ensure((size_t(n_sent) + 1) * 8, 1.25);
+        o.buf[kTokens].ensure(size_t(n_bytes) * 24 + 24, 1.25);  // a token spans >= 1 character >= 1 byte
+        if (theta_ > 0) o.buf[kTokenProb].ensure(size_t(n_bytes) * 4 + 4, 1.25);
+        if (theta_ > 0 || samp_n_) o.buf[kPathProb].ensure((size_t(n_sent) + 1) * 4, 1.25);  // the forward pass writes it
+        if (lattice_) {
+            // a node is a candidate placed in the pool, so the node arrays hold as many entries as the lattice rows of
+            // `w` (enqueue clips cand_cap to them and a larger batch takes the pool-overflow retry)
+            const size_t n = w.ends_cold.cap / 16 + 1;
+            o.buf[kNodeOff].ensure((size_t(n_sent) + 1) * 8, 1.25);
+            o.buf[kNodes].ensure(n * 24);
+            o.buf[kLinks].ensure(n * 8);
+            if (theta_ > 0) o.buf[kNodeProb].ensure(n * 4);
         }
-        if (!lat_fits(r, n_nodes)) grow_lat_host(r, size_t(double(n_nodes) * 1.25) + 64, 0);
-    }
-    static bool lat_fits(const HostResult* r, uint64_t n_nodes) {
-        return n_nodes * 24 <= r->cap_nodes && n_nodes * 8 <= r->cap_links && (!r->has_marg || n_nodes * 4 <= r->cap_nprob);
-    }
-    // Grows the node arrays of `r` to `nodes` entries, keeping the first `keep`.
-    static void grow_lat_host(HostResult* r, size_t nodes, uint64_t keep) {
-        auto grow = [&](void*& p, size_t& cap, size_t rec) {
-            if (nodes * rec <= cap) return;
-            void* bigger = pinned_alloc(nodes * rec);
-            if (keep) std::memcpy(bigger, p, keep * rec);
-            pinned_free(p);
-            p = bigger;
-            cap = nodes * rec;
-        };
-        grow(r->nodes, r->cap_nodes, 24);
-        grow(r->links, r->cap_links, 8);
-        if (r->has_marg) {
-            void* np = r->node_prob;
-            grow(np, r->cap_nprob, 4);
-            r->node_prob = static_cast<float*>(np);
-        }
-    }
-    // D2H of the lattice of slot `o` (n sentences, h_ctrl->n_nodes nodes) to sentence s0 / node `at` of `r`.
-    void copy_lattice(const OutSlot& o, HostResult* r, uint64_t at, uint64_t s0, uint64_t n, bool last, cudaStream_t st) {
-        const uint64_t nn = o.h_ctrl->n_nodes;
-        CK(cudaMemcpyAsync(r->node_off + s0, o.node_off.p, (size_t(n) + (last ? 1 : 0)) * 8, cudaMemcpyDeviceToHost, st));
-        if (!nn) return;
-        CK(cudaMemcpyAsync(static_cast<uint8_t*>(r->nodes) + at * 24, o.nodes.p, nn * 24, cudaMemcpyDeviceToHost, st));
-        CK(cudaMemcpyAsync(static_cast<uint8_t*>(r->links) + at * 8, o.links.p, nn * 8, cudaMemcpyDeviceToHost, st));
-        if (r->has_marg) CK(cudaMemcpyAsync(r->node_prob + at, o.node_prob.p, nn * 4, cudaMemcpyDeviceToHost, st));
-    }
-
-    // Device lattice outputs of slot `o` for (chunks of) up to n_sent sentences: a node is a candidate placed in the
-    // pool, so the node arrays hold as many entries as the lattice rows of `w` (enqueue clips cand_cap to them and
-    // a larger batch takes the pool-overflow retry).
-    void ensure_lat_out(OutSlot& o, const Workspace& w, uint32_t n_sent) {
-        if (!lattice_) return;
-        const size_t n = w.ends_cold.cap / 16 + 1;
-        o.node_off.ensure((size_t(n_sent) + 1) * 8, 1.25);
-        o.nodes.ensure(n * 24);
-        o.links.ensure(n * 8);
-        if (theta_ > 0) o.node_prob.ensure(n * 4);
+        if (samp_n_) o.buf[kSampleOff].ensure((size_t(n_sent) * samp_n_ + 1) * 8, 1.25);
     }
 
     // The nodes' links when lattice text prints %pb (the %pb instantiation of the format kernels), else nullptr.
     const int2* fmt_links(const OutSlot& o) const {
-        return (lattice_ == 2 && output_mode_ == kOutFormat && (fmt_uses_ & kUsesBest)) ? o.links.as<int2>() : nullptr;
+        return (lattice_ == 2 && output_mode_ == kOutFormat && (fmt_uses_ & kUsesBest)) ? o.buf[kLinks].as<int2>() : nullptr;
     }
 
     // Text bytes per input byte expected for the output mode; lattice text is learned apart (about 17x larger).
     double& text_ratio_ref() { return lattice_ == 2 ? text_per_byte_lat_[output_mode_] : text_per_byte_[output_mode_]; }
 
-    // Pinned marginal arrays of `r` for n_sent sentences and n_tokens tokens (contents not kept).
-    static void ensure_marg_host(HostResult* r, uint64_t n_sent, uint64_t n_tokens) {
-        if (n_tokens * 4 > r->cap_tprob) {
-            pinned_free(r->token_prob);
-            r->cap_tprob = size_t(double(n_tokens * 4) * 1.25) + 64;
-            r->token_prob = static_cast<float*>(pinned_alloc(r->cap_tprob));
-        }
-        if (n_sent * 4 > r->cap_pprob) {
-            pinned_free(r->path_prob);
-            r->cap_pprob = size_t(double(n_sent * 4) * 1.25) + 64;
-            r->path_prob = static_cast<float*>(pinned_alloc(r->cap_pprob));
-        }
-    }
-
-    // Device marginal outputs of slot `o` for (chunks of) up to n_sent sentences and n_bytes bytes.
-    void ensure_marg_out(OutSlot& o, uint32_t n_sent, uint64_t n_bytes) {
-        if (theta_ > 0) o.token_prob.ensure(size_t(n_bytes) * 4 + 4, 1.25);  // a token spans >= 1 byte
-        if (theta_ > 0 || samp_n_) o.path_prob.ensure((size_t(n_sent) + 1) * 4, 1.25);  // the forward pass writes it
-    }
-
     // Output stage buffers of slot `o` and scan storage of `w` for (chunks of) up to n_sent sentences.
     void ensure_format(OutSlot& o, Workspace& w, uint32_t n_sent) {
         o.sent_len.ensure((size_t(n_sent) + 1) * 8, 1.25);
-        o.text_off.ensure((size_t(n_sent) + 1) * 8, 1.25);
+        o.buf[kTextOff].ensure((size_t(n_sent) + 1) * 8, 1.25);
         size_t tmp = 0;
         CK(cub::DeviceScan::ExclusiveSum(nullptr, tmp, static_cast<unsigned long long*>(nullptr),
                                          static_cast<unsigned long long*>(nullptr), size_t(n_sent) + 1, w.stream));
         w.scan_tmp.ensure(tmp + 1024, 1.5);
     }
 
-    // Output stage, pass 1 and the scan on w.stream: o.text_off = where each sentence's text starts in o.text
-    // (n_sent + 1 entries, relative to the batch or chunk in `o`).  Returns the arguments of pass 2.
+    // Output stage, pass 1 and the scan on w.stream: the text offsets of `o` = where each sentence's text starts in its
+    // text (n_sent + 1 entries, relative to the batch or chunk in `o`).  Returns the arguments of pass 2.
     FormatArgs format_offsets(Workspace& w, const uint8_t* d_utf8, const unsigned long long* d_off, uint32_t n_sent, OutSlot& o) {
         FormatArgs f{};
         f.utf8 = d_utf8;
         f.byte_off = d_off;
         f.n_sent = n_sent;
         const bool nodes = lattice_ == 2;  // lattice text: the nodes are rendered as tokens
-        f.tok_off = nodes ? o.node_off.as<unsigned long long>() : o.tok_off.as<unsigned long long>();
-        f.tokens = nodes ? o.nodes.as<uint2>() : o.tokens.as<uint2>();
+        f.tok_off = o.buf[nodes ? kNodeOff : kTokOff].as<unsigned long long>();
+        f.tokens = o.buf[nodes ? kNodes : kTokens].as<uint2>();
         f.sent_len = o.sent_len.as<unsigned long long>();
-        f.text_off = o.text_off.as<unsigned long long>();
-        f.text = o.text.as<uint8_t>();
-        f.text_cap = o.text.cap;
+        f.text_off = o.buf[kTextOff].as<unsigned long long>();
+        f.text = o.buf[kText].as<uint8_t>();
+        f.text_cap = o.buf[kText].cap;
         Control* dc = o.ctrl.as<Control>();
         f.flags = &dc->flags;
-        f.text_total = &dc->text_bytes;
+        f.text_total = &dc->total[kGroupText];
         set_mode(f);
-        f.token_prob = (o.marg && (fmt_uses_ & kUsesProb)) ? (nodes ? o.node_prob.as<float>() : o.token_prob.as<float>()) : nullptr;  // %pP
+        f.token_prob = (o.made.marg && (fmt_uses_ & kUsesProb)) ? o.buf[nodes ? kNodeProb : kTokenProb].as<float>() : nullptr;  // %pP
         CK(cudaMemsetAsync(f.sent_len + n_sent, 0, 8, w.stream));
         launch_format_len(dv_, f, w.stream, fmt_links(o));
         exclusive_scan(w, f.sent_len, f.text_off, size_t(n_sent) + 1);
@@ -1344,44 +1022,21 @@ class EngineImpl final : public Engine {
     }
 
     // Output stage of a whole batch (or shard) that run_whole left in out_[0]: the text buffer is sized from the
-    // exact total, read back with one synchronisation.  Returns the text's bytes.
-    uint64_t format_whole(const uint8_t* d_utf8, const unsigned long long* d_off, uint32_t n_sent) {
+    // exact total, read back with one synchronisation, which out_[0] records with the text arrays.
+    void format_whole(const uint8_t* d_utf8, const unsigned long long* d_off, uint32_t n_sent) {
         OutSlot& o = out_[0];
         ensure_format(o, ws_[0], n_sent);
         FormatArgs f = format_offsets(ws_[0], d_utf8, d_off, n_sent, o);
         unsigned long long total = 0;
         CK(cudaMemcpyAsync(&total, f.text_off + n_sent, 8, cudaMemcpyDeviceToHost, stream_));
         CK(cudaStreamSynchronize(stream_));
-        o.text.ensure(total + 16, 1.25);
-        f.text = o.text.as<uint8_t>();
-        f.text_cap = o.text.cap;
+        o.buf[kText].ensure(total + 16, 1.25);
+        f.text = o.buf[kText].as<uint8_t>();
+        f.text_cap = o.buf[kText].cap;
         launch_format_write(dv_, f, stream_, fmt_links(o));
         launches_ += 2;
-        return total;
-    }
-
-    // Pinned text arrays of `r` for n_sent sentences and text_bytes bytes (contents not kept).
-    static void ensure_text(HostResult* r, uint64_t n_sent, uint64_t text_bytes) {
-        if ((n_sent + 1) * 8 > r->cap_text_off) {
-            pinned_free(r->text_off);
-            r->cap_text_off = size_t(double((n_sent + 1) * 8) * 1.25) + 64;
-            r->text_off = static_cast<uint64_t*>(pinned_alloc(r->cap_text_off));
-        }
-        if (text_bytes + 1 > r->cap_text) {
-            pinned_free(r->text);
-            r->cap_text = size_t(double(text_bytes + 1) * 1.25) + 64;
-            r->text = static_cast<char*>(pinned_alloc(r->cap_text));
-        }
-    }
-
-    // Output stage of the whole-batch host path: format, then D2H into `r` on stream_.
-    void format_text(const uint8_t* d_utf8, const unsigned long long* d_off, uint32_t n_sent, HostResult* r) {
-        const uint64_t total = format_whole(d_utf8, d_off, n_sent);
-        ensure_text(r, n_sent, total);
-        CK(cudaMemcpyAsync(r->text_off, out_[0].text_off.p, (size_t(n_sent) + 1) * 8, cudaMemcpyDeviceToHost, stream_));
-        if (total) CK(cudaMemcpyAsync(r->text, out_[0].text.p, total, cudaMemcpyDeviceToHost, stream_));
-        r->text_bytes = total;
-        r->has_text = true;
+        o.h_ctrl->total[kGroupText] = total;
+        o.made.text = true;
     }
 
     // ---- k_small_batch route -------------------------------------------------------------------------------
@@ -1540,15 +1195,12 @@ class EngineImpl final : public Engine {
             if (n_bytes)
                 text_per_byte_[output_mode_] = std::max(text_per_byte_[output_mode_] * 1.5, double(h.text_bytes) / double(n_bytes) * 1.25);
         }
-        HostResult* r = acquire(n_sent, h.n_tokens);
-        std::memcpy(r->tok_off, small_out_h_ + at_tok_off, off_bytes);
-        if (h.n_tokens) std::memcpy(r->tokens, small_out_h_ + at_tokens, h.n_tokens * tb);
+        HostResult* r = pool_.acquire(outputs(), n_sent, Totals{h.n_tokens, fmt ? h.text_bytes : 0, 0, 0});
+        std::memcpy(r->buf[kTokOff].p, small_out_h_ + at_tok_off, off_bytes);
+        if (h.n_tokens) std::memcpy(r->buf[kTokens].p, small_out_h_ + at_tokens, h.n_tokens * tb);
         if (fmt) {
-            ensure_text(r, n_sent, h.text_bytes);
-            std::memcpy(r->text_off, small_out_h_ + at_text_off, off_bytes);
-            if (h.text_bytes) std::memcpy(r->text, small_out_h_ + at_text, h.text_bytes);
-            r->text_bytes = h.text_bytes;
-            r->has_text = true;
+            std::memcpy(r->buf[kTextOff].p, small_out_h_ + at_text_off, off_bytes);
+            if (h.text_bytes) std::memcpy(r->buf[kText].p, small_out_h_ + at_text, h.text_bytes);
         }
         std::memset(stage_ms_, 0, sizeof(stage_ms_));
         CK(cudaEventElapsedTime(&stage_ms_[kSmallBatchStage], o.ev[0], o.ev[1]));
@@ -1721,13 +1373,9 @@ class EngineImpl final : public Engine {
         batch_total_bytes_ = n_bytes;
         for (int attempt = 0;; ++attempt) {
             ensure_workspace(ws_[0], n_sent, n_bytes, bd.off != nullptr);
-            o.tok_off.ensure((size_t(n_sent) + 1) * 8, 1.25);
-            o.tokens.ensure(size_t(n_bytes) * 24 + 24, 1.25);  // a token spans >= 1 character >= 1 byte
-            ensure_marg_out(o, n_sent, n_bytes);
-            ensure_lat_out(o, ws_[0], n_sent);
-            ensure_samp_out(o, n_sent);
+            ensure_out(o, ws_[0], n_sent, n_bytes);
             connid_begin(stream_);
-            enqueue(ws_[0], d_utf8, d_off, n_sent, n_bytes, o, nullptr, nullptr, nullptr, nullptr, bd, sent_base);
+            enqueue(ws_[0], d_utf8, d_off, n_sent, n_bytes, o, nullptr, nullptr, nullptr, bd, sent_base);
             CK(cudaEventSynchronize(o.done));
             CK(cudaGetLastError());
             if (o.h_ctrl->flags & kFlagBadOffsets)
@@ -1759,13 +1407,14 @@ class EngineImpl final : public Engine {
     }
 
     // Queues the whole kernel sequence for one (chunk of a) batch on stream_; no host synchronisation.
-    // `tok_base` (device) makes the chunk's token offsets global and is advanced by its token count.  `text_base`
-    // (device, chunked runs with the output stage only) does the same for the chunk's text, which is formatted into
-    // o.text up to its capacity (kFlagTextOverflow beyond).
+    // `base` (device, chunked runs only: one running total per group) makes the chunk's offsets global and is advanced
+    // by its record counts.  A chunk with the output stage on is formatted into its text buffer up to its capacity
+    // (kFlagTextOverflow beyond).
     void enqueue(Workspace& w, const uint8_t* d_utf8, const unsigned long long* d_off, uint32_t n_sent, uint64_t n_bytes,
-                 OutSlot& o, unsigned long long* tok_base, unsigned long long* text_base, cudaEvent_t base_wait,
-                 cudaEvent_t base_signal, const DevBounds& bd, uint64_t sent0) {
+                 OutSlot& o, unsigned long long* base, cudaEvent_t base_wait, cudaEvent_t base_signal, const DevBounds& bd,
+                 uint64_t sent0) {
         cudaStream_t st = w.stream;
+        o.made = Outputs{tok_bytes_, samp_n_, theta_ > 0, base && output_mode_ != kOutNone, lattice_ != 0};
         // characters <= bytes is the hard bound; the per-character launches are sized from the ratio learned on
         // earlier batches (plus slack), and a batch that exceeds it flags itself and is re-run with the hard bound
         const uint32_t hard_slots = uint32_t(n_bytes + n_sent);
@@ -1778,8 +1427,8 @@ class EngineImpl final : public Engine {
         if (samp) cap_all = std::min<size_t>(cap_all, w.m_lw.cap / 4 - n_sent - 1);
         const bool lat = lattice_ != 0;
         if (lat) {  // nodes <= candidates placed: the node arrays bound the pool too
-            cap_all = std::min<size_t>(cap_all, std::min<size_t>(o.nodes.cap / 24, o.links.cap / 8));
-            if (marg) cap_all = std::min<size_t>(cap_all, o.node_prob.cap / 4);
+            cap_all = std::min<size_t>(cap_all, std::min<size_t>(o.buf[kNodes].cap / 24, o.buf[kLinks].cap / 8));
+            if (marg) cap_all = std::min<size_t>(cap_all, o.buf[kNodeProb].cap / 4);
         }
         const uint32_t cand_cap = uint32_t(cap_all);
         Batch b{};
@@ -1793,7 +1442,7 @@ class EngineImpl final : public Engine {
         b.order = (order_mode_ && n_sent > 1) ? w.order.as<uint32_t>() : nullptr;
         b.eos = w.eos.as<uint4>();
         b.n_tok = w.n_tok.as<uint32_t>();
-        b.tok_off = o.tok_off.as<unsigned long long>();
+        b.tok_off = o.buf[kTokOff].as<unsigned long long>();
         b.code_sys = w.code_sys.as<uint32_t>();
         b.code_usr = w.code_usr.as<uint32_t>();
         b.cinfo = w.cinfo.as<uint32_t>();
@@ -1808,7 +1457,7 @@ class EngineImpl final : public Engine {
         b.cand_cap = cand_cap;
         b.ends_hot = w.ends_hot.as<int2>();
         b.ends_cold = w.ends_cold.as<uint4>();
-        b.tokens = o.tokens.p;
+        b.tokens = o.buf[kTokens].p;
         b.compact = tok_bytes_ == 16 ? 1u : 0u;
         Control* dc = o.ctrl.as<Control>();
         b.pool_ctr = &dc->pool_ctr;
@@ -1867,7 +1516,6 @@ class EngineImpl final : public Engine {
         CK(cudaEventRecord(o.ev[5], st));
         o.launches += launch_viterbi(dv_, b, counting_ ? w.stats.as<uint4>() : nullptr, lanes_, viterbi_kernel_, st, &o.route);
         MargArgs m{};
-        o.marg = marg;
         if (marg || samp) {  // booked with the Viterbi stage; must run before K4a reuses ends_meta
             m.theta = marg ? theta_ : samp_theta_;  // equal when both are on (set_marginals / set_sampling)
             m.fill = w.m_fill.as<uint32_t>();
@@ -1877,30 +1525,28 @@ class EngineImpl final : public Engine {
             m.ab = w.m_ab.as<double2>();
             m.r_eos = w.m_r_eos.as<long long>();
             m.a_eos = w.m_a_eos.as<double>();
-            m.path_prob = o.path_prob.as<float>();
-            m.token_prob = marg ? o.token_prob.as<float>() : nullptr;
+            m.path_prob = o.buf[kPathProb].as<float>();
+            m.token_prob = marg ? o.buf[kTokenProb].as<float>() : nullptr;
             m.lw = samp ? w.m_lw.as<uint32_t>() : nullptr;
             launch_marginals(dv_, b, m, st, marg);  // sampling alone needs no backward pass
             if (n_sent) o.launches += marg ? 2 : 1;
         }
-        o.lat = lat;
         if (lat) {  // booked with the Viterbi stage too, and also before K4a
             LatticeArgs l{};
             l.row_base = w.l_row_base.as<uint32_t>();
             l.n_nodes = w.l_n_nodes.as<uint32_t>();
-            l.node_off = o.node_off.as<unsigned long long>();
-            l.nodes = o.nodes.as<uint2>();
-            l.links = o.links.as<int2>();
-            l.node_prob = marg ? o.node_prob.as<float>() : nullptr;
+            l.node_off = o.buf[kNodeOff].as<unsigned long long>();
+            l.nodes = o.buf[kNodes].as<uint2>();
+            l.links = o.buf[kLinks].as<int2>();
+            l.node_prob = marg ? o.buf[kNodeProb].as<float>() : nullptr;
             launch_lattice_count(b, l, st);
             cub::TransformInputIterator<unsigned long long, CastU64, const uint32_t*> it(l.n_nodes, CastU64());
             if (n_sent == 0) CK(cudaMemsetAsync(l.n_nodes, 0, 4, st));
             exclusive_scan(w, it, l.node_off, size_t(n_sent) + 1);
             launch_lattice_write(b, l, m, st);
-            CK(cudaMemcpyAsync(&dc->n_nodes, l.node_off + n_sent, 8, cudaMemcpyDeviceToDevice, st));
+            CK(cudaMemcpyAsync(&dc->total[kGroupLattice], l.node_off + n_sent, 8, cudaMemcpyDeviceToDevice, st));
             if (n_sent) o.launches += 2;
         }
-        o.samp = samp;
         if (samp) {  // booked with the Viterbi stage too, and also before K4a
             SampleArgs sa{};
             sa.n = samp_n_;
@@ -1908,18 +1554,18 @@ class EngineImpl final : public Engine {
             sa.sent_base = sent0;
             sa.cnt = w.s_cnt.as<uint32_t>();
             sa.total = w.s_total.as<int32_t>();
-            sa.off = o.sample_off.as<unsigned long long>();
+            sa.off = o.buf[kSampleOff].as<unsigned long long>();
             const size_t walks = size_t(n_sent) * samp_n_;
             launch_sample_count(dv_, b, m, sa, st);
             CK(cudaMemsetAsync(sa.cnt + walks, 0, 4, st));
             cub::TransformInputIterator<unsigned long long, CastU64, const uint32_t*> it(sa.cnt, CastU64());
             exclusive_scan(w, it, sa.off, walks + 1);
-            CK(cudaMemcpyAsync(&dc->n_samples, sa.off + walks, 8, cudaMemcpyDeviceToDevice, st));
+            CK(cudaMemcpyAsync(&dc->total[kGroupSamples], sa.off + walks, 8, cudaMemcpyDeviceToDevice, st));
             // the records are sized from the scanned total: one wait for it here
-            CK(cudaMemcpyAsync(&o.h_ctrl->n_samples, sa.off + walks, 8, cudaMemcpyDeviceToHost, st));
+            CK(cudaMemcpyAsync(&o.h_ctrl->total[kGroupSamples], sa.off + walks, 8, cudaMemcpyDeviceToHost, st));
             CK(cudaStreamSynchronize(st));
-            o.samples.ensure(size_t(o.h_ctrl->n_samples) * 24 + 24, 1.25);
-            sa.out = o.samples.as<uint2>();
+            o.buf[kSamples].ensure(size_t(o.h_ctrl->total[kGroupSamples]) * 24 + 24, 1.25);
+            sa.out = o.buf[kSamples].as<uint2>();
             launch_sample_write(dv_, b, m, sa, st);
             if (walks) o.launches += 2;
         }
@@ -1937,43 +1583,27 @@ class EngineImpl final : public Engine {
         else
             launch_backtrack_write(b, st);
         k_publish_totals<<<1, 1, 0, st>>>(b.slot_off, b.tok_off, n_sent, dc);
-        if (text_base) {  // output stage of a chunk: formatted while its token offsets are still chunk-local
+        if (o.made.text) {  // output stage of a chunk: formatted while its token offsets are still chunk-local
             FormatArgs f = format_offsets(w, d_utf8, d_off, n_sent, o);
             launch_format_write(dv_, f, st, fmt_links(o));
             o.launches += 2;
         }
-        if (tok_base) {
+        if (base) {
             if (base_wait) CK(cudaStreamWaitEvent(st, base_wait, 0));  // the previous chunk (other stream) bumped it
-            k_add_base<<<(n_sent + 256) / 256, 256, 0, st>>>(b.tok_off, n_sent + 1, tok_base);
-            k_bump_base<<<1, 1, 0, st>>>(tok_base, &dc->n_tokens);
-            o.launches += 2;
-            if (lat) {  // the same for the node offsets
-                k_add_base<<<(n_sent + 256) / 256, 256, 0, st>>>(o.node_off.as<unsigned long long>(), n_sent + 1, node_base_.as<unsigned long long>());
-                k_bump_base<<<1, 1, 0, st>>>(node_base_.as<unsigned long long>(), &dc->n_nodes);
-                o.launches += 2;
-            }
-            if (samp) {  // and for the sample offsets
-                const size_t walks = size_t(n_sent) * samp_n_;
-                k_add_base<<<unsigned((walks + 256) / 256), 256, 0, st>>>(o.sample_off.as<unsigned long long>(), uint32_t(walks + 1),
-                                                                          samp_base_.as<unsigned long long>());
-                k_bump_base<<<1, 1, 0, st>>>(samp_base_.as<unsigned long long>(), &dc->n_samples);
-                o.launches += 2;
-            }
-            if (text_base) {
-                k_add_base<<<(n_sent + 256) / 256, 256, 0, st>>>(o.text_off.as<unsigned long long>(), n_sent + 1, text_base);
-                k_bump_base<<<1, 1, 0, st>>>(text_base, &dc->text_bytes);
+            for (int g = 0; g < kNumGroups; ++g) {
+                const int a = kOffsetsOf[g];
+                if (!o.made.has(a)) continue;
+                const size_t n = size_t(n_sent) * o.made.stride(a) + 1;
+                k_add_base<<<unsigned((n + 255) / 256), 256, 0, st>>>(o.buf[a].as<unsigned long long>(), uint32_t(n), base + g);
+                k_bump_base<<<1, 1, 0, st>>>(base + g, &dc->total[g]);
                 o.launches += 2;
             }
             if (base_signal) CK(cudaEventRecord(base_signal, st));
         }
         CK(cudaEventRecord(o.ev[9], st));
         CK(cudaMemcpyAsync(o.h_ctrl, dc, sizeof(Control), cudaMemcpyDeviceToHost, st));
-        if (eager_sink_) {  // small batch: results leave in the same breath (sized by their upper bound)
-            CK(cudaMemcpyAsync(eager_sink_->tok_off, o.tok_off.p, (size_t(n_sent) + 1) * 8, cudaMemcpyDeviceToHost, st));
-            if (n_bytes) CK(cudaMemcpyAsync(eager_sink_->tokens, o.tokens.p, size_t(n_bytes) * tok_bytes_, cudaMemcpyDeviceToHost, st));
-            if (marg && n_bytes) CK(cudaMemcpyAsync(eager_sink_->token_prob, o.token_prob.p, size_t(n_bytes) * 4, cudaMemcpyDeviceToHost, st));
-            if (marg && n_sent) CK(cudaMemcpyAsync(eager_sink_->path_prob, o.path_prob.p, size_t(n_sent) * 4, cudaMemcpyDeviceToHost, st));
-        }
+        // small batch: results leave in the same breath (sized by their upper bound, a token per byte)
+        if (eager_sink_) place(o, eager_sink_, 0, n_sent, Totals{n_bytes, 0, 0, 0}, Totals{}, true, st);
         CK(cudaEventRecord(o.done, st));
     }
 
@@ -1993,13 +1623,11 @@ class EngineImpl final : public Engine {
     size_t small_in_cap_ = 0, small_out_cap_ = 0;
     uint64_t staged_bytes_ = 0;  // bytes of pageable caller memory that went through the ring (last batch)
     uint32_t shard_n_sent_ = 0;
-    bool shard_text_ = false;  // the last shard was formatted: shard_text_bytes_ of text in out_[0].text
-    uint64_t shard_text_bytes_ = 0;
     cudaStream_t stream_ = nullptr, own_stream_ = nullptr, in_stream_ = nullptr, out_stream_ = nullptr;
     cudaEvent_t in_done_ = nullptr;
     std::vector<cudaEvent_t> h2d_ev_;
     OutSlot out_[2];
-    DevBuf tok_base_, text_base_, node_base_, samp_base_;
+    DevBuf base_;  // chunked host batches: the running total of each group's records (enqueue)
     uint32_t chunk_sentences_ = 262144;
     uint64_t pool_need_ = 0;
     double tok_per_byte_ = 0.2;
@@ -2016,7 +1644,7 @@ class EngineImpl final : public Engine {
     Workspace ws_[2];
     cudaStream_t aux_stream_ = nullptr;
     cudaEvent_t base_ready_[2] = {nullptr, nullptr};
-    std::vector<HostResult*> pool_, pool_free_;
+    ResultPool pool_;
     std::vector<uint64_t> rebased_;
     double cand_per_byte_ = 4.0;
     double chars_per_byte_ = 1.0;  // learned; 1.0 = the hard bound (every byte a character)
@@ -2044,15 +1672,12 @@ class EngineImpl final : public Engine {
     uint32_t tok_bytes_ = 24;
     int viterbi_kernel_ = 1;  // 1 = k_viterbi2 with pruning (kernels.cuh)
     double theta_ = 0;        // marginals' theta, 0 = off (set_marginals)
-    bool dev_marg_ = false;   // the last run_device computed marginals (device_marginals)
     int lattice_ = 0;         // option "lattice": 0 off, 1 nodes, 2 nodes and lattice text
-    bool dev_lat_ = false;    // the last run_device produced the lattice (device_lattice)
     static constexpr uint32_t kMaxSamples = 1024;
     uint32_t samp_n_ = 0;       // sampling: paths per sentence, 0 = off (set_sampling)
     double samp_theta_ = 0;
     uint64_t samp_seed_ = 0;
-    uint64_t sample_base_ = 0;  // the caller's index of a shard's first sentence (set_sample_base; 0 outside shards)
-    bool dev_samp_ = false;     // the last run_device drew samples (device_samples)
+    Outputs made_;  // the arrays the last run_device produced (device_marginals, _lattice, _samples)
     float stage_ms_[kNumStages];
     uint64_t launches_ = 0;
     uint32_t last_route_ = kRouteNone;  // ViterbiRoute of the last successful call (describe())
@@ -2064,6 +1689,60 @@ class EngineImpl final : public Engine {
 std::unique_ptr<Engine> Engine::create(int device, const uint8_t* host_blob, uint64_t d_blob, uint64_t n_bytes,
                                        bool ignore_space, uint64_t max_grouping_len) {
     return std::unique_ptr<Engine>(new EngineImpl(device, host_blob, d_blob, n_bytes, ignore_space, max_grouping_len));
+}
+
+void DevBuf::ensure(size_t bytes, double slack) {
+    if (bytes <= cap) return;
+    if (p) CK(cudaFree(p));
+    p = nullptr;
+    cap = 0;
+    size_t want = size_t(double(bytes) * slack) + 256;
+    CK(cudaMalloc(&p, want));
+    cap = want;
+}
+
+void DevBuf::release() {
+    if (p) cudaFree(p);
+    p = nullptr;
+    cap = 0;
+}
+
+PinnedBuf::~PinnedBuf() { pinned_free(p); }
+
+void PinnedBuf::ensure(size_t bytes) {
+    if (p && bytes <= cap) return;  // an array is allocated even when empty
+    pinned_free(p);
+    p = nullptr;
+    cap = size_t(double(bytes) * 1.25) + 64;
+    p = pinned_alloc(cap);
+}
+
+void PinnedBuf::grow(size_t bytes, size_t keep_bytes) {
+    if (p && bytes <= cap) return;
+    const size_t want = size_t(double(bytes) * 1.5) + 4096;
+    void* bigger = pinned_alloc(want);
+    if (keep_bytes) std::memcpy(bigger, p, keep_bytes);
+    pinned_free(p);
+    p = bigger;
+    cap = want;
+}
+
+HostResult* ResultPool::acquire(const Outputs& out, uint64_t n_sent, const Totals& total) {
+    if (free_.empty()) {
+        all_.emplace_back(new HostResult());
+        free_.push_back(all_.back().get());
+    }
+    HostResult* r = free_.back();
+    free_.pop_back();
+    r->n_sent = n_sent;
+    r->out = out;
+    r->total = total;
+    for (int a = 0; a < kNumArrays; ++a) {
+        if (!out.has(a)) continue;
+        r->buf[a].ensure(out.bytes(a, n_sent, total, true));
+        if (kArrays[a].kind == kOffsets && n_sent == 0) *r->ptr<uint64_t>(a) = 0;
+    }
+    return r;
 }
 
 void* pinned_alloc(size_t n) {

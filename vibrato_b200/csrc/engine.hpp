@@ -1,6 +1,7 @@
 // Device engine: owns the dictionary image in HBM, the per-batch workspace and the launch sequence.
 #pragma once
 
+#include <array>
 #include <cstdint>
 #include <memory>
 #include <string>
@@ -11,41 +12,120 @@
 
 namespace vbt {
 
-struct HostResult {  // pinned host memory holding one batch's tokens
-    uint64_t n_sent = 0, n_tokens = 0;
-    uint64_t* tok_off = nullptr;  // n_sent + 1
-    void* tokens = nullptr;       // vbt_token[n_tokens], or vbt_token16[n_tokens] when token_bytes == 16
-    uint32_t token_bytes = 24;
-    size_t cap_off = 0, cap_tok = 0;
-    // output stage ("output_mode" option): the text `tokenize` prints for the batch and where each sentence's
-    // part starts (n_sent + 1 offsets); text == nullptr when the stage is off
-    uint64_t text_bytes = 0;
-    uint64_t* text_off = nullptr;
-    char* text = nullptr;
-    size_t cap_text_off = 0, cap_text = 0;
-    bool has_text = false;
-    // marginals (set_marginals): per token and per sentence, has_marg == false when they are off
-    float* token_prob = nullptr;  // n_tokens
-    float* path_prob = nullptr;   // n_sent
-    size_t cap_tprob = 0, cap_pprob = 0;
-    bool has_marg = false;
-    // lattice output (option "lattice" >= 1): every node of each sentence's lattice, has_lat == false when it is off.
-    // node_off[i] .. node_off[i + 1] index sentence i's nodes (kernels.cuh LatticeArgs).
-    uint64_t n_nodes = 0;
-    uint64_t* node_off = nullptr;  // n_sent + 1
-    void* nodes = nullptr;         // vbt_token[n_nodes], always 24 bytes
-    void* links = nullptr;         // vbt_lattice_link[n_nodes]
-    float* node_prob = nullptr;    // n_nodes, with marginals only (has_marg)
-    size_t cap_node_off = 0, cap_nodes = 0, cap_links = 0, cap_nprob = 0;
-    bool has_lat = false;
-    // segmentation sampling (set_sampling): n_samp paths per sentence, has_samp == false when it is off.
-    // sample_off[i * n_samp + j] .. sample_off[i * n_samp + j + 1] index sample j of sentence i (kernels.cuh SampleArgs).
-    uint32_t n_samp = 0;
-    uint64_t n_sample_tokens = 0;
-    uint64_t* sample_off = nullptr;  // n_sent * n_samp + 1
-    void* samples = nullptr;         // vbt_token[n_sample_tokens], always 24 bytes
-    size_t cap_sample_off = 0, cap_samples = 0;
-    bool has_samp = false;
+// ---- the outputs of a batch ------------------------------------------------------------------------
+// A batch produces up to twelve arrays in four ragged groups.  A group's offsets index its records: entries
+// off[i] .. off[i + 1] belong to sentence i (to sample j of sentence i at i * n_samp + j for the samples), and the
+// group's total is the number of its records.  path_prob has one entry per sentence and no offsets.
+enum Group { kGroupTokens, kGroupText, kGroupLattice, kGroupSamples, kNumGroups };
+enum Array {
+    kTokOff, kTokens, kTokenProb, kPathProb,  // vbt_token (or vbt_token16) records; marginals (set_marginals)
+    kTextOff, kText,                          // output stage ("output_mode" or a format): the text `tokenize` prints
+    kNodeOff, kNodes, kLinks, kNodeProb,      // lattice ("lattice" >= 1): vbt_token nodes, vbt_lattice_link, marginals
+    kSampleOff, kSamples,                     // sampling (set_sampling): vbt_token records of every sampled path
+    kNumArrays
+};
+enum ArrayKind { kOffsets, kRecords, kPerSentence };
+struct ArrayInfo {
+    Group group;
+    ArrayKind kind;
+    uint32_t bytes;  // per element; 0 = the token record size
+};
+constexpr ArrayInfo kArrays[kNumArrays] = {
+    {kGroupTokens, kOffsets, 8},   {kGroupTokens, kRecords, 0},  {kGroupTokens, kRecords, 4},   {kGroupTokens, kPerSentence, 4},
+    {kGroupText, kOffsets, 8},     {kGroupText, kRecords, 1},    {kGroupLattice, kOffsets, 8},  {kGroupLattice, kRecords, 24},
+    {kGroupLattice, kRecords, 8},  {kGroupLattice, kRecords, 4}, {kGroupSamples, kOffsets, 8},  {kGroupSamples, kRecords, 24},
+};
+constexpr Array kOffsetsOf[kNumGroups] = {kTokOff, kTextOff, kNodeOff, kSampleOff};
+
+using Totals = std::array<uint64_t, kNumGroups>;  // one count per group
+
+// Which arrays a batch carries, decided by its output options, and where a piece of the batch goes in each.
+struct Outputs {
+    uint32_t token_bytes = 24;  // 24, or 16 with "compact_tokens"
+    uint32_t n_samp = 0;        // sampled paths per sentence, 0 = sampling off
+    bool marg = false, text = false, lat = false;
+
+    bool has(int a) const {
+        switch (a) {
+            case kTokenProb:
+            case kPathProb: return marg;
+            case kTextOff:
+            case kText: return text;
+            case kNodeOff:
+            case kNodes:
+            case kLinks: return lat;
+            case kNodeProb: return lat && marg;
+            case kSampleOff:
+            case kSamples: return n_samp != 0;
+            default: return true;
+        }
+    }
+    uint64_t elem_bytes(int a) const { return kArrays[a].bytes ? kArrays[a].bytes : token_bytes; }
+    uint64_t stride(int a) const { return kArrays[a].kind == kOffsets && kArrays[a].group == kGroupSamples ? n_samp : 1; }
+    // Bytes of array a in a piece of n sentences whose groups hold `count` records; `last`: the piece that ends the
+    // batch also brings the closing offset.
+    uint64_t bytes(int a, uint64_t n, const Totals& count, bool last) const {
+        if (kArrays[a].kind == kRecords) return count[kArrays[a].group] * elem_bytes(a);
+        return (n * stride(a) + (kArrays[a].kind == kOffsets && last ? 1 : 0)) * elem_bytes(a);
+    }
+    // Byte position of that piece in the batch's array: it starts at sentence s0, its records after `base` others.
+    uint64_t at(int a, uint64_t s0, const Totals& base) const {
+        return (kArrays[a].kind == kRecords ? base[kArrays[a].group] : s0 * stride(a)) * elem_bytes(a);
+    }
+};
+
+// Pinned host memory, freed with the buffer.
+struct PinnedBuf {
+    void* p = nullptr;
+    size_t cap = 0;
+    PinnedBuf() = default;
+    PinnedBuf(const PinnedBuf&) = delete;
+    PinnedBuf& operator=(const PinnedBuf&) = delete;
+    ~PinnedBuf();
+    void ensure(size_t bytes);                   // room for `bytes`; the contents are not kept
+    void grow(size_t bytes, size_t keep_bytes);  // room for `bytes`, keeping the first keep_bytes
+};
+
+// Device memory that grows on demand (engine.cu, multi_engine.cu).
+struct DevBuf {
+    void* p = nullptr;
+    size_t cap = 0;
+    void ensure(size_t bytes, double slack = 1.0);  // room for `bytes` (times slack when it grows); contents not kept
+    void release();
+    template <typename T>
+    T* as() const {
+        return static_cast<T*>(p);
+    }
+};
+
+// *dst = the device address of array a in buf[kNumArrays], 0 when `made` lacks it; nothing for a null dst.
+inline void put_address(uint64_t* dst, const Outputs& made, const DevBuf* buf, int a) {
+    if (dst) *dst = made.has(a) ? reinterpret_cast<uint64_t>(buf[a].p) : 0;
+}
+
+struct HostResult {  // one batch's outputs in pinned host memory
+    uint64_t n_sent = 0;
+    Outputs out;
+    Totals total{};
+    PinnedBuf buf[kNumArrays];  // buf[a] holds array a when out.has(a)
+    template <typename T>
+    T* ptr(int a) const {
+        return static_cast<T*>(buf[a].p);
+    }
+};
+
+// Pooled host results, reused across calls.
+class ResultPool {
+   public:
+    // A result for n_sent sentences carrying `out`, with room for `total` records per group.
+    HostResult* acquire(const Outputs& out, uint64_t n_sent, const Totals& total);
+    void release(HostResult* r) {
+        if (r) free_.push_back(r);
+    }
+
+   private:
+    std::vector<std::unique_ptr<HostResult>> all_;
+    std::vector<HostResult*> free_;
 };
 
 // Required token boundaries of a batch (vbt_tokenize_batch_bounded): sentence i's boundaries are the
@@ -84,43 +164,21 @@ class Engine {
     virtual void release(HostResult* r) = 0;
 
     // Building blocks of the multi-device engine (multi_engine.cu); a single-device caller never needs them.
-    // run_shard: host sentences in, tokens left in this device's memory; returns their number (synchronises).
-    // With src_device >= 0 `utf8` is a DEVICE address on that device (peer copy over NVLink) while byte_off is
-    // still a host array.  With text_bytes != nullptr the shard's output text is formatted too ("output_mode";
-    // *text_bytes = its size, 0 when the option is off).
-    // bnd (host memory, may be null) holds the shard's n_sent + 1 boundary offsets.
-    virtual uint64_t run_shard(const char* utf8, const uint64_t* byte_off, uint64_t n_sent, int src_device,
-                               uint64_t* text_bytes, const Bounds* bnd = nullptr) = 0;
-    // fetch_shard: the last shard's token offsets (+ tok_base, n_sent entries, one more when `last`) and token
-    // records into host memory (pinned, or it is slow); with h_text_off != nullptr also its text offsets
-    // (+ text_base, same count) and text, which run_shard must have formatted; with h_token_prob != nullptr also its
-    // marginals (n_tokens and n_sent floats), which it must have computed.
-    virtual void fetch_shard(uint64_t* h_tok_off, void* h_tokens, uint64_t tok_base, bool last, uint64_t* h_text_off,
-                             char* h_text, uint64_t text_base, float* h_token_prob = nullptr, float* h_path_prob = nullptr) = 0;
-    // Device addresses of the last shard's token offsets (uint64[n_sent + 1], already + tok_base after
-    // rebase_shard) and token records.
-    virtual void rebase_shard(uint64_t tok_base) = 0;
-    virtual void shard_outputs(uint64_t* d_tok_off, uint64_t* d_tokens) const = 0;
-    // Device addresses of the last shard's marginals: float token_prob[n_tokens], path_prob[n_sent].
-    virtual void shard_marginals(uint64_t* d_token_prob, uint64_t* d_path_prob) const = 0;
-    // The last shard's lattice (option "lattice"): its node count; fetch_shard_lattice copies its node offsets
-    // (+ node_base, n_sent entries, one more when `last`), nodes, links and, with h_node_prob != nullptr, node marginals
-    // into host memory; rebase_shard_lattice adds node_base to the offsets on the device and shard_lattice gives the
-    // device addresses of the four arrays.
-    virtual uint64_t shard_nodes() const = 0;
-    virtual void fetch_shard_lattice(uint64_t* h_node_off, void* h_nodes, void* h_links, float* h_node_prob,
-                                     uint64_t node_base, bool last) = 0;
-    virtual void rebase_shard_lattice(uint64_t node_base) = 0;
-    virtual void shard_lattice(uint64_t* d_node_off, uint64_t* d_nodes, uint64_t* d_links, uint64_t* d_node_prob) const = 0;
-    // Sampling: set_sample_base gives the caller's index of the next run's first sentence (the i of the draws), so
-    // that a shard draws what the whole batch would.  The last shard's sample-token count; fetch_shard_samples copies
-    // its sample offsets (+ sample_base, n_sent * n entries, one more when `last`) and records into host memory;
-    // rebase_shard_samples adds sample_base on the device and shard_samples_dev gives the two device addresses.
-    virtual void set_sample_base(uint64_t first_sentence) = 0;
-    virtual uint64_t shard_samples() const = 0;
-    virtual void fetch_shard_samples(uint64_t* h_sample_off, void* h_samples, uint64_t sample_base, bool last) = 0;
-    virtual void rebase_shard_samples(uint64_t sample_base) = 0;
-    virtual void shard_samples_dev(uint64_t* d_sample_off, uint64_t* d_samples) const = 0;
+    // run_shard: host sentences in, outputs left in this device's memory; returns their record counts per group
+    // (synchronises).  With src_device >= 0 `utf8` is a DEVICE address on that device (peer copy over NVLink) while
+    // byte_off is still a host array.  first_sentence is the caller's index of the shard's first sentence (the i of the
+    // sampling draws), so that a shard draws what the whole batch would.  With with_text the shard's output text is
+    // formatted too, when an output mode or format is set.  bnd (host memory, may be null) holds the shard's
+    // n_sent + 1 boundary offsets.
+    virtual Totals run_shard(const char* utf8, const uint64_t* byte_off, uint64_t n_sent, int src_device,
+                             uint64_t first_sentence, bool with_text, const Bounds* bnd = nullptr) = 0;
+    // rebase_shard: adds base[g] to the last shard's offsets of every group g it produced, on the device.
+    virtual void rebase_shard(const Totals& base) = 0;
+    // fetch_shard: rebases the last shard like rebase_shard, then copies every array r carries into r at the shard's
+    // place: sentence first_sentence and records after base[g] others (the closing offsets too when `last`).
+    virtual void fetch_shard(HostResult* r, uint64_t first_sentence, const Totals& base, bool last) = 0;
+    // Device address of each array of the last shard, 0 for an array it did not produce.
+    virtual void shard_arrays(uint64_t addr[kNumArrays]) const = 0;
     virtual int device() const = 0;
     virtual uint32_t token_bytes() const = 0;  // 24, or 16 with the "compact_tokens" option
     virtual std::string describe() const = 0;  // JSON: devices, how the dictionary travelled, ...
@@ -128,7 +186,7 @@ class Engine {
     virtual void set_counting(bool on) = 0;
     // Knobs: "lanes_per_sentence" (4/8/16/32), "sort_by_length" (0/1), "counting" (0/1), "chunk_sentences",
     // "dual_stream", "connid_counting", "output_mode" (0 none, 1 mecab, 2 wakati, 3 detail: run_host also
-    // produces HostResult::text, on every host route; run_device stays token-only), "small_batch" (N > 0: run_host
+    // produces the text arrays, on every host route; run_device stays token-only), "small_batch" (N > 0: run_host
     // takes k_small_batch for batches of at most N sentences and 16 KiB without counting; run_device and the shards
     // of a multi-device engine keep the usual route), "lattice" (0 off, 1 results also carry every lattice node,
     // 2 the same and the output text renders the nodes in place of the tokens).
@@ -137,15 +195,15 @@ class Engine {
     // Setting "output_mode" replaces it.  Builds the format's field table on the device.
     virtual void set_format(const FormatProgram* p) = 0;
     // Marginal probabilities (kernels.cuh MargArgs) at temperature theta > 0 on every route except k_small_batch,
-    // which steps aside while they are on; 0 switches them off.  Results then carry HostResult::token_prob /
-    // path_prob, and run_device leaves them in device memory (device_marginals).
+    // which steps aside while they are on; 0 switches them off.  Results then carry kTokenProb / kPathProb (and
+    // kNodeProb with the lattice), and run_device leaves them in device memory (device_marginals).
     virtual void set_marginals(double theta) = 0;
     virtual double marginals() const = 0;
     virtual int lattice() const = 0;  // the option "lattice"
     // Segmentation sampling (kernels.cuh SampleArgs): n (1..1024) paths per sentence drawn from P(path) at temperature
     // theta (> 0, finite; the marginals' theta when they are on), with Philox keyed by seed; n = 0 switches it off.
-    // On every route except k_small_batch, which steps aside.  Results then carry HostResult::sample_off / samples,
-    // and run_device leaves them in device memory (device_samples).
+    // On every route except k_small_batch, which steps aside.  Results then carry kSampleOff / kSamples, and
+    // run_device leaves them in device memory (device_samples).
     virtual void set_sampling(uint32_t n, double theta, uint64_t seed) = 0;
     virtual uint32_t sampling() const = 0;  // n, 0 when off
     // Device addresses of the last run_device's uint64 sample_off[n_sent * n + 1] and vbt_token samples[n_tokens];

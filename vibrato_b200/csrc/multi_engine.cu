@@ -215,28 +215,11 @@ class MultiEngine final : public Engine {
             cudaFree(image_[i]);
             cudaStreamDestroy(stream_[i]);
         }
-        for (auto* r : pool_) {
-            pinned_free(r->tok_off);
-            pinned_free(r->tokens);
-            pinned_free(r->text_off);
-            pinned_free(r->text);
-            pinned_free(r->token_prob);
-            pinned_free(r->path_prob);
-            for (void* p : {static_cast<void*>(r->node_off), r->nodes, r->links, static_cast<void*>(r->node_prob)}) pinned_free(p);
-            pinned_free(r->sample_off);
-            pinned_free(r->samples);
-            delete r;
-        }
         pinned_free(h_off_);
         pinned_free(h_bnd_off_);
         pinned_free(h_bnd_);
         cudaSetDevice(dev_[0]);
-        if (gather_tokens_) cudaFree(gather_tokens_);
-        if (gather_off_) cudaFree(gather_off_);
-        if (gather_tprob_) cudaFree(gather_tprob_);
-        if (gather_pprob_) cudaFree(gather_pprob_);
-        for (void* p : {gather_noff_, gather_nodes_, gather_links_, gather_nprob_, gather_soff_, gather_samples_})
-            if (p) cudaFree(p);
+        for (DevBuf& b : gather_) b.release();
     }
 
     // ---- host batches --------------------------------------------------------------------------------
@@ -249,41 +232,16 @@ class MultiEngine final : public Engine {
         }
         check_samples(n_sent);
         const std::vector<uint64_t> cut = split_by_bytes(byte_off, n_sent, n);
-        std::vector<uint64_t> n_tok(n, 0), n_text(n, 0);
+        std::vector<Totals> count(n);
         run_on_all([&](int i) {
-            const Bounds sb = shard_bounds(bnd, cut[i]);
-            eng_[i]->set_sample_base(cut[i]);  // the draws of sentence k are those of the whole batch
-            n_tok[i] = eng_[i]->run_shard(utf8, byte_off + cut[i], cut[i + 1] - cut[i], -1, text_ ? &n_text[i] : nullptr,
-                                          bnd ? &sb : nullptr);
+            const Bounds sb = shard_bounds(bnd, cut[i]);  // the draws of sentence k are those of the whole batch
+            count[i] = eng_[i]->run_shard(utf8, byte_off + cut[i], cut[i + 1] - cut[i], -1, cut[i], text_, bnd ? &sb : nullptr);
         });
-        std::vector<uint64_t> base(n + 1, 0), text_base(n + 1, 0);
-        for (int i = 0; i < n; ++i) {
-            base[i + 1] = base[i] + n_tok[i];
-            text_base[i + 1] = text_base[i] + n_text[i];
-        }
-        std::vector<uint64_t> node_base(n + 1, 0);  // lattice nodes: merged at their final positions like the tokens
-        if (lattice_)
-            for (int i = 0; i < n; ++i) node_base[i + 1] = node_base[i] + eng_[i]->shard_nodes();
-        const uint64_t ns = sampling();
-        std::vector<uint64_t> samp_base(n + 1, 0);  // sample records: merged at their final positions like the tokens
-        if (ns)
-            for (int i = 0; i < n; ++i) samp_base[i + 1] = samp_base[i] + eng_[i]->shard_samples();
-        HostResult* r = acquire(n_sent, base[n], text_ ? &text_base[n] : nullptr, node_base[n], samp_base[n]);
-        const uint64_t tb = eng_[0]->token_bytes();
-        r->token_bytes = uint32_t(tb);
-        int last = n - 1;  // the shard that also delivers the closing offset: the last one, even when it is empty
-        run_on_all([&](int i) {
-            eng_[i]->fetch_shard(r->tok_off + cut[i], static_cast<uint8_t*>(r->tokens) + base[i] * tb, base[i], i == last,
-                                 text_ ? r->text_off + cut[i] : nullptr, r->text + text_base[i], text_base[i],
-                                 r->has_marg ? r->token_prob + base[i] : nullptr, r->has_marg ? r->path_prob + cut[i] : nullptr);
-            if (r->has_lat)
-                eng_[i]->fetch_shard_lattice(r->node_off + cut[i], static_cast<uint8_t*>(r->nodes) + node_base[i] * 24,
-                                             static_cast<uint8_t*>(r->links) + node_base[i] * 8,
-                                             r->has_marg ? r->node_prob + node_base[i] : nullptr, node_base[i], i == last);
-            if (r->has_samp)
-                eng_[i]->fetch_shard_samples(r->sample_off + cut[i] * ns, static_cast<uint8_t*>(r->samples) + samp_base[i] * 24,
-                                             samp_base[i], i == last);
-        });
+        // every shard's outputs are copied straight to their final positions; the last shard, even when it is empty,
+        // also delivers the closing offsets
+        const std::vector<Totals> base = prefix_sums(count);
+        HostResult* r = pool_.acquire(outputs(), n_sent, base[n]);
+        run_on_all([&](int i) { eng_[i]->fetch_shard(r, cut[i], base[i], i == n - 1); });
         collect_stats();
         return r;
     }
@@ -292,7 +250,7 @@ class MultiEngine final : public Engine {
         if (dev_.size() == 1)
             eng_[0]->release(r);
         else
-            free_.push_back(r);
+            pool_.release(r);
     }
 
     // ---- device-resident batches: input on the first device, results gathered back to it ------------------
@@ -305,7 +263,7 @@ class MultiEngine final : public Engine {
             return;
         }
         check_samples(n_sent);
-        dev_marg_ = dev_lat_ = dev_samp_ = false;
+        made_ = Outputs{};
         CK(cudaSetDevice(dev_[0]));
         // the split needs the offsets on the host (pinned staging buffer, one copy); their validity is checked on
         // the devices like for any device-resident batch (k_count_chars)
@@ -328,152 +286,63 @@ class MultiEngine final : public Engine {
             hb = Bounds{static_cast<const uint64_t*>(h_bnd_off_), static_cast<const uint32_t*>(h_bnd_), bnd->n};
         }
         const std::vector<uint64_t> cut = split_by_bytes(h_off_, n_sent, n);
-        std::vector<uint64_t> n_tok(n, 0);
+        std::vector<Totals> count(n);
         run_on_all([&](int i) {
             const Bounds sb = shard_bounds(bnd ? &hb : nullptr, cut[i]);
-            eng_[i]->set_sample_base(cut[i]);
-            n_tok[i] = eng_[i]->run_shard(reinterpret_cast<const char*>(d_utf8), h_off_ + cut[i], cut[i + 1] - cut[i],
-                                          dev_[0], nullptr, bnd ? &sb : nullptr);  // token-only, like the single-device entry point
+            count[i] = eng_[i]->run_shard(reinterpret_cast<const char*>(d_utf8), h_off_ + cut[i], cut[i + 1] - cut[i], dev_[0],
+                                          cut[i], false, bnd ? &sb : nullptr);  // no text, like the single-device entry point
         });
-        std::vector<uint64_t> base(n + 1, 0);
-        for (int i = 0; i < n; ++i) base[i + 1] = base[i] + n_tok[i];
+        const std::vector<Totals> base = prefix_sums(count);
         run_on_all([&](int i) { eng_[i]->rebase_shard(base[i]); });
-        const bool lat = lattice_ != 0;
-        std::vector<uint64_t> nbase(n + 1, 0), src_noff(n), src_nodes(n), src_links(n), src_nprob(n);
-        if (lat) {  // the lattice travels like the tokens: nodes at their final positions, offsets rebased
-            for (int i = 0; i < n; ++i) nbase[i + 1] = nbase[i] + eng_[i]->shard_nodes();
-            run_on_all([&](int i) { eng_[i]->rebase_shard_lattice(nbase[i]); });
-            for (int i = 0; i < n; ++i) eng_[i]->shard_lattice(&src_noff[i], &src_nodes[i], &src_links[i], &src_nprob[i]);
-        }
-        const uint64_t ns = sampling();
-        std::vector<uint64_t> sbase(n + 1, 0), src_soff(n), src_samp(n);
-        if (ns) {  // the samples too: records at their final positions, offsets rebased
-            for (int i = 0; i < n; ++i) sbase[i + 1] = sbase[i] + eng_[i]->shard_samples();
-            run_on_all([&](int i) { eng_[i]->rebase_shard_samples(sbase[i]); });
-            for (int i = 0; i < n; ++i) eng_[i]->shard_samples_dev(&src_soff[i], &src_samp[i]);
-        }
-        // gather on the first device: token records and offsets of every shard at their final positions
+        // gather on the first device: every array of every shard at its final position
+        Outputs out = outputs();
+        out.text = false;
         CK(cudaSetDevice(dev_[0]));
-        if (base[n] * 24 + 24 > gather_tok_cap_) {
-            if (gather_tokens_) CK(cudaFree(gather_tokens_));
-            gather_tok_cap_ = size_t(double(base[n] * 24) * 1.25) + 4096;
-            CK(cudaMalloc(&gather_tokens_, gather_tok_cap_));
-        }
-        if ((n_sent + 1) * 8 > gather_off_cap_) {
-            if (gather_off_) CK(cudaFree(gather_off_));
-            gather_off_cap_ = size_t(double((n_sent + 1) * 8) * 1.25) + 4096;
-            CK(cudaMalloc(&gather_off_, gather_off_cap_));
-        }
-        const bool marg = marginals() > 0;
-        if (marg) {  // the marginals travel with the token records: float per token, float per sentence
-            grow_device(gather_tprob_, gather_tprob_cap_, base[n] * 4 + 4);
-            grow_device(gather_pprob_, gather_pprob_cap_, n_sent * 4 + 4);
-        }
-        if (lat) {
-            grow_device(gather_noff_, gather_noff_cap_, (n_sent + 1) * 8);
-            grow_device(gather_nodes_, gather_nodes_cap_, nbase[n] * 24 + 24);
-            grow_device(gather_links_, gather_links_cap_, nbase[n] * 8 + 8);
-            if (marg) grow_device(gather_nprob_, gather_nprob_cap_, nbase[n] * 4 + 4);
-        }
-        if (ns) {
-            grow_device(gather_soff_, gather_soff_cap_, (n_sent * ns + 1) * 8);
-            grow_device(gather_samples_, gather_samples_cap_, sbase[n] * 24 + 24);
-        }
-        // the lattice pieces of shard i: {destination on the first device, source on device i, bytes}
+        for (int a = 0; a < kNumArrays; ++a)
+            if (out.has(a)) gather_[a].ensure(out.bytes(a, n_sent, base[n], true) + out.elem_bytes(a), 1.25);
+        // the pieces of shard i: {destination on the first device, source on device i, bytes}
         struct Piece {
             void* dst;
-            uint64_t src, bytes;
+            const void* src;
+            uint64_t bytes;
         };
-        auto lat_pieces = [&](int i) {
+        auto pieces = [&](int i) {
+            uint64_t src[kNumArrays];
+            eng_[i]->shard_arrays(src);
             std::vector<Piece> v;
-            if (!lat) return v;
-            const uint64_t nn = nbase[i + 1] - nbase[i];
-            v.push_back({static_cast<uint8_t*>(gather_noff_) + cut[i] * 8, src_noff[i], (cut[i + 1] - cut[i] + (i == n - 1 ? 1 : 0)) * 8});
-            if (nn) {
-                v.push_back({static_cast<uint8_t*>(gather_nodes_) + nbase[i] * 24, src_nodes[i], nn * 24});
-                v.push_back({static_cast<uint8_t*>(gather_links_) + nbase[i] * 8, src_links[i], nn * 8});
-                if (marg) v.push_back({static_cast<uint8_t*>(gather_nprob_) + nbase[i] * 4, src_nprob[i], nn * 4});
+            for (int a = 0; a < kNumArrays; ++a) {
+                const uint64_t bytes = out.has(a) ? out.bytes(a, cut[i + 1] - cut[i], count[i], i == n - 1) : 0;
+                if (bytes)
+                    v.push_back({gather_[a].as<uint8_t>() + out.at(a, cut[i], base[i]), reinterpret_cast<const void*>(src[a]), bytes});
             }
             return v;
         };
-        auto samp_pieces = [&](int i) {  // the same for the samples
-            std::vector<Piece> v;
-            if (!ns) return v;
-            v.push_back({static_cast<uint8_t*>(gather_soff_) + cut[i] * ns * 8, src_soff[i],
-                         ((cut[i + 1] - cut[i]) * ns + (i == n - 1 ? 1 : 0)) * 8});
-            if (sbase[i + 1] > sbase[i])
-                v.push_back({static_cast<uint8_t*>(gather_samples_) + sbase[i] * 24, src_samp[i], (sbase[i + 1] - sbase[i]) * 24});
-            return v;
-        };
-        std::vector<uint64_t> src_off(n), src_tok(n), src_tp(n), src_pp(n);
-        for (int i = 0; i < n; ++i) {
-            eng_[i]->shard_outputs(&src_off[i], &src_tok[i]);
-            if (marg) eng_[i]->shard_marginals(&src_tp[i], &src_pp[i]);
-        }
-        auto dst_tp = [&](int i) { return static_cast<uint8_t*>(gather_tprob_) + base[i] * 4; };
-        auto dst_pp = [&](int i) { return static_cast<uint8_t*>(gather_pprob_) + cut[i] * 4; };
-        auto n_sh = [&](int i) { return cut[i + 1] - cut[i]; };
-        const uint64_t tb = eng_[0]->token_bytes();
-        auto dst_tok = [&](int i) { return static_cast<uint8_t*>(gather_tokens_) + base[i] * tb; };
-        auto dst_off = [&](int i) { return static_cast<uint8_t*>(gather_off_) + cut[i] * 8; };
-        auto off_bytes = [&](int i) { return (cut[i + 1] - cut[i] + (i == n - 1 ? 1 : 0)) * 8; };
-        // shard 0 is already on the first device
-        CK(cudaMemcpyAsync(dst_tok(0), reinterpret_cast<const void*>(src_tok[0]), n_tok[0] * tb, cudaMemcpyDeviceToDevice, stream_[0]));
-        CK(cudaMemcpyAsync(dst_off(0), reinterpret_cast<const void*>(src_off[0]), off_bytes(0), cudaMemcpyDeviceToDevice, stream_[0]));
-        if (marg) {
-            if (n_tok[0]) CK(cudaMemcpyAsync(dst_tp(0), reinterpret_cast<const void*>(src_tp[0]), n_tok[0] * 4, cudaMemcpyDeviceToDevice, stream_[0]));
-            if (n_sh(0)) CK(cudaMemcpyAsync(dst_pp(0), reinterpret_cast<const void*>(src_pp[0]), n_sh(0) * 4, cudaMemcpyDeviceToDevice, stream_[0]));
-        }
-        for (const Piece& p : samp_pieces(0))
-            CK(cudaMemcpyAsync(p.dst, reinterpret_cast<const void*>(p.src), p.bytes, cudaMemcpyDeviceToDevice, stream_[0]));
-        for (const Piece& p : lat_pieces(0))
-            CK(cudaMemcpyAsync(p.dst, reinterpret_cast<const void*>(p.src), p.bytes, cudaMemcpyDeviceToDevice, stream_[0]));
+        for (const Piece& p : pieces(0))  // shard 0 is already on the first device
+            CK(cudaMemcpyAsync(p.dst, p.src, p.bytes, cudaMemcpyDeviceToDevice, stream_[0]));
         if (n > 1 && nccl_) {
             NK(nccl_->GroupStart());
             for (int i = 1; i < n; ++i) {
+                const std::vector<Piece> v = pieces(i);
                 CK(cudaSetDevice(dev_[i]));
-                if (n_tok[i]) NK(nccl_->Send(reinterpret_cast<const void*>(src_tok[i]), n_tok[i] * tb, ncclUint8, 0, comm_[i], stream_[i]));
-                NK(nccl_->Send(reinterpret_cast<const void*>(src_off[i]), off_bytes(i), ncclUint8, 0, comm_[i], stream_[i]));
-                if (marg && n_tok[i]) NK(nccl_->Send(reinterpret_cast<const void*>(src_tp[i]), n_tok[i] * 4, ncclUint8, 0, comm_[i], stream_[i]));
-                if (marg && n_sh(i)) NK(nccl_->Send(reinterpret_cast<const void*>(src_pp[i]), n_sh(i) * 4, ncclUint8, 0, comm_[i], stream_[i]));
-                std::vector<Piece> lp = lat_pieces(i);
-                for (const Piece& p : samp_pieces(i)) lp.push_back(p);
-                for (const Piece& p : lp) NK(nccl_->Send(reinterpret_cast<const void*>(p.src), p.bytes, ncclUint8, 0, comm_[i], stream_[i]));
+                for (const Piece& p : v) NK(nccl_->Send(p.src, p.bytes, ncclUint8, 0, comm_[i], stream_[i]));
                 CK(cudaSetDevice(dev_[0]));
-                if (n_tok[i]) NK(nccl_->Recv(dst_tok(i), n_tok[i] * tb, ncclUint8, i, comm_[0], stream_[0]));
-                NK(nccl_->Recv(dst_off(i), off_bytes(i), ncclUint8, i, comm_[0], stream_[0]));
-                if (marg && n_tok[i]) NK(nccl_->Recv(dst_tp(i), n_tok[i] * 4, ncclUint8, i, comm_[0], stream_[0]));
-                if (marg && n_sh(i)) NK(nccl_->Recv(dst_pp(i), n_sh(i) * 4, ncclUint8, i, comm_[0], stream_[0]));
-                for (const Piece& p : lp) NK(nccl_->Recv(p.dst, p.bytes, ncclUint8, i, comm_[0], stream_[0]));
+                for (const Piece& p : v) NK(nccl_->Recv(p.dst, p.bytes, ncclUint8, i, comm_[0], stream_[0]));
             }
             NK(nccl_->GroupEnd());
         } else {
-            for (int i = 1; i < n; ++i) {
-                if (n_tok[i]) CK(cudaMemcpyPeerAsync(dst_tok(i), dev_[0], reinterpret_cast<const void*>(src_tok[i]), dev_[i], n_tok[i] * tb, stream_[0]));
-                CK(cudaMemcpyPeerAsync(dst_off(i), dev_[0], reinterpret_cast<const void*>(src_off[i]), dev_[i], off_bytes(i), stream_[0]));
-                if (marg && n_tok[i])
-                    CK(cudaMemcpyPeerAsync(dst_tp(i), dev_[0], reinterpret_cast<const void*>(src_tp[i]), dev_[i], n_tok[i] * 4, stream_[0]));
-                if (marg && n_sh(i))
-                    CK(cudaMemcpyPeerAsync(dst_pp(i), dev_[0], reinterpret_cast<const void*>(src_pp[i]), dev_[i], n_sh(i) * 4, stream_[0]));
-                for (const Piece& p : lat_pieces(i))
-                    CK(cudaMemcpyPeerAsync(p.dst, dev_[0], reinterpret_cast<const void*>(p.src), dev_[i], p.bytes, stream_[0]));
-                for (const Piece& p : samp_pieces(i))
-                    CK(cudaMemcpyPeerAsync(p.dst, dev_[0], reinterpret_cast<const void*>(p.src), dev_[i], p.bytes, stream_[0]));
-            }
+            for (int i = 1; i < n; ++i)
+                for (const Piece& p : pieces(i)) CK(cudaMemcpyPeerAsync(p.dst, dev_[0], p.src, dev_[i], p.bytes, stream_[0]));
         }
         for (int i = 0; i < n; ++i) {
             CK(cudaSetDevice(dev_[i]));
             CK(cudaStreamSynchronize(stream_[i]));
         }
         collect_stats();
-        *d_tok_off = reinterpret_cast<uint64_t>(gather_off_);
-        *d_tokens = reinterpret_cast<uint64_t>(gather_tokens_);
-        *n_tokens = base[n];
-        dev_marg_ = marg;
-        dev_lat_ = lat;
-        dev_nodes_ = nbase[n];
-        dev_samp_ = ns != 0;
-        dev_samples_ = sbase[n];
+        *d_tok_off = reinterpret_cast<uint64_t>(gather_[kTokOff].p);
+        *d_tokens = reinterpret_cast<uint64_t>(gather_[kTokens].p);
+        *n_tokens = base[n][kGroupTokens];
+        made_ = out;
+        made_total_ = base[n];
     }
 
     // ---- everything else is forwarded ------------------------------------------------------------------
@@ -507,27 +376,27 @@ class MultiEngine final : public Engine {
     uint32_t sampling() const override { return eng_[0]->sampling(); }
     void device_samples(uint64_t* d_sample_off, uint64_t* d_samples, uint64_t* n_tokens) const override {
         if (dev_.size() == 1) return eng_[0]->device_samples(d_sample_off, d_samples, n_tokens);
-        if (!dev_samp_) throw Error(kInvalidArgument, "the last device-resident call ran without sampling");
-        if (d_sample_off) *d_sample_off = reinterpret_cast<uint64_t>(gather_soff_);
-        if (d_samples) *d_samples = reinterpret_cast<uint64_t>(gather_samples_);
-        if (n_tokens) *n_tokens = dev_samples_;
+        if (!made_.has(kSamples)) throw Error(kInvalidArgument, "the last device-resident call ran without sampling");
+        put_address(d_sample_off, made_, gather_, kSampleOff);
+        put_address(d_samples, made_, gather_, kSamples);
+        if (n_tokens) *n_tokens = made_total_[kGroupSamples];
     }
     int lattice() const override { return lattice_; }
     void device_marginals(uint64_t* d_token_prob, uint64_t* d_path_prob) const override {
         if (dev_.size() == 1) return eng_[0]->device_marginals(d_token_prob, d_path_prob);
-        if (!dev_marg_) throw Error(kInvalidArgument, "the last device-resident call ran without marginals");
-        if (d_token_prob) *d_token_prob = reinterpret_cast<uint64_t>(gather_tprob_);
-        if (d_path_prob) *d_path_prob = reinterpret_cast<uint64_t>(gather_pprob_);
+        if (!made_.has(kTokenProb)) throw Error(kInvalidArgument, "the last device-resident call ran without marginals");
+        put_address(d_token_prob, made_, gather_, kTokenProb);
+        put_address(d_path_prob, made_, gather_, kPathProb);
     }
     void device_lattice(uint64_t* d_node_off, uint64_t* d_nodes, uint64_t* d_links, uint64_t* d_node_prob,
                         uint64_t* n_nodes) const override {
         if (dev_.size() == 1) return eng_[0]->device_lattice(d_node_off, d_nodes, d_links, d_node_prob, n_nodes);
-        if (!dev_lat_) throw Error(kInvalidArgument, "the last device-resident call ran without the lattice");
-        if (d_node_off) *d_node_off = reinterpret_cast<uint64_t>(gather_noff_);
-        if (d_nodes) *d_nodes = reinterpret_cast<uint64_t>(gather_nodes_);
-        if (d_links) *d_links = reinterpret_cast<uint64_t>(gather_links_);
-        if (d_node_prob) *d_node_prob = dev_marg_ ? reinterpret_cast<uint64_t>(gather_nprob_) : 0;
-        if (n_nodes) *n_nodes = dev_nodes_;
+        if (!made_.has(kNodes)) throw Error(kInvalidArgument, "the last device-resident call ran without the lattice");
+        put_address(d_node_off, made_, gather_, kNodeOff);
+        put_address(d_nodes, made_, gather_, kNodes);
+        put_address(d_links, made_, gather_, kLinks);
+        put_address(d_node_prob, made_, gather_, kNodeProb);
+        if (n_nodes) *n_nodes = made_total_[kGroupLattice];
     }
     void set_stream(uint64_t stream) override {
         if (stream) throw Error(kUnsupported, "a multi-device tokenizer runs on its own streams");
@@ -550,24 +419,12 @@ class MultiEngine final : public Engine {
             for (uint32_t i = 0; i < nr; ++i) rid[i] += r[i];
         }
     }
-    uint64_t run_shard(const char*, const uint64_t*, uint64_t, int, uint64_t*, const Bounds*) override {
+    Totals run_shard(const char*, const uint64_t*, uint64_t, int, uint64_t, bool, const Bounds*) override {
         throw Error(kInternal, "not a shard engine");
     }
-    void fetch_shard(uint64_t*, void*, uint64_t, bool, uint64_t*, char*, uint64_t, float*, float*) override {
-        throw Error(kInternal, "not a shard engine");
-    }
-    void shard_marginals(uint64_t*, uint64_t*) const override { throw Error(kInternal, "not a shard engine"); }
-    uint64_t shard_nodes() const override { throw Error(kInternal, "not a shard engine"); }
-    void fetch_shard_lattice(uint64_t*, void*, void*, float*, uint64_t, bool) override { throw Error(kInternal, "not a shard engine"); }
-    void rebase_shard_lattice(uint64_t) override { throw Error(kInternal, "not a shard engine"); }
-    void shard_lattice(uint64_t*, uint64_t*, uint64_t*, uint64_t*) const override { throw Error(kInternal, "not a shard engine"); }
-    void set_sample_base(uint64_t) override { throw Error(kInternal, "not a shard engine"); }
-    uint64_t shard_samples() const override { throw Error(kInternal, "not a shard engine"); }
-    void fetch_shard_samples(uint64_t*, void*, uint64_t, bool) override { throw Error(kInternal, "not a shard engine"); }
-    void rebase_shard_samples(uint64_t) override { throw Error(kInternal, "not a shard engine"); }
-    void shard_samples_dev(uint64_t*, uint64_t*) const override { throw Error(kInternal, "not a shard engine"); }
-    void rebase_shard(uint64_t) override { throw Error(kInternal, "not a shard engine"); }
-    void shard_outputs(uint64_t*, uint64_t*) const override { throw Error(kInternal, "not a shard engine"); }
+    void rebase_shard(const Totals&) override { throw Error(kInternal, "not a shard engine"); }
+    void fetch_shard(HostResult*, uint64_t, const Totals&, bool) override { throw Error(kInternal, "not a shard engine"); }
+    void shard_arrays(uint64_t*) const override { throw Error(kInternal, "not a shard engine"); }
     int device() const override { return dev_[0]; }
     uint32_t token_bytes() const override { return eng_[0]->token_bytes(); }
     std::string describe() const override {
@@ -597,14 +454,6 @@ class MultiEngine final : public Engine {
     void check_samples(uint64_t n_sent) const {
         if (n_sent * sampling() >= 0xFFFFFFFFull)
             throw Error(kInvalidArgument, "sampling: n_sent * n must stay below 2^32: split the batch or draw fewer samples");
-    }
-
-    static void grow_device(void*& p, size_t& cap, size_t bytes) {
-        if (bytes <= cap) return;
-        if (p) CK(cudaFree(p));
-        p = nullptr;
-        cap = size_t(double(bytes) * 1.25) + 4096;
-        CK(cudaMalloc(&p, cap));
     }
 
     static void grow_pinned(void*& p, size_t& cap, size_t bytes) {
@@ -661,78 +510,15 @@ class MultiEngine final : public Engine {
         }
     }
 
-    // A pooled pinned result for n_sent sentences and n_tokens tokens, and *text_bytes bytes of text when given.
-    HostResult* acquire(uint64_t n_sent, uint64_t n_tokens, const uint64_t* text_bytes, uint64_t n_nodes = 0,
-                        uint64_t n_samples = 0) {
-        HostResult* r = nullptr;
-        if (!free_.empty()) {
-            r = free_.back();
-            free_.pop_back();
-        } else {
-            r = new HostResult();
-            pool_.push_back(r);
-        }
-        if ((n_sent + 1) * 8 > r->cap_off) {
-            pinned_free(r->tok_off);
-            r->cap_off = size_t(double((n_sent + 1) * 8) * 1.25) + 64;
-            r->tok_off = static_cast<uint64_t*>(pinned_alloc(r->cap_off));
-        }
-        if (n_tokens * 24 > r->cap_tok) {
-            pinned_free(r->tokens);
-            r->cap_tok = size_t(double(n_tokens * 24) * 1.25) + 64;
-            r->tokens = pinned_alloc(r->cap_tok);
-        }
-        r->n_sent = n_sent;
-        r->n_tokens = n_tokens;
-        r->has_text = text_bytes != nullptr;
-        r->text_bytes = text_bytes ? *text_bytes : 0;
-        if (text_bytes) {
-            if ((n_sent + 1) * 8 > r->cap_text_off) {
-                pinned_free(r->text_off);
-                r->cap_text_off = size_t(double((n_sent + 1) * 8) * 1.25) + 64;
-                r->text_off = static_cast<uint64_t*>(pinned_alloc(r->cap_text_off));
-            }
-            if (*text_bytes + 1 > r->cap_text) {
-                pinned_free(r->text);
-                r->cap_text = size_t(double(*text_bytes + 1) * 1.25) + 64;
-                r->text = static_cast<char*>(pinned_alloc(r->cap_text));
-            }
-        }
-        r->has_marg = marginals() > 0;
-        if (r->has_marg) {
-            void* tp = r->token_prob;
-            void* pp = r->path_prob;
-            grow_pinned(tp, r->cap_tprob, n_tokens * 4);
-            grow_pinned(pp, r->cap_pprob, n_sent * 4);
-            r->token_prob = static_cast<float*>(tp);
-            r->path_prob = static_cast<float*>(pp);
-        }
-        r->has_lat = lattice_ != 0;
-        r->n_nodes = n_nodes;
-        if (r->has_lat) {
-            void* no = r->node_off;
-            void* np = r->node_prob;
-            grow_pinned(no, r->cap_node_off, (n_sent + 1) * 8);
-            grow_pinned(r->nodes, r->cap_nodes, n_nodes * 24);
-            grow_pinned(r->links, r->cap_links, n_nodes * 8);
-            if (r->has_marg) grow_pinned(np, r->cap_nprob, n_nodes * 4);
-            r->node_off = static_cast<uint64_t*>(no);
-            r->node_prob = static_cast<float*>(np);
-            if (n_sent == 0) r->node_off[0] = 0;
-        }
-        r->n_samp = sampling();
-        r->has_samp = r->n_samp != 0;
-        r->n_sample_tokens = n_samples;
-        if (r->has_samp) {
-            void* so = r->sample_off;
-            grow_pinned(so, r->cap_sample_off, (n_sent * r->n_samp + 1) * 8);
-            grow_pinned(r->samples, r->cap_samples, n_samples * 24);
-            r->sample_off = static_cast<uint64_t*>(so);
-            if (n_sent == 0) r->sample_off[0] = 0;
-        }
-        if (n_sent == 0) r->tok_off[0] = 0;
-        if (n_sent == 0 && text_bytes) r->text_off[0] = 0;
-        return r;
+    // The arrays a host result carries under the current options.
+    Outputs outputs() const { return Outputs{token_bytes(), sampling(), marginals() > 0, text_, lattice_ != 0}; }
+
+    // base[i][g] = the records of group g in the shards before shard i (base[n] = all of them).
+    static std::vector<Totals> prefix_sums(const std::vector<Totals>& count) {
+        std::vector<Totals> base(count.size() + 1, Totals{});
+        for (size_t i = 0; i < count.size(); ++i)
+            for (int g = 0; g < kNumGroups; ++g) base[i + 1][g] = base[i][g] + count[i][g];
+        return base;
     }
 
     std::vector<int> dev_;
@@ -743,7 +529,7 @@ class MultiEngine final : public Engine {
     std::vector<std::vector<int>> cpus_;
     std::vector<std::unique_ptr<Engine>> eng_;
     std::string transport_;
-    std::vector<HostResult*> pool_, free_;
+    ResultPool pool_;
     bool text_ = false;  // "output_mode" or an output format is on: host results carry the formatted text
     bool fixed_mode_ = false;  // "output_mode" 1-3 is on
     uint64_t* h_off_ = nullptr;  // pinned
@@ -751,26 +537,10 @@ class MultiEngine final : public Engine {
     void* h_bnd_off_ = nullptr;  // pinned: the boundary lists of a device-resident batch, cut into shards on the host
     void* h_bnd_ = nullptr;
     size_t h_bnd_off_cap_ = 0, h_bnd_cap_ = 0;
-    void* gather_tokens_ = nullptr;
-    void* gather_off_ = nullptr;
-    size_t gather_tok_cap_ = 0, gather_off_cap_ = 0;
-    void* gather_tprob_ = nullptr;  // marginals of a gathered device-resident batch
-    void* gather_pprob_ = nullptr;
-    size_t gather_tprob_cap_ = 0, gather_pprob_cap_ = 0;
-    bool dev_marg_ = false;
-    void* gather_noff_ = nullptr;  // lattice of a gathered device-resident batch
-    void* gather_nodes_ = nullptr;
-    void* gather_links_ = nullptr;
-    void* gather_nprob_ = nullptr;
-    size_t gather_noff_cap_ = 0, gather_nodes_cap_ = 0, gather_links_cap_ = 0, gather_nprob_cap_ = 0;
+    DevBuf gather_[kNumArrays];  // the outputs of a gathered device-resident batch, on the first device
+    Outputs made_;               // the arrays the last device-resident call produced
+    Totals made_total_{};
     int lattice_ = 0;  // option "lattice"
-    bool dev_lat_ = false;
-    uint64_t dev_nodes_ = 0;
-    void* gather_soff_ = nullptr;  // samples of a gathered device-resident batch
-    void* gather_samples_ = nullptr;
-    size_t gather_soff_cap_ = 0, gather_samples_cap_ = 0;
-    bool dev_samp_ = false;
-    uint64_t dev_samples_ = 0;
     float stage_ms_[kNumStages];
     uint64_t counters_[10];
     uint64_t launches_ = 0;
