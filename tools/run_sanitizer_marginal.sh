@@ -1,6 +1,6 @@
 #!/bin/bash
 # Developer tool (needs a CUDA GPU): compute-sanitizer memcheck over tests/probes/marginal_probe.py, the marginal
-# routes (k_marg_forward, k_marg_backward, k_backtrack_write_marg, the %pP format kernels; whole batch, chunked,
+# routes (k_marg_forward, k_marg_backward, k_backtrack<true>, the %pP format kernels; whole batch, chunked,
 # device-resident and bounded input).
 #     tools/run_sanitizer_marginal.sh [log directory]      (default: a new temporary directory)
 cd "$(dirname "$0")/.."

@@ -38,6 +38,7 @@ struct Control {  // one small block zeroed per batch and read back once
     unsigned long long total[kNumGroups];  // records of each output group in the batch (or chunk)
     uint32_t flags;
     uint32_t total_slots;
+    uint32_t tickets[2];  // tile tickets of k_front and k_backtrack (TileScan)
 };
 
 // Entries the workspace must hold per batch: the segment pool and the lattice rows are sized from one learned count,
@@ -144,7 +145,7 @@ __global__ void k_add_value(unsigned long long* tok_off, uint32_t n_plus_1, unsi
 
 struct Workspace {  // every per-(chunk of a)-batch device array; two of them let consecutive chunks overlap
     DevBuf n_slots, slot_off, eos, n_tok, code_sys, code_usr, cinfo, groupable, byte_pos, info, info_ex, ends_cnt,
-        ends_meta, seg, ends_hot, ends_cold, scan_tmp, stats, iota, sort_keys, order;
+        ends_meta, seg, ends_hot, ends_cold, scan_tmp, stats, iota, sort_keys, order, tiles;
     DevBuf bnd_dist;  // bounded batches only: Batch::bnd_dist
     DevBuf m_fill, m_ncand, m_cand_entry, m_R, m_ab, m_r_eos, m_a_eos;  // marginals only: MargArgs
     DevBuf l_row_base, l_n_nodes;  // lattice output only: LatticeArgs
@@ -153,7 +154,7 @@ struct Workspace {  // every per-(chunk of a)-batch device array; two of them le
     void release() {
         for (DevBuf* b : {&n_slots, &slot_off, &eos, &n_tok, &code_sys, &code_usr, &cinfo, &groupable, &byte_pos, &info,
                           &info_ex, &ends_cnt, &ends_meta, &seg, &ends_hot, &ends_cold, &scan_tmp, &stats, &iota,
-                          &sort_keys, &order, &bnd_dist, &m_fill, &m_ncand, &m_cand_entry, &m_R, &m_ab, &m_r_eos, &m_a_eos,
+                          &sort_keys, &order, &tiles, &bnd_dist, &m_fill, &m_ncand, &m_cand_entry, &m_R, &m_ab, &m_r_eos, &m_a_eos,
                           &l_row_base, &l_n_nodes, &m_lw, &s_cnt, &s_total})
             b->release();
     }
@@ -1303,6 +1304,7 @@ class EngineImpl final : public Engine {
         w.slot_off.ensure(ns * 4, 1.25);
         w.eos.ensure(ns * 16, 1.25);
         w.n_tok.ensure(ns * 4, 1.25);
+        w.tiles.ensure(size_t(scan_tiles(n_sent, kFrontTile) + scan_tiles(n_sent, kBackTileSmall)) * 8 + 8, 1.25);
         if (order_mode_ == 1) {
             w.iota.ensure(ns * 4, 1.25);
             w.sort_keys.ensure(ns * 4, 1.25);
@@ -1476,16 +1478,20 @@ class EngineImpl final : public Engine {
         }
 
         o.launches = 0;
+        const TileScan ts{w.tiles.as<unsigned long long>(), dc->tickets};
         CK(cudaMemsetAsync(dc, 0, sizeof(Control), st));
+        CK(cudaMemsetAsync(ts.state, 0, size_t(scan_tiles(n_sent, kFrontTile) + scan_tiles(n_sent, kBackTileSmall)) * 8, st));
+        // count_chars and scan_slots are folded into k_front, which is booked under decode
         CK(cudaEventRecord(o.ev[0], st));
-        if (n_sent) {
-            launch_count_chars(b, st);
-            o.launches += 6;  // count_chars, decode, candidates, backtrack_count, backtrack_write, publish (+ viterbi below)
-        } else {
-            CK(cudaMemsetAsync(b.n_slots, 0, 4, st));
-        }
         CK(cudaEventRecord(o.ev[1], st));
-        exclusive_scan(w, b.n_slots, b.slot_off, size_t(n_sent) + 1);
+        CK(cudaEventRecord(o.ev[2], st));
+        if (n_sent) {
+            launch_front(dv_, b, ts, st);
+            // front, candidates, the row-offset scan (two cub kernels), backtrack, publish (+ viterbi below)
+            o.launches += 6;
+        } else {
+            CK(cudaMemsetAsync(b.slot_off, 0, 4, st));
+        }
         if (b.order && order_mode_ == 2) {
             k_local_order<<<(n_sent + kOrderTile - 1) / kOrderTile, kOrderTile, 0, st>>>(b.n_slots, n_sent, w.order.as<uint32_t>());
             ++o.launches;
@@ -1499,8 +1505,6 @@ class EngineImpl final : public Engine {
                                                          st));
             ++o.launches;
         }
-        CK(cudaEventRecord(o.ev[2], st));
-        launch_decode(dv_, b, st);
         if (b.bnd_dist && n_sent) {  // the bounded batch's boundaries, booked with the decode stage
             launch_mark_bounds(b, st);
             ++o.launches;
@@ -1516,7 +1520,7 @@ class EngineImpl final : public Engine {
         CK(cudaEventRecord(o.ev[5], st));
         o.launches += launch_viterbi(dv_, b, counting_ ? w.stats.as<uint4>() : nullptr, lanes_, viterbi_kernel_, st, &o.route);
         MargArgs m{};
-        if (marg || samp) {  // booked with the Viterbi stage; must run before K4a reuses ends_meta
+        if (marg || samp) {  // booked with the Viterbi stage; must run before K4 reuses ends_meta
             m.theta = marg ? theta_ : samp_theta_;  // equal when both are on (set_marginals / set_sampling)
             m.fill = w.m_fill.as<uint32_t>();
             m.ncand = w.m_ncand.as<uint32_t>();
@@ -1531,7 +1535,7 @@ class EngineImpl final : public Engine {
             launch_marginals(dv_, b, m, st, marg);  // sampling alone needs no backward pass
             if (n_sent) o.launches += marg ? 2 : 1;
         }
-        if (lat) {  // booked with the Viterbi stage too, and also before K4a
+        if (lat) {  // booked with the Viterbi stage too, and also before K4
             LatticeArgs l{};
             l.row_base = w.l_row_base.as<uint32_t>();
             l.n_nodes = w.l_n_nodes.as<uint32_t>();
@@ -1547,7 +1551,7 @@ class EngineImpl final : public Engine {
             CK(cudaMemcpyAsync(&dc->total[kGroupLattice], l.node_off + n_sent, 8, cudaMemcpyDeviceToDevice, st));
             if (n_sent) o.launches += 2;
         }
-        if (samp) {  // booked with the Viterbi stage too, and also before K4a
+        if (samp) {  // booked with the Viterbi stage too, and also before K4
             SampleArgs sa{};
             sa.n = samp_n_;
             sa.seed = samp_seed_;
@@ -1569,19 +1573,14 @@ class EngineImpl final : public Engine {
             launch_sample_write(dv_, b, m, sa, st);
             if (walks) o.launches += 2;
         }
+        // backtrack_count and scan_tokens are folded into k_backtrack, which is booked under backtrack_write
         CK(cudaEventRecord(o.ev[6], st));
-        launch_backtrack_count(b, st);
         CK(cudaEventRecord(o.ev[7], st));
-        {
-            cub::TransformInputIterator<unsigned long long, CastU64, const uint32_t*> it(b.n_tok, CastU64());
-            if (n_sent == 0) CK(cudaMemsetAsync(b.n_tok, 0, 4, st));
-            exclusive_scan(w, it, b.tok_off, size_t(n_sent) + 1);
-        }
         CK(cudaEventRecord(o.ev[8], st));
-        if (marg)
-            launch_backtrack_write_marg(b, m, st);
+        if (n_sent)
+            launch_backtrack(b, marg ? &m : nullptr, ts, st);
         else
-            launch_backtrack_write(b, st);
+            CK(cudaMemsetAsync(b.tok_off, 0, 8, st));
         k_publish_totals<<<1, 1, 0, st>>>(b.slot_off, b.tok_off, n_sent, dc);
         if (o.made.text) {  // output stage of a chunk: formatted while its token offsets are still chunk-local
             FormatArgs f = format_offsets(w, d_utf8, d_off, n_sent, o);
@@ -1651,7 +1650,7 @@ class EngineImpl final : public Engine {
     bool counting_ = false;
     int order_mode_ = 0;  // K3's sentence order: 0 input order, 1 whole batch by length, 2 by length inside tiles
     uint32_t output_mode_ = 0;
-    uint64_t batch_total_bytes_ = 0;  // size of the input buffer of the batch in flight (bounds check in K1a)
+    uint64_t batch_total_bytes_ = 0;  // size of the input buffer of the batch in flight (bounds check in K1)
     // output text bytes expected per input byte (beyond text_per_sent_ per sentence), by output mode: sizes the text
     // buffers of the chunked host pipeline, learned like cand_per_byte_
     static constexpr double kFormatTextPerByte = 8.0;

@@ -1,11 +1,10 @@
 // Hand-written sm_90a (H100) kernels of the batched Viterbi tokenizer.
 //
-//   K1a count_chars     warp / sentence   UTF-8 validation + character count
-//   K1b decode          warp / sentence   code points -> CharInfo, trie codes, c2b, groupable
+//   K1  front           warp / sentence   UTF-8 validation + character count, slot offsets (look-back scan),
+//                                         code points -> CharInfo, trie codes, c2b, groupable
 //   K2  candidates      thread / char     common-prefix walks (user, system) + unknown words
 //   K3  viterbi         warp / sentence   left-to-right min-plus DP over the lattice + EOS
-//   K4a backtrack_count thread / sentence length of the best path
-//   K4b backtrack_write thread / sentence token records, in sentence order
+//   K4  backtrack       thread / sentence best path, token offsets (look-back scan), then thread / token records
 //
 // Everything is integer gather / compare work: no tensor cores.  Citations are relative to
 // /root/reference/vibrato/src/ and name the reference routine whose RESULT each step reproduces.
@@ -27,7 +26,7 @@ constexpr uint32_t kMask = 0x7FFFFFFFu;
 constexpr uint32_t kFlag = 0x80000000u;
 constexpr unsigned kFull = 0xFFFFFFFFu;
 
-// A batch whose byte offsets k_count_chars refused is not touched by any later kernel: the sizes derived from
+// A batch whose byte offsets k_front refused is not touched by any later kernel: the sizes derived from
 // the offsets (slots, workspace bounds) cannot be trusted.
 __device__ __forceinline__ bool stand_down(uint32_t batch_flags) { return batch_flags & kFlagsStandDown; }
 
@@ -51,7 +50,7 @@ __device__ __forceinline__ unsigned long long warp_sum(unsigned long long v) {
 }
 
 // ---------------------------------------------------------------------------------------------
-// K1a: characters per sentence + UTF-8 validity (what `&str` guarantees before worker.rs:34)
+// Characters per sentence + UTF-8 validity (what `&str` guarantees before worker.rs:34)
 // ---------------------------------------------------------------------------------------------
 
 __device__ __forceinline__ uint32_t utf8_len_checked(const uint8_t* p, unsigned long long i, unsigned long long len,
@@ -83,22 +82,16 @@ __device__ __forceinline__ uint32_t utf8_len_checked(const uint8_t* p, unsigned 
     return L;
 }
 
-// Sentences per warp of the warp-per-sentence kernels (K1a, K1b, K4b): a warp walks a few consecutive sentences so
+// Sentences per warp of the warp-per-sentence kernels (k_mark_bounds, the marginals): a warp walks a few consecutive sentences so
 // that the grid has fewer, longer-lived blocks.
 #ifndef VBT_SENT_PER_WARP
 #define VBT_SENT_PER_WARP 4
 #endif
 
-__device__ __forceinline__ void count_chars_one(const Batch& b, uint32_t s, uint32_t lane) {
-    unsigned long long bo = b.byte_off[s], len = b.byte_off[s + 1] - bo;
-    if (b.byte_off[s + 1] < bo || b.byte_off[s + 1] > b.total_bytes) {  // caller error: nothing of this sentence is read
-        if (lane == 0) {
-            atomicOr(b.flags, kFlagBadOffsets);
-            b.n_slots[s] = 1;
-        }
-        return;
-    }
-    const uint8_t* p = b.utf8 + bo;
+// Characters of the sentence in p[0, len) (shared or global memory) with the validity rules of `&str`; lane 0 raises the
+// batch flags, adds the counters and stores and returns the sentence's slots (characters + 1), 1 for invalid UTF-8.
+__device__ __forceinline__ uint32_t count_chars_at(const Batch& b, const uint8_t* p, unsigned long long len, uint32_t* n_slots,
+                                                   uint32_t lane) {
     unsigned long long nchar = 0, covered = 0;
     bool bad = false;
     for (unsigned long long i0 = 0; i0 < len; i0 += 32) {
@@ -119,28 +112,30 @@ __device__ __forceinline__ void count_chars_one(const Batch& b, uint32_t s, uint
             atomicOr(b.flags, kFlagUtf8Error);
             nchar = 0;  // keep the rest of the pipeline in bounds; the batch is rejected anyway
         }
-        b.n_slots[s] = uint32_t(nchar) + 1;
+        *n_slots = uint32_t(nchar) + 1;
         if (nchar > kPruneMaxChars) atomicOr(b.flags, kFlagLongSentence);
         if (b.counters) {
             atomicAdd(&b.counters[kCntU], len);
             atomicAdd(&b.counters[kCntC], nchar);
         }
     }
+    return uint32_t(nchar) + 1;
 }
 
-__global__ void __launch_bounds__(256) k_count_chars(Batch b) {
-    const uint32_t w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    const uint32_t lane = threadIdx.x & 31;
-#pragma unroll 1
-    for (uint32_t r = 0; r < VBT_SENT_PER_WARP; ++r) {
-        const uint32_t s = w * VBT_SENT_PER_WARP + r;
-        if (s >= b.n_sent) return;
-        count_chars_one(b, s, lane);
+__device__ __forceinline__ void count_chars_one(const Batch& b, uint32_t s, uint32_t lane) {
+    unsigned long long bo = b.byte_off[s], len = b.byte_off[s + 1] - bo;
+    if (b.byte_off[s + 1] < bo || b.byte_off[s + 1] > b.total_bytes) {  // caller error: nothing of this sentence is read
+        if (lane == 0) {
+            atomicOr(b.flags, kFlagBadOffsets);
+            b.n_slots[s] = 1;
+        }
+        return;
     }
+    count_chars_at(b, b.utf8 + bo, len, &b.n_slots[s], lane);
 }
 
 // ---------------------------------------------------------------------------------------------
-// K1b: Sentence::compile (sentence.rs:34-71) for every sentence
+// Sentence::compile (sentence.rs:34-71) for every sentence
 // ---------------------------------------------------------------------------------------------
 
 __device__ __forceinline__ void decode_one(const DictView& d, const Batch& b, uint32_t s, uint32_t lane) {
@@ -209,15 +204,200 @@ __device__ __forceinline__ void decode_one(const DictView& d, const Batch& b, ui
     }
 }
 
-__global__ void __launch_bounds__(256) k_decode(DictView d, Batch b) {
-    if (stand_down(*b.flags)) return;
-    const uint32_t w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    const uint32_t lane = threadIdx.x & 31;
+// decode_one for a sentence of n <= kFrontWarpChars characters in p[0, len) (shared or global memory), a lane per
+// character: buf (the warp's, in shared memory) first maps characters to their lead bytes and then holds their CharInfo
+// for groupable, so that every array is written 32 consecutive slots at a time and nothing is read back.
+constexpr uint32_t kFrontWarpChars = 512;
+__device__ __forceinline__ void decode_sentence_smem(const DictView& d, const Batch& b, const uint8_t* p,
+                                                     unsigned long long len, uint32_t base, uint32_t n, uint32_t* buf,
+                                                     uint32_t lane) {
+    uint32_t running = 0;
+    for (unsigned long long i0 = 0; n > 0 && i0 < len; i0 += 32) {
+        const unsigned long long i = i0 + lane;
+        const bool lead = i < len && (p[i] & 0xC0) != 0x80;
+        const uint32_t m = __ballot_sync(kFull, lead);
+        const uint32_t idx = running + __popc(m & lanemask_lt());
+        if (lead && idx < n) buf[idx] = uint32_t(i);
+        running += __popc(m);
+    }
+    __syncwarp();
+    for (uint32_t idx = lane; idx < n; idx += 32) {
+        const uint32_t i = buf[idx], slot = base + idx;
+        const uint32_t c = p[i], c1 = i + 1 < len ? p[i + 1] : 0, c2 = i + 2 < len ? p[i + 2] : 0,
+                       c3 = i + 3 < len ? p[i + 3] : 0;
+        uint32_t cp;  // compute_basic sentence.rs:40-46
+        if (c < 0x80)
+            cp = c;
+        else if (c < 0xE0)
+            cp = ((c & 0x1F) << 6) | (c1 & 0x3F);
+        else if (c < 0xF0)
+            cp = ((c & 0x0F) << 12) | ((c1 & 0x3F) << 6) | (c2 & 0x3F);
+        else
+            cp = ((c & 0x07) << 18) | ((c1 & 0x3F) << 12) | ((c2 & 0x3F) << 6) | (c3 & 0x3F);
+        b.byte_pos[slot] = i;
+        // CharProperty::char_info character.rs:112-116: out-of-table code points use entry 0
+        const uint32_t ci = __ldg(&d.chr2inf[cp < d.chr2inf_len ? cp : 0]);
+        b.cinfo[slot] = ci;
+        b.code_sys[slot] = cp < d.sys_table_len ? __ldg(&d.sys_table[cp]) : kInvalidCode;
+        if (d.usr_table) b.code_usr[slot] = cp < d.usr_table_len ? __ldg(&d.usr_table[cp]) : kInvalidCode;
+        b.ends_cnt[slot] = idx == 0 ? 1u : 0u;  // BOS lives in ends[0] (lattice.rs:72-83)
+        buf[idx] = ci;
+    }
+    if (lane == 0) {  // sentinel slot == character position n
+        const uint32_t slot = base + n;
+        b.byte_pos[slot] = uint32_t(len);
+        b.cinfo[slot] = 0;
+        b.groupable[slot] = 0;
+        b.code_sys[slot] = kInvalidCode;
+        if (d.usr_table) b.code_usr[slot] = kInvalidCode;
+        b.ends_cnt[slot] = 0;
+        b.info[slot] = make_uint2(0, 0);
+    }
+    __syncwarp();
+    uint32_t carry = 0;  // groupable as decode_one solves it
+    for (int k = int((n + 31) / 32) - 1; k >= 0; --k) {
+        const uint32_t c = uint32_t(k) * 32 + lane;
+        const bool valid = c < n;
+        const uint32_t ci = valid ? buf[c] : 0, cn = (c + 1 < n) ? buf[c + 1] : 0;
+        const bool brk = valid && (c + 1 == n || (ci_cate(ci) & ci_cate(cn)) == 0);
+        const uint32_t m = __ballot_sync(kFull, brk) >> lane;
+        const uint32_t g = m ? uint32_t(__ffs(m)) : (min(32u, n - uint32_t(k) * 32) - lane) + carry;
+        if (valid) b.groupable[base + c] = g;
+        carry = __shfl_sync(kFull, g, 0);
+    }
+    __syncwarp();  // buf is the warp's next sentence's
+}
+
+// ---------------------------------------------------------------------------------------------
+// Single-pass exclusive scans with decoupled look-back (k_front: slots per sentence, k_backtrack: tokens per sentence).
+// A block takes its tile from a ticket counter, so every tile it waits for belongs to a block that is already running.
+// Each tile has one word: its status in the top two bits (kTileAgg: the tile's own total is known, kTileIncl: the
+// total of every tile up to and including it) and the value in the low 62 bits.
+// ---------------------------------------------------------------------------------------------
+
+constexpr unsigned long long kTileAgg = 1ull << 62, kTileIncl = 2ull << 62, kTileValue = kTileAgg - 1;
+
+__device__ __forceinline__ uint32_t take_tile(uint32_t* ticket, uint32_t* s_tile) {
+    if (threadIdx.x == 0) *s_tile = atomicAdd(ticket, 1u);
+    __syncthreads();
+    return *s_tile;
+}
+
+// Warp 0 of the block of `tile`, whose own total is `agg`: returns the total of the tiles before it (every lane) and
+// publishes the inclusive total.  The fences order each tile's batch flags before its published values, so that a
+// tile that has its prefix also sees the flags every tile before it raised.
+__device__ unsigned long long tile_prefix(unsigned long long* state, uint32_t tile, unsigned long long agg, uint32_t lane) {
+    if (lane == 0) {
+        __threadfence();
+        atomicExch(&state[tile], (tile == 0 ? kTileIncl : kTileAgg) | (agg & kTileValue));
+    }
+    unsigned long long excl = 0;
+    for (long long j = (long long)tile - 1; j >= 0; j -= 32) {  // lane l looks at tile j - l
+        const long long t = j - lane;
+        unsigned long long w;
+        do
+            w = t >= 0 ? *reinterpret_cast<volatile unsigned long long*>(&state[t]) : (unsigned long long)kTileIncl;
+        while (__any_sync(kFull, w < kTileAgg));
+        const uint32_t incl = __ballot_sync(kFull, w >= kTileIncl);
+        const uint32_t upto = incl ? uint32_t(__ffs(incl)) - 1 : 31u;  // the nearest inclusive total ends the walk
+        excl += warp_sum(lane <= upto ? (w & kTileValue) : 0ull);
+        if (incl) break;
+    }
+    __threadfence();
+    if (lane == 0 && tile != 0) atomicExch(&state[tile], kTileIncl | ((excl + agg) & kTileValue));
+    return excl;
+}
+
+// ---------------------------------------------------------------------------------------------
+// K1: count_chars + slot-offset scan + Sentence::compile (sentence.rs:34-71), one pass over tiles of kFrontTile
+// consecutive sentences (a warp per sentence).  The tile's text is staged in shared memory when it fits in
+// kFrontStage bytes; otherwise, and for sentences outside the staged range (offsets out of order), it is read from
+// global memory.  n_slots (the sort key of the K3 order) and slot_off are written for every sentence; a tile decodes
+// only when no tile up to it has bad offsets, which could otherwise carry the slots past the arrays' n_bytes + n_sent.
+// ---------------------------------------------------------------------------------------------
+
+static_assert(kFrontTile == 32, "warp 0 scans the tile's counts");
+constexpr uint32_t kFrontStage = 16384;
+
+__global__ void __launch_bounds__(256) k_front(DictView d, Batch b, unsigned long long* tile_state, uint32_t* ticket) {
+    __shared__ __align__(16) uint8_t s_text[kFrontStage + 32];
+    __shared__ uint32_t s_buf[8][kFrontWarpChars];
+    __shared__ uint32_t s_n[kFrontTile], s_off[kFrontTile];
+    __shared__ uint32_t s_tile, s_stand;
+    const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    const uint32_t tile = take_tile(ticket, &s_tile);
+    const uint32_t s0 = tile * kFrontTile, nt = min(kFrontTile, b.n_sent - s0);
+    const unsigned long long lo = b.byte_off[s0], hi = b.byte_off[s0 + nt];
+    const bool staged = lo <= hi && hi <= b.total_bytes && hi - lo <= kFrontStage;
+    // s_text[head + x] = byte lo + x; 16-byte loads between the 16-byte boundaries, single bytes at either end
+    const uint32_t head = uint32_t(reinterpret_cast<uintptr_t>(b.utf8 + lo) & 15u);
+    if (staged) {
+        const uint8_t* a0 = b.utf8 + lo - head;
+        const uint32_t span = head + uint32_t(hi - lo);
+        for (uint32_t c0 = threadIdx.x * 16; c0 < span; c0 += 256 * 16) {
+            if (c0 >= head && c0 + 16 <= span) {
+                *reinterpret_cast<uint4*>(s_text + c0) = __ldg(reinterpret_cast<const uint4*>(a0 + c0));
+            } else {
+                for (uint32_t q = max(c0, head); q < min(c0 + 16, span); ++q) s_text[q] = a0[q];
+            }
+        }
+    }
+    __syncthreads();
+    auto text = [&](unsigned long long bo, unsigned long long eo) -> const uint8_t* {
+        return staged && bo >= lo && eo <= hi ? s_text + head + (bo - lo) : b.utf8 + bo;
+    };
+    constexpr uint32_t kPerWarp = kFrontTile / 8;
 #pragma unroll 1
-    for (uint32_t r = 0; r < VBT_SENT_PER_WARP; ++r) {
-        const uint32_t s = w * VBT_SENT_PER_WARP + r;
-        if (s >= b.n_sent) return;
-        decode_one(d, b, s, lane);
+    for (uint32_t r = 0; r < kPerWarp; ++r) {
+        const uint32_t t = wid * kPerWarp + r;
+        if (t >= nt) break;
+        const uint32_t s = s0 + t;
+        const unsigned long long bo = b.byte_off[s], eo = b.byte_off[s + 1];
+        uint32_t ns = 1;
+        if (eo < bo || eo > b.total_bytes) {  // caller error: nothing of this sentence is read
+            if (lane == 0) {
+                atomicOr(b.flags, kFlagBadOffsets);
+                b.n_slots[s] = 1;
+            }
+        } else {
+            ns = count_chars_at(b, text(bo, eo), eo - bo, &b.n_slots[s], lane);
+        }
+        if (lane == 0) s_n[t] = ns;
+    }
+    __syncthreads();
+    if (wid == 0) {
+        const uint32_t v = lane < nt ? s_n[lane] : 0u;
+        uint32_t x = v;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const uint32_t y = __shfl_up_sync(kFull, x, o);
+            if (lane >= uint32_t(o)) x += y;
+        }
+        const uint32_t agg = __shfl_sync(kFull, x, 31);
+        // slot counts wrap like the u32 slot offsets; a batch where they could is rejected (kFlagBadOffsets)
+        const uint32_t base = uint32_t(tile_prefix(tile_state, tile, agg, lane));
+        if (lane < nt) {
+            s_off[lane] = base + x - v;
+            b.slot_off[s0 + lane] = base + x - v;
+        }
+        if (lane == 0) {
+            // also the next tile's first offset (the same value), which decode_one reads for the tile's last sentence
+            b.slot_off[s0 + nt] = base + agg;
+            s_stand = stand_down(*reinterpret_cast<volatile uint32_t*>(b.flags));
+        }
+    }
+    __syncthreads();
+    if (s_stand) return;
+#pragma unroll 1
+    for (uint32_t r = 0; r < kPerWarp; ++r) {
+        const uint32_t t = wid * kPerWarp + r;
+        if (t >= nt) break;
+        const unsigned long long bo = b.byte_off[s0 + t], eo = b.byte_off[s0 + t + 1];
+        const uint32_t n = s_n[t] - 1;
+        if (n <= kFrontWarpChars)
+            decode_sentence_smem(d, b, text(bo, eo), eo - bo, s_off[t], n, s_buf[wid], lane);
+        else
+            decode_one(d, b, s0 + t, lane);
         __syncwarp();
     }
 }
@@ -1229,11 +1409,10 @@ __global__ void __launch_bounds__(32 * VBT_K3V2_WARPS, CONN == 0 ? VBT_K3V2_MIN_
 // K4: Lattice::append_top_nodes (lattice.rs:159-168) + Token accessors (token.rs:21-92)
 // ---------------------------------------------------------------------------------------------
 
-// K4a walks the best path once (thread / sentence): it counts the tokens and leaves, for the k-th node from the
+// The path walk (backtrack_count_one, a thread per sentence) counts the tokens and leaves, for the k-th node from the
 // end, {lattice entry, end position} in the sentence's own stretch of `ends_meta` (dead after K3, one entry per
-// character, and a path has at most one node per character).  After the token-offset scan K4b turns those entries
-// into token records with a warp per sentence — the pointer chase is not repeated and the 24-byte records of a
-// sentence are written by neighbouring lanes.
+// character, and a path has at most one node per character).  Once the token offsets are known the records are built
+// from those entries — the pointer chase is not repeated and neighbouring lanes write neighbouring records.
 __device__ __forceinline__ void backtrack_count_one(const Batch& b, uint32_t s) {
     uint4 e = b.eos[s];
     uint32_t k = 0;
@@ -1250,13 +1429,6 @@ __device__ __forceinline__ void backtrack_count_one(const Batch& b, uint32_t s) 
     }
     b.n_tok[s] = k;
     if (b.counters && k) atomicAdd(&b.counters[kCntK], (unsigned long long)k);
-}
-
-__global__ void __launch_bounds__(256) k_backtrack_count(Batch b) {
-    if (stand_down(*b.flags)) return;
-    uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
-    if (s >= b.n_sent) return;
-    backtrack_count_one(b, s);
 }
 
 // Token records of sentence s at tok_off[s], from the path entries backtrack_count_one left (a warp per sentence).
@@ -1284,15 +1456,101 @@ __device__ __forceinline__ void backtrack_write_one(const Batch& b, uint32_t s, 
     }
 }
 
-__global__ void __launch_bounds__(256) k_backtrack_write(Batch b) {
-    if (stand_down(*b.flags)) return;
-    const uint32_t w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    const uint32_t lane = threadIdx.x & 31;
+// K4: backtrack_count + token-offset scan + records, one pass over tiles of TILE consecutive sentences: a thread
+// chases each sentence's path, the tile looks back for its token offset (tile_prefix), then the block (256 threads)
+// writes the tile's records, which are contiguous, a thread per record.  MARG: with the marginal of every token,
+// prob = exp(â + b̂ - â(EOS)) of its lattice entry.  A rejected batch (stand_down) gets no records and zero token
+// offsets.  TILE = kBackTile, or kBackTileSmall for batches too small to give every SM a kBackTile tile.
+static_assert(kBackTile == 256, "a thread per sentence, eight warps");
+
+template <bool MARG, uint32_t TILE>
+__global__ void __launch_bounds__(256) k_backtrack(Batch b, MargArgs m, unsigned long long* tile_state,
+                                                   uint32_t* ticket) {
+    __shared__ uint32_t s_off[TILE + 1], s_base[TILE], s_warp[8];
+    __shared__ uint32_t s_tile;
+    __shared__ unsigned long long s_excl;
+    const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    const uint32_t tile = take_tile(ticket, &s_tile);
+    const uint32_t s0 = tile * TILE, nt = min(TILE, b.n_sent - s0);
+    const bool stand = stand_down(*b.flags);
+    const uint32_t s = s0 + threadIdx.x;
+    uint32_t k = 0;
+    if (!stand && threadIdx.x < nt) {
+        backtrack_count_one(b, s);
+        k = b.n_tok[s];
+        s_base[threadIdx.x] = b.slot_off[s];
+    }
+    uint32_t x = k;  // block-wide exclusive scan of the token counts
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const uint32_t y = __shfl_up_sync(kFull, x, o);
+        if (lane >= uint32_t(o)) x += y;
+    }
+    if (lane == 31) s_warp[wid] = x;
+    __syncthreads();
+    uint32_t before = 0, agg = 0;
+    for (uint32_t i = 0; i < 8; ++i) {
+        before += i < wid ? s_warp[i] : 0u;
+        agg += s_warp[i];
+    }
+    const uint32_t local = before + x - k;
+    if (threadIdx.x < TILE) s_off[threadIdx.x] = local;  // == agg from thread nt on
+    if (threadIdx.x == 255) s_off[TILE] = agg;
+    if (wid == 0) {
+        const unsigned long long excl = tile_prefix(tile_state, tile, agg, lane);
+        if (lane == 0) {
+            s_excl = excl;
+            if (s0 + nt == b.n_sent) b.tok_off[b.n_sent] = excl + agg;
+        }
+    }
+    __syncthreads();
+    const unsigned long long excl = s_excl;
+    if (threadIdx.x < nt) b.tok_off[s] = excl + local;
+    if (stand) return;
+    // kRecBatch records per thread at a time, each gather step issued for all of them before the next: the chain
+    // path entry -> ends_cold -> info -> byte_pos is three dependent round trips per record
+    constexpr uint32_t kRecBatch = 4;
 #pragma unroll 1
-    for (uint32_t r = 0; r < VBT_SENT_PER_WARP; ++r) {
-        const uint32_t s = w * VBT_SENT_PER_WARP + r;
-        if (s >= b.n_sent) return;
-        backtrack_write_one(b, s, lane);
+    for (uint32_t i0 = threadIdx.x; i0 < agg; i0 += 256 * kRecBatch) {
+        uint32_t j[kRecBatch];
+        uint2 pe[kRecBatch];
+        uint4 c[kRecBatch];
+        uint2 i8[kRecBatch];
+#pragma unroll
+        for (uint32_t q = 0; q < kRecBatch; ++q) {
+            const uint32_t i = i0 + q * 256;
+            j[q] = 0;  // the tile's sentence of token i: the last j with s_off[j] <= i
+            for (uint32_t step = TILE / 2; step > 0; step >>= 1)
+                if (j[q] + step < nt && s_off[j[q] + step] <= i) j[q] += step;
+            const uint32_t n = s_off[j[q] + 1] - s_off[j[q]];
+            if (i < agg) pe[q] = b.ends_meta[s_base[j[q]] + (n - 1 - (i - s_off[j[q]]))];  // the kk-th node from the end
+        }
+#pragma unroll
+        for (uint32_t q = 0; q < kRecBatch; ++q)
+            if (i0 + q * 256 < agg) c[q] = b.ends_cold[pe[q].x];
+#pragma unroll
+        for (uint32_t q = 0; q < kRecBatch; ++q)
+            if (i0 + q * 256 < agg) i8[q] = b.info[c[q].x];
+#pragma unroll
+        for (uint32_t q = 0; q < kRecBatch; ++q) {
+            const uint32_t i = i0 + q * 256;
+            if (i >= agg) break;
+            const uint32_t base = s_base[j[q]], start_node = c[q].x - base;
+            const uint32_t start_word = start_node + ((i8[q].y & kInfoSpecial) ? b.info_ex[c[q].x].x : 0u);  // token.rs:21-24
+            const uint2 bytes = make_uint2(b.byte_pos[base + start_word], b.byte_pos[base + pe[q].y]);  // token.rs:28-32
+            if (b.compact) {
+                reinterpret_cast<uint4*>(b.tokens)[excl + i] = make_uint4(bytes.x, bytes.y, c[q].z, c[q].w);
+            } else {
+                uint2* t = reinterpret_cast<uint2*>(b.tokens) + (excl + i) * 3;
+                t[0] = make_uint2(start_word, pe[q].y);
+                t[1] = bytes;
+                t[2] = make_uint2(c[q].z, c[q].w);  // word_idx, total_cost
+            }
+            if (MARG) {
+                const double2 ab = m.ab[pe[q].x];
+                m.token_prob[excl + i] = float(exp(ab.x + ab.y - m.a_eos[s0 + j[q]]));
+            }
+        }
     }
 }
 
@@ -1466,27 +1724,6 @@ __global__ void __launch_bounds__(256) k_marg_backward(DictView d, Batch b, Marg
     }
 }
 
-// K4b with the marginal of every token: prob = exp(â + b̂ - â(EOS)) of its lattice entry.
-__global__ void __launch_bounds__(256) k_backtrack_write_marg(Batch b, MargArgs m) {
-    if (stand_down(*b.flags)) return;
-    const uint32_t w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    const uint32_t lane = threadIdx.x & 31;
-#pragma unroll 1
-    for (uint32_t r = 0; r < VBT_SENT_PER_WARP; ++r) {
-        const uint32_t s = w * VBT_SENT_PER_WARP + r;
-        if (s >= b.n_sent) return;
-        backtrack_write_one(b, s, lane);
-        const uint32_t base = b.slot_off[s];
-        const unsigned long long t0 = b.tok_off[s];
-        const uint32_t n = uint32_t(b.tok_off[s + 1] - t0);
-        const double a_eos = n ? m.a_eos[s] : 0.0;
-        for (uint32_t k = lane; k < n; k += 32) {
-            const double2 ab = m.ab[b.ends_meta[base + k].x];
-            m.token_prob[t0 + (n - 1 - k)] = float(exp(ab.x + ab.y - a_eos));
-        }
-    }
-}
-
 // ---------------------------------------------------------------------------------------------
 // Lattice output (LatticeArgs in kernels.cuh): one warp per sentence over the rows K3 filled, ends_meta[slot] =
 // {row offset, fill}.  The first slot's row holds only BOS, which is not a node.
@@ -1553,7 +1790,7 @@ __global__ void __launch_bounds__(256) k_lattice_write(Batch b, LatticeArgs l, M
             l.links[k] = make_int2(prev, 0);
             if (l.node_prob) {
                 const double2 ab = m.ab[e];
-                l.node_prob[k] = float(exp(ab.x + ab.y - a_eos));  // the expression of k_backtrack_write_marg
+                l.node_prob[k] = float(exp(ab.x + ab.y - a_eos));  // the expression of k_backtrack<true>
             }
         }
     }
@@ -2488,16 +2725,9 @@ void launch_field_table_write(const DictView& d, const FieldTableArgs& a, cudaSt
     if (a.n_words) k_field_table_write<<<(a.n_words + 255) / 256, 256, 0, st>>>(d, a);
 }
 
-void launch_count_chars(const Batch& b, cudaStream_t st) {
+void launch_front(const DictView& d, const Batch& b, const TileScan& ts, cudaStream_t st) {
     if (!b.n_sent) return;
-    uint32_t blocks = (b.n_sent + 8 * VBT_SENT_PER_WARP - 1) / (8 * VBT_SENT_PER_WARP);
-    k_count_chars<<<blocks, 256, 0, st>>>(b);
-}
-
-void launch_decode(const DictView& d, const Batch& b, cudaStream_t st) {
-    if (!b.n_sent) return;
-    uint32_t blocks = (b.n_sent + 8 * VBT_SENT_PER_WARP - 1) / (8 * VBT_SENT_PER_WARP);
-    k_decode<<<blocks, 256, 0, st>>>(d, b);
+    k_front<<<scan_tiles(b.n_sent, kFrontTile), 256, 0, st>>>(d, b, ts.state, ts.ticket);
 }
 
 void launch_mark_bounds(const Batch& b, cudaStream_t st) {
@@ -2586,14 +2816,24 @@ int launch_viterbi(const DictView& d, const Batch& b, const uint4* stats, int la
 }
 
 
-void launch_backtrack_count(const Batch& b, cudaStream_t st) {
-    if (!b.n_sent) return;
-    k_backtrack_count<<<(b.n_sent + 255) / 256, 256, 0, st>>>(b);
+template <bool MARG>
+static void launch_backtrack_marg(const Batch& b, const MargArgs& m, const TileScan& ts, cudaStream_t st) {
+    int dev = 0, sms = 0;  // on failure sms stays 0 and the large tile is taken
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    unsigned long long* state = ts.state + scan_tiles(b.n_sent, kFrontTile);
+    if (b.n_sent >= uint64_t(kBackTile) * uint32_t(sms))
+        k_backtrack<MARG, kBackTile><<<scan_tiles(b.n_sent, kBackTile), 256, 0, st>>>(b, m, state, ts.ticket + 1);
+    else
+        k_backtrack<MARG, kBackTileSmall><<<scan_tiles(b.n_sent, kBackTileSmall), 256, 0, st>>>(b, m, state, ts.ticket + 1);
 }
 
-void launch_backtrack_write(const Batch& b, cudaStream_t st) {
+void launch_backtrack(const Batch& b, const MargArgs* m, const TileScan& ts, cudaStream_t st) {
     if (!b.n_sent) return;
-    k_backtrack_write<<<(b.n_sent + 8 * VBT_SENT_PER_WARP - 1) / (8 * VBT_SENT_PER_WARP), 256, 0, st>>>(b);  // warps over sentences
+    if (m)
+        launch_backtrack_marg<true>(b, *m, ts, st);
+    else
+        launch_backtrack_marg<false>(b, MargArgs{}, ts, st);
 }
 
 // The forward pass's instantiation: with m.lw (sampling) the one that also keeps {left id, word cost}.
@@ -2615,11 +2855,6 @@ void launch_marginals(const DictView& d, const Batch& b, const MargArgs& m, cuda
         launch_marg_conn<2>(d, b, m, backward, blocks, st);
     else
         launch_marg_conn<0>(d, b, m, backward, blocks, st);
-}
-
-void launch_backtrack_write_marg(const Batch& b, const MargArgs& m, cudaStream_t st) {
-    if (!b.n_sent) return;
-    k_backtrack_write_marg<<<(b.n_sent + 8 * VBT_SENT_PER_WARP - 1) / (8 * VBT_SENT_PER_WARP), 256, 0, st>>>(b, m);
 }
 
 void launch_lattice_count(const Batch& b, const LatticeArgs& l, cudaStream_t st) {

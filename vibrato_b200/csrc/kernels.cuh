@@ -181,9 +181,17 @@ struct FieldTableArgs {
 void launch_field_table_len(const DictView& d, const FieldTableArgs& a, cudaStream_t st);
 void launch_field_table_write(const DictView& d, const FieldTableArgs& a, cudaStream_t st);
 
-void launch_count_chars(const Batch& b, cudaStream_t st);
-void launch_decode(const DictView& d, const Batch& b, cudaStream_t st);
-// Bounded batches (b.bnd_dist != nullptr): writes bnd_dist from the boundary lists after launch_decode and
+// State of the single-pass scans of k_front and k_backtrack: scan_tiles(n_sent, kFrontTile) +
+// scan_tiles(n_sent, kBackTileSmall) words of `state` and two ticket counters, all zero before the batch.
+struct TileScan {
+    unsigned long long* state;
+    uint32_t* ticket;
+};
+constexpr uint32_t kFrontTile = 32, kBackTile = 256, kBackTileSmall = 32;  // sentences per tile
+inline uint32_t scan_tiles(uint32_t n_sent, uint32_t tile) { return (n_sent + tile - 1) / tile; }
+// count_chars, the slot-offset scan and decode: n_slots, slot_off (n_sent + 1 entries) and every per-slot array.
+void launch_front(const DictView& d, const Batch& b, const TileScan& ts, cudaStream_t st);
+// Bounded batches (b.bnd_dist != nullptr): writes bnd_dist from the boundary lists after launch_front and
 // validates them (kFlagBadBoundary).
 void launch_mark_bounds(const Batch& b, cudaStream_t st);
 // b.bnd_dist != nullptr selects the bounded instantiation of k_candidates: no candidate crosses a marked boundary.
@@ -210,11 +218,9 @@ inline ViterbiRoute resolve_viterbi_route(uint32_t launched, uint32_t batch_flag
 }
 int launch_viterbi(const DictView& d, const Batch& b, const uint4* stats, int lanes_per_sentence, int kernel,
                    cudaStream_t st, uint32_t* route);
-void launch_backtrack_count(const Batch& b, cudaStream_t st);
-void launch_backtrack_write(const Batch& b, cudaStream_t st);
 
-// Marginal probabilities: forward-backward over the lattice K3 left in ends_hot / ends_meta, between K3 and K4a
-// (K4a overwrites ends_meta).  Per lattice entry n, with R(n) the exact (64-bit) minimum cost from BOS to n:
+// Marginal probabilities: forward-backward over the lattice K3 left in ends_hot / ends_meta, between K3 and K4
+// (K4 overwrites ends_meta).  Per lattice entry n, with R(n) the exact (64-bit) minimum cost from BOS to n:
 //   ab[n].x = â(n) = log alpha(n) + theta R(n),   ab[n].y = b̂(n) = log beta(n) + theta (R(EOS) - R(n)),
 // so prob(n) = exp(â(n) + b̂(n) - â(EOS)) and path_prob = exp(-â(EOS)).  Every term of the log-sum-exps is
 // â - theta * (an exact non-negative integer excess), so the values stay within [-inf, log #paths].  Each node sums
@@ -241,11 +247,12 @@ struct MargArgs {
 // k_marg_forward and k_marg_backward (two launches); backward = false runs the forward pass alone (sampling without
 // marginals).  m.lw != nullptr selects the forward pass that also writes MargArgs::lw.
 void launch_marginals(const DictView& d, const Batch& b, const MargArgs& m, cudaStream_t st, bool backward = true);
-// launch_backtrack_write plus MargArgs::token_prob of every token (one launch, in its place).
-void launch_backtrack_write_marg(const Batch& b, const MargArgs& m, cudaStream_t st);
+// backtrack_count, the token-offset scan and backtrack_write: n_tok, tok_off (n_sent + 1 entries) and the token
+// records; with m (marginals) also MargArgs::token_prob of every token.
+void launch_backtrack(const Batch& b, const MargArgs* m, const TileScan& ts, cudaStream_t st);
 
 // Lattice output: every node K3 inserted (the entries of ends[1..=len] without BOS and EOS), after K3 and the
-// marginal kernels and before K4a (which overwrites ends_meta).  A sentence's nodes are listed by end position, and
+// marginal kernels and before K4 (which overwrites ends_meta).  A sentence's nodes are listed by end position, and
 // within a row in insertion order.  Each node gets a vbt_token record (start_char = its start_word, total_cost = its
 // min_cost) and a link {prev, flags}: prev = the sentence-relative node index of the predecessor ends_cold names
 // (the u16-truncated min_idx, as the backtrack follows it), -1 for BOS; flags bit 0 (kNodeBest) = on the best path.
@@ -260,12 +267,12 @@ struct LatticeArgs {
 };
 // k_lattice_count: row_base and n_nodes (a warp per sentence).
 void launch_lattice_count(const Batch& b, const LatticeArgs& l, cudaStream_t st);
-// k_lattice_write: the records, links and, with l.node_prob, prob = exp(â + b̂ - â(EOS)) as k_backtrack_write_marg
+// k_lattice_write: the records, links and, with l.node_prob, prob = exp(â + b̂ - â(EOS)) as k_backtrack<true>
 // computes it (a warp per sentence), after node_off has been scanned.
 void launch_lattice_write(const Batch& b, const LatticeArgs& l, const MargArgs& m, cudaStream_t st);
 
 // Segmentation sampling: n paths per sentence drawn with replacement from P(path) = exp(-theta cost) / Z, by
-// forward-filtering backward-sampling over what k_marg_forward left (R, â and MargArgs::lw), after it and before K4a.
+// forward-filtering backward-sampling over what k_marg_forward left (R, â and MargArgs::lw), after it and before K4.
 // A walk starts at EOS; at node c (EOS: left id 0, word cost 0) its predecessors are the entries k = 0..K-1 of the
 // row c starts at, in row order, with x_k = R(k) + conn(right(k), left(c)) + wcost(c), r = min x_k = R(c),
 // t_k = â(k) - theta (x_k - r), m = max t_k and w_k = exp(t_k - m).  The walk takes the first k whose running sum
