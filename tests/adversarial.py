@@ -16,6 +16,11 @@ do, on every route k_viterbi / k_viterbi2 can take:
                       (the bound prunes hard), others holding -32768 (nothing is pruned);
     ``wrap``          Raw / Dual connector: bigram.cost values near +-2^31, so template sums wrap in i32 and the
                       Dual connector's matrix part hits its i16 clamp.
+
+Two more dictionaries have marginals that are exact rationals (tests/marginal_oracle.exact_marginals):
+    ``pow2``          matrix and word costs from POW2, multiples of 64 across the i16 range: at theta = ln 2 / 64
+                      every path weighs a power of two;
+    zero_dictionary() every cost 0: a node's marginal is a ratio of path counts, at any theta.
 """
 import numpy as np
 
@@ -23,6 +28,8 @@ import numpy as np
 ALPHABET = ["a", "b", "é", "あ", "ア", "漢", "1", "\U00020bb7"]
 FAMILIES = ("ties", "flat_columns", "extreme")
 EXTREME = np.array([-32768, -32767, -1, 0, 1, 32766, 32767], dtype=np.int64)
+POW2 = np.array([-32768, -32704, -4096, -64, 0, 64, 128, 4096, 32704], dtype=np.int64)  # all multiples of 64
+POW2_UNIT = 64
 WRAP_COSTS = np.array([2147483647, 2147480000, -2147483648, -2147480000, 1 << 30, -(1 << 30), 0, 1, -1], dtype=np.int64)
 N_IDS = 10  # connection ids 0..9 (0 = BOS/EOS)
 
@@ -64,11 +71,15 @@ class AdversarialDictionary:
 def _word_costs(family, rng, n):
     if family in ("extreme", "wrap"):
         return rng.choice(EXTREME, n)
+    if family == "pow2":
+        return rng.choice(POW2, n)
     return rng.integers(0, 3, n)
 
 
 def _matrix(family, rng):
     """int16 [num_left, num_right]; column l of the issue's M[r][l] notation is row l here."""
+    if family == "pow2":
+        return rng.choice(POW2, (N_IDS, N_IDS)).astype(np.int16)
     if family == "ties":
         return rng.integers(-1, 2, (N_IDS, N_IDS)).astype(np.int16)
     if family == "flat_columns":
@@ -96,9 +107,10 @@ def _bigram_files(rng, n_templates):
 
 
 def make_dictionary(family, seed=0, n_surfaces=70, dual=False):
-    """family in FAMILIES, or "wrap" (Raw connector; `dual` picks the Dual connector's 10 templates)."""
-    assert family in FAMILIES + ("wrap",)
-    rng = np.random.default_rng([seed, FAMILIES.index(family) if family in FAMILIES else 9, int(dual)])
+    """family in FAMILIES, "pow2", or "wrap" (Raw connector; `dual` picks the Dual connector's 10 templates)."""
+    assert family in FAMILIES + ("wrap", "pow2")
+    fam = FAMILIES.index(family) if family in FAMILIES else {"wrap": 9, "pow2": 10}[family]
+    rng = np.random.default_rng([seed, fam, int(dual)])
     surfaces = []
     while len(surfaces) < n_surfaces:
         s = "".join(rng.choice(ALPHABET, int(rng.integers(1, 5))))
@@ -132,6 +144,30 @@ def make_dictionary(family, seed=0, n_surfaces=70, dual=False):
             user.append(f"{s},{l},{r},{c},u{len(user)}")
     user_csv = "\n".join(user) + "\n"
     return AdversarialDictionary(family, lex_csv, matrix, unk_def, user_csv, surfaces, homographs)
+
+
+ZERO_CHAR_DEF = """\
+DEFAULT 0 1 0
+SPACE 0 1 0
+ALPHA 0 0 0
+BEE 1 1 2
+
+0x0020 SPACE
+0x0061 ALPHA
+0x0062 BEE
+"""
+
+
+def zero_dictionary():
+    """Every word and connection cost 0: the surfaces a, aa and aaa (a sentence of n `a` has T(n) paths, the
+    tribonacci numbers, about 1.84^n), unknown words of `b` (grouped, and of 1 and 2 characters) and of every other
+    character; no user lexicon (user_csv is empty).  The marginals are ratios of path counts at any theta."""
+    lex = "a,1,1,0,A\naa,1,1,0,AA\naaa,1,1,0,AAA\n"
+    matrix = np.zeros((2, 2), dtype=np.int16)
+    unk = "DEFAULT,1,1,0,unk\nSPACE,1,1,0,space\nALPHA,1,1,0,alpha\nBEE,1,1,0,bee\n"
+    d = AdversarialDictionary("zero", lex, matrix, unk, "", ["a", "aa", "aaa", "b"], [1, 1, 1, 0])
+    d.char_def = ZERO_CHAR_DEF
+    return d
 
 
 def make_sentences(d, n_sent, seed=1, max_len=300):

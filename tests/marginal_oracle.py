@@ -6,9 +6,12 @@ with exact (Python int) path costs, the definition of vbt_tokenizer_set_marginal
   P(path) = exp(-theta * cost(path)) / Z,  prob(node) = sum of P over the paths through it,
   path_prob = exp(-theta * min cost) / Z.
 
-Also a brute-force enumeration of every BOS -> EOS path and the large-theta limit (exact counts of minimum-cost
-paths).  Test infrastructure."""
+Also a brute-force enumeration of every BOS -> EOS path, the large-theta limit (exact counts of minimum-cost
+paths), the exact marginals of lattices whose costs are multiples of one unit, and the float32 comparison the device
+outputs are held to.  Test infrastructure."""
 import math
+
+import numpy as np
 
 NEG = -math.inf
 
@@ -132,6 +135,94 @@ def tie_fractions(lat):
     total_min = S[(0, 0)]
     n_min = G[(0, 0)]
     return {n: Fraction(F[n] * G[n], n_min) if n in S and R[n] + S[n] == total_min else Fraction(0) for n in lat.nodes}
+
+
+def exact_marginals(lat, unit, bits=None):
+    """(prob: dict node -> float, path_prob) exactly, for a lattice whose every edge cost is a multiple of `unit`, at
+    theta = ln 2 / unit: a path of cost k * unit then weighs 2^-k, and every forward and backward sum is a dyadic
+    m * 2^e with a Python int m (two sums add at the smaller exponent, so no gcd is taken).  Each value is the exact
+    rational f(n) b(n) / Z rounded once to float64 (int / int is correctly rounded, subnormals included).  With every
+    cost 0 the weights are path counts, and the result holds at any theta.
+
+    An exact m holds as many bits as the weights of the paths into a node span: about 2 000 per character when costs
+    range over i16 at unit 64.  `bits` keeps the leading `bits` bits of every sum instead (truncated; a term more than
+    `bits` + 2 bits below the other is dropped), so each value is within (number of sums) * 2^(2 - bits) of the exact
+    rational, relative: far below a float64 step for bits = 256."""
+    def k(c):
+        q, r = divmod(c, unit)
+        assert r == 0, (c, unit)
+        return q
+
+    def add(acc, m, e):
+        if acc is None:
+            return m, e
+        am, ae = acc
+        if bits:
+            gap = (e + m.bit_length()) - (ae + am.bit_length())
+            if gap < -bits - 2:
+                return acc
+            if gap > bits + 2:
+                return m, e
+        m, e = (am + (m << (e - ae)), ae) if e >= ae else ((am << (ae - e)) + m, e)
+        if bits and m.bit_length() > bits:
+            s = m.bit_length() - bits
+            m, e = m >> s, e + s
+        return m, e
+
+    def ratio(num, den, e):  # num / den * 2^e, correctly rounded
+        return (num << e) / den if e >= 0 else num / (den << -e)
+
+    f, R = {(0, 0): (1, 0)}, {(0, 0): 0}
+    for n in lat.nodes[1:]:
+        acc = None
+        for p in lat.preds(n):
+            m, e = f[p]
+            acc = add(acc, m, e - k(lat.w(p, n)))
+        f[n] = acc
+        R[n] = min(R[p] + lat.w(p, n) for p in lat.preds(n))
+    z = None
+    for i in range(len(lat.ends[lat.eos_row])):
+        m, e = f[(lat.eos_row, i)]
+        z = add(z, m, e - k(lat.w((lat.eos_row, i), None)))
+    r_eos = min(R[(lat.eos_row, i)] + lat.w((lat.eos_row, i), None) for i in range(len(lat.ends[lat.eos_row])))
+    b = {}
+    for n in reversed(lat.nodes):
+        acc = None
+        if n[0] == lat.eos_row:
+            acc = (1, -k(lat.w(n, None)))
+        else:
+            for c in lat.succ.get(n[0], []):
+                if b[c] is not None:
+                    m, e = b[c]
+                    acc = add(acc, m, e - k(lat.w(n, c)))
+        b[n] = acc
+    zm, ze = z
+    prob = {n: 0.0 if b[n] is None else ratio(f[n][0] * b[n][0], zm, f[n][1] + b[n][1] - ze) for n in lat.nodes}
+    return prob, ratio(1, zm, -k(r_eos) - ze)
+
+
+F32_ULPS = {"worst": 0}  # the largest float32 ulp distance assert_f32_close has seen in this session
+
+
+def assert_f32_close(got, exact, ulps=2, what=""):
+    """got (float32 array) is within `ulps` float32 steps of every exact value rounded to float32
+    (np.float32(float(value))), measured between the bit patterns.  NaN, inf and negative values (-0.0 included) are
+    refused on either side; subnormals are compared as they are."""
+    got = np.asarray(got)
+    assert got.dtype == np.float32, got.dtype
+    if not (isinstance(exact, np.ndarray) and exact.dtype == np.float64):
+        exact = np.array([float(v) for v in exact], dtype=np.float64)
+    exp = exact.astype(np.float32)
+    assert got.shape == exp.shape, (what, got.shape, exp.shape)
+    if not got.size:
+        return
+    for name, v in (("got", got), ("expected", exp)):
+        bad = ~np.isfinite(v) | np.signbit(v)
+        assert not bad.any(), (what, name, int(np.argmax(bad)), v[np.argmax(bad)])
+    dist = np.abs(got.view(np.int32).astype(np.int64) - exp.view(np.int32).astype(np.int64))
+    i = int(np.argmax(dist))
+    F32_ULPS["worst"] = max(F32_ULPS["worst"], int(dist[i]))
+    assert dist[i] <= ulps, (what, i, f"{float(got[i])!r} vs {float(exp[i])!r}: {int(dist[i])} ulps")
 
 
 def sentence_marginals(bo, sent, theta, bounds=()):

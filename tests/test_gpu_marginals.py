@@ -17,7 +17,6 @@ from vibrato_b200._native import lib
 pytestmark = pytest.mark.gpu
 ROUTES = ("whole", "chunked", "compact", "small", "device", "viterbi0", "unpruned", "multi", "multi_device")
 THETA = 0.01
-worst = {"err": 0.0}  # the largest |GPU - restatement| / (1e-3 p + 1e-6) seen
 
 
 def n_gpus():
@@ -82,13 +81,8 @@ def check_against(bo, sents, got, theta=THETA, bounds=None):
     for name in vb.TOKEN_DTYPE.names:
         np.testing.assert_array_equal(toks[name], e_toks[name], err_msg=name)
     e_tp, e_pp = mo.batch_marginals(bo, [s.encode() for s in sents], theta, bounds)
-    for got_v, exp_v in ((tp, e_tp), (pp, e_pp)):
-        exp_v = np.asarray(exp_v, dtype=np.float64)
-        assert got_v.shape == exp_v.shape and np.all(np.isfinite(got_v))
-        err = np.abs(got_v.astype(np.float64) - exp_v) / (1e-3 * exp_v + 1e-6)
-        if err.size:
-            worst["err"] = max(worst["err"], float(err.max()))
-            assert err.max() <= 1.0, (np.argmax(err), got_v[np.argmax(err)], exp_v[np.argmax(err)])
+    mo.assert_f32_close(tp, e_tp, what="token_probs")
+    mo.assert_f32_close(pp, e_pp, what="path_probs")
 
 
 def skip_multi(route):
@@ -285,8 +279,9 @@ def test_launch_count_stages_and_worker(golden):
 
 
 def test_report_worst_error():
-    """Prints the largest error relative to the tolerance seen by the tests above (run in the same session)."""
-    print(f"marginals: max |GPU - restatement| / (1e-3 p + 1e-6) = {worst['err']:.4f}")
+    """Prints the largest float32 ulp distance from the reference that the tests of this session have seen (those
+    above, and those of every test file that ran before it)."""
+    print(f"marginals: worst distance from the reference = {mo.F32_ULPS['worst']} float32 ulps")
 
 
 def parse_pp(text, sents):
@@ -316,7 +311,8 @@ def test_pP_format(golden, route):
     bo = BoundedOracle(od, r["char.def"], r["unk.def"], True)
     exp, _ = mo.batch_marginals(bo, [s.encode() for s in sents], THETA)
     exp = np.asarray(exp)
-    assert got.shape == exp.shape and np.all(np.abs(got - exp) <= 1e-3 * exp + 1e-6 + 5e-7)
+    # the printed micro-units are the rounding of a value within two float32 steps (2^-22 relative) of the reference
+    assert got.shape == exp.shape and np.all(np.abs(np.rint(got * 1e6) - exp * 1e6) <= 0.5 + 2.4e-7 * exp * 1e6)
 
 
 def test_pP_refusals(golden):

@@ -71,13 +71,17 @@ def run(tok, route, sents, bounds=None):
 KEY = ("start_char", "end_char", "start_byte", "end_byte", "word_idx")
 
 
-def check_parity(bo, sents, got, n, theta, seed, bounds=None):
+def check_parity(bo, sents, got, n, theta, seed, bounds=None, expected=None):
     """Every sample equals the restatement's byte for byte; after an ambiguous draw t only its last t records (the
-    draws before it) are compared, without their prefix costs."""
+    draws before it) are compared, without their prefix costs.  `expected`: the restatement's samples by sentence
+    index, when the caller has them already (so.sentence_samples of the same arguments)."""
     off, recs = got
     assert len(off) == len(sents) * n + 1 and int(off[-1]) == len(recs)
     for i, s in enumerate(sents):
-        exp = so.sentence_samples(bo, s.encode(), n, theta, seed, i, bounds[i] if bounds else ())
+        if expected is not None:
+            exp = expected[i]
+        else:
+            exp = so.sentence_samples(bo, s.encode(), n, theta, seed, i, bounds[i] if bounds else ())
         for j, (rec, _, amb) in enumerate(exp):
             g = recs[int(off[i * n + j]):int(off[i * n + j + 1])]
             if amb is None:

@@ -250,9 +250,8 @@ def test_marginals_and_lattice(dic):
         n_off, nodes, links, probs = lo.batch_lattice(bo, enc, b, THETA)
         np.testing.assert_array_equal(got[3], n_off)
         assert got[4].tobytes() == nodes.tobytes() and got[5].tobytes() == links.tobytes()
-        for g, e in ((got[2], np.asarray(e_tp, dtype=np.float64)), (got[6], probs)):
-            err = np.abs(g.astype(np.float64) - e) / (1e-3 * e + 1e-6)
-            assert g.shape == e.shape and err.max() <= 1.0
+        mo.assert_f32_close(got[2], e_tp, what="token_probs")
+        mo.assert_f32_close(got[6], probs, what="node_probs")
     far = sf.far_sentences(long_word)
     got = check_routes_identical(dev, far)
     e_off, e_toks, _ = od.tokenize_batch(*adv.pack(far))

@@ -1,7 +1,9 @@
 """Marginal probabilities on the CPU: the forward-backward restatement (tests/marginal_oracle.py) against brute-force
-enumeration of every path on the golden fixture, and its properties over the adversarial dictionaries."""
+enumeration of every path on the golden fixture, its properties over the adversarial dictionaries, and its float32
+rounding against the exact marginals of the zero-cost and power-of-two dictionaries."""
 import math
 
+import numpy as np
 import pytest
 
 import adversarial as adv
@@ -96,6 +98,110 @@ def test_properties(family, ignore_space):
             # minimum-cost path of the exact costs, and only prob <= 1 holds
             assert family not in adv.FAMILIES or pp <= prob[n] * (1 + 1e-9) + 1e-15
             assert prob[n] <= 1 + 1e-9
+
+
+def exact_oracle(d, ignore_space=False):
+    od = vo.OracleDictionary(d.lex_csv, d.matrix, d.char_def, d.unk_def)
+    if d.user_csv:
+        od.set_user_csv(d.user_csv)
+    return BoundedOracle(od, d.char_def, d.unk_def, ignore_space)
+
+
+def tribonacci(n):
+    a, b, c = 0, 0, 1  # T(0) = 1: the empty path
+    for _ in range(n):
+        a, b, c = b, c, a + b + c
+    return c
+
+
+def check_f64_against_exact(lat, theta, exact):
+    prob, pp, _ = mo.marginals(lat, theta)
+    e_prob, e_pp = exact
+    got = np.array([prob[n] for n in lat.nodes] + [pp], dtype=np.float32)
+    mo.assert_f32_close(got, [e_prob[n] for n in lat.nodes] + [e_pp], ulps=1)
+
+
+@pytest.mark.parametrize("n", [1, 2, 3, 31, 33, 160, 1000, 1200, 20000])
+def test_exact_path_counts(n):
+    """On the zero-cost dictionary a sentence of n `a` has T(n) (tribonacci) paths, path_prob = 1 / T(n), and
+    marginals() (float64) rounds to the exact float32 at any theta: through float32's subnormals (n = 160) and past
+    10^308 paths (n = 1200: 1.7e317; n = 20 000: about 10^5292), where only the log-domain sums stay finite."""
+    bo = exact_oracle(adv.zero_dictionary())
+    lat = mo.Lattice(bo, b"a" * n)
+    exact = mo.exact_marginals(lat, 1)
+    assert exact[1] == 1 / tribonacci(n)
+    if n >= 1200:
+        assert tribonacci(n) > 10 ** 308
+    for theta in (1e-6, 0.01, 50.0):
+        check_f64_against_exact(lat, theta, exact)
+    if n == 160:
+        assert 0 < np.float32(exact[1]) < np.finfo(np.float32).tiny  # a float32 subnormal
+
+
+@pytest.mark.parametrize("ignore_space", [False, True])
+def test_exact_zero_mixed(ignore_space):
+    """Zero-cost sentences with unknown words (`b` groups, other characters) and space runs: marginals() within one
+    float32 step of the exact value, and the large-theta tie fractions equal to it (every path is a minimum)."""
+    d = adv.zero_dictionary()
+    bo = exact_oracle(d, ignore_space)
+    sents = adv.make_sentences(d, 80, seed=4, max_len=300) + ["ab" * 50, "b" * 40, "aab  a", "  "]
+    for s in sents:
+        if not s.strip(" ") and ignore_space or not s:
+            continue
+        lat = mo.Lattice(bo, s.encode())
+        exact = mo.exact_marginals(lat, 1)
+        check_f64_against_exact(lat, 0.01, exact)
+        frac = mo.tie_fractions(lat)
+        assert all(float(frac[n]) == exact[0][n] for n in lat.nodes), s
+
+
+@pytest.mark.parametrize("ignore_space", [False, True])
+def test_exact_pow2(ignore_space):
+    """Costs that are multiples of 64 across i16 (homographs, user entries, negative costs) at theta = ln 2 / 64:
+    marginals() within one float32 step of the exact value, on sentences of 0-200 characters and one of 1 000."""
+    d = adv.make_dictionary("pow2")
+    bo = exact_oracle(d, ignore_space)
+    theta = math.log(2) / adv.POW2_UNIT
+    sents = adv.make_sentences(d, 120, seed=3, max_len=200)
+    sents.append(("".join(sents) * 8)[:1000])
+    for s in sents:
+        if not s.strip(" ") and ignore_space or not s:
+            continue
+        lat = mo.Lattice(bo, s.encode())
+        check_f64_against_exact(lat, theta, mo.exact_marginals(lat, adv.POW2_UNIT, bits=256))
+
+
+def test_exact_truncated_equals_exact():
+    """The 256-bit sums give the same float64 values as the exact ones where the exact ones are affordable."""
+    d = adv.make_dictionary("pow2")
+    bo = exact_oracle(d)
+    sents = [s for s in adv.make_sentences(d, 40, seed=8, max_len=30) if s]
+    for s in sents:
+        lat = mo.Lattice(bo, s.encode())
+        assert mo.exact_marginals(lat, adv.POW2_UNIT) == mo.exact_marginals(lat, adv.POW2_UNIT, bits=256), s
+
+
+def test_exact_matches_brute_force():
+    d = adv.make_dictionary("pow2")
+    bo = exact_oracle(d)
+    theta = math.log(2) / adv.POW2_UNIT
+    for s in [s for s in adv.make_sentences(d, 40, seed=2, max_len=4) if s]:
+        lat = mo.Lattice(bo, s.encode())
+        prob, pp = mo.exact_marginals(lat, adv.POW2_UNIT)
+        bprob, bpp = mo.brute_force(lat, theta)
+        assert close(pp, bpp) and all(close(prob[n], bprob[n]) for n in lat.nodes), s
+
+
+def test_f32_close_refusals():
+    exact = [1.0, 0.5, 1e-40]
+    mo.assert_f32_close(np.array(exact, dtype=np.float32), exact)
+    one_up = np.nextafter(np.float32(0.5), np.float32(1))
+    mo.assert_f32_close(np.array([1.0, one_up, 1e-40], dtype=np.float32), exact, ulps=1)
+    for bad in ([np.nan, 0.5, 1e-40], [np.inf, 0.5, 1e-40], [-0.0, 0.5, 1e-40], [1.0, 0.5, 1.5e-40], [1.0, 0.5, 0.0]):
+        with pytest.raises(AssertionError):
+            mo.assert_f32_close(np.array(bad, dtype=np.float32), exact)
+    with pytest.raises(AssertionError):
+        mo.assert_f32_close(np.array([1.0], dtype=np.float64), [1.0])
 
 
 @pytest.mark.parametrize("family", ["ties", "flat_columns"])
