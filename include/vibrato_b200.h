@@ -296,7 +296,10 @@ int32_t vbt_tokenizer_set_counting(vbt_tokenizer *t, int32_t on);
  * the usual route.  vbt_last_launch_count then gives 1 and vbt_last_stage_ms books the whole kernel under
  * "viterbi".  A batch whose candidates or text outgrow the route's fixed scratch runs again on the usual route
  * (describe() names the route that ran).  vbt_tokenize_batch_device and the shards of a multi-device tokenizer
- * keep the usual route. */
+ * keep the usual route.
+ * Output options (results change as documented with them): "compact_tokens", "lattice" (see vbt_result_lattice),
+ * "sample_text" = 0|1 (default 0; 1: the output text renders the samples, see vbt_tokenizer_set_sampling) and
+ * "sample_base" = i in 0..2^32 (default 0: the sentence index at which the calls' draws start, see the same). */
 int32_t vbt_tokenizer_set_option(vbt_tokenizer *t, const char *name, int64_t value);
 /* MeCab-style output formats, rendered on the device in place of the option "output_mode": batches tokenised
  * afterwards carry the text of the format in vbt_result_text, on every host route (whole batch, chunked pipeline,
@@ -378,9 +381,11 @@ int32_t vbt_last_device_lattice(const vbt_tokenizer *t, uint64_t *d_node_offsets
  * walk takes the first k whose running sum w_0 + ... + w_k (float64, in row order) exceeds u * S, S the whole sum,
  * and the last k with w_k > 0 if rounding leaves none.  u = ((x0 >> 5) * 2^26 + (x1 >> 6)) * 2^-53 from the first
  * two words of Philox4x32-10 (standard constants) at counter (t, j, i, 0) and key (seed & 0xFFFFFFFF, seed >> 32):
- * t the draw step (0 at EOS), j the sample, i the sentence's index in the call.  Routes (chunking, devices, the
- * sentence order) do not change i, so the same call with the same seed gives the same bytes everywhere; callers who
- * split a corpus over several calls vary the seed per call.
+ * t the draw step (0 at EOS), j the sample, i = sample_base + the sentence's index in the call (the option
+ * "sample_base", default 0).  Routes (chunking, devices, the sentence order) do not change i, so the same call with
+ * the same seed gives the same bytes everywhere; callers who split a corpus over several calls set "sample_base" to
+ * each call's first index and draw what one call over the whole corpus would.  A call with sample_base + n_sent > 2^32
+ * fails.
  *   Records: each sampled token is a 24-byte vbt_token record, also under "compact_tokens"; start_char, bytes, word_idx
  *   as for tokens, total_cost the sampled path's prefix cost through the token in the tokenizer's wrapping i32
  *   arithmetic.  A sample whose nodes are the best path's has records byte-identical to the sentence's tokens.
@@ -389,7 +394,20 @@ int32_t vbt_last_device_lattice(const vbt_tokenizer *t, uint64_t *d_node_offsets
  * Marginals and sampling share one forward pass: setting either while the other is on with a different theta is
  * VBT_ERR_INVALID_ARGUMENT.  Tokens, marginals, the lattice and the output text do not change.  While on, batches
  * take three more kernel launches and a scan (the forward pass alone when marginals are off; booked under
- * "viterbi") with one host wait for the sample total, and "small_batch" steps aside. */
+ * "viterbi") with one host wait for the sample total, and "small_batch" steps aside.
+ * Sample text, the option "sample_text" = 1 (default 0), needs sampling on: with an output mode or format set, the
+ * output text renders each sentence's n samples, in order j = 0 .. n-1, in place of its best path.  Each sample is
+ * rendered exactly as a sentence whose tokens are its records (BOS format, a node / unk rendering per record, EOS
+ * format; -O mecab / wakati / detail likewise), so a sample whose records equal the sentence's tokens renders to the
+ * bytes of the sentence's text without sample text, and an empty sample renders as an empty sentence does ("\n" in
+ * wakati, "EOS\n" in mecab).  text_offsets keep n_sent + 1 entries: the text of sentence i is its n renderings one
+ * after another.  %pc and detail's total_cost print the record's total_cost (the sampled path's prefix cost); the
+ * "prev" directives %M %pS %pn %pC %pL take the previous record of the same sample (BOS for its first); %S and %L
+ * the sentence.  %pP and %pb have no value: a format that prints them and sample text refuse each other in either
+ * order, naming the directive and its byte position.  Sample text and "lattice" = 2 exclude each other, and
+ * switching sampling off while sample text is on fails (switch it off first).  Every host route renders it (whole
+ * batch, chunked pipeline, multi-device, bounded calls); vbt_tokenize_batch_device stays token-only.  Tokens,
+ * samples, marginals and the lattice do not change. */
 int32_t vbt_tokenizer_set_sampling(vbt_tokenizer *t, uint32_t n, double theta, uint64_t seed);
 /* sample_offsets[n_sent * n + 1] into samples: sample j of sentence i is samples[sample_offsets[i * n + j] ..
  * sample_offsets[i * n + j + 1]); owned by the result.  VBT_ERR_INVALID_ARGUMENT for a result made without sampling. */

@@ -271,10 +271,23 @@ impl Tokenizer {
     }
     /// Segmentation sampling (see `vbt_tokenizer_set_sampling`): `n` (1..1024, 0 = off) paths per sentence drawn from
     /// P(path) at temperature `theta`, keyed by `seed`; batches tokenised afterwards carry `BatchResult::samples`.
-    pub fn sampling(&self, n: u32, theta: f64, seed: u64) -> Result<()> {
+    /// `text`: the output text renders each sentence's `n` samples in place of its best path (option "sample_text").
+    pub fn sampling(&self, n: u32, theta: f64, seed: u64, text: bool) -> Result<()> {
+        let opt = b"sample_text\0".as_ptr() as *const c_char;
+        if !text {
+            check(unsafe { vbt_tokenizer_set_option(self.handle(), opt, 0) })?;
+        }
         check(unsafe { vbt_tokenizer_set_sampling(self.handle(), n, theta, seed) })?;
+        if text {
+            check(unsafe { vbt_tokenizer_set_option(self.handle(), opt, 1) })?;
+        }
         self.samples.set(n);
         Ok(())
+    }
+    /// The draws of the next calls' sentence `s` use the sentence index `i + s` (option "sample_base"; `i + n_sent`
+    /// at most 2^32), so that a corpus tokenised over several calls draws what one call would.
+    pub fn sample_base(&self, i: u64) -> Result<()> {
+        check(unsafe { vbt_tokenizer_set_option(self.handle(), b"sample_base\0".as_ptr() as *const c_char, i as i64) })
     }
     /// The loop of the `evaluate` tool (evaluate/src/main.rs:61-138): (num_ref, num_sys, num_cor).
     pub fn evaluate(&self, corpus: &str, feature_indices: &[usize]) -> Result<(u64, u64, u64)> {

@@ -368,7 +368,9 @@ class BatchResult:
         po, pt, nb = C.c_void_p(), C.c_void_p(), C.c_uint64()
         check(lib().vbt_result_text(self._h, C.byref(po), C.byref(pt), C.byref(nb)))
         offs = np.ctypeslib.as_array(C.cast(po, C.POINTER(C.c_uint64)), shape=(self.n_sent + 1,)).copy()
-        text = C.string_at(pt, nb.value) if nb.value else b""
+        # string_at takes a C int size: texts of 2 GiB and more (n samples of a large batch) are read as an array
+        n = nb.value
+        text = b"" if not n else C.string_at(pt, n) if n < 2 ** 31 else (C.c_char * n).from_address(pt.value).raw
         return offs, text
 
     def sentence_tokens(self, i):
@@ -420,6 +422,7 @@ class Tokenizer:
         self._theta = 0.0  # marginals(), replayed before the format
         self._lattice = 0  # lattice(), replayed before the format
         self._sampling = (0, 0.0, 0)  # sampling() as (n, theta, seed), replayed after the marginals
+        self._sample_text = False  # sampling(text=True), replayed after sampling
         self._stream = 0
         self._counting = False
         self._free = lib().vbt_tokenizer_free
@@ -485,6 +488,8 @@ class Tokenizer:
                 check(lib().vbt_tokenizer_set_option(h, b"lattice", self._lattice))
             if self._sampling[0]:
                 check(lib().vbt_tokenizer_set_sampling(h, *self._sampling))
+            if self._sample_text:
+                check(lib().vbt_tokenizer_set_option(h, b"sample_text", 1))
             if self._format is not None:
                 self._set_format(h, self._format)
             if self._counting:
@@ -573,21 +578,36 @@ class Tokenizer:
         check(lib().vbt_last_device_samples(self.handle(), *[C.byref(x) for x in v]))
         return tuple(x.value for x in v)
 
-    def sampling(self, n, theta=1.0, seed=0):
+    def sampling(self, n, theta=1.0, seed=0, text=False):
         """Segmentation sampling ("subword regularisation"): every result then carries n segmentations per sentence
         drawn with replacement from P(path) = exp(-theta * cost(path)) / Z, the distribution of marginals()
         (BatchResult.samples / sample_offsets, sentence_samples()).  theta > 0 and finite; with marginals on it must be
-        theirs.  seed (u64) keys the draws, which depend only on (seed, sentence index in the call, sample, step):
-        vary it per call when a corpus is split over calls.  n = 0 (or None) switches sampling off.  The tokens do not
-        change; the "small_batch" route steps aside.  Definition: include/vibrato_b200.h."""
+        theirs.  seed (u64) keys the draws, which depend only on (seed, sentence index, sample, step); the sentence
+        index starts at sample_base() in every call.  n = 0 (or None) switches sampling off.  The tokens do not
+        change; the "small_batch" route steps aside.  text=True ("sample_text") also renders each sentence's n samples,
+        one after another, in place of its best path in the output text (BatchResult.text()); set it before a format.
+        Definition: include/vibrato_b200.h."""
         n = 0 if n is None else int(n)
         theta, seed = float(theta), int(seed)
         if not 0 <= seed < 2 ** 64:
             raise VibratoError(1, "sampling: seed must be an unsigned 64-bit integer")
         if not 0 <= n < 2 ** 32:
             raise VibratoError(1, "sampling: n must be between 0 (off) and 1024")
+        if not text and self._sample_text:  # before sampling may switch off, which sample text refuses
+            check(lib().vbt_tokenizer_set_option(self.handle(), b"sample_text", 0))
+            self._sample_text = False
         check(lib().vbt_tokenizer_set_sampling(self.handle(), n, theta, seed))
         self._sampling = (n, theta, seed) if n else (0, 0.0, 0)
+        if text:
+            check(lib().vbt_tokenizer_set_option(self.handle(), b"sample_text", 1))
+            self._sample_text = True
+        return self
+
+    def sample_base(self, i):
+        """The draws of sentence s of the calls that follow use the sentence index i + s (the option "sample_base",
+        default 0), so that a corpus tokenised in pieces draws what one call over all of it would: set it to each
+        piece's first index.  A call with i + n_sent > 2^32 is refused."""
+        self.set_option("sample_base", int(i))
         return self
 
     def lattice(self, on=True, text=False):
@@ -645,6 +665,9 @@ class Tokenizer:
         check(lib().vbt_tokenizer_set_option(self.handle(), name.encode(), int(value)))
         if name == "lattice":  # replayed with lattice()'s state, after the marginals
             self._lattice = int(value)
+            return
+        if name == "sample_text":  # replayed after sampling, which it needs
+            self._sample_text = bool(value)
             return
         if name != "connid_counting":  # accumulated counts cannot be carried into a rebuilt engine
             self._options[name] = int(value)

@@ -3,6 +3,8 @@
 // Lines are shipped in batches; output order and content equal the per-line loop of main.rs:78-128.
 #include <unistd.h>
 
+#include <cerrno>
+#include <cstdint>
 #include <cstdlib>
 #include <cstring>
 
@@ -24,7 +26,13 @@ static void usage() {
                  "         [-m|--marginal -t|--theta F] (marginal probabilities at temperature F > 0: -F may print\n"
                  "                                      each token's with %%pP; -O output is unchanged)\n"
                  "         [-a|--all-morphs]           (every lattice node in place of the tokens, like MeCab -a: -O and\n"
-                 "                                      -F render nodes, -F may print %%pb; needs --format-on device)\n");
+                 "                                      -F render nodes, -F may print %%pb; needs --format-on device)\n"
+                 "         [--sample N -t|--theta F [--seed S]]\n"
+                 "                                     (N segmentations per line, 1..1024, drawn from the lattice's path\n"
+                 "                                      distribution at temperature F, in place of the best path: -O and -F\n"
+                 "                                      print N renderings per line; S (u64, default 0) keys the draws,\n"
+                 "                                      which do not depend on --batch-lines or --devices; not with -a,\n"
+                 "                                      %%pP or %%pb; needs --format-on device)\n");
 }
 
 int main(int argc, char** argv) {
@@ -37,6 +45,18 @@ int main(int argc, char** argv) {
     std::string marker;
     bool marginal = false, has_theta = false, all_morphs = false;
     double theta = 0;
+    uint32_t n_sample = 0;  // --sample
+    uint64_t seed = 0;
+    bool has_seed = false;
+    // a whole decimal number in [lo, hi], else a usage error
+    auto parse_u64 = [](const std::string& v, uint64_t lo, uint64_t hi, uint64_t& out) {
+        if (v.empty() || v.size() > 20 || v.find_first_not_of("0123456789") != std::string::npos) return false;
+        errno = 0;
+        const unsigned long long x = std::strtoull(v.c_str(), nullptr, 10);
+        if (errno == ERANGE || x < lo || x > hi) return false;
+        out = x;
+        return true;
+    };
     for (int i = 1; i < argc; ++i) {
         std::string a = argv[i];
         auto next = [&]() -> std::string {
@@ -61,6 +81,15 @@ int main(int argc, char** argv) {
         else if (a == "--boundary-marker") marker = next();
         else if (a == "-m" || a == "--marginal") marginal = true;
         else if (a == "-a" || a == "--all-morphs") all_morphs = true;
+        else if (a == "--sample" || a == "--seed") {
+            uint64_t v = 0;
+            if (!parse_u64(next(), a == "--sample" ? 1 : 0, a == "--sample" ? 1024 : UINT64_MAX, v)) {
+                usage();
+                return 2;
+            }
+            if (a == "--sample") n_sample = uint32_t(v);
+            else seed = v, has_seed = true;
+        }
         else if (a == "-t" || a == "--theta") {
             const std::string v = next();
             char* end = nullptr;
@@ -78,9 +107,11 @@ int main(int argc, char** argv) {
     }
     // the formats are rendered by the device only; --unk/bos/eos-format complete -F
     const bool bounded = !marker.empty();
-    // -m needs --theta, and --theta belongs to -m
+    // -m and --sample need --theta, and --theta belongs to them; --seed belongs to --sample
+    const bool sample = n_sample != 0;
     if (batch_lines_arg == 0 || (has_node && format_on == "host") || (!has_node && (has_unk || has_bos || has_eos)) ||
-        marginal != has_theta || (all_morphs && format_on == "host") ||
+        (marginal || sample) != has_theta || (all_morphs && format_on == "host") || (has_seed && !sample) ||
+        (sample && (all_morphs || format_on == "host")) ||
         (bounded && (marker.size() != 1 || marker[0] == '\n' || (marker[0] & 0x80)))) {
         usage();
         return 2;
@@ -102,6 +133,7 @@ int main(int argc, char** argv) {
             Tokenizer(std::move(dict)).ignore_space(ignore_space).max_grouping_len(max_grouping_len).devices(devices);
         if (marginal) tokenizer.marginals(theta);  // before -F, which may print %pP
         if (all_morphs) tokenizer.lattice(true, true);  // before -F, which may print %pb
+        if (sample) tokenizer.sampling(n_sample, theta, seed, true);  // before -F, which may not print %pP / %pb
         if (has_node) {
             const std::string_view node = node_format, unk = unk_format, bos = bos_format, eos = eos_format;
             tokenizer.output_format(&node, has_unk ? &unk : nullptr, has_bos ? &bos : nullptr, has_eos ? &eos : nullptr);
@@ -111,13 +143,17 @@ int main(int argc, char** argv) {
         std::fprintf(stderr, "Ready to tokenize\n");
         const bool tty_out = isatty(STDOUT_FILENO), tty_in = isatty(STDIN_FILENO);
         const size_t batch_lines = tty_in ? 1 : batch_lines_arg;
-        // a line at a time: one kernel launch per line (k_small_batch has no lattice: -a takes the usual route)
-        if (batch_lines == 1 && !all_morphs) tokenizer.small_batch(1);
+        // a line at a time: one kernel launch per line (k_small_batch has no lattice and no samples: -a and --sample
+        // take the usual route)
+        if (batch_lines == 1 && !all_morphs && !sample) tokenizer.small_batch(1);
+        uint64_t lines_done = 0;  // input lines before the batch: the sentence index of its first line's draws
         std::string out;
         cli::Packed pk;
         std::string line;
         auto flush_batch = [&]() {
             if (pk.size() == 0) return;
+            if (sample) tokenizer.sample_base(lines_done);
+            lines_done += pk.size();
             BatchResult r = bounded ? tokenizer.tokenize_batch(pk.utf8.data(), pk.off.data(), pk.size(), pk.bnd_off.data(),
                                                                pk.bnd.data())
                                     : tokenizer.tokenize_batch(pk.utf8.data(), pk.off.data(), pk.size());

@@ -299,12 +299,18 @@ class Tokenizer {
     }
     // Segmentation sampling (see vbt_tokenizer_set_sampling): n (1..1024, 0 = off) paths per sentence drawn from
     // P(path) at temperature theta, keyed by seed: BatchResult::samples().  theta must equal the marginals' when both
-    // are on.
-    void sampling(uint32_t n, double theta, uint64_t seed = 0) const {
+    // are on.  text = true also renders the samples in place of the best path in the output text (the option
+    // "sample_text"): n renderings per sentence, one after another.  Set text before a format is set.
+    void sampling(uint32_t n, double theta, uint64_t seed = 0, bool text = false) const {
+        if (!text) check(vbt_tokenizer_set_option(handle(), "sample_text", 0));  // before sampling may switch off
         check(vbt_tokenizer_set_sampling(handle(), n, theta, seed));
+        if (text) check(vbt_tokenizer_set_option(handle(), "sample_text", 1));
         samples_ = n;
     }
     uint32_t samples_per_sentence() const { return samples_; }
+    // The draws of the next calls' sentence s use the sentence index i + s (the option "sample_base"), so that a
+    // corpus tokenised over several calls draws what one call over all of it would.  i + n_sent <= 2^32.
+    void sample_base(uint64_t i) const { check(vbt_tokenizer_set_option(handle(), "sample_base", int64_t(i))); }
     // Device addresses of the last tokenize_batch_device call's samples.
     struct DeviceSamples {
         uint64_t sample_offsets = 0, samples = 0, n_sample_tokens = 0;

@@ -32,6 +32,10 @@ struct vbt_dict {
 };
 struct vbt_tokenizer {
     std::shared_ptr<vbt::Engine> e;
+    // The strings of the output format in force (node, unk, bos, eos; empty when none is), and the option
+    // "sample_text": switching sample text on compiles the format again, so that a refusal names the directive.
+    std::vector<std::pair<bool, std::string>> fmt = {};
+    bool sample_text = false;
 };
 struct vbt_result {
     std::shared_ptr<vbt::Engine> owner;  // keeps the engine (and its pinned pool) alive past vbt_tokenizer_free
@@ -549,7 +553,15 @@ int32_t vbt_tokenizer_set_option(vbt_tokenizer* t, const char* name, int64_t val
     return guarded([&] {
         need(t, "t");
         need(name, "name");
-        t->e->set_option(name, value);
+        const std::string opt = name;
+        if (opt == "sample_text" && value == 1 && !t->fmt.empty()) {
+            vbt::FormatText s[4];
+            for (int i = 0; i < 4; ++i) s[i] = {t->fmt[i].first ? t->fmt[i].second.data() : nullptr, t->fmt[i].second.size()};
+            vbt::compile_format(s[0], s[1], s[2], s[3], t->e->marginals() > 0, false, true);  // throws at %pP / %pb
+        }
+        t->e->set_option(opt, value);
+        if (opt == "sample_text") t->sample_text = value != 0;
+        if (opt == "output_mode") t->fmt.clear();  // a fixed mode replaces the format
     });
 }
 
@@ -559,14 +571,19 @@ int32_t vbt_tokenizer_set_output_format(vbt_tokenizer* t, const char* node, size
         need(t, "t");
         if (!node) {
             t->e->set_format(nullptr);
+            t->fmt.clear();
             return;
         }
         // an empty string may come with any pointer: only NULL means "not given"
         // %pP has a value only while the tokenizer computes marginals, %pb only in lattice text (where the "prev"
-        // directives have none)
+        // directives have none); sample text has neither
         const vbt::FormatProgram p = vbt::compile_format({node, node_len}, {unk, unk_len}, {bos, bos_len}, {eos, eos_len},
-                                                         t->e->marginals() > 0, t->e->lattice() == 2);
+                                                         t->e->marginals() > 0, t->e->lattice() == 2, t->sample_text);
+        t->fmt.clear();  // set_format replaces (or, failing, clears) the format in force
         t->e->set_format(&p);
+        const char* ptr[4] = {node, unk, bos, eos};
+        const size_t len[4] = {node_len, unk_len, bos_len, eos_len};
+        for (int i = 0; i < 4; ++i) t->fmt.emplace_back(ptr[i] != nullptr, ptr[i] ? std::string(ptr[i], len[i]) : std::string());
     });
 }
 

@@ -171,6 +171,7 @@ struct DevBounds {
 struct OutSlot {  // where one (chunk of a) batch leaves its results; two of them alternate in chunked runs
     DevBuf buf[kNumArrays];  // the output arrays; path_prob is written by the forward pass of sampling too
     DevBuf ctrl, sent_len;   // sent_len: output stage (k_format_*)
+    DevBuf walk_off;         // sample text: where each walk's text starts (n_sent * n + 1)
     Outputs made;            // the arrays the (chunk of a) batch in this slot produced
     Control* h_ctrl = nullptr;
     cudaEvent_t ev[kNumStages + 1];
@@ -325,6 +326,7 @@ class EngineImpl final : public Engine {
             for (DevBuf& b : o.buf) b.release();
             o.ctrl.release();
             o.sent_len.release();
+            o.walk_off.release();
             pinned_free(o.h_ctrl);
             for (auto& ev : o.ev) cudaEventDestroy(ev);
             cudaEventDestroy(o.done);
@@ -412,8 +414,24 @@ class EngineImpl final : public Engine {
                             "change the format before setting lattice = 2");
             if (value != 2 && output_mode_ == kOutFormat && (fmt_uses_ & kUsesBest))
                 throw Error(kInvalidArgument, "the output format prints %pb, which only lattice text has: change the format before setting lattice below 2");
+            if (value == 2 && sample_text_)
+                throw Error(kInvalidArgument, "lattice text and sample text both replace the output text: set \"sample_text\" to 0 before setting lattice = 2");
             cudaStreamSynchronize(stream_);
             lattice_ = int(value);
+        } else if (name == "sample_text") {
+            // the output text renders each sentence's samples in place of its best path
+            if (value < 0 || value > 1) throw Error(kInvalidArgument, "sample_text must be 0 (off) or 1 (the text renders the samples)");
+            if (value && !samp_n_) throw Error(kInvalidArgument, "sample_text needs sampling: switch it on with set_sampling first");
+            if (value && lattice_ == 2)
+                throw Error(kInvalidArgument, "lattice text and sample text both replace the output text: set \"lattice\" below 2 before setting sample_text = 1");
+            if (value && output_mode_ == kOutFormat && (fmt_uses_ & (kUsesProb | kUsesBest)))  // capi names the directive
+                throw Error(kInvalidArgument, "the output format prints %pP or %pb, which sample text has no value for: change the format before setting sample_text = 1");
+            cudaStreamSynchronize(stream_);
+            sample_text_ = value != 0;
+        } else if (name == "sample_base") {
+            // the sentence index of the draws starts here: a caller that splits a corpus over calls keeps its draws
+            if (value < 0 || value > kMaxSampleBase) throw Error(kInvalidArgument, "sample_base must be between 0 and 2^32");
+            sample_base_ = uint64_t(value);
         } else if (name == "small_batch") {
             // host batches of at most `value` sentences and kEagerBytes bytes take k_small_batch (0 = never)
             if (value < 0 || value > kSmallBatchMax) throw Error(kInvalidArgument, "small_batch must be between 0 and 65536");
@@ -433,6 +451,8 @@ class EngineImpl final : public Engine {
             throw Error(kInvalidArgument, "%pb needs lattice text: set the option \"lattice\" to 2 before setting the format");
         if ((p->uses & kUsesPrev) && lattice_ == 2)  // compile_format names the directive; this guards other callers
             throw Error(kInvalidArgument, "lattice text has no previous token: the format may not print %M %pS %pn %pC %pL");
+        if ((p->uses & (kUsesProb | kUsesBest)) && sample_text_)  // the same
+            throw Error(kInvalidArgument, "sample text has no marginals or best-path flags: the format may not print %pP or %pb");
         try {
             fmt_prog_.ensure(sizeof(FormatProgram));
             CK(cudaMemcpy(fmt_prog_.p, p, sizeof(FormatProgram), cudaMemcpyHostToDevice));
@@ -446,6 +466,7 @@ class EngineImpl final : public Engine {
         text_per_sent_ = p->per_sentence;
         text_per_byte_[kOutFormat] = kFormatTextPerByte;  // learned anew for every format
         text_per_byte_lat_[kOutFormat] = kFormatTextPerByte * kLatticeTextFactor;
+        text_per_byte_samp_[kOutFormat] = kFormatTextPerByte;
     }
     void set_marginals(double theta) override {
         if (!(theta >= 0) || !std::isfinite(theta))
@@ -465,6 +486,8 @@ class EngineImpl final : public Engine {
         if (n && theta_ > 0 && theta != theta_)
             throw Error(kInvalidArgument, "marginals and sampling share one forward pass: the sampling theta " + num(theta) +
                                               " differs from the marginals' theta " + num(theta_));
+        if (!n && sample_text_)
+            throw Error(kInvalidArgument, "the output text renders the samples: set \"sample_text\" to 0 before switching sampling off");
         cudaStreamSynchronize(stream_);
         samp_n_ = n;
         samp_theta_ = n ? theta : 0.0;
@@ -623,16 +646,19 @@ class EngineImpl final : public Engine {
             // output stage: each slot's text buffer holds the text a chunk is expected to produce (at most 4 bytes per
             // sentence plus the learned ratio per input byte); a chunk with more text flags itself and the batch is
             // re-run with the ratio it measured
-            const double text_ratio = text_ratio_ref();
+            // (sample text: n renderings per sentence, the ratio learned per rendering)
+            const uint32_t renders = sample_text_ ? samp_n_ : 1;
+            const double text_ratio = text_ratio_ref() * renders;
+            const uint64_t per_sent = uint64_t(text_per_sent_) * renders;
             if (fmt)
                 for (int i = 0; i < 2; ++i) {
                     ensure_format(out_[i], ws_[dual_stream_ ? i : 0], max_chunk_sent);
-                    out_[i].buf[kText].ensure(size_t(double(max_chunk_bytes) * text_ratio) + size_t(max_chunk_sent) * text_per_sent_ + 4096);
+                    out_[i].buf[kText].ensure(size_t(double(max_chunk_bytes) * text_ratio) + size_t(max_chunk_sent) * per_sent + 4096);
                 }
             // a pinned result sized from the learned ratios per input byte (grown below if short)
             HostResult* r = pool_.acquire(outputs(), n_sent,
                                           Totals{uint64_t(double(n_bytes) * tok_per_byte_) + 1024,
-                                                 uint64_t(double(n_bytes) * text_ratio) + uint64_t(n_sent) * text_per_sent_ + 1024,
+                                                 uint64_t(double(n_bytes) * text_ratio) + uint64_t(n_sent) * per_sent + 1024,
                                                  uint64_t(double(n_bytes) * node_per_byte_) + 1024,
                                                  uint64_t(double(n_bytes) * tok_per_byte_ * samp_n_) + 1024});
             CK(cudaMemsetAsync(base_.p, 0, kNumGroups * 8, stream_));
@@ -645,7 +671,7 @@ class EngineImpl final : public Engine {
             std::memset(counters_, 0, sizeof(counters_));
             launches_ = 0;
             Totals sum{};  // records per group of the chunks drained so far
-            double text_need = 0;  // text bytes per input byte beyond text_per_sent_ per sentence, largest over the sound chunks
+            double text_need = 0;  // text bytes per input byte beyond per_sent per sentence, largest over the sound chunks
             uint32_t route = kRouteNone;
             bool overflow = false, bad_utf8 = false, bad_offsets = false, slots_overflow = false, text_overflow = false;
             bool bad_bounds = false;
@@ -688,7 +714,7 @@ class EngineImpl final : public Engine {
                 pool_need_ = std::max<uint64_t>(pool_need_, pool_need(*o.h_ctrl));
                 const Totals count = totals(*o.h_ctrl);
                 if (fmt && !(o.h_ctrl->flags & (kFlagsStandDown | kFlagUtf8Error | kFlagPoolOverflow)))
-                    text_need = std::max(text_need, (double(count[kGroupText]) - double(text_per_sent_) * (s1 - s0)) /
+                    text_need = std::max(text_need, (double(count[kGroupText]) - double(per_sent) * (s1 - s0)) /
                                                         double(std::max<uint64_t>(1, off[s1] - off[s0])));
                 if (!overflow && !text_overflow && !bad_utf8 && !bad_offsets && !bad_bounds) {
                     // offsets are global already (base_); a record array that is short grows (rare), keeping what it
@@ -745,14 +771,14 @@ class EngineImpl final : public Engine {
                 if (slots_overflow) chars_per_byte_ = 1.0;
                 if (overflow)
                     cand_per_byte_ = std::max(cand_per_byte_ * 1.5, double(pool_need_) / double(std::max<uint64_t>(1, max_chunk_bytes)) * 1.2);
-                if (text_overflow) text_ratio_ref() = std::max(text_ratio * 1.5, text_need * 1.05);
+                if (text_overflow) text_ratio_ref() = std::max(text_ratio * 1.5, text_need * 1.05) / renders;
                 continue;
             }
             if (max_chunk_bytes)
                 cand_per_byte_ = std::max(0.25, double(pool_need_) / double(max_chunk_bytes) * 1.25);
             if (n_bytes) tok_per_byte_ = std::max(0.02, double(sum[kGroupTokens]) / double(n_bytes) * 1.1);
             if (n_bytes) chars_per_byte_ = std::min(1.0, double(slots_seen - n_sent) / double(n_bytes) * 1.10);
-            if (fmt) text_ratio_ref() = std::max(0.5, text_need * 1.25);
+            if (fmt) text_ratio_ref() = std::max(0.5, text_need * 1.25 / renders);
             if (n_bytes && lattice_) node_per_byte_ = std::max(0.1, double(sum[kGroupLattice]) / double(n_bytes) * 1.1);
             connid_commit(stream_);
             last_route_ = route;
@@ -875,6 +901,8 @@ class EngineImpl final : public Engine {
             throw Error(kInvalidArgument, "batch too large: split it (at most 2^27 sentences / 2^32 characters per call)");
         if (n_sent * samp_n_ >= 0xFFFFFFFFull)
             throw Error(kInvalidArgument, "sampling: n_sent * n must stay below 2^32: split the batch or draw fewer samples");
+        if (sample_base_ + n_sent > kMaxSampleBase)
+            throw Error(kInvalidArgument, "sampling: sample_base + n_sent exceeds 2^32, the range of the draws' sentence index");
     }
 
     static constexpr const char* kBadBoundsMsg =
@@ -984,29 +1012,57 @@ class EngineImpl final : public Engine {
         return (lattice_ == 2 && output_mode_ == kOutFormat && (fmt_uses_ & kUsesBest)) ? o.buf[kLinks].as<int2>() : nullptr;
     }
 
-    // Text bytes per input byte expected for the output mode; lattice text is learned apart (about 17x larger).
-    double& text_ratio_ref() { return lattice_ == 2 ? text_per_byte_lat_[output_mode_] : text_per_byte_[output_mode_]; }
+    // Text bytes per input byte expected for the output mode; lattice text is learned apart (about 17x larger), and so
+    // is sample text, per rendering of a sentence.
+    double& text_ratio_ref() {
+        return lattice_ == 2 ? text_per_byte_lat_[output_mode_] : sample_text_ ? text_per_byte_samp_[output_mode_] : text_per_byte_[output_mode_];
+    }
 
     // Output stage buffers of slot `o` and scan storage of `w` for (chunks of) up to n_sent sentences.
     void ensure_format(OutSlot& o, Workspace& w, uint32_t n_sent) {
-        o.sent_len.ensure((size_t(n_sent) + 1) * 8, 1.25);
+        const size_t units = size_t(n_sent) * (sample_text_ ? samp_n_ : 1) + 1;  // sentences, or walks in sample text
+        o.sent_len.ensure(units * 8, 1.25);
+        if (sample_text_) o.walk_off.ensure(units * 8, 1.25);
         o.buf[kTextOff].ensure((size_t(n_sent) + 1) * 8, 1.25);
         size_t tmp = 0;
         CK(cub::DeviceScan::ExclusiveSum(nullptr, tmp, static_cast<unsigned long long*>(nullptr),
-                                         static_cast<unsigned long long*>(nullptr), size_t(n_sent) + 1, w.stream));
+                                         static_cast<unsigned long long*>(nullptr), units, w.stream));
         w.scan_tmp.ensure(tmp + 1024, 1.5);
     }
 
     // Output stage, pass 1 and the scan on w.stream: the text offsets of `o` = where each sentence's text starts in its
-    // text (n_sent + 1 entries, relative to the batch or chunk in `o`).  Returns the arguments of pass 2.
+    // text (n_sent + 1 entries, relative to the batch or chunk in `o`).  Returns the arguments of pass 2.  Sample text
+    // renders the walks of the samples instead: its offsets per walk go to o.walk_off, and pass 2 (format_write)
+    // takes those of each sentence's first walk into the text offsets.
     FormatArgs format_offsets(Workspace& w, const uint8_t* d_utf8, const unsigned long long* d_off, uint32_t n_sent, OutSlot& o) {
+        if (sample_text_) {
+            FormatArgs f = format_args(d_utf8, d_off, n_sent, o, o.buf[kSampleOff], o.buf[kSamples]);
+            const size_t walks = size_t(n_sent) * samp_n_;
+            f.text_off = o.walk_off.as<unsigned long long>();
+            CK(cudaMemsetAsync(f.sent_len + walks, 0, 8, w.stream));
+            if (!n_sent) CK(cudaMemsetAsync(o.buf[kTextOff].p, 0, 8, w.stream));  // no walk writes it
+            launch_format_len_samples(dv_, f, samp_n_, w.stream);
+            exclusive_scan(w, f.sent_len, f.text_off, walks + 1);
+            return f;
+        }
+        const bool nodes = lattice_ == 2;  // lattice text: the nodes are rendered as tokens
+        FormatArgs f = format_args(d_utf8, d_off, n_sent, o, o.buf[nodes ? kNodeOff : kTokOff], o.buf[nodes ? kNodes : kTokens]);
+        f.token_prob = (o.made.marg && (fmt_uses_ & kUsesProb)) ? o.buf[nodes ? kNodeProb : kTokenProb].as<float>() : nullptr;  // %pP
+        CK(cudaMemsetAsync(f.sent_len + n_sent, 0, 8, w.stream));
+        launch_format_len(dv_, f, w.stream, fmt_links(o));
+        exclusive_scan(w, f.sent_len, f.text_off, size_t(n_sent) + 1);
+        return f;
+    }
+
+    // The arguments of the output stage for slot `o`, rendering the records `tokens` at the offsets `tok_off`.
+    FormatArgs format_args(const uint8_t* d_utf8, const unsigned long long* d_off, uint32_t n_sent, OutSlot& o,
+                           const DevBuf& tok_off, const DevBuf& tokens) const {
         FormatArgs f{};
         f.utf8 = d_utf8;
         f.byte_off = d_off;
         f.n_sent = n_sent;
-        const bool nodes = lattice_ == 2;  // lattice text: the nodes are rendered as tokens
-        f.tok_off = o.buf[nodes ? kNodeOff : kTokOff].as<unsigned long long>();
-        f.tokens = o.buf[nodes ? kNodes : kTokens].as<uint2>();
+        f.tok_off = tok_off.as<unsigned long long>();
+        f.tokens = tokens.as<uint2>();
         f.sent_len = o.sent_len.as<unsigned long long>();
         f.text_off = o.buf[kTextOff].as<unsigned long long>();
         f.text = o.buf[kText].as<uint8_t>();
@@ -1015,11 +1071,15 @@ class EngineImpl final : public Engine {
         f.flags = &dc->flags;
         f.text_total = &dc->total[kGroupText];
         set_mode(f);
-        f.token_prob = (o.made.marg && (fmt_uses_ & kUsesProb)) ? o.buf[nodes ? kNodeProb : kTokenProb].as<float>() : nullptr;  // %pP
-        CK(cudaMemsetAsync(f.sent_len + n_sent, 0, 8, w.stream));
-        launch_format_len(dv_, f, w.stream, fmt_links(o));
-        exclusive_scan(w, f.sent_len, f.text_off, size_t(n_sent) + 1);
         return f;
+    }
+
+    // Output stage, pass 2 on `st`, after format_offsets.
+    void format_write(const FormatArgs& f, OutSlot& o, cudaStream_t st) {
+        if (sample_text_)
+            launch_format_write_samples(dv_, f, samp_n_, o.buf[kTextOff].as<unsigned long long>(), st);
+        else
+            launch_format_write(dv_, f, st, fmt_links(o));
     }
 
     // Output stage of a whole batch (or shard) that run_whole left in out_[0]: the text buffer is sized from the
@@ -1029,12 +1089,13 @@ class EngineImpl final : public Engine {
         ensure_format(o, ws_[0], n_sent);
         FormatArgs f = format_offsets(ws_[0], d_utf8, d_off, n_sent, o);
         unsigned long long total = 0;
-        CK(cudaMemcpyAsync(&total, f.text_off + n_sent, 8, cudaMemcpyDeviceToHost, stream_));
+        const size_t units = size_t(n_sent) * (sample_text_ ? samp_n_ : 1);  // the scan's last entry is the total
+        CK(cudaMemcpyAsync(&total, f.text_off + units, 8, cudaMemcpyDeviceToHost, stream_));
         CK(cudaStreamSynchronize(stream_));
         o.buf[kText].ensure(total + 16, 1.25);
         f.text = o.buf[kText].as<uint8_t>();
         f.text_cap = o.buf[kText].cap;
-        launch_format_write(dv_, f, stream_, fmt_links(o));
+        format_write(f, o, stream_);
         launches_ += 2;
         o.h_ctrl->total[kGroupText] = total;
         o.made.text = true;
@@ -1555,7 +1616,7 @@ class EngineImpl final : public Engine {
             SampleArgs sa{};
             sa.n = samp_n_;
             sa.seed = samp_seed_;
-            sa.sent_base = sent0;
+            sa.sent_base = sample_base_ + sent0;
             sa.cnt = w.s_cnt.as<uint32_t>();
             sa.total = w.s_total.as<int32_t>();
             sa.off = o.buf[kSampleOff].as<unsigned long long>();
@@ -1584,7 +1645,7 @@ class EngineImpl final : public Engine {
         k_publish_totals<<<1, 1, 0, st>>>(b.slot_off, b.tok_off, n_sent, dc);
         if (o.made.text) {  // output stage of a chunk: formatted while its token offsets are still chunk-local
             FormatArgs f = format_offsets(w, d_utf8, d_off, n_sent, o);
-            launch_format_write(dv_, f, st, fmt_links(o));
+            format_write(f, o, st);
             o.launches += 2;
         }
         if (base) {
@@ -1659,6 +1720,8 @@ class EngineImpl final : public Engine {
     static constexpr double kLatticeTextFactor = 17.0;
     double text_per_byte_lat_[5] = {0.0, 8.0 * kLatticeTextFactor, 2.0 * kLatticeTextFactor, 16.0 * kLatticeTextFactor,
                                     kFormatTextPerByte * kLatticeTextFactor};
+    // and for sample text ("sample_text" = 1), per rendering of a sentence: each sentence renders samp_n_ times
+    double text_per_byte_samp_[5] = {0.0, 8.0, 2.0, 16.0, kFormatTextPerByte};
     double node_per_byte_ = 2.0;  // lattice nodes per input byte: sizes the host result of the chunked pipeline
     uint32_t text_per_sent_ = 4;  // "EOS\n"; an output format: what its BOS and EOS print (FormatProgram::per_sentence)
     // output format (set_format): the compiled program and its field table, with the table's size and build time
@@ -1676,6 +1739,9 @@ class EngineImpl final : public Engine {
     uint32_t samp_n_ = 0;       // sampling: paths per sentence, 0 = off (set_sampling)
     double samp_theta_ = 0;
     uint64_t samp_seed_ = 0;
+    bool sample_text_ = false;  // option "sample_text": the output text renders the samples
+    static constexpr long long kMaxSampleBase = 0x100000000ll;
+    uint64_t sample_base_ = 0;  // option "sample_base": the draws' index of the call's first sentence
     Outputs made_;  // the arrays the last run_device produced (device_marginals, _lattice, _samples)
     float stage_ms_[kNumStages];
     uint64_t launches_ = 0;

@@ -14,7 +14,8 @@ namespace {
 
 class Compiler {
    public:
-    Compiler(FormatProgram& p, bool marginals, bool lattice_text) : p_(p), marginals_(marginals), lattice_text_(lattice_text) {}
+    Compiler(FormatProgram& p, bool marginals, bool lattice_text, bool sample_text)
+        : p_(p), marginals_(marginals), lattice_text_(lattice_text), sample_text_(sample_text) {}
 
     // Appends the ops of one format string as section `sec`; `tokens` = false admits only what BOS / EOS can print.
     void section(uint32_t sec, const char* name, const char* s, size_t n, bool tokens) {
@@ -54,6 +55,9 @@ class Compiler {
                 dir += s[i++];
                 if (dir == "%ph" && i < n && (s[i] == 'l' || s[i] == 'r')) dir += s[i++];
             }
+            if (sample_text_ && (dir == "%pP" || dir == "%pb"))
+                fail(at, dir + " has no value in sample text (option \"sample_text\" = 1): a sampled token has no " +
+                             (dir == "%pP" ? "marginal" : "best-path flag"));
             if (dir == "%pP" && marginals_) {
                 if (!tokens) fail(at, dir + " is not allowed here (only literals, %%, %S and %L)");
                 op(kOpProb, at);
@@ -204,6 +208,7 @@ class Compiler {
     const char* name_ = "";
     bool marginals_ = false;
     bool lattice_text_ = false;
+    bool sample_text_ = false;
     bool open_lit_ = false;
     std::vector<uint32_t> raw_;
 };
@@ -218,10 +223,10 @@ uint32_t fixed_bytes(const FormatProgram& p, uint32_t a, uint32_t b) {
 }  // namespace
 
 FormatProgram compile_format(FormatText node, FormatText unk, FormatText bos, FormatText eos, bool marginals,
-                             bool lattice_text) {
+                             bool lattice_text, bool sample_text) {
     FormatProgram p;
     std::memset(&p, 0, sizeof p);
-    Compiler c(p, marginals, lattice_text);
+    Compiler c(p, marginals, lattice_text, sample_text);
     if (!node.ptr) throw Error(kInvalidArgument, "format: the node format must be given");
     c.section(kSecNode, "node", node.ptr, node.len, true);
     if (unk.ptr) {

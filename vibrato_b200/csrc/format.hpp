@@ -11,6 +11,8 @@
 //   %pP the token's marginal probability as d.dddddd (only while marginals are on)
 //   %pb '*' for a node of the best path, ' ' otherwise (only in lattice text, option "lattice" = 2, where the "prev"
 //   directives %M %pS %pn %pC %pL are refused: a node has no previous token)
+// Sample text ("sample_text" = 1) renders each sampled path like a sentence's tokens: "prev" is the previous record of
+// the same sample, and %pP / %pb are refused (a sampled record has no marginal and no best-path flag).
 // Escapes \0 \a \b \t \n \v \f \r \s(space) \\ are replaced by the compiler.  BOS / EOS take literals, %%, %S, %L.
 #pragma once
 
@@ -78,8 +80,9 @@ struct FormatText {  // one format string: ptr == nullptr means "not given"
 // Error(kInvalidArgument, "<which> format, byte <pos>: ...") naming the offending directive or escape.
 // `marginals`: the tokenizer computes marginal probabilities, so %pP has a value (otherwise it is refused).
 // `lattice_text`: the text renders lattice nodes ("lattice" = 2), so %pb has a value and the "prev" directives do not.
+// `sample_text`: the text renders the samples ("sample_text" = 1), so neither %pP nor %pb has a value.
 FormatProgram compile_format(FormatText node, FormatText unk, FormatText bos, FormatText eos, bool marginals = false,
-                             bool lattice_text = false);
+                             bool lattice_text = false, bool sample_text = false);
 #endif
 
 }  // namespace vbt

@@ -2174,14 +2174,16 @@ __device__ __forceinline__ const FormatProgram* stage_program(const FormatArgs& 
 }
 
 // Pass 1 for sentence s (a warp per sentence): lane 0 stores its text length in sent_len[s].  PROG: f.mode is
-// kOutFormat (a separate instantiation, so that the fixed modes keep their registers).
+// kOutFormat (a separate instantiation, so that the fixed modes keep their registers).  Sample text (n_samp > 1):
+// s is the walk s' * n_samp + j, whose records are tok_off[s] .. tok_off[s + 1], rendered with sentence s' = s / n_samp.
 template <bool PROG, bool PROB = false, bool BEST = false>
 __device__ __forceinline__ void format_len_one(const DictView& d, const FormatArgs& f, const FormatProgram* P, uint32_t s,
-                                               uint32_t lane, const int2* links = nullptr) {
+                                               uint32_t lane, const int2* links = nullptr, uint32_t n_samp = 1) {
     const unsigned long long t0 = f.tok_off[s], t1 = f.tok_off[s + 1];
     unsigned long long len = 0;
     if constexpr (PROG) {
-        const uint32_t sl = uint32_t(f.byte_off[s + 1] - f.byte_off[s]);
+        const uint32_t si = s / n_samp;
+        const uint32_t sl = uint32_t(f.byte_off[si + 1] - f.byte_off[si]);
         for (unsigned long long t = t0 + lane; t < t1; t += 32) {
             const FmtTok v = fmt_tok<PROB, BEST>(d, f, *P, t, t0, links);
             const uint32_t sec = v.x.lex == 2 ? kSecUnk : kSecNode;
@@ -2382,15 +2384,17 @@ __global__ void __launch_bounds__(256) k_field_table_write(DictView d, FieldTabl
     });
 }
 
-// Pass 2 for sentence s (a warp per sentence): its text at text_off[s], which must fit in text_cap.
+// Pass 2 for sentence s (a warp per sentence): its text at text_off[s], which must fit in text_cap.  n_samp > 1: s
+// is a walk, as in format_len_one.
 template <bool PROG, bool PROB = false, bool BEST = false>
 __device__ __forceinline__ void format_write_one(const DictView& d, const FormatArgs& f, const FormatProgram* P, uint32_t s,
-                                                 uint32_t lane, const int2* links = nullptr) {
+                                                 uint32_t lane, const int2* links = nullptr, uint32_t n_samp = 1) {
     const unsigned long long t0 = f.tok_off[s], t1 = f.tok_off[s + 1];
-    const uint8_t* __restrict__ sent = f.utf8 + f.byte_off[s];
+    const uint32_t si = s / n_samp;
+    const uint8_t* __restrict__ sent = f.utf8 + f.byte_off[si];
     unsigned long long base = f.text_off[s];  // where the next group of 32 tokens starts
     const bool prog = PROG;
-    const uint32_t sl = prog ? uint32_t(f.byte_off[s + 1] - f.byte_off[s]) : 0u;
+    const uint32_t sl = prog ? uint32_t(f.byte_off[si + 1] - f.byte_off[si]) : 0u;
     if (prog) {
         const FmtTok none{};
         base = fmt_write<PROB, BEST>(d, *P, P->sec[kSecBos][0], P->sec[kSecBos][1], f, none, sent, sl, f.text + base, lane) - f.text;
@@ -2512,6 +2516,43 @@ __global__ void __launch_bounds__(256) k_format_write_best(DictView d, FormatArg
     }
     if (total > f.text_cap) return;
     format_write_one<true, PROB, true>(d, f, P, s, lane, links);
+}
+
+// Sample text: a warp per walk w = s * n + j of the samples (f.tok_off / f.tokens are the sample offsets and records;
+// f.sent_len and f.text_off have an entry per walk), rendered with the text of sentence s (separate kernels, so that
+// the instantiations above keep their code).  The write pass also stores each sentence's text offset, that of its
+// first walk, in sent_text_off[0 .. n_sent].
+__device__ __forceinline__ unsigned long long walk_of_warp() {
+    return ((unsigned long long)(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
+}
+
+template <bool PROG>
+__global__ void __launch_bounds__(256) k_format_len_samples(DictView d, FormatArgs f, uint32_t n) {
+    extern __shared__ uint4 s_dyn[];
+    const FormatProgram* P = PROG ? stage_program(f, reinterpret_cast<FormatProgram*>(s_dyn)) : nullptr;
+    const unsigned long long w = walk_of_warp();
+    const uint32_t lane = threadIdx.x & 31;
+    if (w >= (unsigned long long)(f.n_sent) * n || format_stands_down(f)) return;
+    format_len_one<PROG>(d, f, P, uint32_t(w), lane, nullptr, n);
+}
+
+template <bool PROG>
+__global__ void __launch_bounds__(256) k_format_write_samples(DictView d, FormatArgs f, uint32_t n,
+                                                              unsigned long long* sent_text_off) {
+    extern __shared__ uint4 s_dyn[];
+    const FormatProgram* P = PROG ? stage_program(f, reinterpret_cast<FormatProgram*>(s_dyn)) : nullptr;
+    const unsigned long long w = walk_of_warp(), walks = (unsigned long long)(f.n_sent) * n;
+    const uint32_t lane = threadIdx.x & 31;
+    if (w >= walks || format_stands_down(f)) return;
+    const unsigned long long total = f.text_off[walks];
+    if (lane == 0 && w % n == 0) sent_text_off[w / n] = f.text_off[w];
+    if (w == 0 && lane == 0) {
+        sent_text_off[f.n_sent] = total;
+        *f.text_total = total;
+        if (total > f.text_cap) atomicOr(f.flags, kFlagTextOverflow);
+    }
+    if (total > f.text_cap) return;
+    format_write_one<PROG>(d, f, P, uint32_t(w), lane, nullptr, n);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -2715,6 +2756,25 @@ void launch_format_write(const DictView& d, const FormatArgs& f, cudaStream_t st
                      : k_format_write<true><<<(f.n_sent + 7) / 8, 256, sizeof(FormatProgram), st>>>(d, f);
     else
         k_format_write<false><<<(f.n_sent + 7) / 8, 256, 0, st>>>(d, f);
+}
+
+void launch_format_len_samples(const DictView& d, const FormatArgs& f, uint32_t n, cudaStream_t st) {
+    const unsigned long long blocks = ((unsigned long long)(f.n_sent) * n + 7) / 8;
+    if (!blocks) return;
+    if (f.mode == kOutFormat)
+        k_format_len_samples<true><<<unsigned(blocks), 256, sizeof(FormatProgram), st>>>(d, f, n);
+    else
+        k_format_len_samples<false><<<unsigned(blocks), 256, 0, st>>>(d, f, n);
+}
+
+void launch_format_write_samples(const DictView& d, const FormatArgs& f, uint32_t n, unsigned long long* sent_text_off,
+                                 cudaStream_t st) {
+    const unsigned long long blocks = ((unsigned long long)(f.n_sent) * n + 7) / 8;
+    if (!blocks) return;
+    if (f.mode == kOutFormat)
+        k_format_write_samples<true><<<unsigned(blocks), 256, sizeof(FormatProgram), st>>>(d, f, n, sent_text_off);
+    else
+        k_format_write_samples<false><<<unsigned(blocks), 256, 0, st>>>(d, f, n, sent_text_off);
 }
 
 void launch_field_table_len(const DictView& d, const FieldTableArgs& a, cudaStream_t st) {

@@ -166,6 +166,13 @@ struct FormatArgs {
 // links != nullptr (lattice text whose program prints %pb; f.tokens are then the nodes): the %pb instantiation.
 void launch_format_len(const DictView& d, const FormatArgs& f, cudaStream_t st, const int2* links = nullptr);
 void launch_format_write(const DictView& d, const FormatArgs& f, cudaStream_t st, const int2* links = nullptr);
+// Sample text ("sample_text" = 1): the n samples of every sentence rendered in order, each as a sentence whose tokens
+// are the walk's records.  f.tok_off / f.tokens are the samples' offsets (n_sent * n + 1) and records; f.sent_len and
+// f.text_off have n_sent * n + 1 entries, one per walk s * n + j; the write pass also stores sent_text_off[s] =
+// f.text_off[s * n] for s = 0 .. n_sent (not for an empty batch).  The program may not print %pP or %pb.
+void launch_format_len_samples(const DictView& d, const FormatArgs& f, uint32_t n, cudaStream_t st);
+void launch_format_write_samples(const DictView& d, const FormatArgs& f, uint32_t n, unsigned long long* sent_text_off,
+                                 cudaStream_t st);
 
 // Field table of a format program, built once per format and device from the feature strings of the image.
 struct FieldTableArgs {

@@ -353,6 +353,7 @@ class MultiEngine final : public Engine {
         if (name == "chunk_sentences") return;  // shards are not chunked (see the constructor)
         for (auto& e : eng_) e->set_option(name, value);
         if (name == "lattice") lattice_ = int(value);
+        if (name == "sample_base") sample_base_ = uint64_t(value);
         if (name == "output_mode") text_ = fixed_mode_ = value != 0;
     }
     void set_format(const FormatProgram* p) override {
@@ -454,6 +455,8 @@ class MultiEngine final : public Engine {
     void check_samples(uint64_t n_sent) const {
         if (n_sent * sampling() >= 0xFFFFFFFFull)
             throw Error(kInvalidArgument, "sampling: n_sent * n must stay below 2^32: split the batch or draw fewer samples");
+        if (sample_base_ + n_sent > 0x100000000ull)
+            throw Error(kInvalidArgument, "sampling: sample_base + n_sent exceeds 2^32, the range of the draws' sentence index");
     }
 
     static void grow_pinned(void*& p, size_t& cap, size_t bytes) {
@@ -541,6 +544,7 @@ class MultiEngine final : public Engine {
     Outputs made_;               // the arrays the last device-resident call produced
     Totals made_total_{};
     int lattice_ = 0;  // option "lattice"
+    uint64_t sample_base_ = 0;  // option "sample_base" (every engine adds it to its shard's first sentence)
     float stage_ms_[kNumStages];
     uint64_t counters_[10];
     uint64_t launches_ = 0;
