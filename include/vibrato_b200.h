@@ -239,6 +239,41 @@ int32_t vbt_tokenize_batch(vbt_tokenizer *t, const char *utf8, const uint64_t *b
  * describe the unconstrained walk. */
 int32_t vbt_tokenize_batch_bounded(vbt_tokenizer *t, const char *utf8, const uint64_t *byte_offsets, uint64_t n_sent,
                                    const uint64_t *bnd_offsets, const uint32_t *bnd, vbt_result **out);
+/* Required tokens (MeCab's partial analysis, -p, with feature patterns): a span [start_byte, end_byte) of a sentence
+ * that must be exactly one token, optionally one whose feature matches a pattern.  Byte offsets are
+ * sentence-relative; pattern is VBT_SPAN_ANY or an index into the call's pattern table. */
+#define VBT_SPAN_ANY 0xFFFFFFFFu
+typedef struct vbt_span {
+    uint32_t start_byte, end_byte, pattern;
+} vbt_span;
+/* As vbt_tokenize_batch_bounded, with required tokens.  Sentence i's spans are spans[span_offsets[i] ..
+ * span_offsets[i+1]); bnd_offsets / bnd may both be null (no explicit boundary), and span_offsets may not.  Pattern k
+ * is the bytes patterns[pattern_offsets[k] .. pattern_offsets[k+1]) (n_patterns of them; both pointers may be null
+ * when n_patterns is 0).
+ * Definition, in character positions, for a span [a, b): (1) a and b are required boundaries, exactly as in
+ * vbt_tokenize_batch_bounded; (2) no lattice node ends strictly inside the span; (3) where a word starts at a, its
+ * candidates are the user-, then the system-lexicon words of surface [a, b) whose feature matches the pattern, in
+ * lattice order; without any, one unknown word over [a, b) per unk.def entry of the category of character a that
+ * matches (all of the category's entries when none matches), whatever max_grouping_len and the category's
+ * invoke / group / length say; (4) a pattern is split into fields like a feature (csv); a word matches when each
+ * pattern field that is not exactly "*" equals the word's field of the same index byte for byte, and a field the
+ * word lacks never matches; an empty pattern matches every word; (5) the space skip of ignore_space is unchanged;
+ * (6) nothing else changes.  Guarantee: each span is exactly one token, no token starts or ends inside it, and when
+ * some lexicon word of its surface matches the pattern, the token is one of them.  The token keeps its word's own
+ * feature (MeCab would print the pattern).
+ * Input rules, checked on the device: within a sentence spans are sorted and do not overlap (adjacent is allowed);
+ * start < end <= the sentence's byte length, both on a UTF-8 lead byte or at the end; pattern is VBT_SPAN_ANY or
+ * below n_patterns; no explicit boundary lies strictly inside a span; with ignore_space no span starts at a SPACE
+ * character; span_offsets is non-decreasing.  Anything else fails with VBT_ERR_INVALID_ARGUMENT, after the errors of
+ * vbt_tokenize_batch_bounded.  Patterns are compiled on the host: at most 16 constrained fields and field indices up
+ * to 255 (VBT_ERR_INVALID_ARGUMENT naming the pattern and byte position).  A batch whose span lists are all empty is
+ * the bounded (or the plain) call.  Works on single- and multi-device tokenizers, on the whole-batch and chunked host
+ * routes ("small_batch" steps aside), with marginals, the lattice, sampling, output modes and formats,
+ * "compact_tokens" and "connid_counting"; "counting" refuses it. */
+int32_t vbt_tokenize_batch_spans(vbt_tokenizer *t, const char *utf8, const uint64_t *byte_offsets, uint64_t n_sent,
+                                 const uint64_t *bnd_offsets, const uint32_t *bnd, const uint64_t *span_offsets,
+                                 const vbt_span *spans, const char *patterns, const uint64_t *pattern_offsets,
+                                 uint64_t n_patterns, vbt_result **out);
 /* Worker::num_tokens / token(i) / token_iter (worker.rs:59-74) for the whole batch:
  * tokens of sentence i are toks[tok_offsets[i] .. tok_offsets[i+1]), in sentence order. */
 int32_t vbt_result_view(const vbt_result *r, const uint64_t **tok_offsets, const vbt_token **toks,
@@ -275,6 +310,15 @@ int32_t vbt_tokenize_batch_device(vbt_tokenizer *t, uint64_t d_utf8, uint64_t d_
 int32_t vbt_tokenize_batch_device_bounded(vbt_tokenizer *t, uint64_t d_utf8, uint64_t d_byte_offsets, uint64_t n_sent,
                                           uint64_t n_bytes, uint64_t d_bnd_offsets, uint64_t d_bnd, uint64_t n_bnd,
                                           uint64_t *d_tok_offsets, uint64_t *d_tokens, uint64_t *n_tokens);
+
+/* As vbt_tokenize_batch_device with the required tokens of vbt_tokenize_batch_spans: d_bnd_offsets / d_bnd (may be 0:
+ * no explicit boundary), d_span_offsets (uint64[n_sent+1]) and d_spans (vbt_span[n_spans]) are DEVICE addresses, every
+ * offset must be <= its array's length; the patterns stay in HOST memory. */
+int32_t vbt_tokenize_batch_device_spans(vbt_tokenizer *t, uint64_t d_utf8, uint64_t d_byte_offsets, uint64_t n_sent,
+                                        uint64_t n_bytes, uint64_t d_bnd_offsets, uint64_t d_bnd, uint64_t n_bnd,
+                                        uint64_t d_span_offsets, uint64_t d_spans, uint64_t n_spans,
+                                        const char *patterns, const uint64_t *pattern_offsets, uint64_t n_patterns,
+                                        uint64_t *d_tok_offsets, uint64_t *d_tokens, uint64_t *n_tokens);
 
 /* Pinned host memory for callers that want full-speed host<->device copies. */
 int32_t vbt_host_alloc(size_t n_bytes, void **out);

@@ -36,6 +36,10 @@ extern "C" {
     fn vbt_tokenizer_free(t: *mut vbt_tokenizer);
     fn vbt_tokenize_batch(t: *mut vbt_tokenizer, utf8: *const c_char, byte_offsets: *const u64, n_sent: u64,
                           out: *mut *mut vbt_result) -> i32;
+    fn vbt_tokenize_batch_spans(t: *mut vbt_tokenizer, utf8: *const c_char, byte_offsets: *const u64, n_sent: u64,
+                                bnd_offsets: *const u64, bnd: *const u32, span_offsets: *const u64, spans: *const Span,
+                                patterns: *const c_char, pattern_offsets: *const u64, n_patterns: u64,
+                                out: *mut *mut vbt_result) -> i32;
     fn vbt_result_view(r: *const vbt_result, tok_offsets: *mut *const u64, toks: *mut *const vbt_token,
                        n_sent: *mut u64, n_tokens: *mut u64) -> i32;
     fn vbt_result_free(r: *mut vbt_result);
@@ -307,7 +311,42 @@ impl Tokenizer {
                                           lines.len() as u64, &mut r) })?;
         Ok(BatchResult { r, n_samples: self.samples.get() })
     }
+    /// Required tokens (vbt_tokenize_batch_spans): `spans[i]` are line i's spans, byte ranges that must each be one
+    /// token, with a feature pattern (csv fields, `*` for any) or `None` for any feature.  No explicit boundaries.
+    pub fn tokenize_batch_spans(&self, lines: &[String], spans: &[Vec<(u32, u32, Option<String>)>]) -> Result<BatchResult> {
+        let mut utf8 = Vec::new();
+        let mut off = vec![0u64];
+        for l in lines { utf8.extend_from_slice(l.as_bytes()); off.push(utf8.len() as u64); }
+        let (mut span_off, mut recs) = (vec![0u64], Vec::new());
+        let (mut pat, mut pat_off, mut index) = (Vec::new(), vec![0u64], std::collections::HashMap::new());
+        for i in 0..lines.len() {
+            for (a, b, p) in spans.get(i).map(|v| v.as_slice()).unwrap_or(&[]) {
+                let k = match p {
+                    None => SPAN_ANY,
+                    Some(p) => *index.entry(p.clone()).or_insert_with(|| {
+                        pat.extend_from_slice(p.as_bytes());
+                        pat_off.push(pat.len() as u64);
+                        (pat_off.len() - 2) as u32
+                    }),
+                };
+                recs.push(Span { start_byte: *a, end_byte: *b, pattern: k });
+            }
+            span_off.push(recs.len() as u64);
+        }
+        let mut r = std::ptr::null_mut();
+        check(unsafe { vbt_tokenize_batch_spans(self.handle(), utf8.as_ptr() as *const c_char, off.as_ptr(),
+                                                lines.len() as u64, std::ptr::null(), std::ptr::null(), span_off.as_ptr(),
+                                                recs.as_ptr(), pat.as_ptr() as *const c_char, pat_off.as_ptr(),
+                                                (pat_off.len() - 1) as u64, &mut r) })?;
+        Ok(BatchResult { r, n_samples: self.samples.get() })
+    }
 }
+
+/// vbt_span: a required token of vbt_tokenize_batch_spans.
+#[repr(C)]
+pub struct Span { pub start_byte: u32, pub end_byte: u32, pub pattern: u32 }
+/// VBT_SPAN_ANY: a required token of any feature.
+pub const SPAN_ANY: u32 = 0xFFFF_FFFF;
 
 pub struct BatchResult { r: *mut vbt_result, n_samples: u32 }
 impl Drop for BatchResult { fn drop(&mut self) { unsafe { vbt_result_free(self.r) } } }

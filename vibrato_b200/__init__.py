@@ -6,6 +6,6 @@ libvibrato_b200.so), `api` (host-side mirror of the reference's Rust API over th
 """
 from .api import (BatchResult, Dictionary, SystemDictionaryBuilder, Token, Tokenizer, VibratoError, WordIdx,  # noqa: F401
                   Worker, TOKEN_DTYPE, COMPACT_TOKEN_DTYPE, LEX_TYPE_NAMES, expand_compact_tokens,
-                  generate_bigram_info, LatticeNode, LINK_DTYPE, NODE_BEST)
+                  generate_bigram_info, LatticeNode, LINK_DTYPE, NODE_BEST, SPAN_ANY)
 
 __version__ = "0.1.0"

@@ -99,6 +99,10 @@ def lib():
     sig("vbt_tokenize_batch_bounded", i32, [vp, vp, vp, u64, vp, vp, pp])
     sig("vbt_tokenize_batch_device_bounded", i32,
         [vp, u64, u64, u64, u64, u64, u64, u64, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64)])
+    sig("vbt_tokenize_batch_spans", i32, [vp, vp, vp, u64, vp, vp, vp, vp, vp, vp, u64, pp])
+    sig("vbt_tokenize_batch_device_spans", i32,
+        [vp, u64, u64, u64, u64, u64, u64, u64, u64, u64, u64, vp, vp, u64, C.POINTER(u64), C.POINTER(u64),
+         C.POINTER(u64)])
     sig("vbt_host_alloc", i32, [sz, pp])
     sig("vbt_host_free", None, [vp])
     sig("vbt_tokenizer_set_counting", i32, [vp, i32])

@@ -27,6 +27,7 @@ TOKEN_DTYPE = np.dtype(
 )
 LINK_DTYPE = np.dtype([("prev", "<i4"), ("flags", "<u4")])  # vbt_lattice_link
 NODE_BEST = 1  # VBT_NODE_BEST
+SPAN_ANY = 0xFFFFFFFF  # VBT_SPAN_ANY: a required token of any feature
 LEX_TYPE_NAMES = ("System", "User", "Unknown")  # dictionary.rs:30-40 (Debug names used by tokenize -O detail)
 
 
@@ -516,21 +517,73 @@ class Tokenizer:
         flat = [v for b in boundaries for v in b]
         return off, np.array(flat, dtype=np.uint32)
 
-    def tokenize_batch(self, sentences=None, utf8=None, byte_offsets=None, boundaries=None, bnd_offsets=None, bnd=None):
+    @staticmethod
+    def pack_spans(spans):
+        """list[list[(start, end) | (start, end, pattern)]] (per-sentence byte offsets; pattern str or bytes) ->
+        (span_offsets uint64[n+1], span_records uint32[k, 3], patterns list[bytes]).  Equal patterns share one entry;
+        a span without a pattern gets VBT_SPAN_ANY."""
+        off = np.zeros(len(spans) + 1, dtype=np.uint64)
+        if spans:
+            off[1:] = np.cumsum([len(s) for s in spans], dtype=np.uint64)
+        index, patterns, rec = {}, [], []
+        for sent in spans:
+            for sp in sent:
+                p = SPAN_ANY
+                if len(sp) > 2 and sp[2] is not None:
+                    b = sp[2].encode("utf-8") if isinstance(sp[2], str) else bytes(sp[2])
+                    if b not in index:
+                        index[b] = len(patterns)
+                        patterns.append(b)
+                    p = index[b]
+                rec.append((sp[0], sp[1], p))
+        return off, np.array(rec, dtype=np.uint32).reshape(-1, 3), patterns
+
+    @staticmethod
+    def _pattern_table(patterns):
+        blobs = [p.encode("utf-8") if isinstance(p, str) else bytes(p) for p in patterns]
+        off = np.zeros(len(blobs) + 1, dtype=np.uint64)
+        if blobs:
+            off[1:] = np.cumsum([len(b) for b in blobs], dtype=np.uint64)
+        return np.frombuffer(b"".join(blobs) + b"\0", dtype=np.uint8), off
+
+    def tokenize_batch(self, sentences=None, utf8=None, byte_offsets=None, boundaries=None, bnd_offsets=None, bnd=None,
+                       spans=None, span_offsets=None, span_records=None, patterns=None):
         """reset_sentence + tokenize for every sentence of the batch on the GPU (host in, host out).
 
         Required boundaries (vbt_tokenize_batch_bounded): `boundaries` = one list of sentence-relative byte offsets
         per sentence, or the packed form bnd_offsets (uint64[n+1]) / bnd (uint32[]).  No token of a sentence crosses
-        one of its boundaries; the library validates them."""
+        one of its boundaries; the library validates them.
+
+        Required tokens (vbt_tokenize_batch_spans): `spans` = one list per sentence of (start, end) or
+        (start, end, pattern) byte ranges, each of which must be exactly one token (whose feature matches the
+        pattern, README "Required tokens"); or the packed form span_offsets (uint64[n+1]) / span_records
+        (uint32[k, 3]: start, end, pattern index or SPAN_ANY) / patterns (list of str or bytes).  Boundaries may
+        come with them."""
         if sentences is not None:
             utf8, byte_offsets = self.pack(sentences)
         if boundaries is not None:
             bnd_offsets, bnd = self.pack_bounds(boundaries)
+        if spans is not None:
+            span_offsets, span_records, patterns = self.pack_spans(spans)
         utf8 = np.ascontiguousarray(utf8, dtype=np.uint8)
         byte_offsets = np.ascontiguousarray(byte_offsets, dtype=np.uint64)
         n = len(byte_offsets) - 1
         h = C.c_void_p()
-        if bnd_offsets is None:
+        if span_offsets is not None:
+            span_offsets = np.ascontiguousarray(span_offsets, dtype=np.uint64)
+            recs = np.ascontiguousarray(span_records if span_records is not None else np.zeros((0, 3)),
+                                        dtype=np.uint32).reshape(-1, 3)
+            pat, pat_off = self._pattern_table(patterns or [])
+            if bnd_offsets is not None:
+                bnd_offsets = np.ascontiguousarray(bnd_offsets, dtype=np.uint64)
+                bnd = np.ascontiguousarray(bnd if bnd is not None else [], dtype=np.uint32)
+            check(lib().vbt_tokenize_batch_spans(
+                self.handle(), utf8.ctypes.data if utf8.size else None, byte_offsets.ctypes.data, n,
+                bnd_offsets.ctypes.data if bnd_offsets is not None else None,
+                bnd.ctypes.data if bnd_offsets is not None and bnd.size else None, span_offsets.ctypes.data,
+                recs.ctypes.data if recs.size else None, pat.ctypes.data, pat_off.ctypes.data, len(pat_off) - 1,
+                C.byref(h)))
+        elif bnd_offsets is None:
             check(lib().vbt_tokenize_batch(self.handle(), utf8.ctypes.data if utf8.size else None,
                                            byte_offsets.ctypes.data, n, C.byref(h)))
         else:
@@ -542,12 +595,20 @@ class Tokenizer:
         return BatchResult(self, h, utf8, byte_offsets, compact=bool(self._options.get("compact_tokens", 0)),
                            marginals=self._theta > 0, lattice=self._lattice > 0, samples=self._sampling[0])
 
-    def tokenize_batch_device(self, d_utf8, d_byte_offsets, n_sent, n_bytes, d_bnd_offsets=None, d_bnd=None, n_bnd=0):
+    def tokenize_batch_device(self, d_utf8, d_byte_offsets, n_sent, n_bytes, d_bnd_offsets=None, d_bnd=None, n_bnd=0,
+                              d_span_offsets=None, d_spans=None, n_spans=0, patterns=None):
         """Device-resident variant: addresses in, (d_tok_offsets, d_tokens, n_tokens) out.  With d_bnd_offsets
         (uint64[n_sent+1]) and d_bnd (uint32[n_bnd]), also device addresses: required boundaries as in
-        tokenize_batch."""
+        tokenize_batch.  With d_span_offsets (uint64[n_sent+1]) and d_spans (uint32[n_spans, 3]), device addresses,
+        and `patterns` (a host list): required tokens as in tokenize_batch."""
         a, b, n = C.c_uint64(), C.c_uint64(), C.c_uint64()
-        if d_bnd_offsets is None:
+        if d_span_offsets is not None:
+            pat, pat_off = self._pattern_table(patterns or [])
+            check(lib().vbt_tokenize_batch_device_spans(
+                self.handle(), int(d_utf8), int(d_byte_offsets), int(n_sent), int(n_bytes), int(d_bnd_offsets or 0),
+                int(d_bnd or 0), int(n_bnd), int(d_span_offsets), int(d_spans or 0), int(n_spans), pat.ctypes.data,
+                pat_off.ctypes.data, len(pat_off) - 1, C.byref(a), C.byref(b), C.byref(n)))
+        elif d_bnd_offsets is None:
             check(lib().vbt_tokenize_batch_device(self.handle(), int(d_utf8), int(d_byte_offsets), int(n_sent),
                                                   int(n_bytes), C.byref(a), C.byref(b), C.byref(n)))
         else:
@@ -839,14 +900,17 @@ class Worker:
         self._tok = tokenizer
         self._sent = b""
         self._bounds = None
+        self._spans = None
         self._tokens = []
         self._nodes = []
         self._samples = []
 
-    def reset_sentence(self, text, boundaries=None):
-        """boundaries: required token boundaries, byte offsets into the sentence (see Tokenizer.tokenize_batch)."""
+    def reset_sentence(self, text, boundaries=None, spans=None):
+        """boundaries: required token boundaries, byte offsets into the sentence; spans: required tokens, (start, end)
+        or (start, end, pattern) byte ranges (see Tokenizer.tokenize_batch)."""
         self._sent = text.encode("utf-8") if isinstance(text, str) else bytes(text)
         self._bounds = None if boundaries is None else list(boundaries)
+        self._spans = None if spans is None else list(spans)
         self._tokens = []
         self._nodes = []
         self._samples = []
@@ -855,7 +919,8 @@ class Worker:
         if not self._sent:  # worker.rs:50-52
             self._samples = [[] for _ in range(self._tok._sampling[0])]
             return
-        res = self._tok.tokenize_batch([self._sent], boundaries=None if self._bounds is None else [self._bounds])
+        res = self._tok.tokenize_batch([self._sent], boundaries=None if self._bounds is None else [self._bounds],
+                                       spans=None if self._spans is None else [self._spans])
         tp = res.token_probs
         self._tokens = [Token(self._tok, self._sent, r.copy(), None if tp is None else float(tp[k]))
                         for k, r in enumerate(res.tokens)]

@@ -8,6 +8,7 @@
 #include <cstdio>
 #include <fstream>
 #include <iostream>
+#include <map>
 #include <sstream>
 #include <string>
 #include <vector>
@@ -73,15 +74,64 @@ inline std::vector<uint32_t> strip_boundary_markers(std::string& line, char mark
     return bnd;
 }
 
+// tokenize -p: MeCab's partial-analysis input.  Lines up to a line that is exactly "EOS" form one sentence (lines
+// after the last "EOS" one more).  A line with a TAB is a required token: its surface is the text before the first
+// TAB, its feature pattern the rest.  Every line's start and end are required boundaries.
+struct PartialSentence {
+    std::string text;
+    std::vector<uint32_t> bnd;
+    std::vector<std::pair<std::pair<uint32_t, uint32_t>, std::string>> toks;  // {{start, end}, pattern}
+    bool pending = false;  // lines since the last EOS
+    // false for a line that starts with a TAB (an empty token)
+    bool add_line(const std::string& line) {
+        pending = true;
+        const size_t tab = line.find('\t');
+        if (tab == 0) return false;
+        const uint32_t start = uint32_t(text.size());
+        text.append(line, 0, tab);
+        if (tab != std::string::npos) toks.push_back({{start, uint32_t(text.size())}, line.substr(tab + 1)});
+        bnd.push_back(start);
+        bnd.push_back(uint32_t(text.size()));
+        return true;
+    }
+    void clear() {
+        text.clear();
+        bnd.clear();
+        toks.clear();
+        pending = false;
+    }
+};
+
 struct Packed {
     std::string utf8;
     std::vector<uint64_t> off{0};
     std::vector<uint64_t> bnd_off{0};  // required boundaries per line (--boundary-marker), bnd_off / bnd as CSR
     std::vector<uint32_t> bnd;
+    // required tokens per sentence (tokenize -p), span_off / spans as CSR; the batch's distinct patterns in pat / pat_off
+    std::vector<uint64_t> span_off{0};
+    std::vector<vbt_span> spans;
+    std::string pat;
+    std::vector<uint64_t> pat_off{0};
+    std::map<std::string, uint32_t> pat_idx;
     void add(const std::string& s) {
         utf8 += s;
         off.push_back(utf8.size());
         bnd_off.push_back(bnd.size());
+        span_off.push_back(spans.size());
+    }
+    // A span of the sentence about to be added; an empty pattern or "*" matches any feature.
+    void add_span(uint32_t start, uint32_t end, const std::string& pattern) {
+        uint32_t k = VBT_SPAN_ANY;
+        if (!pattern.empty() && pattern != "*") {
+            auto it = pat_idx.find(pattern);
+            if (it == pat_idx.end()) {
+                it = pat_idx.emplace(pattern, uint32_t(pat_off.size() - 1)).first;
+                pat += pattern;
+                pat_off.push_back(pat.size());
+            }
+            k = it->second;
+        }
+        spans.push_back(vbt_span{start, end, k});
     }
     void add(const std::string& s, const std::vector<uint32_t>& b) {
         bnd.insert(bnd.end(), b.begin(), b.end());
@@ -93,6 +143,11 @@ struct Packed {
         off.assign(1, 0);
         bnd_off.assign(1, 0);
         bnd.clear();
+        span_off.assign(1, 0);
+        spans.clear();
+        pat.clear();
+        pat_off.assign(1, 0);
+        pat_idx.clear();
     }
 };
 

@@ -23,6 +23,10 @@ static void usage() {
                  "         [--batch-lines N]           (lines per batch when stdin is not a terminal; default 65536)\n"
                  "         [--boundary-marker C]       (an ASCII byte other than newline: removed from every line, it\n"
                  "                                      marks a required token boundary where it stood)\n"
+                 "         [-p|--partial]              (MeCab's partial-analysis input: lines up to a line \"EOS\" form a\n"
+                 "                                      sentence; a line `surface\\tpattern` is one token of a feature\n"
+                 "                                      matching the pattern (\"*\" or nothing: any); every line starts\n"
+                 "                                      and ends a token; not with --boundary-marker)\n"
                  "         [-m|--marginal -t|--theta F] (marginal probabilities at temperature F > 0: -F may print\n"
                  "                                      each token's with %%pP; -O output is unchanged)\n"
                  "         [-a|--all-morphs]           (every lattice node in place of the tokens, like MeCab -a: -O and\n"
@@ -43,6 +47,7 @@ int main(int argc, char** argv) {
     std::string node_format, unk_format, bos_format, eos_format;
     bool has_node = false, has_unk = false, has_bos = false, has_eos = false;
     std::string marker;
+    bool partial = false;
     bool marginal = false, has_theta = false, all_morphs = false;
     double theta = 0;
     uint32_t n_sample = 0;  // --sample
@@ -79,6 +84,7 @@ int main(int argc, char** argv) {
         else if (a == "--bos-format") bos_format = next(), has_bos = true;
         else if (a == "--eos-format") eos_format = next(), has_eos = true;
         else if (a == "--boundary-marker") marker = next();
+        else if (a == "-p" || a == "--partial") partial = true;
         else if (a == "-m" || a == "--marginal") marginal = true;
         else if (a == "-a" || a == "--all-morphs") all_morphs = true;
         else if (a == "--sample" || a == "--seed") {
@@ -112,7 +118,7 @@ int main(int argc, char** argv) {
     if (batch_lines_arg == 0 || (has_node && format_on == "host") || (!has_node && (has_unk || has_bos || has_eos)) ||
         (marginal || sample) != has_theta || (all_morphs && format_on == "host") || (has_seed && !sample) ||
         (sample && (all_morphs || format_on == "host")) ||
-        (bounded && (marker.size() != 1 || marker[0] == '\n' || (marker[0] & 0x80)))) {
+        (bounded && (marker.size() != 1 || marker[0] == '\n' || (marker[0] & 0x80))) || (bounded && partial)) {
         usage();
         return 2;
     }
@@ -154,9 +160,12 @@ int main(int argc, char** argv) {
             if (pk.size() == 0) return;
             if (sample) tokenizer.sample_base(lines_done);
             lines_done += pk.size();
-            BatchResult r = bounded ? tokenizer.tokenize_batch(pk.utf8.data(), pk.off.data(), pk.size(), pk.bnd_off.data(),
-                                                               pk.bnd.data())
-                                    : tokenizer.tokenize_batch(pk.utf8.data(), pk.off.data(), pk.size());
+            BatchResult r = partial ? tokenizer.tokenize_batch(pk.utf8.data(), pk.off.data(), pk.size(), pk.bnd_off.data(),
+                                                               pk.bnd.data(), pk.span_off.data(), pk.spans.data(),
+                                                               pk.pat.data(), pk.pat_off.data(), pk.pat_off.size() - 1)
+                            : bounded ? tokenizer.tokenize_batch(pk.utf8.data(), pk.off.data(), pk.size(), pk.bnd_off.data(),
+                                                                 pk.bnd.data())
+                                      : tokenizer.tokenize_batch(pk.utf8.data(), pk.off.data(), pk.size());
             if (format_on == "device") {
                 std::string_view text = r.text();
                 std::fwrite(text.data(), 1, text.size(), stdout);
@@ -192,7 +201,26 @@ int main(int argc, char** argv) {
             }
             pk.clear();
         };
+        cli::PartialSentence ps;
+        uint64_t line_no = 0;
+        auto add_partial = [&]() {  // the sentence gathered so far, as one entry of the batch
+            for (const auto& t : ps.toks) pk.add_span(t.first.first, t.first.second, t.second);
+            pk.add(ps.text, ps.bnd);
+            ps.clear();
+            if (pk.size() >= batch_lines) flush_batch();
+        };
         while (cli::read_line(std::cin, line)) {
+            ++line_no;
+            if (partial) {
+                if (line == "EOS") {
+                    add_partial();
+                } else if (!ps.add_line(line)) {
+                    std::fprintf(stderr, "Error: line %llu: a required token line starts with a TAB (empty surface)\n",
+                                 (unsigned long long)line_no);
+                    return 1;
+                }
+                continue;
+            }
             if (bounded) {
                 const std::vector<uint32_t> bnd = cli::strip_boundary_markers(line, marker[0]);
                 pk.add(line, bnd);
@@ -201,6 +229,7 @@ int main(int argc, char** argv) {
             }
             if (pk.size() >= batch_lines) flush_batch();
         }
+        if (partial && ps.pending) add_partial();
         flush_batch();
         std::fwrite(out.data(), 1, out.size(), stdout);
         std::fflush(stdout);

@@ -343,6 +343,16 @@ class Tokenizer {
         check(vbt_tokenize_batch_bounded(handle(), utf8, byte_offsets, n_sent, bnd_offsets, bnd, &r));
         return BatchResult(r);
     }
+    // With required tokens (vbt_tokenize_batch_spans): sentence i's spans are spans[span_offsets[i] .. span_offsets[i+1]),
+    // pattern k the bytes patterns[pattern_offsets[k] .. pattern_offsets[k+1]); bnd_offsets / bnd may be null.
+    BatchResult tokenize_batch(const char* utf8, const uint64_t* byte_offsets, uint64_t n_sent, const uint64_t* bnd_offsets,
+                               const uint32_t* bnd, const uint64_t* span_offsets, const vbt_span* spans,
+                               const char* patterns, const uint64_t* pattern_offsets, uint64_t n_patterns) const {
+        vbt_result* r = nullptr;
+        check(vbt_tokenize_batch_spans(handle(), utf8, byte_offsets, n_sent, bnd_offsets, bnd, span_offsets, spans, patterns,
+                                       pattern_offsets, n_patterns, &r));
+        return BatchResult(r);
+    }
     // Device-resident batches (device addresses in, device addresses of the results out; see vibrato_b200.h).
     void tokenize_batch_device(uint64_t d_utf8, uint64_t d_byte_offsets, uint64_t n_sent, uint64_t n_bytes,
                                uint64_t& d_tok_offsets, uint64_t& d_tokens, uint64_t& n_tokens) const {
@@ -354,6 +364,15 @@ class Tokenizer {
                                uint64_t& d_tokens, uint64_t& n_tokens) const {
         check(vbt_tokenize_batch_device_bounded(handle(), d_utf8, d_byte_offsets, n_sent, n_bytes, d_bnd_offsets, d_bnd,
                                                 n_bnd, &d_tok_offsets, &d_tokens, &n_tokens));
+    }
+    // With required tokens: d_span_offsets / d_spans are device addresses, the patterns host memory.
+    void tokenize_batch_device(uint64_t d_utf8, uint64_t d_byte_offsets, uint64_t n_sent, uint64_t n_bytes,
+                               uint64_t d_bnd_offsets, uint64_t d_bnd, uint64_t n_bnd, uint64_t d_span_offsets,
+                               uint64_t d_spans, uint64_t n_spans, const char* patterns, const uint64_t* pattern_offsets,
+                               uint64_t n_patterns, uint64_t& d_tok_offsets, uint64_t& d_tokens, uint64_t& n_tokens) const {
+        check(vbt_tokenize_batch_device_spans(handle(), d_utf8, d_byte_offsets, n_sent, n_bytes, d_bnd_offsets, d_bnd, n_bnd,
+                                              d_span_offsets, d_spans, n_spans, patterns, pattern_offsets, n_patterns,
+                                              &d_tok_offsets, &d_tokens, &n_tokens));
     }
 
    private:
@@ -438,6 +457,9 @@ class Worker {  // worker.rs:13-74
         sent_.assign(s);
         bnd_.clear();
         bounded_ = false;
+        spans_.clear();
+        patterns_.clear();
+        pat_off_.assign(1, 0);
         toks_.clear();
         nodes_.clear();
         links_.clear();
@@ -450,13 +472,26 @@ class Worker {  // worker.rs:13-74
         bnd_ = std::move(boundaries);
         bounded_ = true;
     }
+    // With required tokens as well: spans (byte ranges into s) whose pattern indexes `patterns` or is VBT_SPAN_ANY.
+    void reset_sentence(std::string_view s, std::vector<uint32_t> boundaries, std::vector<vbt_span> spans,
+                        const std::vector<std::string>& patterns) {
+        reset_sentence(s, std::move(boundaries));
+        spans_ = std::move(spans);
+        for (const std::string& p : patterns) {
+            patterns_ += p;
+            pat_off_.push_back(patterns_.size());
+        }
+    }
     void tokenize() {
         samples_.assign(t_->samples_per_sentence(), {});
         if (sent_.empty()) return;  // worker.rs:50-52
         uint64_t off[2] = {0, sent_.size()};
         uint64_t boff[2] = {0, bnd_.size()};
-        BatchResult r = bounded_ ? t_->tokenize_batch(sent_.data(), off, 1, boff, bnd_.data())
-                                 : t_->tokenize_batch(sent_.data(), off, 1);
+        uint64_t soff[2] = {0, spans_.size()};
+        BatchResult r = !spans_.empty() ? t_->tokenize_batch(sent_.data(), off, 1, boff, bnd_.data(), soff, spans_.data(),
+                                                             patterns_.data(), pat_off_.data(), pat_off_.size() - 1)
+                        : bounded_      ? t_->tokenize_batch(sent_.data(), off, 1, boff, bnd_.data())
+                                        : t_->tokenize_batch(sent_.data(), off, 1);
         toks_.assign(r.tokens(), r.tokens() + r.n_tokens());
         probs_.clear();
         if (t_->has_marginals() && r.n_tokens()) probs_.assign(r.token_probs(), r.token_probs() + r.n_tokens());
@@ -491,6 +526,9 @@ class Worker {  // worker.rs:13-74
     std::string sent_;
     std::vector<uint32_t> bnd_;
     bool bounded_ = false;
+    std::vector<vbt_span> spans_;
+    std::string patterns_;
+    std::vector<uint64_t> pat_off_{0};
     std::vector<vbt_token> toks_;
     std::vector<float> probs_;
     std::vector<vbt_token> nodes_;  // Tokenizer::lattice

@@ -443,7 +443,110 @@ int32_t vbt_tokenize_batch_bounded(vbt_tokenizer* t, const char* utf8, const uin
         if (bnd_offsets[n_sent] > bnd_offsets[0]) need(bnd, "bnd");
         for (uint64_t i = 0; i < n_sent; ++i)
             if (byte_offsets[i] > byte_offsets[i + 1]) throw vbt::Error(vbt::kInvalidArgument, "byte_offsets must be non-decreasing");
-        const vbt::Bounds b{bnd_offsets, bnd, bnd_offsets[n_sent]};  // the boundary lists are checked on the device
+        const vbt::Bounds b{bnd_offsets, bnd, bnd_offsets[n_sent], {}};  // the boundary lists are checked on the device
+        vbt::HostResult* r = t->e->run_host(utf8, byte_offsets, n_sent, &b);
+        *out = new vbt_result{t->e, r};
+    });
+}
+
+namespace {
+// The pattern table of vbt_tokenize_batch_spans (engine.hpp Spans): each pattern split like a feature (csv_fields in
+// kernels.cu), every field that is not exactly "*" kept as {field index, first byte, length}.
+struct SpanPatterns {
+    std::vector<uint32_t> off{0}, pf;
+    std::vector<uint8_t> bytes;
+
+    SpanPatterns(const char* patterns, const uint64_t* pattern_offsets, uint64_t n) {
+        if (n >= VBT_SPAN_ANY) throw vbt::Error(vbt::kInvalidArgument, "too many patterns");
+        if (n) need(pattern_offsets, "pattern_offsets");
+        for (uint64_t k = 0; k < n; ++k) {
+            if (pattern_offsets[k + 1] < pattern_offsets[k])
+                throw vbt::Error(vbt::kInvalidArgument, "pattern_offsets must be non-decreasing");
+            const uint64_t len = pattern_offsets[k + 1] - pattern_offsets[k];
+            if (len) need(patterns, "patterns");
+            if (len) add(k, reinterpret_cast<const uint8_t*>(patterns) + pattern_offsets[k], len);
+            off.push_back(uint32_t(pf.size() / 3));
+        }
+    }
+
+   private:
+    void add(uint64_t k, const uint8_t* p, uint64_t n) {
+        uint32_t field = 0, kept = 0;
+        uint64_t start = 0;
+        std::string cur;
+        auto close = [&] {
+            if (cur == "*") return;
+            auto fail = [&](const char* why) {
+                throw vbt::Error(vbt::kInvalidArgument, "pattern " + std::to_string(k) + ", byte " + std::to_string(start) +
+                                                            ": " + why);
+            };
+            if (field > vbt::kFmtMaxFieldIndex) fail("field index above 255");
+            if (kept == vbt::kFmtMaxFields) fail("more than 16 constrained fields");
+            ++kept;
+            pf.insert(pf.end(), {field, uint32_t(bytes.size()), uint32_t(cur.size())});
+            bytes.insert(bytes.end(), cur.begin(), cur.end());
+        };
+        bool quoted = false, at_start = true;
+        for (uint64_t i = 0; i < n; ++i) {  // csv_fields of kernels.cu
+            const uint8_t c = p[i];
+            if (quoted) {
+                if (c != '"') {
+                    cur.push_back(char(c));
+                } else if (i + 1 < n && p[i + 1] == '"') {
+                    cur.push_back(char(c));
+                    ++i;
+                } else {
+                    quoted = false;
+                }
+            } else if (c == '"' && at_start) {
+                quoted = true;
+            } else if (c == ',') {
+                close();
+                ++field;
+                cur.clear();
+                start = i + 1;
+                at_start = true;
+                continue;
+            } else {
+                cur.push_back(char(c));
+            }
+            at_start = false;
+        }
+        close();
+    }
+
+   public:
+    void fill(vbt::Spans& s) const {
+        s.pat_off = off.data();
+        s.pf = pf.data();
+        s.pat_bytes = bytes.data();
+        s.n_pat = uint32_t(off.size() - 1);
+        s.n_pat_bytes = bytes.size();
+    }
+};
+}  // namespace
+
+int32_t vbt_tokenize_batch_spans(vbt_tokenizer* t, const char* utf8, const uint64_t* byte_offsets, uint64_t n_sent,
+                                 const uint64_t* bnd_offsets, const uint32_t* bnd, const uint64_t* span_offsets,
+                                 const vbt_span* spans, const char* patterns, const uint64_t* pattern_offsets,
+                                 uint64_t n_patterns, vbt_result** out) {
+    return guarded([&] {
+        need(t, "t");
+        need(out, "out");
+        need(byte_offsets, "byte_offsets");
+        need(span_offsets, "span_offsets");
+        if (n_sent && byte_offsets[n_sent] > byte_offsets[0]) need(utf8, "utf8");
+        if (bnd_offsets && bnd_offsets[n_sent] > bnd_offsets[0]) need(bnd, "bnd");
+        if (span_offsets[n_sent] > span_offsets[0]) need(spans, "spans");
+        for (uint64_t i = 0; i < n_sent; ++i)
+            if (byte_offsets[i] > byte_offsets[i + 1]) throw vbt::Error(vbt::kInvalidArgument, "byte_offsets must be non-decreasing");
+        const SpanPatterns pat(patterns, pattern_offsets, n_patterns);
+        vbt::Bounds b;  // the lists themselves are checked on the device
+        if (bnd_offsets) b = vbt::Bounds{bnd_offsets, bnd, bnd_offsets[n_sent], {}};
+        b.spans.off = span_offsets;
+        b.spans.rec = reinterpret_cast<const uint32_t*>(spans);
+        b.spans.n = span_offsets[n_sent];
+        pat.fill(b.spans);
         vbt::HostResult* r = t->e->run_host(utf8, byte_offsets, n_sent, &b);
         *out = new vbt_result{t->e, r};
     });
@@ -528,7 +631,32 @@ int32_t vbt_tokenize_batch_device_bounded(vbt_tokenizer* t, uint64_t d_utf8, uin
         need(n_tokens, "n_tokens");
         if (!d_bnd_offsets) throw vbt::Error(vbt::kInvalidArgument, "d_bnd_offsets is null");
         if (n_bnd && !d_bnd) throw vbt::Error(vbt::kInvalidArgument, "d_bnd is null");
-        const vbt::Bounds b{reinterpret_cast<const uint64_t*>(d_bnd_offsets), reinterpret_cast<const uint32_t*>(d_bnd), n_bnd};
+        const vbt::Bounds b{reinterpret_cast<const uint64_t*>(d_bnd_offsets), reinterpret_cast<const uint32_t*>(d_bnd), n_bnd, {}};
+        t->e->run_device(d_utf8, d_byte_offsets, n_sent, n_bytes, d_tok_offsets, d_tokens, n_tokens, &b);
+    });
+}
+
+int32_t vbt_tokenize_batch_device_spans(vbt_tokenizer* t, uint64_t d_utf8, uint64_t d_byte_offsets, uint64_t n_sent,
+                                        uint64_t n_bytes, uint64_t d_bnd_offsets, uint64_t d_bnd, uint64_t n_bnd,
+                                        uint64_t d_span_offsets, uint64_t d_spans, uint64_t n_spans, const char* patterns,
+                                        const uint64_t* pattern_offsets, uint64_t n_patterns, uint64_t* d_tok_offsets,
+                                        uint64_t* d_tokens, uint64_t* n_tokens) {
+    return guarded([&] {
+        need(t, "t");
+        need(d_tok_offsets, "d_tok_offsets");
+        need(d_tokens, "d_tokens");
+        need(n_tokens, "n_tokens");
+        if (n_bnd && !d_bnd) throw vbt::Error(vbt::kInvalidArgument, "d_bnd is null");
+        if (!d_span_offsets) throw vbt::Error(vbt::kInvalidArgument, "d_span_offsets is null");
+        if (n_spans && !d_spans) throw vbt::Error(vbt::kInvalidArgument, "d_spans is null");
+        const SpanPatterns pat(patterns, pattern_offsets, n_patterns);
+        vbt::Bounds b;
+        if (d_bnd_offsets)
+            b = vbt::Bounds{reinterpret_cast<const uint64_t*>(d_bnd_offsets), reinterpret_cast<const uint32_t*>(d_bnd), n_bnd, {}};
+        b.spans.off = reinterpret_cast<const uint64_t*>(d_span_offsets);
+        b.spans.rec = reinterpret_cast<const uint32_t*>(d_spans);
+        b.spans.n = n_spans;
+        pat.fill(b.spans);
         t->e->run_device(d_utf8, d_byte_offsets, n_sent, n_bytes, d_tok_offsets, d_tokens, n_tokens, &b);
     });
 }

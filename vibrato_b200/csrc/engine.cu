@@ -147,6 +147,7 @@ struct Workspace {  // every per-(chunk of a)-batch device array; two of them le
     DevBuf n_slots, slot_off, eos, n_tok, code_sys, code_usr, cinfo, groupable, byte_pos, info, info_ex, ends_cnt,
         ends_meta, seg, ends_hot, ends_cold, scan_tmp, stats, iota, sort_keys, order, tiles;
     DevBuf bnd_dist;  // bounded batches only: Batch::bnd_dist
+    DevBuf span_tag;  // span batches only: SpanArgs::tag
     DevBuf m_fill, m_ncand, m_cand_entry, m_R, m_ab, m_r_eos, m_a_eos;  // marginals only: MargArgs
     DevBuf l_row_base, l_n_nodes;  // lattice output only: LatticeArgs
     DevBuf m_lw, s_cnt, s_total;   // sampling only: MargArgs::lw, SampleArgs::cnt / total
@@ -154,7 +155,7 @@ struct Workspace {  // every per-(chunk of a)-batch device array; two of them le
     void release() {
         for (DevBuf* b : {&n_slots, &slot_off, &eos, &n_tok, &code_sys, &code_usr, &cinfo, &groupable, &byte_pos, &info,
                           &info_ex, &ends_cnt, &ends_meta, &seg, &ends_hot, &ends_cold, &scan_tmp, &stats, &iota,
-                          &sort_keys, &order, &tiles, &bnd_dist, &m_fill, &m_ncand, &m_cand_entry, &m_R, &m_ab, &m_r_eos, &m_a_eos,
+                          &sort_keys, &order, &tiles, &bnd_dist, &span_tag, &m_fill, &m_ncand, &m_cand_entry, &m_R, &m_ab, &m_r_eos, &m_a_eos,
                           &l_row_base, &l_n_nodes, &m_lw, &s_cnt, &s_total})
             b->release();
     }
@@ -162,10 +163,19 @@ struct Workspace {  // every per-(chunk of a)-batch device array; two of them le
 
 // The required boundaries of a batch (or chunk) in device memory: bnd_off[n_sent + 1] into bnd[n]; off == nullptr
 // for an unbounded batch.
+// A span batch also has the span records (span_off[n_sent + 1] into span_rec[n_spans]) and the compiled pattern table
+// (shared by every chunk); its off is never nullptr (all zero without explicit boundaries).
 struct DevBounds {
     const unsigned long long* off = nullptr;
     const uint32_t* bnd = nullptr;
     uint64_t n = 0;
+    const unsigned long long* span_off = nullptr;
+    const uint3* span_rec = nullptr;
+    uint64_t n_spans = 0;
+    const uint32_t* pat_off = nullptr;
+    const uint3* pf = nullptr;
+    const uint8_t* pat_bytes = nullptr;
+    uint32_t n_pat = 0;
 };
 
 struct OutSlot {  // where one (chunk of a) batch leaves its results; two of them alternate in chunked runs
@@ -341,7 +351,9 @@ class EngineImpl final : public Engine {
         cudaStreamDestroy(out_stream_);
         base_.release();
         for (DevBuf* b : {&fmt_prog_, &ft_keep_, &ft_off_, &ft_bytes_}) b->release();
-        for (auto* b : {&blob_own_, &in_utf8_, &in_off_, &in_bnd_off_, &in_bnd_, &connid_, &connid_try_}) b->release();
+        for (auto* b : {&blob_own_, &in_utf8_, &in_off_, &in_bnd_off_, &in_bnd_, &in_span_off_, &in_span_, &in_pat_, &connid_,
+                        &connid_try_})
+            b->release();
         for (auto& w : ws_) w.release();
         ws_small_.release();
         small_in_.release();
@@ -540,9 +552,26 @@ class EngineImpl final : public Engine {
         CK(cudaSetDevice(device_));
         check_size(n_sent, n_bytes);
         check_bounded(bnd);
-        if (bnd && bnd->n == 0 && device_offsets_zero(bnd->off, n_sent)) bnd = nullptr;  // no boundary at all
+        Bounds nb;
+        if (bnd) {  // no boundary and no span at all: the unbounded kernels
+            nb = *bnd;
+            if (nb.spans.off && nb.spans.n == 0 && device_offsets_zero(nb.spans.off, n_sent)) nb.spans = Spans{};
+            if (nb.off && nb.n == 0 && device_offsets_zero(nb.off, n_sent)) nb.off = nullptr;
+            bnd = (nb.off || nb.spans.off) ? &nb : nullptr;
+        }
         DevBounds bd;
-        if (bnd) bd = DevBounds{reinterpret_cast<const unsigned long long*>(bnd->off), bnd->bnd, bnd->n};
+        if (bnd) {
+            if (bnd->off)
+                bd = DevBounds{reinterpret_cast<const unsigned long long*>(bnd->off), bnd->bnd, bnd->n};
+            else
+                bd.off = zero_offsets(uint32_t(n_sent), stream_);
+            if (bnd->spans.off) {
+                bd.span_off = reinterpret_cast<const unsigned long long*>(bnd->spans.off);
+                bd.span_rec = reinterpret_cast<const uint3*>(bnd->spans.rec);
+                bd.n_spans = bnd->spans.n;
+                upload_patterns(bnd->spans, bd, stream_);
+            }
+        }
         made_ = Outputs{};
         run_whole(reinterpret_cast<const uint8_t*>(d_utf8), reinterpret_cast<const unsigned long long*>(d_byte_off),
                   uint32_t(n_sent), n_bytes, bd);
@@ -561,7 +590,8 @@ class EngineImpl final : public Engine {
         const uint64_t n_bytes = n_sent64 ? byte_off[n_sent64] - first : 0;
         check_size(n_sent64, n_bytes);
         check_bounded(bnd);
-        if (bnd && host_lists_empty(*bnd, n_sent64)) bnd = nullptr;  // no boundary at all: the unbounded kernels
+        Bounds nb;
+        bnd = drop_empty(bnd, n_sent64, nb);  // no boundary and no span at all: the unbounded kernels
         const uint32_t n_sent = uint32_t(n_sent64);
         in_utf8_.ensure(n_bytes + 16, 1.25);
         in_off_.ensure((size_t(n_sent) + 1) * 8, 1.25);
@@ -582,7 +612,7 @@ class EngineImpl final : public Engine {
         // k_small_batch computes no marginals, no lattice and no samples: with any on, small batches take the usual route
         if (small_batch_ && n_sent <= small_batch_ && !chunked && n_bytes <= kEagerBytes && !counting_ && !connid_on_ && theta_ == 0 && !lattice_ &&
             !samp_n_ &&
-            (!bnd || small_bounds_fit(*bnd, n_sent))) {
+            (!bnd || (!bnd->spans.off && small_bounds_fit(*bnd, n_sent)))) {  // k_small_batch has no span rules
             if (HostResult* r = run_small(utf8 + first, off, n_sent, n_bytes, bnd)) return r;
             // the batch outgrew the scratch of k_small_batch: it runs again on the route below
         }
@@ -641,7 +671,7 @@ class EngineImpl final : public Engine {
             ws_[1].stream = aux_stream_;
             const uint32_t n_ws = dual_stream_ ? 2 : 1;
             for (uint32_t i = 0; i < n_ws; ++i)
-                ensure_workspace(ws_[i], max_chunk_sent, max_chunk_bytes, bd.off != nullptr);  // sized once: no cudaMalloc in the pipeline
+                ensure_workspace(ws_[i], max_chunk_sent, max_chunk_bytes, bd.off != nullptr, bd.span_off != nullptr);  // sized once: no cudaMalloc in the pipeline
             for (auto& o : out_) ensure_out(o, ws_[0], max_chunk_sent, max_chunk_bytes);
             // output stage: each slot's text buffer holds the text a chunk is expected to produce (at most 4 bytes per
             // sentence plus the learned ratio per input byte); a chunk with more text flags itself and the batch is
@@ -674,7 +704,7 @@ class EngineImpl final : public Engine {
             double text_need = 0;  // text bytes per input byte beyond per_sent per sentence, largest over the sound chunks
             uint32_t route = kRouteNone;
             bool overflow = false, bad_utf8 = false, bad_offsets = false, slots_overflow = false, text_overflow = false;
-            bool bad_bounds = false;
+            bool bad_bounds = false, bad_spans = false;
             uint64_t slots_seen = 0;
             batch_total_bytes_ = n_bytes;
             std::vector<cudaEvent_t>& h2d_ev = h2d_events(n_chunks);
@@ -697,6 +727,7 @@ class EngineImpl final : public Engine {
                 if (o.h_ctrl->flags & kFlagUtf8Error) bad_utf8 = true;
                 if (o.h_ctrl->flags & kFlagBadOffsets) bad_offsets = true;
                 if (o.h_ctrl->flags & kFlagBadBoundary) bad_bounds = true;
+                if (o.h_ctrl->flags & kFlagBadSpan) bad_spans = true;
                 if (o.h_ctrl->flags & kFlagPoolOverflow) overflow = true;
                 if (o.h_ctrl->flags & kFlagSlotsOverflow) overflow = slots_overflow = true;
                 if (o.h_ctrl->flags & kFlagTextOverflow) text_overflow = true;
@@ -716,7 +747,7 @@ class EngineImpl final : public Engine {
                 if (fmt && !(o.h_ctrl->flags & (kFlagsStandDown | kFlagUtf8Error | kFlagPoolOverflow)))
                     text_need = std::max(text_need, (double(count[kGroupText]) - double(per_sent) * (s1 - s0)) /
                                                         double(std::max<uint64_t>(1, off[s1] - off[s0])));
-                if (!overflow && !text_overflow && !bad_utf8 && !bad_offsets && !bad_bounds) {
+                if (!overflow && !text_overflow && !bad_utf8 && !bad_offsets && !bad_bounds && !bad_spans) {
                     // offsets are global already (base_); a record array that is short grows (rare), keeping what it
                     // holds once the copies into it have landed
                     for (int a = 0; a < kNumArrays; ++a) {
@@ -743,6 +774,7 @@ class EngineImpl final : public Engine {
                 if (c >= 2) CK(cudaStreamWaitEvent(w.stream, o.drained, 0));  // slot reused: its D2H must be done
                 DevBounds cb = bd;  // the chunk's slice of the boundary offsets (they index the whole bnd array)
                 if (cb.off) cb.off += s0;
+                if (cb.span_off) cb.span_off += s0;
                 enqueue(w, d_utf8, d_off + s0, s1 - s0, off[s1] - off[s0], o, base_.as<unsigned long long>(),
                         c >= 1 ? base_ready_[(c - 1) & 1] : nullptr, base_ready_[c & 1], cb, s0);
                 if (!utf8_pinned && c + 1 < n_chunks) issue_h2d(c + 1);
@@ -764,6 +796,10 @@ class EngineImpl final : public Engine {
             if (bad_bounds) {
                 release(r);
                 throw Error(kInvalidArgument, kBadBoundsMsg);
+            }
+            if (bad_spans) {
+                release(r);
+                throw Error(kInvalidArgument, kBadSpansMsg);
             }
             if (overflow || text_overflow) {
                 release(r);
@@ -797,7 +833,8 @@ class EngineImpl final : public Engine {
         const uint64_t n_bytes = n_sent64 ? byte_off[n_sent64] - first : 0;
         check_size(n_sent64, n_bytes);
         check_bounded(bnd);
-        if (bnd && host_lists_empty(*bnd, n_sent64)) bnd = nullptr;
+        Bounds nb;
+        bnd = drop_empty(bnd, n_sent64, nb);
         const uint32_t n_sent = uint32_t(n_sent64);
         const DevBounds bd = bnd ? upload_bounds(*bnd, n_sent, stream_) : DevBounds{};
         in_utf8_.ensure(n_bytes + 16, 1.25);
@@ -909,6 +946,12 @@ class EngineImpl final : public Engine {
         "required boundaries must be non-decreasing, at most the sentence's byte length and on a UTF-8 lead byte, "
         "and their offsets non-decreasing and within the boundary array";
 
+    static constexpr const char* kBadSpansMsg =
+        "required tokens (spans) must have start < end <= the sentence's byte length, both on a UTF-8 lead byte or at the "
+        "end, be sorted and non-overlapping, name VBT_SPAN_ANY or a pattern of the call, hold no explicit boundary "
+        "inside, not start at a space when ignore_space is on, and their offsets must be non-decreasing and within the "
+        "span array";
+
     void check_bounded(const Bounds* bnd) const {
         if (bnd && counting_)
             throw Error(kInvalidArgument, "the \"counting\" hook measures the unconstrained lattice: it refuses bounded batches");
@@ -916,10 +959,38 @@ class EngineImpl final : public Engine {
 
     // A batch whose boundary lists are all empty (every offset the same) runs the unbounded kernels.  Broken offsets
     // are not empty: they take the bounded route, which reports them after the errors that take precedence.
-    static bool host_lists_empty(const Bounds& hb, uint64_t n_sent) {
+    static bool host_lists_empty(const uint64_t* off, uint64_t n_sent) {
         for (uint64_t i = 0; i < n_sent; ++i)
-            if (hb.off[i + 1] != hb.off[0]) return false;
+            if (off[i + 1] != off[0]) return false;
         return true;
+    }
+    // bnd without its empty boundary or span lists (in nb), or nullptr when both are empty.
+    static const Bounds* drop_empty(const Bounds* bnd, uint64_t n_sent, Bounds& nb) {
+        if (!bnd) return nullptr;
+        nb = *bnd;
+        if (nb.spans.off && host_lists_empty(nb.spans.off, n_sent)) nb.spans = Spans{};
+        if (nb.off && host_lists_empty(nb.off, n_sent)) nb.off = nullptr;
+        return (nb.off || nb.spans.off) ? &nb : nullptr;
+    }
+    // n_sent + 1 zero offsets on the device (in_bnd_off_): a span batch without explicit boundaries.
+    const unsigned long long* zero_offsets(uint32_t n_sent, cudaStream_t st) {
+        in_bnd_off_.ensure((size_t(n_sent) + 1) * 8, 1.25);
+        CK(cudaMemsetAsync(in_bnd_off_.p, 0, (size_t(n_sent) + 1) * 8, st));
+        return in_bnd_off_.as<unsigned long long>();
+    }
+    // The compiled patterns of s (host) -> one device block [pat_off | pf | bytes] (in_pat_).
+    void upload_patterns(const Spans& s, DevBounds& d, cudaStream_t st) {
+        const size_t n_off = size_t(s.n_pat) + 1, n_pf = s.pat_off[s.n_pat];
+        const size_t at_pf = (n_off * 4 + 15) & ~size_t(15), at_bytes = at_pf + n_pf * 12;
+        in_pat_.ensure(at_bytes + s.n_pat_bytes + 16, 1.25);
+        uint8_t* p = in_pat_.as<uint8_t>();
+        h2d(p, s.pat_off, n_off * 4, st, false);
+        if (n_pf) h2d(p + at_pf, s.pf, n_pf * 12, st, false);
+        if (s.n_pat_bytes) h2d(p + at_bytes, s.pat_bytes, s.n_pat_bytes, st, false);
+        d.pat_off = reinterpret_cast<const uint32_t*>(p);
+        d.pf = reinterpret_cast<const uint3*>(p + at_pf);
+        d.pat_bytes = p + at_bytes;
+        d.n_pat = s.n_pat;
     }
     // The same for device-resident lists with n_bnd == 0: valid offsets are then all 0 (one copy of them to the host).
     bool device_offsets_zero(const uint64_t* d_off, uint64_t n_sent) {
@@ -940,16 +1011,33 @@ class EngineImpl final : public Engine {
     // bnd[off[0] .. off[n_sent]).  A list whose window is inverted or leaves bnd ships no boundaries and keeps
     // offsets that k_mark_bounds refuses (some sentence's end offset then lies below its start or beyond 0).
     DevBounds upload_bounds(const Bounds& hb, uint32_t n_sent, cudaStream_t st) {
-        const uint64_t first = hb.off[0], last = hb.off[n_sent];
-        const bool sound = first <= last && last <= hb.n;
+        DevBounds d = hb.off ? upload_list(hb.off, hb.bnd, hb.n, n_sent, st) : DevBounds{zero_offsets(n_sent, st)};
+        if (hb.spans.off) {  // the same for the span records (12 bytes each) into in_span_off_ / in_span_
+            const DevBounds s = upload_list(hb.spans.off, hb.spans.rec, hb.spans.n, n_sent, st, 12);
+            d.span_off = s.off;
+            d.span_rec = reinterpret_cast<const uint3*>(s.bnd);
+            d.n_spans = s.n;
+            upload_patterns(hb.spans, d, st);
+        }
+        return d;
+    }
+    DevBounds upload_list(const uint64_t* hoff, const void* hrec, uint64_t hn, uint32_t n_sent, cudaStream_t st,
+                          size_t rec_bytes = 4) {
+        const bool spans = rec_bytes != 4;
+        std::vector<uint64_t>& rebased = spans ? span_rebased_ : bnd_rebased_;
+        DevBuf& d_off = spans ? in_span_off_ : in_bnd_off_;
+        DevBuf& d_rec = spans ? in_span_ : in_bnd_;
+        const uint64_t first = hoff[0], last = hoff[n_sent];
+        const bool sound = first <= last && last <= hn;
         const uint64_t lo = sound ? first : 0, n = sound ? last - first : 0;
-        bnd_rebased_.resize(size_t(n_sent) + 1);
-        for (uint32_t i = 0; i <= n_sent; ++i) bnd_rebased_[i] = hb.off[i] - lo;  // wraps for a broken list: refused
-        in_bnd_off_.ensure((size_t(n_sent) + 1) * 8, 1.25);
-        in_bnd_.ensure(n * 4 + 4, 1.25);
-        h2d(in_bnd_off_.p, bnd_rebased_.data(), (size_t(n_sent) + 1) * 8, st, false);
-        if (n) h2d(in_bnd_.p, hb.bnd + lo, n * 4, st, is_pinned(hb.bnd + lo));
-        return DevBounds{in_bnd_off_.as<unsigned long long>(), in_bnd_.as<uint32_t>(), n};
+        rebased.resize(size_t(n_sent) + 1);
+        for (uint32_t i = 0; i <= n_sent; ++i) rebased[i] = hoff[i] - lo;  // wraps for a broken list: refused
+        d_off.ensure((size_t(n_sent) + 1) * 8, 1.25);
+        d_rec.ensure(n * rec_bytes + 16, 1.25);
+        h2d(d_off.p, rebased.data(), (size_t(n_sent) + 1) * 8, st, false);
+        const uint8_t* src = static_cast<const uint8_t*>(hrec) + lo * rec_bytes;
+        if (n) h2d(d_rec.p, src, n * rec_bytes, st, is_pinned(src));
+        return DevBounds{d_off.as<unsigned long long>(), d_rec.as<uint32_t>(), n};
     }
 
     std::vector<cudaEvent_t>& h2d_events(uint32_t n) {
@@ -1359,7 +1447,7 @@ class EngineImpl final : public Engine {
 
     // Sizes every workspace array for batches of up to n_sent sentences / n_bytes bytes (upper
     // bounds: characters <= bytes, one sentinel slot per sentence).
-    void ensure_workspace(Workspace& w, uint32_t n_sent, uint64_t n_bytes, bool bounded) {
+    void ensure_workspace(Workspace& w, uint32_t n_sent, uint64_t n_bytes, bool bounded, bool spans = false) {
         const size_t ns = size_t(n_sent) + 1;
         w.n_slots.ensure(ns * 4, 1.25);
         w.slot_off.ensure(ns * 4, 1.25);
@@ -1382,6 +1470,7 @@ class EngineImpl final : public Engine {
         w.ends_cnt.ensure(ms * 4, 1.25);
         w.ends_meta.ensure(ms * 8, 1.25);
         if (bounded) w.bnd_dist.ensure(ms * 4, 1.25);
+        if (spans) w.span_tag.ensure(ms * 8, 1.25);
         const bool fwd = theta_ > 0 || samp_n_;  // the forward pass runs
         if (fwd) {
             w.m_fill.ensure(ms * 4, 1.25);
@@ -1435,7 +1524,7 @@ class EngineImpl final : public Engine {
         ws_[0].stream = stream_;
         batch_total_bytes_ = n_bytes;
         for (int attempt = 0;; ++attempt) {
-            ensure_workspace(ws_[0], n_sent, n_bytes, bd.off != nullptr);
+            ensure_workspace(ws_[0], n_sent, n_bytes, bd.off != nullptr, bd.span_off != nullptr);
             ensure_out(o, ws_[0], n_sent, n_bytes);
             connid_begin(stream_);
             enqueue(ws_[0], d_utf8, d_off, n_sent, n_bytes, o, nullptr, nullptr, nullptr, bd, sent_base);
@@ -1446,6 +1535,7 @@ class EngineImpl final : public Engine {
             if (o.h_ctrl->flags & kFlagUtf8Error)
                 throw Error(kUtf8, "stream did not contain valid UTF-8");  // what `stdin.lines()` reports
             if (o.h_ctrl->flags & kFlagBadBoundary) throw Error(kInvalidArgument, kBadBoundsMsg);
+            if (o.h_ctrl->flags & kFlagBadSpan) throw Error(kInvalidArgument, kBadSpansMsg);
             if (o.h_ctrl->flags & kFlagSlotsOverflow) {  // more characters per byte than any batch before: hard bound
                 if (attempt >= 3) throw Error(kInternal, "slot overflow persists");
                 chars_per_byte_ = 1.0;
@@ -1537,6 +1627,11 @@ class EngineImpl final : public Engine {
             b.n_bnd = bd.n;
             b.bnd_dist = w.bnd_dist.as<uint32_t>();
         }
+        SpanArgs sp{};
+        if (bd.span_off) {
+            sp = SpanArgs{bd.span_off, bd.span_rec, bd.n_spans, bd.pat_off, bd.pf, bd.pat_bytes, bd.n_pat, dv_.space_mask,
+                          w.span_tag.as<uint2>()};
+        }
 
         o.launches = 0;
         const TileScan ts{w.tiles.as<unsigned long long>(), dc->tickets};
@@ -1566,12 +1661,15 @@ class EngineImpl final : public Engine {
                                                          st));
             ++o.launches;
         }
-        if (b.bnd_dist && n_sent) {  // the bounded batch's boundaries, booked with the decode stage
-            launch_mark_bounds(b, st);
+        if (b.bnd_dist && n_sent) {  // the bounded batch's boundaries (and spans), booked with the decode stage
+            if (sp.off)
+                launch_mark_spans(b, sp, st);
+            else
+                launch_mark_bounds(b, st);
             ++o.launches;
         }
         CK(cudaEventRecord(o.ev[3], st));
-        launch_candidates(dv_, b, max_slots, st);
+        launch_candidates(dv_, b, max_slots, st, sp.off ? &sp : nullptr);
         if (counting_) {
             launch_candidate_stats(dv_, b, max_slots, w.stats.as<uint4>(), st);
             ++o.launches;
@@ -1695,7 +1793,8 @@ class EngineImpl final : public Engine {
     const uint8_t* blob_ = nullptr;
     DevBuf blob_own_, in_utf8_, in_off_, connid_, connid_try_;
     DevBuf in_bnd_off_, in_bnd_;           // boundary lists of a bounded host batch (upload_bounds)
-    std::vector<uint64_t> bnd_rebased_;
+    DevBuf in_span_off_, in_span_, in_pat_;  // span lists of a host batch, and any span batch's compiled patterns
+    std::vector<uint64_t> bnd_rebased_, span_rebased_;
     uint64_t* bnd_stage_ = nullptr;  // pinned: device-resident boundary offsets checked for emptiness
     size_t bnd_stage_cap_ = 0;
     bool connid_on_ = false;

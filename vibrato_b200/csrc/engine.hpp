@@ -128,13 +128,28 @@ class ResultPool {
     std::vector<HostResult*> free_;
 };
 
+// Required tokens of a batch (vbt_tokenize_batch_spans): sentence i's spans are rec[off[i] .. off[i+1]), three words
+// {start_byte, end_byte, pattern} each, in host or device memory like the boundaries they travel with; the compiled
+// patterns (kernels.cuh SpanArgs) are always in host memory: pat_off[n_pat + 1] into pf, whose fields index pat_bytes.
+struct Spans {
+    const uint64_t* off = nullptr;  // n_sent + 1; nullptr = no spans
+    const uint32_t* rec = nullptr;
+    uint64_t n = 0;
+    const uint32_t* pat_off = nullptr;
+    const uint32_t* pf = nullptr;  // 3 words per field: {field index, first byte, length}
+    const uint8_t* pat_bytes = nullptr;
+    uint32_t n_pat = 0;
+    uint64_t n_pat_bytes = 0;
+};
 // Required token boundaries of a batch (vbt_tokenize_batch_bounded): sentence i's boundaries are the
 // sentence-relative byte offsets bnd[off[i] .. off[i+1]), and bnd holds n entries.  Host or device addresses, as the
 // call that takes them says.  A null pointer to Bounds = an unbounded batch.
+// With spans, off may be nullptr (no explicit boundary) and the batch is still bounded: the span ends are boundaries.
 struct Bounds {
     const uint64_t* off = nullptr;  // n_sent + 1
     const uint32_t* bnd = nullptr;
     uint64_t n = 0;
+    Spans spans;
 };
 
 constexpr int kNumStages = 9;

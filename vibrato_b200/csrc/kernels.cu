@@ -619,9 +619,120 @@ __device__ __forceinline__ void store_info(const Batch& b, uint32_t slot, uint32
     if (special) b.info_ex[slot] = make_uint2(w.skip, w.flags);
 }
 
+template <class Out>
+__device__ __forceinline__ uint32_t csv_fields(const uint8_t* __restrict__ p, uint32_t n, Out out);
+
+// Required tokens: does the feature of word `id` of lexicon `lex` (0 system, 1 user, 2 unknown entries) match
+// pattern p?  Each constrained field (SpanArgs::pf, ascending field index) must equal its bytes; a field past the
+// feature's last one does not match (it reads as '*', which no constrained field is).
+__device__ __forceinline__ bool span_match(const DictView& d, const SpanArgs& sp, uint32_t lex, uint32_t id, uint32_t p) {
+    if (p == kSpanAny) return true;
+    const uint32_t k1 = sp.pat_off[p + 1];
+    uint32_t k = sp.pat_off[p], pos = 0;
+    if (k == k1) return true;
+    const uint32_t a = d.feat_off[lex][id];
+    uint3 c = sp.pf[k];
+    bool ok = true;
+    const uint32_t nf = csv_fields(d.feat[lex] + a, d.feat_off[lex][id + 1] - a, [&](uint32_t field, uint8_t ch) {
+        while (k < k1 && c.x < field) {  // the constrained field before this one is complete
+            ok &= pos == c.z;
+            if (++k < k1) c = sp.pf[k];
+            pos = 0;
+        }
+        if (k < k1 && c.x == field) {
+            ok &= pos < c.z && sp.pat_bytes[c.y + pos] == ch;
+            ++pos;
+        }
+    });
+    for (; k < k1; pos = 0) {
+        ok &= c.x < nf && pos == c.z;
+        if (++k < k1) c = sp.pf[k];
+    }
+    return ok;
+}
+
+// The postings of the one key of a lexicon that spans [sw, end) exactly, filtered by pattern p: every maximal run of
+// matching records is one segment (its index one before the run's first record, as SegOut::push continues a list).
+__device__ __forceinline__ uint32_t span_postings(const DictView& d, const SpanArgs& sp, const uint4* __restrict__ nodes,
+                                                  uint32_t num_nodes, const uint4* __restrict__ post,
+                                                  const uint32_t* __restrict__ codes, uint32_t sw, uint32_t end,
+                                                  uint32_t p, uint32_t lex_flag, SegOut& so) {
+    if (num_nodes == 0) return 0;
+    uint32_t node = 0, nbase = __ldg(&nodes[0].x), hit = kNone, plen = 0;
+    for (uint32_t q = sw; q < end; ++q) {  // walk_lexicon, to `end` only
+        const uint32_t code = codes[q];
+        if (code == kInvalidCode || (nbase & kFlag)) return 0;
+        const uint32_t child = nbase ^ code;
+        if (child >= num_nodes) return 0;
+        const uint4 nd = __ldg(&nodes[child]);
+        if ((nd.y & kMask) != node) return 0;
+        node = child;
+        nbase = nd.x;
+        hit = nd.z;
+        plen = nd.w;
+    }
+    if (hit == kNone) return 0;
+    uint32_t count = 0;
+    for (uint32_t j = 0; j < plen;) {
+        uint32_t j1 = j;
+        while (j1 < plen) {
+            const uint32_t widx = __ldg(&post[hit + 1 + j1]).z;
+            if (!span_match(d, sp, widx >> 30, widx & 0x3FFFFFFFu, p)) break;
+            ++j1;
+        }
+        so.push((hit + j) | lex_flag, end, j1 - j);
+        count += j1 - j;
+        j = j1 + 1;
+    }
+    return count;
+}
+
+// Candidates of a start position whose word starts a span (tag = {length in characters, pattern}): the user, then
+// the system lexicon's words of exactly the span's surface that match the pattern; without any, one unknown word
+// over the whole span per unk.def entry of the start character's category that matches (all of them when none does).
+__device__ __forceinline__ uint32_t count_span(const DictView& d, const Batch& b, const SpanArgs& sp, const StartWord& w,
+                                               uint2 tag, SegOut& so) {
+    const uint32_t end = w.sw + tag.x;
+    uint32_t cnt = 0;
+    if (d.usr_table) cnt = span_postings(d, sp, d.usr_nodes, d.usr_num_nodes, d.usr_post, b.code_usr, w.sw, end, tag.y, kSegUser, so);
+    cnt += span_postings(d, sp, d.sys_nodes, d.sys_num_nodes, d.sys_post, b.code_sys, w.sw, end, tag.y, 0, so);
+    if (cnt) return cnt;
+    const uint32_t e0 = __ldg(&d.unk_off[ci_base(w.ci)]), e1 = __ldg(&d.unk_off[ci_base(w.ci) + 1]);
+    bool all = true;
+    for (uint32_t e = e0; all && e < e1; ++e) all = !span_match(d, sp, 2, e, tag.y);
+    for (uint32_t e = e0; e < e1;) {
+        uint32_t e2 = e;
+        while (e2 < e1 && (all || span_match(d, sp, 2, e2, tag.y))) ++e2;
+        so.push(kSegUnk | e, end, e2 - e);
+        cnt += e2 - e;
+        e = e2 + 1;
+    }
+    return cnt;
+}
+
+// start_word of a span batch: a position strictly inside a span gets no candidates (no node ends there, so the
+// reference's loop skips it); *tag receives the span tag of the word's start.  A space skip that lands strictly inside
+// a span (the skipped run continues into it through a category the space shares) would start a word there: the batch
+// is refused (kFlagBadSpan).
+__device__ __forceinline__ StartWord start_word_spans(const DictView& d, const Batch& b, const SpanArgs& sp, uint32_t slot,
+                                                      uint32_t g0, uint2* tag) {
+    *tag = make_uint2(0, 0);
+    const StartWord none{slot, 0, 0, 0, 0, false, 0};
+    if (g0 != 0 && sp.tag[slot].x == kSpanInside) return none;
+    const StartWord w = start_word<true>(d, b, slot, g0);
+    if (w.active) *tag = sp.tag[w.sw];
+    if (tag->x == kSpanInside) {
+        atomicOr(b.flags, kFlagBadSpan);
+        *tag = make_uint2(0, 0);
+        return none;
+    }
+    return w;
+}
+
 // BND: the bounded instantiation (required boundaries in b.bnd_dist); the unbounded one is the code as it was.
-template <bool BND>
-__global__ void __launch_bounds__(256) k_candidates(DictView d, Batch b) {
+// SPAN (k_candidates_spans, BND too): the span rules of count_span / start_word_spans on top.
+template <bool BND, bool SPAN>
+__device__ __forceinline__ void candidates_body(const DictView& d, const Batch& b, const SpanArgs& sp) {
     const uint32_t slot = blockIdx.x * blockDim.x + threadIdx.x;
     const uint32_t lane = threadIdx.x & 31;
     // A rejected batch (see stand_down) leaves every thread out of range.  The flag word is read next to the slot
@@ -632,12 +743,13 @@ __global__ void __launch_bounds__(256) k_candidates(DictView d, Batch b) {
     if (slot == 0 && total_slots > b.launch_slots) atomicOr(b.flags, kFlagSlotsOverflow);
     const bool in_range = slot < total_slots && !(batch_flags & kFlagBadOffsets);
     uint32_t g0 = in_range ? b.groupable[slot] : 0;
-    const StartWord sw = start_word<BND>(d, b, slot, g0);
+    uint2 tag = make_uint2(0, 0);
+    const StartWord sw = SPAN ? start_word_spans(d, b, sp, slot, g0, &tag) : start_word<BND>(d, b, slot, g0);
     const bool active = sw.active;
     uint32_t cnt = 0;
     __shared__ uint2 s_segs[kMaxSegs][256];
     SegOut so{&s_segs[0][threadIdx.x], 256, kMaxSegs, 0, slot, nullptr};
-    if (active) cnt = count_candidates<BND>(d, b, sw, so);
+    if (active) cnt = (SPAN && tag.x) ? count_span(d, b, sp, sw, tag, so) : count_candidates<BND>(d, b, sw, so);
     const uint32_t nseg = so.n;
     // Block-aggregated allocation from the segment pool: a scan inside each warp, the eight warp totals through
     // shared memory, ONE atomicAdd per block.  (One atomic per warp was 1.3 M same-address atomics per batch, and
@@ -692,8 +804,20 @@ __global__ void __launch_bounds__(256) k_candidates(DictView d, Batch b) {
         }
     } else {  // more segments than the buffer holds: walk again, straight into the pool
         SegOut out{b.seg + ptr, 1, nseg, 0, slot, b.ends_cnt};
-        count_candidates<BND>(d, b, sw, out);
+        if (SPAN && tag.x)
+            count_span(d, b, sp, sw, tag, out);
+        else
+            count_candidates<BND>(d, b, sw, out);
     }
+}
+
+template <bool BND>
+__global__ void __launch_bounds__(256) k_candidates(DictView d, Batch b) {
+    candidates_body<BND, false>(d, b, SpanArgs{});
+}
+
+__global__ void __launch_bounds__(256) k_candidates_spans(DictView d, Batch b, SpanArgs sp) {
+    candidates_body<true, true>(d, b, sp);
 }
 
 // Required boundaries of sentence s -> bnd_dist, in two passes of the warp.  (1) One lane per boundary: a boundary b
@@ -703,7 +827,12 @@ __global__ void __launch_bounds__(256) k_candidates(DictView d, Batch b) {
 // the same sentence.
 // Validates the list on the way: offsets in order and inside bnd, values non-decreasing, <= len and on a UTF-8 lead
 // byte; anything else raises kFlagBadBoundary.  A boundary at 0 or len marks nothing: every token already ends there.
-__device__ __forceinline__ void mark_bounds_one(const Batch& b, uint32_t s, uint32_t lane) {
+// `extra(mark, base, n, bo, len)` runs between the two passes, once the boundaries are marked (mark_spans_one).
+struct NoMarks {
+    __device__ void operator()(uint32_t*, uint32_t, uint32_t, unsigned long long, unsigned long long) const {}
+};
+template <class Extra = NoMarks>
+__device__ __forceinline__ void mark_bounds_one(const Batch& b, uint32_t s, uint32_t lane, Extra extra = {}) {
     const unsigned long long j0 = b.bnd_off[s], j1 = b.bnd_off[s + 1];
     const bool listed = !(j1 < j0 || j1 > b.n_bnd);
     const unsigned long long bo = b.byte_off[s], len = b.byte_off[s + 1] - bo;
@@ -730,6 +859,7 @@ __device__ __forceinline__ void mark_bounds_one(const Batch& b, uint32_t s, uint
         mark[lo] = 1;
     }
     if (__any_sync(kFull, bad) && lane == 0) atomicOr(b.flags, kFlagBadBoundary);
+    extra(mark, base, n, bo, len);
     __syncwarp();
     uint32_t next = n;  // the first marked position right of the chunks done so far
     for (int k = int((n + 31) / 32) - 1; k >= 0; --k) {
@@ -751,6 +881,85 @@ __global__ void __launch_bounds__(256) k_mark_bounds(Batch b) {
         const uint32_t s = w * VBT_SENT_PER_WARP + r;
         if (s >= b.n_sent) return;
         mark_bounds_one(b, s, lane);
+    }
+}
+
+// Required tokens of sentence s, between the passes of mark_bounds_one: one lane per span marks its start and end
+// as boundaries and tags its start; then the warp tags the interiors in one left-to-right pass over 32-character
+// chunks (a prefix max of the span ends started so far), so a long span costs no lane more than its share.  Validates the list (offsets in order and inside sp.rec; start < end <= len,
+// both on UTF-8 lead bytes or at len; no overlap with the span before; a known pattern; no explicit boundary strictly
+// inside; with ignore_space no start at a SPACE character) and raises kFlagBadSpan otherwise.  An invalid span marks
+// nothing.
+__device__ __forceinline__ void mark_spans_one(const Batch& b, const SpanArgs& sp, uint32_t s, uint32_t lane) {
+    mark_bounds_one(b, s, lane, [&](uint32_t* mark, uint32_t base, uint32_t n, unsigned long long bo, unsigned long long len) {
+        uint2* tag = sp.tag + base;
+        for (uint32_t i = lane; i <= n; i += 32) tag[i] = make_uint2(0, 0);
+        __syncwarp();
+        const unsigned long long j0 = sp.off[s], j1 = sp.off[s + 1];
+        const bool listed = !(j1 < j0 || j1 > sp.n);
+        bool bad = !listed;
+        auto slot_of = [&](uint32_t v) {  // the character that starts at byte v (n for v == len)
+            uint32_t lo = 0, hi = n;
+            while (lo < hi) {
+                const uint32_t mid = (lo + hi) >> 1;
+                if (b.byte_pos[base + mid] < v)
+                    lo = mid + 1;
+                else
+                    hi = mid;
+            }
+            return lo;
+        };
+        for (unsigned long long j = j0 + lane; listed && j < j1; j += 32) {
+            const uint3 r = sp.rec[j];
+            if (r.x >= r.y || r.y > len || (b.utf8[bo + r.x] & 0xC0) == 0x80 ||
+                (r.y < len && (b.utf8[bo + r.y] & 0xC0) == 0x80) || (j > j0 && sp.rec[j - 1].y > r.x) ||
+                (r.z != kSpanAny && r.z >= sp.n_pat)) {
+                bad = true;
+                continue;
+            }
+            const uint32_t ca = slot_of(r.x), cb = slot_of(r.y);
+            if (ci_cate(b.cinfo[base + ca]) & sp.space_mask) {  // the space skip would move the word's start past it
+                bad = true;
+                continue;
+            }
+            tag[ca] = make_uint2(cb - ca, r.z);
+            if (ca > 0) mark[ca] = 1;
+            if (cb < n) mark[cb] = 1;
+        }
+        __syncwarp();
+        // Interiors: c is inside a span when a span started before c ends after it.  The spans of a valid list are
+        // disjoint, so a mark found there is an explicit boundary, not another span's end.
+        uint32_t open_end = 0;  // the largest span end started in the chunks done so far
+        for (uint32_t c0 = 0; c0 < n; c0 += 32) {
+            const uint32_t c = c0 + lane;
+            const uint32_t len_c = c < n ? tag[c].x : 0u;
+            uint32_t e = len_c ? c + len_c : 0u;
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const uint32_t v = __shfl_up_sync(kFull, e, o);
+                if (lane >= uint32_t(o)) e = max(e, v);
+            }
+            const uint32_t before = __shfl_up_sync(kFull, e, 1);
+            const uint32_t reach = max(open_end, lane ? before : 0u);
+            if (c < n && !len_c && reach > c) {
+                if (mark[c]) bad = true;  // an explicit boundary inside the span
+                tag[c] = make_uint2(kSpanInside, 0);
+            }
+            open_end = max(open_end, __shfl_sync(kFull, e, 31));
+        }
+        if (__any_sync(kFull, bad) && lane == 0) atomicOr(b.flags, kFlagBadSpan);
+    });
+}
+
+__global__ void __launch_bounds__(256) k_mark_spans(Batch b, SpanArgs sp) {
+    if (stand_down(*b.flags)) return;
+    const uint32_t w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const uint32_t lane = threadIdx.x & 31;
+#pragma unroll 1
+    for (uint32_t r = 0; r < VBT_SENT_PER_WARP; ++r) {
+        const uint32_t s = w * VBT_SENT_PER_WARP + r;
+        if (s >= b.n_sent) return;
+        mark_spans_one(b, sp, s, lane);
     }
 }
 
@@ -2796,10 +3005,18 @@ void launch_mark_bounds(const Batch& b, cudaStream_t st) {
     k_mark_bounds<<<blocks, 256, 0, st>>>(b);
 }
 
-void launch_candidates(const DictView& d, const Batch& b, uint32_t max_slots, cudaStream_t st) {
+void launch_mark_spans(const Batch& b, const SpanArgs& sp, cudaStream_t st) {
+    if (!b.n_sent) return;
+    uint32_t blocks = (b.n_sent + 8 * VBT_SENT_PER_WARP - 1) / (8 * VBT_SENT_PER_WARP);
+    k_mark_spans<<<blocks, 256, 0, st>>>(b, sp);
+}
+
+void launch_candidates(const DictView& d, const Batch& b, uint32_t max_slots, cudaStream_t st, const SpanArgs* sp) {
     if (!max_slots) return;
     uint32_t blocks = (max_slots + 255) / 256;
-    if (b.bnd_dist)
+    if (sp)
+        k_candidates_spans<<<blocks, 256, 0, st>>>(d, b, *sp);
+    else if (b.bnd_dist)
         k_candidates<true><<<blocks, 256, 0, st>>>(d, b);
     else
         k_candidates<false><<<blocks, 256, 0, st>>>(d, b);

@@ -70,6 +70,10 @@ enum : uint32_t {
     // a required boundary list is out of order, past its sentence's end or inside a multi-byte character, or the
     // boundary offsets themselves are out of order or past n_bnd (k_mark_bounds)
     kFlagBadBoundary = 64u,
+    // a required token list is out of order, overlapping, empty-spanned, past its sentence's end, off a UTF-8 lead
+    // byte, names no pattern, holds an explicit boundary or (ignore_space) starts at a space, or its offsets are out of
+    // order or past n (k_mark_spans)
+    kFlagBadSpan = 128u,
 };
 constexpr uint32_t kFlagsStandDown = kFlagBadOffsets | kFlagSlotsOverflow;
 constexpr uint32_t kPruneMaxChars = 16000;  // (chars + 1) nodes x 65 535 per node < 2^30
@@ -201,8 +205,34 @@ void launch_front(const DictView& d, const Batch& b, const TileScan& ts, cudaStr
 // Bounded batches (b.bnd_dist != nullptr): writes bnd_dist from the boundary lists after launch_front and
 // validates them (kFlagBadBoundary).
 void launch_mark_bounds(const Batch& b, cudaStream_t st);
+// Required tokens (vbt_tokenize_batch_spans): sentence s's spans are the records rec[off[s] .. off[s+1]), each
+// {start byte, end byte, pattern} relative to the sentence, the pattern VBT_SPAN_ANY (kSpanAny) or an index into the
+// compiled pattern table.  Pattern p constrains the fields pf[pat_off[p] .. pat_off[p+1]), each {feature field index,
+// first byte in pat_bytes, byte length}, sorted by field index: a word matches when each of those fields of its
+// feature (csv_fields) equals the bytes.  Passed to k_mark_spans and k_candidates_spans as a separate argument, so
+// the Batch of every other kernel stays as it was.  A span batch is a bounded batch (b.bnd_dist, b.bnd_off set).
+constexpr uint32_t kSpanAny = 0xFFFFFFFFu;
+constexpr uint32_t kSpanInside = 0xFFFFFFFFu;  // SpanArgs::tag[slot].x of a position strictly inside a span
+struct SpanArgs {
+    const unsigned long long* off;  // n_sent + 1
+    const uint3* rec;
+    unsigned long long n;           // records behind rec: no offset may exceed it
+    const uint32_t* pat_off;        // n_pat + 1
+    const uint3* pf;
+    const uint8_t* pat_bytes;
+    uint32_t n_pat;
+    uint32_t space_mask;            // DictView::space_mask: a span may not start at a skipped space
+    // per slot, written by k_mark_spans: {0, 0} outside spans, {kSpanInside, 0} strictly inside one, {end - start in
+    // characters, pattern} at a span's start
+    uint2* tag;
+};
+// Span batches: marks the boundary lists and the span ends into bnd_dist, writes sp.tag and validates both
+// (kFlagBadBoundary, kFlagBadSpan); in place of launch_mark_bounds.
+void launch_mark_spans(const Batch& b, const SpanArgs& sp, cudaStream_t st);
 // b.bnd_dist != nullptr selects the bounded instantiation of k_candidates: no candidate crosses a marked boundary.
-void launch_candidates(const DictView& d, const Batch& b, uint32_t max_slots, cudaStream_t st);
+// sp != nullptr (a span batch) selects k_candidates_spans: the bounded candidates, none strictly inside a span, and at
+// a span's start only the words of the span's surface that match its pattern (or its unknown words).
+void launch_candidates(const DictView& d, const Batch& b, uint32_t max_slots, cudaStream_t st, const SpanArgs* sp = nullptr);
 // Counted runs only: per-slot {M | walks << 24, T, P, W} of SURVEY.md §8(d), summed by K3 over visited positions.
 void launch_candidate_stats(const DictView& d, const Batch& b, uint32_t max_slots, uint4* stats, cudaStream_t st);
 // lanes_per_sentence in {4, 8, 16, 32}: how many lanes of a warp cooperate on one sentence.

@@ -218,6 +218,8 @@ class MultiEngine final : public Engine {
         pinned_free(h_off_);
         pinned_free(h_bnd_off_);
         pinned_free(h_bnd_);
+        pinned_free(h_span_off_);
+        pinned_free(h_span_);
         cudaSetDevice(dev_[0]);
         for (DevBuf& b : gather_) b.release();
     }
@@ -278,12 +280,26 @@ class MultiEngine final : public Engine {
         // validated on the devices)
         Bounds hb;
         if (bnd) {
-            grow_pinned(h_bnd_off_, h_bnd_off_cap_, (n_sent + 1) * 8);
-            grow_pinned(h_bnd_, h_bnd_cap_, bnd->n * 4 + 4);
-            CK(cudaMemcpyAsync(h_bnd_off_, bnd->off, (n_sent + 1) * 8, cudaMemcpyDeviceToHost, stream_[0]));
-            if (bnd->n) CK(cudaMemcpyAsync(h_bnd_, bnd->bnd, bnd->n * 4, cudaMemcpyDeviceToHost, stream_[0]));
+            hb.spans = bnd->spans;  // the patterns are host memory already
+            if (bnd->off) {
+                grow_pinned(h_bnd_off_, h_bnd_off_cap_, (n_sent + 1) * 8);
+                grow_pinned(h_bnd_, h_bnd_cap_, bnd->n * 4 + 4);
+                CK(cudaMemcpyAsync(h_bnd_off_, bnd->off, (n_sent + 1) * 8, cudaMemcpyDeviceToHost, stream_[0]));
+                if (bnd->n) CK(cudaMemcpyAsync(h_bnd_, bnd->bnd, bnd->n * 4, cudaMemcpyDeviceToHost, stream_[0]));
+                hb.off = static_cast<const uint64_t*>(h_bnd_off_);
+                hb.bnd = static_cast<const uint32_t*>(h_bnd_);
+                hb.n = bnd->n;
+            }
+            if (bnd->spans.off) {
+                grow_pinned(h_span_off_, h_span_off_cap_, (n_sent + 1) * 8);
+                grow_pinned(h_span_, h_span_cap_, bnd->spans.n * 12 + 12);
+                CK(cudaMemcpyAsync(h_span_off_, bnd->spans.off, (n_sent + 1) * 8, cudaMemcpyDeviceToHost, stream_[0]));
+                if (bnd->spans.n)
+                    CK(cudaMemcpyAsync(h_span_, bnd->spans.rec, bnd->spans.n * 12, cudaMemcpyDeviceToHost, stream_[0]));
+                hb.spans.off = static_cast<const uint64_t*>(h_span_off_);
+                hb.spans.rec = static_cast<const uint32_t*>(h_span_);
+            }
             CK(cudaStreamSynchronize(stream_[0]));
-            hb = Bounds{static_cast<const uint64_t*>(h_bnd_off_), static_cast<const uint32_t*>(h_bnd_), bnd->n};
         }
         const std::vector<uint64_t> cut = split_by_bytes(h_off_, n_sent, n);
         std::vector<Totals> count(n);
@@ -468,7 +484,11 @@ class MultiEngine final : public Engine {
 
     // The boundary lists of the shard that starts at sentence `first` (host memory): its slice of the offsets.
     static Bounds shard_bounds(const Bounds* bnd, uint64_t first) {
-        return bnd ? Bounds{bnd->off + first, bnd->bnd, bnd->n} : Bounds{};
+        if (!bnd) return Bounds{};
+        Bounds sb = *bnd;
+        if (sb.off) sb.off += first;
+        if (sb.spans.off) sb.spans.off += first;
+        return sb;
     }
 
     // One host thread per device (the calling thread takes the first): each call blocks on its own device.
@@ -540,6 +560,9 @@ class MultiEngine final : public Engine {
     void* h_bnd_off_ = nullptr;  // pinned: the boundary lists of a device-resident batch, cut into shards on the host
     void* h_bnd_ = nullptr;
     size_t h_bnd_off_cap_ = 0, h_bnd_cap_ = 0;
+    void* h_span_off_ = nullptr;  // pinned: the span lists of a device-resident batch, likewise
+    void* h_span_ = nullptr;
+    size_t h_span_off_cap_ = 0, h_span_cap_ = 0;
     DevBuf gather_[kNumArrays];  // the outputs of a gathered device-resident batch, on the first device
     Outputs made_;               // the arrays the last device-resident call produced
     Totals made_total_{};
