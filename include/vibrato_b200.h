@@ -395,8 +395,8 @@ int32_t vbt_result_marginals(const vbt_result *r, const float **token_prob, cons
 int32_t vbt_last_device_marginals(const vbt_tokenizer *t, uint64_t *d_token_prob, uint64_t *d_path_prob);
 /* Lattice output, the option "lattice" of vbt_tokenizer_set_option: 0 off (default); 1 every result also carries
  * every node of each sentence's lattice; 2 the same, and the output text ("output_mode" 1-3 or a format) renders the
- * nodes in place of the tokens, like MeCab's -a (BOS / EOS formats still print once per sentence).  Single-device
- * tokenizers only (a multi-device one refuses it with VBT_ERR_UNSUPPORTED).
+ * nodes in place of the tokens, like MeCab's -a (BOS / EOS formats still print once per sentence).  Multi-device
+ * tokenizers give the bytes of one device.
  *   Nodes: the entries of the reference's Lattice::ends once build_lattice has finished, without BOS and EOS; exactly
  *   the nodes the tokenizer inserts (ignore_space, max_grouping_len, the user lexicon and required boundaries
  *   included), dead ends and nodes ending inside a trailing space run included.  An empty sentence has none.
@@ -407,7 +407,23 @@ int32_t vbt_last_device_marginals(const vbt_tokenizer *t, uint64_t *d_token_prob
  *   With marginals on, node_prob[k] is the node's marginal (vbt_tokenizer_set_marginals); on the best path it equals
  *   token_prob bit for bit.
  * While on, batches take three more kernel launches and a scan (booked under "viterbi"), "small_batch" steps aside,
- * and with 2 a format may not print the "prev" directives %M %pS %pn %pC %pL (setting either order fails). */
+ * and with 2 a format may not print the "prev" directives %M %pS %pn %pC %pL (setting either order fails).
+ *
+ * Near-best lattice, the option "lattice_margin" = D (0 <= D <= 2^62; -1 = off, the default; it changes nothing while
+ * "lattice" is 0).  Edges and exact int64 path costs are those of the marginals.  For a node n, F(n) is the least cost
+ * of a path from BOS to n (the edge into n included), G(n) the least cost from n to EOS (the edges after n; undefined
+ * without such a path), best the least cost of the sentence, and margin(n) = F(n) + G(n) - best >= 0 (0 on every
+ * minimum-cost path).  The lattice group then keeps:
+ *   Nodes: every node with a path to EOS and margin(n) <= D, and every node flagged VBT_NODE_BEST (where the
+ *   tokenizer's i32 costs wrap, a best-path node can have margin > 0: it is kept, so the guarantee above holds).  An
+ *   empty sentence, or one without a path, keeps none.  Without i32 wrap the kept set is the union of the nodes of
+ *   every BOS -> EOS path of cost <= best + D; with D = 2^62 it is every node that has a path to EOS.
+ *   Order and record: as above, restricted to the kept nodes.
+ *   Link: prev is the index, in the kept list, of the node the full lattice's link names; -1 for BOS, -2 when that
+ *   node was not kept (only where i32 costs wrap or a row holds more than 65 536 entries).  flags as above.
+ *   node_margin[k]: the node's exact margin (vbt_result_lattice_margins).  node_prob is unchanged in meaning.
+ * Margins are integers: the kept set is the same on every route, chunk size, sentence order and device count.  With the
+ * margin on, batches take two or three more kernel launches (booked under "viterbi"). */
 /* node_offsets[n_sent + 1] into nodes / links / node_prob (NULL without marginals) of a result made with the lattice;
  * owned by the result.  VBT_ERR_INVALID_ARGUMENT for a result made without it. */
 int32_t vbt_result_lattice(const vbt_result *r, const uint64_t **node_offsets, const vbt_token **nodes,
@@ -416,6 +432,12 @@ int32_t vbt_result_lattice(const vbt_result *r, const uint64_t **node_offsets, c
  * marginals), valid until the next call; VBT_ERR_INVALID_ARGUMENT when it ran without the lattice. */
 int32_t vbt_last_device_lattice(const vbt_tokenizer *t, uint64_t *d_node_offsets, uint64_t *d_nodes, uint64_t *d_links,
                                 uint64_t *d_node_prob, uint64_t *n_nodes);
+/* node_margin[n_nodes] (int64, indexed like nodes) of a result made with the lattice and "lattice_margin" >= 0; owned by
+ * the result.  VBT_ERR_INVALID_ARGUMENT for a result made without them. */
+int32_t vbt_result_lattice_margins(const vbt_result *r, const int64_t **node_margin);
+/* Device address of the node margins of the last vbt_tokenize_batch_device* call, valid until the next call;
+ * VBT_ERR_INVALID_ARGUMENT when it ran without the lattice or without "lattice_margin". */
+int32_t vbt_last_device_lattice_margins(const vbt_tokenizer *t, uint64_t *d_node_margin);
 /* Segmentation sampling ("subword regularisation"): n paths per sentence drawn independently, with replacement, from
  * P(path) = exp(-theta * cost(path)) / Z over the lattice, edges and exact int64 path costs of the marginals above.
  * Forward-filtering backward-sampling on the device: a walk starts at EOS and repeats until BOS.  At the current

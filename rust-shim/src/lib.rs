@@ -71,6 +71,7 @@ extern "C" {
     fn vbt_result_marginals(r: *const vbt_result, token_prob: *mut *const f32, path_prob: *mut *const f32) -> i32;
     fn vbt_result_lattice(r: *const vbt_result, node_offsets: *mut *const u64, nodes: *mut *const vbt_token,
                           links: *mut *const vbt_lattice_link, node_prob: *mut *const f32, n_nodes: *mut u64) -> i32;
+    fn vbt_result_lattice_margins(r: *const vbt_result, node_margin: *mut *const i64) -> i32;
     fn vbt_evaluate(d: *const vbt_dict, t: *mut vbt_tokenizer, corpus: *const c_char, len: usize,
                     feature_indices: *const u64, n_indices: usize, num_ref: *mut u64, num_sys: *mut u64,
                     num_cor: *mut u64) -> i32;
@@ -273,6 +274,12 @@ impl Tokenizer {
         let v = if !on { 0 } else if text { 2 } else { 1 };
         check(unsafe { vbt_tokenizer_set_option(self.handle(), b"lattice\0".as_ptr() as *const c_char, v) })
     }
+    /// Near-best lattice (option "lattice_margin"): `Some(d)` (0..=2^62) keeps only the nodes of paths whose cost is
+    /// within `d` of the best one, plus the best path, and adds `BatchResult::lattice_margins`; `None` keeps every node.
+    pub fn lattice_margin(&self, d: Option<i64>) -> Result<()> {
+        let opt = b"lattice_margin\0".as_ptr() as *const c_char;
+        check(unsafe { vbt_tokenizer_set_option(self.handle(), opt, d.unwrap_or(-1)) })
+    }
     /// Segmentation sampling (see `vbt_tokenizer_set_sampling`): `n` (1..1024, 0 = off) paths per sentence drawn from
     /// P(path) at temperature `theta`, keyed by `seed`; batches tokenised afterwards carry `BatchResult::samples`.
     /// `text`: the output text renders each sentence's `n` samples in place of its best path (option "sample_text").
@@ -387,6 +394,14 @@ impl BatchResult {
             let probs = if p.is_null() { None } else if n == 0 { Some(&[][..]) } else { Some(std::slice::from_raw_parts(p, n)) };
             Ok((std::slice::from_raw_parts(o, ns as usize + 1), nodes, links, probs))
         }
+    }
+    /// The exact cost margin of every node of `lattice()`; an error for a batch tokenised without the lattice or without
+    /// `Tokenizer::lattice_margin`.
+    pub fn lattice_margins(&self) -> Result<&[i64]> {
+        let mut m = std::ptr::null();
+        check(unsafe { vbt_result_lattice_margins(self.r, &mut m) })?;
+        let n = self.lattice()?.1.len();
+        Ok(if n == 0 { &[] } else { unsafe { std::slice::from_raw_parts(m, n) } })
     }
     /// (sample offsets, sampled tokens): sample j of sentence i is `samples[offsets[i * n + j]..offsets[i * n + j + 1]]`;
     /// an error for a batch tokenised without sampling.

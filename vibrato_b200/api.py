@@ -280,12 +280,14 @@ class BatchResult:
     and `path_probs` (float32[n_sent]) hold the marginal of every token and the probability of each sentence's best
     path; both are None otherwise.  With Tokenizer.lattice() on, `node_offsets[i]..node_offsets[i+1]` index `nodes`
     (TOKEN_DTYPE), `node_links` (LINK_DTYPE) and `node_probs` (float32, None without marginals): every node of sentence
-    i's lattice (include/vibrato_b200.h); all four are None otherwise.  With Tokenizer.sampling(n, theta) on,
+    i's lattice (include/vibrato_b200.h); all four are None otherwise.  With Tokenizer.lattice(margin=D), the nodes are
+    the near-best ones and `node_margins` (int64) holds each one's exact cost margin; None otherwise.  With
+    Tokenizer.sampling(n, theta) on,
     `sample_offsets[i * n + j]..sample_offsets[i * n + j + 1]` index `samples` (TOKEN_DTYPE): sample j of sentence i
     (sentence_samples()); both are None otherwise."""
 
     def __init__(self, tokenizer, handle, sentences_utf8, byte_offsets, compact=False, marginals=False, lattice=False,
-                 samples=0):
+                 samples=0, margins=False):
         self._tok = tokenizer
         self._h = handle
         self._free = lib().vbt_result_free
@@ -311,7 +313,7 @@ class BatchResult:
                                 else np.empty(0, dtype=np.float32))
             self.path_probs = (np.ctypeslib.as_array(C.cast(pp, f32), shape=(self.n_sent,)) if self.n_sent
                                else np.empty(0, dtype=np.float32))
-        self.node_offsets = self.nodes = self.node_links = self.node_probs = None
+        self.node_offsets = self.nodes = self.node_links = self.node_probs = self.node_margins = None
         if lattice:
             po, pn, pl, pp, nn = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_uint64()
             check(lib().vbt_result_lattice(handle, C.byref(po), C.byref(pn), C.byref(pl), C.byref(pp), C.byref(nn)))
@@ -325,6 +327,11 @@ class BatchResult:
             if pp.value:
                 self.node_probs = (np.ctypeslib.as_array(C.cast(pp, C.POINTER(C.c_float)), shape=(n,)) if n
                                    else np.empty(0, dtype=np.float32))
+            if margins:
+                pm = C.c_void_p()
+                check(lib().vbt_result_lattice_margins(handle, C.byref(pm)))
+                self.node_margins = (np.ctypeslib.as_array(C.cast(pm, C.POINTER(C.c_int64)), shape=(n,)) if n
+                                     else np.empty(0, dtype=np.int64))
         self.n_samples = int(samples)  # samples per sentence, 0 without sampling
         self.sample_offsets = self.samples = None
         if samples:
@@ -348,7 +355,7 @@ class BatchResult:
             if self.token_probs is not None:
                 self.token_probs = self.token_probs.copy()
                 self.path_probs = self.path_probs.copy()
-            for name in ("node_offsets", "nodes", "node_links", "node_probs", "sample_offsets", "samples"):
+            for name in ("node_offsets", "nodes", "node_links", "node_probs", "node_margins", "sample_offsets", "samples"):
                 if getattr(self, name) is not None:
                     setattr(self, name, getattr(self, name).copy())
             self._free(h)
@@ -400,8 +407,9 @@ class BatchResult:
             raise VibratoError(1, "no lattice: switch it on with Tokenizer.lattice() before tokenising")
         s = bytes(self._utf8[int(self._off[i]):int(self._off[i + 1])])
         a, b = int(self.node_offsets[i]), int(self.node_offsets[i + 1])
-        npb = self.node_probs
-        return [LatticeNode(self._tok, s, self.nodes[k], self.node_links[k], None if npb is None else float(npb[k]))
+        npb, nm = self.node_probs, self.node_margins
+        return [LatticeNode(self._tok, s, self.nodes[k], self.node_links[k], None if npb is None else float(npb[k]),
+                            None if nm is None else int(nm[k]))
                 for k in range(a, b)]
 
 
@@ -422,6 +430,7 @@ class Tokenizer:
         self._format = None  # (node, unk, bos, eos) of output_format(), replayed after the options
         self._theta = 0.0  # marginals(), replayed before the format
         self._lattice = 0  # lattice(), replayed before the format
+        self._lattice_margin = -1  # lattice(margin=D), replayed with it
         self._sampling = (0, 0.0, 0)  # sampling() as (n, theta, seed), replayed after the marginals
         self._sample_text = False  # sampling(text=True), replayed after sampling
         self._stream = 0
@@ -487,6 +496,8 @@ class Tokenizer:
                 check(lib().vbt_tokenizer_set_marginals(h, self._theta))
             if self._lattice:
                 check(lib().vbt_tokenizer_set_option(h, b"lattice", self._lattice))
+            if self._lattice_margin >= 0:
+                check(lib().vbt_tokenizer_set_option(h, b"lattice_margin", self._lattice_margin))
             if self._sampling[0]:
                 check(lib().vbt_tokenizer_set_sampling(h, *self._sampling))
             if self._sample_text:
@@ -593,7 +604,8 @@ class Tokenizer:
                                                    byte_offsets.ctypes.data, n, bnd_offsets.ctypes.data,
                                                    bnd.ctypes.data if bnd.size else None, C.byref(h)))
         return BatchResult(self, h, utf8, byte_offsets, compact=bool(self._options.get("compact_tokens", 0)),
-                           marginals=self._theta > 0, lattice=self._lattice > 0, samples=self._sampling[0])
+                           marginals=self._theta > 0, lattice=self._lattice > 0, samples=self._sampling[0],
+                           margins=self._lattice > 0 and self._lattice_margin >= 0)
 
     def tokenize_batch_device(self, d_utf8, d_byte_offsets, n_sent, n_bytes, d_bnd_offsets=None, d_bnd=None, n_bnd=0,
                               d_span_offsets=None, d_spans=None, n_spans=0, patterns=None):
@@ -631,6 +643,13 @@ class Tokenizer:
         v = [C.c_uint64() for _ in range(5)]
         check(lib().vbt_last_device_lattice(self.handle(), *[C.byref(x) for x in v]))
         return tuple(x.value for x in v)
+
+    def last_device_lattice_margins(self):
+        """-> d_node_margins: device address (int64[n_nodes]) of the node margins of the last tokenize_batch_device
+        call made with lattice(margin=D), valid until the next call."""
+        v = C.c_uint64()
+        check(lib().vbt_last_device_lattice_margins(self.handle(), C.byref(v)))
+        return v.value
 
     def last_device_samples(self):
         """-> (d_sample_offsets, d_samples, n_sample_tokens): device addresses (uint64[n_sent * n + 1],
@@ -671,12 +690,19 @@ class Tokenizer:
         self.set_option("sample_base", int(i))
         return self
 
-    def lattice(self, on=True, text=False):
+    def lattice(self, on=True, text=False, margin=None):
         """Lattice output: results then carry every node of each sentence's lattice (BatchResult.nodes /
         node_links / node_probs, sentence_nodes()), with its best predecessor, a best-path flag and, with marginals,
         its marginal.  text=True also renders the nodes in place of the tokens in the output text (MeCab -a).
-        Single-device tokenizers only; the "small_batch" route steps aside.  Definition: include/vibrato_b200.h."""
+        margin=D (an integer, 0 <= D <= 2^62; the option "lattice_margin") keeps only the nodes on paths whose cost is
+        within D of the best one, plus the best path, and adds BatchResult.node_margins; None keeps every node.
+        The "small_batch" route steps aside.  Definition: include/vibrato_b200.h."""
         value = (2 if text else 1) if on else 0
+        m = -1 if margin is None else int(margin)
+        if margin is not None and m < 0:
+            raise VibratoError(1, "lattice: margin must be None or a cost margin between 0 and 2^62")
+        check(lib().vbt_tokenizer_set_option(self.handle(), b"lattice_margin", m))
+        self._lattice_margin = m
         check(lib().vbt_tokenizer_set_option(self.handle(), b"lattice", value))
         self._lattice = value
         return self
@@ -726,6 +752,9 @@ class Tokenizer:
         check(lib().vbt_tokenizer_set_option(self.handle(), name.encode(), int(value)))
         if name == "lattice":  # replayed with lattice()'s state, after the marginals
             self._lattice = int(value)
+            return
+        if name == "lattice_margin":  # replayed with lattice()'s state
+            self._lattice_margin = int(value)
             return
         if name == "sample_text":  # replayed after sampling, which it needs
             self._sample_text = bool(value)
@@ -875,16 +904,24 @@ class Token:
 
 class LatticeNode(Token):
     """One node of a sentence's lattice (Tokenizer.lattice): Token's accessors (start_char is the node's start_word,
-    total_cost its min_cost), plus its best predecessor, best-path flag and marginal."""
+    total_cost its min_cost), plus its best predecessor, best-path flag, marginal and, in a near-best lattice, margin."""
 
-    __slots__ = ("_link",)
+    __slots__ = ("_link", "_margin")
 
-    def __init__(self, tokenizer, sentence_bytes, rec, link, prob=None):
+    def __init__(self, tokenizer, sentence_bytes, rec, link, prob=None, margin=None):
         super().__init__(tokenizer, sentence_bytes, rec, prob)
         self._link = link
+        self._margin = margin
+
+    def margin(self):
+        """The node's exact cost margin over the best path (Tokenizer.lattice(margin=D))."""
+        if self._margin is None:
+            raise VibratoError(1, "no margins: pass margin= to Tokenizer.lattice() before tokenising")
+        return self._margin
 
     def prev(self):
-        """Index of the best predecessor in the sentence's node list, or None for BOS."""
+        """Index of the best predecessor in the sentence's node list, or None for BOS and, in a near-best lattice,
+        for a predecessor that was not kept (link prev -2)."""
         p = int(self._link["prev"])
         return None if p < 0 else p
 

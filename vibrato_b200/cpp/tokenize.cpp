@@ -31,6 +31,8 @@ static void usage() {
                  "                                      each token's with %%pP; -O output is unchanged)\n"
                  "         [-a|--all-morphs]           (every lattice node in place of the tokens, like MeCab -a: -O and\n"
                  "                                      -F render nodes, -F may print %%pb; needs --format-on device)\n"
+                 "         [--cost-margin D]           (with -a: only the nodes of paths whose cost is within D, 0..2^62,\n"
+                 "                                      of the best path's, plus the best path)\n"
                  "         [--sample N -t|--theta F [--seed S]]\n"
                  "                                     (N segmentations per line, 1..1024, drawn from the lattice's path\n"
                  "                                      distribution at temperature F, in place of the best path: -O and -F\n"
@@ -53,6 +55,7 @@ int main(int argc, char** argv) {
     uint32_t n_sample = 0;  // --sample
     uint64_t seed = 0;
     bool has_seed = false;
+    int64_t cost_margin = -1;  // --cost-margin, -1 = every node
     // a whole decimal number in [lo, hi], else a usage error
     auto parse_u64 = [](const std::string& v, uint64_t lo, uint64_t hi, uint64_t& out) {
         if (v.empty() || v.size() > 20 || v.find_first_not_of("0123456789") != std::string::npos) return false;
@@ -96,6 +99,14 @@ int main(int argc, char** argv) {
             if (a == "--sample") n_sample = uint32_t(v);
             else seed = v, has_seed = true;
         }
+        else if (a == "--cost-margin") {
+            uint64_t v = 0;
+            if (!parse_u64(next(), 0, uint64_t(1) << 62, v)) {
+                usage();
+                return 2;
+            }
+            cost_margin = int64_t(v);
+        }
         else if (a == "-t" || a == "--theta") {
             const std::string v = next();
             char* end = nullptr;
@@ -117,7 +128,7 @@ int main(int argc, char** argv) {
     const bool sample = n_sample != 0;
     if (batch_lines_arg == 0 || (has_node && format_on == "host") || (!has_node && (has_unk || has_bos || has_eos)) ||
         (marginal || sample) != has_theta || (all_morphs && format_on == "host") || (has_seed && !sample) ||
-        (sample && (all_morphs || format_on == "host")) ||
+        (sample && (all_morphs || format_on == "host")) || (cost_margin >= 0 && !all_morphs) ||
         (bounded && (marker.size() != 1 || marker[0] == '\n' || (marker[0] & 0x80))) || (bounded && partial)) {
         usage();
         return 2;
@@ -138,7 +149,7 @@ int main(int argc, char** argv) {
         Tokenizer tokenizer =
             Tokenizer(std::move(dict)).ignore_space(ignore_space).max_grouping_len(max_grouping_len).devices(devices);
         if (marginal) tokenizer.marginals(theta);  // before -F, which may print %pP
-        if (all_morphs) tokenizer.lattice(true, true);  // before -F, which may print %pb
+        if (all_morphs) tokenizer.lattice(true, true, cost_margin);  // before -F, which may print %pb
         if (sample) tokenizer.sampling(n_sample, theta, seed, true);  // before -F, which may not print %pP / %pb
         if (has_node) {
             const std::string_view node = node_format, unk = unk_format, bos = bos_format, eos = eos_format;

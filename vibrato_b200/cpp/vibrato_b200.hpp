@@ -177,6 +177,13 @@ class BatchResult {
         check(vbt_result_lattice(r_.get(), &l.node_offsets, &l.nodes, &l.links, &l.node_probs, &l.n_nodes));
         return l;
     }
+    // The near-best lattice's node margins (Tokenizer::lattice with a margin), indexed like lattice().nodes.  Throws
+    // on a result made without them.
+    const int64_t* lattice_margins() const {
+        const int64_t* m = nullptr;
+        check(vbt_result_lattice_margins(r_.get(), &m));
+        return m;
+    }
     // Segmentation sampling (Tokenizer::sampling before the batch, see vbt_tokenizer_set_sampling): sample j of
     // sentence i is samples[sample_offsets[i * n + j] .. sample_offsets[i * n + j + 1]).  Throws on a result made
     // without sampling.
@@ -283,11 +290,16 @@ class Tokenizer {
     bool has_marginals() const { return marginals_; }
     // Lattice output (the option "lattice", see vbt_result_lattice): BatchResult::lattice(); text = true also renders
     // the nodes in place of the tokens in the output text (MeCab -a).  Set text before a format that prints %pb.
-    void lattice(bool on = true, bool text = false) const {
+    // margin = D (0 .. 2^62; the option "lattice_margin") keeps only the nodes within cost D of the best path, plus the
+    // best path, with BatchResult::lattice_margins(); -1 keeps every node.
+    void lattice(bool on = true, bool text = false, int64_t margin = -1) const {
+        check(vbt_tokenizer_set_option(handle(), "lattice_margin", margin));
         check(vbt_tokenizer_set_option(handle(), "lattice", on ? (text ? 2 : 1) : 0));
         lattice_ = on;
+        margin_ = margin >= 0;
     }
     bool has_lattice() const { return lattice_; }
+    bool has_lattice_margins() const { return lattice_ && margin_; }
     // Device addresses of the last tokenize_batch_device call's lattice (node_prob 0 without marginals).
     struct DeviceLattice {
         uint64_t node_offsets = 0, nodes = 0, links = 0, node_probs = 0, n_nodes = 0;
@@ -395,6 +407,7 @@ class Tokenizer {
     uint64_t max_grouping_len_ = 0;
     mutable bool marginals_ = false;
     mutable bool lattice_ = false;
+    mutable bool margin_ = false;  // lattice(..., margin >= 0)
     mutable uint32_t samples_ = 0;
     mutable std::shared_ptr<vbt_tokenizer> h_;
 };
@@ -437,17 +450,24 @@ class Token {  // token.rs:8-92
 };
 
 // One node of a sentence's lattice (Tokenizer::lattice): Token's accessors (start_char = start_word, total_cost =
-// min_cost), plus its best predecessor, best-path flag and marginal.
+// min_cost), plus its best predecessor, best-path flag, marginal and, in a near-best lattice, margin.
 class LatticeNode : public Token {
    public:
     LatticeNode(const Tokenizer* t, std::string_view sentence, vbt_token rec, vbt_lattice_link link,
-                float prob = std::numeric_limits<float>::quiet_NaN())
-        : Token(t, sentence, rec, prob), link_(link) {}
-    int32_t prev() const { return link_.prev; }  // index in the sentence's node list, -1 for BOS
+                float prob = std::numeric_limits<float>::quiet_NaN(), int64_t margin = -1)
+        : Token(t, sentence, rec, prob), link_(link), margin_(margin) {}
+    // index in the sentence's node list, -1 for BOS, -2 for a predecessor a near-best lattice did not keep
+    int32_t prev() const { return link_.prev; }
     bool is_best() const { return (link_.flags & VBT_NODE_BEST) != 0; }
+    // the exact cost margin over the best path (Tokenizer::lattice with a margin); throws without one
+    int64_t margin() const {
+        if (margin_ < 0) throw VibratoError(VBT_ERR_INVALID_ARGUMENT, "no margins: pass a margin to Tokenizer::lattice before tokenising");
+        return margin_;
+    }
 
    private:
     vbt_lattice_link link_;
+    int64_t margin_;
 };
 
 class Worker {  // worker.rs:13-74
@@ -498,11 +518,16 @@ class Worker {  // worker.rs:13-74
         nodes_.clear();
         links_.clear();
         nprobs_.clear();
+        margins_.clear();
         if (t_->has_lattice()) {
             const BatchResult::Lattice l = r.lattice();
             nodes_.assign(l.nodes, l.nodes + l.n_nodes);
             links_.assign(l.links, l.links + l.n_nodes);
             if (l.node_probs) nprobs_.assign(l.node_probs, l.node_probs + l.n_nodes);
+            if (t_->has_lattice_margins() && l.n_nodes) {
+                const int64_t* m = r.lattice_margins();
+                margins_.assign(m, m + l.n_nodes);
+            }
         }
         if (!samples_.empty()) {
             const BatchResult::Samples s = r.samples();
@@ -514,7 +539,8 @@ class Worker {  // worker.rs:13-74
     Token sample_token(size_t j, size_t i) const { return Token(t_, sent_, samples_.at(j)[i]); }
     size_t num_nodes() const { return nodes_.size(); }
     LatticeNode node(size_t i) const {
-        return nprobs_.empty() ? LatticeNode(t_, sent_, nodes_[i], links_[i]) : LatticeNode(t_, sent_, nodes_[i], links_[i], nprobs_[i]);
+        return LatticeNode(t_, sent_, nodes_[i], links_[i], nprobs_.empty() ? std::numeric_limits<float>::quiet_NaN() : nprobs_[i],
+                           margins_.empty() ? -1 : margins_[i]);
     }
     size_t num_tokens() const { return toks_.size(); }
     Token token(size_t i) const {
@@ -534,6 +560,7 @@ class Worker {  // worker.rs:13-74
     std::vector<vbt_token> nodes_;  // Tokenizer::lattice
     std::vector<vbt_lattice_link> links_;
     std::vector<float> nprobs_;
+    std::vector<int64_t> margins_;  // Tokenizer::lattice with a margin
     std::vector<std::vector<vbt_token>> samples_;  // Tokenizer::sampling
 };
 

@@ -761,6 +761,23 @@ int32_t vbt_last_device_lattice(const vbt_tokenizer* t, uint64_t* d_node_offsets
     });
 }
 
+int32_t vbt_result_lattice_margins(const vbt_result* r, const int64_t** node_margin) {
+    return guarded([&] {
+        need(r, "r");
+        if (!r->r->out.has(vbt::kNodeMargin))
+            throw vbt::Error(vbt::kInvalidArgument,
+                             "no lattice margins: set the tokenizer options \"lattice\" and \"lattice_margin\" before tokenising");
+        if (node_margin) *node_margin = r->r->ptr<const int64_t>(vbt::kNodeMargin);
+    });
+}
+
+int32_t vbt_last_device_lattice_margins(const vbt_tokenizer* t, uint64_t* d_node_margin) {
+    return guarded([&] {
+        need(t, "t");
+        t->e->device_lattice_margins(d_node_margin);
+    });
+}
+
 int32_t vbt_tokenizer_set_sampling(vbt_tokenizer* t, uint32_t n, double theta, uint64_t seed) {
     return guarded([&] {
         need(t, "t");

@@ -150,13 +150,14 @@ struct Workspace {  // every per-(chunk of a)-batch device array; two of them le
     DevBuf span_tag;  // span batches only: SpanArgs::tag
     DevBuf m_fill, m_ncand, m_cand_entry, m_R, m_ab, m_r_eos, m_a_eos;  // marginals only: MargArgs
     DevBuf l_row_base, l_n_nodes;  // lattice output only: LatticeArgs
+    DevBuf g_G, g_keep;            // near-best lattice only: MarginArgs::G / keep
     DevBuf m_lw, s_cnt, s_total;   // sampling only: MargArgs::lw, SampleArgs::cnt / total
     cudaStream_t stream = nullptr;
     void release() {
         for (DevBuf* b : {&n_slots, &slot_off, &eos, &n_tok, &code_sys, &code_usr, &cinfo, &groupable, &byte_pos, &info,
                           &info_ex, &ends_cnt, &ends_meta, &seg, &ends_hot, &ends_cold, &scan_tmp, &stats, &iota,
                           &sort_keys, &order, &tiles, &bnd_dist, &span_tag, &m_fill, &m_ncand, &m_cand_entry, &m_R, &m_ab, &m_r_eos, &m_a_eos,
-                          &l_row_base, &l_n_nodes, &m_lw, &s_cnt, &s_total})
+                          &l_row_base, &l_n_nodes, &g_G, &g_keep, &m_lw, &s_cnt, &s_total})
             b->release();
     }
 };
@@ -430,6 +431,12 @@ class EngineImpl final : public Engine {
                 throw Error(kInvalidArgument, "lattice text and sample text both replace the output text: set \"sample_text\" to 0 before setting lattice = 2");
             cudaStreamSynchronize(stream_);
             lattice_ = int(value);
+        } else if (name == "lattice_margin") {
+            // the lattice keeps the nodes of the paths within cost D of the best one (-1: every node)
+            if (value < -1 || value > kMaxLatticeMargin)
+                throw Error(kInvalidArgument, "lattice_margin must be -1 (off) or a cost margin between 0 and 2^62");
+            cudaStreamSynchronize(stream_);
+            lat_margin_ = value;
         } else if (name == "sample_text") {
             // the output text renders each sentence's samples in place of its best path
             if (value < 0 || value > 1) throw Error(kInvalidArgument, "sample_text must be 0 (off) or 1 (the text renders the samples)");
@@ -518,6 +525,11 @@ class EngineImpl final : public Engine {
         if (!made_.has(kTokenProb)) throw Error(kInvalidArgument, "the last device-resident call ran without marginals");
         put_address(d_token_prob, made_, out_[0].buf, kTokenProb);
         put_address(d_path_prob, made_, out_[0].buf, kPathProb);
+    }
+    void device_lattice_margins(uint64_t* d_node_margin) const override {
+        if (!made_.has(kNodeMargin))
+            throw Error(kInvalidArgument, "the last device-resident call ran without the lattice's cost margin");
+        put_address(d_node_margin, made_, out_[0].buf, kNodeMargin);
     }
     void device_lattice(uint64_t* d_node_off, uint64_t* d_nodes, uint64_t* d_links, uint64_t* d_node_prob,
                         uint64_t* n_nodes) const override {
@@ -1050,7 +1062,10 @@ class EngineImpl final : public Engine {
     }
 
     // The arrays a host result carries under the current options.
-    Outputs outputs() const { return Outputs{tok_bytes_, samp_n_, theta_ > 0, output_mode_ != kOutNone, lattice_ != 0}; }
+    Outputs outputs() const {
+        return Outputs{tok_bytes_, samp_n_, theta_ > 0, output_mode_ != kOutNone, lattice_ != 0, lat_margin_ >= 0};
+    }
+    bool margin_on() const { return lattice_ && lat_margin_ >= 0; }  // the near-best lattice's kernels run
 
     // D2H on `st` of every array r carries, from slot `o` holding n sentences and `count` records per group: to
     // sentence s0 of r and after `base` records per group; `last` brings the closing offsets too.
@@ -1091,6 +1106,7 @@ class EngineImpl final : public Engine {
             o.buf[kNodes].ensure(n * 24);
             o.buf[kLinks].ensure(n * 8);
             if (theta_ > 0) o.buf[kNodeProb].ensure(n * 4);
+            if (margin_on()) o.buf[kNodeMargin].ensure(n * 8);
         }
         if (samp_n_) o.buf[kSampleOff].ensure((size_t(n_sent) * samp_n_ + 1) * 8, 1.25);
     }
@@ -1472,12 +1488,13 @@ class EngineImpl final : public Engine {
         if (bounded) w.bnd_dist.ensure(ms * 4, 1.25);
         if (spans) w.span_tag.ensure(ms * 8, 1.25);
         const bool fwd = theta_ > 0 || samp_n_;  // the forward pass runs
-        if (fwd) {
+        const bool rfwd = fwd || margin_on();    // ... or its R-only instantiation
+        if (rfwd) {
             w.m_fill.ensure(ms * 4, 1.25);
             w.m_ncand.ensure(ms * 4, 1.25);
             w.m_r_eos.ensure(ns * 8, 1.25);
-            w.m_a_eos.ensure(ns * 8, 1.25);
         }
+        if (fwd) w.m_a_eos.ensure(ns * 8, 1.25);
         if (lattice_) {
             w.l_row_base.ensure(ms * 4, 1.25);
             w.l_n_nodes.ensure(ns * 4, 1.25);
@@ -1488,10 +1505,14 @@ class EngineImpl final : public Engine {
         w.seg.ensure(want_cand * 8);  // sized like the candidates; move segments can outnumber them (overflow retry)
         w.ends_hot.ensure((want_cand + ns) * 8);
         w.ends_cold.ensure((want_cand + ns) * 16);
-        if (fwd) {
+        if (rfwd) {
             w.m_cand_entry.ensure((want_cand + ns) * 4);
             w.m_R.ensure((want_cand + ns) * 8);
-            w.m_ab.ensure((want_cand + ns) * 16);
+        }
+        if (fwd) w.m_ab.ensure((want_cand + ns) * 16);
+        if (margin_on()) {
+            w.g_G.ensure((want_cand + ns) * 8);
+            w.g_keep.ensure((want_cand + ns) * 4);
         }
         if (samp_n_) {
             w.m_lw.ensure((want_cand + ns) * 4);
@@ -1567,7 +1588,7 @@ class EngineImpl final : public Engine {
                  OutSlot& o, unsigned long long* base, cudaEvent_t base_wait, cudaEvent_t base_signal, const DevBounds& bd,
                  uint64_t sent0) {
         cudaStream_t st = w.stream;
-        o.made = Outputs{tok_bytes_, samp_n_, theta_ > 0, base && output_mode_ != kOutNone, lattice_ != 0};
+        o.made = Outputs{tok_bytes_, samp_n_, theta_ > 0, base && output_mode_ != kOutNone, lattice_ != 0, lat_margin_ >= 0};
         // characters <= bytes is the hard bound; the per-character launches are sized from the ratio learned on
         // earlier batches (plus slack), and a batch that exceeds it flags itself and is re-run with the hard bound
         const uint32_t hard_slots = uint32_t(n_bytes + n_sent);
@@ -1578,10 +1599,14 @@ class EngineImpl final : public Engine {
             cap_all = std::min<size_t>(cap_all, std::min<size_t>(w.m_cand_entry.cap / 4,
                                                                  std::min<size_t>(w.m_R.cap / 8, w.m_ab.cap / 16)) - n_sent - 1);
         if (samp) cap_all = std::min<size_t>(cap_all, w.m_lw.cap / 4 - n_sent - 1);
-        const bool lat = lattice_ != 0;
+        const bool lat = lattice_ != 0, mlat = margin_on();
+        if (mlat)
+            cap_all = std::min<size_t>(cap_all, std::min<size_t>({w.m_cand_entry.cap / 4, w.m_R.cap / 8, w.g_G.cap / 8,
+                                                                  w.g_keep.cap / 4}) - n_sent - 1);
         if (lat) {  // nodes <= candidates placed: the node arrays bound the pool too
             cap_all = std::min<size_t>(cap_all, std::min<size_t>(o.buf[kNodes].cap / 24, o.buf[kLinks].cap / 8));
             if (marg) cap_all = std::min<size_t>(cap_all, o.buf[kNodeProb].cap / 4);
+            if (mlat) cap_all = std::min<size_t>(cap_all, o.buf[kNodeMargin].cap / 8);
         }
         const uint32_t cand_cap = uint32_t(cap_all);
         Batch b{};
@@ -1694,6 +1719,17 @@ class EngineImpl final : public Engine {
             launch_marginals(dv_, b, m, st, marg);  // sampling alone needs no backward pass
             if (n_sent) o.launches += marg ? 2 : 1;
         }
+        MarginArgs g{};
+        if (mlat) {  // G of every entry, from the R the forward pass above left (or its R-only instantiation here)
+            m.fill = w.m_fill.as<uint32_t>();
+            m.ncand = w.m_ncand.as<uint32_t>();
+            m.cand_entry = w.m_cand_entry.as<uint32_t>();
+            m.R = w.m_R.as<long long>();
+            m.r_eos = w.m_r_eos.as<long long>();
+            g = MarginArgs{lat_margin_, w.g_G.as<long long>(), w.g_keep.as<uint32_t>(), o.buf[kNodeMargin].as<long long>()};
+            launch_margin_backward(dv_, b, m, g, !(marg || samp), st);
+            if (n_sent) o.launches += (marg || samp) ? 1 : 2;
+        }
         if (lat) {  // booked with the Viterbi stage too, and also before K4
             LatticeArgs l{};
             l.row_base = w.l_row_base.as<uint32_t>();
@@ -1702,11 +1738,17 @@ class EngineImpl final : public Engine {
             l.nodes = o.buf[kNodes].as<uint2>();
             l.links = o.buf[kLinks].as<int2>();
             l.node_prob = marg ? o.buf[kNodeProb].as<float>() : nullptr;
-            launch_lattice_count(b, l, st);
+            if (mlat)
+                launch_lattice_count(b, l, m, g, st);
+            else
+                launch_lattice_count(b, l, st);
             cub::TransformInputIterator<unsigned long long, CastU64, const uint32_t*> it(l.n_nodes, CastU64());
             if (n_sent == 0) CK(cudaMemsetAsync(l.n_nodes, 0, 4, st));
             exclusive_scan(w, it, l.node_off, size_t(n_sent) + 1);
-            launch_lattice_write(b, l, m, st);
+            if (mlat)
+                launch_lattice_write(b, l, m, g, st);
+            else
+                launch_lattice_write(b, l, m, st);
             CK(cudaMemcpyAsync(&dc->total[kGroupLattice], l.node_off + n_sent, 8, cudaMemcpyDeviceToDevice, st));
             if (n_sent) o.launches += 2;
         }
@@ -1834,6 +1876,8 @@ class EngineImpl final : public Engine {
     int viterbi_kernel_ = 1;  // 1 = k_viterbi2 with pruning (kernels.cuh)
     double theta_ = 0;        // marginals' theta, 0 = off (set_marginals)
     int lattice_ = 0;         // option "lattice": 0 off, 1 nodes, 2 nodes and lattice text
+    static constexpr long long kMaxLatticeMargin = 1ll << 62;
+    long long lat_margin_ = -1;  // option "lattice_margin": the near-best lattice's D, -1 = off
     static constexpr uint32_t kMaxSamples = 1024;
     uint32_t samp_n_ = 0;       // sampling: paths per sentence, 0 = off (set_sampling)
     double samp_theta_ = 0;

@@ -13,7 +13,7 @@
 namespace vbt {
 
 // ---- the outputs of a batch ------------------------------------------------------------------------
-// A batch produces up to twelve arrays in four ragged groups.  A group's offsets index its records: entries
+// A batch produces up to thirteen arrays in four ragged groups.  A group's offsets index its records: entries
 // off[i] .. off[i + 1] belong to sentence i (to sample j of sentence i at i * n_samp + j for the samples), and the
 // group's total is the number of its records.  path_prob has one entry per sentence and no offsets.
 enum Group { kGroupTokens, kGroupText, kGroupLattice, kGroupSamples, kNumGroups };
@@ -21,6 +21,7 @@ enum Array {
     kTokOff, kTokens, kTokenProb, kPathProb,  // vbt_token (or vbt_token16) records; marginals (set_marginals)
     kTextOff, kText,                          // output stage ("output_mode" or a format): the text `tokenize` prints
     kNodeOff, kNodes, kLinks, kNodeProb,      // lattice ("lattice" >= 1): vbt_token nodes, vbt_lattice_link, marginals
+    kNodeMargin,                              // near-best lattice ("lattice_margin" >= 0): each kept node's margin (int64)
     kSampleOff, kSamples,                     // sampling (set_sampling): vbt_token records of every sampled path
     kNumArrays
 };
@@ -33,7 +34,8 @@ struct ArrayInfo {
 constexpr ArrayInfo kArrays[kNumArrays] = {
     {kGroupTokens, kOffsets, 8},   {kGroupTokens, kRecords, 0},  {kGroupTokens, kRecords, 4},   {kGroupTokens, kPerSentence, 4},
     {kGroupText, kOffsets, 8},     {kGroupText, kRecords, 1},    {kGroupLattice, kOffsets, 8},  {kGroupLattice, kRecords, 24},
-    {kGroupLattice, kRecords, 8},  {kGroupLattice, kRecords, 4}, {kGroupSamples, kOffsets, 8},  {kGroupSamples, kRecords, 24},
+    {kGroupLattice, kRecords, 8},  {kGroupLattice, kRecords, 4}, {kGroupLattice, kRecords, 8},  {kGroupSamples, kOffsets, 8},
+    {kGroupSamples, kRecords, 24},
 };
 constexpr Array kOffsetsOf[kNumGroups] = {kTokOff, kTextOff, kNodeOff, kSampleOff};
 
@@ -44,6 +46,7 @@ struct Outputs {
     uint32_t token_bytes = 24;  // 24, or 16 with "compact_tokens"
     uint32_t n_samp = 0;        // sampled paths per sentence, 0 = sampling off
     bool marg = false, text = false, lat = false;
+    bool margin = false;  // "lattice_margin" >= 0: the lattice keeps the near-best nodes and carries their margins
 
     bool has(int a) const {
         switch (a) {
@@ -55,6 +58,7 @@ struct Outputs {
             case kNodes:
             case kLinks: return lat;
             case kNodeProb: return lat && marg;
+            case kNodeMargin: return lat && margin;
             case kSampleOff:
             case kSamples: return n_samp != 0;
             default: return true;
@@ -204,7 +208,8 @@ class Engine {
     // produces the text arrays, on every host route; run_device stays token-only), "small_batch" (N > 0: run_host
     // takes k_small_batch for batches of at most N sentences and 16 KiB without counting; run_device and the shards
     // of a multi-device engine keep the usual route), "lattice" (0 off, 1 results also carry every lattice node,
-    // 2 the same and the output text renders the nodes in place of the tokens).
+    // 2 the same and the output text renders the nodes in place of the tokens), "lattice_margin" (-1 off; D in
+    // 0 .. 2^62: the lattice keeps only the nodes within cost D of the best path, kernels.cuh MarginArgs).
     virtual void set_option(const std::string& name, long long value) = 0;
     // An output format (format.hpp) in place of "output_mode" 1-3, on every host route; nullptr switches it off.
     // Setting "output_mode" replaces it.  Builds the format's field table on the device.
@@ -232,6 +237,9 @@ class Engine {
     // valid until the next call.  Throws when that call ran without the lattice.
     virtual void device_lattice(uint64_t* d_node_off, uint64_t* d_nodes, uint64_t* d_links, uint64_t* d_node_prob,
                                 uint64_t* n_nodes) const = 0;
+    // Device address of the last run_device's int64 node_margin[n_nodes] ("lattice_margin" >= 0); valid until the next
+    // call.  Throws when that call ran without the lattice or without the margin.
+    virtual void device_lattice_margins(uint64_t* d_node_margin) const = 0;
     // Launch on a caller-owned CUDA stream (0 restores the engine's own stream).
     virtual void set_stream(uint64_t stream) = 0;
     virtual const float* stage_ms() const = 0;

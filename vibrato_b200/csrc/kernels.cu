@@ -1793,8 +1793,9 @@ __device__ __forceinline__ bool marg_sentence(const Batch& b, uint32_t sidx, uin
     return true;
 }
 
-// LW: the sampling instantiation, which also keeps each entry's {left id, word cost} in m.lw.
-template <int CONN, bool LW = false>
+// LW: the sampling instantiation, which also keeps each entry's {left id, word cost} in m.lw.  LSE = false: the
+// near-best lattice's instantiation, which writes only R, r_eos, ncand and cand_entry (no log-sum-exp, m.ab unread).
+template <int CONN, bool LW = false, bool LSE = true>
 __global__ void __launch_bounds__(256) k_marg_forward(DictView d, Batch b, MargArgs m) {
     if (stand_down(*b.flags)) return;
     const uint32_t lane = threadIdx.x & 31;
@@ -1803,8 +1804,10 @@ __global__ void __launch_bounds__(256) k_marg_forward(DictView d, Batch b, MargA
     if (base == last) {  // an empty sentence: one (empty) path
         if (lane == 0) {
             m.r_eos[s] = 0;
-            m.a_eos[s] = 0.0;
-            m.path_prob[s] = 1.f;
+            if (LSE) {
+                m.a_eos[s] = 0.0;
+                m.path_prob[s] = 1.f;
+            }
         }
         return;
     }
@@ -1812,7 +1815,7 @@ __global__ void __launch_bounds__(256) k_marg_forward(DictView d, Batch b, MargA
     if (lane == 0) {  // BOS
         const uint32_t bos = b.ends_meta[base].x;
         m.R[bos] = 0;
-        m.ab[bos] = make_double2(0.0, -INFINITY);
+        if (LSE) m.ab[bos] = make_double2(0.0, -INFINITY);
     }
     __syncwarp();
     const double th = m.theta;
@@ -1857,10 +1860,13 @@ __global__ void __launch_bounds__(256) k_marg_forward(DictView d, Batch b, MargA
                 double L = -INFINITY;
                 for (uint32_t k = 0; k < K; ++k) {
                     const long long x = m.R[eo + k] + conn.cost(d, uint32_t(b.ends_hot[eo + k].y)) + wc;
-                    marg_push(x, m.ab[eo + k].x, th, rmin, L);
+                    if (LSE)
+                        marg_push(x, m.ab[eo + k].x, th, rmin, L);
+                    else
+                        rmin = min(rmin, x);
                 }
                 m.R[idx] = rmin;
-                m.ab[idx].x = L;
+                if (LSE) m.ab[idx].x = L;
                 if (LW) m.lw[idx] = (cd.x & 0xFFFFu) | (cd.y << 16);
             }
             __syncwarp();
@@ -1873,11 +1879,18 @@ __global__ void __launch_bounds__(256) k_marg_forward(DictView d, Batch b, MargA
         const ConnRow<CONN> conn(d, 0);
         long long rmin = LLONG_MAX;
         double L = -INFINITY;
-        for (uint32_t k = 0; k < K; ++k)
-            marg_push(m.R[me.x + k] + conn.cost(d, uint32_t(b.ends_hot[me.x + k].y)), m.ab[me.x + k].x, th, rmin, L);
+        for (uint32_t k = 0; k < K; ++k) {
+            const long long x = m.R[me.x + k] + conn.cost(d, uint32_t(b.ends_hot[me.x + k].y));
+            if (LSE)
+                marg_push(x, m.ab[me.x + k].x, th, rmin, L);
+            else
+                rmin = min(rmin, x);
+        }
         m.r_eos[s] = rmin;
-        m.a_eos[s] = L;
-        m.path_prob[s] = K ? float(exp(-L)) : 0.f;
+        if (LSE) {
+            m.a_eos[s] = L;
+            m.path_prob[s] = K ? float(exp(-L)) : 0.f;
+        }
     }
 }
 
@@ -1927,6 +1940,52 @@ __global__ void __launch_bounds__(256) k_marg_backward(DictView d, Batch b, Marg
                     }
                 }
                 m.ab[eo + k].y = L;
+            }
+        }
+        __syncwarp();
+    }
+}
+
+// Near-best lattice (MarginArgs in kernels.cuh): G(n), the least exact cost from entry n to EOS, shaped like
+// k_marg_backward (a warp per sentence, rows right to left, a lane per entry) with min-plus in place of log-sum-exp.
+template <int CONN>
+__global__ void __launch_bounds__(256) k_margin_backward(DictView d, Batch b, MargArgs m, MarginArgs g) {
+    if (stand_down(*b.flags)) return;
+    const uint32_t lane = threadIdx.x & 31;
+    uint32_t s, base, last;
+    if (!marg_sentence(b, (blockIdx.x * blockDim.x + threadIdx.x) >> 5, s, base, last) || base == last) return;
+    const uint32_t slot_end = base + b.eos[s].y;  // the row EOS connects to
+    uint32_t centry = 0;  // one past the last candidate entry k_marg_forward numbered, as in k_marg_backward
+    for (uint32_t slot = base + lane; slot < slot_end; slot += 32) centry += m.ncand[slot];
+    centry = b.ends_meta[base].x + __reduce_add_sync(kFull, centry);
+    for (uint32_t slot = last + 1; slot-- > base;) {
+        const uint2 me = b.ends_meta[slot];
+        const uint32_t eo = me.x, K = me.y - me.x;
+        if (slot == slot_end) {
+            const ConnRow<CONN> conn(d, 0);
+            for (uint32_t k = lane; k < K; k += 32) g.G[eo + k] = conn.cost(d, uint32_t(b.ends_hot[eo + k].y));
+        } else {  // no successor beyond EOS's row or at a position the sweep skips: LLONG_MAX
+            const uint32_t nc = slot < slot_end ? m.ncand[slot] : 0u;
+            const uint32_t sptr = nc ? b.info[slot].x : 0u;
+            centry -= nc;
+            for (uint32_t k = lane; k < K; k += 32) {
+                long long best = LLONG_MAX;
+                if (nc) {
+                    const uint32_t right = uint32_t(b.ends_hot[eo + k].y);
+                    uint32_t c = 0, end = slot;
+                    for (uint32_t h = 0; c < nc; ++h) {
+                        const uint2 sg = __ldg(&b.seg[sptr + h]);
+                        end += uint32_t(int32_t(sg.y) >> 16);
+                        for (uint32_t j = 0; j < (sg.y & 0xFFFFu); ++j, ++c) {
+                            const uint4 cd = seg_record(d, sg, j, end);
+                            const long long ge = g.G[m.cand_entry[centry + c]];
+                            if (ge == LLONG_MAX) continue;
+                            const ConnRow<CONN> conn(d, cd.x & 0xFFFFu);
+                            best = min(best, ge + conn.cost(d, right) + int16_t(cd.y & 0xFFFFu));
+                        }
+                    }
+                }
+                g.G[eo + k] = best;
             }
         }
         __syncwarp();
@@ -2017,6 +2076,93 @@ __global__ void __launch_bounds__(256) k_lattice_write(Batch b, LatticeArgs l, M
             }
         }
     }
+}
+
+// The near-best lattice's count and write (MarginArgs): the kept nodes in node order, numbered through g.keep.
+
+// f(entry) for each node of sentence s's best path, from EOS back, as backtrack_count_one walks it.
+template <class F>
+__device__ __forceinline__ void walk_best(const Batch& b, uint32_t s, uint32_t base, F f) {
+    const uint4 eo = b.eos[s];
+    if (eo.x == kNone) return;
+    uint32_t cur = eo.x, end_node = eo.y;
+    while (end_node != 0) {
+        const uint4 c = b.ends_cold[cur];
+        f(cur);
+        end_node = c.x - base;
+        cur = c.y;
+    }
+}
+
+__global__ void __launch_bounds__(256) k_lattice_count_margin(Batch b, LatticeArgs l, MargArgs m, MarginArgs g) {
+    const uint32_t s = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const uint32_t lane = threadIdx.x & 31;
+    if (s >= b.n_sent) return;
+    const uint32_t base = b.slot_off[s], last = b.slot_off[s + 1] - 1;
+    // a re-run or refused batch keeps nothing, and neither does an empty sentence or one without a path
+    if ((*b.flags & (kFlagsStandDown | kFlagPoolOverflow)) || base == last || b.eos[s].x == kNone) {
+        if (lane == 0) l.n_nodes[s] = 0;
+        return;
+    }
+    const long long best = m.r_eos[s];
+    for (uint32_t slot = base; slot <= last; ++slot) {  // the margin rule
+        const uint2 me = b.ends_meta[slot];
+        for (uint32_t e = me.x + (slot == base ? 1u : 0u) + lane; e < me.y; e += 32) {
+            const long long ge = g.G[e];
+            g.keep[e] = (ge != LLONG_MAX && m.R[e] + ge - best <= g.D) ? 0u : kNone;
+        }
+    }
+    __syncwarp();
+    if (lane == 0) walk_best(b, s, base, [&](uint32_t e) { g.keep[e] = 0; });  // the best path is always kept
+    __syncwarp();
+    uint32_t run = 0;
+    for (uint32_t slot = base; slot <= last; ++slot) {  // kept indices in node order
+        const uint2 me = b.ends_meta[slot];
+        for (uint32_t e0 = me.x + (slot == base ? 1u : 0u); e0 < me.y; e0 += 32) {
+            const uint32_t e = e0 + lane;
+            const bool kept = e < me.y && g.keep[e] == 0;
+            const uint32_t bal = __ballot_sync(kFull, kept);
+            if (kept) g.keep[e] = run + __popc(bal & lanemask_lt());
+            run += __popc(bal);
+        }
+    }
+    if (lane == 0) l.n_nodes[s] = run;
+}
+
+__global__ void __launch_bounds__(256) k_lattice_write_margin(Batch b, LatticeArgs l, MargArgs m, MarginArgs g) {
+    const uint32_t s = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const uint32_t lane = threadIdx.x & 31;
+    if (s >= b.n_sent || (*b.flags & (kFlagsStandDown | kFlagPoolOverflow))) return;
+    const uint32_t base = b.slot_off[s], last = b.slot_off[s + 1] - 1;
+    if (base == last || b.eos[s].x == kNone) return;  // nothing kept
+    const unsigned long long n0 = l.node_off[s];
+    const double a_eos = l.node_prob ? m.a_eos[s] : 0.0;
+    const long long best = m.r_eos[s];
+    for (uint32_t slot = base; slot <= last; ++slot) {
+        const uint2 me = b.ends_meta[slot];
+        for (uint32_t e = me.x + (slot == base ? 1u : 0u) + lane; e < me.y; e += 32) {
+            const uint32_t kept = g.keep[e];
+            if (kept == kNone) continue;
+            const uint4 c = b.ends_cold[e];  // {start_node slot, best prev entry, word_idx, min_cost}
+            const unsigned long long k = n0 + kept;
+            const uint32_t start_node = c.x - base;
+            const uint2 i8 = b.info[c.x];
+            const uint32_t start_word = start_node + ((i8.y & kInfoSpecial) ? b.info_ex[c.x].x : 0u);  // as k_lattice_write
+            uint2* t = l.nodes + k * 3;
+            t[0] = make_uint2(start_word, slot - base);
+            t[1] = make_uint2(b.byte_pos[base + start_word], b.byte_pos[slot]);
+            t[2] = make_uint2(c.z, c.w);
+            const uint32_t pk = c.x == base ? 0u : g.keep[c.y];
+            l.links[k] = make_int2(c.x == base ? -1 : pk == kNone ? -2 : int32_t(pk), 0);
+            g.node_margin[k] = m.R[e] + g.G[e] - best;
+            if (l.node_prob) {
+                const double2 ab = m.ab[e];
+                l.node_prob[k] = float(exp(ab.x + ab.y - a_eos));  // the expression of k_backtrack<true>
+            }
+        }
+    }
+    __syncwarp();
+    if (lane == 0) walk_best(b, s, base, [&](uint32_t e) { l.links[n0 + g.keep[e]].y = int32_t(kNodeBest); });
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -3142,6 +3288,35 @@ void launch_lattice_count(const Batch& b, const LatticeArgs& l, cudaStream_t st)
 void launch_lattice_write(const Batch& b, const LatticeArgs& l, const MargArgs& m, cudaStream_t st) {
     if (!b.n_sent) return;
     k_lattice_write<<<(b.n_sent + 7) / 8, 256, 0, st>>>(b, l, m);
+}
+
+template <int CONN>
+static void launch_margin_conn(const DictView& d, const Batch& b, const MargArgs& m, const MarginArgs& g, bool forward,
+                               uint32_t blocks, cudaStream_t st) {
+    if (forward) k_marg_forward<CONN, false, false><<<blocks, 256, 0, st>>>(d, b, m);
+    k_margin_backward<CONN><<<blocks, 256, 0, st>>>(d, b, m, g);
+}
+
+void launch_margin_backward(const DictView& d, const Batch& b, const MargArgs& m, const MarginArgs& g, bool forward,
+                            cudaStream_t st) {
+    if (!b.n_sent) return;
+    const uint32_t blocks = (b.n_sent + 7) / 8;  // a warp per sentence
+    if (d.connector_kind == 1)
+        launch_margin_conn<1>(d, b, m, g, forward, blocks, st);
+    else if (d.connector_kind == 2)
+        launch_margin_conn<2>(d, b, m, g, forward, blocks, st);
+    else
+        launch_margin_conn<0>(d, b, m, g, forward, blocks, st);
+}
+
+void launch_lattice_count(const Batch& b, const LatticeArgs& l, const MargArgs& m, const MarginArgs& g, cudaStream_t st) {
+    if (!b.n_sent) return;
+    k_lattice_count_margin<<<(b.n_sent + 7) / 8, 256, 0, st>>>(b, l, m, g);
+}
+
+void launch_lattice_write(const Batch& b, const LatticeArgs& l, const MargArgs& m, const MarginArgs& g, cudaStream_t st) {
+    if (!b.n_sent) return;
+    k_lattice_write_margin<<<(b.n_sent + 7) / 8, 256, 0, st>>>(b, l, m, g);
 }
 
 void launch_sample_count(const DictView& d, const Batch& b, const MargArgs& m, const SampleArgs& s, cudaStream_t st) {

@@ -308,6 +308,25 @@ void launch_lattice_count(const Batch& b, const LatticeArgs& l, cudaStream_t st)
 // computes it (a warp per sentence), after node_off has been scanned.
 void launch_lattice_write(const Batch& b, const LatticeArgs& l, const MargArgs& m, cudaStream_t st);
 
+// Near-best lattice (option "lattice_margin" = D >= 0): the lattice output keeps the nodes n with a path to EOS and
+// margin(n) = R(n) + G(n) - R(EOS) <= D, and every node of the best path.  G(n) is the least exact (64-bit) cost from
+// n to EOS over the edges after it; margins are exact integers, so the kept set does not depend on the route, the
+// chunking or the sentence order.  Links name the predecessor's index in the kept list, -2 when it was not kept.
+struct MarginArgs {
+    long long D;               // 0 .. 2^62
+    long long* G;              // per lattice entry; LLONG_MAX = no path to EOS
+    uint32_t* keep;            // per lattice entry: the sentence-relative index in the kept list, or kNone
+    long long* node_margin;    // per kept node
+};
+// The R-only instantiation of k_marg_forward when `forward` (neither marginals nor sampling ran it), then
+// k_margin_backward: G of every lattice entry.  After K3 and before K4, like launch_marginals.
+void launch_margin_backward(const DictView& d, const Batch& b, const MargArgs& m, const MarginArgs& g, bool forward,
+                            cudaStream_t st);
+// k_lattice_count_margin: g.keep and l.n_nodes (the kept count); the scan of n_nodes then gives l.node_off.
+void launch_lattice_count(const Batch& b, const LatticeArgs& l, const MargArgs& m, const MarginArgs& g, cudaStream_t st);
+// k_lattice_write_margin: the kept nodes' records, links and g.node_margin (and l.node_prob), after the scan.
+void launch_lattice_write(const Batch& b, const LatticeArgs& l, const MargArgs& m, const MarginArgs& g, cudaStream_t st);
+
 // Segmentation sampling: n paths per sentence drawn with replacement from P(path) = exp(-theta cost) / Z, by
 // forward-filtering backward-sampling over what k_marg_forward left (R, â and MargArgs::lw), after it and before K4.
 // A walk starts at EOS; at node c (EOS: left id 0, word cost 0) its predecessors are the entries k = 0..K-1 of the

@@ -369,6 +369,7 @@ class MultiEngine final : public Engine {
         if (name == "chunk_sentences") return;  // shards are not chunked (see the constructor)
         for (auto& e : eng_) e->set_option(name, value);
         if (name == "lattice") lattice_ = int(value);
+        if (name == "lattice_margin") lat_margin_ = value;
         if (name == "sample_base") sample_base_ = uint64_t(value);
         if (name == "output_mode") text_ = fixed_mode_ = value != 0;
     }
@@ -414,6 +415,12 @@ class MultiEngine final : public Engine {
         put_address(d_links, made_, gather_, kLinks);
         put_address(d_node_prob, made_, gather_, kNodeProb);
         if (n_nodes) *n_nodes = made_total_[kGroupLattice];
+    }
+    void device_lattice_margins(uint64_t* d_node_margin) const override {
+        if (dev_.size() == 1) return eng_[0]->device_lattice_margins(d_node_margin);
+        if (!made_.has(kNodeMargin))
+            throw Error(kInvalidArgument, "the last device-resident call ran without the lattice's cost margin");
+        put_address(d_node_margin, made_, gather_, kNodeMargin);
     }
     void set_stream(uint64_t stream) override {
         if (stream) throw Error(kUnsupported, "a multi-device tokenizer runs on its own streams");
@@ -534,7 +541,7 @@ class MultiEngine final : public Engine {
     }
 
     // The arrays a host result carries under the current options.
-    Outputs outputs() const { return Outputs{token_bytes(), sampling(), marginals() > 0, text_, lattice_ != 0}; }
+    Outputs outputs() const { return Outputs{token_bytes(), sampling(), marginals() > 0, text_, lattice_ != 0, lat_margin_ >= 0}; }
 
     // base[i][g] = the records of group g in the shards before shard i (base[n] = all of them).
     static std::vector<Totals> prefix_sums(const std::vector<Totals>& count) {
@@ -567,6 +574,7 @@ class MultiEngine final : public Engine {
     Outputs made_;               // the arrays the last device-resident call produced
     Totals made_total_{};
     int lattice_ = 0;  // option "lattice"
+    long long lat_margin_ = -1;  // option "lattice_margin"
     uint64_t sample_base_ = 0;  // option "sample_base" (every engine adds it to its shard's first sentence)
     float stage_ms_[kNumStages];
     uint64_t counters_[10];
