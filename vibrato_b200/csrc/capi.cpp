@@ -66,6 +66,29 @@ int32_t guarded(F&& f) {
 void need(const void* p, const char* what) {
     if (!p) throw vbt::Error(vbt::kInvalidArgument, std::string(what) + " must not be NULL");
 }
+
+void put(uint64_t* dst, uint64_t value) {
+    if (dst) *dst = value;
+}
+
+// A device-resident batch (vbt_tokenize_batch_device*): its token arrays, left on the device.
+void run_device(vbt_tokenizer* t, uint64_t d_utf8, uint64_t d_byte_offsets, uint64_t n_sent, uint64_t n_bytes,
+                const vbt::Bounds* b, uint64_t* d_tok_offsets, uint64_t* d_tokens, uint64_t* n_tokens) {
+    t->e->run_device(d_utf8, d_byte_offsets, n_sent, n_bytes, b);
+    const vbt::DeviceOutputs& d = t->e->last_device();
+    *d_tok_offsets = d.addr[vbt::kTokOff];
+    *d_tokens = d.addr[vbt::kTokens];
+    *n_tokens = d.total[vbt::kGroupTokens];
+}
+
+// What the last device-resident call left on the device (vbt_last_device_*), refused when that call did not produce
+// array a: it ran without `what`, or it failed.
+const vbt::DeviceOutputs& last_device(const vbt_tokenizer* t, int a, const char* what) {
+    need(t, "t");
+    const vbt::DeviceOutputs& d = t->e->last_device();
+    if (!d.made.has(a)) throw vbt::Error(vbt::kInvalidArgument, std::string("the last device-resident call ran without ") + what);
+    return d;
+}
 }  // namespace
 
 extern "C" {
@@ -617,7 +640,7 @@ int32_t vbt_tokenize_batch_device(vbt_tokenizer* t, uint64_t d_utf8, uint64_t d_
         need(d_tok_offsets, "d_tok_offsets");
         need(d_tokens, "d_tokens");
         need(n_tokens, "n_tokens");
-        t->e->run_device(d_utf8, d_byte_offsets, n_sent, n_bytes, d_tok_offsets, d_tokens, n_tokens);
+        run_device(t, d_utf8, d_byte_offsets, n_sent, n_bytes, nullptr, d_tok_offsets, d_tokens, n_tokens);
     });
 }
 
@@ -632,7 +655,7 @@ int32_t vbt_tokenize_batch_device_bounded(vbt_tokenizer* t, uint64_t d_utf8, uin
         if (!d_bnd_offsets) throw vbt::Error(vbt::kInvalidArgument, "d_bnd_offsets is null");
         if (n_bnd && !d_bnd) throw vbt::Error(vbt::kInvalidArgument, "d_bnd is null");
         const vbt::Bounds b{reinterpret_cast<const uint64_t*>(d_bnd_offsets), reinterpret_cast<const uint32_t*>(d_bnd), n_bnd, {}};
-        t->e->run_device(d_utf8, d_byte_offsets, n_sent, n_bytes, d_tok_offsets, d_tokens, n_tokens, &b);
+        run_device(t, d_utf8, d_byte_offsets, n_sent, n_bytes, &b, d_tok_offsets, d_tokens, n_tokens);
     });
 }
 
@@ -657,7 +680,7 @@ int32_t vbt_tokenize_batch_device_spans(vbt_tokenizer* t, uint64_t d_utf8, uint6
         b.spans.rec = reinterpret_cast<const uint32_t*>(d_spans);
         b.spans.n = n_spans;
         pat.fill(b.spans);
-        t->e->run_device(d_utf8, d_byte_offsets, n_sent, n_bytes, d_tok_offsets, d_tokens, n_tokens, &b);
+        run_device(t, d_utf8, d_byte_offsets, n_sent, n_bytes, &b, d_tok_offsets, d_tokens, n_tokens);
     });
 }
 
@@ -734,8 +757,9 @@ int32_t vbt_result_marginals(const vbt_result* r, const float** token_prob, cons
 
 int32_t vbt_last_device_marginals(const vbt_tokenizer* t, uint64_t* d_token_prob, uint64_t* d_path_prob) {
     return guarded([&] {
-        need(t, "t");
-        t->e->device_marginals(d_token_prob, d_path_prob);
+        const vbt::DeviceOutputs& d = last_device(t, vbt::kTokenProb, "marginals");
+        put(d_token_prob, d.addr[vbt::kTokenProb]);
+        put(d_path_prob, d.addr[vbt::kPathProb]);
     });
 }
 
@@ -756,8 +780,12 @@ int32_t vbt_result_lattice(const vbt_result* r, const uint64_t** node_offsets, c
 int32_t vbt_last_device_lattice(const vbt_tokenizer* t, uint64_t* d_node_offsets, uint64_t* d_nodes, uint64_t* d_links,
                                 uint64_t* d_node_prob, uint64_t* n_nodes) {
     return guarded([&] {
-        need(t, "t");
-        t->e->device_lattice(d_node_offsets, d_nodes, d_links, d_node_prob, n_nodes);
+        const vbt::DeviceOutputs& d = last_device(t, vbt::kNodes, "the lattice");
+        put(d_node_offsets, d.addr[vbt::kNodeOff]);
+        put(d_nodes, d.addr[vbt::kNodes]);
+        put(d_links, d.addr[vbt::kLinks]);
+        put(d_node_prob, d.addr[vbt::kNodeProb]);  // 0 without marginals
+        put(n_nodes, d.total[vbt::kGroupLattice]);
     });
 }
 
@@ -773,8 +801,7 @@ int32_t vbt_result_lattice_margins(const vbt_result* r, const int64_t** node_mar
 
 int32_t vbt_last_device_lattice_margins(const vbt_tokenizer* t, uint64_t* d_node_margin) {
     return guarded([&] {
-        need(t, "t");
-        t->e->device_lattice_margins(d_node_margin);
+        put(d_node_margin, last_device(t, vbt::kNodeMargin, "the lattice's cost margin").addr[vbt::kNodeMargin]);
     });
 }
 
@@ -800,8 +827,10 @@ int32_t vbt_result_samples(const vbt_result* r, const uint64_t** sample_offsets,
 int32_t vbt_last_device_samples(const vbt_tokenizer* t, uint64_t* d_sample_offsets, uint64_t* d_samples,
                                 uint64_t* n_sample_tokens) {
     return guarded([&] {
-        need(t, "t");
-        t->e->device_samples(d_sample_offsets, d_samples, n_sample_tokens);
+        const vbt::DeviceOutputs& d = last_device(t, vbt::kSamples, "sampling");
+        put(d_sample_offsets, d.addr[vbt::kSampleOff]);
+        put(d_samples, d.addr[vbt::kSamples]);
+        put(n_sample_tokens, d.total[vbt::kGroupSamples]);
     });
 }
 

@@ -513,33 +513,12 @@ class EngineImpl final : public Engine {
         samp_seed_ = seed;
     }
     uint32_t sampling() const override { return samp_n_; }
-    void device_samples(uint64_t* d_sample_off, uint64_t* d_samples, uint64_t* n_tokens) const override {
-        if (!made_.has(kSamples)) throw Error(kInvalidArgument, "the last device-resident call ran without sampling");
-        put_address(d_sample_off, made_, out_[0].buf, kSampleOff);
-        put_address(d_samples, made_, out_[0].buf, kSamples);
-        if (n_tokens) *n_tokens = out_[0].h_ctrl->total[kGroupSamples];
-    }
     double marginals() const override { return theta_; }
     int lattice() const override { return lattice_; }
-    void device_marginals(uint64_t* d_token_prob, uint64_t* d_path_prob) const override {
-        if (!made_.has(kTokenProb)) throw Error(kInvalidArgument, "the last device-resident call ran without marginals");
-        put_address(d_token_prob, made_, out_[0].buf, kTokenProb);
-        put_address(d_path_prob, made_, out_[0].buf, kPathProb);
+    Outputs outputs() const override {
+        return Outputs{tok_bytes_, samp_n_, theta_ > 0, output_mode_ != kOutNone, lattice_ != 0, lat_margin_ >= 0};
     }
-    void device_lattice_margins(uint64_t* d_node_margin) const override {
-        if (!made_.has(kNodeMargin))
-            throw Error(kInvalidArgument, "the last device-resident call ran without the lattice's cost margin");
-        put_address(d_node_margin, made_, out_[0].buf, kNodeMargin);
-    }
-    void device_lattice(uint64_t* d_node_off, uint64_t* d_nodes, uint64_t* d_links, uint64_t* d_node_prob,
-                        uint64_t* n_nodes) const override {
-        if (!made_.has(kNodes)) throw Error(kInvalidArgument, "the last device-resident call ran without the lattice");
-        put_address(d_node_off, made_, out_[0].buf, kNodeOff);
-        put_address(d_nodes, made_, out_[0].buf, kNodes);
-        put_address(d_links, made_, out_[0].buf, kLinks);
-        put_address(d_node_prob, made_, out_[0].buf, kNodeProb);
-        if (n_nodes) *n_nodes = out_[0].h_ctrl->total[kGroupLattice];
-    }
+    const DeviceOutputs& last_device() const override { return last_; }
     void set_stream(uint64_t stream) override {
         cudaStreamSynchronize(stream_);
         stream_ = stream ? reinterpret_cast<cudaStream_t>(stream) : own_stream_;
@@ -559,8 +538,8 @@ class EngineImpl final : public Engine {
         for (uint32_t i = 0; i < num_right_; ++i) rid[right_ids_[i]] = raw[num_left_ + i];
     }
 
-    void run_device(uint64_t d_utf8, uint64_t d_byte_off, uint64_t n_sent, uint64_t n_bytes, uint64_t* d_tok_off,
-                    uint64_t* d_tokens, uint64_t* n_tokens, const Bounds* bnd) override {
+    void run_device(uint64_t d_utf8, uint64_t d_byte_off, uint64_t n_sent, uint64_t n_bytes, const Bounds* bnd) override {
+        last_ = DeviceOutputs{};
         CK(cudaSetDevice(device_));
         check_size(n_sent, n_bytes);
         check_bounded(bnd);
@@ -584,13 +563,9 @@ class EngineImpl final : public Engine {
                 upload_patterns(bnd->spans, bd, stream_);
             }
         }
-        made_ = Outputs{};
         run_whole(reinterpret_cast<const uint8_t*>(d_utf8), reinterpret_cast<const unsigned long long*>(d_byte_off),
                   uint32_t(n_sent), n_bytes, bd);
-        *d_tok_off = reinterpret_cast<uint64_t>(out_[0].buf[kTokOff].p);
-        *d_tokens = reinterpret_cast<uint64_t>(out_[0].buf[kTokens].p);
-        *n_tokens = out_[0].h_ctrl->total[kGroupTokens];
-        made_ = out_[0].made;
+        keep_device_outputs();
     }
 
     // Host path.  Large batches are cut into chunks that flow through three streams: the H2D copy of
@@ -681,10 +656,15 @@ class EngineImpl final : public Engine {
             }
             ws_[0].stream = stream_;
             ws_[1].stream = aux_stream_;
+            // sized once: no cudaMalloc in the pipeline
+            const size_t cands = want_cand(max_chunk_bytes);
             const uint32_t n_ws = dual_stream_ ? 2 : 1;
             for (uint32_t i = 0; i < n_ws; ++i)
-                ensure_workspace(ws_[i], max_chunk_sent, max_chunk_bytes, bd.off != nullptr, bd.span_off != nullptr);  // sized once: no cudaMalloc in the pipeline
-            for (auto& o : out_) ensure_out(o, ws_[0], max_chunk_sent, max_chunk_bytes);
+                ensure_workspace(ws_[i], max_chunk_sent, max_chunk_bytes, cands, bd.off != nullptr, bd.span_off != nullptr);
+            for (int i = 0; i < 2; ++i) {  // chunk c runs in slot c & 1 and workspace c & 1 (dual_stream) or 0
+                ensure_out(out_[i], max_chunk_sent, max_chunk_bytes);
+                ensure_entries(ws_[dual_stream_ ? i : 0], out_[i], cands + max_chunk_sent + 1);
+            }
             // output stage: each slot's text buffer holds the text a chunk is expected to produce (at most 4 bytes per
             // sentence plus the learned ratio per input byte); a chunk with more text flags itself and the batch is
             // re-run with the ratio it measured
@@ -840,6 +820,7 @@ class EngineImpl final : public Engine {
     // ---- shard-level entry points (multi_engine.cu) -------------------------------------------------
     Totals run_shard(const char* utf8, const uint64_t* byte_off, uint64_t n_sent64, int src_device, uint64_t first_sentence,
                      bool with_text, const Bounds* bnd) override {
+        last_ = DeviceOutputs{};
         CK(cudaSetDevice(device_));
         const uint64_t first = n_sent64 ? byte_off[0] : 0;
         const uint64_t n_bytes = n_sent64 ? byte_off[n_sent64] - first : 0;
@@ -869,7 +850,8 @@ class EngineImpl final : public Engine {
         run_whole(in_utf8_.as<uint8_t>(), in_off_.as<unsigned long long>(), n_sent, n_bytes, bd, first_sentence);
         shard_n_sent_ = n_sent;
         if (with_text && output_mode_ != kOutNone) format_whole(in_utf8_.as<uint8_t>(), in_off_.as<unsigned long long>(), n_sent);
-        return totals(*out_[0].h_ctrl);
+        keep_device_outputs();
+        return last_.total;
     }
     void rebase_shard(const Totals& base) override {
         CK(cudaSetDevice(device_));
@@ -881,9 +863,6 @@ class EngineImpl final : public Engine {
         add_bases(base);
         place(out_[0], r, first_sentence, shard_n_sent_, totals(*out_[0].h_ctrl), base, last, stream_);
         CK(cudaStreamSynchronize(stream_));
-    }
-    void shard_arrays(uint64_t addr[kNumArrays]) const override {
-        for (int a = 0; a < kNumArrays; ++a) put_address(&addr[a], out_[0].made, out_[0].buf, a);
     }
     int device() const override { return device_; }
     uint32_t token_bytes() const override { return tok_bytes_; }
@@ -1061,9 +1040,12 @@ class EngineImpl final : public Engine {
         return h2d_ev_;
     }
 
-    // The arrays a host result carries under the current options.
-    Outputs outputs() const {
-        return Outputs{tok_bytes_, samp_n_, theta_ > 0, output_mode_ != kOutNone, lattice_ != 0, lat_margin_ >= 0};
+    // last_ = the arrays a whole batch or shard left in out_[0].
+    void keep_device_outputs() {
+        const OutSlot& o = out_[0];
+        last_.made = o.made;
+        last_.total = totals(*o.h_ctrl);
+        for (int a = 0; a < kNumArrays; ++a) last_.addr[a] = o.made.has(a) ? reinterpret_cast<uint64_t>(o.buf[a].p) : 0;
     }
     bool margin_on() const { return lattice_ && lat_margin_ >= 0; }  // the near-best lattice's kernels run
 
@@ -1092,22 +1074,14 @@ class EngineImpl final : public Engine {
     }
 
     // Device outputs of slot `o` for (chunks of) up to n_sent sentences and n_bytes bytes, except the text (sized by
-    // the output stage) and the sample records (sized by enqueue from the scanned total).
-    void ensure_out(OutSlot& o, const Workspace& w, uint32_t n_sent, uint64_t n_bytes) {
+    // the output stage), the sample records (sized by enqueue from the scanned total) and the lattice records (one
+    // per lattice entry: ensure_entries).
+    void ensure_out(OutSlot& o, uint32_t n_sent, uint64_t n_bytes) {
         o.buf[kTokOff].ensure((size_t(n_sent) + 1) * 8, 1.25);
         o.buf[kTokens].ensure(size_t(n_bytes) * 24 + 24, 1.25);  // a token spans >= 1 character >= 1 byte
         if (theta_ > 0) o.buf[kTokenProb].ensure(size_t(n_bytes) * 4 + 4, 1.25);
         if (theta_ > 0 || samp_n_) o.buf[kPathProb].ensure((size_t(n_sent) + 1) * 4, 1.25);  // the forward pass writes it
-        if (lattice_) {
-            // a node is a candidate placed in the pool, so the node arrays hold as many entries as the lattice rows of
-            // `w` (enqueue clips cand_cap to them and a larger batch takes the pool-overflow retry)
-            const size_t n = w.ends_cold.cap / 16 + 1;
-            o.buf[kNodeOff].ensure((size_t(n_sent) + 1) * 8, 1.25);
-            o.buf[kNodes].ensure(n * 24);
-            o.buf[kLinks].ensure(n * 8);
-            if (theta_ > 0) o.buf[kNodeProb].ensure(n * 4);
-            if (margin_on()) o.buf[kNodeMargin].ensure(n * 8);
-        }
+        if (lattice_) o.buf[kNodeOff].ensure((size_t(n_sent) + 1) * 8, 1.25);
         if (samp_n_) o.buf[kSampleOff].ensure((size_t(n_sent) * samp_n_ + 1) * 8, 1.25);
     }
 
@@ -1461,9 +1435,40 @@ class EngineImpl final : public Engine {
         CK(cub::DeviceScan::ExclusiveSum(w.scan_tmp.p, cap, in, out, n, w.stream));
     }
 
-    // Sizes every workspace array for batches of up to n_sent sentences / n_bytes bytes (upper
-    // bounds: characters <= bytes, one sentinel slot per sentence).
-    void ensure_workspace(Workspace& w, uint32_t n_sent, uint64_t n_bytes, bool bounded, bool spans = false) {
+    // Candidates a batch (or chunk) of n_bytes bytes is given room for, from the ratio learned on earlier batches.
+    size_t want_cand(uint64_t n_bytes) const {
+        return std::min<size_t>(std::max<size_t>(1 << 16, size_t(double(n_bytes) * cand_per_byte_) + 4096), 0xFFFFFFF0ull);
+    }
+
+    // Every array indexed by lattice entry under the current options, with its bytes per entry: f(buffer, width) for
+    // the rows of workspace w and the lattice records of slot o.  ensure_entries sizes them and enqueue bounds the
+    // pool by them, both from this one list.
+    template <typename F>
+    void per_entry(Workspace& w, OutSlot& o, F&& f) const {
+        const bool fwd = theta_ > 0 || samp_n_;  // the forward pass runs
+        f(w.ends_hot, 8);
+        f(w.ends_cold, 16);
+        if (fwd || margin_on()) {  // ... or its R-only instantiation for the near-best lattice
+            f(w.m_cand_entry, 4);
+            f(w.m_R, 8);
+        }
+        if (fwd) f(w.m_ab, 16);
+        if (samp_n_) f(w.m_lw, 4);
+        if (margin_on()) {
+            f(w.g_G, 8);
+            f(w.g_keep, 4);
+        }
+        const Outputs out = outputs();  // a lattice node is a candidate placed in the pool
+        for (int a = 0; a < kNumArrays; ++a)
+            if (kArrays[a].group == kGroupLattice && kArrays[a].kind == kRecords && out.has(a)) f(o.buf[a], out.elem_bytes(a));
+    }
+    void ensure_entries(Workspace& w, OutSlot& o, size_t entries) {
+        per_entry(w, o, [&](DevBuf& buf, size_t width) { buf.ensure(entries * width); });
+    }
+
+    // Sizes every workspace array but the per-entry ones (ensure_entries) for batches of up to n_sent sentences /
+    // n_bytes bytes (upper bounds: characters <= bytes, one sentinel slot per sentence) and `cands` candidates.
+    void ensure_workspace(Workspace& w, uint32_t n_sent, uint64_t n_bytes, size_t cands, bool bounded, bool spans) {
         const size_t ns = size_t(n_sent) + 1;
         w.n_slots.ensure(ns * 4, 1.25);
         w.slot_off.ensure(ns * 4, 1.25);
@@ -1500,22 +1505,8 @@ class EngineImpl final : public Engine {
             w.l_n_nodes.ensure(ns * 4, 1.25);
         }
         if (counting_) w.stats.ensure(ms * 16, 1.25);
-        size_t want_cand = std::max<size_t>(1 << 16, size_t(double(n_bytes) * cand_per_byte_) + 4096);
-        want_cand = std::min<size_t>(want_cand, 0xFFFFFFF0ull);
-        w.seg.ensure(want_cand * 8);  // sized like the candidates; move segments can outnumber them (overflow retry)
-        w.ends_hot.ensure((want_cand + ns) * 8);
-        w.ends_cold.ensure((want_cand + ns) * 16);
-        if (rfwd) {
-            w.m_cand_entry.ensure((want_cand + ns) * 4);
-            w.m_R.ensure((want_cand + ns) * 8);
-        }
-        if (fwd) w.m_ab.ensure((want_cand + ns) * 16);
-        if (margin_on()) {
-            w.g_G.ensure((want_cand + ns) * 8);
-            w.g_keep.ensure((want_cand + ns) * 4);
-        }
+        w.seg.ensure(cands * 8);  // sized like the candidates; move segments can outnumber them (overflow retry)
         if (samp_n_) {
-            w.m_lw.ensure((want_cand + ns) * 4);
             const size_t walks = size_t(n_sent) * samp_n_ + 1;
             w.s_cnt.ensure(walks * 4, 1.25);
             w.s_total.ensure(walks * 4, 1.25);
@@ -1545,8 +1536,10 @@ class EngineImpl final : public Engine {
         ws_[0].stream = stream_;
         batch_total_bytes_ = n_bytes;
         for (int attempt = 0;; ++attempt) {
-            ensure_workspace(ws_[0], n_sent, n_bytes, bd.off != nullptr, bd.span_off != nullptr);
-            ensure_out(o, ws_[0], n_sent, n_bytes);
+            const size_t cands = want_cand(n_bytes);
+            ensure_workspace(ws_[0], n_sent, n_bytes, cands, bd.off != nullptr, bd.span_off != nullptr);
+            ensure_out(o, n_sent, n_bytes);
+            ensure_entries(ws_[0], o, cands + n_sent + 1);
             connid_begin(stream_);
             enqueue(ws_[0], d_utf8, d_off, n_sent, n_bytes, o, nullptr, nullptr, nullptr, bd, sent_base);
             CK(cudaEventSynchronize(o.done));
@@ -1588,27 +1581,21 @@ class EngineImpl final : public Engine {
                  OutSlot& o, unsigned long long* base, cudaEvent_t base_wait, cudaEvent_t base_signal, const DevBounds& bd,
                  uint64_t sent0) {
         cudaStream_t st = w.stream;
-        o.made = Outputs{tok_bytes_, samp_n_, theta_ > 0, base && output_mode_ != kOutNone, lattice_ != 0, lat_margin_ >= 0};
+        o.made = outputs();
+        if (!base) o.made.text = false;  // whole batches and shards are formatted by format_whole
         // characters <= bytes is the hard bound; the per-character launches are sized from the ratio learned on
         // earlier batches (plus slack), and a batch that exceeds it flags itself and is re-run with the hard bound
         const uint32_t hard_slots = uint32_t(n_bytes + n_sent);
         const uint32_t max_slots = uint32_t(std::min<uint64_t>(hard_slots, uint64_t(double(n_bytes) * chars_per_byte_) + n_sent + 4096));
-        size_t cap_all = std::min<size_t>(0xFFFFFFF0ull, std::min<size_t>(w.ends_hot.cap / 8 - n_sent - 1, w.ends_cold.cap / 16 - n_sent - 1));
-        const bool marg = theta_ > 0, samp = samp_n_ != 0;
-        if (marg || samp)
-            cap_all = std::min<size_t>(cap_all, std::min<size_t>(w.m_cand_entry.cap / 4,
-                                                                 std::min<size_t>(w.m_R.cap / 8, w.m_ab.cap / 16)) - n_sent - 1);
-        if (samp) cap_all = std::min<size_t>(cap_all, w.m_lw.cap / 4 - n_sent - 1);
-        const bool lat = lattice_ != 0, mlat = margin_on();
-        if (mlat)
-            cap_all = std::min<size_t>(cap_all, std::min<size_t>({w.m_cand_entry.cap / 4, w.m_R.cap / 8, w.g_G.cap / 8,
-                                                                  w.g_keep.cap / 4}) - n_sent - 1);
-        if (lat) {  // nodes <= candidates placed: the node arrays bound the pool too
-            cap_all = std::min<size_t>(cap_all, std::min<size_t>(o.buf[kNodes].cap / 24, o.buf[kLinks].cap / 8));
-            if (marg) cap_all = std::min<size_t>(cap_all, o.buf[kNodeProb].cap / 4);
-            if (mlat) cap_all = std::min<size_t>(cap_all, o.buf[kNodeMargin].cap / 8);
-        }
+        // the candidates the pool may take: every per-entry array also holds one EOS entry per sentence
+        size_t cap_all = 0xFFFFFFF0ull;
+        per_entry(w, o, [&](const DevBuf& buf, size_t width) {
+            const size_t rows = buf.cap / width;
+            cap_all = std::min<size_t>(cap_all, rows > n_sent ? rows - n_sent - 1 : 0);
+        });
         const uint32_t cand_cap = uint32_t(cap_all);
+        const bool marg = theta_ > 0, samp = samp_n_ != 0;
+        const bool lat = lattice_ != 0, mlat = margin_on();
         Batch b{};
         b.utf8 = d_utf8;
         b.byte_off = d_off;
@@ -1885,7 +1872,7 @@ class EngineImpl final : public Engine {
     bool sample_text_ = false;  // option "sample_text": the output text renders the samples
     static constexpr long long kMaxSampleBase = 0x100000000ll;
     uint64_t sample_base_ = 0;  // option "sample_base": the draws' index of the call's first sentence
-    Outputs made_;  // the arrays the last run_device produced (device_marginals, _lattice, _samples)
+    DeviceOutputs last_;  // what the last run_device or run_shard left in out_[0] (last_device)
     float stage_ms_[kNumStages];
     uint64_t launches_ = 0;
     uint32_t last_route_ = kRouteNone;  // ViterbiRoute of the last successful call (describe())

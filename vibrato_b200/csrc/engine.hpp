@@ -102,10 +102,12 @@ struct DevBuf {
     }
 };
 
-// *dst = the device address of array a in buf[kNumArrays], 0 when `made` lacks it; nothing for a null dst.
-inline void put_address(uint64_t* dst, const Outputs& made, const DevBuf* buf, int a) {
-    if (dst) *dst = made.has(a) ? reinterpret_cast<uint64_t>(buf[a].p) : 0;
-}
+// What the last run_device (on a shard engine: run_shard) left in device memory, valid until the next call.
+struct DeviceOutputs {
+    Outputs made{};                  // the arrays it produced
+    Totals total{};                  // records per group
+    uint64_t addr[kNumArrays] = {};  // device address of array a, 0 when !made.has(a)
+};
 
 struct HostResult {  // one batch's outputs in pinned host memory
     uint64_t n_sent = 0;
@@ -174,10 +176,12 @@ class Engine {
                                                 bool ignore_space, uint64_t max_grouping_len);
     virtual ~Engine() = default;
 
-    // Inputs/outputs in device memory; outputs owned by the engine until the next call.
+    // Inputs/outputs in device memory; outputs owned by the engine until the next call, described by last_device().
     // With bnd: a bounded batch, its boundary arrays in device memory too.  Bounded batches refuse "counting".
-    virtual void run_device(uint64_t d_utf8, uint64_t d_byte_off, uint64_t n_sent, uint64_t n_bytes,
-                            uint64_t* d_tok_off, uint64_t* d_tokens, uint64_t* n_tokens, const Bounds* bnd = nullptr) = 0;
+    virtual void run_device(uint64_t d_utf8, uint64_t d_byte_off, uint64_t n_sent, uint64_t n_bytes, const Bounds* bnd = nullptr) = 0;
+    // The arrays the last run_device (or run_shard) left in device memory.  After a run_device that failed, `made`
+    // holds no optional array; run_host leaves the record alone.
+    virtual const DeviceOutputs& last_device() const = 0;
     // Inputs/outputs in host memory (copies inside); bnd in host memory.
     virtual HostResult* run_host(const char* utf8, const uint64_t* byte_off, uint64_t n_sent, const Bounds* bnd = nullptr) = 0;
     virtual void release(HostResult* r) = 0;
@@ -188,7 +192,7 @@ class Engine {
     // byte_off is still a host array.  first_sentence is the caller's index of the shard's first sentence (the i of the
     // sampling draws), so that a shard draws what the whole batch would.  With with_text the shard's output text is
     // formatted too, when an output mode or format is set.  bnd (host memory, may be null) holds the shard's
-    // n_sent + 1 boundary offsets.
+    // n_sent + 1 boundary offsets.  last_device() then describes the shard's arrays.
     virtual Totals run_shard(const char* utf8, const uint64_t* byte_off, uint64_t n_sent, int src_device,
                              uint64_t first_sentence, bool with_text, const Bounds* bnd = nullptr) = 0;
     // rebase_shard: adds base[g] to the last shard's offsets of every group g it produced, on the device.
@@ -196,8 +200,6 @@ class Engine {
     // fetch_shard: rebases the last shard like rebase_shard, then copies every array r carries into r at the shard's
     // place: sentence first_sentence and records after base[g] others (the closing offsets too when `last`).
     virtual void fetch_shard(HostResult* r, uint64_t first_sentence, const Totals& base, bool last) = 0;
-    // Device address of each array of the last shard, 0 for an array it did not produce.
-    virtual void shard_arrays(uint64_t addr[kNumArrays]) const = 0;
     virtual int device() const = 0;
     virtual uint32_t token_bytes() const = 0;  // 24, or 16 with the "compact_tokens" option
     virtual std::string describe() const = 0;  // JSON: devices, how the dictionary travelled, ...
@@ -214,32 +216,20 @@ class Engine {
     // An output format (format.hpp) in place of "output_mode" 1-3, on every host route; nullptr switches it off.
     // Setting "output_mode" replaces it.  Builds the format's field table on the device.
     virtual void set_format(const FormatProgram* p) = 0;
+    // The arrays a host result carries under the current options.
+    virtual Outputs outputs() const = 0;
     // Marginal probabilities (kernels.cuh MargArgs) at temperature theta > 0 on every route except k_small_batch,
     // which steps aside while they are on; 0 switches them off.  Results then carry kTokenProb / kPathProb (and
-    // kNodeProb with the lattice), and run_device leaves them in device memory (device_marginals).
+    // kNodeProb with the lattice), and run_device leaves them in device memory (last_device).
     virtual void set_marginals(double theta) = 0;
     virtual double marginals() const = 0;
     virtual int lattice() const = 0;  // the option "lattice"
     // Segmentation sampling (kernels.cuh SampleArgs): n (1..1024) paths per sentence drawn from P(path) at temperature
     // theta (> 0, finite; the marginals' theta when they are on), with Philox keyed by seed; n = 0 switches it off.
     // On every route except k_small_batch, which steps aside.  Results then carry kSampleOff / kSamples, and
-    // run_device leaves them in device memory (device_samples).
+    // run_device leaves them in device memory (last_device).
     virtual void set_sampling(uint32_t n, double theta, uint64_t seed) = 0;
     virtual uint32_t sampling() const = 0;  // n, 0 when off
-    // Device addresses of the last run_device's uint64 sample_off[n_sent * n + 1] and vbt_token samples[n_tokens];
-    // valid until the next call.  Throws when that call ran without sampling.
-    virtual void device_samples(uint64_t* d_sample_off, uint64_t* d_samples, uint64_t* n_tokens) const = 0;
-    // Device addresses of the last run_device's float token_prob[n_tokens] and path_prob[n_sent]; valid until the
-    // next call.  Throws when that call ran without marginals.
-    virtual void device_marginals(uint64_t* d_token_prob, uint64_t* d_path_prob) const = 0;
-    // Device addresses of the last run_device's lattice (option "lattice" >= 1): uint64 node_off[n_sent + 1],
-    // vbt_token nodes[n_nodes], vbt_lattice_link links[n_nodes] and float node_prob[n_nodes] (0 without marginals);
-    // valid until the next call.  Throws when that call ran without the lattice.
-    virtual void device_lattice(uint64_t* d_node_off, uint64_t* d_nodes, uint64_t* d_links, uint64_t* d_node_prob,
-                                uint64_t* n_nodes) const = 0;
-    // Device address of the last run_device's int64 node_margin[n_nodes] ("lattice_margin" >= 0); valid until the next
-    // call.  Throws when that call ran without the lattice or without the margin.
-    virtual void device_lattice_margins(uint64_t* d_node_margin) const = 0;
     // Launch on a caller-owned CUDA stream (0 restores the engine's own stream).
     virtual void set_stream(uint64_t stream) = 0;
     virtual const float* stage_ms() const = 0;

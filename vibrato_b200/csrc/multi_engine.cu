@@ -234,15 +234,16 @@ class MultiEngine final : public Engine {
         }
         check_samples(n_sent);
         const std::vector<uint64_t> cut = split_by_bytes(byte_off, n_sent, n);
+        const Outputs out = outputs();
         std::vector<Totals> count(n);
         run_on_all([&](int i) {
             const Bounds sb = shard_bounds(bnd, cut[i]);  // the draws of sentence k are those of the whole batch
-            count[i] = eng_[i]->run_shard(utf8, byte_off + cut[i], cut[i + 1] - cut[i], -1, cut[i], text_, bnd ? &sb : nullptr);
+            count[i] = eng_[i]->run_shard(utf8, byte_off + cut[i], cut[i + 1] - cut[i], -1, cut[i], out.text, bnd ? &sb : nullptr);
         });
         // every shard's outputs are copied straight to their final positions; the last shard, even when it is empty,
         // also delivers the closing offsets
         const std::vector<Totals> base = prefix_sums(count);
-        HostResult* r = pool_.acquire(outputs(), n_sent, base[n]);
+        HostResult* r = pool_.acquire(out, n_sent, base[n]);
         run_on_all([&](int i) { eng_[i]->fetch_shard(r, cut[i], base[i], i == n - 1); });
         collect_stats();
         return r;
@@ -256,16 +257,15 @@ class MultiEngine final : public Engine {
     }
 
     // ---- device-resident batches: input on the first device, results gathered back to it ------------------
-    void run_device(uint64_t d_utf8, uint64_t d_byte_off, uint64_t n_sent, uint64_t n_bytes, uint64_t* d_tok_off,
-                    uint64_t* d_tokens, uint64_t* n_tokens, const Bounds* bnd) override {
+    void run_device(uint64_t d_utf8, uint64_t d_byte_off, uint64_t n_sent, uint64_t n_bytes, const Bounds* bnd) override {
         const int n = int(dev_.size());
         if (n == 1) {
-            eng_[0]->run_device(d_utf8, d_byte_off, n_sent, n_bytes, d_tok_off, d_tokens, n_tokens, bnd);
+            eng_[0]->run_device(d_utf8, d_byte_off, n_sent, n_bytes, bnd);
             collect_stats();
             return;
         }
+        last_ = DeviceOutputs{};
         check_samples(n_sent);
-        made_ = Outputs{};
         CK(cudaSetDevice(dev_[0]));
         // the split needs the offsets on the host (pinned staging buffer, one copy); their validity is checked on
         // the devices like for any device-resident batch (k_count_chars)
@@ -323,8 +323,7 @@ class MultiEngine final : public Engine {
             uint64_t bytes;
         };
         auto pieces = [&](int i) {
-            uint64_t src[kNumArrays];
-            eng_[i]->shard_arrays(src);
+            const uint64_t* src = eng_[i]->last_device().addr;
             std::vector<Piece> v;
             for (int a = 0; a < kNumArrays; ++a) {
                 const uint64_t bytes = out.has(a) ? out.bytes(a, cut[i + 1] - cut[i], count[i], i == n - 1) : 0;
@@ -354,12 +353,11 @@ class MultiEngine final : public Engine {
             CK(cudaStreamSynchronize(stream_[i]));
         }
         collect_stats();
-        *d_tok_off = reinterpret_cast<uint64_t>(gather_[kTokOff].p);
-        *d_tokens = reinterpret_cast<uint64_t>(gather_[kTokens].p);
-        *n_tokens = base[n][kGroupTokens];
-        made_ = out;
-        made_total_ = base[n];
+        last_.made = out;
+        last_.total = base[n];
+        for (int a = 0; a < kNumArrays; ++a) last_.addr[a] = out.has(a) ? reinterpret_cast<uint64_t>(gather_[a].p) : 0;
     }
+    const DeviceOutputs& last_device() const override { return dev_.size() == 1 ? eng_[0]->last_device() : last_; }
 
     // ---- everything else is forwarded ------------------------------------------------------------------
     void set_counting(bool on) override {
@@ -368,22 +366,17 @@ class MultiEngine final : public Engine {
     void set_option(const std::string& name, long long value) override {
         if (name == "chunk_sentences") return;  // shards are not chunked (see the constructor)
         for (auto& e : eng_) e->set_option(name, value);
-        if (name == "lattice") lattice_ = int(value);
-        if (name == "lattice_margin") lat_margin_ = value;
         if (name == "sample_base") sample_base_ = uint64_t(value);
-        if (name == "output_mode") text_ = fixed_mode_ = value != 0;
     }
     void set_format(const FormatProgram* p) override {
         try {
             for (auto& e : eng_) e->set_format(p);  // each device builds its own field table
         } catch (...) {
             for (auto& e : eng_) e->set_format(nullptr);
-            text_ = fixed_mode_;
             throw;
         }
-        if (p) fixed_mode_ = false;  // the format replaced it
-        text_ = p != nullptr || fixed_mode_;
     }
+    Outputs outputs() const override { return eng_[0]->outputs(); }
     void set_marginals(double theta) override {
         for (auto& e : eng_) e->set_marginals(theta);
     }
@@ -392,36 +385,7 @@ class MultiEngine final : public Engine {
         for (auto& e : eng_) e->set_sampling(n, theta, seed);  // the first refuses what all would
     }
     uint32_t sampling() const override { return eng_[0]->sampling(); }
-    void device_samples(uint64_t* d_sample_off, uint64_t* d_samples, uint64_t* n_tokens) const override {
-        if (dev_.size() == 1) return eng_[0]->device_samples(d_sample_off, d_samples, n_tokens);
-        if (!made_.has(kSamples)) throw Error(kInvalidArgument, "the last device-resident call ran without sampling");
-        put_address(d_sample_off, made_, gather_, kSampleOff);
-        put_address(d_samples, made_, gather_, kSamples);
-        if (n_tokens) *n_tokens = made_total_[kGroupSamples];
-    }
-    int lattice() const override { return lattice_; }
-    void device_marginals(uint64_t* d_token_prob, uint64_t* d_path_prob) const override {
-        if (dev_.size() == 1) return eng_[0]->device_marginals(d_token_prob, d_path_prob);
-        if (!made_.has(kTokenProb)) throw Error(kInvalidArgument, "the last device-resident call ran without marginals");
-        put_address(d_token_prob, made_, gather_, kTokenProb);
-        put_address(d_path_prob, made_, gather_, kPathProb);
-    }
-    void device_lattice(uint64_t* d_node_off, uint64_t* d_nodes, uint64_t* d_links, uint64_t* d_node_prob,
-                        uint64_t* n_nodes) const override {
-        if (dev_.size() == 1) return eng_[0]->device_lattice(d_node_off, d_nodes, d_links, d_node_prob, n_nodes);
-        if (!made_.has(kNodes)) throw Error(kInvalidArgument, "the last device-resident call ran without the lattice");
-        put_address(d_node_off, made_, gather_, kNodeOff);
-        put_address(d_nodes, made_, gather_, kNodes);
-        put_address(d_links, made_, gather_, kLinks);
-        put_address(d_node_prob, made_, gather_, kNodeProb);
-        if (n_nodes) *n_nodes = made_total_[kGroupLattice];
-    }
-    void device_lattice_margins(uint64_t* d_node_margin) const override {
-        if (dev_.size() == 1) return eng_[0]->device_lattice_margins(d_node_margin);
-        if (!made_.has(kNodeMargin))
-            throw Error(kInvalidArgument, "the last device-resident call ran without the lattice's cost margin");
-        put_address(d_node_margin, made_, gather_, kNodeMargin);
-    }
+    int lattice() const override { return eng_[0]->lattice(); }
     void set_stream(uint64_t stream) override {
         if (stream) throw Error(kUnsupported, "a multi-device tokenizer runs on its own streams");
     }
@@ -448,7 +412,6 @@ class MultiEngine final : public Engine {
     }
     void rebase_shard(const Totals&) override { throw Error(kInternal, "not a shard engine"); }
     void fetch_shard(HostResult*, uint64_t, const Totals&, bool) override { throw Error(kInternal, "not a shard engine"); }
-    void shard_arrays(uint64_t*) const override { throw Error(kInternal, "not a shard engine"); }
     int device() const override { return dev_[0]; }
     uint32_t token_bytes() const override { return eng_[0]->token_bytes(); }
     std::string describe() const override {
@@ -540,9 +503,6 @@ class MultiEngine final : public Engine {
         }
     }
 
-    // The arrays a host result carries under the current options.
-    Outputs outputs() const { return Outputs{token_bytes(), sampling(), marginals() > 0, text_, lattice_ != 0, lat_margin_ >= 0}; }
-
     // base[i][g] = the records of group g in the shards before shard i (base[n] = all of them).
     static std::vector<Totals> prefix_sums(const std::vector<Totals>& count) {
         std::vector<Totals> base(count.size() + 1, Totals{});
@@ -560,8 +520,6 @@ class MultiEngine final : public Engine {
     std::vector<std::unique_ptr<Engine>> eng_;
     std::string transport_;
     ResultPool pool_;
-    bool text_ = false;  // "output_mode" or an output format is on: host results carry the formatted text
-    bool fixed_mode_ = false;  // "output_mode" 1-3 is on
     uint64_t* h_off_ = nullptr;  // pinned
     size_t h_off_cap_ = 0;
     void* h_bnd_off_ = nullptr;  // pinned: the boundary lists of a device-resident batch, cut into shards on the host
@@ -571,10 +529,7 @@ class MultiEngine final : public Engine {
     void* h_span_ = nullptr;
     size_t h_span_off_cap_ = 0, h_span_cap_ = 0;
     DevBuf gather_[kNumArrays];  // the outputs of a gathered device-resident batch, on the first device
-    Outputs made_;               // the arrays the last device-resident call produced
-    Totals made_total_{};
-    int lattice_ = 0;  // option "lattice"
-    long long lat_margin_ = -1;  // option "lattice_margin"
+    DeviceOutputs last_;         // what the last device-resident call gathered there (last_device)
     uint64_t sample_base_ = 0;  // option "sample_base" (every engine adds it to its shard's first sentence)
     float stage_ms_[kNumStages];
     uint64_t counters_[10];
