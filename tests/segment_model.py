@@ -36,22 +36,32 @@ def lex_type(x):
     return 1 if x & USER else 2 if x & UNK else 0
 
 
-def sources(cands):
-    """cands: [(end, word_idx)] of one position in insertion order -> [(lex type, end, [word_idx...])]."""
+def follows(prev, widx):
+    """Does word_idx `widx` come right after `prev` in its postings list (word ids are consecutive there: see
+    test_span_limits_model) or in unk.def (the 16-bit entry index, mod 2^16)?"""
+    if widx >> 30 == 2:
+        return widx & 0xFFFF == (prev + 1) & 0xFFFF
+    return widx == prev + 1
+
+
+def sources(cands, spans=False):
+    """cands: [(end, word_idx)] of one position in insertion order -> [(lex type, end, [word_idx...])].  spans: a
+    source also breaks where a record is skipped (span_postings and count_span push one segment per run of records
+    that match a span's pattern)."""
     out = []
     for end, widx in cands:
         lt = widx >> 30
-        if out and out[-1][0] == lt and out[-1][1] == end:
+        if out and out[-1][0] == lt and out[-1][1] == end and (not spans or follows(out[-1][2][-1], widx)):
             out[-1][2].append(widx)
         else:
             out.append((lt, end, [widx]))
     return out
 
 
-def encode(slot, cands):
+def encode(slot, cands, spans=False):
     """SegOut::push over the sources of the position at `slot` -> (segments [(x, y)], image)."""
     segs, image, last = [], [], slot
-    for lt, end, words in sources(cands):
+    for lt, end, words in sources(cands, spans):
         if lt == 2:
             v = UNK | len(image)
         else:

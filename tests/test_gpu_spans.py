@@ -11,6 +11,7 @@ import vibrato_b200 as vb
 from span_oracle import Constraints, SpanOracle, constraints, csv_fields
 from oracle import vibrato_oracle as vo
 from test_gpu_bounded import CHUNK_COPIES, d2h, golden_dicts, lead_bytes, make_tokenizer, skip_multi
+from test_gpu_sampling import check_parity
 
 pytestmark = pytest.mark.gpu
 ROUTES = ("whole", "chunked", "small", "device", "multi", "multi_device")
@@ -219,8 +220,8 @@ def test_invariants(golden):
 
 
 def test_downstream(golden):
-    """Marginals, lattice and samples over the span lattice; each span's nodes carry probability 1 in total, and every
-    sample holds each span's token."""
+    """Marginals, lattice and samples over the span lattice; each span's nodes carry probability 1 in total, every
+    sample holds each span's token, and the samples equal the sampling restatement's byte for byte."""
     d, od, r = golden_dicts(golden, True)
     so = SpanOracle(od, r["char.def"], r["unk.def"])
     sents = [c["input"] for c in golden["tokenizer_cases"]] + GOLDEN_EXTRA
@@ -252,6 +253,7 @@ def test_downstream(golden):
             smp = res.samples[int(res.sample_offsets[k]):int(res.sample_offsets[k + 1])]
             for a, e, *_ in recs:
                 assert sum(1 for x in smp if x["start_byte"] == a and x["end_byte"] == e) == 1
+    check_parity(so, sents, (res.sample_offsets, res.samples), 4, theta, 5, bounds=cons)
 
 
 def test_output_and_counts(golden):
