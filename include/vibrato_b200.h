@@ -393,6 +393,38 @@ int32_t vbt_result_marginals(const vbt_result *r, const float **token_prob, cons
 /* Device addresses (float32) of the marginals of the last vbt_tokenize_batch_device{,_bounded} call, valid until the
  * next call; VBT_ERR_INVALID_ARGUMENT when it ran without marginals. */
 int32_t vbt_last_device_marginals(const vbt_tokenizer *t, uint64_t *d_token_prob, uint64_t *d_path_prob);
+/* Segmentation uncertainty, the option "uncertainty" of vbt_tokenizer_set_option: 0 off (default); 1 every result
+ * also carries entropy and log_path_prob per sentence; 2 also the boundary probabilities of every character position.
+ * Lattice, edges, exact int64 path costs, theta and P(path) are those of the marginals above (over the constrained
+ * lattice in bounded and span calls); â / b̂ / â(EOS) / R(EOS) as in the marginals' forward-backward pass.
+ *   entropy[s] (float64, nats) = -sum over paths of P ln P = ln Z + theta * E[cost], computed as
+ *   â(EOS) + theta * E[delta]: every edge k -> c (c = EOS included, with R(EOS) in place of R(c)) has the slack
+ *   delta = R(k) + cost(k -> c) - R(c) >= 0 against the prefix minima R, which telescopes along a path to
+ *   cost - R(EOS); E[delta] = sum over edges of P(edge) delta(edge).  Both terms are sums of non-negative values.
+ *   An empty sentence, or one without a path, gives 0.
+ *   log_path_prob[s] (float64) = -â(EOS) = ln(exp(-theta * min cost) / Z) <= 0, the log form of path_prob (which
+ *   underflows to 0 past about 103 nats); path_prob[s] == float32(exp(log_path_prob[s])) to 1 float32 ulp.  An empty
+ *   sentence gives 0, one without a path -inf.
+ *   Boundary probabilities (level 2): boundary_offsets[n_sent + 1] (the slot offsets) index boundary_prob (float32);
+ *   sentence s owns n_chars + 1 entries, one per character position p = 0..n.  Entry p = P(some token of the path
+ *   ends at p) = the sum of the marginals of the nodes of ends[p], summed in float64 in row order and rounded once;
+ *   1 at p = 0 (BOS).  A sentence without a path has all entries 0, an empty sentence one entry, 1.  So a required
+ *   boundary or span end has an entry within 2 ulps of 1, every position strictly inside a span 0, positions the sweep
+ *   skips 0, and the sum over p >= 1 is the expected number of tokens.
+ * Every sum runs in a fixed order: all three arrays are bit-identical across routes, chunk sizes, sentence orders, K3
+ * variants and device counts.  A non-zero value while marginals are off, switching marginals off while it is on, or a
+ * value outside 0..2: VBT_ERR_INVALID_ARGUMENT.  Level 1 runs the marginals' backward pass in an instantiation that
+ * also sums P * delta; level 2 adds one kernel launch (both booked under "viterbi").  The "small_batch" route steps
+ * aside while it is on.  Multi-device tokenizers give the bytes of one device. */
+/* entropy[n_sent], log_path_prob[n_sent] and, at level 2, boundary_offsets[n_sent + 1] into boundary_prob (NULL at
+ * level 1) of a result made with "uncertainty"; owned by the result.  VBT_ERR_INVALID_ARGUMENT for a result made
+ * without it. */
+int32_t vbt_result_uncertainty(const vbt_result *r, const double **entropy, const double **log_path_prob,
+                               const uint64_t **boundary_offsets, const float **boundary_prob);
+/* Device addresses of the same arrays of the last vbt_tokenize_batch_device* call (boundary arrays 0 and n_positions 0
+ * at level 1), valid until the next call; VBT_ERR_INVALID_ARGUMENT when it ran without the option. */
+int32_t vbt_last_device_uncertainty(const vbt_tokenizer *t, uint64_t *d_entropy, uint64_t *d_log_path_prob,
+                                    uint64_t *d_boundary_offsets, uint64_t *d_boundary_prob, uint64_t *n_positions);
 /* Lattice output, the option "lattice" of vbt_tokenizer_set_option: 0 off (default); 1 every result also carries
  * every node of each sentence's lattice; 2 the same, and the output text ("output_mode" 1-3 or a format) renders the
  * nodes in place of the tokens, like MeCab's -a (BOS / EOS formats still print once per sentence).  Multi-device

@@ -72,6 +72,8 @@ extern "C" {
     fn vbt_result_lattice(r: *const vbt_result, node_offsets: *mut *const u64, nodes: *mut *const vbt_token,
                           links: *mut *const vbt_lattice_link, node_prob: *mut *const f32, n_nodes: *mut u64) -> i32;
     fn vbt_result_lattice_margins(r: *const vbt_result, node_margin: *mut *const i64) -> i32;
+    fn vbt_result_uncertainty(r: *const vbt_result, entropy: *mut *const f64, log_path_prob: *mut *const f64,
+                              boundary_offsets: *mut *const u64, boundary_prob: *mut *const f32) -> i32;
     fn vbt_evaluate(d: *const vbt_dict, t: *mut vbt_tokenizer, corpus: *const c_char, len: usize,
                     feature_indices: *const u64, n_indices: usize, num_ref: *mut u64, num_sys: *mut u64,
                     num_cor: *mut u64) -> i32;
@@ -280,6 +282,12 @@ impl Tokenizer {
         let opt = b"lattice_margin\0".as_ptr() as *const c_char;
         check(unsafe { vbt_tokenizer_set_option(self.handle(), opt, d.unwrap_or(-1)) })
     }
+    /// Segmentation uncertainty (option "uncertainty"; needs `marginals`): batches tokenised afterwards carry
+    /// `BatchResult::uncertainty`; `boundary_probs` also carries each character position's boundary probability.
+    pub fn uncertainty(&self, on: bool, boundary_probs: bool) -> Result<()> {
+        let v = if !on { 0 } else if boundary_probs { 2 } else { 1 };
+        check(unsafe { vbt_tokenizer_set_option(self.handle(), b"uncertainty\0".as_ptr() as *const c_char, v) })
+    }
     /// Segmentation sampling (see `vbt_tokenizer_set_sampling`): `n` (1..1024, 0 = off) paths per sentence drawn from
     /// P(path) at temperature `theta`, keyed by `seed`; batches tokenised afterwards carry `BatchResult::samples`.
     /// `text`: the output text renders each sentence's `n` samples in place of its best path (option "sample_text").
@@ -402,6 +410,26 @@ impl BatchResult {
         check(unsafe { vbt_result_lattice_margins(self.r, &mut m) })?;
         let n = self.lattice()?.1.len();
         Ok(if n == 0 { &[] } else { unsafe { std::slice::from_raw_parts(m, n) } })
+    }
+    /// (entropy, log_path_prob, Some((boundary offsets, boundary probabilities)) or None without boundary
+    /// probabilities): sentence i's positions 0..n are `probs[offsets[i]..offsets[i + 1]]`; an error for a batch
+    /// tokenised without `Tokenizer::uncertainty`.
+    pub fn uncertainty(&self) -> Result<(&[f64], &[f64], Option<(&[u64], &[f32])>)> {
+        let (mut e, mut l, mut o, mut b) = (std::ptr::null(), std::ptr::null(), std::ptr::null(), std::ptr::null());
+        check(unsafe { vbt_result_uncertainty(self.r, &mut e, &mut l, &mut o, &mut b) })?;
+        let (mut to, mut t, mut ns, mut nt) = (std::ptr::null(), std::ptr::null(), 0u64, 0u64);
+        unsafe {
+            vbt_result_view(self.r, &mut to, &mut t, &mut ns, &mut nt);
+            let f = |p: *const f64| if ns == 0 { &[][..] } else { std::slice::from_raw_parts(p, ns as usize) };
+            let bnd = if o.is_null() {
+                None
+            } else {
+                let off = std::slice::from_raw_parts(o, ns as usize + 1);
+                let n = off[ns as usize] as usize;
+                Some((off, if n == 0 { &[][..] } else { std::slice::from_raw_parts(b, n) }))
+            };
+            Ok((f(e), f(l), bnd))
+        }
     }
     /// (sample offsets, sampled tokens): sample j of sentence i is `samples[offsets[i * n + j]..offsets[i * n + j + 1]]`;
     /// an error for a batch tokenised without sampling.

@@ -114,6 +114,8 @@ def lib():
     sig("vbt_last_device_marginals", i32, [vp, C.POINTER(u64), C.POINTER(u64)])
     sig("vbt_result_lattice", i32, [vp, pp, pp, pp, pp, C.POINTER(u64)])
     sig("vbt_last_device_lattice", i32, [vp] + [C.POINTER(u64)] * 5)
+    sig("vbt_result_uncertainty", i32, [vp, pp, pp, pp, pp])
+    sig("vbt_last_device_uncertainty", i32, [vp] + [C.POINTER(u64)] * 5)
     sig("vbt_result_lattice_margins", i32, [vp, pp])
     sig("vbt_last_device_lattice_margins", i32, [vp, C.POINTER(u64)])
     sig("vbt_tokenizer_set_sampling", i32, [vp, C.c_uint32, C.c_double, u64])

@@ -284,10 +284,13 @@ class BatchResult:
     the near-best ones and `node_margins` (int64) holds each one's exact cost margin; None otherwise.  With
     Tokenizer.sampling(n, theta) on,
     `sample_offsets[i * n + j]..sample_offsets[i * n + j + 1]` index `samples` (TOKEN_DTYPE): sample j of sentence i
-    (sentence_samples()); both are None otherwise."""
+    (sentence_samples()); both are None otherwise.  With Tokenizer.uncertainty() on, `entropies` and `log_path_probs`
+    (float64[n_sent]) hold each sentence's path entropy (nats) and best-path log-probability, and with
+    boundary_probs=True `boundary_offsets[i]..boundary_offsets[i+1]` index `boundary_probs` (float32): the probability
+    that a token ends at each character position 0..n of sentence i (sentence_boundary_probs()); None otherwise."""
 
     def __init__(self, tokenizer, handle, sentences_utf8, byte_offsets, compact=False, marginals=False, lattice=False,
-                 samples=0, margins=False):
+                 samples=0, margins=False, uncertainty=0):
         self._tok = tokenizer
         self._h = handle
         self._free = lib().vbt_result_free
@@ -332,6 +335,20 @@ class BatchResult:
                 check(lib().vbt_result_lattice_margins(handle, C.byref(pm)))
                 self.node_margins = (np.ctypeslib.as_array(C.cast(pm, C.POINTER(C.c_int64)), shape=(n,)) if n
                                      else np.empty(0, dtype=np.int64))
+        self.entropies = self.log_path_probs = self.boundary_offsets = self.boundary_probs = None
+        if uncertainty:
+            pe, pl, po, pb = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_void_p()
+            check(lib().vbt_result_uncertainty(handle, C.byref(pe), C.byref(pl), C.byref(po), C.byref(pb)))
+            f64 = C.POINTER(C.c_double)
+            n = self.n_sent
+            self.entropies = np.ctypeslib.as_array(C.cast(pe, f64), shape=(n,)) if n else np.empty(0, dtype=np.float64)
+            self.log_path_probs = (np.ctypeslib.as_array(C.cast(pl, f64), shape=(n,)) if n
+                                   else np.empty(0, dtype=np.float64))
+            if uncertainty >= 2:
+                self.boundary_offsets = np.ctypeslib.as_array(C.cast(po, C.POINTER(C.c_uint64)), shape=(n + 1,))
+                npos = int(self.boundary_offsets[n])
+                self.boundary_probs = (np.ctypeslib.as_array(C.cast(pb, C.POINTER(C.c_float)), shape=(npos,)) if npos
+                                       else np.empty(0, dtype=np.float32))
         self.n_samples = int(samples)  # samples per sentence, 0 without sampling
         self.sample_offsets = self.samples = None
         if samples:
@@ -355,7 +372,8 @@ class BatchResult:
             if self.token_probs is not None:
                 self.token_probs = self.token_probs.copy()
                 self.path_probs = self.path_probs.copy()
-            for name in ("node_offsets", "nodes", "node_links", "node_probs", "node_margins", "sample_offsets", "samples"):
+            for name in ("node_offsets", "nodes", "node_links", "node_probs", "node_margins", "sample_offsets", "samples",
+                         "entropies", "log_path_probs", "boundary_offsets", "boundary_probs"):
                 if getattr(self, name) is not None:
                     setattr(self, name, getattr(self, name).copy())
             self._free(h)
@@ -401,6 +419,14 @@ class BatchResult:
         return [[Token(self._tok, s, self.samples[k]) for k in range(int(so[i * n + j]), int(so[i * n + j + 1]))]
                 for j in range(n)]
 
+    def sentence_boundary_probs(self, i):
+        """float32[n_chars + 1]: P(a token ends at character position p) for p = 0..n of sentence i (needs
+        Tokenizer.uncertainty(boundary_probs=True))."""
+        if self.boundary_probs is None:
+            raise VibratoError(1, "no boundary probabilities: switch them on with "
+                                  "Tokenizer.uncertainty(boundary_probs=True) before tokenising")
+        return self.boundary_probs[int(self.boundary_offsets[i]):int(self.boundary_offsets[i + 1])]
+
     def sentence_nodes(self, i):
         """LatticeNode views of sentence i's lattice, in node order (needs Tokenizer.lattice())."""
         if self.nodes is None:
@@ -431,6 +457,7 @@ class Tokenizer:
         self._theta = 0.0  # marginals(), replayed before the format
         self._lattice = 0  # lattice(), replayed before the format
         self._lattice_margin = -1  # lattice(margin=D), replayed with it
+        self._uncertainty = 0  # uncertainty(), replayed after the marginals
         self._sampling = (0, 0.0, 0)  # sampling() as (n, theta, seed), replayed after the marginals
         self._sample_text = False  # sampling(text=True), replayed after sampling
         self._stream = 0
@@ -498,6 +525,8 @@ class Tokenizer:
                 check(lib().vbt_tokenizer_set_option(h, b"lattice", self._lattice))
             if self._lattice_margin >= 0:
                 check(lib().vbt_tokenizer_set_option(h, b"lattice_margin", self._lattice_margin))
+            if self._uncertainty:
+                check(lib().vbt_tokenizer_set_option(h, b"uncertainty", self._uncertainty))
             if self._sampling[0]:
                 check(lib().vbt_tokenizer_set_sampling(h, *self._sampling))
             if self._sample_text:
@@ -605,7 +634,8 @@ class Tokenizer:
                                                    bnd.ctypes.data if bnd.size else None, C.byref(h)))
         return BatchResult(self, h, utf8, byte_offsets, compact=bool(self._options.get("compact_tokens", 0)),
                            marginals=self._theta > 0, lattice=self._lattice > 0, samples=self._sampling[0],
-                           margins=self._lattice > 0 and self._lattice_margin >= 0)
+                           margins=self._lattice > 0 and self._lattice_margin >= 0,
+                           uncertainty=self._uncertainty if self._theta > 0 else 0)
 
     def tokenize_batch_device(self, d_utf8, d_byte_offsets, n_sent, n_bytes, d_bnd_offsets=None, d_bnd=None, n_bnd=0,
                               d_span_offsets=None, d_spans=None, n_spans=0, patterns=None):
@@ -635,6 +665,14 @@ class Tokenizer:
         a, b = C.c_uint64(), C.c_uint64()
         check(lib().vbt_last_device_marginals(self.handle(), C.byref(a), C.byref(b)))
         return a.value, b.value
+
+    def last_device_uncertainty(self):
+        """-> (d_entropies, d_log_path_probs, d_boundary_offsets, d_boundary_probs, n_positions): device addresses
+        (float64[n_sent], float64[n_sent], uint64[n_sent + 1], float32[n_positions]; the last three 0 without
+        boundary_probs) of the uncertainty of the last tokenize_batch_device call, valid until the next call."""
+        v = [C.c_uint64() for _ in range(5)]
+        check(lib().vbt_last_device_uncertainty(self.handle(), *[C.byref(x) for x in v]))
+        return tuple(x.value for x in v)
 
     def last_device_lattice(self):
         """-> (d_node_offsets, d_nodes, d_links, d_node_probs, n_nodes): device addresses (uint64[n_sent + 1],
@@ -717,6 +755,18 @@ class Tokenizer:
         self._theta = theta
         return self
 
+    def uncertainty(self, on=True, boundary_probs=False):
+        """Segmentation uncertainty (the option "uncertainty"; needs marginals() on): results then carry each
+        sentence's path entropy in nats and best-path log-probability (BatchResult.entropies / log_path_probs, float64),
+        and with boundary_probs=True the probability that a token ends at each character position 0..n
+        (BatchResult.boundary_offsets / boundary_probs, sentence_boundary_probs()).  on=False switches it off.  The
+        tokens and every other output do not change; the "small_batch" route steps aside.  Definition:
+        include/vibrato_b200.h."""
+        value = (2 if boundary_probs else 1) if on else 0
+        check(lib().vbt_tokenizer_set_option(self.handle(), b"uncertainty", value))
+        self._uncertainty = value
+        return self
+
     # connection-id statistics (worker.rs:77-103) ---------------------------------------------------
     def init_connid_counter(self):
         """Worker::init_connid_counter: zero the counters; every batch tokenised afterwards is counted."""
@@ -755,6 +805,9 @@ class Tokenizer:
             return
         if name == "lattice_margin":  # replayed with lattice()'s state
             self._lattice_margin = int(value)
+            return
+        if name == "uncertainty":  # replayed with uncertainty()'s state, after the marginals it needs
+            self._uncertainty = int(value)
             return
         if name == "sample_text":  # replayed after sampling, which it needs
             self._sample_text = bool(value)
@@ -941,6 +994,7 @@ class Worker:
         self._tokens = []
         self._nodes = []
         self._samples = []
+        self._unc = None  # (entropy, log_path_prob, boundary probabilities or None) with Tokenizer.uncertainty()
 
     def reset_sentence(self, text, boundaries=None, spans=None):
         """boundaries: required token boundaries, byte offsets into the sentence; spans: required tokens, (start, end)
@@ -951,10 +1005,14 @@ class Worker:
         self._tokens = []
         self._nodes = []
         self._samples = []
+        self._unc = None
 
     def tokenize(self):
         if not self._sent:  # worker.rs:50-52
             self._samples = [[] for _ in range(self._tok._sampling[0])]
+            level = self._tok._uncertainty if self._tok._theta > 0 else 0
+            if level:  # the one empty path: no uncertainty, and it ends where it starts
+                self._unc = (0.0, 0.0, np.ones(1, dtype=np.float32) if level >= 2 else None)
             return
         res = self._tok.tokenize_batch([self._sent], boundaries=None if self._bounds is None else [self._bounds],
                                        spans=None if self._spans is None else [self._spans])
@@ -968,6 +1026,9 @@ class Worker:
         for sample in self._samples:
             for t in sample:
                 t._r = t._r.copy()
+        if res.entropies is not None:
+            self._unc = (float(res.entropies[0]), float(res.log_path_probs[0]),
+                         None if res.boundary_probs is None else res.sentence_boundary_probs(0).copy())
         res.close()
 
     def num_tokens(self):
@@ -988,6 +1049,28 @@ class Worker:
 
     def node_iter(self):
         return iter(self._nodes)
+
+    def _uncertainty(self, k):
+        if self._unc is None:
+            raise VibratoError(1, "no uncertainty: switch it on with Tokenizer.uncertainty() and tokenize first")
+        return self._unc[k]
+
+    def entropy(self):
+        """The sentence's path entropy in nats (Tokenizer.uncertainty())."""
+        return self._uncertainty(0)
+
+    def log_path_prob(self):
+        """ln P(best path) of the sentence (Tokenizer.uncertainty())."""
+        return self._uncertainty(1)
+
+    def boundary_probs(self):
+        """float32[n_chars + 1]: P(a token ends at character position p), p = 0..n (Tokenizer.uncertainty(
+        boundary_probs=True))."""
+        b = self._uncertainty(2)
+        if b is None:
+            raise VibratoError(1, "no boundary probabilities: switch them on with "
+                                  "Tokenizer.uncertainty(boundary_probs=True) before tokenising")
+        return b
 
     def sample_tokens(self, j):
         """The tokens of sample j of the sentence (Tokenizer.sampling())."""

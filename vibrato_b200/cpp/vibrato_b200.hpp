@@ -184,6 +184,21 @@ class BatchResult {
         check(vbt_result_lattice_margins(r_.get(), &m));
         return m;
     }
+    // Segmentation uncertainty (Tokenizer::uncertainty before the batch, see vbt_result_uncertainty): entropy and
+    // log_path_prob per sentence; with boundary probabilities, sentence i's positions 0..n are
+    // boundary_prob[boundary_offsets[i] .. boundary_offsets[i + 1]) (both nullptr without them).  Throws on a result
+    // made without the option.
+    struct Uncertainty {
+        const double* entropy = nullptr;
+        const double* log_path_prob = nullptr;
+        const uint64_t* boundary_offsets = nullptr;
+        const float* boundary_prob = nullptr;
+    };
+    Uncertainty uncertainty() const {
+        Uncertainty u;
+        check(vbt_result_uncertainty(r_.get(), &u.entropy, &u.log_path_prob, &u.boundary_offsets, &u.boundary_prob));
+        return u;
+    }
     // Segmentation sampling (Tokenizer::sampling before the batch, see vbt_tokenizer_set_sampling): sample j of
     // sentence i is samples[sample_offsets[i * n + j] .. sample_offsets[i * n + j + 1]).  Throws on a result made
     // without sampling.
@@ -288,6 +303,24 @@ class Tokenizer {
         return {tp, pp};
     }
     bool has_marginals() const { return marginals_; }
+    // Segmentation uncertainty (the option "uncertainty", see vbt_result_uncertainty; needs marginals):
+    // BatchResult::uncertainty(); boundary_probs = true also carries each character position's boundary probability.
+    void uncertainty(bool on = true, bool boundary_probs = false) const {
+        const int level = on ? (boundary_probs ? 2 : 1) : 0;
+        check(vbt_tokenizer_set_option(handle(), "uncertainty", level));
+        uncertainty_ = level;
+    }
+    int uncertainty_level() const { return marginals_ ? uncertainty_ : 0; }
+    // Device addresses of the last tokenize_batch_device call's uncertainty (the boundary arrays 0 at level 1).
+    struct DeviceUncertainty {
+        uint64_t entropy = 0, log_path_prob = 0, boundary_offsets = 0, boundary_prob = 0, n_positions = 0;
+    };
+    DeviceUncertainty last_device_uncertainty() const {
+        DeviceUncertainty d;
+        check(vbt_last_device_uncertainty(handle(), &d.entropy, &d.log_path_prob, &d.boundary_offsets, &d.boundary_prob,
+                                          &d.n_positions));
+        return d;
+    }
     // Lattice output (the option "lattice", see vbt_result_lattice): BatchResult::lattice(); text = true also renders
     // the nodes in place of the tokens in the output text (MeCab -a).  Set text before a format that prints %pb.
     // margin = D (0 .. 2^62; the option "lattice_margin") keeps only the nodes within cost D of the best path, plus the
@@ -408,6 +441,7 @@ class Tokenizer {
     mutable bool marginals_ = false;
     mutable bool lattice_ = false;
     mutable bool margin_ = false;  // lattice(..., margin >= 0)
+    mutable int uncertainty_ = 0;  // uncertainty(): 0, 1 or 2
     mutable uint32_t samples_ = 0;
     mutable std::shared_ptr<vbt_tokenizer> h_;
 };
@@ -504,7 +538,14 @@ class Worker {  // worker.rs:13-74
     }
     void tokenize() {
         samples_.assign(t_->samples_per_sentence(), {});
-        if (sent_.empty()) return;  // worker.rs:50-52
+        const int level = t_->uncertainty_level();
+        has_unc_ = level != 0;
+        bprobs_.clear();
+        if (sent_.empty()) {  // worker.rs:50-52; the one empty path has no uncertainty and ends where it starts
+            entropy_ = log_path_prob_ = 0.0;
+            if (level >= 2) bprobs_.assign(1, 1.f);
+            return;
+        }
         uint64_t off[2] = {0, sent_.size()};
         uint64_t boff[2] = {0, bnd_.size()};
         uint64_t soff[2] = {0, spans_.size()};
@@ -529,6 +570,12 @@ class Worker {  // worker.rs:13-74
                 margins_.assign(m, m + l.n_nodes);
             }
         }
+        if (has_unc_) {
+            const BatchResult::Uncertainty u = r.uncertainty();
+            entropy_ = u.entropy[0];
+            log_path_prob_ = u.log_path_prob[0];
+            if (u.boundary_prob) bprobs_.assign(u.boundary_prob + u.boundary_offsets[0], u.boundary_prob + u.boundary_offsets[1]);
+        }
         if (!samples_.empty()) {
             const BatchResult::Samples s = r.samples();
             for (size_t j = 0; j < samples_.size(); ++j) samples_[j].assign(s.samples + s.sample_offsets[j], s.samples + s.sample_offsets[j + 1]);
@@ -542,12 +589,31 @@ class Worker {  // worker.rs:13-74
         return LatticeNode(t_, sent_, nodes_[i], links_[i], nprobs_.empty() ? std::numeric_limits<float>::quiet_NaN() : nprobs_[i],
                            margins_.empty() ? -1 : margins_[i]);
     }
+    // Tokenizer::uncertainty: the sentence's path entropy (nats), ln P(best path) and, with boundary probabilities,
+    // P(a token ends at position p) for p = 0..n; each throws without the option.
+    double entropy() const {
+        need_uncertainty();
+        return entropy_;
+    }
+    double log_path_prob() const {
+        need_uncertainty();
+        return log_path_prob_;
+    }
+    const std::vector<float>& boundary_probs() const {
+        need_uncertainty();
+        if (t_->uncertainty_level() < 2)
+            throw VibratoError(VBT_ERR_INVALID_ARGUMENT, "no boundary probabilities: pass boundary_probs to Tokenizer::uncertainty");
+        return bprobs_;
+    }
     size_t num_tokens() const { return toks_.size(); }
     Token token(size_t i) const {
         return probs_.empty() ? Token(t_, sent_, toks_[i]) : Token(t_, sent_, toks_[i], probs_[i]);
     }
 
    private:
+    void need_uncertainty() const {
+        if (!has_unc_) throw VibratoError(VBT_ERR_INVALID_ARGUMENT, "no uncertainty: switch it on with Tokenizer::uncertainty and tokenize first");
+    }
     const Tokenizer* t_;
     std::string sent_;
     std::vector<uint32_t> bnd_;
@@ -561,6 +627,9 @@ class Worker {  // worker.rs:13-74
     std::vector<vbt_lattice_link> links_;
     std::vector<float> nprobs_;
     std::vector<int64_t> margins_;  // Tokenizer::lattice with a margin
+    bool has_unc_ = false;          // Tokenizer::uncertainty
+    double entropy_ = 0.0, log_path_prob_ = 0.0;
+    std::vector<float> bprobs_;
     std::vector<std::vector<vbt_token>> samples_;  // Tokenizer::sampling
 };
 

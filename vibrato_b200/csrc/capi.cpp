@@ -763,6 +763,33 @@ int32_t vbt_last_device_marginals(const vbt_tokenizer* t, uint64_t* d_token_prob
     });
 }
 
+int32_t vbt_result_uncertainty(const vbt_result* r, const double** entropy, const double** log_path_prob,
+                               const uint64_t** boundary_offsets, const float** boundary_prob) {
+    return guarded([&] {
+        need(r, "r");
+        if (!r->r->out.has(vbt::kEntropy))
+            throw vbt::Error(vbt::kInvalidArgument,
+                             "no uncertainty: set the tokenizer option \"uncertainty\" (with marginals on) before tokenising");
+        if (entropy) *entropy = r->r->ptr<const double>(vbt::kEntropy);
+        if (log_path_prob) *log_path_prob = r->r->ptr<const double>(vbt::kLogPathProb);
+        const bool pos = r->r->out.has(vbt::kBoundaryProb);  // level 2
+        if (boundary_offsets) *boundary_offsets = pos ? r->r->ptr<const uint64_t>(vbt::kPosOff) : nullptr;
+        if (boundary_prob) *boundary_prob = pos ? r->r->ptr<const float>(vbt::kBoundaryProb) : nullptr;
+    });
+}
+
+int32_t vbt_last_device_uncertainty(const vbt_tokenizer* t, uint64_t* d_entropy, uint64_t* d_log_path_prob,
+                                    uint64_t* d_boundary_offsets, uint64_t* d_boundary_prob, uint64_t* n_positions) {
+    return guarded([&] {
+        const vbt::DeviceOutputs& d = last_device(t, vbt::kEntropy, "the option \"uncertainty\"");
+        put(d_entropy, d.addr[vbt::kEntropy]);
+        put(d_log_path_prob, d.addr[vbt::kLogPathProb]);
+        put(d_boundary_offsets, d.addr[vbt::kPosOff]);  // 0 at level 1
+        put(d_boundary_prob, d.addr[vbt::kBoundaryProb]);
+        put(n_positions, d.made.has(vbt::kBoundaryProb) ? d.total[vbt::kGroupPositions] : 0);
+    });
+}
+
 int32_t vbt_result_lattice(const vbt_result* r, const uint64_t** node_offsets, const vbt_token** nodes,
                            const vbt_lattice_link** links, const float** node_prob, uint64_t* n_nodes) {
     return guarded([&] {

@@ -437,6 +437,14 @@ class EngineImpl final : public Engine {
                 throw Error(kInvalidArgument, "lattice_margin must be -1 (off) or a cost margin between 0 and 2^62");
             cudaStreamSynchronize(stream_);
             lat_margin_ = value;
+        } else if (name == "uncertainty") {
+            // each sentence's path entropy and best-path log-probability (1), and each position's boundary probability (2)
+            if (value < 0 || value > 2)
+                throw Error(kInvalidArgument, "uncertainty must be 0 (off), 1 (entropy and log_path_prob) or 2 (also boundary probabilities)");
+            if (value != 0 && theta_ == 0)
+                throw Error(kInvalidArgument, "uncertainty needs marginals: switch them on with set_marginals before setting it");
+            cudaStreamSynchronize(stream_);
+            unc_ = uint32_t(value);
         } else if (name == "sample_text") {
             // the output text renders each sentence's samples in place of its best path
             if (value < 0 || value > 1) throw Error(kInvalidArgument, "sample_text must be 0 (off) or 1 (the text renders the samples)");
@@ -492,6 +500,8 @@ class EngineImpl final : public Engine {
             throw Error(kInvalidArgument, "the marginals' theta must be a finite number >= 0 (0 switches them off)");
         if (theta == 0 && output_mode_ == kOutFormat && (fmt_uses_ & kUsesProb))
             throw Error(kInvalidArgument, "the output format prints %pP: change the format before switching marginals off");
+        if (theta == 0 && unc_)
+            throw Error(kInvalidArgument, "uncertainty needs marginals: set the option \"uncertainty\" to 0 before switching marginals off");
         if (theta > 0 && samp_n_ && theta != samp_theta_)
             throw Error(kInvalidArgument, "marginals and sampling share one forward pass: the marginals' theta " + num(theta) +
                                               " differs from the sampling theta " + num(samp_theta_));
@@ -516,7 +526,7 @@ class EngineImpl final : public Engine {
     double marginals() const override { return theta_; }
     int lattice() const override { return lattice_; }
     Outputs outputs() const override {
-        return Outputs{tok_bytes_, samp_n_, theta_ > 0, output_mode_ != kOutNone, lattice_ != 0, lat_margin_ >= 0};
+        return Outputs{tok_bytes_, samp_n_, theta_ > 0, output_mode_ != kOutNone, lattice_ != 0, lat_margin_ >= 0, unc_};
     }
     const DeviceOutputs& last_device() const override { return last_; }
     void set_stream(uint64_t stream) override {
@@ -608,7 +618,7 @@ class EngineImpl final : public Engine {
             if (!chunked) {
                 h2d(in_off_.p, off, (size_t(n_sent) + 1) * 8, stream_, off_pinned && off == byte_off);
                 h2d(in_utf8_.p, utf8 + first, n_bytes, stream_, utf8_pinned);
-                if (n_bytes <= kEagerBytes && output_mode_ == kOutNone && !lattice_ && !samp_n_) {
+                if (n_bytes <= kEagerBytes && output_mode_ == kOutNone && !lattice_ && !samp_n_ && !unc_) {
                     // Small batches (a per-sentence Worker loop ends up here) are all latency: the result copies are
                     // queued behind the kernels with an upper bound for the token count (a token spans >= 1 byte), so
                     // that the call makes ONE host synchronisation instead of two.
@@ -682,7 +692,8 @@ class EngineImpl final : public Engine {
                                           Totals{uint64_t(double(n_bytes) * tok_per_byte_) + 1024,
                                                  uint64_t(double(n_bytes) * text_ratio) + uint64_t(n_sent) * per_sent + 1024,
                                                  uint64_t(double(n_bytes) * node_per_byte_) + 1024,
-                                                 uint64_t(double(n_bytes) * tok_per_byte_ * samp_n_) + 1024});
+                                                 uint64_t(double(n_bytes) * tok_per_byte_ * samp_n_) + 1024,
+                                                 uint64_t(double(n_bytes) * chars_per_byte_) + n_sent + 1024});
             CK(cudaMemsetAsync(base_.p, 0, kNumGroups * 8, stream_));
             connid_begin(stream_);
             h2d(in_off_.p, off, (size_t(n_sent) + 1) * 8, stream_, off_pinned && off == byte_off);
@@ -1081,6 +1092,14 @@ class EngineImpl final : public Engine {
         o.buf[kTokens].ensure(size_t(n_bytes) * 24 + 24, 1.25);  // a token spans >= 1 character >= 1 byte
         if (theta_ > 0) o.buf[kTokenProb].ensure(size_t(n_bytes) * 4 + 4, 1.25);
         if (theta_ > 0 || samp_n_) o.buf[kPathProb].ensure((size_t(n_sent) + 1) * 4, 1.25);  // the forward pass writes it
+        if (unc_) {
+            o.buf[kEntropy].ensure((size_t(n_sent) + 1) * 8, 1.25);
+            o.buf[kLogPathProb].ensure((size_t(n_sent) + 1) * 8, 1.25);
+        }
+        if (unc_ >= 2) {  // a record per slot: characters <= bytes, one sentinel slot per sentence
+            o.buf[kPosOff].ensure((size_t(n_sent) + 1) * 8, 1.25);
+            o.buf[kBoundaryProb].ensure((size_t(n_bytes) + n_sent + 1) * 4, 1.25);
+        }
         if (lattice_) o.buf[kNodeOff].ensure((size_t(n_sent) + 1) * 8, 1.25);
         if (samp_n_) o.buf[kSampleOff].ensure((size_t(n_sent) * samp_n_ + 1) * 8, 1.25);
     }
@@ -1703,8 +1722,20 @@ class EngineImpl final : public Engine {
             m.path_prob = o.buf[kPathProb].as<float>();
             m.token_prob = marg ? o.buf[kTokenProb].as<float>() : nullptr;
             m.lw = samp ? w.m_lw.as<uint32_t>() : nullptr;
-            launch_marginals(dv_, b, m, st, marg);  // sampling alone needs no backward pass
-            if (n_sent) o.launches += marg ? 2 : 1;
+            UncertaintyArgs u{};
+            if (unc_) {  // the backward pass's uncertainty instantiation, and with 2 the boundary probabilities
+                u.entropy = o.buf[kEntropy].as<double>();
+                u.log_path_prob = o.buf[kLogPathProb].as<double>();
+                if (unc_ >= 2) {
+                    u.pos_off = o.buf[kPosOff].as<unsigned long long>();
+                    u.boundary_prob = o.buf[kBoundaryProb].as<float>();
+                    if (n_sent == 0) CK(cudaMemsetAsync(u.pos_off, 0, 8, st));
+                    // the group's records: one per slot (the low word of a total zeroed with the rest of Control)
+                    CK(cudaMemcpyAsync(&dc->total[kGroupPositions], b.slot_off + n_sent, 4, cudaMemcpyDeviceToDevice, st));
+                }
+            }
+            launch_marginals(dv_, b, m, st, marg, unc_ ? &u : nullptr);  // sampling alone needs no backward pass
+            if (n_sent) o.launches += (marg ? 2 : 1) + (unc_ >= 2 ? 1 : 0);
         }
         MarginArgs g{};
         if (mlat) {  // G of every entry, from the R the forward pass above left (or its R-only instantiation here)
@@ -1865,6 +1896,7 @@ class EngineImpl final : public Engine {
     int lattice_ = 0;         // option "lattice": 0 off, 1 nodes, 2 nodes and lattice text
     static constexpr long long kMaxLatticeMargin = 1ll << 62;
     long long lat_margin_ = -1;  // option "lattice_margin": the near-best lattice's D, -1 = off
+    uint32_t unc_ = 0;           // option "uncertainty": 0 off, 1 entropy and log_path_prob, 2 also boundary probabilities
     static constexpr uint32_t kMaxSamples = 1024;
     uint32_t samp_n_ = 0;       // sampling: paths per sentence, 0 = off (set_sampling)
     double samp_theta_ = 0;

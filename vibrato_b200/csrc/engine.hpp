@@ -13,16 +13,20 @@
 namespace vbt {
 
 // ---- the outputs of a batch ------------------------------------------------------------------------
-// A batch produces up to thirteen arrays in four ragged groups.  A group's offsets index its records: entries
+// A batch produces up to seventeen arrays in five ragged groups.  A group's offsets index its records: entries
 // off[i] .. off[i + 1] belong to sentence i (to sample j of sentence i at i * n_samp + j for the samples), and the
-// group's total is the number of its records.  path_prob has one entry per sentence and no offsets.
-enum Group { kGroupTokens, kGroupText, kGroupLattice, kGroupSamples, kNumGroups };
+// group's total is the number of its records.  path_prob, entropy and log_path_prob have one entry per sentence and no
+// offsets.  The positions group has one record per character position 0..n of every sentence: its offsets are the
+// slot offsets and its total is the batch's slot count.
+enum Group { kGroupTokens, kGroupText, kGroupLattice, kGroupSamples, kGroupPositions, kNumGroups };
 enum Array {
     kTokOff, kTokens, kTokenProb, kPathProb,  // vbt_token (or vbt_token16) records; marginals (set_marginals)
+    kEntropy, kLogPathProb,                   // uncertainty ("uncertainty" >= 1): float64 per sentence
     kTextOff, kText,                          // output stage ("output_mode" or a format): the text `tokenize` prints
     kNodeOff, kNodes, kLinks, kNodeProb,      // lattice ("lattice" >= 1): vbt_token nodes, vbt_lattice_link, marginals
     kNodeMargin,                              // near-best lattice ("lattice_margin" >= 0): each kept node's margin (int64)
     kSampleOff, kSamples,                     // sampling (set_sampling): vbt_token records of every sampled path
+    kPosOff, kBoundaryProb,                   // uncertainty 2: float32 boundary probability of every character position
     kNumArrays
 };
 enum ArrayKind { kOffsets, kRecords, kPerSentence };
@@ -33,11 +37,12 @@ struct ArrayInfo {
 };
 constexpr ArrayInfo kArrays[kNumArrays] = {
     {kGroupTokens, kOffsets, 8},   {kGroupTokens, kRecords, 0},  {kGroupTokens, kRecords, 4},   {kGroupTokens, kPerSentence, 4},
+    {kGroupTokens, kPerSentence, 8}, {kGroupTokens, kPerSentence, 8},
     {kGroupText, kOffsets, 8},     {kGroupText, kRecords, 1},    {kGroupLattice, kOffsets, 8},  {kGroupLattice, kRecords, 24},
     {kGroupLattice, kRecords, 8},  {kGroupLattice, kRecords, 4}, {kGroupLattice, kRecords, 8},  {kGroupSamples, kOffsets, 8},
-    {kGroupSamples, kRecords, 24},
+    {kGroupSamples, kRecords, 24}, {kGroupPositions, kOffsets, 8}, {kGroupPositions, kRecords, 4},
 };
-constexpr Array kOffsetsOf[kNumGroups] = {kTokOff, kTextOff, kNodeOff, kSampleOff};
+constexpr Array kOffsetsOf[kNumGroups] = {kTokOff, kTextOff, kNodeOff, kSampleOff, kPosOff};
 
 using Totals = std::array<uint64_t, kNumGroups>;  // one count per group
 
@@ -47,11 +52,16 @@ struct Outputs {
     uint32_t n_samp = 0;        // sampled paths per sentence, 0 = sampling off
     bool marg = false, text = false, lat = false;
     bool margin = false;  // "lattice_margin" >= 0: the lattice keeps the near-best nodes and carries their margins
+    uint32_t unc = 0;     // "uncertainty": 1 entropy and log_path_prob, 2 also the boundary probabilities
 
     bool has(int a) const {
         switch (a) {
             case kTokenProb:
             case kPathProb: return marg;
+            case kEntropy:
+            case kLogPathProb: return marg && unc >= 1;
+            case kPosOff:
+            case kBoundaryProb: return marg && unc >= 2;
             case kTextOff:
             case kText: return text;
             case kNodeOff:
@@ -211,7 +221,9 @@ class Engine {
     // takes k_small_batch for batches of at most N sentences and 16 KiB without counting; run_device and the shards
     // of a multi-device engine keep the usual route), "lattice" (0 off, 1 results also carry every lattice node,
     // 2 the same and the output text renders the nodes in place of the tokens), "lattice_margin" (-1 off; D in
-    // 0 .. 2^62: the lattice keeps only the nodes within cost D of the best path, kernels.cuh MarginArgs).
+    // 0 .. 2^62: the lattice keeps only the nodes within cost D of the best path, kernels.cuh MarginArgs),
+    // "uncertainty" (0 off; with marginals on, 1 results also carry kEntropy / kLogPathProb, 2 also kPosOff /
+    // kBoundaryProb, kernels.cuh UncertaintyArgs; k_small_batch and the eager small-batch copies step aside).
     virtual void set_option(const std::string& name, long long value) = 0;
     // An output format (format.hpp) in place of "output_mode" 1-3, on every host route; nullptr switches it off.
     // Setting "output_mode" replaces it.  Builds the format's field table on the device.

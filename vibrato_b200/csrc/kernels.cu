@@ -1894,15 +1894,28 @@ __global__ void __launch_bounds__(256) k_marg_forward(DictView d, Batch b, MargA
     }
 }
 
-template <int CONN>
-__global__ void __launch_bounds__(256) k_marg_backward(DictView d, Batch b, MargArgs m) {
+// UNC: the uncertainty instantiation (UncertaintyArgs in kernels.cuh), which also folds P(edge) * delta(edge) of every
+// edge it visits into a float64 per lane and writes u.entropy and u.log_path_prob; the other reads no u.
+template <int CONN, bool UNC = false>
+__global__ void __launch_bounds__(256) k_marg_backward(DictView d, Batch b, MargArgs m, UncertaintyArgs u) {
     if (stand_down(*b.flags)) return;
     const uint32_t lane = threadIdx.x & 31;
     uint32_t s, base, last;
-    if (!marg_sentence(b, (blockIdx.x * blockDim.x + threadIdx.x) >> 5, s, base, last) || base == last) return;
+    if (!marg_sentence(b, (blockIdx.x * blockDim.x + threadIdx.x) >> 5, s, base, last)) return;
+    if (base == last) {  // an empty sentence: one empty path
+        if (UNC && lane == 0) {
+            u.entropy[s] = 0.0;
+            u.log_path_prob[s] = 0.0;
+        }
+        return;
+    }
     const uint32_t slot_end = base + b.eos[s].y;  // the row EOS connects to
     const long long r_eos = m.r_eos[s];
     const double th = m.theta;
+    // UNC: P(edge) = exp(â(k) + [b̂(c) - theta delta] - â(EOS)); no path at all (â(EOS) = -inf) folds nothing
+    const double a_eos = UNC ? m.a_eos[s] : 0.0;
+    const bool fold = UNC && a_eos != -INFINITY;
+    double ed = 0.0;  // this lane's sum of P delta
     // one past the last candidate entry k_marg_forward numbered (it counts from the sentence's first row offset)
     uint32_t centry = 0;
     for (uint32_t slot = base + lane; slot < slot_end; slot += 32) centry += m.ncand[slot];
@@ -1915,6 +1928,7 @@ __global__ void __launch_bounds__(256) k_marg_backward(DictView d, Batch b, Marg
             for (uint32_t k = lane; k < K; k += 32) {
                 const long long x = m.R[eo + k] + conn.cost(d, uint32_t(b.ends_hot[eo + k].y));
                 m.ab[eo + k].y = -th * double(x - r_eos);
+                if (fold) ed += exp(m.ab[eo + k].x - th * double(x - r_eos) - a_eos) * double(x - r_eos);
             }
         } else {  // no successor at all beyond EOS's row or at a position the sweep skips: -inf
             const uint32_t nc = slot < slot_end ? m.ncand[slot] : 0u;
@@ -1925,6 +1939,7 @@ __global__ void __launch_bounds__(256) k_marg_backward(DictView d, Batch b, Marg
                 if (nc) {
                     const long long rk = m.R[eo + k];
                     const uint32_t right = uint32_t(b.ends_hot[eo + k].y);
+                    const double ak = fold ? m.ab[eo + k].x - a_eos : 0.0;  // UNC: â(k) - â(EOS)
                     // the position's candidates in candidate order, segment by segment
                     uint32_t c = 0, end = slot;
                     for (uint32_t h = 0; c < nc; ++h) {
@@ -1935,7 +1950,9 @@ __global__ void __launch_bounds__(256) k_marg_backward(DictView d, Batch b, Marg
                             const uint32_t e = m.cand_entry[centry + c];
                             const ConnRow<CONN> conn(d, cd.x & 0xFFFFu);
                             const long long x = rk + conn.cost(d, right) + int16_t(cd.y & 0xFFFFu);
-                            L = lse2(L, m.ab[e].y - th * double(x - m.R[e]));
+                            const double t = m.ab[e].y - th * double(x - m.R[e]);
+                            L = lse2(L, t);
+                            if (fold) ed += exp(ak + t) * double(x - m.R[e]);
                         }
                     }
                 }
@@ -1943,6 +1960,49 @@ __global__ void __launch_bounds__(256) k_marg_backward(DictView d, Batch b, Marg
             }
         }
         __syncwarp();
+    }
+    if (UNC) {  // the lanes' sums in a fixed order: a butterfly over lane indices
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) ed += __shfl_xor_sync(kFull, ed, o);
+        if (lane == 0) {
+            u.entropy[s] = fold ? a_eos + th * ed : 0.0;
+            u.log_path_prob[s] = fold ? -a_eos : -INFINITY;  // ln P(best) of no path at all: ln 0
+        }
+    }
+}
+
+// Boundary probabilities (UncertaintyArgs): a warp per sentence, a lane per row (position).  After k_marg_backward.
+__global__ void __launch_bounds__(256) k_boundary_probs(Batch b, MargArgs m, UncertaintyArgs u) {
+    const uint32_t s = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const uint32_t lane = threadIdx.x & 31;
+    if (s >= b.n_sent) return;
+    const uint32_t base = b.slot_off[s], last = b.slot_off[s + 1] - 1;
+    if (lane == 0) {
+        u.pos_off[s] = base;
+        if (s + 1 == b.n_sent) u.pos_off[s + 1] = last + 1;
+    }
+    // a re-run or refused batch: its rows cannot be trusted, and nothing is read from it
+    if (*b.flags & (kFlagsStandDown | kFlagPoolOverflow)) return;
+    if (base == last) {  // an empty sentence: its one (empty) path ends where it starts
+        if (lane == 0) u.boundary_prob[base] = 1.f;
+        return;
+    }
+    const double a_eos = m.a_eos[s];
+    const bool path = a_eos != -INFINITY;
+    for (uint32_t slot = base + lane; slot <= last; slot += 32) {
+        float p = 0.f;
+        if (path && slot == base) {
+            p = 1.f;  // BOS
+        } else if (path) {
+            const uint2 me = b.ends_meta[slot];
+            double sum = 0.0;
+            for (uint32_t e = me.x; e < me.y; ++e) {
+                const double2 ab = m.ab[e];
+                sum += exp(ab.x + ab.y - a_eos);
+            }
+            p = float(sum);
+        }
+        u.boundary_prob[slot] = p;
     }
 }
 
@@ -3260,24 +3320,31 @@ void launch_backtrack(const Batch& b, const MargArgs* m, const TileScan& ts, cud
 }
 
 // The forward pass's instantiation: with m.lw (sampling) the one that also keeps {left id, word cost}.
+// With u: the uncertainty instantiation of the backward pass.
 template <int CONN>
-static void launch_marg_conn(const DictView& d, const Batch& b, const MargArgs& m, bool backward, uint32_t blocks, cudaStream_t st) {
+static void launch_marg_conn(const DictView& d, const Batch& b, const MargArgs& m, bool backward, const UncertaintyArgs* u,
+                             uint32_t blocks, cudaStream_t st) {
     if (m.lw)
         k_marg_forward<CONN, true><<<blocks, 256, 0, st>>>(d, b, m);
     else
         k_marg_forward<CONN><<<blocks, 256, 0, st>>>(d, b, m);
-    if (backward) k_marg_backward<CONN><<<blocks, 256, 0, st>>>(d, b, m);
+    if (backward && u)
+        k_marg_backward<CONN, true><<<blocks, 256, 0, st>>>(d, b, m, *u);
+    else if (backward)
+        k_marg_backward<CONN><<<blocks, 256, 0, st>>>(d, b, m, UncertaintyArgs{});
 }
 
-void launch_marginals(const DictView& d, const Batch& b, const MargArgs& m, cudaStream_t st, bool backward) {
+void launch_marginals(const DictView& d, const Batch& b, const MargArgs& m, cudaStream_t st, bool backward,
+                      const UncertaintyArgs* u) {
     if (!b.n_sent) return;
     const uint32_t blocks = (b.n_sent + 7) / 8;  // a warp per sentence
     if (d.connector_kind == 1)
-        launch_marg_conn<1>(d, b, m, backward, blocks, st);
+        launch_marg_conn<1>(d, b, m, backward, u, blocks, st);
     else if (d.connector_kind == 2)
-        launch_marg_conn<2>(d, b, m, backward, blocks, st);
+        launch_marg_conn<2>(d, b, m, backward, u, blocks, st);
     else
-        launch_marg_conn<0>(d, b, m, backward, blocks, st);
+        launch_marg_conn<0>(d, b, m, backward, u, blocks, st);
+    if (backward && u && u->boundary_prob) k_boundary_probs<<<blocks, 256, 0, st>>>(b, m, *u);
 }
 
 void launch_lattice_count(const Batch& b, const LatticeArgs& l, cudaStream_t st) {

@@ -281,9 +281,24 @@ struct MargArgs {
     // instantiation of k_marg_forward only (lw != nullptr selects it); BOS's entry is not written
     uint32_t* lw;
 };
+// Segmentation uncertainty (option "uncertainty"), over the edges, exact path costs and theta of the marginals.  Per
+// edge k -> c (c = EOS included, with R(EOS) = r_eos and b̂(EOS) = 0) the slack delta = R(k) + cost(k -> c) - R(c) >= 0
+// telescopes along a path to cost - r_eos, so the path entropy is H = â(EOS) + theta * sum_edges P(edge) delta(edge),
+// P(k -> c) = exp(â(k) + b̂(c) - theta delta - â(EOS)): two sums of non-negative terms.  The uncertainty instantiation
+// of k_marg_backward folds P delta into a float64 per lane (a lane owns the same entries on every route) and reduces
+// the warp in a fixed order.  k_boundary_probs writes, per slot, the sum of the marginals of the row's entries
+// (float64, in row order, one lane per row, rounded once): P(a token of the path ends at that position).
+struct UncertaintyArgs {
+    double* entropy;               // per sentence: H (nats); 0 for an empty sentence or one without a path
+    double* log_path_prob;         // per sentence: -â(EOS); 0 for an empty sentence, -inf without a path
+    unsigned long long* pos_off;   // n_sent + 1: the slot offsets widened, or nullptr (no boundary probabilities)
+    float* boundary_prob;          // per slot; 1 at a sentence's first slot (BOS) when it has a path
+};
 // k_marg_forward and k_marg_backward (two launches); backward = false runs the forward pass alone (sampling without
-// marginals).  m.lw != nullptr selects the forward pass that also writes MargArgs::lw.
-void launch_marginals(const DictView& d, const Batch& b, const MargArgs& m, cudaStream_t st, bool backward = true);
+// marginals).  m.lw != nullptr selects the forward pass that also writes MargArgs::lw.  With u (backward only): the
+// uncertainty instantiation of k_marg_backward, then k_boundary_probs when u->boundary_prob != nullptr.
+void launch_marginals(const DictView& d, const Batch& b, const MargArgs& m, cudaStream_t st, bool backward = true,
+                      const UncertaintyArgs* u = nullptr);
 // backtrack_count, the token-offset scan and backtrack_write: n_tok, tok_off (n_sent + 1 entries) and the token
 // records; with m (marginals) also MargArgs::token_prob of every token.
 void launch_backtrack(const Batch& b, const MargArgs* m, const TileScan& ts, cudaStream_t st);
