@@ -1,8 +1,9 @@
 #!/usr/bin/env python3
 """Small run of the bounded routes for compute-sanitizer memcheck, checked against the bounded oracle: whole batch,
 the chunked pipeline, k_small_batch and device-resident input, with valid lists, a bad list and empty lists.
+Kernels: k_mark_bounds, k_candidates<true>, k_small_batch<CONN, true>.
 
-    compute-sanitizer --tool memcheck python tests/probes/bounded_probe.py"""
+    tools/run_sanitizer.sh bounded memcheck"""
 import json
 import os
 import sys

@@ -3,7 +3,7 @@
 the format program staged in shared memory and interpreted by k_format_len / k_format_write (whole batch) and by
 k_small_batch, with fields, quoted features, unknown words and %S; checked against tests/format_oracle.py.
 
-    compute-sanitizer --tool memcheck python tests/probes/format_probe.py"""
+    tools/run_sanitizer.sh format memcheck"""
 import json
 import os
 import sys

@@ -2,8 +2,9 @@
 """Small run of the single-pass front and back kernels (k_front, k_backtrack) for compute-sanitizer (memcheck /
 racecheck), checked against the oracle: the inputs of tests/test_gpu_fused_scans.py on the whole-batch, chunked and
 compact routes, an input error in the last tile and the slot-overflow re-run.
+Kernels: k_front and k_backtrack (tile tickets, look-back scans, staged text in shared memory).
 
-    compute-sanitizer --tool racecheck python tests/probes/fused_scans_probe.py"""
+    tools/run_sanitizer.sh fused_scans memcheck racecheck"""
 import json
 import os
 import sys

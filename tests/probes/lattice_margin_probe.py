@@ -2,8 +2,9 @@
 """Small run of the near-best lattice for compute-sanitizer memcheck, checked against the restatement
 (tests/margin_oracle.py): whole batch, the chunked pipeline (empty sentences at chunk edges) and device-resident input,
 with and without marginals (the R-only forward pass and the shared one), ignore_space on, then lattice text with %pb.
+Kernels: k_marg_forward's R-only instantiation, k_margin_backward, k_lattice_count_margin, k_lattice_write<true>.
 
-    compute-sanitizer --tool memcheck python tests/probes/lattice_margin_probe.py"""
+    tools/run_sanitizer.sh lattice_margin memcheck"""
 import json
 import os
 import sys

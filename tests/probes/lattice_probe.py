@@ -2,8 +2,9 @@
 """Small run of the lattice routes for compute-sanitizer memcheck, checked against the restatement
 (tests/lattice_oracle.py): whole batch, the chunked pipeline (empty sentences at chunk edges) and device-resident
 input, with marginals and ignore_space on, then lattice text with a %pb / %pP format.
+Kernels: k_lattice_count, k_lattice_write<false>, the %pb format kernels.
 
-    compute-sanitizer --tool memcheck python tests/probes/lattice_probe.py"""
+    tools/run_sanitizer.sh lattice memcheck"""
 import json
 import os
 import sys

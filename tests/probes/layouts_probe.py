@@ -3,9 +3,9 @@
 sentences per warp, dealt through Batch::order), for compute-sanitizer memcheck and racecheck, checked against the
 restatements as tests/test_gpu_prob_layouts.py checks them: the ties adversarial dictionary (rows longer than one
 staging pass, positions with more than 32 candidates), ignore_space on, whole batch and device-resident input.
+Kernels: k_viterbi2<4>, k_marg_forward / k_marg_backward through Batch::order, k_lattice_*, k_sample_*.
 
-    compute-sanitizer --tool memcheck python tests/probes/layouts_probe.py
-    compute-sanitizer --tool racecheck python tests/probes/layouts_probe.py"""
+    tools/run_sanitizer.sh layouts memcheck racecheck"""
 import os
 import sys
 

@@ -3,8 +3,9 @@
 (tests/marginal_oracle.py): whole batch, the chunked pipeline (empty sentences at chunk edges), device-resident
 input, a bounded call and a %pP output format, on the Matrix fixture and the Raw adversarial dictionary, with
 ignore_space on (skipped and trailing space runs).
+Kernels: k_marg_forward, k_marg_backward, k_backtrack<true>, the %pP format kernels.
 
-    compute-sanitizer --tool memcheck python tests/probes/marginal_probe.py"""
+    tools/run_sanitizer.sh marginal memcheck"""
 import json
 import os
 import sys

@@ -2,8 +2,9 @@
 """Small run of sample text ("sample_text" = 1) for compute-sanitizer memcheck: the whole batch, the chunked
 pipeline (empty sentences at chunk edges) and the text-overflow retry, with a format that prints the "prev"
 directives and BOS / EOS with %S %L, and -O mecab / wakati.  Each route's text is checked against the whole batch.
+Kernels: k_format_len_samples, k_format_write_samples.
 
-    compute-sanitizer --tool memcheck python tests/probes/sample_text_probe.py"""
+    tools/run_sanitizer.sh sample_text memcheck"""
 import json
 import os
 import sys

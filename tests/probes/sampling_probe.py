@@ -3,8 +3,9 @@
 (tests/sampling_oracle.py) up to each sample's first ambiguous draw: whole batch, the chunked pipeline (empty
 sentences at chunk edges), device-resident input and a bounded call, on the Matrix fixture and the Raw adversarial
 dictionary, with ignore_space on (skipped and trailing space runs), sampling alone and next to marginals.
+Kernels: k_marg_forward's sampling instantiation, k_sample_count, k_sample_write.
 
-    compute-sanitizer --tool memcheck python tests/probes/sampling_probe.py"""
+    tools/run_sanitizer.sh sampling memcheck"""
 import json
 import os
 import sys

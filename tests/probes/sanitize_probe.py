@@ -1,6 +1,8 @@
 #!/usr/bin/env python3
 """Small end-to-end run for compute-sanitizer (memcheck / racecheck / initcheck), checked against the oracle;
-lives under tests/ because only tests may use oracle/.   compute-sanitizer python tests/probes/sanitize_probe.py"""
+lives under tests/ because only tests may use oracle/.
+
+    tools/run_sanitizer.sh sanitize memcheck racecheck"""
 import json
 import os
 import sys

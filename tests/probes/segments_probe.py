@@ -3,8 +3,9 @@
 oracle: far end slots (move segments), 2^16-candidate sources, crowded positions (tests/segment_fixtures.py), on
 the whole batch, k_small_batch and with marginals and the lattice on, then the pool-overflow retry that only the
 segments cause.
+Kernels: k_candidates, every Viterbi kernel, k_small_batch, the marginal and lattice kernels.
 
-    compute-sanitizer --tool memcheck python tests/probes/segments_probe.py"""
+    tools/run_sanitizer.sh segments memcheck"""
 import os
 import sys
 

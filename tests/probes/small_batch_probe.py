@@ -3,7 +3,7 @@
 the block scans, the shared batch flags and the per-warp stages of the one-block kernel, on the Matrix, Raw and Dual
 connectors, with the output stage, compact records, an input error and the overflow fallback.
 
-    compute-sanitizer --tool racecheck python tests/probes/small_batch_probe.py"""
+    tools/run_sanitizer.sh small_batch memcheck racecheck"""
 import json
 import os
 import sys

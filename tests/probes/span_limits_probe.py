@@ -3,7 +3,7 @@
 a start with more segments than the shared-memory pass keeps (re-walked into the pool), far spans with move segments,
 65 spans in one sentence, the quoted-feature battery, and the pool-overflow re-run.
 
-    compute-sanitizer --tool memcheck python tests/probes/span_limits_probe.py"""
+    tools/run_sanitizer.sh span_limits memcheck"""
 import os
 import sys
 

@@ -3,7 +3,7 @@
 the chunked pipeline and device-resident input (k_mark_spans, k_candidates_spans), with spans with and without
 patterns, a refused list, empty lists, and a batch re-run after a candidate pool overflow.
 
-    compute-sanitizer --tool memcheck python tests/probes/spans_probe.py"""
+    tools/run_sanitizer.sh spans memcheck"""
 import json
 import os
 import sys

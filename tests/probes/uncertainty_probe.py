@@ -2,8 +2,9 @@
 """Small run of the segmentation uncertainty for compute-sanitizer memcheck, checked against the restatement
 (tests/uncertainty_oracle.py): whole batch, the chunked pipeline (empty sentences at chunk edges) and device-resident
 input, at levels 1 and 2, ignore_space on, with a no-path span call.
+Kernels: k_marg_backward's uncertainty instantiation and k_boundary_probs.
 
-    compute-sanitizer --tool memcheck python tests/probes/uncertainty_probe.py"""
+    tools/run_sanitizer.sh uncertainty memcheck"""
 import json
 import os
 import sys

@@ -1710,7 +1710,7 @@ class EngineImpl final : public Engine {
         CK(cudaEventRecord(o.ev[5], st));
         o.launches += launch_viterbi(dv_, b, counting_ ? w.stats.as<uint4>() : nullptr, lanes_, viterbi_kernel_, st, &o.route);
         MargArgs m{};
-        if (marg || samp) {  // booked with the Viterbi stage; must run before K4 reuses ends_meta
+        if (marg || samp || mlat) {
             m.theta = marg ? theta_ : samp_theta_;  // equal when both are on (set_marginals / set_sampling)
             m.fill = w.m_fill.as<uint32_t>();
             m.ncand = w.m_ncand.as<uint32_t>();
@@ -1722,6 +1722,8 @@ class EngineImpl final : public Engine {
             m.path_prob = o.buf[kPathProb].as<float>();
             m.token_prob = marg ? o.buf[kTokenProb].as<float>() : nullptr;
             m.lw = samp ? w.m_lw.as<uint32_t>() : nullptr;
+        }
+        if (marg || samp) {  // booked with the Viterbi stage; must run before K4 reuses ends_meta
             UncertaintyArgs u{};
             if (unc_) {  // the backward pass's uncertainty instantiation, and with 2 the boundary probabilities
                 u.entropy = o.buf[kEntropy].as<double>();
@@ -1739,11 +1741,6 @@ class EngineImpl final : public Engine {
         }
         MarginArgs g{};
         if (mlat) {  // G of every entry, from the R the forward pass above left (or its R-only instantiation here)
-            m.fill = w.m_fill.as<uint32_t>();
-            m.ncand = w.m_ncand.as<uint32_t>();
-            m.cand_entry = w.m_cand_entry.as<uint32_t>();
-            m.R = w.m_R.as<long long>();
-            m.r_eos = w.m_r_eos.as<long long>();
             g = MarginArgs{lat_margin_, w.g_G.as<long long>(), w.g_keep.as<uint32_t>(), o.buf[kNodeMargin].as<long long>()};
             launch_margin_backward(dv_, b, m, g, !(marg || samp), st);
             if (n_sent) o.launches += (marg || samp) ? 1 : 2;
@@ -1756,17 +1753,11 @@ class EngineImpl final : public Engine {
             l.nodes = o.buf[kNodes].as<uint2>();
             l.links = o.buf[kLinks].as<int2>();
             l.node_prob = marg ? o.buf[kNodeProb].as<float>() : nullptr;
-            if (mlat)
-                launch_lattice_count(b, l, m, g, st);
-            else
-                launch_lattice_count(b, l, st);
+            launch_lattice_count(b, l, m, mlat ? &g : nullptr, st);
             cub::TransformInputIterator<unsigned long long, CastU64, const uint32_t*> it(l.n_nodes, CastU64());
             if (n_sent == 0) CK(cudaMemsetAsync(l.n_nodes, 0, 4, st));
             exclusive_scan(w, it, l.node_off, size_t(n_sent) + 1);
-            if (mlat)
-                launch_lattice_write(b, l, m, g, st);
-            else
-                launch_lattice_write(b, l, m, st);
+            launch_lattice_write(b, l, m, mlat ? &g : nullptr, st);
             CK(cudaMemcpyAsync(&dc->total[kGroupLattice], l.node_off + n_sent, 8, cudaMemcpyDeviceToDevice, st));
             if (n_sent) o.launches += 2;
         }

@@ -11,6 +11,7 @@
 #include "kernels.cuh"
 
 #include <climits>
+#include <type_traits>
 
 // Minimum resident blocks per SM asked of ptxas for k_viterbi (128 threads each): 16 -> 32 registers,
 // 64 warps/SM.  The counting and Raw/Dual instantiations are not on the timed path and get 64 registers.
@@ -29,6 +30,11 @@ constexpr unsigned kFull = 0xFFFFFFFFu;
 // A batch whose byte offsets k_front refused is not touched by any later kernel: the sizes derived from
 // the offsets (slots, workspace bounds) cannot be trusted.
 __device__ __forceinline__ bool stand_down(uint32_t batch_flags) { return batch_flags & kFlagsStandDown; }
+// The lattice rows of a batch that overflowed its candidate pool (it is run again) cannot be read either: the
+// boundary-probability, lattice and sampling kernels take nothing from such a batch or a refused one.
+__device__ __forceinline__ bool rows_unreadable(uint32_t batch_flags) {
+    return batch_flags & (kFlagsStandDown | kFlagPoolOverflow);
+}
 
 // CharInfo bit fields (dictionary/character.rs:10-24,72-94)
 __device__ __forceinline__ uint32_t ci_cate(uint32_t ci) { return ci & 0x3FFFFu; }
@@ -1618,10 +1624,38 @@ __global__ void __launch_bounds__(32 * VBT_K3V2_WARPS, CONN == 0 ? VBT_K3V2_MIN_
 // K4: Lattice::append_top_nodes (lattice.rs:159-168) + Token accessors (token.rs:21-92)
 // ---------------------------------------------------------------------------------------------
 
+// f(entry, end position) for each node of sentence s's best path, from EOS back (base = the sentence's first slot).
+template <class F>
+__device__ __forceinline__ void walk_best(const Batch& b, uint32_t s, uint32_t base, F f) {
+    const uint4 eo = b.eos[s];
+    if (eo.x == kNone) return;
+    uint32_t cur = eo.x, end_node = eo.y;
+    while (end_node != 0) {
+        const uint4 c = b.ends_cold[cur];
+        f(cur, end_node);
+        end_node = c.x - base;
+        cur = c.y;
+    }
+}
+
+// The 24-byte vbt_token record at t of the lattice entry whose ends_cold word is c, ending at slot end_slot of the
+// sentence whose first slot is base, with `total` as its total cost.  start_char is the entry's start_word
+// (token.rs:21-24), the bytes are those of start_word and the end (token.rs:28-32).
+__device__ __forceinline__ void write_node_record(const Batch& b, uint2* t, uint32_t base, uint32_t end_slot, const uint4& c,
+                                                  uint32_t total) {
+    const uint32_t start_node = c.x - base;
+    const uint32_t start_word = start_node + ((b.info[c.x].y & kInfoSpecial) ? b.info_ex[c.x].x : 0u);
+    t[0] = make_uint2(start_word, end_slot - base);
+    t[1] = make_uint2(b.byte_pos[base + start_word], b.byte_pos[end_slot]);
+    t[2] = make_uint2(c.z, total);  // word_idx, total_cost
+}
+
 // The path walk (backtrack_count_one, a thread per sentence) counts the tokens and leaves, for the k-th node from the
 // end, {lattice entry, end position} in the sentence's own stretch of `ends_meta` (dead after K3, one entry per
 // character, and a path has at most one node per character).  Once the token offsets are known the records are built
 // from those entries — the pointer chase is not repeated and neighbouring lanes write neighbouring records.
+// It chases the path itself rather than through walk_best: that would load the slot offset before the EOS entry, and
+// k_backtrack, which inlines this, is on the hot path.
 __device__ __forceinline__ void backtrack_count_one(const Batch& b, uint32_t s) {
     uint4 e = b.eos[s];
     uint32_t k = 0;
@@ -1646,6 +1680,7 @@ __device__ __forceinline__ void backtrack_write_one(const Batch& b, uint32_t s, 
     const unsigned long long t0 = b.tok_off[s];
     const uint32_t n = uint32_t(b.tok_off[s + 1] - t0);
     uint2* out = reinterpret_cast<uint2*>(b.tokens);
+    // the record of write_node_record, spelled out: k_small_batch, which inlines this, keeps its code that way
     for (uint32_t k = lane; k < n; k += 32) {
         const uint2 pe = b.ends_meta[base + k];  // k-th node from the end of the path
         const uint4 c = b.ends_cold[pe.x];
@@ -1894,6 +1929,54 @@ __global__ void __launch_bounds__(256) k_marg_forward(DictView d, Batch b, MargA
     }
 }
 
+// The rows of a non-empty sentence right to left, as the backward passes walk them (a warp per sentence, a lane per
+// entry; slot_end = the row EOS connects to), with the successors of each entry in the numbering k_marg_forward gave
+// the candidates' entries:
+//   eos(n, c)         each entry n of the row EOS connects to, c = conn(right(n), 0) (EOS: left id 0, no word cost);
+//   row(n, nc, succ)  each entry n of every other row, nc = the candidates of its position (0 beyond EOS's row and at
+//                     a position the sweep skips: n has no successor), and with nc > 0, succ(f) calls f(e, cost) for
+//                     each successor entry e in candidate order, segment by segment; cost() = conn(right(n), left(e)) +
+//                     wcost(e), looked up only when called.
+template <int CONN, class Eos, class Row>
+__device__ __forceinline__ void backward_rows(const DictView& d, const Batch& b, const MargArgs& m, uint32_t base, uint32_t last,
+                                              uint32_t slot_end, uint32_t lane, Eos eos, Row row) {
+    // one past the last candidate entry k_marg_forward numbered (it counts from the sentence's first row offset)
+    uint32_t centry = 0;
+    for (uint32_t slot = base + lane; slot < slot_end; slot += 32) centry += m.ncand[slot];
+    centry = b.ends_meta[base].x + __reduce_add_sync(kFull, centry);
+    for (uint32_t slot = last + 1; slot-- > base;) {
+        const uint2 me = b.ends_meta[slot];
+        const uint32_t eo = me.x, K = me.y - me.x;
+        if (slot == slot_end) {
+            const ConnRow<CONN> conn(d, 0);
+            for (uint32_t k = lane; k < K; k += 32) eos(eo + k, conn.cost(d, uint32_t(b.ends_hot[eo + k].y)));
+        } else {
+            const uint32_t nc = slot < slot_end ? m.ncand[slot] : 0u;
+            const uint32_t sptr = nc ? b.info[slot].x : 0u;
+            centry -= nc;
+            for (uint32_t k = lane; k < K; k += 32) {
+                row(eo + k, nc, [&](auto f) {
+                    const uint32_t right = uint32_t(b.ends_hot[eo + k].y);
+                    uint32_t c = 0, end = slot;
+                    for (uint32_t h = 0; c < nc; ++h) {
+                        const uint2 sg = __ldg(&b.seg[sptr + h]);
+                        end += uint32_t(int32_t(sg.y) >> 16);
+                        for (uint32_t j = 0; j < (sg.y & 0xFFFFu); ++j, ++c) {
+                            const uint4 cd = seg_record(d, sg, j, end);
+                            const uint32_t e = m.cand_entry[centry + c];
+                            f(e, [&] {
+                                const ConnRow<CONN> conn(d, cd.x & 0xFFFFu);
+                                return (long long)conn.cost(d, right) + int16_t(cd.y & 0xFFFFu);
+                            });
+                        }
+                    }
+                });
+            }
+        }
+        __syncwarp();
+    }
+}
+
 // UNC: the uncertainty instantiation (UncertaintyArgs in kernels.cuh), which also folds P(edge) * delta(edge) of every
 // edge it visits into a float64 per lane and writes u.entropy and u.log_path_prob; the other reads no u.
 template <int CONN, bool UNC = false>
@@ -1916,51 +1999,27 @@ __global__ void __launch_bounds__(256) k_marg_backward(DictView d, Batch b, Marg
     const double a_eos = UNC ? m.a_eos[s] : 0.0;
     const bool fold = UNC && a_eos != -INFINITY;
     double ed = 0.0;  // this lane's sum of P delta
-    // one past the last candidate entry k_marg_forward numbered (it counts from the sentence's first row offset)
-    uint32_t centry = 0;
-    for (uint32_t slot = base + lane; slot < slot_end; slot += 32) centry += m.ncand[slot];
-    centry = b.ends_meta[base].x + __reduce_add_sync(kFull, centry);
-    for (uint32_t slot = last + 1; slot-- > base;) {
-        const uint2 me = b.ends_meta[slot];
-        const uint32_t eo = me.x, K = me.y - me.x;
-        if (slot == slot_end) {
-            const ConnRow<CONN> conn(d, 0);
-            for (uint32_t k = lane; k < K; k += 32) {
-                const long long x = m.R[eo + k] + conn.cost(d, uint32_t(b.ends_hot[eo + k].y));
-                m.ab[eo + k].y = -th * double(x - r_eos);
-                if (fold) ed += exp(m.ab[eo + k].x - th * double(x - r_eos) - a_eos) * double(x - r_eos);
+    backward_rows<CONN>(
+        d, b, m, base, last, slot_end, lane,
+        [&](uint32_t n, long long c) {
+            const long long x = m.R[n] + c;
+            m.ab[n].y = -th * double(x - r_eos);
+            if (fold) ed += exp(m.ab[n].x - th * double(x - r_eos) - a_eos) * double(x - r_eos);
+        },
+        [&](uint32_t n, uint32_t nc, auto succ) {
+            double L = -INFINITY;  // no successor at all: -inf
+            if (nc) {
+                const long long rk = m.R[n];
+                const double ak = fold ? m.ab[n].x - a_eos : 0.0;  // UNC: â(n) - â(EOS)
+                succ([&](uint32_t e, auto cost) {
+                    const long long x = rk + cost();
+                    const double t = m.ab[e].y - th * double(x - m.R[e]);
+                    L = lse2(L, t);
+                    if (fold) ed += exp(ak + t) * double(x - m.R[e]);
+                });
             }
-        } else {  // no successor at all beyond EOS's row or at a position the sweep skips: -inf
-            const uint32_t nc = slot < slot_end ? m.ncand[slot] : 0u;
-            const uint32_t sptr = nc ? b.info[slot].x : 0u;
-            centry -= nc;
-            for (uint32_t k = lane; k < K; k += 32) {
-                double L = -INFINITY;
-                if (nc) {
-                    const long long rk = m.R[eo + k];
-                    const uint32_t right = uint32_t(b.ends_hot[eo + k].y);
-                    const double ak = fold ? m.ab[eo + k].x - a_eos : 0.0;  // UNC: â(k) - â(EOS)
-                    // the position's candidates in candidate order, segment by segment
-                    uint32_t c = 0, end = slot;
-                    for (uint32_t h = 0; c < nc; ++h) {
-                        const uint2 sg = __ldg(&b.seg[sptr + h]);
-                        end += uint32_t(int32_t(sg.y) >> 16);
-                        for (uint32_t j = 0; j < (sg.y & 0xFFFFu); ++j, ++c) {
-                            const uint4 cd = seg_record(d, sg, j, end);
-                            const uint32_t e = m.cand_entry[centry + c];
-                            const ConnRow<CONN> conn(d, cd.x & 0xFFFFu);
-                            const long long x = rk + conn.cost(d, right) + int16_t(cd.y & 0xFFFFu);
-                            const double t = m.ab[e].y - th * double(x - m.R[e]);
-                            L = lse2(L, t);
-                            if (fold) ed += exp(ak + t) * double(x - m.R[e]);
-                        }
-                    }
-                }
-                m.ab[eo + k].y = L;
-            }
-        }
-        __syncwarp();
-    }
+            m.ab[n].y = L;
+        });
     if (UNC) {  // the lanes' sums in a fixed order: a butterfly over lane indices
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) ed += __shfl_xor_sync(kFull, ed, o);
@@ -1981,8 +2040,7 @@ __global__ void __launch_bounds__(256) k_boundary_probs(Batch b, MargArgs m, Unc
         u.pos_off[s] = base;
         if (s + 1 == b.n_sent) u.pos_off[s + 1] = last + 1;
     }
-    // a re-run or refused batch: its rows cannot be trusted, and nothing is read from it
-    if (*b.flags & (kFlagsStandDown | kFlagPoolOverflow)) return;
+    if (rows_unreadable(*b.flags)) return;
     if (base == last) {  // an empty sentence: its one (empty) path ends where it starts
         if (lane == 0) u.boundary_prob[base] = 1.f;
         return;
@@ -2006,50 +2064,25 @@ __global__ void __launch_bounds__(256) k_boundary_probs(Batch b, MargArgs m, Unc
     }
 }
 
-// Near-best lattice (MarginArgs in kernels.cuh): G(n), the least exact cost from entry n to EOS, shaped like
-// k_marg_backward (a warp per sentence, rows right to left, a lane per entry) with min-plus in place of log-sum-exp.
+// Near-best lattice (MarginArgs in kernels.cuh): G(n), the least exact cost from entry n to EOS, over k_marg_backward's
+// row walk (backward_rows) with min-plus in place of log-sum-exp.
 template <int CONN>
 __global__ void __launch_bounds__(256) k_margin_backward(DictView d, Batch b, MargArgs m, MarginArgs g) {
     if (stand_down(*b.flags)) return;
     const uint32_t lane = threadIdx.x & 31;
     uint32_t s, base, last;
     if (!marg_sentence(b, (blockIdx.x * blockDim.x + threadIdx.x) >> 5, s, base, last) || base == last) return;
-    const uint32_t slot_end = base + b.eos[s].y;  // the row EOS connects to
-    uint32_t centry = 0;  // one past the last candidate entry k_marg_forward numbered, as in k_marg_backward
-    for (uint32_t slot = base + lane; slot < slot_end; slot += 32) centry += m.ncand[slot];
-    centry = b.ends_meta[base].x + __reduce_add_sync(kFull, centry);
-    for (uint32_t slot = last + 1; slot-- > base;) {
-        const uint2 me = b.ends_meta[slot];
-        const uint32_t eo = me.x, K = me.y - me.x;
-        if (slot == slot_end) {
-            const ConnRow<CONN> conn(d, 0);
-            for (uint32_t k = lane; k < K; k += 32) g.G[eo + k] = conn.cost(d, uint32_t(b.ends_hot[eo + k].y));
-        } else {  // no successor beyond EOS's row or at a position the sweep skips: LLONG_MAX
-            const uint32_t nc = slot < slot_end ? m.ncand[slot] : 0u;
-            const uint32_t sptr = nc ? b.info[slot].x : 0u;
-            centry -= nc;
-            for (uint32_t k = lane; k < K; k += 32) {
-                long long best = LLONG_MAX;
-                if (nc) {
-                    const uint32_t right = uint32_t(b.ends_hot[eo + k].y);
-                    uint32_t c = 0, end = slot;
-                    for (uint32_t h = 0; c < nc; ++h) {
-                        const uint2 sg = __ldg(&b.seg[sptr + h]);
-                        end += uint32_t(int32_t(sg.y) >> 16);
-                        for (uint32_t j = 0; j < (sg.y & 0xFFFFu); ++j, ++c) {
-                            const uint4 cd = seg_record(d, sg, j, end);
-                            const long long ge = g.G[m.cand_entry[centry + c]];
-                            if (ge == LLONG_MAX) continue;
-                            const ConnRow<CONN> conn(d, cd.x & 0xFFFFu);
-                            best = min(best, ge + conn.cost(d, right) + int16_t(cd.y & 0xFFFFu));
-                        }
-                    }
-                }
-                g.G[eo + k] = best;
-            }
-        }
-        __syncwarp();
-    }
+    backward_rows<CONN>(
+        d, b, m, base, last, base + b.eos[s].y, lane, [&](uint32_t n, long long c) { g.G[n] = c; },
+        [&](uint32_t n, uint32_t nc, auto succ) {
+            long long best = LLONG_MAX;  // no successor with a path to EOS: LLONG_MAX
+            if (nc)
+                succ([&](uint32_t e, auto cost) {
+                    const long long ge = g.G[e];
+                    if (ge != LLONG_MAX) best = min(best, ge + cost());
+                });
+            g.G[n] = best;
+        });
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -2063,12 +2096,12 @@ __device__ __forceinline__ uint32_t lattice_row_nodes(const Batch& b, uint32_t s
     return me.y - me.x - ((i == 0 && !empty) ? 1u : 0u);
 }
 
+// The full lattice's numbering: row_base and n_nodes.
 __global__ void __launch_bounds__(256) k_lattice_count(Batch b, LatticeArgs l) {
     const uint32_t s = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const uint32_t lane = threadIdx.x & 31;
     if (s >= b.n_sent) return;
-    // a batch that is re-run or refused: its rows cannot be trusted, and nothing is read from it
-    if (*b.flags & (kFlagsStandDown | kFlagPoolOverflow)) {
+    if (rows_unreadable(*b.flags)) {
         if (lane == 0) l.n_nodes[s] = 0;
         return;
     }
@@ -2090,77 +2123,14 @@ __global__ void __launch_bounds__(256) k_lattice_count(Batch b, LatticeArgs l) {
     if (lane == 0) l.n_nodes[s] = run;
 }
 
-__global__ void __launch_bounds__(256) k_lattice_write(Batch b, LatticeArgs l, MargArgs m) {
-    const uint32_t s = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    const uint32_t lane = threadIdx.x & 31;
-    if (s >= b.n_sent || (*b.flags & (kFlagsStandDown | kFlagPoolOverflow))) return;
-    const uint32_t base = b.slot_off[s], last = b.slot_off[s + 1] - 1;
-    if (base == last) return;  // an empty sentence has no nodes
-    const unsigned long long n0 = l.node_off[s];
-    const double a_eos = l.node_prob ? m.a_eos[s] : 0.0;
-    for (uint32_t slot = base; slot <= last; ++slot) {
-        const uint2 me = b.ends_meta[slot];
-        const uint32_t skip_bos = slot == base ? 1u : 0u;
-        const uint32_t rb = l.row_base[slot];
-        for (uint32_t e = me.x + skip_bos + lane; e < me.y; e += 32) {
-            const uint4 c = b.ends_cold[e];  // {start_node slot, best prev entry, word_idx, min_cost}
-            const unsigned long long k = n0 + rb + (e - me.x - skip_bos);
-            const uint32_t end_node = slot - base;
-            const uint32_t start_node = c.x - base;
-            const uint2 i8 = b.info[c.x];
-            const uint32_t start_word = start_node + ((i8.y & kInfoSpecial) ? b.info_ex[c.x].x : 0u);  // as backtrack_write_one
-            uint2* t = l.nodes + k * 3;
-            t[0] = make_uint2(start_word, end_node);
-            t[1] = make_uint2(b.byte_pos[base + start_word], b.byte_pos[slot]);
-            t[2] = make_uint2(c.z, c.w);
-            // the predecessor's row starts at ends_meta[c.x].x; the first slot's row holds only BOS
-            const int32_t prev = c.x == base ? -1 : int32_t(l.row_base[c.x] + (c.y - b.ends_meta[c.x].x));
-            l.links[k] = make_int2(prev, 0);
-            if (l.node_prob) {
-                const double2 ab = m.ab[e];
-                l.node_prob[k] = float(exp(ab.x + ab.y - a_eos));  // the expression of k_backtrack<true>
-            }
-        }
-    }
-    __syncwarp();
-    if (lane == 0) {  // the chain backtrack_count_one walks
-        const uint4 eo = b.eos[s];
-        if (eo.x != kNone) {
-            uint32_t cur = eo.x, end_node = eo.y;
-            while (end_node != 0) {
-                const uint32_t slot = base + end_node;
-                const uint4 c = b.ends_cold[cur];
-                l.links[n0 + l.row_base[slot] + (cur - b.ends_meta[slot].x)].y = int32_t(kNodeBest);  // never the BOS row
-                end_node = c.x - base;
-                cur = c.y;
-            }
-        }
-    }
-}
-
-// The near-best lattice's count and write (MarginArgs): the kept nodes in node order, numbered through g.keep.
-
-// f(entry) for each node of sentence s's best path, from EOS back, as backtrack_count_one walks it.
-template <class F>
-__device__ __forceinline__ void walk_best(const Batch& b, uint32_t s, uint32_t base, F f) {
-    const uint4 eo = b.eos[s];
-    if (eo.x == kNone) return;
-    uint32_t cur = eo.x, end_node = eo.y;
-    while (end_node != 0) {
-        const uint4 c = b.ends_cold[cur];
-        f(cur);
-        end_node = c.x - base;
-        cur = c.y;
-    }
-}
-
+// The near-best lattice's numbering (MarginArgs): the kept nodes in node order, numbered through g.keep.
 __global__ void __launch_bounds__(256) k_lattice_count_margin(Batch b, LatticeArgs l, MargArgs m, MarginArgs g) {
     const uint32_t s = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const uint32_t lane = threadIdx.x & 31;
     if (s >= b.n_sent) return;
     const uint32_t base = b.slot_off[s], last = b.slot_off[s + 1] - 1;
-    // a re-run or refused batch keeps nothing, and neither does an empty sentence or one without a path
-    if ((*b.flags & (kFlagsStandDown | kFlagPoolOverflow)) || base == last || b.eos[s].x == kNone) {
+    // an empty sentence keeps nothing, and neither does one without a path
+    if (rows_unreadable(*b.flags) || base == last || b.eos[s].x == kNone) {
         if (lane == 0) l.n_nodes[s] = 0;
         return;
     }
@@ -2173,7 +2143,7 @@ __global__ void __launch_bounds__(256) k_lattice_count_margin(Batch b, LatticeAr
         }
     }
     __syncwarp();
-    if (lane == 0) walk_best(b, s, base, [&](uint32_t e) { g.keep[e] = 0; });  // the best path is always kept
+    if (lane == 0) walk_best(b, s, base, [&](uint32_t e, uint32_t) { g.keep[e] = 0; });  // the best path is always kept
     __syncwarp();
     uint32_t run = 0;
     for (uint32_t slot = base; slot <= last; ++slot) {  // kept indices in node order
@@ -2189,32 +2159,35 @@ __global__ void __launch_bounds__(256) k_lattice_count_margin(Batch b, LatticeAr
     if (lane == 0) l.n_nodes[s] = run;
 }
 
-__global__ void __launch_bounds__(256) k_lattice_write_margin(Batch b, LatticeArgs l, MargArgs m, MarginArgs g) {
+// The records, links and (with l.node_prob) node marginals, after the scan of n_nodes gave node_off.  MARGIN = false:
+// every node, numbered row_base[slot] + its place in the row.  MARGIN = true: the kept nodes only, numbered by g.keep,
+// with `prev` remapped to the kept list (-2 for a predecessor that was not kept) and g.node_margin.
+template <bool MARGIN>
+__global__ void __launch_bounds__(256) k_lattice_write(Batch b, LatticeArgs l, MargArgs m, MarginArgs g) {
     const uint32_t s = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const uint32_t lane = threadIdx.x & 31;
-    if (s >= b.n_sent || (*b.flags & (kFlagsStandDown | kFlagPoolOverflow))) return;
+    if (s >= b.n_sent || rows_unreadable(*b.flags)) return;
     const uint32_t base = b.slot_off[s], last = b.slot_off[s + 1] - 1;
-    if (base == last || b.eos[s].x == kNone) return;  // nothing kept
+    // an empty sentence has no nodes; one without a path keeps none
+    if (base == last || (MARGIN && b.eos[s].x == kNone)) return;
     const unsigned long long n0 = l.node_off[s];
     const double a_eos = l.node_prob ? m.a_eos[s] : 0.0;
-    const long long best = m.r_eos[s];
+    const long long best = MARGIN ? m.r_eos[s] : 0;
+    // the sentence-relative index of entry e of the row of `slot`, any row but the first (or kNone: not kept)
+    auto node = [&](uint32_t e, uint32_t slot) { return MARGIN ? g.keep[e] : l.row_base[slot] + (e - b.ends_meta[slot].x); };
     for (uint32_t slot = base; slot <= last; ++slot) {
         const uint2 me = b.ends_meta[slot];
-        for (uint32_t e = me.x + (slot == base ? 1u : 0u) + lane; e < me.y; e += 32) {
-            const uint32_t kept = g.keep[e];
-            if (kept == kNone) continue;
+        const uint32_t skip_bos = slot == base ? 1u : 0u;
+        const uint32_t rb = MARGIN ? 0u : l.row_base[slot];
+        for (uint32_t e = me.x + skip_bos + lane; e < me.y; e += 32) {
+            const uint32_t i = MARGIN ? g.keep[e] : rb + (e - me.x - skip_bos);
+            if (MARGIN && i == kNone) continue;
             const uint4 c = b.ends_cold[e];  // {start_node slot, best prev entry, word_idx, min_cost}
-            const unsigned long long k = n0 + kept;
-            const uint32_t start_node = c.x - base;
-            const uint2 i8 = b.info[c.x];
-            const uint32_t start_word = start_node + ((i8.y & kInfoSpecial) ? b.info_ex[c.x].x : 0u);  // as k_lattice_write
-            uint2* t = l.nodes + k * 3;
-            t[0] = make_uint2(start_word, slot - base);
-            t[1] = make_uint2(b.byte_pos[base + start_word], b.byte_pos[slot]);
-            t[2] = make_uint2(c.z, c.w);
-            const uint32_t pk = c.x == base ? 0u : g.keep[c.y];
-            l.links[k] = make_int2(c.x == base ? -1 : pk == kNone ? -2 : int32_t(pk), 0);
-            g.node_margin[k] = m.R[e] + g.G[e] - best;
+            const unsigned long long k = n0 + i;
+            write_node_record(b, l.nodes + k * 3, base, slot, c, c.w);
+            const uint32_t p = c.x == base ? 0u : node(c.y, c.x);  // the first slot's row holds only BOS
+            l.links[k] = make_int2(c.x == base ? -1 : (MARGIN && p == kNone) ? -2 : int32_t(p), 0);
+            if (MARGIN) g.node_margin[k] = m.R[e] + g.G[e] - best;
             if (l.node_prob) {
                 const double2 ab = m.ab[e];
                 l.node_prob[k] = float(exp(ab.x + ab.y - a_eos));  // the expression of k_backtrack<true>
@@ -2222,7 +2195,8 @@ __global__ void __launch_bounds__(256) k_lattice_write_margin(Batch b, LatticeAr
         }
     }
     __syncwarp();
-    if (lane == 0) walk_best(b, s, base, [&](uint32_t e) { l.links[n0 + g.keep[e]].y = int32_t(kNodeBest); });
+    if (lane == 0)  // never the BOS row
+        walk_best(b, s, base, [&](uint32_t e, uint32_t end_node) { l.links[n0 + node(e, base + end_node)].y = int32_t(kNodeBest); });
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -2259,7 +2233,7 @@ __device__ __forceinline__ void sample_walk(const DictView& d, const Batch& b, c
     const uint32_t sidx = uint32_t(w / sa.n), j = uint32_t(w % sa.n);
     const uint32_t s = b.order ? b.order[sidx] : sidx;
     const unsigned long long walk = (unsigned long long)s * sa.n + j;
-    const bool sound = !(*b.flags & (kFlagsStandDown | kFlagPoolOverflow));  // else the rows cannot be trusted
+    const bool sound = !rows_unreadable(*b.flags);
     const uint32_t base = sound ? b.slot_off[s] : 0u, last = sound ? b.slot_off[s + 1] - 1 : 0u;
     const uint4 eos = sound && base != last ? b.eos[s] : make_uint4(kNone, 0, 0, 0);
     if (eos.x == kNone) {  // an empty sentence, one without a path, or a batch that is re-run or refused
@@ -2323,13 +2297,7 @@ __device__ __forceinline__ void sample_walk(const DictView& d, const Batch& b, c
         if (WRITE) {  // the token's prefix cost = the path's cost through c minus the edge into c
             sum -= uint32_t(step);
             const uint4 c = b.ends_cold[e];
-            const uint32_t start_node = c.x - base;
-            const uint2 i8 = b.info[c.x];
-            const uint32_t start_word = start_node + ((i8.y & kInfoSpecial) ? b.info_ex[c.x].x : 0u);  // as backtrack_write_one
-            uint2* out = sa.out + (--at) * 3;
-            out[0] = make_uint2(start_word, row - base);
-            out[1] = make_uint2(b.byte_pos[base + start_word], b.byte_pos[row]);
-            out[2] = make_uint2(c.z, sum);
+            write_node_record(b, sa.out + (--at) * 3, base, row, c, sum);
             row = c.x;
         } else {
             sum += uint32_t(step);
@@ -3131,22 +3099,26 @@ __global__ void __launch_bounds__(kSmallThreads, 1) k_small_batch(DictView d, Ba
 
 }  // namespace
 
-template <bool BND>
-static void launch_small_batch_b(const DictView& d, const Batch& b, const FormatArgs& f, SmallBatchOut* out, cudaStream_t st) {
-    const size_t smem = f.mode == kOutFormat ? sizeof(FormatProgram) : 0;
+// f(conn) with conn = std::integral_constant<int, CONN> of the dictionary's connector kind, for the kernels that are
+// instantiated per connector (0 Matrix, 1 Raw, 2 Dual).
+template <class F>
+static void with_connector(const DictView& d, F f) {
     if (d.connector_kind == 1)
-        k_small_batch<1, BND><<<1, kSmallThreads, smem, st>>>(d, b, f, out);
+        f(std::integral_constant<int, 1>{});
     else if (d.connector_kind == 2)
-        k_small_batch<2, BND><<<1, kSmallThreads, smem, st>>>(d, b, f, out);
+        f(std::integral_constant<int, 2>{});
     else
-        k_small_batch<0, BND><<<1, kSmallThreads, smem, st>>>(d, b, f, out);
+        f(std::integral_constant<int, 0>{});
 }
 
 void launch_small_batch(const DictView& d, const Batch& b, const FormatArgs& f, SmallBatchOut* out, cudaStream_t st) {
-    if (b.bnd_dist)
-        launch_small_batch_b<true>(d, b, f, out, st);
-    else
-        launch_small_batch_b<false>(d, b, f, out, st);
+    const size_t smem = f.mode == kOutFormat ? sizeof(FormatProgram) : 0;
+    with_connector(d, [&](auto conn) {
+        if (b.bnd_dist)
+            k_small_batch<conn, true><<<1, kSmallThreads, smem, st>>>(d, b, f, out);
+        else
+            k_small_batch<conn, false><<<1, kSmallThreads, smem, st>>>(d, b, f, out);
+    });
 }
 
 void launch_format_len(const DictView& d, const FormatArgs& f, cudaStream_t st, const int2* links) {
@@ -3321,93 +3293,63 @@ void launch_backtrack(const Batch& b, const MargArgs* m, const TileScan& ts, cud
 
 // The forward pass's instantiation: with m.lw (sampling) the one that also keeps {left id, word cost}.
 // With u: the uncertainty instantiation of the backward pass.
-template <int CONN>
-static void launch_marg_conn(const DictView& d, const Batch& b, const MargArgs& m, bool backward, const UncertaintyArgs* u,
-                             uint32_t blocks, cudaStream_t st) {
-    if (m.lw)
-        k_marg_forward<CONN, true><<<blocks, 256, 0, st>>>(d, b, m);
-    else
-        k_marg_forward<CONN><<<blocks, 256, 0, st>>>(d, b, m);
-    if (backward && u)
-        k_marg_backward<CONN, true><<<blocks, 256, 0, st>>>(d, b, m, *u);
-    else if (backward)
-        k_marg_backward<CONN><<<blocks, 256, 0, st>>>(d, b, m, UncertaintyArgs{});
-}
-
 void launch_marginals(const DictView& d, const Batch& b, const MargArgs& m, cudaStream_t st, bool backward,
                       const UncertaintyArgs* u) {
     if (!b.n_sent) return;
     const uint32_t blocks = (b.n_sent + 7) / 8;  // a warp per sentence
-    if (d.connector_kind == 1)
-        launch_marg_conn<1>(d, b, m, backward, u, blocks, st);
-    else if (d.connector_kind == 2)
-        launch_marg_conn<2>(d, b, m, backward, u, blocks, st);
-    else
-        launch_marg_conn<0>(d, b, m, backward, u, blocks, st);
+    with_connector(d, [&](auto conn) {
+        if (m.lw)
+            k_marg_forward<conn, true><<<blocks, 256, 0, st>>>(d, b, m);
+        else
+            k_marg_forward<conn><<<blocks, 256, 0, st>>>(d, b, m);
+        if (backward && u)
+            k_marg_backward<conn, true><<<blocks, 256, 0, st>>>(d, b, m, *u);
+        else if (backward)
+            k_marg_backward<conn><<<blocks, 256, 0, st>>>(d, b, m, UncertaintyArgs{});
+    });
     if (backward && u && u->boundary_prob) k_boundary_probs<<<blocks, 256, 0, st>>>(b, m, *u);
-}
-
-void launch_lattice_count(const Batch& b, const LatticeArgs& l, cudaStream_t st) {
-    if (!b.n_sent) return;
-    k_lattice_count<<<(b.n_sent + 7) / 8, 256, 0, st>>>(b, l);  // a warp per sentence
-}
-
-void launch_lattice_write(const Batch& b, const LatticeArgs& l, const MargArgs& m, cudaStream_t st) {
-    if (!b.n_sent) return;
-    k_lattice_write<<<(b.n_sent + 7) / 8, 256, 0, st>>>(b, l, m);
-}
-
-template <int CONN>
-static void launch_margin_conn(const DictView& d, const Batch& b, const MargArgs& m, const MarginArgs& g, bool forward,
-                               uint32_t blocks, cudaStream_t st) {
-    if (forward) k_marg_forward<CONN, false, false><<<blocks, 256, 0, st>>>(d, b, m);
-    k_margin_backward<CONN><<<blocks, 256, 0, st>>>(d, b, m, g);
 }
 
 void launch_margin_backward(const DictView& d, const Batch& b, const MargArgs& m, const MarginArgs& g, bool forward,
                             cudaStream_t st) {
     if (!b.n_sent) return;
     const uint32_t blocks = (b.n_sent + 7) / 8;  // a warp per sentence
-    if (d.connector_kind == 1)
-        launch_margin_conn<1>(d, b, m, g, forward, blocks, st);
-    else if (d.connector_kind == 2)
-        launch_margin_conn<2>(d, b, m, g, forward, blocks, st);
+    with_connector(d, [&](auto conn) {
+        if (forward) k_marg_forward<conn, false, false><<<blocks, 256, 0, st>>>(d, b, m);
+        k_margin_backward<conn><<<blocks, 256, 0, st>>>(d, b, m, g);
+    });
+}
+
+void launch_lattice_count(const Batch& b, const LatticeArgs& l, const MargArgs& m, const MarginArgs* g, cudaStream_t st) {
+    if (!b.n_sent) return;
+    const uint32_t blocks = (b.n_sent + 7) / 8;  // a warp per sentence
+    if (g)
+        k_lattice_count_margin<<<blocks, 256, 0, st>>>(b, l, m, *g);
     else
-        launch_margin_conn<0>(d, b, m, g, forward, blocks, st);
+        k_lattice_count<<<blocks, 256, 0, st>>>(b, l);
 }
 
-void launch_lattice_count(const Batch& b, const LatticeArgs& l, const MargArgs& m, const MarginArgs& g, cudaStream_t st) {
+void launch_lattice_write(const Batch& b, const LatticeArgs& l, const MargArgs& m, const MarginArgs* g, cudaStream_t st) {
     if (!b.n_sent) return;
-    k_lattice_count_margin<<<(b.n_sent + 7) / 8, 256, 0, st>>>(b, l, m, g);
-}
-
-void launch_lattice_write(const Batch& b, const LatticeArgs& l, const MargArgs& m, const MarginArgs& g, cudaStream_t st) {
-    if (!b.n_sent) return;
-    k_lattice_write_margin<<<(b.n_sent + 7) / 8, 256, 0, st>>>(b, l, m, g);
+    const uint32_t blocks = (b.n_sent + 7) / 8;
+    if (g)
+        k_lattice_write<true><<<blocks, 256, 0, st>>>(b, l, m, *g);
+    else
+        k_lattice_write<false><<<blocks, 256, 0, st>>>(b, l, m, MarginArgs{});
 }
 
 void launch_sample_count(const DictView& d, const Batch& b, const MargArgs& m, const SampleArgs& s, cudaStream_t st) {
     const unsigned long long walks = (unsigned long long)b.n_sent * s.n;
     if (!walks) return;
     const uint32_t blocks = uint32_t((walks + 255) / 256);  // a lane per walk
-    if (d.connector_kind == 1)
-        k_sample_count<1><<<blocks, 256, 0, st>>>(d, b, m, s);
-    else if (d.connector_kind == 2)
-        k_sample_count<2><<<blocks, 256, 0, st>>>(d, b, m, s);
-    else
-        k_sample_count<0><<<blocks, 256, 0, st>>>(d, b, m, s);
+    with_connector(d, [&](auto conn) { k_sample_count<conn><<<blocks, 256, 0, st>>>(d, b, m, s); });
 }
 
 void launch_sample_write(const DictView& d, const Batch& b, const MargArgs& m, const SampleArgs& s, cudaStream_t st) {
     const unsigned long long walks = (unsigned long long)b.n_sent * s.n;
     if (!walks) return;
     const uint32_t blocks = uint32_t((walks + 255) / 256);
-    if (d.connector_kind == 1)
-        k_sample_write<1><<<blocks, 256, 0, st>>>(d, b, m, s);
-    else if (d.connector_kind == 2)
-        k_sample_write<2><<<blocks, 256, 0, st>>>(d, b, m, s);
-    else
-        k_sample_write<0><<<blocks, 256, 0, st>>>(d, b, m, s);
+    with_connector(d, [&](auto conn) { k_sample_write<conn><<<blocks, 256, 0, st>>>(d, b, m, s); });
 }
 
 }  // namespace vbt

@@ -317,11 +317,6 @@ struct LatticeArgs {
     int2* links;                  // {prev, flags}
     float* node_prob;             // per node, or nullptr without marginals (then MargArgs is not read)
 };
-// k_lattice_count: row_base and n_nodes (a warp per sentence).
-void launch_lattice_count(const Batch& b, const LatticeArgs& l, cudaStream_t st);
-// k_lattice_write: the records, links and, with l.node_prob, prob = exp(â + b̂ - â(EOS)) as k_backtrack<true>
-// computes it (a warp per sentence), after node_off has been scanned.
-void launch_lattice_write(const Batch& b, const LatticeArgs& l, const MargArgs& m, cudaStream_t st);
 
 // Near-best lattice (option "lattice_margin" = D >= 0): the lattice output keeps the nodes n with a path to EOS and
 // margin(n) = R(n) + G(n) - R(EOS) <= D, and every node of the best path.  G(n) is the least exact (64-bit) cost from
@@ -337,10 +332,13 @@ struct MarginArgs {
 // k_margin_backward: G of every lattice entry.  After K3 and before K4, like launch_marginals.
 void launch_margin_backward(const DictView& d, const Batch& b, const MargArgs& m, const MarginArgs& g, bool forward,
                             cudaStream_t st);
-// k_lattice_count_margin: g.keep and l.n_nodes (the kept count); the scan of n_nodes then gives l.node_off.
-void launch_lattice_count(const Batch& b, const LatticeArgs& l, const MargArgs& m, const MarginArgs& g, cudaStream_t st);
-// k_lattice_write_margin: the kept nodes' records, links and g.node_margin (and l.node_prob), after the scan.
-void launch_lattice_write(const Batch& b, const LatticeArgs& l, const MargArgs& m, const MarginArgs& g, cudaStream_t st);
+// A warp per sentence; g == nullptr: the full lattice, else the near-best one.
+// k_lattice_count: row_base and l.n_nodes; k_lattice_count_margin: g->keep and l.n_nodes (the kept count).  The scan
+// of n_nodes then gives l.node_off.
+void launch_lattice_count(const Batch& b, const LatticeArgs& l, const MargArgs& m, const MarginArgs* g, cudaStream_t st);
+// k_lattice_write<MARGIN>, after the scan: the (kept) nodes' records, links, with g also g->node_margin, and with
+// l.node_prob prob = exp(â + b̂ - â(EOS)) as k_backtrack<true> computes it.
+void launch_lattice_write(const Batch& b, const LatticeArgs& l, const MargArgs& m, const MarginArgs* g, cudaStream_t st);
 
 // Segmentation sampling: n paths per sentence drawn with replacement from P(path) = exp(-theta cost) / Z, by
 // forward-filtering backward-sampling over what k_marg_forward left (R, â and MargArgs::lw), after it and before K4.
