@@ -873,7 +873,7 @@ static int encode_cate_info(const int *cats, int n, const uint32_t *cate_info, c
     uint32_t idset = ci_cate_idset(base);
     for (int i = 0; i < n; i++) {
         if (cats[i] < 0 || !defined[cats[i]]) return 0; /* `.unwrap()` panics in the reference */
-        idset |= 1u << ci_base_id(cate_info[cats[i]]);
+        idset |= 1u << (ci_base_id(cate_info[cats[i]]) & 31); /* release-build `1 << id`: the shift wraps at 32 */
     }
     *out = (base & ~CI_CATE_MASK) | idset; /* reset_cate_idset :66-69: OR-ed unchecked */
     return 1;
@@ -1118,6 +1118,14 @@ static vo_dict *dict_finish(vo_dict *d, const char *lex_csv, size_t lex_len, con
         raw_entries_free(&ents);
         goto fail;
     }
+    /* A category id OR-ed past bit 17 (encode_cate_info) can move a base id past the last category, whose unk.def
+     * slot the reference would index out of bounds; the device image refuses such a dictionary, and so does this. */
+    for (uint32_t c = 0; c < d->chr2inf_len; c++)
+        if (ci_base_id(d->chr2inf[c]) >= d->n_categories) {
+            set_err(err, errcap, "BincodeDecode: CharInfo base_id has no unk.def slot");
+            raw_entries_free(&ents);
+            goto fail;
+        }
     lexicon_build(&d->sys, &ents, 0); /* builder.rs:22 */
     raw_entries_free(&ents);
     if (!lexicon_verify(&d->sys, d->num_left, d->num_right)) { /* :24-29 */
@@ -1321,7 +1329,7 @@ vo_worker *vo_worker_new(const vo_dict *d, int ignore_space, uint64_t max_groupi
             return NULL;
         }
         w->has_space_cateset = 1;
-        w->space_cateset = 1u << id;
+        w->space_cateset = 1u << (id & 31); /* release-build `1 << id` */
     }
     if (max_grouping_len != 0) { /* tokenizer.rs:67-74 */
         w->has_max_grouping = 1;

@@ -69,6 +69,26 @@ class BoundedOracle:
             c = self._conn[(right, left)] = self.od.conn_cost(right, left)
         return c
 
+    def char_infos(self, text):
+        """CharInfo of each character (Sentence::compute_basic, sentence.rs:48-55): out-of-table code points take
+        entry 0 (character.rs:112-116)."""
+        return [self.od.char_info(ord(ch)) for ch in text]
+
+    @staticmethod
+    def groupable(ci):
+        """compute_groupable (sentence.rs:57-71): the length of the run from each character in which every two
+        adjacent characters share a category bit."""
+        n = len(ci)
+        grp = [0] * n
+        for i in range(n - 1, -1, -1):
+            grp[i] = 1 if i == n - 1 or (ci[i] & ci[i + 1] & 0x3FFFF) == 0 else grp[i + 1] + 1
+        return grp
+
+    def skips(self, c):
+        """Whether the ignore_space skip runs from a character of CharInfo c (tokenizer.rs:117-125): SPACE in its id
+        set, secondary categories included."""
+        return bool(self.space_mask and c & self.space_mask)
+
     def lattice(self, sent, bounds, trace=None):
         """sent: bytes.  Returns (ends, eos, c2b): ends[i] = nodes ending at character i, a node being
         [start_node, start_word, word_idx, left, right, min_idx, min_cost, word_cost] (word_cost from the entry
@@ -81,10 +101,8 @@ class BoundedOracle:
             c2b[i + 1] = c2b[i] + len(ch.encode("utf-8"))
         b2c = {b: i for i, b in enumerate(c2b)}
         brk = sorted({b2c[b] for b in bounds if 0 < b < len(sent)})
-        ci = [self.od.char_info(ord(ch)) for ch in text]
-        grp = [0] * n
-        for i in range(n - 1, -1, -1):
-            grp[i] = 1 if i == n - 1 or (ci[i] & ci[i + 1] & 0x3FFFF) == 0 else grp[i + 1] + 1
+        ci = self.char_infos(text)
+        grp = self.groupable(ci)
         ends = [[] for _ in range(n + 1)]
         ends[0].append([0, 0, 0xFFFFFFFF, 0, 0, 0, 0, 0])  # BOS
 
@@ -110,7 +128,7 @@ class BoundedOracle:
                 start_word += 1
                 start_node = start_word
                 continue
-            if self.space_mask and (ci[start_node] & self.space_mask):
+            if self.skips(ci[start_node]):
                 start_word += grp[start_node]
             if start_word == n:
                 break

@@ -106,7 +106,7 @@ class SpanOracle(BoundedOracle):
         for i, ch in enumerate(text):
             c2b[i + 1] = c2b[i] + len(ch.encode("utf-8"))
         b2c = {b: i for i, b in enumerate(c2b)}
-        ci = [self.od.char_info(ord(ch)) for ch in text]
+        ci = self.char_infos(text)
         start_of, inside = {}, set()
         brk = {b2c[b] for b in bounds.bounds if 0 < b < len(sent)}
         prev_end = 0
@@ -115,7 +115,7 @@ class SpanOracle(BoundedOracle):
             if not (prev_end <= a < b <= len(sent)) or a not in b2c or b not in b2c:
                 raise ValueError(f"invalid span {sp}")
             ca, cb = b2c[a], b2c[b]
-            if self.space_mask and ci[ca] & self.space_mask:
+            if self.skips(ci[ca]):
                 raise ValueError(f"span {sp} starts at a skipped space")
             if any(ca < c < cb for c in brk):
                 raise ValueError(f"explicit boundary inside span {sp}")
@@ -124,11 +124,9 @@ class SpanOracle(BoundedOracle):
             brk.update(c for c in (ca, cb) if 0 < c < n)
             prev_end = b
         brk = sorted(brk)
-        grp = [0] * n
-        for i in range(n - 1, -1, -1):
-            grp[i] = 1 if i == n - 1 or (ci[i] & ci[i + 1] & 0x3FFFF) == 0 else grp[i + 1] + 1
+        grp = self.groupable(ci)
         for p in range(n):  # rule 5: a space skip may not land strictly inside a span
-            if p not in inside and self.space_mask and ci[p] & self.space_mask and p + grp[p] in inside:
+            if p not in inside and self.skips(ci[p]) and p + grp[p] in inside:
                 raise ValueError(f"the space skip from character {p} lands inside a span")
         ends = [[] for _ in range(n + 1)]
         ends[0].append([0, 0, 0xFFFFFFFF, 0, 0, 0, 0, 0])  # BOS
@@ -157,7 +155,7 @@ class SpanOracle(BoundedOracle):
                 start_node = start_word
                 continue
             assert start_node not in inside  # rule 2: no node ends there
-            if self.space_mask and (ci[start_node] & self.space_mask):
+            if self.skips(ci[start_node]):
                 start_word += grp[start_node]
             if start_word == n:
                 break

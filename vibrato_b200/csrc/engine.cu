@@ -319,7 +319,7 @@ class EngineImpl final : public Engine {
         if (ignore_space) {  // Tokenizer::ignore_space tokenizer.rs:42-55
             if (h.space_cate_id < 0)
                 throw Error(kInvalidArgument, "dict: SPACE is not defined in the input dictionary (i.e., char.def).");
-            dv_.space_mask = 1u << h.space_cate_id;
+            dv_.space_mask = 1u << (h.space_cate_id & 31);  // release-build `1 << id`
         } else {
             dv_.space_mask = 0;
         }

@@ -756,7 +756,7 @@ CharProperty CharProperty::from_text(std::string_view text) {
             int id = cp.cate_id(t);
             auto jt = id < 0 ? cate2info.end() : cate2info.find(uint32_t(id));
             if (jt == cate2info.end()) throw Error(kInvalidFormat, "char.def: Undefined category: " + std::string(t));
-            idset |= 1u << ((jt->second >> kCateBits) & 0xFF);
+            idset |= 1u << (((jt->second >> kCateBits) & 0xFF) & 31);  // release-build `1 << id`: the shift wraps at 32
         }
         return (info & ~kCateMask) | idset;  // reset_cate_idset :66-69
     };
