@@ -343,7 +343,8 @@ int32_t vbt_tokenizer_set_counting(vbt_tokenizer *t, int32_t on);
  * keep the usual route.
  * Output options (results change as documented with them): "compact_tokens", "lattice" (see vbt_result_lattice),
  * "sample_text" = 0|1 (default 0; 1: the output text renders the samples, see vbt_tokenizer_set_sampling) and
- * "sample_base" = i in 0..2^32 (default 0: the sentence index at which the calls' draws start, see the same). */
+ * "sample_base" = i in 0..2^32 (default 0: the sentence index at which the calls' draws start, see the same) and
+ * "posterior_text" = 0|1 (default 0; 1: the output text renders the posterior path, see vbt_tokenizer_set_posterior). */
 int32_t vbt_tokenizer_set_option(vbt_tokenizer *t, const char *name, int64_t value);
 /* MeCab-style output formats, rendered on the device in place of the option "output_mode": batches tokenised
  * afterwards carry the text of the format in vbt_result_text, on every host route (whole batch, chunked pipeline,
@@ -515,6 +516,47 @@ int32_t vbt_result_samples(const vbt_result *r, const uint64_t **sample_offsets,
  * VBT_ERR_INVALID_ARGUMENT when it ran without sampling. */
 int32_t vbt_last_device_samples(const vbt_tokenizer *t, uint64_t *d_sample_offsets, uint64_t *d_samples,
                                 uint64_t *n_sample_tokens);
+/* Posterior decoding (maximum expected accuracy, gamma-centroid): per sentence the path whose tokens have the largest
+ * total gain, chosen from the marginals above, which must be on.  Lattice, edges and theta are those of the marginals
+ * (the constrained lattice in bounded and span calls).  A node is valid when it has a path to EOS (from the integer
+ * graph, not from p).  For a valid node, p(n) is the float32 value vbt_result_lattice publishes as its node_prob,
+ * exp(â + b̂ - â(EOS)), and gain(n) = (g1 * p(n)) - 1 in float64 with g1 = gamma + 1 computed once and each operation
+ * rounded to nearest (no fused multiply-add).  Equivalently a token earns p - 1/(gamma + 1); gamma = 1 is the
+ * centroid estimator, larger gammas favour recall, smaller ones precision.
+ *   Sweep over character positions: V(0) = 0 (BOS); for q = 1..n in order, over the entries e of ends[q] in row order,
+ *   with s(e) the position e starts at: if e is valid and V(s(e)) > -inf, x(e) = V(s(e)) + gain(e), one add.  V(q) is
+ *   the largest x, A(q) the first entry in row order that attains it (V(q) = -inf and no A(q) without one).  The path
+ *   is A(EOS's row), A(s(that node)), ... back to BOS; predecessors are chosen by position, never through the
+ *   u16-truncated min_idx.
+ *   posterior_offsets[n_sent + 1] index posterior_tokens: 24-byte vbt_token records (also under "compact_tokens") with
+ *   start_char = the node's start_word, bytes and word_idx as for tokens, and total_cost the posterior path's prefix
+ *   cost through the token in the tokenizer's wrapping i32 arithmetic; posterior_probs[k] = p of token k (float32);
+ *   posterior_gains[n_sent] (float64) = V at EOS: 0 for an empty sentence, -inf for one without a path (both without
+ *   tokens).
+ * Guarantees: the tokens are a BOS -> EOS path of the (constrained) lattice; posterior_gains[s] is the left fold
+ * ((0 + gain_1) + gain_2) + ... over the chosen path, and so at least that fold over every path, the best path's
+ * included; where the chosen nodes are the best path's, the records equal the sentence's tokens byte for byte and
+ * posterior_probs equals token_prob bit for bit; max is exact and every node takes one add in a fixed order, so all
+ * four arrays are bit-identical across routes, chunk sizes, sentence orders, K3 variants and device counts.  Tokens,
+ * marginals, the lattice, the samples, the uncertainty and the text (unless "posterior_text" is on) do not change.
+ * on != 0 switches it on with gamma (>= 0, finite), 0 off.  VBT_ERR_INVALID_ARGUMENT: a negative or non-finite gamma,
+ * switching it on while marginals are off, switching marginals off while it is on, switching it off while
+ * "posterior_text" is on.  While on, batches take two more kernel launches and a scan (booked under "viterbi"), the
+ * marginals' forward pass keeps each node's left id and word cost, and "small_batch" steps aside.
+ * Posterior text, the option "posterior_text" = 1 (default 0), needs posterior decoding on: with an output mode or
+ * format set, the output text renders each sentence's posterior path in place of its best path, through the same
+ * renderer (%pP prints the token's p, %pc and detail's total_cost its prefix cost, the "prev" directives take the
+ * previous posterior token).  It excludes "lattice" = 2 and "sample_text" in either order; %pb stays an error.  Every
+ * host route renders it; vbt_tokenize_batch_device stays token-only. */
+int32_t vbt_tokenizer_set_posterior(vbt_tokenizer *t, int32_t on, double gamma);
+/* posterior_offsets[n_sent + 1] into posterior_tokens / posterior_probs, and posterior_gains[n_sent], of a result made
+ * with posterior decoding; owned by the result.  VBT_ERR_INVALID_ARGUMENT for a result made without it. */
+int32_t vbt_result_posterior(const vbt_result *r, const uint64_t **posterior_offsets, const vbt_token **posterior_tokens,
+                             const float **posterior_probs, const double **posterior_gains, uint64_t *n_posterior_tokens);
+/* Device addresses of the same arrays of the last vbt_tokenize_batch_device* call, valid until the next call;
+ * VBT_ERR_INVALID_ARGUMENT when it ran without posterior decoding. */
+int32_t vbt_last_device_posterior(const vbt_tokenizer *t, uint64_t *d_posterior_offsets, uint64_t *d_posterior_tokens,
+                                  uint64_t *d_posterior_probs, uint64_t *d_posterior_gains, uint64_t *n_posterior_tokens);
 /* Launch the kernels on a caller-owned CUDA stream (a cudaStream_t passed as an integer; 0 restores
  * the tokenizer's own stream), so callers can bracket batches with their own events. */
 int32_t vbt_tokenizer_set_stream(vbt_tokenizer *t, uint64_t stream);

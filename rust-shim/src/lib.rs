@@ -74,6 +74,10 @@ extern "C" {
     fn vbt_result_lattice_margins(r: *const vbt_result, node_margin: *mut *const i64) -> i32;
     fn vbt_result_uncertainty(r: *const vbt_result, entropy: *mut *const f64, log_path_prob: *mut *const f64,
                               boundary_offsets: *mut *const u64, boundary_prob: *mut *const f32) -> i32;
+    fn vbt_tokenizer_set_posterior(t: *mut vbt_tokenizer, on: i32, gamma: f64) -> i32;
+    fn vbt_result_posterior(r: *const vbt_result, posterior_offsets: *mut *const u64,
+                            posterior_tokens: *mut *const vbt_token, posterior_probs: *mut *const f32,
+                            posterior_gains: *mut *const f64, n_posterior_tokens: *mut u64) -> i32;
     fn vbt_evaluate(d: *const vbt_dict, t: *mut vbt_tokenizer, corpus: *const c_char, len: usize,
                     feature_indices: *const u64, n_indices: usize, num_ref: *mut u64, num_sys: *mut u64,
                     num_cor: *mut u64) -> i32;
@@ -288,6 +292,20 @@ impl Tokenizer {
         let v = if !on { 0 } else if boundary_probs { 2 } else { 1 };
         check(unsafe { vbt_tokenizer_set_option(self.handle(), b"uncertainty\0".as_ptr() as *const c_char, v) })
     }
+    /// Posterior decoding (see `vbt_tokenizer_set_posterior`; needs `marginals`): batches tokenised afterwards carry
+    /// `BatchResult::posterior`, each sentence's path of the largest total gain at weight `gamma` >= 0; `None` switches
+    /// it off.  `text`: the output text renders the posterior path in place of the best path (option "posterior_text").
+    pub fn posterior(&self, gamma: Option<f64>, text: bool) -> Result<()> {
+        let opt = b"posterior_text\0".as_ptr() as *const c_char;
+        if !text {
+            check(unsafe { vbt_tokenizer_set_option(self.handle(), opt, 0) })?;
+        }
+        check(unsafe { vbt_tokenizer_set_posterior(self.handle(), gamma.is_some() as i32, gamma.unwrap_or(0.0)) })?;
+        if text {
+            check(unsafe { vbt_tokenizer_set_option(self.handle(), opt, 1) })?;
+        }
+        Ok(())
+    }
     /// Segmentation sampling (see `vbt_tokenizer_set_sampling`): `n` (1..1024, 0 = off) paths per sentence drawn from
     /// P(path) at temperature `theta`, keyed by `seed`; batches tokenised afterwards carry `BatchResult::samples`.
     /// `text`: the output text renders each sentence's `n` samples in place of its best path (option "sample_text").
@@ -429,6 +447,23 @@ impl BatchResult {
                 Some((off, if n == 0 { &[][..] } else { std::slice::from_raw_parts(b, n) }))
             };
             Ok((f(e), f(l), bnd))
+        }
+    }
+    /// (posterior offsets, posterior tokens, their marginals, gains): sentence i's posterior-decoded path is
+    /// `tokens[offsets[i]..offsets[i + 1]]` and its total gain `gains[i]`; an error for a batch tokenised without
+    /// `Tokenizer::posterior`.
+    pub fn posterior(&self) -> Result<(&[u64], &[vbt_token], &[f32], &[f64])> {
+        let (mut o, mut t, mut p, mut g, mut n) =
+            (std::ptr::null(), std::ptr::null(), std::ptr::null(), std::ptr::null(), 0u64);
+        check(unsafe { vbt_result_posterior(self.r, &mut o, &mut t, &mut p, &mut g, &mut n) })?;
+        let (mut to, mut tt, mut ns, mut nt) = (std::ptr::null(), std::ptr::null(), 0u64, 0u64);
+        unsafe {
+            vbt_result_view(self.r, &mut to, &mut tt, &mut ns, &mut nt);
+            let n = n as usize;
+            Ok((std::slice::from_raw_parts(o, ns as usize + 1),
+                if n == 0 { &[][..] } else { std::slice::from_raw_parts(t, n) },
+                if n == 0 { &[][..] } else { std::slice::from_raw_parts(p, n) },
+                if ns == 0 { &[][..] } else { std::slice::from_raw_parts(g, ns as usize) }))
         }
     }
     /// (sample offsets, sampled tokens): sample j of sentence i is `samples[offsets[i * n + j]..offsets[i * n + j + 1]]`;

@@ -121,6 +121,9 @@ def lib():
     sig("vbt_tokenizer_set_sampling", i32, [vp, C.c_uint32, C.c_double, u64])
     sig("vbt_result_samples", i32, [vp, pp, pp, C.POINTER(u64)])
     sig("vbt_last_device_samples", i32, [vp] + [C.POINTER(u64)] * 3)
+    sig("vbt_tokenizer_set_posterior", i32, [vp, C.c_int32, C.c_double])
+    sig("vbt_result_posterior", i32, [vp, pp, pp, pp, pp, C.POINTER(u64)])
+    sig("vbt_last_device_posterior", i32, [vp] + [C.POINTER(u64)] * 5)
     sig("vbt_last_stage_ms", i32, [vp, C.POINTER(C.c_float), i32, C.POINTER(i32)])
     sig("vbt_stage_names", cp, [])
     sig("vbt_last_launch_count", i32, [vp, C.POINTER(u64)])

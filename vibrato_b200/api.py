@@ -287,10 +287,13 @@ class BatchResult:
     (sentence_samples()); both are None otherwise.  With Tokenizer.uncertainty() on, `entropies` and `log_path_probs`
     (float64[n_sent]) hold each sentence's path entropy (nats) and best-path log-probability, and with
     boundary_probs=True `boundary_offsets[i]..boundary_offsets[i+1]` index `boundary_probs` (float32): the probability
-    that a token ends at each character position 0..n of sentence i (sentence_boundary_probs()); None otherwise."""
+    that a token ends at each character position 0..n of sentence i (sentence_boundary_probs()); None otherwise.  With
+    Tokenizer.posterior(gamma) on, `posterior_offsets[i]..posterior_offsets[i+1]` index `posterior_tokens`
+    (TOKEN_DTYPE) and `posterior_probs` (float32): sentence i's posterior-decoded path and each token's marginal
+    (sentence_posterior()), and `posterior_gains` (float64[n_sent]) its total gain; all four are None otherwise."""
 
     def __init__(self, tokenizer, handle, sentences_utf8, byte_offsets, compact=False, marginals=False, lattice=False,
-                 samples=0, margins=False, uncertainty=0):
+                 samples=0, margins=False, uncertainty=0, posterior=False):
         self._tok = tokenizer
         self._h = handle
         self._free = lib().vbt_result_free
@@ -359,6 +362,19 @@ class BatchResult:
                                                         shape=(self.n_sent * self.n_samples + 1,))
             self.samples = (np.ctypeslib.as_array(C.cast(ps, C.POINTER(C.c_uint8)), shape=(n * TOKEN_DTYPE.itemsize,))
                             .view(TOKEN_DTYPE) if n else np.empty(0, dtype=TOKEN_DTYPE))
+        self.posterior_offsets = self.posterior_tokens = self.posterior_probs = self.posterior_gains = None
+        if posterior:
+            po, pt, pp, pg, nn = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_uint64()
+            check(lib().vbt_result_posterior(handle, C.byref(po), C.byref(pt), C.byref(pp), C.byref(pg), C.byref(nn)))
+            n, ns = nn.value, self.n_sent
+            self.posterior_offsets = np.ctypeslib.as_array(C.cast(po, C.POINTER(C.c_uint64)), shape=(ns + 1,))
+            self.posterior_tokens = (np.ctypeslib.as_array(C.cast(pt, C.POINTER(C.c_uint8)),
+                                                           shape=(n * TOKEN_DTYPE.itemsize,)).view(TOKEN_DTYPE)
+                                     if n else np.empty(0, dtype=TOKEN_DTYPE))
+            self.posterior_probs = (np.ctypeslib.as_array(C.cast(pp, C.POINTER(C.c_float)), shape=(n,)) if n
+                                    else np.empty(0, dtype=np.float32))
+            self.posterior_gains = (np.ctypeslib.as_array(C.cast(pg, C.POINTER(C.c_double)), shape=(ns,)) if ns
+                                    else np.empty(0, dtype=np.float64))
         self._utf8 = sentences_utf8
         self._off = byte_offsets
 
@@ -373,7 +389,8 @@ class BatchResult:
                 self.token_probs = self.token_probs.copy()
                 self.path_probs = self.path_probs.copy()
             for name in ("node_offsets", "nodes", "node_links", "node_probs", "node_margins", "sample_offsets", "samples",
-                         "entropies", "log_path_probs", "boundary_offsets", "boundary_probs"):
+                         "entropies", "log_path_probs", "boundary_offsets", "boundary_probs", "posterior_offsets",
+                         "posterior_tokens", "posterior_probs", "posterior_gains"):
                 if getattr(self, name) is not None:
                     setattr(self, name, getattr(self, name).copy())
             self._free(h)
@@ -419,6 +436,16 @@ class BatchResult:
         return [[Token(self._tok, s, self.samples[k]) for k in range(int(so[i * n + j]), int(so[i * n + j + 1]))]
                 for j in range(n)]
 
+    def sentence_posterior(self, i):
+        """Token views of sentence i's posterior-decoded path (Tokenizer.posterior), in order; Token.prob() gives
+        each token's marginal."""
+        if self.posterior_tokens is None:
+            raise VibratoError(1, "no posterior paths: switch posterior decoding on with Tokenizer.posterior() "
+                                  "before tokenising")
+        s = bytes(self._utf8[int(self._off[i]):int(self._off[i + 1])])
+        a, b = int(self.posterior_offsets[i]), int(self.posterior_offsets[i + 1])
+        return [Token(self._tok, s, self.posterior_tokens[k], float(self.posterior_probs[k])) for k in range(a, b)]
+
     def sentence_boundary_probs(self, i):
         """float32[n_chars + 1]: P(a token ends at character position p) for p = 0..n of sentence i (needs
         Tokenizer.uncertainty(boundary_probs=True))."""
@@ -460,6 +487,8 @@ class Tokenizer:
         self._uncertainty = 0  # uncertainty(), replayed after the marginals
         self._sampling = (0, 0.0, 0)  # sampling() as (n, theta, seed), replayed after the marginals
         self._sample_text = False  # sampling(text=True), replayed after sampling
+        self._posterior = None  # posterior()'s gamma, replayed after the marginals
+        self._posterior_text = False  # posterior(text=True), replayed after it
         self._stream = 0
         self._counting = False
         self._free = lib().vbt_tokenizer_free
@@ -531,6 +560,10 @@ class Tokenizer:
                 check(lib().vbt_tokenizer_set_sampling(h, *self._sampling))
             if self._sample_text:
                 check(lib().vbt_tokenizer_set_option(h, b"sample_text", 1))
+            if self._posterior is not None:
+                check(lib().vbt_tokenizer_set_posterior(h, 1, self._posterior))
+            if self._posterior_text:
+                check(lib().vbt_tokenizer_set_option(h, b"posterior_text", 1))
             if self._format is not None:
                 self._set_format(h, self._format)
             if self._counting:
@@ -635,7 +668,8 @@ class Tokenizer:
         return BatchResult(self, h, utf8, byte_offsets, compact=bool(self._options.get("compact_tokens", 0)),
                            marginals=self._theta > 0, lattice=self._lattice > 0, samples=self._sampling[0],
                            margins=self._lattice > 0 and self._lattice_margin >= 0,
-                           uncertainty=self._uncertainty if self._theta > 0 else 0)
+                           uncertainty=self._uncertainty if self._theta > 0 else 0,
+                           posterior=self._posterior is not None and self._theta > 0)
 
     def tokenize_batch_device(self, d_utf8, d_byte_offsets, n_sent, n_bytes, d_bnd_offsets=None, d_bnd=None, n_bnd=0,
                               d_span_offsets=None, d_spans=None, n_spans=0, patterns=None):
@@ -695,6 +729,33 @@ class Tokenizer:
         v = [C.c_uint64() for _ in range(3)]
         check(lib().vbt_last_device_samples(self.handle(), *[C.byref(x) for x in v]))
         return tuple(x.value for x in v)
+
+    def last_device_posterior(self):
+        """-> (d_posterior_offsets, d_posterior_tokens, d_posterior_probs, d_posterior_gains, n_posterior_tokens):
+        device addresses (uint64[n_sent + 1], vbt_token[n], float32[n], float64[n_sent]) of the posterior paths of the
+        last tokenize_batch_device call, valid until the next call."""
+        v = [C.c_uint64() for _ in range(5)]
+        check(lib().vbt_last_device_posterior(self.handle(), *[C.byref(x) for x in v]))
+        return tuple(x.value for x in v)
+
+    def posterior(self, gamma=1.0, text=False):
+        """Posterior decoding (maximum expected accuracy; needs marginals() on): every result then also carries each
+        sentence's path whose tokens have the largest total gain (gamma + 1) * p - 1, p the token's marginal
+        (BatchResult.posterior_offsets / posterior_tokens / posterior_probs / posterior_gains, sentence_posterior()).
+        gamma >= 0 and finite; 1 is the centroid estimator, larger values favour recall.  None switches it off.
+        text=True ("posterior_text") renders the posterior path in place of the best path in the output text.  The
+        tokens and every other output do not change; the "small_batch" route steps aside.  Definition:
+        include/vibrato_b200.h."""
+        if not text and self._posterior_text:  # before posterior decoding may switch off, which posterior text refuses
+            check(lib().vbt_tokenizer_set_option(self.handle(), b"posterior_text", 0))
+            self._posterior_text = False
+        on = gamma is not None
+        check(lib().vbt_tokenizer_set_posterior(self.handle(), int(on), float(gamma) if on else 0.0))
+        self._posterior = float(gamma) if on else None
+        if text:
+            check(lib().vbt_tokenizer_set_option(self.handle(), b"posterior_text", 1))
+            self._posterior_text = True
+        return self
 
     def sampling(self, n, theta=1.0, seed=0, text=False):
         """Segmentation sampling ("subword regularisation"): every result then carries n segmentations per sentence
@@ -811,6 +872,9 @@ class Tokenizer:
             return
         if name == "sample_text":  # replayed after sampling, which it needs
             self._sample_text = bool(value)
+            return
+        if name == "posterior_text":  # replayed after posterior decoding, which it needs
+            self._posterior_text = bool(value)
             return
         if name != "connid_counting":  # accumulated counts cannot be carried into a rebuilt engine
             self._options[name] = int(value)
@@ -995,6 +1059,7 @@ class Worker:
         self._nodes = []
         self._samples = []
         self._unc = None  # (entropy, log_path_prob, boundary probabilities or None) with Tokenizer.uncertainty()
+        self._post = []  # the posterior path's tokens with Tokenizer.posterior()
 
     def reset_sentence(self, text, boundaries=None, spans=None):
         """boundaries: required token boundaries, byte offsets into the sentence; spans: required tokens, (start, end)
@@ -1006,6 +1071,7 @@ class Worker:
         self._nodes = []
         self._samples = []
         self._unc = None
+        self._post = []
 
     def tokenize(self):
         if not self._sent:  # worker.rs:50-52
@@ -1029,6 +1095,9 @@ class Worker:
         if res.entropies is not None:
             self._unc = (float(res.entropies[0]), float(res.log_path_probs[0]),
                          None if res.boundary_probs is None else res.sentence_boundary_probs(0).copy())
+        self._post = res.sentence_posterior(0) if res.posterior_tokens is not None else []
+        for t in self._post:
+            t._r = t._r.copy()
         res.close()
 
     def num_tokens(self):
@@ -1071,6 +1140,21 @@ class Worker:
             raise VibratoError(1, "no boundary probabilities: switch them on with "
                                   "Tokenizer.uncertainty(boundary_probs=True) before tokenising")
         return b
+
+    def _posterior_on(self):
+        if self._tok._posterior is None or not self._tok._theta:
+            raise VibratoError(1, "no posterior path: switch posterior decoding on with Tokenizer.posterior() "
+                                  "before tokenising")
+
+    def num_posterior_tokens(self):
+        """Tokens of the sentence's posterior-decoded path (Tokenizer.posterior())."""
+        self._posterior_on()
+        return len(self._post)
+
+    def posterior_token(self, i):
+        """Token i of the sentence's posterior-decoded path; its prob() is the token's marginal."""
+        self._posterior_on()
+        return self._post[i]
 
     def sample_tokens(self, j):
         """The tokens of sample j of the sentence (Tokenizer.sampling())."""

@@ -6,6 +6,7 @@
 #include <cerrno>
 #include <cstdint>
 #include <cstdlib>
+#include <cmath>
 #include <cstring>
 
 #include "cli_common.hpp"
@@ -38,7 +39,10 @@ static void usage() {
                  "                                      distribution at temperature F, in place of the best path: -O and -F\n"
                  "                                      print N renderings per line; S (u64, default 0) keys the draws,\n"
                  "                                      which do not depend on --batch-lines or --devices; not with -a,\n"
-                 "                                      %%pP or %%pb; needs --format-on device)\n");
+                 "                                      %%pP or %%pb; needs --format-on device)\n"
+                 "         [--posterior G]             (with -m -t F: each line's posterior-decoded path at weight G >= 0\n"
+                 "                                      in place of the best path: -O and -F render it, %%pP prints its\n"
+                 "                                      tokens' marginals; not with -a or --sample; needs --format-on device)\n");
 }
 
 int main(int argc, char** argv) {
@@ -56,6 +60,8 @@ int main(int argc, char** argv) {
     uint64_t seed = 0;
     bool has_seed = false;
     int64_t cost_margin = -1;  // --cost-margin, -1 = every node
+    double gamma = 0;          // --posterior
+    bool posterior = false;
     // a whole decimal number in [lo, hi], else a usage error
     auto parse_u64 = [](const std::string& v, uint64_t lo, uint64_t hi, uint64_t& out) {
         if (v.empty() || v.size() > 20 || v.find_first_not_of("0123456789") != std::string::npos) return false;
@@ -107,6 +113,16 @@ int main(int argc, char** argv) {
             }
             cost_margin = int64_t(v);
         }
+        else if (a == "--posterior") {
+            const std::string v = next();
+            char* end = nullptr;
+            gamma = std::strtod(v.c_str(), &end);
+            if (v.empty() || *end || !(gamma >= 0) || !std::isfinite(gamma)) {
+                usage();
+                return 2;
+            }
+            posterior = true;
+        }
         else if (a == "-t" || a == "--theta") {
             const std::string v = next();
             char* end = nullptr;
@@ -129,6 +145,7 @@ int main(int argc, char** argv) {
     if (batch_lines_arg == 0 || (has_node && format_on == "host") || (!has_node && (has_unk || has_bos || has_eos)) ||
         (marginal || sample) != has_theta || (all_morphs && format_on == "host") || (has_seed && !sample) ||
         (sample && (all_morphs || format_on == "host")) || (cost_margin >= 0 && !all_morphs) ||
+        (posterior && (!marginal || all_morphs || sample || format_on == "host")) ||
         (bounded && (marker.size() != 1 || marker[0] == '\n' || (marker[0] & 0x80))) || (bounded && partial)) {
         usage();
         return 2;
@@ -151,6 +168,7 @@ int main(int argc, char** argv) {
         if (marginal) tokenizer.marginals(theta);  // before -F, which may print %pP
         if (all_morphs) tokenizer.lattice(true, true, cost_margin);  // before -F, which may print %pb
         if (sample) tokenizer.sampling(n_sample, theta, seed, true);  // before -F, which may not print %pP / %pb
+        if (posterior) tokenizer.posterior(true, gamma, true);  // the text renders the posterior path
         if (has_node) {
             const std::string_view node = node_format, unk = unk_format, bos = bos_format, eos = eos_format;
             tokenizer.output_format(&node, has_unk ? &unk : nullptr, has_bos ? &bos : nullptr, has_eos ? &eos : nullptr);

@@ -212,6 +212,21 @@ class BatchResult {
         check(vbt_result_samples(r_.get(), &s.sample_offsets, &s.samples, &s.n_sample_tokens));
         return s;
     }
+    // Posterior decoding (Tokenizer::posterior before the batch, see vbt_tokenizer_set_posterior): sentence i's path is
+    // tokens[offsets[i] .. offsets[i + 1]) with probs at the same indices, and gains[i] its total gain.  Throws on a
+    // result made without it.
+    struct Posterior {
+        const uint64_t* offsets = nullptr;
+        const vbt_token* tokens = nullptr;
+        const float* probs = nullptr;
+        const double* gains = nullptr;
+        uint64_t n_tokens = 0;
+    };
+    Posterior posterior() const {
+        Posterior p;
+        check(vbt_result_posterior(r_.get(), &p.offsets, &p.tokens, &p.probs, &p.gains, &p.n_tokens));
+        return p;
+    }
 
    private:
     std::unique_ptr<vbt_result, void (*)(vbt_result*)> r_;
@@ -363,6 +378,23 @@ class Tokenizer {
     DeviceSamples last_device_samples() const {
         DeviceSamples d;
         check(vbt_last_device_samples(handle(), &d.sample_offsets, &d.samples, &d.n_sample_tokens));
+        return d;
+    }
+    // Posterior decoding (see vbt_tokenizer_set_posterior; needs marginals): BatchResult::posterior(), each sentence's
+    // path of the largest total gain at weight gamma >= 0.  text = true also renders it in place of the best path in
+    // the output text (the option "posterior_text").  on = false switches both off.
+    void posterior(bool on, double gamma = 1.0, bool text = false) const {
+        if (!text) check(vbt_tokenizer_set_option(handle(), "posterior_text", 0));  // before posterior may switch off
+        check(vbt_tokenizer_set_posterior(handle(), on ? 1 : 0, gamma));
+        if (text) check(vbt_tokenizer_set_option(handle(), "posterior_text", 1));
+    }
+    // Device addresses of the last tokenize_batch_device call's posterior paths.
+    struct DevicePosterior {
+        uint64_t offsets = 0, tokens = 0, probs = 0, gains = 0, n_tokens = 0;
+    };
+    DevicePosterior last_device_posterior() const {
+        DevicePosterior d;
+        check(vbt_last_device_posterior(handle(), &d.offsets, &d.tokens, &d.probs, &d.gains, &d.n_tokens));
         return d;
     }
     // Worker::init_connid_counter / update_connid_counts / compute_connid_probs (worker.rs:77-103): after

@@ -861,6 +861,39 @@ int32_t vbt_last_device_samples(const vbt_tokenizer* t, uint64_t* d_sample_offse
     });
 }
 
+int32_t vbt_tokenizer_set_posterior(vbt_tokenizer* t, int32_t on, double gamma) {
+    return guarded([&] {
+        need(t, "t");
+        t->e->set_posterior(on != 0, gamma);
+    });
+}
+
+int32_t vbt_result_posterior(const vbt_result* r, const uint64_t** posterior_offsets, const vbt_token** posterior_tokens,
+                             const float** posterior_probs, const double** posterior_gains, uint64_t* n_posterior_tokens) {
+    return guarded([&] {
+        need(r, "r");
+        if (!r->r->out.has(vbt::kPostTokens))
+            throw vbt::Error(vbt::kInvalidArgument, "no posterior paths: switch posterior decoding on with vbt_tokenizer_set_posterior before tokenising");
+        if (posterior_offsets) *posterior_offsets = r->r->ptr<const uint64_t>(vbt::kPostOff);
+        if (posterior_tokens) *posterior_tokens = r->r->ptr<const vbt_token>(vbt::kPostTokens);
+        if (posterior_probs) *posterior_probs = r->r->ptr<const float>(vbt::kPostProb);
+        if (posterior_gains) *posterior_gains = r->r->ptr<const double>(vbt::kPostGain);
+        if (n_posterior_tokens) *n_posterior_tokens = r->r->total[vbt::kGroupPosterior];
+    });
+}
+
+int32_t vbt_last_device_posterior(const vbt_tokenizer* t, uint64_t* d_posterior_offsets, uint64_t* d_posterior_tokens,
+                                  uint64_t* d_posterior_probs, uint64_t* d_posterior_gains, uint64_t* n_posterior_tokens) {
+    return guarded([&] {
+        const vbt::DeviceOutputs& d = last_device(t, vbt::kPostTokens, "posterior decoding");
+        put(d_posterior_offsets, d.addr[vbt::kPostOff]);
+        put(d_posterior_tokens, d.addr[vbt::kPostTokens]);
+        put(d_posterior_probs, d.addr[vbt::kPostProb]);
+        put(d_posterior_gains, d.addr[vbt::kPostGain]);
+        put(n_posterior_tokens, d.total[vbt::kGroupPosterior]);
+    });
+}
+
 int32_t vbt_tokenizer_set_stream(vbt_tokenizer* t, uint64_t stream) {
     return guarded([&] {
         need(t, "t");

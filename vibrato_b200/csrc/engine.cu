@@ -152,12 +152,13 @@ struct Workspace {  // every per-(chunk of a)-batch device array; two of them le
     DevBuf l_row_base, l_n_nodes;  // lattice output only: LatticeArgs
     DevBuf g_G, g_keep;            // near-best lattice only: MarginArgs::G / keep
     DevBuf m_lw, s_cnt, s_total;   // sampling only: MargArgs::lw, SampleArgs::cnt / total
+    DevBuf p_V, p_A, p_cnt, p_total;  // posterior decoding only: PosteriorArgs (MargArgs::lw too)
     cudaStream_t stream = nullptr;
     void release() {
         for (DevBuf* b : {&n_slots, &slot_off, &eos, &n_tok, &code_sys, &code_usr, &cinfo, &groupable, &byte_pos, &info,
                           &info_ex, &ends_cnt, &ends_meta, &seg, &ends_hot, &ends_cold, &scan_tmp, &stats, &iota,
                           &sort_keys, &order, &tiles, &bnd_dist, &span_tag, &m_fill, &m_ncand, &m_cand_entry, &m_R, &m_ab, &m_r_eos, &m_a_eos,
-                          &l_row_base, &l_n_nodes, &g_G, &g_keep, &m_lw, &s_cnt, &s_total})
+                          &l_row_base, &l_n_nodes, &g_G, &g_keep, &m_lw, &s_cnt, &s_total, &p_V, &p_A, &p_cnt, &p_total})
             b->release();
     }
 };
@@ -429,6 +430,8 @@ class EngineImpl final : public Engine {
                 throw Error(kInvalidArgument, "the output format prints %pb, which only lattice text has: change the format before setting lattice below 2");
             if (value == 2 && sample_text_)
                 throw Error(kInvalidArgument, "lattice text and sample text both replace the output text: set \"sample_text\" to 0 before setting lattice = 2");
+            if (value == 2 && post_text_)
+                throw Error(kInvalidArgument, "lattice text and posterior text both replace the output text: set \"posterior_text\" to 0 before setting lattice = 2");
             cudaStreamSynchronize(stream_);
             lattice_ = int(value);
         } else if (name == "lattice_margin") {
@@ -451,10 +454,22 @@ class EngineImpl final : public Engine {
             if (value && !samp_n_) throw Error(kInvalidArgument, "sample_text needs sampling: switch it on with set_sampling first");
             if (value && lattice_ == 2)
                 throw Error(kInvalidArgument, "lattice text and sample text both replace the output text: set \"lattice\" below 2 before setting sample_text = 1");
+            if (value && post_text_)
+                throw Error(kInvalidArgument, "posterior text and sample text both replace the output text: set \"posterior_text\" to 0 before setting sample_text = 1");
             if (value && output_mode_ == kOutFormat && (fmt_uses_ & (kUsesProb | kUsesBest)))  // capi names the directive
                 throw Error(kInvalidArgument, "the output format prints %pP or %pb, which sample text has no value for: change the format before setting sample_text = 1");
             cudaStreamSynchronize(stream_);
             sample_text_ = value != 0;
+        } else if (name == "posterior_text") {
+            // the output text renders each sentence's posterior path in place of its best path
+            if (value < 0 || value > 1) throw Error(kInvalidArgument, "posterior_text must be 0 (off) or 1 (the text renders the posterior path)");
+            if (value && !post_) throw Error(kInvalidArgument, "posterior_text needs posterior decoding: switch it on with set_posterior first");
+            if (value && lattice_ == 2)
+                throw Error(kInvalidArgument, "lattice text and posterior text both replace the output text: set \"lattice\" below 2 before setting posterior_text = 1");
+            if (value && sample_text_)
+                throw Error(kInvalidArgument, "posterior text and sample text both replace the output text: set \"sample_text\" to 0 before setting posterior_text = 1");
+            cudaStreamSynchronize(stream_);
+            post_text_ = value != 0;
         } else if (name == "sample_base") {
             // the sentence index of the draws starts here: a caller that splits a corpus over calls keeps its draws
             if (value < 0 || value > kMaxSampleBase) throw Error(kInvalidArgument, "sample_base must be between 0 and 2^32");
@@ -502,6 +517,8 @@ class EngineImpl final : public Engine {
             throw Error(kInvalidArgument, "the output format prints %pP: change the format before switching marginals off");
         if (theta == 0 && unc_)
             throw Error(kInvalidArgument, "uncertainty needs marginals: set the option \"uncertainty\" to 0 before switching marginals off");
+        if (theta == 0 && post_)
+            throw Error(kInvalidArgument, "posterior decoding needs marginals: switch it off with set_posterior before switching marginals off");
         if (theta > 0 && samp_n_ && theta != samp_theta_)
             throw Error(kInvalidArgument, "marginals and sampling share one forward pass: the marginals' theta " + num(theta) +
                                               " differs from the sampling theta " + num(samp_theta_));
@@ -523,10 +540,22 @@ class EngineImpl final : public Engine {
         samp_seed_ = seed;
     }
     uint32_t sampling() const override { return samp_n_; }
+    void set_posterior(bool on, double gamma) override {
+        if (on && (!(gamma >= 0) || !std::isfinite(gamma)))
+            throw Error(kInvalidArgument, "posterior decoding: gamma must be a finite number >= 0");
+        if (on && theta_ == 0)
+            throw Error(kInvalidArgument, "posterior decoding needs marginals: switch them on with set_marginals first");
+        if (!on && post_text_)
+            throw Error(kInvalidArgument, "the output text renders the posterior path: set \"posterior_text\" to 0 before switching posterior decoding off");
+        cudaStreamSynchronize(stream_);
+        post_ = on;
+        post_g1_ = on ? gamma + 1.0 : 0.0;
+    }
+    bool posterior() const override { return post_; }
     double marginals() const override { return theta_; }
     int lattice() const override { return lattice_; }
     Outputs outputs() const override {
-        return Outputs{tok_bytes_, samp_n_, theta_ > 0, output_mode_ != kOutNone, lattice_ != 0, lat_margin_ >= 0, unc_};
+        return Outputs{tok_bytes_, samp_n_, theta_ > 0, output_mode_ != kOutNone, lattice_ != 0, lat_margin_ >= 0, unc_, post_};
     }
     const DeviceOutputs& last_device() const override { return last_; }
     void set_stream(uint64_t stream) override {
@@ -618,7 +647,7 @@ class EngineImpl final : public Engine {
             if (!chunked) {
                 h2d(in_off_.p, off, (size_t(n_sent) + 1) * 8, stream_, off_pinned && off == byte_off);
                 h2d(in_utf8_.p, utf8 + first, n_bytes, stream_, utf8_pinned);
-                if (n_bytes <= kEagerBytes && output_mode_ == kOutNone && !lattice_ && !samp_n_ && !unc_) {
+                if (n_bytes <= kEagerBytes && output_mode_ == kOutNone && !lattice_ && !samp_n_ && !unc_ && !post_) {
                     // Small batches (a per-sentence Worker loop ends up here) are all latency: the result copies are
                     // queued behind the kernels with an upper bound for the token count (a token spans >= 1 byte), so
                     // that the call makes ONE host synchronisation instead of two.
@@ -693,7 +722,8 @@ class EngineImpl final : public Engine {
                                                  uint64_t(double(n_bytes) * text_ratio) + uint64_t(n_sent) * per_sent + 1024,
                                                  uint64_t(double(n_bytes) * node_per_byte_) + 1024,
                                                  uint64_t(double(n_bytes) * tok_per_byte_ * samp_n_) + 1024,
-                                                 uint64_t(double(n_bytes) * chars_per_byte_) + n_sent + 1024});
+                                                 uint64_t(double(n_bytes) * chars_per_byte_) + n_sent + 1024,
+                                                 uint64_t(double(n_bytes) * tok_per_byte_) + 1024});
             CK(cudaMemsetAsync(base_.p, 0, kNumGroups * 8, stream_));
             connid_begin(stream_);
             h2d(in_off_.p, off, (size_t(n_sent) + 1) * 8, stream_, off_pinned && off == byte_off);
@@ -1102,6 +1132,12 @@ class EngineImpl final : public Engine {
         }
         if (lattice_) o.buf[kNodeOff].ensure((size_t(n_sent) + 1) * 8, 1.25);
         if (samp_n_) o.buf[kSampleOff].ensure((size_t(n_sent) * samp_n_ + 1) * 8, 1.25);
+        if (post_) {  // a path has at most one token per character
+            o.buf[kPostOff].ensure((size_t(n_sent) + 1) * 8, 1.25);
+            o.buf[kPostTokens].ensure(size_t(n_bytes) * 24 + 24, 1.25);
+            o.buf[kPostProb].ensure(size_t(n_bytes) * 4 + 4, 1.25);
+            o.buf[kPostGain].ensure((size_t(n_sent) + 1) * 8, 1.25);
+        }
     }
 
     // The nodes' links when lattice text prints %pb (the %pb instantiation of the format kernels), else nullptr.
@@ -1142,9 +1178,12 @@ class EngineImpl final : public Engine {
             exclusive_scan(w, f.sent_len, f.text_off, walks + 1);
             return f;
         }
-        const bool nodes = lattice_ == 2;  // lattice text: the nodes are rendered as tokens
-        FormatArgs f = format_args(d_utf8, d_off, n_sent, o, o.buf[nodes ? kNodeOff : kTokOff], o.buf[nodes ? kNodes : kTokens]);
-        f.token_prob = (o.made.marg && (fmt_uses_ & kUsesProb)) ? o.buf[nodes ? kNodeProb : kTokenProb].as<float>() : nullptr;  // %pP
+        // lattice text renders the nodes as tokens, posterior text the posterior path
+        const bool nodes = lattice_ == 2, post = post_text_;
+        const int off = nodes ? kNodeOff : post ? kPostOff : kTokOff, recs = nodes ? kNodes : post ? kPostTokens : kTokens;
+        const int prob = nodes ? kNodeProb : post ? kPostProb : kTokenProb;
+        FormatArgs f = format_args(d_utf8, d_off, n_sent, o, o.buf[off], o.buf[recs]);
+        f.token_prob = (o.made.marg && (fmt_uses_ & kUsesProb)) ? o.buf[prob].as<float>() : nullptr;  // %pP
         CK(cudaMemsetAsync(f.sent_len + n_sent, 0, 8, w.stream));
         launch_format_len(dv_, f, w.stream, fmt_links(o));
         exclusive_scan(w, f.sent_len, f.text_off, size_t(n_sent) + 1);
@@ -1472,7 +1511,7 @@ class EngineImpl final : public Engine {
             f(w.m_R, 8);
         }
         if (fwd) f(w.m_ab, 16);
-        if (samp_n_) f(w.m_lw, 4);
+        if (samp_n_ || post_) f(w.m_lw, 4);
         if (margin_on()) {
             f(w.g_G, 8);
             f(w.g_keep, 4);
@@ -1530,9 +1569,20 @@ class EngineImpl final : public Engine {
             w.s_cnt.ensure(walks * 4, 1.25);
             w.s_total.ensure(walks * 4, 1.25);
         }
+        if (post_) {
+            w.p_V.ensure(ms * 8, 1.25);
+            w.p_A.ensure(ms * 4, 1.25);
+            w.p_cnt.ensure(ns * 4, 1.25);
+            w.p_total.ensure(ns * 4, 1.25);
+        }
         size_t tmp = 0;  // cub temp storage for the largest scan / sort of this size
         cub::DeviceScan::ExclusiveSum(nullptr, tmp, static_cast<uint32_t*>(nullptr), static_cast<uint32_t*>(nullptr), ms, w.stream);
         w.scan_tmp.ensure(tmp + 1024, 1.5);
+        if (post_) {  // the scan of the posterior paths' token counts
+            cub::TransformInputIterator<unsigned long long, CastU64, const uint32_t*> it(static_cast<const uint32_t*>(nullptr), CastU64());
+            cub::DeviceScan::ExclusiveSum(nullptr, tmp, it, static_cast<unsigned long long*>(nullptr), ns, w.stream);
+            w.scan_tmp.ensure(tmp + 1024, 1.5);
+        }
         if (samp_n_) {  // the scan of the walks' token counts
             cub::TransformInputIterator<unsigned long long, CastU64, const uint32_t*> it(static_cast<const uint32_t*>(nullptr), CastU64());
             cub::DeviceScan::ExclusiveSum(nullptr, tmp, it, static_cast<unsigned long long*>(nullptr),
@@ -1721,7 +1771,7 @@ class EngineImpl final : public Engine {
             m.a_eos = w.m_a_eos.as<double>();
             m.path_prob = o.buf[kPathProb].as<float>();
             m.token_prob = marg ? o.buf[kTokenProb].as<float>() : nullptr;
-            m.lw = samp ? w.m_lw.as<uint32_t>() : nullptr;
+            m.lw = (samp || post_) ? w.m_lw.as<uint32_t>() : nullptr;  // the prefix costs of samples and posterior paths
         }
         if (marg || samp) {  // booked with the Viterbi stage; must run before K4 reuses ends_meta
             UncertaintyArgs u{};
@@ -1782,6 +1832,25 @@ class EngineImpl final : public Engine {
             sa.out = o.buf[kSamples].as<uint2>();
             launch_sample_write(dv_, b, m, sa, st);
             if (walks) o.launches += 2;
+        }
+        if (post_) {  // booked with the Viterbi stage too, and also before K4; marginals are on (set_posterior)
+            PosteriorArgs p{};
+            p.g1 = post_g1_;
+            p.V = w.p_V.as<double>();
+            p.A = w.p_A.as<uint32_t>();
+            p.cnt = w.p_cnt.as<uint32_t>();
+            p.total = w.p_total.as<int32_t>();
+            p.off = o.buf[kPostOff].as<unsigned long long>();
+            p.out = o.buf[kPostTokens].as<uint2>();
+            p.prob = o.buf[kPostProb].as<float>();
+            p.gain = o.buf[kPostGain].as<double>();
+            launch_posterior_sweep(dv_, b, m, p, st);
+            CK(cudaMemsetAsync(p.cnt + n_sent, 0, 4, st));
+            cub::TransformInputIterator<unsigned long long, CastU64, const uint32_t*> it(p.cnt, CastU64());
+            exclusive_scan(w, it, p.off, size_t(n_sent) + 1);
+            CK(cudaMemcpyAsync(&dc->total[kGroupPosterior], p.off + n_sent, 8, cudaMemcpyDeviceToDevice, st));
+            launch_posterior_write(dv_, b, m, p, st);
+            if (n_sent) o.launches += 2;
         }
         // backtrack_count and scan_tokens are folded into k_backtrack, which is booked under backtrack_write
         CK(cudaEventRecord(o.ev[6], st));
@@ -1893,6 +1962,9 @@ class EngineImpl final : public Engine {
     double samp_theta_ = 0;
     uint64_t samp_seed_ = 0;
     bool sample_text_ = false;  // option "sample_text": the output text renders the samples
+    bool post_ = false;         // posterior decoding (set_posterior)
+    double post_g1_ = 0;        // its gamma + 1
+    bool post_text_ = false;    // option "posterior_text": the output text renders the posterior paths
     static constexpr long long kMaxSampleBase = 0x100000000ll;
     uint64_t sample_base_ = 0;  // option "sample_base": the draws' index of the call's first sentence
     DeviceOutputs last_;  // what the last run_device or run_shard left in out_[0] (last_device)

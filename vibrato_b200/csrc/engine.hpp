@@ -13,12 +13,12 @@
 namespace vbt {
 
 // ---- the outputs of a batch ------------------------------------------------------------------------
-// A batch produces up to seventeen arrays in five ragged groups.  A group's offsets index its records: entries
+// A batch produces up to twenty-one arrays in six ragged groups.  A group's offsets index its records: entries
 // off[i] .. off[i + 1] belong to sentence i (to sample j of sentence i at i * n_samp + j for the samples), and the
 // group's total is the number of its records.  path_prob, entropy and log_path_prob have one entry per sentence and no
 // offsets.  The positions group has one record per character position 0..n of every sentence: its offsets are the
-// slot offsets and its total is the batch's slot count.
-enum Group { kGroupTokens, kGroupText, kGroupLattice, kGroupSamples, kGroupPositions, kNumGroups };
+// slot offsets and its total is the batch's slot count.  The posterior group holds each sentence's posterior path.
+enum Group { kGroupTokens, kGroupText, kGroupLattice, kGroupSamples, kGroupPositions, kGroupPosterior, kNumGroups };
 enum Array {
     kTokOff, kTokens, kTokenProb, kPathProb,  // vbt_token (or vbt_token16) records; marginals (set_marginals)
     kEntropy, kLogPathProb,                   // uncertainty ("uncertainty" >= 1): float64 per sentence
@@ -27,6 +27,8 @@ enum Array {
     kNodeMargin,                              // near-best lattice ("lattice_margin" >= 0): each kept node's margin (int64)
     kSampleOff, kSamples,                     // sampling (set_sampling): vbt_token records of every sampled path
     kPosOff, kBoundaryProb,                   // uncertainty 2: float32 boundary probability of every character position
+    kPostOff, kPostTokens, kPostProb,         // posterior decoding (set_posterior): vbt_token records and their marginals
+    kPostGain,                                // ... and each sentence's total gain (float64)
     kNumArrays
 };
 enum ArrayKind { kOffsets, kRecords, kPerSentence };
@@ -41,8 +43,10 @@ constexpr ArrayInfo kArrays[kNumArrays] = {
     {kGroupText, kOffsets, 8},     {kGroupText, kRecords, 1},    {kGroupLattice, kOffsets, 8},  {kGroupLattice, kRecords, 24},
     {kGroupLattice, kRecords, 8},  {kGroupLattice, kRecords, 4}, {kGroupLattice, kRecords, 8},  {kGroupSamples, kOffsets, 8},
     {kGroupSamples, kRecords, 24}, {kGroupPositions, kOffsets, 8}, {kGroupPositions, kRecords, 4},
+    {kGroupPosterior, kOffsets, 8}, {kGroupPosterior, kRecords, 24}, {kGroupPosterior, kRecords, 4},
+    {kGroupPosterior, kPerSentence, 8},
 };
-constexpr Array kOffsetsOf[kNumGroups] = {kTokOff, kTextOff, kNodeOff, kSampleOff, kPosOff};
+constexpr Array kOffsetsOf[kNumGroups] = {kTokOff, kTextOff, kNodeOff, kSampleOff, kPosOff, kPostOff};
 
 using Totals = std::array<uint64_t, kNumGroups>;  // one count per group
 
@@ -53,6 +57,7 @@ struct Outputs {
     bool marg = false, text = false, lat = false;
     bool margin = false;  // "lattice_margin" >= 0: the lattice keeps the near-best nodes and carries their margins
     uint32_t unc = 0;     // "uncertainty": 1 entropy and log_path_prob, 2 also the boundary probabilities
+    bool post = false;    // posterior decoding (set_posterior)
 
     bool has(int a) const {
         switch (a) {
@@ -71,6 +76,10 @@ struct Outputs {
             case kNodeMargin: return lat && margin;
             case kSampleOff:
             case kSamples: return n_samp != 0;
+            case kPostOff:
+            case kPostTokens:
+            case kPostProb:
+            case kPostGain: return marg && post;
             default: return true;
         }
     }
@@ -223,7 +232,9 @@ class Engine {
     // 2 the same and the output text renders the nodes in place of the tokens), "lattice_margin" (-1 off; D in
     // 0 .. 2^62: the lattice keeps only the nodes within cost D of the best path, kernels.cuh MarginArgs),
     // "uncertainty" (0 off; with marginals on, 1 results also carry kEntropy / kLogPathProb, 2 also kPosOff /
-    // kBoundaryProb, kernels.cuh UncertaintyArgs; k_small_batch and the eager small-batch copies step aside).
+    // kBoundaryProb, kernels.cuh UncertaintyArgs; k_small_batch and the eager small-batch copies step aside),
+    // "posterior_text" (0 off; 1 with posterior decoding on: the output text renders the posterior path in place of
+    // the best path; excludes lattice text and sample text).
     virtual void set_option(const std::string& name, long long value) = 0;
     // An output format (format.hpp) in place of "output_mode" 1-3, on every host route; nullptr switches it off.
     // Setting "output_mode" replaces it.  Builds the format's field table on the device.
@@ -242,6 +253,11 @@ class Engine {
     // run_device leaves them in device memory (last_device).
     virtual void set_sampling(uint32_t n, double theta, uint64_t seed) = 0;
     virtual uint32_t sampling() const = 0;  // n, 0 when off
+    // Posterior decoding (kernels.cuh PosteriorArgs) with weight gamma (>= 0, finite), which needs marginals on; off
+    // switches it off.  On every route except k_small_batch and the eager small-batch copies, which step aside.
+    // Results then carry kPostOff / kPostTokens / kPostProb / kPostGain, and run_device leaves them in device memory.
+    virtual void set_posterior(bool on, double gamma) = 0;
+    virtual bool posterior() const = 0;
     // Launch on a caller-owned CUDA stream (0 restores the engine's own stream).
     virtual void set_stream(uint64_t stream) = 0;
     virtual const float* stage_ms() const = 0;

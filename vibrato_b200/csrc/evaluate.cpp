@@ -77,7 +77,9 @@ EvalCounts evaluate(const Dictionary& d, Engine& e, std::string_view corpus, con
         uint32_t start_char, end_char, start_byte, end_byte, word_idx;
         int32_t total_cost;
     };
-    const Tok* toks = r->ptr<const Tok>(kTokens);
+    const bool post = r->out.has(kPostTokens);  // posterior decoding on: its paths are scored
+    const Tok* toks = r->ptr<const Tok>(post ? kPostTokens : kTokens);
+    const uint64_t* tok_off = r->ptr<const uint64_t>(post ? kPostOff : kTokOff);
 
     EvalCounts c{0, 0, 0};
     std::vector<std::string> refs, syss, both;
@@ -91,7 +93,7 @@ EvalCounts evaluate(const Dictionary& d, Engine& e, std::string_view corpus, con
             refs.push_back(make_key(start, start + len, t.feature, feature_indices));
             start += len;
         }
-        for (uint64_t k = r->ptr<uint64_t>(kTokOff)[i]; k < r->ptr<uint64_t>(kTokOff)[i + 1]; ++k)
+        for (uint64_t k = tok_off[i]; k < tok_off[i + 1]; ++k)
             syss.push_back(make_key(toks[k].start_char, toks[k].end_char, d.word_feature(toks[k].word_idx), feature_indices));
         auto uniq = [](std::vector<std::string>& v) {  // HashSet semantics: duplicates count once
             std::sort(v.begin(), v.end());

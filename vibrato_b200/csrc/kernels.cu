@@ -2326,6 +2326,112 @@ __global__ void __launch_bounds__(256) k_sample_write(DictView d, Batch b, MargA
     sample_walk<CONN, true>(d, b, m, sa);
 }
 
+// ---------------------------------------------------------------------------------------------
+// Posterior decoding (PosteriorArgs in kernels.cuh)
+// ---------------------------------------------------------------------------------------------
+
+// p of lattice entry e, as k_lattice_write publishes it
+__device__ __forceinline__ float posterior_p(const MargArgs& m, uint32_t e, double a_eos) {
+    const double2 ab = m.ab[e];
+    return float(exp(ab.x + ab.y - a_eos));
+}
+
+// The edge into the node {left, wc} from entry e: conn(right(e), left) + wc, wrapping like the tokenizer's i32.
+template <int CONN>
+__device__ __forceinline__ uint32_t posterior_step(const DictView& d, const Batch& b, uint32_t e, uint32_t left, int32_t wc) {
+    return uint32_t(ConnRow<CONN>(d, left).cost(d, uint32_t(b.ends_hot[e].y))) + uint32_t(wc);
+}
+
+template <int CONN>
+__global__ void __launch_bounds__(256) k_posterior_sweep(DictView d, Batch b, MargArgs m, PosteriorArgs p) {
+    const uint32_t lane = threadIdx.x & 31;
+    const uint32_t sidx = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (sidx >= b.n_sent) return;
+    const uint32_t s = b.order ? b.order[sidx] : sidx;
+    const bool sound = !rows_unreadable(*b.flags);
+    const uint32_t base = sound ? b.slot_off[s] : 0u, last = sound ? b.slot_off[s + 1] - 1 : 0u;
+    const uint4 eos = sound && base != last ? b.eos[s] : make_uint4(kNone, 0, 0, 0);
+    if (eos.x == kNone) {  // an empty sentence, one without a path, or a batch that is re-run or refused
+        if (lane == 0) {
+            p.cnt[s] = 0;
+            p.total[s] = 0;
+            p.gain[s] = base == last ? 0.0 : -INFINITY;
+        }
+        return;
+    }
+    const double a_eos = m.a_eos[s], g1 = p.g1;
+    const uint32_t slot_end = base + eos.y;
+    if (lane == 0) p.V[base] = 0.0;  // BOS
+    __syncwarp();
+    for (uint32_t slot = base + 1; slot <= slot_end; ++slot) {
+        const uint2 me = b.ends_meta[slot];
+        double bx = -INFINITY;
+        uint32_t be = kNone;
+        for (uint32_t e = me.x + lane; e < me.y; e += 32) {  // a lane's entries in row order: keep the first maximum
+            const double vs = p.V[b.ends_cold[e].x];
+            if (vs == -INFINITY) continue;
+            const double g = __dsub_rn(__dmul_rn(g1, double(posterior_p(m, e, a_eos))), 1.0);
+            const double x = __dadd_rn(vs, g);
+            if (x > bx) {
+                bx = x;
+                be = e;
+            }
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {  // the largest x, then the lowest entry
+            const double ox = __shfl_xor_sync(kFull, bx, o);
+            const uint32_t oe = __shfl_xor_sync(kFull, be, o);
+            if (ox > bx || (ox == bx && oe < be)) {
+                bx = ox;
+                be = oe;
+            }
+        }
+        if (lane == 0) {
+            p.V[slot] = bx;
+            p.A[slot] = be;
+        }
+        __syncwarp();
+    }
+    if (lane != 0) return;
+    p.gain[s] = p.V[slot_end];
+    uint32_t row = slot_end, left = 0, tokens = 0, sum = 0;  // EOS: left id 0, no word cost
+    int32_t wc = 0;
+    while (row != base) {
+        const uint32_t e = p.A[row];
+        sum += posterior_step<CONN>(d, b, e, left, wc);
+        ++tokens;
+        const uint32_t lw = m.lw[e];
+        left = lw & 0xFFFFu;
+        wc = int16_t(lw >> 16);
+        row = b.ends_cold[e].x;
+    }
+    sum += uint32_t(ConnRow<CONN>(d, left).cost(d, 0u)) + uint32_t(wc);  // the first token's edge from BOS
+    p.cnt[s] = tokens;
+    p.total[s] = int32_t(sum);
+}
+
+template <int CONN>
+__global__ void __launch_bounds__(256) k_posterior_write(DictView d, Batch b, MargArgs m, PosteriorArgs p) {
+    const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= b.n_sent || p.cnt[s] == 0) return;
+    const uint32_t base = b.slot_off[s];
+    const double a_eos = m.a_eos[s];
+    uint32_t row = base + b.eos[s].y, left = 0, sum = uint32_t(p.total[s]);
+    int32_t wc = 0;
+    unsigned long long at = p.off[s] + p.cnt[s];
+    while (row != base) {  // a token's prefix cost = the path's cost through its successor minus the edge between them
+        const uint32_t e = p.A[row];
+        sum -= posterior_step<CONN>(d, b, e, left, wc);
+        const uint4 c = b.ends_cold[e];
+        write_node_record(b, p.out + (--at) * 3, base, row, c, sum);
+        p.prob[at] = posterior_p(m, e, a_eos);
+        const uint32_t lw = m.lw[e];
+        left = lw & 0xFFFFu;
+        wc = int16_t(lw >> 16);
+        row = c.x;
+    }
+}
+
 
 // ---------------------------------------------------------------------------------------------
 // Output stage: the text `tokenize` writes per sentence (tokenize/src/main.rs:83-127):
@@ -3350,6 +3456,18 @@ void launch_sample_write(const DictView& d, const Batch& b, const MargArgs& m, c
     if (!walks) return;
     const uint32_t blocks = uint32_t((walks + 255) / 256);
     with_connector(d, [&](auto conn) { k_sample_write<conn><<<blocks, 256, 0, st>>>(d, b, m, s); });
+}
+
+void launch_posterior_sweep(const DictView& d, const Batch& b, const MargArgs& m, const PosteriorArgs& p, cudaStream_t st) {
+    if (!b.n_sent) return;
+    const uint32_t blocks = (b.n_sent + 7) / 8;  // a warp per sentence
+    with_connector(d, [&](auto conn) { k_posterior_sweep<conn><<<blocks, 256, 0, st>>>(d, b, m, p); });
+}
+
+void launch_posterior_write(const DictView& d, const Batch& b, const MargArgs& m, const PosteriorArgs& p, cudaStream_t st) {
+    if (!b.n_sent) return;
+    const uint32_t blocks = (b.n_sent + 255) / 256;  // a thread per sentence
+    with_connector(d, [&](auto conn) { k_posterior_write<conn><<<blocks, 256, 0, st>>>(d, b, m, p); });
 }
 
 }  // namespace vbt

@@ -364,6 +364,32 @@ void launch_sample_count(const DictView& d, const Batch& b, const MargArgs& m, c
 // k_sample_write: the same walks again, writing each walk's records at off[walk] from its last token back.
 void launch_sample_write(const DictView& d, const Batch& b, const MargArgs& m, const SampleArgs& s, cudaStream_t st);
 
+// Posterior decoding (set_posterior): per sentence the path whose tokens have the largest total gain, over the lattice,
+// edges and marginals of k_marg_forward / k_marg_backward, after them and before K4.  A node's p is the float32
+// exp(â + b̂ - â(EOS)) that k_lattice_write publishes, its gain (g1 p) - 1 in float64 with g1 = gamma + 1 and no FMA.
+// Sweep: V(BOS) = 0; for q = 1 .. EOS's row in order, over the entries e of row q in row order, x(e) = V(s(e)) + gain(e)
+// (one round-to-nearest add) where V(s(e)) > -inf, s(e) the row e starts at; V(q) = max x, A(q) = the first entry that
+// attains it (-inf / none without one).  The path is A(EOS's row), A(s(that entry)), ... back to BOS.  A node is valid
+// when it has a path to EOS; every entry of a row has the same successors, so validity belongs to the row, and a row
+// off every path to EOS never feeds V of a row on one: the sweep need not test it.  max is exact and each x is one add
+// in a fixed order, so every output is independent of the route, the chunking and the sentence order.
+struct PosteriorArgs {
+    double g1;                 // gamma + 1, computed on the host
+    double* V;                 // per slot: V(q) (scratch)
+    uint32_t* A;               // per slot: A(q) (scratch)
+    uint32_t* cnt;             // per sentence (+ 1 for the scan): the path's tokens
+    int32_t* total;            // per sentence: the path's total cost (wrapping i32)
+    unsigned long long* off;   // n_sent + 1: exclusive scan of cnt
+    uint2* out;                // vbt_token as 3 x uint2, always 24 bytes; total_cost = the prefix cost (wrapping i32)
+    float* prob;               // per token: its p
+    double* gain;              // per sentence: V at EOS; 0 for an empty sentence, -inf without a path
+};
+// k_posterior_sweep (a warp per sentence in b.order): V, A, gain, cnt and total (0 for every sentence of a re-run batch).
+// Needs MargArgs::lw (the sampling instantiation of k_marg_forward) for the prefix costs.
+void launch_posterior_sweep(const DictView& d, const Batch& b, const MargArgs& m, const PosteriorArgs& p, cudaStream_t st);
+// k_posterior_write (a thread per sentence), after the scan of cnt: the records and probabilities from the last back.
+void launch_posterior_write(const DictView& d, const Batch& b, const MargArgs& m, const PosteriorArgs& p, cudaStream_t st);
+
 // What k_small_batch reports besides its outputs: the batch flags and the totals of its scans.
 struct SmallBatchOut {
     uint32_t flags;

@@ -385,6 +385,10 @@ class MultiEngine final : public Engine {
         for (auto& e : eng_) e->set_sampling(n, theta, seed);  // the first refuses what all would
     }
     uint32_t sampling() const override { return eng_[0]->sampling(); }
+    void set_posterior(bool on, double gamma) override {
+        for (auto& e : eng_) e->set_posterior(on, gamma);  // the first refuses what all would
+    }
+    bool posterior() const override { return eng_[0]->posterior(); }
     int lattice() const override { return eng_[0]->lattice(); }
     void set_stream(uint64_t stream) override {
         if (stream) throw Error(kUnsupported, "a multi-device tokenizer runs on its own streams");
