@@ -195,7 +195,9 @@ int32_t vbt_tokenizer_new_from_device_blob(uint64_t d_blob, uint64_t n_bytes, in
  * engine per device on its own host thread (pinned to the GPU's NUMA node) and returns ONE result in input order,
  * identical to a single-device one, the text of the output stage ("output_mode") included: each device formats its
  * shard.  vbt_tokenize_batch_device expects its input on devices[0] and gathers the token records back to it over
- * NVLink (ncclSend / ncclRecv).  Not available on such a tokenizer: a caller-owned stream. */
+ * NVLink (ncclSend / ncclRecv).  Not available on such a tokenizer: a caller-owned stream.  A device listed more than
+ * once runs one shard per entry on it (peer copies in place of NCCL): this runs the sharded path on one GPU and is
+ * not faster. */
 int32_t vbt_tokenizer_new_multi(const vbt_dict *d, int32_t ignore_space, uint64_t max_grouping_len,
                                 const int32_t *devices, int32_t n_devices, vbt_tokenizer **out);
 /* JSON description of how the tokenizer is laid out: {"devices": [...], "dictionary_transport": "nccl 22703" |

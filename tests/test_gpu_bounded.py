@@ -1,6 +1,6 @@
 """Required token boundaries on the GPU (vbt_tokenize_batch_bounded / vbt_tokenize_batch_device_bounded): tokens
 bit-identical to the bounded oracle (tests/bounded_oracle.py) on every route — whole batch, the chunked host pipeline,
-"small_batch", device-resident input and, with two GPUs, a multi-device tokenizer (host and device-resident input) —
+"small_batch", device-resident input and a multi-device tokenizer (host and device-resident input) —
 plus the output text, connection id counts, the input errors and `tokenize --boundary-marker`."""
 import os
 import subprocess
@@ -12,17 +12,13 @@ import adversarial as adv
 import vibrato_b200 as vb
 from bounded_oracle import BoundedOracle
 from oracle import vibrato_oracle as vo
+from test_gpu_marginals import shard_devices, shard_devices_arg
 
 pytestmark = pytest.mark.gpu
 ROUTES = ("whole", "chunked", "small", "device", "multi", "multi_device")
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CHUNK_COPIES = 2100  # "chunked": batches are repeated to at least this many sentences, so that the pipeline cuts them
 # into several chunks (its first chunk holds 1024 sentences)
-
-
-def n_gpus():
-    import torch
-    return torch.cuda.device_count()
 
 
 def lead_bytes(b):
@@ -58,7 +54,7 @@ def d2h(ptr, n, dtype):
 
 def make_tokenizer(d, route, ignore_space=False, mgl=0):
     if route.startswith("multi"):
-        tok = vb.Tokenizer.new(d, devices=[0, 1])
+        tok = vb.Tokenizer.new(d, devices=shard_devices(2))
     else:
         tok = vb.Tokenizer.new(d)
     tok.ignore_space(ignore_space).max_grouping_len(mgl)
@@ -104,11 +100,6 @@ def check(tok, route, bo, sents, bounds):
         np.testing.assert_array_equal(toks[name], e_toks[name], err_msg=name)
 
 
-def skip_multi(route):
-    if route.startswith("multi") and n_gpus() < 2:
-        pytest.skip("needs two GPUs")
-
-
 def golden_dicts(golden, user):
     r = golden["resources"]
     d = vb.SystemDictionaryBuilder.from_readers(r["lex.csv"], r["matrix.def"], r["char.def"], r["unk.def"])
@@ -121,7 +112,6 @@ def golden_dicts(golden, user):
 
 @pytest.mark.parametrize("route", ROUTES)
 def test_golden_fixture(golden, route):
-    skip_multi(route)
     # (the fixture's unk.def has no KATAKANA entry, so a katakana run keeps a path only where lexicon words cover it:
     # アイアイウ is split after アイ, never inside アイウ)
     sents = [c["input"] for c in golden["tokenizer_cases"]] + ["京都東京都京都", "abcdefgh", "東京   都"]
@@ -139,7 +129,6 @@ def test_golden_fixture(golden, route):
 @pytest.mark.parametrize("ignore_space", [False, True])
 @pytest.mark.parametrize("dictionary", list(adv.FAMILIES) + ["raw", "dual"])
 def test_adversarial(dictionary, ignore_space, route):
-    skip_multi(route)
     if dictionary in adv.FAMILIES:
         d, connector = adv.make_dictionary(dictionary), "matrix"
     else:
@@ -163,7 +152,6 @@ def test_adversarial(dictionary, ignore_space, route):
 @pytest.mark.parametrize("route", ROUTES)
 @pytest.mark.parametrize("mgl", [0, 1, 24])
 def test_max_grouping_len_and_compact(route, mgl):
-    skip_multi(route)
     d = adv.make_dictionary("ties", seed=3)
     dev = vb.SystemDictionaryBuilder.from_readers(d.lex_csv, d.matrix, d.char_def, d.unk_def)
     od = vo.OracleDictionary(d.lex_csv, d.matrix, d.char_def, d.unk_def)
@@ -199,7 +187,6 @@ def test_long_sentence_and_extreme_costs(route):
 
 @pytest.mark.parametrize("route", ["whole", "chunked", "small", "multi"])
 def test_output_text_and_connid_counts(golden, route):
-    skip_multi(route)
     d = adv.make_dictionary("ties", seed=2)
     dev = vb.SystemDictionaryBuilder.from_readers(d.lex_csv, d.matrix, d.char_def, d.unk_def)
     od = vo.OracleDictionary(d.lex_csv, d.matrix, d.char_def, d.unk_def)
@@ -243,7 +230,6 @@ def test_output_text_and_connid_counts(golden, route):
 
 @pytest.mark.parametrize("route", ROUTES)
 def test_invalid_boundaries(golden, route):
-    skip_multi(route)
     d, od, r = golden_dicts(golden, False)
     tok = make_tokenizer(d, route)
     sents = ["東京都に行く", "京都", "abc"]
@@ -318,7 +304,7 @@ def test_worker_reset_sentence_with_boundaries(golden):
 
 def test_tokenize_cli_boundary_marker(golden, tmp_path):
     """`tokenize --boundary-marker '|'`: the same bytes with every batching (whole input, --batch-lines, one line at a
-    time on a terminal, two devices when present) and each output mode, equal to the bounded tokens of the API."""
+    time on a terminal, a two-entry --devices) and each output mode, equal to the bounded tokens of the API."""
     from test_gpu_small_batch import _run_on_pty
     exe = os.path.join(ROOT, "vibrato_b200", "bin", "tokenize")
     if not os.path.exists(exe):
@@ -347,7 +333,7 @@ def test_tokenize_cli_boundary_marker(golden, tmp_path):
             ref = subprocess.run(base, input=text, capture_output=True, timeout=120)
             assert ref.returncode == 0, ref.stderr.decode()
             assert ref.stdout == expect, (mode, where)
-            runs = [base + ["--batch-lines", "2"]] + ([base + ["--devices", "0,1"]] if n_gpus() >= 2 else [])
+            runs = [base + ["--batch-lines", "2"]] + [base + ["--devices", shard_devices_arg(2)]]
             for cmd in runs:
                 out = subprocess.run(cmd, input=text, capture_output=True, timeout=120)
                 assert out.returncode == 0, out.stderr.decode()

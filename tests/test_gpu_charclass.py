@@ -17,16 +17,12 @@ from bounded_oracle import BoundedOracle
 from oracle import vibrato_oracle as vo
 from span_oracle import Constraints, SpanOracle
 from test_gpu_bounded import d2h, lead_bytes
+from test_gpu_marginals import shard_devices
 
 pytestmark = pytest.mark.gpu
 ROUTES = ("whole", "chunked", "device", "compact", "small", "viterbi0", "unpruned", "multi", "multi_device")
 SETTINGS = [(isp, mgl) for isp in (False, True) for mgl in cf.MGLS]
 SMALL_BYTES = 16384  # host batches of at most this much text take k_small_batch
-
-
-def n_gpus():
-    import torch
-    return torch.cuda.device_count()
 
 
 @functools.lru_cache(maxsize=None)
@@ -62,7 +58,7 @@ def device_call(tok, sents):
 
 
 def tokenizer(d, route, isp=False, mgl=0):
-    tok = vb.Tokenizer.new(d, devices=[0, 1]) if route.startswith("multi") else vb.Tokenizer.new(d)
+    tok = vb.Tokenizer.new(d, devices=shard_devices(2)) if route.startswith("multi") else vb.Tokenizer.new(d)
     tok.ignore_space(isp).max_grouping_len(mgl)
     if route == "chunked":
         tok.set_option("chunk_sentences", 7)
@@ -114,8 +110,6 @@ def batches(route, sents):
 def test_tokens_match_oracle(name, route):
     """Every fixture sentence, with and without ignore_space, at every max_grouping_len, byte-identical to the
     oracle."""
-    if route.startswith("multi") and n_gpus() < 2:
-        pytest.skip("needs two GPUs")
     f, d, od = family(name)
     sents = sentences(f)
     for isp, mgl in SETTINGS:

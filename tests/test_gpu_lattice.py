@@ -10,7 +10,7 @@ import marginal_oracle as mo
 import vibrato_b200 as vb
 from bounded_oracle import BoundedOracle
 from oracle import vibrato_oracle as vo
-from test_gpu_marginals import adversarial_dicts, d2h, golden_dicts, golden_sents
+from test_gpu_marginals import adversarial_dicts, d2h, golden_dicts, golden_sents, shard_devices, shard_devices_arg
 
 pytestmark = pytest.mark.gpu
 ROUTES = ("whole", "chunked", "compact", "small", "device", "viterbi0", "unpruned")
@@ -240,25 +240,18 @@ def test_pb_format(golden):
         lat2.output_format("%m%pn\n")
 
 
-def n_gpus():
-    import torch
-    return torch.cuda.device_count()
-
-
 @pytest.mark.parametrize("route", ["multi", "multi_device"])
 def test_multi_device(golden, route):
-    if n_gpus() < 2:
-        pytest.skip("needs two GPUs")
     d, od, r = golden_dicts(golden, True)
     sents = golden_sents(golden) * 40 + [""] * 70 + golden_sents(golden) * 30
     ref = run(make(d, theta=THETA), "whole", sents)
-    tok = vb.Tokenizer.new(d, devices=[0, 1]).marginals(THETA).lattice(True)
+    tok = vb.Tokenizer.new(d, devices=shard_devices(2)).marginals(THETA).lattice(True)
     got = run(tok, "device" if route == "multi_device" else "whole", sents)
     for a, b in zip(ref, got):
         assert a.tobytes() == b.tobytes()
     if route == "multi":  # lattice text is merged like the tokens' text
         single = make(d, lattice=2).output_mode("mecab").tokenize_batch(sents).text()[1]
-        multi = vb.Tokenizer.new(d, devices=[0, 1]).lattice(True, text=True).output_mode("mecab").tokenize_batch(sents)
+        multi = vb.Tokenizer.new(d, devices=shard_devices(2)).lattice(True, text=True).output_mode("mecab").tokenize_batch(sents)
         assert multi.text()[1] == single
 
 
@@ -281,7 +274,7 @@ def test_cli_all_morphs(golden, tmp_path):
     want_mecab = make(d, lattice=2).output_mode("mecab").tokenize_batch(plain, boundaries=bnds).text()[1]
     fmt = "%pb%m\t%pP\n"
     want_fmt = make(d, theta=THETA, lattice=2).output_format(fmt).tokenize_batch(plain, boundaries=bnds).text()[1]
-    devs = [["--devices", "0,1"]] if n_gpus() >= 2 else []
+    devs = [["--devices", shard_devices_arg(2)]]
     for flags in [[], ["--batch-lines", "4"], ["--batch-lines", "1"]] + devs:
         p = subprocess.run(base + ["-a", "-O", "mecab", "--boundary-marker", "|"] + flags, input=data, capture_output=True,
                            timeout=120)

@@ -18,7 +18,7 @@ from bounded_oracle import BoundedOracle
 from oracle import vibrato_oracle as vo
 from span_oracle import Constraints, SpanOracle
 from test_gpu_lattice import ROUTES
-from test_gpu_marginals import adversarial_dicts, d2h, golden_dicts, golden_sents
+from test_gpu_marginals import adversarial_dicts, d2h, golden_dicts, golden_sents, shard_devices, shard_devices_arg
 
 pytestmark = pytest.mark.gpu
 THETA = 0.01
@@ -276,19 +276,12 @@ def test_python_views_and_errors(golden):
         plain.last_device_lattice_margins()
 
 
-def n_gpus():
-    import torch
-    return torch.cuda.device_count()
-
-
 @pytest.mark.parametrize("route", ["multi", "multi_device"])
 def test_multi_device(golden, route):
-    if n_gpus() < 2:
-        pytest.skip("needs two GPUs")
     d, od, r = golden_dicts(golden, True)
     sents = golden_sents(golden) * 40 + [""] * 70 + golden_sents(golden) * 30
     ref = run(make(d, 2000, theta=THETA), "whole", sents)
-    tok = vb.Tokenizer.new(d, devices=[0, 1]).marginals(THETA).lattice(True, margin=2000)
+    tok = vb.Tokenizer.new(d, devices=shard_devices(2)).marginals(THETA).lattice(True, margin=2000)
     got = run(tok, "device" if route == "multi_device" else "whole", sents)
     for a, b in zip(ref, got):
         assert (a is None and b is None) or a.tobytes() == b.tobytes()
@@ -307,7 +300,7 @@ def test_cli_cost_margin(golden, tmp_path):
     bnds = [[len(s[:s.index("|")].encode())] if "|" in s else [] for s in lines]
     d, _, _ = golden_dicts(golden, True)
     base = [exe, "-i", str(tmp_path), "-u", str(tmp_path / "user.csv")]
-    devs = [["--devices", "0,1"]] if n_gpus() >= 2 else []
+    devs = [["--devices", shard_devices_arg(2)]]
     for D in (0, 2000):
         want = make(d, D, text=True).output_mode("wakati").tokenize_batch(plain, boundaries=bnds).text()[1]
         fmt = "%pb%m\t%pP\n"

@@ -1,7 +1,7 @@
 """Marginal probabilities on the GPU (vbt_tokenizer_set_marginals): the tokens are unchanged, the probabilities match
 the forward-backward restatement (tests/marginal_oracle.py), and they are bit-identical on every route — whole
 batch, the chunked host pipeline, compact records, "small_batch" (which steps aside), device-resident input,
-bounded calls, every K3 variant and, with two GPUs, multi-device tokenizers."""
+bounded calls, every K3 variant and multi-device tokenizers."""
 import ctypes as C
 
 import numpy as np
@@ -24,6 +24,17 @@ def n_gpus():
     return torch.cuda.device_count()
 
 
+def shard_devices(n):
+    """The devices of an n-entry multi-device tokenizer: n distinct GPUs when the machine has them, else device 0 n
+    times (each entry is its own shard engine, so the sharded path runs on one GPU too)."""
+    return list(range(n)) if n_gpus() >= n else [0] * n
+
+
+def shard_devices_arg(n):
+    """shard_devices(n) as a `--devices` value."""
+    return ",".join(map(str, shard_devices(n)))
+
+
 def d2h(ptr, n, dtype):
     from cuda.bindings import runtime as cudart
     host = np.empty(n, dtype=dtype)
@@ -34,7 +45,7 @@ def d2h(ptr, n, dtype):
 
 
 def make_tokenizer(d, route, ignore_space=False, mgl=0, theta=THETA):
-    tok = vb.Tokenizer.new(d, devices=[0, 1]) if route.startswith("multi") else vb.Tokenizer.new(d)
+    tok = vb.Tokenizer.new(d, devices=shard_devices(2)) if route.startswith("multi") else vb.Tokenizer.new(d)
     tok.ignore_space(ignore_space).max_grouping_len(mgl)
     if route == "chunked":
         tok.set_option("chunk_sentences", 64)
@@ -85,11 +96,6 @@ def check_against(bo, sents, got, theta=THETA, bounds=None):
     mo.assert_f32_close(pp, e_pp, what="path_probs")
 
 
-def skip_multi(route):
-    if route.startswith("multi") and n_gpus() < 2:
-        pytest.skip("needs two GPUs")
-
-
 def golden_dicts(golden, user):
     r = golden["resources"]
     d = vb.SystemDictionaryBuilder.from_readers(r["lex.csv"], r["matrix.def"], r["char.def"], r["unk.def"])
@@ -138,7 +144,6 @@ def test_tokens_unchanged_and_probabilities_match(golden):
 
 @pytest.mark.parametrize("route", ROUTES)
 def test_routes_bit_identical(golden, route):
-    skip_multi(route)
     d, od, r = golden_dicts(golden, True)
     sents = golden_sents(golden) * 40 + [""] * 70 + golden_sents(golden) * 30  # empty runs across chunk edges
     ref = run(make_tokenizer(d, "whole", True), "whole", sents)
@@ -152,7 +157,6 @@ def test_routes_bit_identical(golden, route):
 
 @pytest.mark.parametrize("route", ("whole", "chunked", "device", "multi", "multi_device"))
 def test_bounded(golden, route):
-    skip_multi(route)
     d, od, r = golden_dicts(golden, False)
     sents = ["京都東京都京都", "アイアイウ", "東京   都", ""] * 30
     bounds = [[12], [6], [], []] * 30
@@ -296,7 +300,6 @@ def parse_pp(text, sents):
 @pytest.mark.parametrize("route", ("whole", "chunked", "multi"))
 def test_pP_format(golden, route):
     """%pP prints round(p * 1e6) as d.dddddd, on the host routes that format on the device."""
-    skip_multi(route)
     d, od, r = golden_dicts(golden, True)
     sents = golden_sents(golden) * (30 if route == "chunked" else 1)
     tok = make_tokenizer(d, route, True).output_format("%m\t%pP\n", eos="EOS\n")

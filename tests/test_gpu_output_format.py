@@ -14,6 +14,7 @@ import format_oracle as fo
 import vibrato_b200 as vb
 from vibrato_b200 import synth
 from oracle import vibrato_oracle as vo
+from test_gpu_marginals import shard_devices
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -251,16 +252,9 @@ def test_text_too_large_for_the_device_is_an_error():
     assert text == b"a,a,a,EOS\n"
 
 
-def _device_count():
-    import torch
-    return torch.cuda.device_count()
-
-
 def test_multi_device(syn):
-    if _device_count() < 2:
-        pytest.skip("needs 2 GPUs")
     utf8, off = syn.corpus(3000, seed=21)
-    multi = vb.Tokenizer.new(syn.d, devices=[0, 1]).ignore_space(True)
+    multi = vb.Tokenizer.new(syn.d, devices=shard_devices(2)).ignore_space(True)
     for fmt in FORMATS:
         eoff, etext = expected(syn.od, fmt, utf8, off, True)
         assert_text(multi.output_format(*fmt).tokenize_batch(utf8=utf8, byte_offsets=off), eoff, etext)

@@ -11,6 +11,7 @@ import pytest
 import vibrato_b200 as vb
 from vibrato_b200 import synth
 from oracle import vibrato_oracle as vo
+from test_gpu_marginals import shard_devices, shard_devices_arg
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -129,7 +130,7 @@ def _device_count():
 
 @pytest.mark.parametrize("n_dev", [1, 2, 4, 8])
 def test_multi_device_text_matches_single_device(n_dev):
-    if _device_count() < n_dev:
+    if n_dev > 2 and _device_count() < n_dev:
         pytest.skip(f"needs {n_dev} GPUs")
     sd, user, d, od = synth_user_dictionary()
     utf8, off = synth.make_corpus(sd, 5000, seed=78, log_uniform=(1, 200), unk_frac=0.1, space_frac=0.02, user_csv=user,
@@ -137,7 +138,7 @@ def test_multi_device_text_matches_single_device(n_dev):
     tok_off, toks = od.tokenize_batch(utf8, off, True, n_threads=8)[:2]
     single = vb.Tokenizer.new(d).ignore_space(True)
     single.set_option("chunk_sentences", 0)
-    multi = vb.Tokenizer.new(d, devices=list(range(n_dev))).ignore_space(True)
+    multi = vb.Tokenizer.new(d, devices=shard_devices(n_dev)).ignore_space(True)
     for mode in MODES + ("wakati",):  # modes switch between calls (and back)
         eoff, etext = vo.format_batch(od, utf8, off, tok_off, toks, mode)
         assert_text_equal(single.output_mode(mode).tokenize_batch(utf8=utf8, byte_offsets=off), eoff, etext)
@@ -160,9 +161,9 @@ def test_multi_device_text_matches_single_device(n_dev):
         res.text()
     # the output stage needs full token records, on every device
     with pytest.raises(vb.VibratoError):
-        vb.Tokenizer.new(d, devices=list(range(n_dev))).output_mode("mecab").compact_tokens(True)
+        vb.Tokenizer.new(d, devices=shard_devices(n_dev)).output_mode("mecab").compact_tokens(True)
     with pytest.raises(vb.VibratoError):
-        vb.Tokenizer.new(d, devices=list(range(n_dev))).compact_tokens(True).output_mode("mecab")
+        vb.Tokenizer.new(d, devices=shard_devices(n_dev)).compact_tokens(True).output_mode("mecab")
 
 
 def test_tokenize_cli_devices_and_batch_lines(golden, tmp_path):
@@ -174,8 +175,7 @@ def test_tokenize_cli_devices_and_batch_lines(golden, tmp_path):
     lines = ["京都東京都京都", "東京 都", "", "kampersanda", "東京県に行く", "", ""] * 3
     text = ("\n".join(lines) + "\n").encode()
     flag_sets = [["--devices", "0", "--batch-lines", "2"], ["--batch-lines", "1"], ["--batch-lines", "1000000"]]
-    if _device_count() >= 2:
-        flag_sets += [["--devices", "0,1"], ["--devices", "0,1", "--batch-lines", "3"]]
+    flag_sets += [["--devices", shard_devices_arg(2)], ["--devices", shard_devices_arg(2), "--batch-lines", "3"]]
     for mode in MODES:
         for where in ("device", "host"):
             base = [exe, "-i", str(tmp_path), "-u", str(tmp_path / "user.csv"), "-O", mode, "-S", "-M", "24", "--format-on", where]

@@ -9,7 +9,7 @@ import pytest
 
 import adversarial as adv
 import vibrato_b200 as vb
-from test_gpu_marginals import d2h, golden_dicts, golden_sents, skip_multi
+from test_gpu_marginals import d2h, golden_dicts, golden_sents, shard_devices
 
 pytestmark = pytest.mark.gpu
 THETA = 0.001
@@ -21,7 +21,7 @@ MARGIN = 2000  # the near-best lattice's cost margin when it is on
 
 
 def make(d, route, text=True, margin=None):
-    tok = vb.Tokenizer.new(d, devices=[0, 1]) if route.startswith("multi") else vb.Tokenizer.new(d)
+    tok = vb.Tokenizer.new(d, devices=shard_devices(2)) if route.startswith("multi") else vb.Tokenizer.new(d)
     if route == "chunked":
         tok.set_option("chunk_sentences", 64)
     tok.marginals(THETA).lattice(True, margin=margin).sampling(N_SAMP, THETA, 7)
@@ -72,7 +72,6 @@ def assert_same(got, ref):
 
 
 def check_all_outputs(golden, route, margin):
-    skip_multi(route)
     d, _, _ = golden_dicts(golden, True)
     sents = golden_sents(golden) * 40 + [""] * 70 + golden_sents(golden) * 30  # empty runs across chunk edges
     ref = run(make(d, "whole", margin=margin), "whole", sents, margin=margin)
@@ -129,7 +128,6 @@ REFUSALS = {"last_device_marginals": "marginals", "last_device_lattice": "the la
 def test_last_device_accessors_refuse(golden, route):
     """Each last_device_* accessor names what the last device-resident call ran without: after a call made with none
     of the features, and after a call with every feature on that failed (invalid UTF-8)."""
-    skip_multi(route)
     d, _, _ = golden_dicts(golden, True)
     utf8, off = adv.pack(["京都東京都京都", "abc"])
 
@@ -138,7 +136,7 @@ def test_last_device_accessors_refuse(golden, route):
             with pytest.raises(vb.VibratoError, match=re.escape(f"the last device-resident call ran without {what}") + "$"):
                 getattr(tok, name)()
 
-    plain = vb.Tokenizer.new(d, devices=[0, 1]) if route == "multi_device" else vb.Tokenizer.new(d)
+    plain = vb.Tokenizer.new(d, devices=shard_devices(2)) if route == "multi_device" else vb.Tokenizer.new(d)
     device_call(plain, utf8, off)
     assert_refused(plain)
     full = make(d, route, text=False, margin=MARGIN)

@@ -8,6 +8,7 @@ import pytest
 import vibrato_b200 as vb
 from vibrato_b200 import synth
 from oracle import vibrato_oracle as vo
+from test_gpu_marginals import shard_devices
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -689,18 +690,19 @@ def _device_count():
 def test_multi_device_tokenizer_matches_single_device(n_dev):
     """vbt_tokenizer_new_multi (SURVEY.md 8(e)): shards by bytes, one result in input order, byte-identical to the
     single-device tokenizer and to the oracle; the device-resident route gathers the same records on devices[0].
-    n_dev = 1 runs the multi-device code path on one GPU; larger counts need that many GPUs (gpurun --gpus N)."""
+    n_dev = 1 hands every call to its one engine; n_dev = 2 cuts the batch into shards, on device 0 twice when there
+    is one GPU (shard_devices); 4 and 8 need that many GPUs."""
     import torch
-    if _device_count() < n_dev:
+    if n_dev > 2 and _device_count() < n_dev:
         pytest.skip(f"needs {n_dev} GPUs")
     sd = synth.make_dictionary("synth-small")
     d = vb.SystemDictionaryBuilder.from_readers(sd.lex_csv, sd.matrix, sd.char_def, sd.unk_def)
     od = vo.OracleDictionary(sd.lex_csv, sd.matrix, sd.char_def, sd.unk_def)
     utf8, off = synth.make_corpus(sd, 5000, seed=77, log_uniform=(1, 200), unk_frac=0.1, space_frac=0.02)
     single = vb.Tokenizer.new(d).ignore_space(True)
-    multi = vb.Tokenizer.new(d, devices=list(range(n_dev))).ignore_space(True)
+    multi = vb.Tokenizer.new(d, devices=shard_devices(n_dev)).ignore_space(True)
     info = multi.describe()
-    assert info["devices"] == list(range(n_dev))
+    assert info["devices"] == shard_devices(n_dev)
     if n_dev > 1:
         assert info["dictionary_transport"].startswith("nccl") or info["dictionary_transport"] == "cudaMemcpyPeer"
     otok_off, otoks, _ = od.tokenize_batch(utf8, off, ignore_space=True, n_threads=8)
@@ -727,7 +729,7 @@ def test_multi_device_tokenizer_matches_single_device(n_dev):
     for name in vb.TOKEN_DTYPE.names:
         np.testing.assert_array_equal(got_tok[name], otoks[name], err_msg=name)
     # connection-id counters add up over the devices
-    multi2 = vb.Tokenizer.new(d, devices=list(range(n_dev)))
+    multi2 = vb.Tokenizer.new(d, devices=shard_devices(n_dev))
     multi2.init_connid_counter()
     multi2.tokenize_batch(utf8=utf8, byte_offsets=off)
     lid, rid = multi2.connid_counts()

@@ -16,7 +16,7 @@ import vibrato_b200 as vb
 from bounded_oracle import BoundedOracle
 from oracle import vibrato_oracle as vo
 from span_oracle import Constraints, SpanOracle
-from test_gpu_marginals import adversarial_dicts, d2h, golden_dicts, golden_sents
+from test_gpu_marginals import adversarial_dicts, d2h, golden_dicts, golden_sents, shard_devices, shard_devices_arg
 from vibrato_b200 import synth
 from vibrato_b200._native import check as vb_check, lib as vb_lib
 
@@ -24,14 +24,9 @@ pytestmark = pytest.mark.gpu
 THETA = 0.01
 
 
-def n_gpus():
-    import torch
-    return torch.cuda.device_count()
-
-
 def make(d, route="whole", gamma=1.0, isp=False, mgl=0, theta=THETA, chunk=64, lanes=None, sort=None, lattice=False,
          samples=0, unc=0, text=False):
-    tok = vb.Tokenizer.new(d, devices=[0, 1]) if route.startswith("multi") else vb.Tokenizer.new(d)
+    tok = vb.Tokenizer.new(d, devices=shard_devices(2)) if route.startswith("multi") else vb.Tokenizer.new(d)
     tok.ignore_space(isp).max_grouping_len(mgl)
     if route == "chunked":
         tok.set_option("chunk_sentences", chunk)
@@ -299,8 +294,6 @@ def test_routes_byte_for_byte(golden):
 
 @pytest.mark.parametrize("route", ["multi", "multi_device"])
 def test_multi_device(golden, route):
-    if n_gpus() < 2:
-        pytest.skip("needs two GPUs")
     d, od, r = golden_dicts(golden, True)
     sents = golden_sents(golden) * 40 + [""] * 70 + golden_sents(golden) * 30
     ref = run(make(d), "whole", sents)
@@ -478,8 +471,7 @@ def test_tokenize_cli_posterior(golden, tmp_path):
     text = ("\n".join(lines) + "\n").encode()
     base = [exe, "-i", str(tmp_path), "-u", str(tmp_path / "user.csv"), "-m", "-t", "0.001", "--posterior", "4"]
     flag_sets = [["--batch-lines", "1"], ["--batch-lines", "7"], ["--batch-lines", "65536"], ["--devices", "0"]]
-    if n_gpus() >= 2:
-        flag_sets.append(["--devices", "0,1"])
+    flag_sets.append(["--devices", shard_devices_arg(2)])
     for flags, style in ((["-O", "wakati"], "wakati"), (["-O", "detail"], "detail"), (["-F", "%m\t%pP\t%pc\n"], None)):
         tok = vb.Tokenizer.new(d).marginals(0.001).posterior(4.0, text=True)
         if style:

@@ -12,7 +12,7 @@ import pytest
 import adversarial as adv
 import format_oracle as fo
 import vibrato_b200 as vb
-from test_gpu_marginals import adversarial_dicts, golden_dicts, golden_sents, n_gpus, skip_multi
+from test_gpu_marginals import adversarial_dicts, golden_dicts, golden_sents, shard_devices, shard_devices_arg
 from vibrato_b200 import VibratoError
 from oracle import vibrato_oracle as vo
 
@@ -107,7 +107,6 @@ def long_feature_dict():
 
 @pytest.mark.parametrize("route", ["chunked", "retry", "multi"])
 def test_routes_are_byte_identical(golden, route):
-    skip_multi(route)
     if route == "retry":
         d, od, sents = long_feature_dict()
         styles = ("mecab", "detail")
@@ -117,7 +116,7 @@ def test_routes_are_byte_identical(golden, route):
         styles = MODES + (FORMATS[3], FORMATS[4])
     for style in styles:
         ref = call(style_of(vb.Tokenizer.new(d).sampling(3, THETA, 5, text=True), style), sents)
-        tok = vb.Tokenizer.new(d, devices=[0, 1]) if route == "multi" else vb.Tokenizer.new(d)
+        tok = vb.Tokenizer.new(d, devices=shard_devices(2)) if route == "multi" else vb.Tokenizer.new(d)
         if route != "multi":
             tok.set_option("chunk_sentences", 64 if route == "chunked" else 256)
         style_of(tok.sampling(3, THETA, 5, text=True), style)
@@ -249,8 +248,7 @@ def test_tokenize_cli_sample(golden, tmp_path):
     d, od, _ = golden_dicts(golden, True)
     base = [exe, "-i", str(tmp_path), "-u", str(tmp_path / "user.csv"), "--sample", "3", "-t", "0.01", "--seed", "5"]
     flag_sets = [["--batch-lines", "1"], ["--batch-lines", "7"], ["--batch-lines", "65536"], ["--devices", "0"]]
-    if n_gpus() >= 2:
-        flag_sets += [["--devices", "0,1"], ["--devices", "0,1", "--batch-lines", "7"]]
+    flag_sets += [["--devices", shard_devices_arg(2)], ["--devices", shard_devices_arg(2), "--batch-lines", "7"]]
     for style, flags in (("wakati", ["-O", "wakati"]), (FORMATS[3], ["-F", FORMATS[3][0], "--eos-format", "\n"])):
         tok = style_of(vb.Tokenizer.new(d).sampling(3, 0.01, 5, text=True), style)
         expected = call(tok, lines)[1]

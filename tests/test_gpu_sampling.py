@@ -14,7 +14,7 @@ import marginal_oracle as mo
 import sampling_oracle as so
 import vibrato_b200 as vb
 from bounded_oracle import BoundedOracle
-from test_gpu_marginals import adversarial_dicts, d2h, golden_dicts, golden_sents, skip_multi
+from test_gpu_marginals import adversarial_dicts, d2h, golden_dicts, golden_sents, shard_devices
 from vibrato_b200 import synth
 from vibrato_b200._native import lib
 from oracle import vibrato_oracle as vo
@@ -27,7 +27,7 @@ ambiguous = {"samples": 0}  # samples compared only up to an ambiguous draw, ove
 
 
 def make_tokenizer(d, route, n, theta=THETA, seed=0, ignore_space=False, mgl=0):
-    tok = vb.Tokenizer.new(d, devices=[0, 1]) if route.startswith("multi") else vb.Tokenizer.new(d)
+    tok = vb.Tokenizer.new(d, devices=shard_devices(2)) if route.startswith("multi") else vb.Tokenizer.new(d)
     tok.ignore_space(ignore_space).max_grouping_len(mgl)
     if route == "chunked":
         tok.set_option("chunk_sentences", 64)
@@ -146,7 +146,6 @@ def test_parity_synth():
 
 @pytest.mark.parametrize("route", ROUTES + ("retry",))
 def test_routes_bit_identical(golden, route):
-    skip_multi(route)
     d, od, r = golden_dicts(golden, True)
     sents = golden_sents(golden) * 40 + [""] * 70 + golden_sents(golden) * 30  # empty runs across chunk edges
     ref = run(make_tokenizer(d, "whole", 3, seed=2 ** 64 - 1, ignore_space=True), "whole", sents)
@@ -159,7 +158,6 @@ def test_routes_bit_identical(golden, route):
 def test_other_outputs_unchanged(golden, route):
     """Tokens, marginals, lattice and text are byte-identical with sampling on and off; the marginals' theta is
     shared."""
-    skip_multi(route)
     d, _, _ = golden_dicts(golden, True)
     sents = golden_sents(golden) * 20
     outs = []

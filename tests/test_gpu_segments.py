@@ -19,7 +19,7 @@ import segment_fixtures as sf
 import vibrato_b200 as vb
 from bounded_oracle import BoundedOracle
 from oracle import vibrato_oracle as vo
-from test_gpu_marginals import d2h
+from test_gpu_marginals import d2h, shard_devices
 from test_gpu_viterbi_routes import expected_route
 
 pytestmark = pytest.mark.gpu
@@ -61,7 +61,7 @@ def device_call(tok, sents, bounds=None):
 
 def every_route(dev, od, sents, long_sentence, isp=False, mgl=0):
     """viterbi_kernel 0 / 1 / 2 x lanes, counted, connid_counting, chunked (a sentence per chunk), compact records,
-    device-resident input and a multi-device tokenizer on device 0, all against the C oracle."""
+    device-resident input and a two-entry multi-device tokenizer (shard_devices), all against the C oracle."""
     utf8, off = adv.pack(sents)
     e_off, e_toks, e_cnt = od.tokenize_batch(utf8, off, isp, mgl, n_threads=8, want_counters=True)
     tok = vb.Tokenizer.new(dev).ignore_space(isp).max_grouping_len(mgl)
@@ -95,7 +95,7 @@ def every_route(dev, od, sents, long_sentence, isp=False, mgl=0):
     res = compact.tokenize_batch(utf8=utf8, byte_offsets=off)
     assert_tokens(res.tok_offsets, res.tokens, e_off, e_toks, "compact")
     assert_tokens(*device_call(vb.Tokenizer.new(dev).ignore_space(isp).max_grouping_len(mgl), sents), e_off, e_toks, "device")
-    multi = vb.Tokenizer.new(dev, devices=[0]).ignore_space(isp).max_grouping_len(mgl)
+    multi = vb.Tokenizer.new(dev, devices=shard_devices(2)).ignore_space(isp).max_grouping_len(mgl)
     res = multi.tokenize_batch(utf8=utf8, byte_offsets=off)
     assert_tokens(res.tok_offsets, res.tokens, e_off, e_toks, "multi")
 

@@ -15,6 +15,7 @@ import pytest
 import adversarial as adv
 import vibrato_b200 as vb
 from oracle import vibrato_oracle as vo
+from test_gpu_marginals import shard_devices
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -276,19 +277,12 @@ def test_worker_loop():
     assert p.small.describe()["last_viterbi"] == "k_small_batch" and p.small.last_launch_count() == 1
 
 
-def _device_count():
-    import torch
-    return torch.cuda.device_count()
-
-
 def test_multi_device_equals_single_device(golden):
-    if _device_count() < 2:
-        pytest.skip("needs 2 GPUs")
     d = adv.make_dictionary("ties", seed=6)
     p = adversarial_pair(d, ignore_space=True)
     dev = vb.SystemDictionaryBuilder.from_readers(d.lex_csv, d.matrix, d.char_def, d.unk_def)
     dev.reset_user_lexicon_from_reader(d.user_csv)
-    multi = vb.Tokenizer.new(dev, devices=[0, 1]).ignore_space(True).small_batch(64)
+    multi = vb.Tokenizer.new(dev, devices=shard_devices(2)).ignore_space(True).small_batch(64)
     sents = adv.make_sentences(d, 200, seed=2, max_len=60)
     for mode in (None,) + MODES:
         p.set(lambda t: t.output_mode(mode))

@@ -10,7 +10,7 @@ import marginal_oracle as mo
 import vibrato_b200 as vb
 from span_oracle import Constraints, SpanOracle, constraints, csv_fields
 from oracle import vibrato_oracle as vo
-from test_gpu_bounded import CHUNK_COPIES, d2h, golden_dicts, lead_bytes, make_tokenizer, skip_multi
+from test_gpu_bounded import CHUNK_COPIES, d2h, golden_dicts, lead_bytes, make_tokenizer
 from test_gpu_sampling import check_parity
 
 pytestmark = pytest.mark.gpu
@@ -133,7 +133,6 @@ GOLDEN_EXTRA = ["京都東京都京都", "abcdefgh", "東京   都", "東京都 
 
 @pytest.mark.parametrize("route", ROUTES)
 def test_golden_fixture(golden, route):
-    skip_multi(route)
     sents = [c["input"] for c in golden["tokenizer_cases"]] + GOLDEN_EXTRA
     for user in (False, True):
         d, od, r = golden_dicts(golden, user)
@@ -387,7 +386,7 @@ def test_tokenize_cli_partial(golden, tmp_path):
     and -F, across --batch-lines and --devices; the usage errors and the empty-token line error."""
     import os
     import subprocess
-    from test_gpu_bounded import ROOT, n_gpus
+    from test_gpu_bounded import ROOT, shard_devices_arg
     exe = os.path.join(ROOT, "vibrato_b200", "bin", "tokenize")
     if not os.path.exists(exe):
         pytest.skip("CLIs not built")
@@ -412,7 +411,7 @@ def test_tokenize_cli_partial(golden, tmp_path):
             t.output_format("%m[%ps]\n", eos="%S\n")
         expect = t.tokenize_batch(plain, boundaries=bnds, spans=spans).text()[1]
         base = [exe, "-i", str(tmp_path), "-p"] + opts
-        for extra in [[], ["--batch-lines", "2"], ["--batch-lines", "1"]] + ([["--devices", "0,1"]] if n_gpus() >= 2 else []):
+        for extra in [[], ["--batch-lines", "2"], ["--batch-lines", "1"]] + [["--devices", shard_devices_arg(2)]]:
             for inp in (text, text_last):
                 out = subprocess.run(base + extra, input=inp, capture_output=True, timeout=120)
                 assert out.returncode == 0, out.stderr.decode()

@@ -16,21 +16,16 @@ import vibrato_b200 as vb
 from bounded_oracle import BoundedOracle
 from oracle import vibrato_oracle as vo
 from span_oracle import Constraints, SpanOracle
-from test_gpu_marginals import adversarial_dicts, d2h, golden_dicts, golden_sents
+from test_gpu_marginals import adversarial_dicts, d2h, golden_dicts, golden_sents, shard_devices
 
 pytestmark = pytest.mark.gpu
 THETA = 0.01
 
 
-def n_gpus():
-    import torch
-    return torch.cuda.device_count()
-
-
 def make(d, route="whole", level=2, isp=False, mgl=0, theta=THETA, chunk=64, lanes=None, sort=None, lattice=False,
          margin=None, samples=0):
     if route.startswith("multi"):
-        tok = vb.Tokenizer.new(d, devices=[0, 1])
+        tok = vb.Tokenizer.new(d, devices=shard_devices(2))
     else:
         tok = vb.Tokenizer.new(d)
     tok.ignore_space(isp).max_grouping_len(mgl)
@@ -282,8 +277,6 @@ def test_routes_byte_for_byte(golden):
 
 @pytest.mark.parametrize("route", ["multi", "multi_device"])
 def test_multi_device(golden, route):
-    if n_gpus() < 2:
-        pytest.skip("needs two GPUs")
     d, od, r = golden_dicts(golden, True)
     sents = golden_sents(golden) * 40 + [""] * 70 + golden_sents(golden) * 30
     ref = run(make(d), "whole", sents)

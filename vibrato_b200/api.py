@@ -496,7 +496,8 @@ class Tokenizer:
     @staticmethod
     def new(dict_, device=0, devices=None):
         """`devices=[...]`: one tokenizer over several GPUs of this node (vbt_tokenizer_new_multi): the batch is split
-        by bytes, the dictionary image is uploaded once and broadcast, one result comes back in input order."""
+        by bytes, the dictionary image is uploaded once and broadcast, one result comes back in input order.  A device
+        listed more than once runs one shard per entry on it: this runs the sharded path on one GPU and is not faster."""
         return Tokenizer(dict_, device, devices)
 
     def __del__(self):

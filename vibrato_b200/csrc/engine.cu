@@ -820,11 +820,11 @@ class EngineImpl final : public Engine {
             CK(cudaStreamSynchronize(stream_));
             if (bad_offsets) {
                 release(r);
-                throw Error(kInvalidArgument, "byte_offsets must be non-decreasing and end within the input buffer");
+                throw Error(kInvalidArgument, kBadOffsetsMsg);
             }
             if (bad_utf8) {
                 release(r);
-                throw Error(kUtf8, "stream did not contain valid UTF-8");
+                throw Error(kUtf8, kBadUtf8Msg);
             }
             if (bad_bounds) {
                 release(r);
@@ -973,16 +973,6 @@ class EngineImpl final : public Engine {
         if (sample_base_ + n_sent > kMaxSampleBase)
             throw Error(kInvalidArgument, "sampling: sample_base + n_sent exceeds 2^32, the range of the draws' sentence index");
     }
-
-    static constexpr const char* kBadBoundsMsg =
-        "required boundaries must be non-decreasing, at most the sentence's byte length and on a UTF-8 lead byte, "
-        "and their offsets non-decreasing and within the boundary array";
-
-    static constexpr const char* kBadSpansMsg =
-        "required tokens (spans) must have start < end <= the sentence's byte length, both on a UTF-8 lead byte or at the "
-        "end, be sorted and non-overlapping, name VBT_SPAN_ANY or a pattern of the call, hold no explicit boundary "
-        "inside, not start at a space when ignore_space is on, and their offsets must be non-decreasing and within the "
-        "span array";
 
     void check_bounded(const Bounds* bnd) const {
         if (bnd && counting_)
@@ -1382,8 +1372,8 @@ class EngineImpl final : public Engine {
         SmallBatchOut h;
         std::memcpy(&h, small_out_h_, sizeof h);
         if (h.flags & kFlagBadOffsets)
-            throw Error(kInvalidArgument, "byte_offsets must be non-decreasing and end within the input buffer");
-        if (h.flags & kFlagUtf8Error) throw Error(kUtf8, "stream did not contain valid UTF-8");
+            throw Error(kInvalidArgument, kBadOffsetsMsg);
+        if (h.flags & kFlagUtf8Error) throw Error(kUtf8, kBadUtf8Msg);
         if (h.flags & kFlagBadBoundary) throw Error(kInvalidArgument, kBadBoundsMsg);
         if (h.flags & (kFlagPoolOverflow | kFlagTextOverflow)) return nullptr;
         if (fmt && h.text_bytes > text_guess) {
@@ -1614,9 +1604,9 @@ class EngineImpl final : public Engine {
             CK(cudaEventSynchronize(o.done));
             CK(cudaGetLastError());
             if (o.h_ctrl->flags & kFlagBadOffsets)
-                throw Error(kInvalidArgument, "byte_offsets must be non-decreasing and end within the input buffer");
+                throw Error(kInvalidArgument, kBadOffsetsMsg);
             if (o.h_ctrl->flags & kFlagUtf8Error)
-                throw Error(kUtf8, "stream did not contain valid UTF-8");  // what `stdin.lines()` reports
+                throw Error(kUtf8, kBadUtf8Msg);
             if (o.h_ctrl->flags & kFlagBadBoundary) throw Error(kInvalidArgument, kBadBoundsMsg);
             if (o.h_ctrl->flags & kFlagBadSpan) throw Error(kInvalidArgument, kBadSpansMsg);
             if (o.h_ctrl->flags & kFlagSlotsOverflow) {  // more characters per byte than any batch before: hard bound

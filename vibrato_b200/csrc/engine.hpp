@@ -177,6 +177,19 @@ struct Bounds {
     Spans spans;
 };
 
+// The input errors a batch can hold, in the order it reports them: a batch with several reports the first of these,
+// whichever sentences hold them (the multi-device engine keeps that order across its shards).
+constexpr const char* kBadOffsetsMsg = "byte_offsets must be non-decreasing and end within the input buffer";
+constexpr const char* kBadUtf8Msg = "stream did not contain valid UTF-8";  // what `stdin.lines()` reports
+constexpr const char* kBadBoundsMsg =
+    "required boundaries must be non-decreasing, at most the sentence's byte length and on a UTF-8 lead byte, "
+    "and their offsets non-decreasing and within the boundary array";
+constexpr const char* kBadSpansMsg =
+    "required tokens (spans) must have start < end <= the sentence's byte length, both on a UTF-8 lead byte or at the "
+    "end, be sorted and non-overlapping, name VBT_SPAN_ANY or a pattern of the call, hold no explicit boundary "
+    "inside, not start at a space when ignore_space is on, and their offsets must be non-decreasing and within the "
+    "span array";
+
 constexpr int kNumStages = 9;
 extern const char* const kStageNames;  // comma-separated, kNumStages entries
 // A call on the k_small_batch route ("small_batch" option) runs every stage in one kernel: its whole time is booked

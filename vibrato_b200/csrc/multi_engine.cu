@@ -147,12 +147,14 @@ class MultiEngine final : public Engine {
         int count = 0;
         if (cudaGetDeviceCount(&count) != cudaSuccess || count == 0)
             throw Error(kNoDevice, "no CUDA device available: the tokenizer has no CPU fallback");
+        // A device listed more than once runs one shard per entry (an engine with its own streams and image copy):
+        // the sharded path on one GPU, not a faster one.  NCCL refuses a repeated device, so peer copies serve then.
+        bool distinct = true;
         for (int i = 0; i < n; ++i) {
             if (dev_[i] < 0 || dev_[i] >= count) throw Error(kInvalidArgument, "device ordinal out of range");
-            for (int j = 0; j < i; ++j)
-                if (dev_[j] == dev_[i]) throw Error(kInvalidArgument, "the same device is listed twice");
+            for (int j = 0; j < i; ++j) distinct = distinct && dev_[j] != dev_[i];
         }
-        nccl_ = Nccl::get();
+        nccl_ = distinct ? Nccl::get() : nullptr;
         stream_.resize(n);
         image_.resize(n, nullptr);
         cpus_.resize(n);
@@ -162,7 +164,7 @@ class MultiEngine final : public Engine {
             CK(cudaMalloc(&image_[i], n_bytes));
             cpus_[i] = numa_cpus_of_device(dev_[i]);
             for (int j = 0; j < n; ++j) {  // peer access for the device-resident route (NVLink / NVSwitch)
-                if (i == j) continue;
+                if (dev_[i] == dev_[j]) continue;
                 int can = 0;
                 cudaDeviceCanAccessPeer(&can, dev_[i], dev_[j]);
                 if (can) {
@@ -233,6 +235,9 @@ class MultiEngine final : public Engine {
             return r;
         }
         check_samples(n_sent);
+        // offsets whose last lies below their first are a batch too large on one device (check_size), and so in the
+        // shard whose window then wraps; the others are checked here, before the split
+        if (n_sent && byte_off[n_sent] >= byte_off[0]) check_offsets(byte_off, n_sent, ~0ull);
         const std::vector<uint64_t> cut = split_by_bytes(byte_off, n_sent, n);
         const Outputs out = outputs();
         std::vector<Totals> count(n);
@@ -267,8 +272,8 @@ class MultiEngine final : public Engine {
         last_ = DeviceOutputs{};
         check_samples(n_sent);
         CK(cudaSetDevice(dev_[0]));
-        // the split needs the offsets on the host (pinned staging buffer, one copy); their validity is checked on
-        // the devices like for any device-resident batch (k_count_chars)
+        // the split needs the offsets on the host (pinned staging buffer, one copy); they are checked there, before
+        // the shards size their copies of the input from them
         if ((n_sent + 1) * 8 > h_off_cap_) {
             pinned_free(h_off_);
             h_off_cap_ = size_t(double((n_sent + 1) * 8) * 1.25) + 64;
@@ -276,6 +281,7 @@ class MultiEngine final : public Engine {
         }
         CK(cudaMemcpyAsync(h_off_, reinterpret_cast<const void*>(d_byte_off), (n_sent + 1) * 8, cudaMemcpyDeviceToHost, stream_[0]));
         CK(cudaStreamSynchronize(stream_[0]));
+        check_offsets(h_off_, n_sent, n_bytes);
         // boundary lists: to the host as well, and from there to every shard like those of a host batch (they are
         // validated on the devices)
         Bounds hb;
@@ -441,6 +447,13 @@ class MultiEngine final : public Engine {
         return cut;
     }
 
+    // What k_count_chars refuses on one device: a sentence that ends before it starts or beyond `end` bytes.  A shard
+    // cut from such offsets would copy a wrapped window or bytes past the caller's buffer.
+    static void check_offsets(const uint64_t* off, uint64_t n_sent, uint64_t end) {
+        for (uint64_t i = 0; i < n_sent; ++i)
+            if (off[i + 1] < off[i] || off[i + 1] > end) throw Error(kInvalidArgument, kBadOffsetsMsg);
+    }
+
     // The sample offsets of a whole batch are indexed in 32 bits (every shard checks its own part too).
     void check_samples(uint64_t n_sent) const {
         if (n_sent * sampling() >= 0xFFFFFFFFull)
@@ -465,7 +478,9 @@ class MultiEngine final : public Engine {
         return sb;
     }
 
-    // One host thread per device (the calling thread takes the first): each call blocks on its own device.
+    // One host thread per device (the calling thread takes the first): each call blocks on its own device.  Of the
+    // shards that failed, the error one device would report for the whole batch wins: any other error before the
+    // input errors, those in their order (kBadOffsetsMsg ..), then the first shard.
     template <typename F>
     void run_on_all(F&& f) {
         const int n = int(dev_.size());
@@ -490,8 +505,16 @@ class MultiEngine final : public Engine {
             });
         body(0);
         for (auto& t : th) t.join();
+        auto rank = [&](int i) {
+            const char* const order[] = {kBadOffsetsMsg, kBadUtf8Msg, kBadBoundsMsg, kBadSpansMsg};
+            for (int k = 0; k < 4; ++k)
+                if (err[i] == order[k]) return k + 1;
+            return 0;
+        };
+        int worst = -1;
         for (int i = 0; i < n; ++i)
-            if (st[i] != kOk) throw Error(st[i], err[i]);
+            if (st[i] != kOk && (worst < 0 || rank(i) < rank(worst))) worst = i;
+        if (worst >= 0) throw Error(st[worst], err[worst]);
     }
 
     void collect_stats() {
