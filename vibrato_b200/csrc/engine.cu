@@ -85,6 +85,7 @@ static std::string num(double v) {
 struct CastU64 {
     __host__ __device__ unsigned long long operator()(uint32_t v) const { return v; }
 };
+using CountsU64 = cub::TransformInputIterator<unsigned long long, CastU64, const uint32_t*>;  // u32 counts read as u64
 
 __global__ void k_iota(uint32_t* v, uint32_t n) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -178,6 +179,38 @@ struct DevBounds {
     const uint3* pf = nullptr;
     const uint8_t* pat_bytes = nullptr;
     uint32_t n_pat = 0;
+};
+
+// What the output text renders in place of the tokens (options "lattice" = 2, "sample_text", "posterior_text"): at most
+// one source replaces the best path.  Per source its name and option in the refusals, its offsets, records and their
+// marginals (%pP), and the row of learned text ratios it sizes its text from.
+enum TextSrc { kTextBest, kTextNodes, kTextPosterior, kTextSamples, kNumTextSrcs };
+struct TextSrcInfo {
+    const char *name, *off, *on;  // "<name> text", and how its option switches it off and on
+    Array tok_off, tokens, prob;  // prob: kNumArrays = none (sample text refuses %pP)
+    int ratio;                    // posterior text renders a path like the best one: it shares that ratio
+};
+constexpr TextSrcInfo kTextSrcs[kNumTextSrcs] = {
+    {nullptr, nullptr, nullptr, kTokOff, kTokens, kTokenProb, 0},
+    {"lattice", "\"lattice\" below 2", "lattice = 2", kNodeOff, kNodes, kNodeProb, 1},
+    {"posterior", "\"posterior_text\" to 0", "posterior_text = 1", kPostOff, kPostTokens, kPostProb, 0},
+    {"sample", "\"sample_text\" to 0", "sample_text = 1", kSampleOff, kSamples, kNumArrays, 2},
+};
+// Output text bytes expected per input byte (beyond text_per_sent_ per sentence) by [TextSrcInfo::ratio][output mode],
+// before any is learned: the best path, lattice text (~17 nodes per token) and sample text (per rendering of a sentence).
+constexpr int kTextRatios = 3;
+using TextRatios = std::array<std::array<double, 5>, kTextRatios>;
+constexpr TextRatios kTextPerByte = {{{0.0, 8.0, 2.0, 16.0, 8.0},
+                                      {0.0, 8.0 * 17, 2.0 * 17, 16.0 * 17, 8.0 * 17},
+                                      {0.0, 8.0, 2.0, 16.0, 8.0}}};
+
+// The passes a batch runs between K3 and K4 and the host routes it may take, derived from the options (plan()).
+struct PassPlan {
+    FwdKind fwd;
+    BwdKind bwd;                    // kBwdNone <=> marginals off
+    bool bprob, margin, lat, post;  // k_boundary_probs (uncertainty 2), k_margin_backward, the lattice, posterior kernels
+    uint32_t samp;                  // sampled paths per sentence, 0 = no sampling kernels
+    bool small, eager;              // a small host batch may take k_small_batch / queue its copies behind the kernels
 };
 
 struct OutSlot {  // where one (chunk of a) batch leaves its results; two of them alternate in chunked runs
@@ -422,18 +455,8 @@ class EngineImpl final : public Engine {
         } else if (name == "lattice") {
             // every lattice node next to the tokens (1), and in place of them in the output text (2)
             if (value < 0 || value > 2) throw Error(kInvalidArgument, "lattice must be 0 (off), 1 (nodes) or 2 (nodes, and the text renders them)");
-            if (value == 2 && output_mode_ == kOutFormat && (fmt_uses_ & kUsesPrev))
-                throw Error(kInvalidArgument,
-                            "the output format prints a \"prev\" directive (%M %pS %pn %pC %pL), which lattice text has no value for: "
-                            "change the format before setting lattice = 2");
-            if (value != 2 && output_mode_ == kOutFormat && (fmt_uses_ & kUsesBest))
-                throw Error(kInvalidArgument, "the output format prints %pb, which only lattice text has: change the format before setting lattice below 2");
-            if (value == 2 && sample_text_)
-                throw Error(kInvalidArgument, "lattice text and sample text both replace the output text: set \"sample_text\" to 0 before setting lattice = 2");
-            if (value == 2 && post_text_)
-                throw Error(kInvalidArgument, "lattice text and posterior text both replace the output text: set \"posterior_text\" to 0 before setting lattice = 2");
-            cudaStreamSynchronize(stream_);
-            lattice_ = int(value);
+            set_text(kTextNodes, value == 2);
+            lattice_ = value != 0;
         } else if (name == "lattice_margin") {
             // the lattice keeps the nodes of the paths within cost D of the best one (-1: every node)
             if (value < -1 || value > kMaxLatticeMargin)
@@ -451,25 +474,11 @@ class EngineImpl final : public Engine {
         } else if (name == "sample_text") {
             // the output text renders each sentence's samples in place of its best path
             if (value < 0 || value > 1) throw Error(kInvalidArgument, "sample_text must be 0 (off) or 1 (the text renders the samples)");
-            if (value && !samp_n_) throw Error(kInvalidArgument, "sample_text needs sampling: switch it on with set_sampling first");
-            if (value && lattice_ == 2)
-                throw Error(kInvalidArgument, "lattice text and sample text both replace the output text: set \"lattice\" below 2 before setting sample_text = 1");
-            if (value && post_text_)
-                throw Error(kInvalidArgument, "posterior text and sample text both replace the output text: set \"posterior_text\" to 0 before setting sample_text = 1");
-            if (value && output_mode_ == kOutFormat && (fmt_uses_ & (kUsesProb | kUsesBest)))  // capi names the directive
-                throw Error(kInvalidArgument, "the output format prints %pP or %pb, which sample text has no value for: change the format before setting sample_text = 1");
-            cudaStreamSynchronize(stream_);
-            sample_text_ = value != 0;
+            set_text(kTextSamples, value != 0);
         } else if (name == "posterior_text") {
             // the output text renders each sentence's posterior path in place of its best path
             if (value < 0 || value > 1) throw Error(kInvalidArgument, "posterior_text must be 0 (off) or 1 (the text renders the posterior path)");
-            if (value && !post_) throw Error(kInvalidArgument, "posterior_text needs posterior decoding: switch it on with set_posterior first");
-            if (value && lattice_ == 2)
-                throw Error(kInvalidArgument, "lattice text and posterior text both replace the output text: set \"lattice\" below 2 before setting posterior_text = 1");
-            if (value && sample_text_)
-                throw Error(kInvalidArgument, "posterior text and sample text both replace the output text: set \"sample_text\" to 0 before setting posterior_text = 1");
-            cudaStreamSynchronize(stream_);
-            post_text_ = value != 0;
+            set_text(kTextPosterior, value != 0);
         } else if (name == "sample_base") {
             // the sentence index of the draws starts here: a caller that splits a corpus over calls keeps its draws
             if (value < 0 || value > kMaxSampleBase) throw Error(kInvalidArgument, "sample_base must be between 0 and 2^32");
@@ -489,11 +498,11 @@ class EngineImpl final : public Engine {
         if (tok_bytes_ != 24) throw Error(kInvalidArgument, "compact_tokens and output formats exclude each other");
         if ((p->uses & kUsesProb) && theta_ == 0)
             throw Error(kInvalidArgument, "%pP needs marginals: switch them on before setting the format");
-        if ((p->uses & kUsesBest) && lattice_ != 2)
+        if ((p->uses & kUsesBest) && text_src_ != kTextNodes)
             throw Error(kInvalidArgument, "%pb needs lattice text: set the option \"lattice\" to 2 before setting the format");
-        if ((p->uses & kUsesPrev) && lattice_ == 2)  // compile_format names the directive; this guards other callers
+        if ((p->uses & kUsesPrev) && text_src_ == kTextNodes)  // compile_format names the directive; this guards other callers
             throw Error(kInvalidArgument, "lattice text has no previous token: the format may not print %M %pS %pn %pC %pL");
-        if ((p->uses & (kUsesProb | kUsesBest)) && sample_text_)  // the same
+        if ((p->uses & (kUsesProb | kUsesBest)) && text_src_ == kTextSamples)  // the same
             throw Error(kInvalidArgument, "sample text has no marginals or best-path flags: the format may not print %pP or %pb");
         try {
             fmt_prog_.ensure(sizeof(FormatProgram));
@@ -506,9 +515,7 @@ class EngineImpl final : public Engine {
         output_mode_ = kOutFormat;
         fmt_uses_ = p->uses;
         text_per_sent_ = p->per_sentence;
-        text_per_byte_[kOutFormat] = kFormatTextPerByte;  // learned anew for every format
-        text_per_byte_lat_[kOutFormat] = kFormatTextPerByte * kLatticeTextFactor;
-        text_per_byte_samp_[kOutFormat] = kFormatTextPerByte;
+        for (int s = 0; s < kTextRatios; ++s) text_per_byte_[s][kOutFormat] = kTextPerByte[s][kOutFormat];  // learned anew
     }
     void set_marginals(double theta) override {
         if (!(theta >= 0) || !std::isfinite(theta))
@@ -532,7 +539,7 @@ class EngineImpl final : public Engine {
         if (n && theta_ > 0 && theta != theta_)
             throw Error(kInvalidArgument, "marginals and sampling share one forward pass: the sampling theta " + num(theta) +
                                               " differs from the marginals' theta " + num(theta_));
-        if (!n && sample_text_)
+        if (!n && text_src_ == kTextSamples)
             throw Error(kInvalidArgument, "the output text renders the samples: set \"sample_text\" to 0 before switching sampling off");
         cudaStreamSynchronize(stream_);
         samp_n_ = n;
@@ -545,7 +552,7 @@ class EngineImpl final : public Engine {
             throw Error(kInvalidArgument, "posterior decoding: gamma must be a finite number >= 0");
         if (on && theta_ == 0)
             throw Error(kInvalidArgument, "posterior decoding needs marginals: switch them on with set_marginals first");
-        if (!on && post_text_)
+        if (!on && text_src_ == kTextPosterior)
             throw Error(kInvalidArgument, "the output text renders the posterior path: set \"posterior_text\" to 0 before switching posterior decoding off");
         cudaStreamSynchronize(stream_);
         post_ = on;
@@ -553,7 +560,7 @@ class EngineImpl final : public Engine {
     }
     bool posterior() const override { return post_; }
     double marginals() const override { return theta_; }
-    int lattice() const override { return lattice_; }
+    int lattice() const override { return text_src_ == kTextNodes ? 2 : lattice_; }
     Outputs outputs() const override {
         return Outputs{tok_bytes_, samp_n_, theta_ > 0, output_mode_ != kOutNone, lattice_ != 0, lat_margin_ >= 0, unc_, post_};
     }
@@ -635,9 +642,8 @@ class EngineImpl final : public Engine {
         const uint32_t chunk = chunk_sentences_;
         const bool chunked = chunk > 0 && n_sent > chunk + chunk / 2;
         const bool fmt = output_mode_ != kOutNone;
-        // k_small_batch computes no marginals, no lattice and no samples: with any on, small batches take the usual route
-        if (small_batch_ && n_sent <= small_batch_ && !chunked && n_bytes <= kEagerBytes && !counting_ && !connid_on_ && theta_ == 0 && !lattice_ &&
-            !samp_n_ &&
+        const PassPlan p = plan();
+        if (p.small && n_sent <= small_batch_ && !chunked && n_bytes <= kEagerBytes &&
             (!bnd || (!bnd->spans.off && small_bounds_fit(*bnd, n_sent)))) {  // k_small_batch has no span rules
             if (HostResult* r = run_small(utf8 + first, off, n_sent, n_bytes, bnd)) return r;
             // the batch outgrew the scratch of k_small_batch: it runs again on the route below
@@ -647,7 +653,7 @@ class EngineImpl final : public Engine {
             if (!chunked) {
                 h2d(in_off_.p, off, (size_t(n_sent) + 1) * 8, stream_, off_pinned && off == byte_off);
                 h2d(in_utf8_.p, utf8 + first, n_bytes, stream_, utf8_pinned);
-                if (n_bytes <= kEagerBytes && output_mode_ == kOutNone && !lattice_ && !samp_n_ && !unc_ && !post_) {
+                if (p.eager && n_bytes <= kEagerBytes) {
                     // Small batches (a per-sentence Worker loop ends up here) are all latency: the result copies are
                     // queued behind the kernels with an upper bound for the token count (a token spans >= 1 byte), so
                     // that the call makes ONE host synchronisation instead of two.
@@ -708,7 +714,7 @@ class EngineImpl final : public Engine {
             // sentence plus the learned ratio per input byte); a chunk with more text flags itself and the batch is
             // re-run with the ratio it measured
             // (sample text: n renderings per sentence, the ratio learned per rendering)
-            const uint32_t renders = sample_text_ ? samp_n_ : 1;
+            const uint32_t renders = text_view(out_[0]).units;
             const double text_ratio = text_ratio_ref() * renders;
             const uint64_t per_sent = uint64_t(text_per_sent_) * renders;
             if (fmt)
@@ -1078,7 +1084,53 @@ class EngineImpl final : public Engine {
         last_.total = totals(*o.h_ctrl);
         for (int a = 0; a < kNumArrays; ++a) last_.addr[a] = o.made.has(a) ? reinterpret_cast<uint64_t>(o.buf[a].p) : 0;
     }
-    bool margin_on() const { return lattice_ && lat_margin_ >= 0; }  // the near-best lattice's kernels run
+
+    // Switches text source src on (it replaces the best path in the output text) or off (back to the best path when
+    // it was the source): the rules of every source, in the order they are reported.
+    void set_text(TextSrc src, bool on) {
+        const uint32_t uses = output_mode_ == kOutFormat ? fmt_uses_ : 0;
+        if (on) {
+            if (src == kTextSamples && !samp_n_)
+                throw Error(kInvalidArgument, "sample_text needs sampling: switch it on with set_sampling first");
+            if (src == kTextPosterior && !post_)
+                throw Error(kInvalidArgument, "posterior_text needs posterior decoding: switch it on with set_posterior first");
+            if (src == kTextNodes && (uses & kUsesPrev))
+                throw Error(kInvalidArgument,
+                            "the output format prints a \"prev\" directive (%M %pS %pn %pC %pL), which lattice text has no value for: "
+                            "change the format before setting lattice = 2");
+            if (text_src_ != kTextBest && text_src_ != src)
+                throw Error(kInvalidArgument, std::string(kTextSrcs[std::min(text_src_, src)].name) + " text and " +
+                                                  kTextSrcs[std::max(text_src_, src)].name + " text both replace the output text: set " +
+                                                  kTextSrcs[text_src_].off + " before setting " + kTextSrcs[src].on);
+            if (src == kTextSamples && (uses & (kUsesProb | kUsesBest)))  // capi names the directive
+                throw Error(kInvalidArgument, "the output format prints %pP or %pb, which sample text has no value for: change the format before setting sample_text = 1");
+        } else if (src == kTextNodes && (uses & kUsesBest)) {
+            throw Error(kInvalidArgument, "the output format prints %pb, which only lattice text has: change the format before setting lattice below 2");
+        }
+        cudaStreamSynchronize(stream_);
+        if (on || text_src_ == src) text_src_ = on ? src : kTextBest;
+    }
+
+    PassPlan plan() const {
+        const bool marg = theta_ > 0, margin = lattice_ && lat_margin_ >= 0;
+        const FwdKind fwd = (samp_n_ || post_) ? kFwdLseLw : marg ? kFwdLse : margin ? kFwdR : kFwdNone;
+        return PassPlan{fwd, !marg ? kBwdNone : unc_ ? kBwdUnc : kBwdPlain, marg && unc_ >= 2, margin, lattice_, post_, samp_n_,
+                        // k_small_batch runs none of the passes and counts nothing
+                        small_batch_ && fwd == kFwdNone && !lattice_ && !counting_ && !connid_on_,
+                        // the eager copies are sized by the token bound alone
+                        output_mode_ == kOutNone && !lattice_ && !samp_n_ && !unc_ && !post_};
+    }
+
+    // What the output stage renders from slot o (text_src_): offsets, records and the marginals %pP prints, the
+    // renderings per sentence (each of its samples in sample text), and the nodes' links when lattice text prints %pb.
+    struct TextView { const DevBuf *tok_off, *tokens; const float* prob; uint32_t units; const int2* links; };
+    TextView text_view(const OutSlot& o) const {
+        const TextSrcInfo& t = kTextSrcs[text_src_];
+        const bool prob = o.made.marg && output_mode_ == kOutFormat && (fmt_uses_ & kUsesProb) && t.prob != kNumArrays;
+        const bool links = text_src_ == kTextNodes && output_mode_ == kOutFormat && (fmt_uses_ & kUsesBest);
+        return TextView{&o.buf[t.tok_off], &o.buf[t.tokens], prob ? o.buf[t.prob].as<float>() : nullptr,
+                        text_src_ == kTextSamples ? samp_n_ : 1, links ? o.buf[kLinks].as<int2>() : nullptr};
+    }
 
     // D2H on `st` of every array r carries, from slot `o` holding n sentences and `count` records per group: to
     // sentence s0 of r and after `base` records per group; `last` brings the closing offsets too.
@@ -1108,44 +1160,28 @@ class EngineImpl final : public Engine {
     // the output stage), the sample records (sized by enqueue from the scanned total) and the lattice records (one
     // per lattice entry: ensure_entries).
     void ensure_out(OutSlot& o, uint32_t n_sent, uint64_t n_bytes) {
-        o.buf[kTokOff].ensure((size_t(n_sent) + 1) * 8, 1.25);
-        o.buf[kTokens].ensure(size_t(n_bytes) * 24 + 24, 1.25);  // a token spans >= 1 character >= 1 byte
-        if (theta_ > 0) o.buf[kTokenProb].ensure(size_t(n_bytes) * 4 + 4, 1.25);
-        if (theta_ > 0 || samp_n_) o.buf[kPathProb].ensure((size_t(n_sent) + 1) * 4, 1.25);  // the forward pass writes it
-        if (unc_) {
-            o.buf[kEntropy].ensure((size_t(n_sent) + 1) * 8, 1.25);
-            o.buf[kLogPathProb].ensure((size_t(n_sent) + 1) * 8, 1.25);
-        }
-        if (unc_ >= 2) {  // a record per slot: characters <= bytes, one sentinel slot per sentence
-            o.buf[kPosOff].ensure((size_t(n_sent) + 1) * 8, 1.25);
-            o.buf[kBoundaryProb].ensure((size_t(n_bytes) + n_sent + 1) * 4, 1.25);
-        }
-        if (lattice_) o.buf[kNodeOff].ensure((size_t(n_sent) + 1) * 8, 1.25);
-        if (samp_n_) o.buf[kSampleOff].ensure((size_t(n_sent) * samp_n_ + 1) * 8, 1.25);
-        if (post_) {  // a path has at most one token per character
-            o.buf[kPostOff].ensure((size_t(n_sent) + 1) * 8, 1.25);
-            o.buf[kPostTokens].ensure(size_t(n_bytes) * 24 + 24, 1.25);
-            o.buf[kPostProb].ensure(size_t(n_bytes) * 4 + 4, 1.25);
-            o.buf[kPostGain].ensure((size_t(n_sent) + 1) * 8, 1.25);
+        const Outputs out = outputs();
+        const PassPlan p = plan();
+        Totals most{};  // records per group: a token spans >= 1 character >= 1 byte, and a slot is a character or a sentinel
+        most[kGroupTokens] = most[kGroupPosterior] = n_bytes + 1;
+        most[kGroupPositions] = n_bytes + n_sent + 1;
+        for (int a = 0; a < kNumArrays; ++a) {
+            const ArrayInfo& k = kArrays[a];
+            // sampling without marginals: the forward pass still writes path_prob
+            const bool need = out.has(a) || (a == kPathProb && p.fwd >= kFwdLse);
+            if (!need || k.group == kGroupText || (k.kind == kRecords && !most[k.group])) continue;
+            const uint64_t rows = k.kind == kRecords ? most[k.group] : uint64_t(n_sent) * out.stride(a) + 1;
+            o.buf[a].ensure(rows * out.elem_bytes(a), 1.25);
         }
     }
 
-    // The nodes' links when lattice text prints %pb (the %pb instantiation of the format kernels), else nullptr.
-    const int2* fmt_links(const OutSlot& o) const {
-        return (lattice_ == 2 && output_mode_ == kOutFormat && (fmt_uses_ & kUsesBest)) ? o.buf[kLinks].as<int2>() : nullptr;
-    }
-
-    // Text bytes per input byte expected for the output mode; lattice text is learned apart (about 17x larger), and so
-    // is sample text, per rendering of a sentence.
-    double& text_ratio_ref() {
-        return lattice_ == 2 ? text_per_byte_lat_[output_mode_] : sample_text_ ? text_per_byte_samp_[output_mode_] : text_per_byte_[output_mode_];
-    }
+    double& text_ratio_ref() { return text_per_byte_[kTextSrcs[text_src_].ratio][output_mode_]; }
 
     // Output stage buffers of slot `o` and scan storage of `w` for (chunks of) up to n_sent sentences.
     void ensure_format(OutSlot& o, Workspace& w, uint32_t n_sent) {
-        const size_t units = size_t(n_sent) * (sample_text_ ? samp_n_ : 1) + 1;  // sentences, or walks in sample text
+        const size_t units = size_t(n_sent) * text_view(o).units + 1;
         o.sent_len.ensure(units * 8, 1.25);
-        if (sample_text_) o.walk_off.ensure(units * 8, 1.25);
+        if (text_src_ == kTextSamples) o.walk_off.ensure(units * 8, 1.25);
         o.buf[kTextOff].ensure((size_t(n_sent) + 1) * 8, 1.25);
         size_t tmp = 0;
         CK(cub::DeviceScan::ExclusiveSum(nullptr, tmp, static_cast<unsigned long long*>(nullptr),
@@ -1158,54 +1194,40 @@ class EngineImpl final : public Engine {
     // renders the walks of the samples instead: its offsets per walk go to o.walk_off, and pass 2 (format_write)
     // takes those of each sentence's first walk into the text offsets.
     FormatArgs format_offsets(Workspace& w, const uint8_t* d_utf8, const unsigned long long* d_off, uint32_t n_sent, OutSlot& o) {
-        if (sample_text_) {
-            FormatArgs f = format_args(d_utf8, d_off, n_sent, o, o.buf[kSampleOff], o.buf[kSamples]);
-            const size_t walks = size_t(n_sent) * samp_n_;
-            f.text_off = o.walk_off.as<unsigned long long>();
-            CK(cudaMemsetAsync(f.sent_len + walks, 0, 8, w.stream));
-            if (!n_sent) CK(cudaMemsetAsync(o.buf[kTextOff].p, 0, 8, w.stream));  // no walk writes it
-            launch_format_len_samples(dv_, f, samp_n_, w.stream);
-            exclusive_scan(w, f.sent_len, f.text_off, walks + 1);
-            return f;
-        }
-        // lattice text renders the nodes as tokens, posterior text the posterior path
-        const bool nodes = lattice_ == 2, post = post_text_;
-        const int off = nodes ? kNodeOff : post ? kPostOff : kTokOff, recs = nodes ? kNodes : post ? kPostTokens : kTokens;
-        const int prob = nodes ? kNodeProb : post ? kPostProb : kTokenProb;
-        FormatArgs f = format_args(d_utf8, d_off, n_sent, o, o.buf[off], o.buf[recs]);
-        f.token_prob = (o.made.marg && (fmt_uses_ & kUsesProb)) ? o.buf[prob].as<float>() : nullptr;  // %pP
-        CK(cudaMemsetAsync(f.sent_len + n_sent, 0, 8, w.stream));
-        launch_format_len(dv_, f, w.stream, fmt_links(o));
-        exclusive_scan(w, f.sent_len, f.text_off, size_t(n_sent) + 1);
-        return f;
-    }
-
-    // The arguments of the output stage for slot `o`, rendering the records `tokens` at the offsets `tok_off`.
-    FormatArgs format_args(const uint8_t* d_utf8, const unsigned long long* d_off, uint32_t n_sent, OutSlot& o,
-                           const DevBuf& tok_off, const DevBuf& tokens) const {
+        const TextView t = text_view(o);
         FormatArgs f{};
         f.utf8 = d_utf8;
         f.byte_off = d_off;
         f.n_sent = n_sent;
-        f.tok_off = tok_off.as<unsigned long long>();
-        f.tokens = tokens.as<uint2>();
+        f.tok_off = t.tok_off->as<unsigned long long>();
+        f.tokens = t.tokens->as<uint2>();
+        f.token_prob = t.prob;
         f.sent_len = o.sent_len.as<unsigned long long>();
-        f.text_off = o.buf[kTextOff].as<unsigned long long>();
+        f.text_off = (text_src_ == kTextSamples ? o.walk_off : o.buf[kTextOff]).as<unsigned long long>();
         f.text = o.buf[kText].as<uint8_t>();
         f.text_cap = o.buf[kText].cap;
         Control* dc = o.ctrl.as<Control>();
         f.flags = &dc->flags;
         f.text_total = &dc->total[kGroupText];
         set_mode(f);
+        const size_t units = size_t(n_sent) * t.units;
+        CK(cudaMemsetAsync(f.sent_len + units, 0, 8, w.stream));
+        if (text_src_ == kTextSamples) {
+            if (!n_sent) CK(cudaMemsetAsync(o.buf[kTextOff].p, 0, 8, w.stream));  // no walk writes it
+            launch_format_len_samples(dv_, f, samp_n_, w.stream);
+        } else {
+            launch_format_len(dv_, f, w.stream, t.links);
+        }
+        exclusive_scan(w, f.sent_len, f.text_off, units + 1);
         return f;
     }
 
     // Output stage, pass 2 on `st`, after format_offsets.
     void format_write(const FormatArgs& f, OutSlot& o, cudaStream_t st) {
-        if (sample_text_)
+        if (text_src_ == kTextSamples)
             launch_format_write_samples(dv_, f, samp_n_, o.buf[kTextOff].as<unsigned long long>(), st);
         else
-            launch_format_write(dv_, f, st, fmt_links(o));
+            launch_format_write(dv_, f, st, text_view(o).links);
     }
 
     // Output stage of a whole batch (or shard) that run_whole left in out_[0]: the text buffer is sized from the
@@ -1215,7 +1237,7 @@ class EngineImpl final : public Engine {
         ensure_format(o, ws_[0], n_sent);
         FormatArgs f = format_offsets(ws_[0], d_utf8, d_off, n_sent, o);
         unsigned long long total = 0;
-        const size_t units = size_t(n_sent) * (sample_text_ ? samp_n_ : 1);  // the scan's last entry is the total
+        const size_t units = size_t(n_sent) * text_view(o).units;  // the scan's last entry is the total
         CK(cudaMemcpyAsync(&total, f.text_off + units, 8, cudaMemcpyDeviceToHost, stream_));
         CK(cudaStreamSynchronize(stream_));
         o.buf[kText].ensure(total + 16, 1.25);
@@ -1359,7 +1381,7 @@ class EngineImpl final : public Engine {
         set_mode(f);
 
         // the first copy brings the text expected from the learned ratio; more comes in a second one
-        const size_t text_guess = fmt ? std::min<size_t>(f.text_cap, size_t(double(n_bytes) * text_per_byte_[output_mode_]) +
+        const size_t text_guess = fmt ? std::min<size_t>(f.text_cap, size_t(double(n_bytes) * text_per_byte_[0][output_mode_]) +
                                                                          size_t(n_sent) * text_per_sent_ + 256)
                                       : 0;
         OutSlot& o = out_[0];
@@ -1381,7 +1403,7 @@ class EngineImpl final : public Engine {
                                cudaMemcpyDeviceToHost, stream_));
             CK(cudaStreamSynchronize(stream_));
             if (n_bytes)
-                text_per_byte_[output_mode_] = std::max(text_per_byte_[output_mode_] * 1.5, double(h.text_bytes) / double(n_bytes) * 1.25);
+                text_per_byte_[0][output_mode_] = std::max(text_per_byte_[0][output_mode_] * 1.5, double(h.text_bytes) / double(n_bytes) * 1.25);
         }
         HostResult* r = pool_.acquire(outputs(), n_sent, Totals{h.n_tokens, fmt ? h.text_bytes : 0, 0, 0});
         std::memcpy(r->buf[kTokOff].p, small_out_h_ + at_tok_off, off_bytes);
@@ -1482,6 +1504,13 @@ class EngineImpl final : public Engine {
         size_t cap = w.scan_tmp.cap;  // sized by ensure_workspace
         CK(cub::DeviceScan::ExclusiveSum(w.scan_tmp.p, cap, in, out, n, w.stream));
     }
+    // A ragged group's offsets on w.stream: off[0..n] = the exclusive scan of the n counts cnt (cnt[n], which the scan
+    // reads, zeroed first), and the group's total off[n] into Control.
+    void scan_group(Workspace& w, uint32_t* cnt, unsigned long long* off, size_t n, unsigned long long* total) {
+        CK(cudaMemsetAsync(cnt + n, 0, 4, w.stream));
+        exclusive_scan(w, CountsU64(cnt, CastU64()), off, n + 1);
+        CK(cudaMemcpyAsync(total, off + n, 8, cudaMemcpyDeviceToDevice, w.stream));
+    }
 
     // Candidates a batch (or chunk) of n_bytes bytes is given room for, from the ratio learned on earlier batches.
     size_t want_cand(uint64_t n_bytes) const {
@@ -1493,16 +1522,16 @@ class EngineImpl final : public Engine {
     // pool by them, both from this one list.
     template <typename F>
     void per_entry(Workspace& w, OutSlot& o, F&& f) const {
-        const bool fwd = theta_ > 0 || samp_n_;  // the forward pass runs
+        const PassPlan p = plan();
         f(w.ends_hot, 8);
         f(w.ends_cold, 16);
-        if (fwd || margin_on()) {  // ... or its R-only instantiation for the near-best lattice
+        if (p.fwd != kFwdNone) {
             f(w.m_cand_entry, 4);
             f(w.m_R, 8);
         }
-        if (fwd) f(w.m_ab, 16);
-        if (samp_n_ || post_) f(w.m_lw, 4);
-        if (margin_on()) {
+        if (p.fwd >= kFwdLse) f(w.m_ab, 16);
+        if (p.fwd == kFwdLseLw) f(w.m_lw, 4);
+        if (p.margin) {
             f(w.g_G, 8);
             f(w.g_keep, 4);
         }
@@ -1540,26 +1569,25 @@ class EngineImpl final : public Engine {
         w.ends_meta.ensure(ms * 8, 1.25);
         if (bounded) w.bnd_dist.ensure(ms * 4, 1.25);
         if (spans) w.span_tag.ensure(ms * 8, 1.25);
-        const bool fwd = theta_ > 0 || samp_n_;  // the forward pass runs
-        const bool rfwd = fwd || margin_on();    // ... or its R-only instantiation
-        if (rfwd) {
+        const PassPlan p = plan();
+        if (p.fwd != kFwdNone) {
             w.m_fill.ensure(ms * 4, 1.25);
             w.m_ncand.ensure(ms * 4, 1.25);
             w.m_r_eos.ensure(ns * 8, 1.25);
         }
-        if (fwd) w.m_a_eos.ensure(ns * 8, 1.25);
-        if (lattice_) {
+        if (p.fwd >= kFwdLse) w.m_a_eos.ensure(ns * 8, 1.25);
+        if (p.lat) {
             w.l_row_base.ensure(ms * 4, 1.25);
             w.l_n_nodes.ensure(ns * 4, 1.25);
         }
         if (counting_) w.stats.ensure(ms * 16, 1.25);
         w.seg.ensure(cands * 8);  // sized like the candidates; move segments can outnumber them (overflow retry)
-        if (samp_n_) {
-            const size_t walks = size_t(n_sent) * samp_n_ + 1;
+        const size_t walks = size_t(n_sent) * p.samp + 1;
+        if (p.samp) {
             w.s_cnt.ensure(walks * 4, 1.25);
             w.s_total.ensure(walks * 4, 1.25);
         }
-        if (post_) {
+        if (p.post) {
             w.p_V.ensure(ms * 8, 1.25);
             w.p_A.ensure(ms * 4, 1.25);
             w.p_cnt.ensure(ns * 4, 1.25);
@@ -1568,15 +1596,9 @@ class EngineImpl final : public Engine {
         size_t tmp = 0;  // cub temp storage for the largest scan / sort of this size
         cub::DeviceScan::ExclusiveSum(nullptr, tmp, static_cast<uint32_t*>(nullptr), static_cast<uint32_t*>(nullptr), ms, w.stream);
         w.scan_tmp.ensure(tmp + 1024, 1.5);
-        if (post_) {  // the scan of the posterior paths' token counts
-            cub::TransformInputIterator<unsigned long long, CastU64, const uint32_t*> it(static_cast<const uint32_t*>(nullptr), CastU64());
-            cub::DeviceScan::ExclusiveSum(nullptr, tmp, it, static_cast<unsigned long long*>(nullptr), ns, w.stream);
-            w.scan_tmp.ensure(tmp + 1024, 1.5);
-        }
-        if (samp_n_) {  // the scan of the walks' token counts
-            cub::TransformInputIterator<unsigned long long, CastU64, const uint32_t*> it(static_cast<const uint32_t*>(nullptr), CastU64());
-            cub::DeviceScan::ExclusiveSum(nullptr, tmp, it, static_cast<unsigned long long*>(nullptr),
-                                          size_t(n_sent) * samp_n_ + 1, w.stream);
+        const size_t group = std::max(p.lat || p.post ? ns : 0, p.samp ? walks : 0);  // the longest scan_group
+        if (group) {
+            cub::DeviceScan::ExclusiveSum(nullptr, tmp, CountsU64(nullptr, CastU64()), static_cast<unsigned long long*>(nullptr), group, w.stream);
             w.scan_tmp.ensure(tmp + 1024, 1.5);
         }
         if (order_mode_ == 1) {
@@ -1653,8 +1675,7 @@ class EngineImpl final : public Engine {
             cap_all = std::min<size_t>(cap_all, rows > n_sent ? rows - n_sent - 1 : 0);
         });
         const uint32_t cand_cap = uint32_t(cap_all);
-        const bool marg = theta_ > 0, samp = samp_n_ != 0;
-        const bool lat = lattice_ != 0, mlat = margin_on();
+        const PassPlan p = plan();
         Batch b{};
         b.utf8 = d_utf8;
         b.byte_off = d_off;
@@ -1750,8 +1771,10 @@ class EngineImpl final : public Engine {
         CK(cudaEventRecord(o.ev[5], st));
         o.launches += launch_viterbi(dv_, b, counting_ ? w.stats.as<uint4>() : nullptr, lanes_, viterbi_kernel_, st, &o.route);
         MargArgs m{};
-        if (marg || samp || mlat) {
-            m.theta = marg ? theta_ : samp_theta_;  // equal when both are on (set_marginals / set_sampling)
+        UncertaintyArgs u{};
+        MarginArgs g{};
+        if (p.fwd != kFwdNone) {  // booked with the Viterbi stage; must run before K4 reuses ends_meta
+            m.theta = theta_ > 0 ? theta_ : samp_theta_;  // equal when both are on (set_marginals / set_sampling)
             m.fill = w.m_fill.as<uint32_t>();
             m.ncand = w.m_ncand.as<uint32_t>();
             m.cand_entry = w.m_cand_entry.as<uint32_t>();
@@ -1760,61 +1783,45 @@ class EngineImpl final : public Engine {
             m.r_eos = w.m_r_eos.as<long long>();
             m.a_eos = w.m_a_eos.as<double>();
             m.path_prob = o.buf[kPathProb].as<float>();
-            m.token_prob = marg ? o.buf[kTokenProb].as<float>() : nullptr;
-            m.lw = (samp || post_) ? w.m_lw.as<uint32_t>() : nullptr;  // the prefix costs of samples and posterior paths
-        }
-        if (marg || samp) {  // booked with the Viterbi stage; must run before K4 reuses ends_meta
-            UncertaintyArgs u{};
-            if (unc_) {  // the backward pass's uncertainty instantiation, and with 2 the boundary probabilities
-                u.entropy = o.buf[kEntropy].as<double>();
-                u.log_path_prob = o.buf[kLogPathProb].as<double>();
-                if (unc_ >= 2) {
-                    u.pos_off = o.buf[kPosOff].as<unsigned long long>();
-                    u.boundary_prob = o.buf[kBoundaryProb].as<float>();
-                    if (n_sent == 0) CK(cudaMemsetAsync(u.pos_off, 0, 8, st));
-                    // the group's records: one per slot (the low word of a total zeroed with the rest of Control)
-                    CK(cudaMemcpyAsync(&dc->total[kGroupPositions], b.slot_off + n_sent, 4, cudaMemcpyDeviceToDevice, st));
-                }
+            m.token_prob = p.bwd != kBwdNone ? o.buf[kTokenProb].as<float>() : nullptr;
+            m.lw = p.fwd == kFwdLseLw ? w.m_lw.as<uint32_t>() : nullptr;
+            if (p.bwd == kBwdUnc) u = UncertaintyArgs{o.buf[kEntropy].as<double>(), o.buf[kLogPathProb].as<double>()};
+            if (p.bprob) {
+                u.pos_off = o.buf[kPosOff].as<unsigned long long>();
+                u.boundary_prob = o.buf[kBoundaryProb].as<float>();
+                if (n_sent == 0) CK(cudaMemsetAsync(u.pos_off, 0, 8, st));
+                // the group's records: one per slot (the low word of a total zeroed with the rest of Control)
+                CK(cudaMemcpyAsync(&dc->total[kGroupPositions], b.slot_off + n_sent, 4, cudaMemcpyDeviceToDevice, st));
             }
-            launch_marginals(dv_, b, m, st, marg, unc_ ? &u : nullptr);  // sampling alone needs no backward pass
-            if (n_sent) o.launches += (marg ? 2 : 1) + (unc_ >= 2 ? 1 : 0);
+            if (p.margin)  // G of every entry, from the R of the forward pass
+                g = MarginArgs{lat_margin_, w.g_G.as<long long>(), w.g_keep.as<uint32_t>(), o.buf[kNodeMargin].as<long long>()};
+            launch_marginals(dv_, b, m, p.fwd, p.bwd, u, p.margin ? &g : nullptr, st);
+            if (n_sent) o.launches += 1 + (p.bwd != kBwdNone) + p.bprob + p.margin;
         }
-        MarginArgs g{};
-        if (mlat) {  // G of every entry, from the R the forward pass above left (or its R-only instantiation here)
-            g = MarginArgs{lat_margin_, w.g_G.as<long long>(), w.g_keep.as<uint32_t>(), o.buf[kNodeMargin].as<long long>()};
-            launch_margin_backward(dv_, b, m, g, !(marg || samp), st);
-            if (n_sent) o.launches += (marg || samp) ? 1 : 2;
-        }
-        if (lat) {  // booked with the Viterbi stage too, and also before K4
+        if (p.lat) {  // booked with the Viterbi stage too, and also before K4
             LatticeArgs l{};
             l.row_base = w.l_row_base.as<uint32_t>();
             l.n_nodes = w.l_n_nodes.as<uint32_t>();
             l.node_off = o.buf[kNodeOff].as<unsigned long long>();
             l.nodes = o.buf[kNodes].as<uint2>();
             l.links = o.buf[kLinks].as<int2>();
-            l.node_prob = marg ? o.buf[kNodeProb].as<float>() : nullptr;
-            launch_lattice_count(b, l, m, mlat ? &g : nullptr, st);
-            cub::TransformInputIterator<unsigned long long, CastU64, const uint32_t*> it(l.n_nodes, CastU64());
-            if (n_sent == 0) CK(cudaMemsetAsync(l.n_nodes, 0, 4, st));
-            exclusive_scan(w, it, l.node_off, size_t(n_sent) + 1);
-            launch_lattice_write(b, l, m, mlat ? &g : nullptr, st);
-            CK(cudaMemcpyAsync(&dc->total[kGroupLattice], l.node_off + n_sent, 8, cudaMemcpyDeviceToDevice, st));
+            l.node_prob = p.bwd != kBwdNone ? o.buf[kNodeProb].as<float>() : nullptr;
+            launch_lattice_count(b, l, m, p.margin ? &g : nullptr, st);
+            scan_group(w, l.n_nodes, l.node_off, n_sent, &dc->total[kGroupLattice]);
+            launch_lattice_write(b, l, m, p.margin ? &g : nullptr, st);
             if (n_sent) o.launches += 2;
         }
-        if (samp) {  // booked with the Viterbi stage too, and also before K4
+        if (p.samp) {  // booked with the Viterbi stage too, and also before K4
             SampleArgs sa{};
-            sa.n = samp_n_;
+            sa.n = p.samp;
             sa.seed = samp_seed_;
             sa.sent_base = sample_base_ + sent0;
             sa.cnt = w.s_cnt.as<uint32_t>();
             sa.total = w.s_total.as<int32_t>();
             sa.off = o.buf[kSampleOff].as<unsigned long long>();
-            const size_t walks = size_t(n_sent) * samp_n_;
+            const size_t walks = size_t(n_sent) * p.samp;
             launch_sample_count(dv_, b, m, sa, st);
-            CK(cudaMemsetAsync(sa.cnt + walks, 0, 4, st));
-            cub::TransformInputIterator<unsigned long long, CastU64, const uint32_t*> it(sa.cnt, CastU64());
-            exclusive_scan(w, it, sa.off, walks + 1);
-            CK(cudaMemcpyAsync(&dc->total[kGroupSamples], sa.off + walks, 8, cudaMemcpyDeviceToDevice, st));
+            scan_group(w, sa.cnt, sa.off, walks, &dc->total[kGroupSamples]);
             // the records are sized from the scanned total: one wait for it here
             CK(cudaMemcpyAsync(&o.h_ctrl->total[kGroupSamples], sa.off + walks, 8, cudaMemcpyDeviceToHost, st));
             CK(cudaStreamSynchronize(st));
@@ -1823,23 +1830,20 @@ class EngineImpl final : public Engine {
             launch_sample_write(dv_, b, m, sa, st);
             if (walks) o.launches += 2;
         }
-        if (post_) {  // booked with the Viterbi stage too, and also before K4; marginals are on (set_posterior)
-            PosteriorArgs p{};
-            p.g1 = post_g1_;
-            p.V = w.p_V.as<double>();
-            p.A = w.p_A.as<uint32_t>();
-            p.cnt = w.p_cnt.as<uint32_t>();
-            p.total = w.p_total.as<int32_t>();
-            p.off = o.buf[kPostOff].as<unsigned long long>();
-            p.out = o.buf[kPostTokens].as<uint2>();
-            p.prob = o.buf[kPostProb].as<float>();
-            p.gain = o.buf[kPostGain].as<double>();
-            launch_posterior_sweep(dv_, b, m, p, st);
-            CK(cudaMemsetAsync(p.cnt + n_sent, 0, 4, st));
-            cub::TransformInputIterator<unsigned long long, CastU64, const uint32_t*> it(p.cnt, CastU64());
-            exclusive_scan(w, it, p.off, size_t(n_sent) + 1);
-            CK(cudaMemcpyAsync(&dc->total[kGroupPosterior], p.off + n_sent, 8, cudaMemcpyDeviceToDevice, st));
-            launch_posterior_write(dv_, b, m, p, st);
+        if (p.post) {  // booked with the Viterbi stage too, and also before K4; marginals are on (set_posterior)
+            PosteriorArgs q{};
+            q.g1 = post_g1_;
+            q.V = w.p_V.as<double>();
+            q.A = w.p_A.as<uint32_t>();
+            q.cnt = w.p_cnt.as<uint32_t>();
+            q.total = w.p_total.as<int32_t>();
+            q.off = o.buf[kPostOff].as<unsigned long long>();
+            q.out = o.buf[kPostTokens].as<uint2>();
+            q.prob = o.buf[kPostProb].as<float>();
+            q.gain = o.buf[kPostGain].as<double>();
+            launch_posterior_sweep(dv_, b, m, q, st);
+            scan_group(w, q.cnt, q.off, n_sent, &dc->total[kGroupPosterior]);
+            launch_posterior_write(dv_, b, m, q, st);
             if (n_sent) o.launches += 2;
         }
         // backtrack_count and scan_tokens are folded into k_backtrack, which is booked under backtrack_write
@@ -1847,7 +1851,7 @@ class EngineImpl final : public Engine {
         CK(cudaEventRecord(o.ev[7], st));
         CK(cudaEventRecord(o.ev[8], st));
         if (n_sent)
-            launch_backtrack(b, marg ? &m : nullptr, ts, st);
+            launch_backtrack(b, p.bwd != kBwdNone ? &m : nullptr, ts, st);
         else
             CK(cudaMemsetAsync(b.tok_off, 0, 8, st));
         k_publish_totals<<<1, 1, 0, st>>>(b.slot_off, b.tok_off, n_sent, dc);
@@ -1921,16 +1925,7 @@ class EngineImpl final : public Engine {
     int order_mode_ = 0;  // K3's sentence order: 0 input order, 1 whole batch by length, 2 by length inside tiles
     uint32_t output_mode_ = 0;
     uint64_t batch_total_bytes_ = 0;  // size of the input buffer of the batch in flight (bounds check in K1)
-    // output text bytes expected per input byte (beyond text_per_sent_ per sentence), by output mode: sizes the text
-    // buffers of the chunked host pipeline, learned like cand_per_byte_
-    static constexpr double kFormatTextPerByte = 8.0;
-    double text_per_byte_[5] = {0.0, 8.0, 2.0, 16.0, kFormatTextPerByte};
-    // the same for lattice text ("lattice" = 2), which renders ~17 nodes per token
-    static constexpr double kLatticeTextFactor = 17.0;
-    double text_per_byte_lat_[5] = {0.0, 8.0 * kLatticeTextFactor, 2.0 * kLatticeTextFactor, 16.0 * kLatticeTextFactor,
-                                    kFormatTextPerByte * kLatticeTextFactor};
-    // and for sample text ("sample_text" = 1), per rendering of a sentence: each sentence renders samp_n_ times
-    double text_per_byte_samp_[5] = {0.0, 8.0, 2.0, 16.0, kFormatTextPerByte};
+    TextRatios text_per_byte_ = kTextPerByte;  // sizes the text buffers of the chunked pipeline, learned like cand_per_byte_
     double node_per_byte_ = 2.0;  // lattice nodes per input byte: sizes the host result of the chunked pipeline
     uint32_t text_per_sent_ = 4;  // "EOS\n"; an output format: what its BOS and EOS print (FormatProgram::per_sentence)
     // output format (set_format): the compiled program and its field table, with the table's size and build time
@@ -1943,7 +1938,8 @@ class EngineImpl final : public Engine {
     uint32_t tok_bytes_ = 24;
     int viterbi_kernel_ = 1;  // 1 = k_viterbi2 with pruning (kernels.cuh)
     double theta_ = 0;        // marginals' theta, 0 = off (set_marginals)
-    int lattice_ = 0;         // option "lattice": 0 off, 1 nodes, 2 nodes and lattice text
+    bool lattice_ = false;    // option "lattice" >= 1
+    TextSrc text_src_ = kTextBest;  // what the output text renders (set_text)
     static constexpr long long kMaxLatticeMargin = 1ll << 62;
     long long lat_margin_ = -1;  // option "lattice_margin": the near-best lattice's D, -1 = off
     uint32_t unc_ = 0;           // option "uncertainty": 0 off, 1 entropy and log_path_prob, 2 also boundary probabilities
@@ -1951,10 +1947,8 @@ class EngineImpl final : public Engine {
     uint32_t samp_n_ = 0;       // sampling: paths per sentence, 0 = off (set_sampling)
     double samp_theta_ = 0;
     uint64_t samp_seed_ = 0;
-    bool sample_text_ = false;  // option "sample_text": the output text renders the samples
     bool post_ = false;         // posterior decoding (set_posterior)
     double post_g1_ = 0;        // its gamma + 1
-    bool post_text_ = false;    // option "posterior_text": the output text renders the posterior paths
     static constexpr long long kMaxSampleBase = 0x100000000ll;
     uint64_t sample_base_ = 0;  // option "sample_base": the draws' index of the call's first sentence
     DeviceOutputs last_;  // what the last run_device or run_shard left in out_[0] (last_device)

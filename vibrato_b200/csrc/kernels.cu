@@ -3397,33 +3397,24 @@ void launch_backtrack(const Batch& b, const MargArgs* m, const TileScan& ts, cud
         launch_backtrack_marg<false>(b, MargArgs{}, ts, st);
 }
 
-// The forward pass's instantiation: with m.lw (sampling) the one that also keeps {left id, word cost}.
-// With u: the uncertainty instantiation of the backward pass.
-void launch_marginals(const DictView& d, const Batch& b, const MargArgs& m, cudaStream_t st, bool backward,
-                      const UncertaintyArgs* u) {
+void launch_marginals(const DictView& d, const Batch& b, const MargArgs& m, FwdKind fwd, BwdKind bwd,
+                      const UncertaintyArgs& u, const MarginArgs* g, cudaStream_t st) {
     if (!b.n_sent) return;
     const uint32_t blocks = (b.n_sent + 7) / 8;  // a warp per sentence
     with_connector(d, [&](auto conn) {
-        if (m.lw)
+        if (fwd == kFwdLseLw)
             k_marg_forward<conn, true><<<blocks, 256, 0, st>>>(d, b, m);
-        else
+        else if (fwd == kFwdLse)
             k_marg_forward<conn><<<blocks, 256, 0, st>>>(d, b, m);
-        if (backward && u)
-            k_marg_backward<conn, true><<<blocks, 256, 0, st>>>(d, b, m, *u);
-        else if (backward)
+        else if (fwd == kFwdR)
+            k_marg_forward<conn, false, false><<<blocks, 256, 0, st>>>(d, b, m);
+        if (bwd == kBwdUnc)
+            k_marg_backward<conn, true><<<blocks, 256, 0, st>>>(d, b, m, u);
+        else if (bwd == kBwdPlain)
             k_marg_backward<conn><<<blocks, 256, 0, st>>>(d, b, m, UncertaintyArgs{});
     });
-    if (backward && u && u->boundary_prob) k_boundary_probs<<<blocks, 256, 0, st>>>(b, m, *u);
-}
-
-void launch_margin_backward(const DictView& d, const Batch& b, const MargArgs& m, const MarginArgs& g, bool forward,
-                            cudaStream_t st) {
-    if (!b.n_sent) return;
-    const uint32_t blocks = (b.n_sent + 7) / 8;  // a warp per sentence
-    with_connector(d, [&](auto conn) {
-        if (forward) k_marg_forward<conn, false, false><<<blocks, 256, 0, st>>>(d, b, m);
-        k_margin_backward<conn><<<blocks, 256, 0, st>>>(d, b, m, g);
-    });
+    if (u.boundary_prob) k_boundary_probs<<<blocks, 256, 0, st>>>(b, m, u);
+    if (g) with_connector(d, [&](auto conn) { k_margin_backward<conn><<<blocks, 256, 0, st>>>(d, b, m, *g); });
 }
 
 void launch_lattice_count(const Batch& b, const LatticeArgs& l, const MargArgs& m, const MarginArgs* g, cudaStream_t st) {

@@ -294,11 +294,15 @@ struct UncertaintyArgs {
     unsigned long long* pos_off;   // n_sent + 1: the slot offsets widened, or nullptr (no boundary probabilities)
     float* boundary_prob;          // per slot; 1 at a sentence's first slot (BOS) when it has a path
 };
-// k_marg_forward and k_marg_backward (two launches); backward = false runs the forward pass alone (sampling without
-// marginals).  m.lw != nullptr selects the forward pass that also writes MargArgs::lw.  With u (backward only): the
-// uncertainty instantiation of k_marg_backward, then k_boundary_probs when u->boundary_prob != nullptr.
-void launch_marginals(const DictView& d, const Batch& b, const MargArgs& m, cudaStream_t st, bool backward = true,
-                      const UncertaintyArgs* u = nullptr);
+// The instantiations of k_marg_forward: R only (the near-best lattice alone), the log-sum-exp, and the log-sum-exp
+// that also writes MargArgs::lw (samples and posterior paths); and of k_marg_backward: plain or uncertainty.
+enum FwdKind { kFwdNone, kFwdR, kFwdLse, kFwdLseLw };
+enum BwdKind { kBwdNone, kBwdPlain, kBwdUnc };
+struct MarginArgs;
+// k_marg_forward of kind fwd, k_marg_backward of kind bwd, k_boundary_probs when u.boundary_prob != nullptr, then
+// k_margin_backward when g != nullptr; each kind but None is one launch.  u is read by kBwdUnc and k_boundary_probs.
+void launch_marginals(const DictView& d, const Batch& b, const MargArgs& m, FwdKind fwd, BwdKind bwd,
+                      const UncertaintyArgs& u, const MarginArgs* g, cudaStream_t st);
 // backtrack_count, the token-offset scan and backtrack_write: n_tok, tok_off (n_sent + 1 entries) and the token
 // records; with m (marginals) also MargArgs::token_prob of every token.
 void launch_backtrack(const Batch& b, const MargArgs* m, const TileScan& ts, cudaStream_t st);
@@ -328,10 +332,7 @@ struct MarginArgs {
     uint32_t* keep;            // per lattice entry: the sentence-relative index in the kept list, or kNone
     long long* node_margin;    // per kept node
 };
-// The R-only instantiation of k_marg_forward when `forward` (neither marginals nor sampling ran it), then
-// k_margin_backward: G of every lattice entry.  After K3 and before K4, like launch_marginals.
-void launch_margin_backward(const DictView& d, const Batch& b, const MargArgs& m, const MarginArgs& g, bool forward,
-                            cudaStream_t st);
+// k_margin_backward (launch_marginals): G of every lattice entry, from the R of any forward pass.
 // A warp per sentence; g == nullptr: the full lattice, else the near-best one.
 // k_lattice_count: row_base and l.n_nodes; k_lattice_count_margin: g->keep and l.n_nodes (the kept count).  The scan
 // of n_nodes then gives l.node_off.
