@@ -205,7 +205,10 @@ int32_t vbt_tokenizer_new_multi(const vbt_dict *d, int32_t ignore_space, uint64_
  * names the Viterbi kernel that did the work in its last call: "last_viterbi": "k_viterbi" (round 1; every counted
  * run) | "k_viterbi2" (with lower-bound pruning) | "k_viterbi2_unpruned" (viterbi_kernel 2, the Raw and Dual
  * connectors, or a batch holding a sentence of more than 16 000 characters) | "k_small_batch" (the whole call in one
- * kernel, see the option "small_batch") | "none" (no call yet, or no sentence). */
+ * kernel, see the option "small_batch") | "none" (no call yet, or no sentence).  Every tokenizer also counts the
+ * attempts its last call ran again, by reason (summed over the shards of a multi-device one): "last_reruns": {"pool":
+ * the candidate pool outgrew its estimate, "slots": more characters per byte than estimated, "text": a chunk's output
+ * text outgrew its buffer}; the options "pool_estimate_permille" and "chars_estimate_permille" set those estimates. */
 int32_t vbt_tokenizer_describe(const vbt_tokenizer *t, char *buf, size_t cap);
 /* Restricts the calling thread to the CPUs of the NUMA node `device` hangs off (host-side copies of a rank then
  * stay on its socket); never widens the process's own affinity mask. */

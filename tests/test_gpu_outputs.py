@@ -1,6 +1,6 @@
-"""Every batch output at once (tokens, marginals, lattice, node margins, samples and text) on every route, the
-chunked pipeline's host result growing past its initial estimates while keeping what it already holds, and the
-refusals of the device-resident accessors."""
+"""Every batch output at once (tokens, marginals, uncertainty, lattice, node margins, samples, posterior paths and
+text) on every route, the chunked pipeline's host result growing past its initial estimates while keeping what it
+already holds, and the refusals of the device-resident accessors."""
 import re
 import string
 
@@ -15,8 +15,9 @@ pytestmark = pytest.mark.gpu
 THETA = 0.001
 N_SAMP = 3
 ROUTES = ("whole", "chunked", "device", "multi", "multi_device")
-NAMES = ("tok_offsets", "tokens", "token_probs", "path_probs", "node_offsets", "nodes", "node_links", "node_probs",
-         "node_margins", "sample_offsets", "samples")
+NAMES = ("tok_offsets", "tokens", "token_probs", "path_probs", "entropies", "log_path_probs", "boundary_offsets",
+         "boundary_probs", "node_offsets", "nodes", "node_links", "node_probs", "node_margins", "sample_offsets", "samples",
+         "posterior_offsets", "posterior_tokens", "posterior_probs", "posterior_gains")
 MARGIN = 2000  # the near-best lattice's cost margin when it is on
 
 
@@ -24,7 +25,8 @@ def make(d, route, text=True, margin=None):
     tok = vb.Tokenizer.new(d, devices=shard_devices(2)) if route.startswith("multi") else vb.Tokenizer.new(d)
     if route == "chunked":
         tok.set_option("chunk_sentences", 64)
-    tok.marginals(THETA).lattice(True, margin=margin).sampling(N_SAMP, THETA, 7)
+    tok.marginals(THETA).uncertainty(True, boundary_probs=True).posterior(2.0)
+    tok.lattice(True, margin=margin).sampling(N_SAMP, THETA, 7)
     return tok.output_mode("mecab") if text else tok
 
 
@@ -49,10 +51,14 @@ def run(tok, route, sents, text=True, margin=None):
         no, nodes, links, nprob, nn = tok.last_device_lattice()
         nm = tok.last_device_lattice_margins() if margin is not None else None
         so, s, ns = tok.last_device_samples()
+        ent, lpp, boff, bprob, npos = tok.last_device_uncertainty()
+        poff, ptok, pprob, pgain, npost = tok.last_device_posterior()
         arrays = (d2h(a, n + 1, np.uint64), d2h(b, nt, vb.TOKEN_DTYPE), d2h(tp, nt, np.float32), d2h(pp, n, np.float32),
-                  d2h(no, n + 1, np.uint64), d2h(nodes, nn, vb.TOKEN_DTYPE), d2h(links, nn, vb.LINK_DTYPE),
-                  d2h(nprob, nn, np.float32), None if nm is None else d2h(nm, nn, np.int64),
-                  d2h(so, n * N_SAMP + 1, np.uint64), d2h(s, ns, vb.TOKEN_DTYPE))
+                  d2h(ent, n, np.float64), d2h(lpp, n, np.float64), d2h(boff, n + 1, np.uint64),
+                  d2h(bprob, npos, np.float32), d2h(no, n + 1, np.uint64), d2h(nodes, nn, vb.TOKEN_DTYPE),
+                  d2h(links, nn, vb.LINK_DTYPE), d2h(nprob, nn, np.float32), None if nm is None else d2h(nm, nn, np.int64),
+                  d2h(so, n * N_SAMP + 1, np.uint64), d2h(s, ns, vb.TOKEN_DTYPE), d2h(poff, n + 1, np.uint64),
+                  d2h(ptok, npost, vb.TOKEN_DTYPE), d2h(pprob, npost, np.float32), d2h(pgain, n, np.float64))
         return {name: x for name, x in zip(NAMES, arrays) if name in names}
     res = tok.tokenize_batch(utf8=utf8, byte_offsets=off)
     got = {name: getattr(res, name).copy() for name in names}
@@ -83,8 +89,8 @@ def check_all_outputs(golden, route, margin):
 
 @pytest.mark.parametrize("route", ROUTES)
 def test_all_outputs_on_every_route(golden, route):
-    """Marginals, lattice, three samples and mecab text together: every array is byte-identical to the whole
-    batch's (the device routes produce no text)."""
+    """Marginals, uncertainty, lattice, three samples, posterior paths and mecab text together: every array is
+    byte-identical to the whole batch's (the device routes produce no text)."""
     check_all_outputs(golden, route, None)
 
 

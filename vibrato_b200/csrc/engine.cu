@@ -586,6 +586,7 @@ class EngineImpl final : public Engine {
 
     void run_device(uint64_t d_utf8, uint64_t d_byte_off, uint64_t n_sent, uint64_t n_bytes, const Bounds* bnd) override {
         last_ = DeviceOutputs{};
+        reruns_ = Reruns{};
         CK(cudaSetDevice(device_));
         check_size(n_sent, n_bytes);
         check_bounded(bnd);
@@ -617,6 +618,7 @@ class EngineImpl final : public Engine {
     // Host path.  Large batches are cut into chunks that flow through three streams: the H2D copy of
     // chunk i+1 and the D2H copy of chunk i-1 overlap the kernels of chunk i (PCIe is full duplex).
     HostResult* run_host(const char* utf8, const uint64_t* byte_off, uint64_t n_sent64, const Bounds* bnd) override {
+        reruns_ = Reruns{};
         CK(cudaSetDevice(device_));
         // offsets may start anywhere in the caller's buffer; ship only the used window
         const uint64_t first = n_sent64 ? byte_off[0] : 0;
@@ -743,6 +745,7 @@ class EngineImpl final : public Engine {
             double text_need = 0;  // text bytes per input byte beyond per_sent per sentence, largest over the sound chunks
             uint32_t route = kRouteNone;
             bool overflow = false, bad_utf8 = false, bad_offsets = false, slots_overflow = false, text_overflow = false;
+            bool pool_overflow = false;
             bool bad_bounds = false, bad_spans = false;
             uint64_t slots_seen = 0;
             batch_total_bytes_ = n_bytes;
@@ -767,7 +770,7 @@ class EngineImpl final : public Engine {
                 if (o.h_ctrl->flags & kFlagBadOffsets) bad_offsets = true;
                 if (o.h_ctrl->flags & kFlagBadBoundary) bad_bounds = true;
                 if (o.h_ctrl->flags & kFlagBadSpan) bad_spans = true;
-                if (o.h_ctrl->flags & kFlagPoolOverflow) overflow = true;
+                if (o.h_ctrl->flags & kFlagPoolOverflow) overflow = pool_overflow = true;
                 if (o.h_ctrl->flags & kFlagSlotsOverflow) overflow = slots_overflow = true;
                 if (o.h_ctrl->flags & kFlagTextOverflow) text_overflow = true;
                 slots_seen += o.h_ctrl->total_slots;
@@ -843,6 +846,9 @@ class EngineImpl final : public Engine {
             if (overflow || text_overflow) {
                 release(r);
                 if (attempt >= 3) throw Error(kInternal, overflow ? "candidate pool overflow persists" : "text buffer overflow persists");
+                reruns_[kRerunPool] += pool_overflow;
+                reruns_[kRerunSlots] += slots_overflow;
+                reruns_[kRerunText] += text_overflow;
                 if (slots_overflow) chars_per_byte_ = 1.0;
                 if (overflow)
                     cand_per_byte_ = std::max(cand_per_byte_ * 1.5, double(pool_need_) / double(std::max<uint64_t>(1, max_chunk_bytes)) * 1.2);
@@ -868,6 +874,7 @@ class EngineImpl final : public Engine {
     Totals run_shard(const char* utf8, const uint64_t* byte_off, uint64_t n_sent64, int src_device, uint64_t first_sentence,
                      bool with_text, const Bounds* bnd) override {
         last_ = DeviceOutputs{};
+        reruns_ = Reruns{};
         CK(cudaSetDevice(device_));
         const uint64_t first = n_sent64 ? byte_off[0] : 0;
         const uint64_t n_bytes = n_sent64 ? byte_off[n_sent64] - first : 0;
@@ -919,8 +926,9 @@ class EngineImpl final : public Engine {
         if (output_mode_ == kOutFormat)  // the field table of the output format: device bytes and build time
             ft = ", \"field_table\": {\"bytes\": " + std::to_string(ft_size_) + ", \"build_ms\": " + std::to_string(ft_ms_) + "}";
         return "{\"devices\": [" + std::to_string(device_) + "], \"dictionary_transport\": \"single device\", \"token_gather\": \"none\", " +
-               "\"last_viterbi\": \"" + kRouteNames[last_route_] + "\"" + ft + "}";
+               "\"last_viterbi\": \"" + kRouteNames[last_route_] + "\"" + ft + ", " + reruns_json(reruns_) + "}";
     }
+    Reruns last_reruns() const override { return reruns_; }
 
    private:
     // Host -> device copy of caller memory.  Pinned (page-locked) memory goes straight to the copy engine; pageable
@@ -1397,7 +1405,11 @@ class EngineImpl final : public Engine {
             throw Error(kInvalidArgument, kBadOffsetsMsg);
         if (h.flags & kFlagUtf8Error) throw Error(kUtf8, kBadUtf8Msg);
         if (h.flags & kFlagBadBoundary) throw Error(kInvalidArgument, kBadBoundsMsg);
-        if (h.flags & (kFlagPoolOverflow | kFlagTextOverflow)) return nullptr;
+        if (h.flags & (kFlagPoolOverflow | kFlagTextOverflow)) {
+            reruns_[kRerunPool] += (h.flags & kFlagPoolOverflow) != 0;
+            reruns_[kRerunText] += (h.flags & kFlagTextOverflow) != 0;
+            return nullptr;
+        }
         if (fmt && h.text_bytes > text_guess) {
             CK(cudaMemcpyAsync(small_out_h_ + at_text + text_guess, region + at_text + text_guess, h.text_bytes - text_guess,
                                cudaMemcpyDeviceToHost, stream_));
@@ -1633,6 +1645,7 @@ class EngineImpl final : public Engine {
             if (o.h_ctrl->flags & kFlagBadSpan) throw Error(kInvalidArgument, kBadSpansMsg);
             if (o.h_ctrl->flags & kFlagSlotsOverflow) {  // more characters per byte than any batch before: hard bound
                 if (attempt >= 3) throw Error(kInternal, "slot overflow persists");
+                ++reruns_[kRerunSlots];
                 chars_per_byte_ = 1.0;
                 continue;
             }
@@ -1641,6 +1654,7 @@ class EngineImpl final : public Engine {
                 if (double(pool_need(*o.h_ctrl)) * 1.05 + 4096 >= double(0xFFFFFFF0ull))
                     throw Error(kInvalidArgument, "batch produces more than 2^32 lattice nodes: split it");
                 cand_per_byte_ = double(pool_need(*o.h_ctrl)) / double(std::max<uint64_t>(1, n_bytes)) * 1.05 + 1e-3;
+                ++reruns_[kRerunPool];
                 continue;
             }
             if (n_bytes) cand_per_byte_ = std::max(0.25, double(pool_need(*o.h_ctrl)) / double(n_bytes) * 1.15);
@@ -1955,6 +1969,7 @@ class EngineImpl final : public Engine {
     float stage_ms_[kNumStages];
     uint64_t launches_ = 0;
     uint32_t last_route_ = kRouteNone;  // ViterbiRoute of the last successful call (describe())
+    Reruns reruns_{};                    // the attempts the last call re-ran, by reason (describe())
     uint64_t counters_[kNumCounters];
 };
 

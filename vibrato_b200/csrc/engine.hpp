@@ -190,6 +190,16 @@ constexpr const char* kBadSpansMsg =
     "inside, not start at a space when ignore_space is on, and their offsets must be non-decreasing and within the "
     "span array";
 
+// Why a call ran an attempt again: its candidate pool, its per-character slots or (chunked host batches) the output
+// text of a chunk outgrew the size learned from earlier batches.  An attempt with several counts under each.
+enum Rerun { kRerunPool, kRerunSlots, kRerunText, kNumReruns };
+using Reruns = std::array<uint64_t, kNumReruns>;
+// describe()'s "last_reruns" entry: the attempts the last call re-ran, by reason.
+inline std::string reruns_json(const Reruns& r) {
+    return "\"last_reruns\": {\"pool\": " + std::to_string(r[kRerunPool]) + ", \"slots\": " + std::to_string(r[kRerunSlots]) +
+           ", \"text\": " + std::to_string(r[kRerunText]) + "}";
+}
+
 constexpr int kNumStages = 9;
 extern const char* const kStageNames;  // comma-separated, kNumStages entries
 // A call on the k_small_batch route ("small_batch" option) runs every stage in one kernel: its whole time is booked
@@ -235,6 +245,7 @@ class Engine {
     virtual int device() const = 0;
     virtual uint32_t token_bytes() const = 0;  // 24, or 16 with the "compact_tokens" option
     virtual std::string describe() const = 0;  // JSON: devices, how the dictionary travelled, ...
+    virtual Reruns last_reruns() const = 0;    // the attempts the last call re-ran (a multi-device one: over its shards)
 
     virtual void set_counting(bool on) = 0;
     // Knobs: "lanes_per_sentence" (4/8/16/32), "sort_by_length" (0/1), "counting" (0/1), "chunk_sentences",

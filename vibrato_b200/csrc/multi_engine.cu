@@ -229,6 +229,7 @@ class MultiEngine final : public Engine {
     // ---- host batches --------------------------------------------------------------------------------
     HostResult* run_host(const char* utf8, const uint64_t* byte_off, uint64_t n_sent, const Bounds* bnd) override {
         const int n = int(dev_.size());
+        reruns_ = Reruns{};
         if (n == 1) {  // nothing to split: the device's own chunked, overlapped host pipeline
             HostResult* r = eng_[0]->run_host(utf8, byte_off, n_sent, bnd);
             collect_stats();
@@ -264,6 +265,7 @@ class MultiEngine final : public Engine {
     // ---- device-resident batches: input on the first device, results gathered back to it ------------------
     void run_device(uint64_t d_utf8, uint64_t d_byte_off, uint64_t n_sent, uint64_t n_bytes, const Bounds* bnd) override {
         const int n = int(dev_.size());
+        reruns_ = Reruns{};
         if (n == 1) {
             eng_[0]->run_device(d_utf8, d_byte_off, n_sent, n_bytes, bnd);
             collect_stats();
@@ -430,8 +432,9 @@ class MultiEngine final : public Engine {
         s += "], \"dictionary_transport\": \"" + transport_ + "\", \"token_gather\": \"" +
              std::string(dev_.size() > 1 ? (nccl_ ? "ncclSend/ncclRecv" : "cudaMemcpyPeer") : "none") + "\", \"numa_pinned\": [";
         for (size_t i = 0; i < dev_.size(); ++i) s += (i ? ", " : "") + std::string(cpus_[i].empty() ? "false" : "true");
-        return s + "]}";
+        return s + "], " + reruns_json(reruns_) + "}";
     }
+    Reruns last_reruns() const override { return reruns_; }
 
    private:
     // Contiguous shards of about equal bytes: cut[i] = first sentence of shard i, cut[n] = n_sent.
@@ -522,6 +525,8 @@ class MultiEngine final : public Engine {
         std::memset(counters_, 0, sizeof counters_);
         launches_ = 0;
         for (auto& e : eng_) {
+            const Reruns r = e->last_reruns();  // the shards' attempts add up
+            for (int k = 0; k < kNumReruns; ++k) reruns_[k] += r[k];
             const float* s = e->stage_ms();
             for (int i = 0; i < kNumStages; ++i) stage_ms_[i] = std::max(stage_ms_[i], s[i]);  // devices run side by side
             const uint64_t* c = e->counters();
@@ -561,6 +566,7 @@ class MultiEngine final : public Engine {
     float stage_ms_[kNumStages];
     uint64_t counters_[10];
     uint64_t launches_ = 0;
+    Reruns reruns_{};  // the attempts the last call re-ran over all its shards (describe())
 };
 
 }  // namespace
