@@ -1,7 +1,8 @@
 """Every batch output at once (tokens, marginals, uncertainty with boundary probabilities, posterior paths, samples,
 the lattice and the output text) through each way the engine aborts an attempt and runs the batch again: a candidate
-pool, per-character slot count or chunk text buffer that outgrew its estimate, on every route that can hit it; and the
-chunked host result growing past its estimates in every record group but the text.
+pool, per-character slot count or chunk text buffer that outgrew its estimate, on every route that can hit it; the
+chunked host result growing past its estimates in every record group but the text; and input errors in different
+chunks, alone or beside an overflow, which every route reports like the whole batch.
 
 Each case asserts, through describe()["last_reruns"], that the re-run it targets happened (and that the reference call
 re-ran nothing), that every array is byte-identical to a whole-batch call sized large enough from the start, that the
@@ -24,6 +25,7 @@ import vibrato_b200 as vb
 from bounded_oracle import BoundedOracle, vo_dictionary
 from test_gpu_marginals import d2h, shard_devices
 from test_gpu_sampling import check_parity
+from test_gpu_shards import device_call as device_call_bounded, error_of
 from test_gpu_uncertainty import close64
 from oracle import vibrato_oracle as vo
 
@@ -368,3 +370,60 @@ def test_result_grows_in_every_record_group():
         assert int(got[name][-1]) > est, (name, int(got[name][-1]), est)
     assert_same(got, reference("best", None, tuple(sents)), "grown")
     restate(got, sents, "best", None)
+
+
+# Input errors in different chunks of CUTS (sentence 100 of the chunk holds each): every route reports the one the whole
+# batch reports, the first in the engine's order (bad offsets, bad UTF-8, bad boundaries, bad spans) wherever it lies,
+# also where a chunk overflowed its candidate pool or text buffer on the same attempt.
+ERROR_CASES = {  # name: (setup, style, dense chunk, options, {error: chunk}, the error reported)
+    "bound0-utf8_2": ("best", "mecab", 1, dict(pool_estimate_permille=BIG_PERMILLE), dict(bound=0, utf8=2), "utf8"),
+    "span1-bound2": ("best", "mecab", 1, dict(pool_estimate_permille=BIG_PERMILLE), dict(span=1, bound=2), "bound"),
+    "pool0-utf8_2": ("best", "mecab", 0, dict(pool_estimate_permille=1), dict(utf8=2), "utf8"),
+    "text0-bound2": ("lattice", FMT_BIG, 0, dict(pool_estimate_permille=BIG_PERMILLE), dict(bound=2), "bound"),
+}
+MESSAGES = {"utf8": "stream did not contain valid UTF-8", "bound": "required boundaries must be non-decreasing"}
+
+
+def refused(route, case):
+    """((status, message), describe()["last_reruns"]) of the case's call on a fresh tokenizer, and the tokenizer."""
+    setup, style, dense, options, errors, _ = ERROR_CASES[case]
+    sents = list(batch(dense))
+    at = {kind: CUTS[c] + 100 for kind, c in errors.items()}
+    utf8, off = vb.Tokenizer.pack(sents)
+    if "utf8" in at:
+        assert sents[at["utf8"]]
+        utf8 = utf8.copy()
+        utf8[int(off[at["utf8"]])] = 0xFF  # never a UTF-8 byte
+    far = 1 << 20  # beyond every sentence's end
+    kw = {}
+    if "bound" in at:
+        kw["boundaries"] = [[far] if i == at["bound"] else [] for i in range(len(sents))]
+    if "span" in at:
+        kw["spans"] = [[(0, far)] if i == at["span"] else [] for i in range(len(sents))]
+    tok = make(route, setup, style, **options)
+    if route == "device":
+        err = error_of(lambda: device_call_bounded(tok, utf8, off, bounds=kw.get("boundaries"), spans=kw.get("spans")))
+    else:
+        err = error_of(lambda: tok.tokenize_batch(utf8=utf8, byte_offsets=off, **kw))
+    return err, tok.describe()["last_reruns"], tok
+
+
+@functools.lru_cache(maxsize=None)
+def whole_error(case):
+    err, _, _ = refused("whole", case)
+    return err
+
+
+@pytest.mark.parametrize("case", list(ERROR_CASES))
+@pytest.mark.parametrize("route", ["whole", "chunked", "dual", "device", "multi"])
+def test_input_errors_across_chunks(route, case):
+    """The case's call is refused with the whole batch's status and message, and books no re-run (a refused call
+    reports none); the tokenizer's next call, on OTHER, equals a fresh whole-batch call."""
+    setup, style, _, _, _, reported = ERROR_CASES[case]
+    err, reruns, tok = refused(route, case)
+    assert MESSAGES[reported] in whole_error(case)[1]
+    assert err == whole_error(case), (route, case)
+    assert reruns == NONE, (route, case, reruns)
+    style = style if route != "device" else None
+    again, _ = call(tok, route, list(OTHER))
+    assert_same(again, reference(setup, style, OTHER), (route, case, "again"))

@@ -21,6 +21,13 @@ namespace vbt {
 const char* const kStageNames =
     "count_chars,scan_slots,decode,candidates,scan_ends,viterbi,backtrack_count,scan_tokens,backtrack_write";
 
+const InputError kInputErrors[kNumInputErrors] = {
+    {kFlagBadOffsets, kInvalidArgument, kBadOffsetsMsg},
+    {kFlagUtf8Error, kUtf8, kBadUtf8Msg},
+    {kFlagBadBoundary, kInvalidArgument, kBadBoundsMsg},
+    {kFlagBadSpan, kInvalidArgument, kBadSpansMsg},
+};
+
 namespace {
 
 void cuda_check(cudaError_t e, const char* what) {
@@ -30,6 +37,28 @@ void cuda_check(cudaError_t e, const char* what) {
     }
 }
 #define CK(x) cuda_check((x), #x)
+
+// Throws the first input error (kInputErrors) that the flags of a finished attempt hold.
+void throw_input_error(uint32_t flags) {
+    for (const InputError& e : kInputErrors)
+        if (flags & e.flag) throw Error(e.status, e.msg);
+}
+
+// The flag of each re-run reason (Rerun), and what a call reports when it persists.
+constexpr uint32_t kRerunFlags[kNumReruns] = {kFlagPoolOverflow, kFlagSlotsOverflow, kFlagTextOverflow};
+const char* const kRerunPersists[kNumReruns] = {"candidate pool overflow persists", "slot overflow persists",
+                                                "text buffer overflow persists"};
+// The flags that end an attempt without a result: an input error (kInputErrors) or a re-run reason.
+constexpr uint32_t kFlagsEndAttempt = kFlagBadOffsets | kFlagUtf8Error | kFlagBadBoundary | kFlagBadSpan | kFlagPoolOverflow |
+                                      kFlagSlotsOverflow | kFlagTextOverflow;
+
+// A pooled host result that goes back to its pool unless release() hands it to the caller: an attempt that throws or
+// runs again does not keep it.
+struct ReturnTo {
+    ResultPool* pool;
+    void operator()(HostResult* r) const { pool->release(r); }
+};
+using PooledResult = std::unique_ptr<HostResult, ReturnTo>;
 
 struct Control {  // one small block zeroed per batch and read back once
     unsigned long long pool_ctr;  // candidates
@@ -620,27 +649,16 @@ class EngineImpl final : public Engine {
     HostResult* run_host(const char* utf8, const uint64_t* byte_off, uint64_t n_sent64, const Bounds* bnd) override {
         reruns_ = Reruns{};
         CK(cudaSetDevice(device_));
-        // offsets may start anywhere in the caller's buffer; ship only the used window
-        const uint64_t first = n_sent64 ? byte_off[0] : 0;
-        const uint64_t n_bytes = n_sent64 ? byte_off[n_sent64] - first : 0;
-        check_size(n_sent64, n_bytes);
-        check_bounded(bnd);
         Bounds nb;
-        bnd = drop_empty(bnd, n_sent64, nb);  // no boundary and no span at all: the unbounded kernels
+        const HostWindow hw = host_window(byte_off, n_sent64, bnd, nb);
+        const uint64_t first = hw.first, n_bytes = hw.n_bytes;
+        const uint64_t* off = hw.off;
+        bnd = hw.bnd;
         const uint32_t n_sent = uint32_t(n_sent64);
-        in_utf8_.ensure(n_bytes + 16, 1.25);
-        in_off_.ensure((size_t(n_sent) + 1) * 8, 1.25);
-        const uint64_t* off = byte_off;
-        if (first != 0) {
-            rebased_.resize(size_t(n_sent) + 1);
-            for (uint64_t i = 0; i <= n_sent; ++i) rebased_[i] = byte_off[i] - first;
-            off = rebased_.data();
-        }
         const uint8_t* d_utf8 = in_utf8_.as<uint8_t>();
         const unsigned long long* d_off = in_off_.as<unsigned long long>();
         const bool utf8_pinned = n_bytes == 0 || is_pinned(utf8 + first);
         const bool off_pinned = off != byte_off || is_pinned(byte_off);  // rebased_ is ours (pageable, small)
-        staged_bytes_ = 0;
         const uint32_t chunk = chunk_sentences_;
         const bool chunked = chunk > 0 && n_sent > chunk + chunk / 2;
         const bool fmt = output_mode_ != kOutNone;
@@ -659,26 +677,18 @@ class EngineImpl final : public Engine {
                     // Small batches (a per-sentence Worker loop ends up here) are all latency: the result copies are
                     // queued behind the kernels with an upper bound for the token count (a token spans >= 1 byte), so
                     // that the call makes ONE host synchronisation instead of two.
-                    HostResult* r = pool_.acquire(outputs(), n_sent, Totals{n_bytes, 0, 0, 0});
-                    eager_sink_ = r;
-                    try {
-                        run_whole(d_utf8, d_off, n_sent, n_bytes, bd);
-                    } catch (...) {
-                        eager_sink_ = nullptr;
-                        release(r);
-                        throw;
-                    }
-                    eager_sink_ = nullptr;
+                    PooledResult r(pool_.acquire(outputs(), n_sent, Totals{n_bytes, 0, 0, 0}), ReturnTo{&pool_});
+                    run_whole(d_utf8, d_off, n_sent, n_bytes, bd, 0, r.get());
                     r->total[kGroupTokens] = out_[0].h_ctrl->total[kGroupTokens];
-                    return r;
+                    return r.release();
                 }
                 run_whole(d_utf8, d_off, n_sent, n_bytes, bd);
                 if (fmt) format_whole(d_utf8, d_off, n_sent);
                 OutSlot& o = out_[0];
-                HostResult* r = pool_.acquire(outputs(), n_sent, totals(*o.h_ctrl));
-                place(o, r, 0, n_sent, r->total, Totals{}, true, stream_);
+                PooledResult r(pool_.acquire(outputs(), n_sent, totals(*o.h_ctrl)), ReturnTo{&pool_});
+                place(o, r.get(), 0, n_sent, r->total, Totals{}, true, stream_);
                 CK(cudaStreamSynchronize(stream_));
-                return r;
+                return r.release();
             }
             // ---- chunked, pipelined -------------------------------------------------------------
             // Chunk plan: a small first chunk (its H2D copy is the pipeline's fill), then halving sizes
@@ -725,28 +735,27 @@ class EngineImpl final : public Engine {
                     out_[i].buf[kText].ensure(size_t(double(max_chunk_bytes) * text_ratio) + size_t(max_chunk_sent) * per_sent + 4096);
                 }
             // a pinned result sized from the learned ratios per input byte (grown below if short)
-            HostResult* r = pool_.acquire(outputs(), n_sent,
+            PooledResult pr(pool_.acquire(outputs(), n_sent,
                                           Totals{uint64_t(double(n_bytes) * tok_per_byte_) + 1024,
                                                  uint64_t(double(n_bytes) * text_ratio) + uint64_t(n_sent) * per_sent + 1024,
                                                  uint64_t(double(n_bytes) * node_per_byte_) + 1024,
                                                  uint64_t(double(n_bytes) * tok_per_byte_ * samp_n_) + 1024,
                                                  uint64_t(double(n_bytes) * chars_per_byte_) + n_sent + 1024,
-                                                 uint64_t(double(n_bytes) * tok_per_byte_) + 1024});
+                                                 uint64_t(double(n_bytes) * tok_per_byte_) + 1024}),
+                            ReturnTo{&pool_});
+            HostResult* r = pr.get();
             CK(cudaMemsetAsync(base_.p, 0, kNumGroups * 8, stream_));
             connid_begin(stream_);
             h2d(in_off_.p, off, (size_t(n_sent) + 1) * 8, stream_, off_pinned && off == byte_off);
             CK(cudaEventRecord(in_done_, stream_));
             CK(cudaStreamWaitEvent(in_stream_, in_done_, 0));
             CK(cudaStreamWaitEvent(aux_stream_, in_done_, 0));
-            std::memset(stage_ms_, 0, sizeof(stage_ms_));
-            std::memset(counters_, 0, sizeof(counters_));
-            launches_ = 0;
+            clear_stats();
             Totals sum{};  // records per group of the chunks drained so far
             double text_need = 0;  // text bytes per input byte beyond per_sent per sentence, largest over the sound chunks
             uint32_t route = kRouteNone;
-            bool overflow = false, bad_utf8 = false, bad_offsets = false, slots_overflow = false, text_overflow = false;
-            bool pool_overflow = false;
-            bool bad_bounds = false, bad_spans = false;
+            uint32_t seen = 0;       // the flags of the chunks drained so far
+            uint64_t pool_most = 0;  // pool_need of the largest chunk
             uint64_t slots_seen = 0;
             batch_total_bytes_ = n_bytes;
             std::vector<cudaEvent_t>& h2d_ev = h2d_events(n_chunks);
@@ -766,30 +775,16 @@ class EngineImpl final : public Engine {
                 OutSlot& o = out_[c & 1];
                 uint32_t s0 = bounds[c], s1 = bounds[c + 1];
                 CK(cudaEventSynchronize(o.done));
-                if (o.h_ctrl->flags & kFlagUtf8Error) bad_utf8 = true;
-                if (o.h_ctrl->flags & kFlagBadOffsets) bad_offsets = true;
-                if (o.h_ctrl->flags & kFlagBadBoundary) bad_bounds = true;
-                if (o.h_ctrl->flags & kFlagBadSpan) bad_spans = true;
-                if (o.h_ctrl->flags & kFlagPoolOverflow) overflow = pool_overflow = true;
-                if (o.h_ctrl->flags & kFlagSlotsOverflow) overflow = slots_overflow = true;
-                if (o.h_ctrl->flags & kFlagTextOverflow) text_overflow = true;
+                seen |= o.h_ctrl->flags;
                 slots_seen += o.h_ctrl->total_slots;
-                for (int i = 0; i < kNumStages; ++i) {
-                    float ms = 0;
-                    CK(cudaEventElapsedTime(&ms, o.ev[i], o.ev[i + 1]));
-                    stage_ms_[i] += ms;
-                }
-                launches_ += o.launches;
                 // chunks share one static route; a chunk holding a very long sentence takes the unpruned twin
-                route = std::max<uint32_t>(route, resolve_viterbi_route(o.route, o.h_ctrl->flags));
-                if (counting_)
-                    for (int i = 0; i < kNumCounters; ++i) counters_[i] += o.h_ctrl->counters[i];
-                pool_need_ = std::max<uint64_t>(pool_need_, pool_need(*o.h_ctrl));
+                route = std::max(route, add_stats(o));
+                pool_most = std::max<uint64_t>(pool_most, pool_need(*o.h_ctrl));
                 const Totals count = totals(*o.h_ctrl);
                 if (fmt && !(o.h_ctrl->flags & (kFlagsStandDown | kFlagUtf8Error | kFlagPoolOverflow)))
                     text_need = std::max(text_need, (double(count[kGroupText]) - double(per_sent) * (s1 - s0)) /
                                                         double(std::max<uint64_t>(1, off[s1] - off[s0])));
-                if (!overflow && !text_overflow && !bad_utf8 && !bad_offsets && !bad_bounds && !bad_spans) {
+                if (!(seen & kFlagsEndAttempt)) {  // else nothing of the attempt is kept: it throws or runs again
                     // offsets are global already (base_); a record array that is short grows (rare), keeping what it
                     // holds once the copies into it have landed
                     for (int a = 0; a < kNumArrays; ++a) {
@@ -804,7 +799,6 @@ class EngineImpl final : public Engine {
                 CK(cudaEventRecord(o.drained, out_stream_));
                 for (int g = 0; g < kNumGroups; ++g) sum[g] += count[g];
             };
-            pool_need_ = 0;
             for (uint32_t c = 0; c < n_chunks; ++c) {
                 OutSlot& o = out_[c & 1];
                 uint32_t s0 = bounds[c], s1 = bounds[c + 1];
@@ -827,36 +821,16 @@ class EngineImpl final : public Engine {
             CK(cudaStreamSynchronize(in_stream_));
             CK(cudaStreamSynchronize(aux_stream_));
             CK(cudaStreamSynchronize(stream_));
-            if (bad_offsets) {
-                release(r);
-                throw Error(kInvalidArgument, kBadOffsetsMsg);
-            }
-            if (bad_utf8) {
-                release(r);
-                throw Error(kUtf8, kBadUtf8Msg);
-            }
-            if (bad_bounds) {
-                release(r);
-                throw Error(kInvalidArgument, kBadBoundsMsg);
-            }
-            if (bad_spans) {
-                release(r);
-                throw Error(kInvalidArgument, kBadSpansMsg);
-            }
-            if (overflow || text_overflow) {
-                release(r);
-                if (attempt >= 3) throw Error(kInternal, overflow ? "candidate pool overflow persists" : "text buffer overflow persists");
-                reruns_[kRerunPool] += pool_overflow;
-                reruns_[kRerunSlots] += slots_overflow;
-                reruns_[kRerunText] += text_overflow;
-                if (slots_overflow) chars_per_byte_ = 1.0;
-                if (overflow)
-                    cand_per_byte_ = std::max(cand_per_byte_ * 1.5, double(pool_need_) / double(std::max<uint64_t>(1, max_chunk_bytes)) * 1.2);
-                if (text_overflow) text_ratio_ref() = std::max(text_ratio * 1.5, text_need * 1.05) / renders;
+            throw_input_error(seen);
+            if (rerun(seen, attempt)) {
+                if (seen & kFlagSlotsOverflow) chars_per_byte_ = 1.0;
+                if (seen & (kFlagPoolOverflow | kFlagSlotsOverflow))
+                    cand_per_byte_ = std::max(cand_per_byte_ * 1.5, double(pool_most) / double(std::max<uint64_t>(1, max_chunk_bytes)) * 1.2);
+                if (seen & kFlagTextOverflow) text_ratio_ref() = std::max(text_ratio * 1.5, text_need * 1.05) / renders;
                 continue;
             }
             if (max_chunk_bytes)
-                cand_per_byte_ = std::max(0.25, double(pool_need_) / double(max_chunk_bytes) * 1.25);
+                cand_per_byte_ = std::max(0.25, double(pool_most) / double(max_chunk_bytes) * 1.25);
             if (n_bytes) tok_per_byte_ = std::max(0.02, double(sum[kGroupTokens]) / double(n_bytes) * 1.1);
             if (n_bytes) chars_per_byte_ = std::min(1.0, double(slots_seen - n_sent) / double(n_bytes) * 1.10);
             if (fmt) text_ratio_ref() = std::max(0.5, text_need * 1.25 / renders);
@@ -864,7 +838,7 @@ class EngineImpl final : public Engine {
             connid_commit(stream_);
             last_route_ = route;
             r->total = sum;
-            return r;
+            return pr.release();
         }
     }
 
@@ -876,23 +850,12 @@ class EngineImpl final : public Engine {
         last_ = DeviceOutputs{};
         reruns_ = Reruns{};
         CK(cudaSetDevice(device_));
-        const uint64_t first = n_sent64 ? byte_off[0] : 0;
-        const uint64_t n_bytes = n_sent64 ? byte_off[n_sent64] - first : 0;
-        check_size(n_sent64, n_bytes);
-        check_bounded(bnd);
         Bounds nb;
-        bnd = drop_empty(bnd, n_sent64, nb);
+        const HostWindow hw = host_window(byte_off, n_sent64, bnd, nb);
+        const uint64_t first = hw.first, n_bytes = hw.n_bytes;
         const uint32_t n_sent = uint32_t(n_sent64);
-        const DevBounds bd = bnd ? upload_bounds(*bnd, n_sent, stream_) : DevBounds{};
-        in_utf8_.ensure(n_bytes + 16, 1.25);
-        in_off_.ensure((size_t(n_sent) + 1) * 8, 1.25);
-        const uint64_t* off = byte_off;
-        if (first != 0) {
-            rebased_.resize(size_t(n_sent) + 1);
-            for (uint64_t i = 0; i <= n_sent; ++i) rebased_[i] = byte_off[i] - first;
-            off = rebased_.data();
-        }
-        h2d(in_off_.p, off, (size_t(n_sent) + 1) * 8, stream_, off == byte_off && is_pinned(byte_off));
+        const DevBounds bd = hw.bnd ? upload_bounds(*hw.bnd, n_sent, stream_) : DevBounds{};
+        h2d(in_off_.p, hw.off, (size_t(n_sent) + 1) * 8, stream_, hw.off == byte_off && is_pinned(byte_off));
         if (n_bytes) {
             if (src_device >= 0 && src_device != device_)
                 CK(cudaMemcpyPeerAsync(in_utf8_.p, device_, utf8 + first, src_device, n_bytes, stream_));
@@ -963,7 +926,6 @@ class EngineImpl final : public Engine {
             CK(cudaMemcpyAsync(static_cast<uint8_t*>(dst) + o, ring_[slot], len, cudaMemcpyHostToDevice, st));
             CK(cudaEventRecord(ring_ev_[slot], st));
         }
-        staged_bytes_ += bytes;
     }
 
     // One attempt at a batch = connid_begin, its enqueue(s), then connid_commit once it is known to have succeeded.
@@ -1007,6 +969,29 @@ class EngineImpl final : public Engine {
         if (nb.spans.off && host_lists_empty(nb.spans.off, n_sent)) nb.spans = Spans{};
         if (nb.off && host_lists_empty(nb.off, n_sent)) nb.off = nullptr;
         return (nb.off || nb.spans.off) ? &nb : nullptr;
+    }
+    // The window of the caller's buffer a host batch uses (its offsets may start anywhere in it; only the window is
+    // copied): the checks of the call, its offsets rebased to the window's first byte (into rebased_ unless that is
+    // 0), its bounds without empty lists (drop_empty, into nb) and in_utf8_ / in_off_ sized for it.
+    struct HostWindow {
+        uint64_t first, n_bytes;
+        const uint64_t* off;
+        const Bounds* bnd;
+    };
+    HostWindow host_window(const uint64_t* byte_off, uint64_t n_sent, const Bounds* bnd, Bounds& nb) {
+        const uint64_t first = n_sent ? byte_off[0] : 0;
+        HostWindow w{first, n_sent ? byte_off[n_sent] - first : 0, byte_off, nullptr};
+        check_size(n_sent, w.n_bytes);
+        check_bounded(bnd);
+        w.bnd = drop_empty(bnd, n_sent, nb);  // no boundary and no span at all: the unbounded kernels
+        in_utf8_.ensure(w.n_bytes + 16, 1.25);
+        in_off_.ensure((size_t(n_sent) + 1) * 8, 1.25);
+        if (first != 0) {
+            rebased_.resize(size_t(n_sent) + 1);
+            for (uint64_t i = 0; i <= n_sent; ++i) rebased_[i] = byte_off[i] - first;
+            w.off = rebased_.data();
+        }
+        return w;
     }
     // n_sent + 1 zero offsets on the device (in_bnd_off_): a span batch without explicit boundaries.
     const unsigned long long* zero_offsets(uint32_t n_sent, cudaStream_t st) {
@@ -1401,15 +1386,8 @@ class EngineImpl final : public Engine {
         CK(cudaStreamSynchronize(stream_));
         SmallBatchOut h;
         std::memcpy(&h, small_out_h_, sizeof h);
-        if (h.flags & kFlagBadOffsets)
-            throw Error(kInvalidArgument, kBadOffsetsMsg);
-        if (h.flags & kFlagUtf8Error) throw Error(kUtf8, kBadUtf8Msg);
-        if (h.flags & kFlagBadBoundary) throw Error(kInvalidArgument, kBadBoundsMsg);
-        if (h.flags & (kFlagPoolOverflow | kFlagTextOverflow)) {
-            reruns_[kRerunPool] += (h.flags & kFlagPoolOverflow) != 0;
-            reruns_[kRerunText] += (h.flags & kFlagTextOverflow) != 0;
-            return nullptr;
-        }
+        throw_input_error(h.flags);
+        if (rerun(h.flags, 0)) return nullptr;
         if (fmt && h.text_bytes > text_guess) {
             CK(cudaMemcpyAsync(small_out_h_ + at_text + text_guess, region + at_text + text_guess, h.text_bytes - text_guess,
                                cudaMemcpyDeviceToHost, stream_));
@@ -1424,7 +1402,7 @@ class EngineImpl final : public Engine {
             std::memcpy(r->buf[kTextOff].p, small_out_h_ + at_text_off, off_bytes);
             if (h.text_bytes) std::memcpy(r->buf[kText].p, small_out_h_ + at_text, h.text_bytes);
         }
-        std::memset(stage_ms_, 0, sizeof(stage_ms_));
+        clear_stats();
         CK(cudaEventElapsedTime(&stage_ms_[kSmallBatchStage], o.ev[0], o.ev[1]));
         launches_ = 1;
         last_route_ = kRouteSmallBatch;
@@ -1623,8 +1601,9 @@ class EngineImpl final : public Engine {
 
     // One whole batch from device-resident input into out_[0]; synchronises, retries on pool overflow.
     // sent_base: the caller's index of the first sentence (a shard's place in the batch), for the sampling draws.
+    // sink (small host batches): a result the outputs are copied into right behind the kernels (enqueue).
     void run_whole(const uint8_t* d_utf8, const unsigned long long* d_off, uint32_t n_sent, uint64_t n_bytes,
-                   const DevBounds& bd, uint64_t sent_base = 0) {
+                   const DevBounds& bd, uint64_t sent_base = 0, HostResult* sink = nullptr) {
         OutSlot& o = out_[0];
         ws_[0].stream = stream_;
         batch_total_bytes_ = n_bytes;
@@ -1634,38 +1613,60 @@ class EngineImpl final : public Engine {
             ensure_out(o, n_sent, n_bytes);
             ensure_entries(ws_[0], o, cands + n_sent + 1);
             connid_begin(stream_);
-            enqueue(ws_[0], d_utf8, d_off, n_sent, n_bytes, o, nullptr, nullptr, nullptr, bd, sent_base);
+            enqueue(ws_[0], d_utf8, d_off, n_sent, n_bytes, o, nullptr, nullptr, nullptr, bd, sent_base, sink);
             CK(cudaEventSynchronize(o.done));
             CK(cudaGetLastError());
-            if (o.h_ctrl->flags & kFlagBadOffsets)
-                throw Error(kInvalidArgument, kBadOffsetsMsg);
-            if (o.h_ctrl->flags & kFlagUtf8Error)
-                throw Error(kUtf8, kBadUtf8Msg);
-            if (o.h_ctrl->flags & kFlagBadBoundary) throw Error(kInvalidArgument, kBadBoundsMsg);
-            if (o.h_ctrl->flags & kFlagBadSpan) throw Error(kInvalidArgument, kBadSpansMsg);
-            if (o.h_ctrl->flags & kFlagSlotsOverflow) {  // more characters per byte than any batch before: hard bound
-                if (attempt >= 3) throw Error(kInternal, "slot overflow persists");
-                ++reruns_[kRerunSlots];
-                chars_per_byte_ = 1.0;
+            throw_input_error(o.h_ctrl->flags);
+            // more characters per byte than any batch before: the next attempt takes the hard bound, and only then
+            // counts its candidates in full
+            const uint32_t why = o.h_ctrl->flags & kFlagSlotsOverflow ? kFlagSlotsOverflow : o.h_ctrl->flags;
+            const double need = double(pool_need(*o.h_ctrl));
+            if ((why & kFlagPoolOverflow) && need * 1.05 + 4096 >= double(0xFFFFFFF0ull))
+                throw Error(kInvalidArgument, "batch produces more than 2^32 lattice nodes: split it");
+            if (rerun(why, attempt)) {
+                if (why & kFlagSlotsOverflow) chars_per_byte_ = 1.0;
+                if (why & kFlagPoolOverflow) cand_per_byte_ = need / double(std::max<uint64_t>(1, n_bytes)) * 1.05 + 1e-3;
                 continue;
             }
-            if (o.h_ctrl->flags & kFlagPoolOverflow) {
-                if (attempt >= 3) throw Error(kInternal, "candidate pool overflow persists");
-                if (double(pool_need(*o.h_ctrl)) * 1.05 + 4096 >= double(0xFFFFFFF0ull))
-                    throw Error(kInvalidArgument, "batch produces more than 2^32 lattice nodes: split it");
-                cand_per_byte_ = double(pool_need(*o.h_ctrl)) / double(std::max<uint64_t>(1, n_bytes)) * 1.05 + 1e-3;
-                ++reruns_[kRerunPool];
-                continue;
-            }
-            if (n_bytes) cand_per_byte_ = std::max(0.25, double(pool_need(*o.h_ctrl)) / double(n_bytes) * 1.15);
+            if (n_bytes) cand_per_byte_ = std::max(0.25, need / double(n_bytes) * 1.15);
             if (n_bytes) chars_per_byte_ = std::min(1.0, double(o.h_ctrl->total_slots - n_sent) / double(n_bytes) * 1.10);
             connid_commit(stream_);
             break;
         }
-        for (int i = 0; i < kNumStages; ++i) CK(cudaEventElapsedTime(&stage_ms_[i], o.ev[i], o.ev[i + 1]));
-        launches_ = o.launches;
-        last_route_ = resolve_viterbi_route(o.route, o.h_ctrl->flags);
-        if (counting_) std::memcpy(counters_, o.h_ctrl->counters, sizeof(counters_));
+        clear_stats();
+        last_route_ = add_stats(o);
+    }
+
+    // Ends an attempt that finished with `flags` and no input error: books each re-run reason they hold in reruns_ and
+    // says whether to run again.  An overflow that persists after three re-runs throws.
+    bool rerun(uint32_t flags, int attempt) {
+        bool again = false;
+        for (int k = 0; k < kNumReruns; ++k) {
+            if (!(flags & kRerunFlags[k])) continue;
+            if (attempt >= 3) throw Error(kInternal, kRerunPersists[k]);
+            ++reruns_[k];
+            again = true;
+        }
+        return again;
+    }
+
+    // The statistics of a call: zeroed once per attempt, then each finished slot (a whole batch, or every chunk) adds
+    // its stage times, launches and counters.  add_stats returns the slot's Viterbi route as resolved by its flags.
+    void clear_stats() {
+        std::memset(stage_ms_, 0, sizeof(stage_ms_));
+        std::memset(counters_, 0, sizeof(counters_));
+        launches_ = 0;
+    }
+    uint32_t add_stats(const OutSlot& o) {
+        for (int i = 0; i < kNumStages; ++i) {
+            float ms = 0;
+            CK(cudaEventElapsedTime(&ms, o.ev[i], o.ev[i + 1]));
+            stage_ms_[i] += ms;
+        }
+        launches_ += o.launches;
+        if (counting_)
+            for (int i = 0; i < kNumCounters; ++i) counters_[i] += o.h_ctrl->counters[i];
+        return resolve_viterbi_route(o.route, o.h_ctrl->flags);
     }
 
     // Queues the whole kernel sequence for one (chunk of a) batch on stream_; no host synchronisation.
@@ -1674,7 +1675,7 @@ class EngineImpl final : public Engine {
     // (kFlagTextOverflow beyond).
     void enqueue(Workspace& w, const uint8_t* d_utf8, const unsigned long long* d_off, uint32_t n_sent, uint64_t n_bytes,
                  OutSlot& o, unsigned long long* base, cudaEvent_t base_wait, cudaEvent_t base_signal, const DevBounds& bd,
-                 uint64_t sent0) {
+                 uint64_t sent0, HostResult* sink = nullptr) {
         cudaStream_t st = w.stream;
         o.made = outputs();
         if (!base) o.made.text = false;  // whole batches and shards are formatted by format_whole
@@ -1889,7 +1890,7 @@ class EngineImpl final : public Engine {
         CK(cudaEventRecord(o.ev[9], st));
         CK(cudaMemcpyAsync(o.h_ctrl, dc, sizeof(Control), cudaMemcpyDeviceToHost, st));
         // small batch: results leave in the same breath (sized by their upper bound, a token per byte)
-        if (eager_sink_) place(o, eager_sink_, 0, n_sent, Totals{n_bytes, 0, 0, 0}, Totals{}, true, st);
+        if (sink) place(o, sink, 0, n_sent, Totals{n_bytes, 0, 0, 0}, Totals{}, true, st);
         CK(cudaEventRecord(o.done, st));
     }
 
@@ -1900,14 +1901,12 @@ class EngineImpl final : public Engine {
     cudaEvent_t ring_ev_[kRingSlots] = {nullptr, nullptr, nullptr, nullptr};
     int ring_next_ = 0;
     static constexpr uint64_t kEagerBytes = 16384;
-    HostResult* eager_sink_ = nullptr;
     uint32_t small_batch_ = 0;  // "small_batch": the most sentences k_small_batch takes (0 = the route is off)
     Workspace ws_small_;        // scratch of k_small_batch (its stream is unused)
     DevBuf small_in_, small_out_;
     uint8_t* small_in_h_ = nullptr;  // pinned staging of the input / output region (ensure_small)
     uint8_t* small_out_h_ = nullptr;
     size_t small_in_cap_ = 0, small_out_cap_ = 0;
-    uint64_t staged_bytes_ = 0;  // bytes of pageable caller memory that went through the ring (last batch)
     uint32_t shard_n_sent_ = 0;
     cudaStream_t stream_ = nullptr, own_stream_ = nullptr, in_stream_ = nullptr, out_stream_ = nullptr;
     cudaEvent_t in_done_ = nullptr;
@@ -1915,7 +1914,6 @@ class EngineImpl final : public Engine {
     OutSlot out_[2];
     DevBuf base_;  // chunked host batches: the running total of each group's records (enqueue)
     uint32_t chunk_sentences_ = 262144;
-    uint64_t pool_need_ = 0;
     double tok_per_byte_ = 0.2;
     DictView dv_{};
     const uint8_t* blob_ = nullptr;

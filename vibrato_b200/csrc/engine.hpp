@@ -189,6 +189,13 @@ constexpr const char* kBadSpansMsg =
     "end, be sorted and non-overlapping, name VBT_SPAN_ANY or a pattern of the call, hold no explicit boundary "
     "inside, not start at a space when ignore_space is on, and their offsets must be non-decreasing and within the "
     "span array";
+struct InputError {
+    uint32_t flag;  // the kernels' batch flag (kernels.cuh kFlag*)
+    Status status;
+    const char* msg;
+};
+constexpr int kNumInputErrors = 4;
+extern const InputError kInputErrors[kNumInputErrors];  // engine.cu: the four above, in that order
 
 // Why a call ran an attempt again: its candidate pool, its per-character slots or (chunked host batches) the output
 // text of a chunk outgrew the size learned from earlier batches.  An attempt with several counts under each.

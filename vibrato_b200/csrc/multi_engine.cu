@@ -483,7 +483,7 @@ class MultiEngine final : public Engine {
 
     // One host thread per device (the calling thread takes the first): each call blocks on its own device.  Of the
     // shards that failed, the error one device would report for the whole batch wins: any other error before the
-    // input errors, those in their order (kBadOffsetsMsg ..), then the first shard.
+    // input errors, those in their order (kInputErrors), then the first shard.
     template <typename F>
     void run_on_all(F&& f) {
         const int n = int(dev_.size());
@@ -509,9 +509,8 @@ class MultiEngine final : public Engine {
         body(0);
         for (auto& t : th) t.join();
         auto rank = [&](int i) {
-            const char* const order[] = {kBadOffsetsMsg, kBadUtf8Msg, kBadBoundsMsg, kBadSpansMsg};
-            for (int k = 0; k < 4; ++k)
-                if (err[i] == order[k]) return k + 1;
+            for (int k = 0; k < kNumInputErrors; ++k)
+                if (err[i] == kInputErrors[k].msg) return k + 1;
             return 0;
         };
         int worst = -1;
